@@ -24,6 +24,16 @@ class TdnnArgs(C.Structure):
 MAX_TAPS = 16
 
 
+class Conv2dArgs(C.Structure):
+    """xvb_conv2d_args_t (include/xvb200.h)."""
+    _fields_ = [("x_hi", C.c_void_p), ("x_lo", C.c_void_p), ("w_hi", C.c_void_p), ("w_lo", C.c_void_p),
+                ("B", C.c_int), ("T", C.c_int), ("F", C.c_int), ("Cin", C.c_int), ("Cout", C.c_int),
+                ("ksize", C.c_int), ("stride", C.c_int),
+                ("scale", C.c_void_p), ("shift", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
+                ("relu", C.c_int), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("y_f32", C.c_void_p),
+                ("scale2", C.c_void_p), ("shift2", C.c_void_p), ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p)]
+
+
 class XvbError(RuntimeError):
     pass
 
@@ -102,6 +112,9 @@ SIGNATURES = {
     "xvb_plda_normalize_rows": (_i, [_p, _p, _p, _i64, _i, _i, _p]),
     "xvb_plda_llr_operands": (_i, [_p, _p, _p, _i64, _i, _i, _p, _p, _p]),
     "xvb_trial_histogram": (_i, [_p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i, _i, _i, _f, _f, _i, _p, _p]),
+    "xvb_conv2d": (_i, [_p, _p]),
+    "xvb_conv2d_head": (_i, [_p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_extractor_add_segment_layer": (_i, [_p, _i, _p, _p, _p, _p, _i]),

@@ -1,0 +1,514 @@
+// 2-D convolution of the ResNet x-vector (pytorch/libs/nnet/resnet.py BasicBlock, pytorch/model/resnet_xvector.py)
+// as an implicit-GEMM warpgroup-MMA kernel (sm_90a), plus the two bandwidth-bound pieces around it.
+//
+//   y[b,t,f,n] = epi( sum_{kf,kt} sum_c W[n, c, kf, kt] * x[b, t*s + kt - p, f*s + kf - p, c] )
+//
+// The reference feeds (1, 1, F, T) to Conv2d: "H" is the feature axis, "W" is time.  Here a frame tensor is a
+// channel-contiguous (B, T, F, C) split-plane pair, and the kernel reads it through a 4-D tensor map (C, F, T, B):
+//   * M = output positions, N = Cout, K = k*k taps x Cin, tap-major (the xvb_pack_tdnn_weight layout of the weight
+//     viewed as (Cout, Cin, k*k));
+//   * an M tile is 128 positions = Bb utterances x Tb frames x Fb feature bins (powers of two, chosen on the host for
+//     the fewest padded rows); tap (kf, kt) is only a coordinate offset, so TMA's out-of-bounds zero fill is exactly
+//     the convolution's zero padding and never reads a neighbouring utterance;
+//   * stride 2 uses the tensor map's element strides: the box traverses 2*Fb x 2*Tb input positions and lands Fb x Tb
+//     of them, so no output is computed and thrown away;
+//   * Cin = 32 (the first stage) loads 64-channel boxes whose upper half TMA zero-fills; the MMA loop stops after the
+//     real 32 channels, so the padding costs shared-memory traffic and no tensor-core work;
+//   * numerics and pipeline are the TDNN layer's (tdnn_gemm.cu): bf16 hi/lo planes, three wgmma per K step into fp32
+//     register accumulators, one TMA producer warp feeding an mbarrier operand ring, two consumer warpgroups;
+//   * epilogue: y = acc * scale[n] + shift[n] (eval BatchNorm after the bias-free conv) [+ residual] [ReLU] -> planes
+//     and/or fp32, and optionally a second output relu(y * scale2[n] + shift2[n]) (the next pre-activation block's
+//     BN-ReLU, which cannot be folded into that block's conv because the zero padding comes after it).
+#include <cuda.h>
+#include <cuda_bf16.h>
+#include <cuda_runtime.h>
+
+#include "common.cuh"
+#include "ptx.cuh"
+
+namespace xvb {
+namespace {
+
+constexpr int kBlockM = 128;
+constexpr int kBlockK = 64;                      // bf16 elements = one 128-byte swizzle row
+constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB per plane per stage
+constexpr int kNumConsumers = 256;
+constexpr int kProducerWarp = kNumConsumers / 32;
+constexpr int kNumThreads = kNumConsumers + 32;
+
+struct Conv2dParams {
+  int B, T, F, Cin, To, Fo, Cout;
+  int ks, stride, pad;
+  int Fb, Tb, Bb, log2_fb, log2_tb;
+  int num_f_blk, num_t_blk, num_n_blk, num_tiles;
+  int cin_p16, num_cblk;
+  int relu;
+  const float* scale;
+  const float* shift;
+  const __nv_bfloat16* res_hi;
+  const __nv_bfloat16* res_lo;
+  __nv_bfloat16* y_hi;
+  __nv_bfloat16* y_lo;
+  float* y_f32;
+  const float* scale2;
+  const float* shift2;
+  __nv_bfloat16* y2_hi;
+  __nv_bfloat16* y2_lo;
+};
+
+template <int BLOCK_N>
+struct ConvCfg {
+  static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
+  static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
+  static constexpr int kStages = (192 * 1024) / kStageBytes > 6 ? 6 : (192 * 1024) / kStageBytes;
+  static constexpr int kAccRegs = BLOCK_N / 2;
+  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared memory of an sm_90 CTA");
+  static_assert(kStages >= 2, "need at least a double-buffered operand pipeline");
+};
+
+// tile -> (first output position of the M tile, N block); N fastest so that CTAs running together share the A tile
+__device__ __forceinline__ void decode_conv_tile(const Conv2dParams& p, int tile, int& b0, int& t0, int& f0, int& n_blk) {
+  n_blk = tile % p.num_n_blk;
+  int m = tile / p.num_n_blk;
+  f0 = (m % p.num_f_blk) * p.Fb;
+  m /= p.num_f_blk;
+  t0 = (m % p.num_t_blk) * p.Tb;
+  b0 = (m / p.num_t_blk) * p.Bb;
+}
+
+template <int BLOCK_N>
+__global__ void __launch_bounds__(kNumThreads, 1)
+conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
+                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                     const __grid_constant__ Conv2dParams p) {
+  using Cfg = ConvCfg<BLOCK_N>;
+  constexpr int kStages = Cfg::kStages;
+  constexpr int kBBytes = Cfg::kBBytes;
+  constexpr int kStageBytes = Cfg::kStageBytes;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * kStageBytes);
+  uint64_t* empty_bar = full_bar + kStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(&map_x_hi);
+    tma_prefetch_desc(&map_x_lo);
+    tma_prefetch_desc(&map_w_hi);
+    tma_prefetch_desc(&map_w_lo);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], kNumConsumers / 32);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("fence.proxy.async;" ::: "memory");   // operands may come from generic-proxy stores of the previous kernel
+
+  const int num_kblk = p.ks * p.ks * p.num_cblk;
+
+  if (warp == kProducerWarp) {
+    if (lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        int b0, t0, f0, n_blk;
+        decode_conv_tile(p, tile, b0, t0, f0, n_blk);
+        const int n0 = n_blk * BLOCK_N;
+        for (int kf = 0; kf < p.ks; ++kf) {
+          const int fi = f0 * p.stride + kf - p.pad;
+          for (int kt = 0; kt < p.ks; ++kt) {
+            const int ti = t0 * p.stride + kt - p.pad;
+            const int tap = kf * p.ks + kt;
+            for (int cb = 0; cb < p.num_cblk; ++cb) {
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              uint8_t* s = smem + stage * kStageBytes;
+              mbar_expect_tx(&full_bar[stage], kStageBytes);
+              tma_load_4d(s, &map_x_hi, &full_bar[stage], cb * kBlockK, fi, ti, b0);
+              tma_load_4d(s + kABytes, &map_x_lo, &full_bar[stage], cb * kBlockK, fi, ti, b0);
+              tma_load_2d(s + 2 * kABytes, &map_w_hi, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
+              tma_load_2d(s + 2 * kABytes + kBBytes, &map_w_lo, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
+              if (++stage == kStages) { stage = 0; phase ^= 1; }
+            }
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // ================================ consumers: wgmma + epilogue ================================
+  const int wg = warp >> 2;
+  const int q4 = lane & 3;
+  const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+  const float relu_floor = p.relu ? 0.f : -INFINITY;
+  float acc[Cfg::kAccRegs];
+#pragma unroll
+  for (int i = 0; i < Cfg::kAccRegs; ++i) acc[i] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+    int prev_stage = -1;
+    uint32_t scale_d = 0;
+    for (int kb = 0; kb < num_kblk; ++kb) {
+      const int cb = kb % p.num_cblk;
+      int nsteps = (p.Cin - cb * kBlockK + 15) >> 4;
+      nsteps = nsteps > 4 ? 4 : nsteps;
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+      const uint64_t m_off = (uint64_t)((wg * 64 * 128) >> 4);
+      const uint64_t da_hi = make_sw128_desc(sa) + m_off, da_lo = make_sw128_desc(sa + kABytes) + m_off;
+      const uint64_t db_hi = make_sw128_desc(sa + 2 * kABytes), db_lo = make_sw128_desc(sa + 2 * kABytes + kBBytes);
+      wgmma_fence();
+      for (int s = 0; s < nsteps; ++s) {
+        const uint64_t koff = (uint64_t)(s * 32 >> 4);
+        wgmma_bf16<BLOCK_N>(acc, da_lo + koff, db_hi + koff, scale_d);
+        wgmma_bf16<BLOCK_N>(acc, da_hi + koff, db_lo + koff, 1);
+        wgmma_bf16<BLOCK_N>(acc, da_hi + koff, db_hi + koff, 1);
+        scale_d = 1;
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+
+    // ---- epilogue: BN -> [+ residual] -> [ReLU] -> planes / fp32 [, relu(BN2) planes]
+    int b0, t0, f0, n_blk;
+    decode_conv_tile(p, tile, b0, t0, f0, n_blk);
+    const int n0 = n_blk * BLOCK_N;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      const int f = f0 + (row & (p.Fb - 1));
+      const int t = t0 + ((row >> p.log2_fb) & (p.Tb - 1));
+      const int b = b0 + (row >> (p.log2_fb + p.log2_tb));
+      if (f >= p.Fo || t >= p.To || b >= p.B) continue;
+      const long long off = (((long long)b * p.To + t) * p.Fo + f) * p.Cout;
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const int c = n0 + 8 * i + 2 * q4;   // Cout % 16 == 0: c and c + 1 both exist or neither
+        if (c >= p.Cout) break;
+        float x[2] = {acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]};
+        if (p.scale) {
+          x[0] = fmaf(x[0], __ldg(p.scale + c), __ldg(p.shift + c));
+          x[1] = fmaf(x[1], __ldg(p.scale + c + 1), __ldg(p.shift + c + 1));
+        }
+        if (p.res_hi) {
+          const uint32_t rh = *reinterpret_cast<const uint32_t*>(p.res_hi + off + c);
+          const uint32_t rl = *reinterpret_cast<const uint32_t*>(p.res_lo + off + c);
+          x[0] += __uint_as_float(rh << 16) + __uint_as_float(rl << 16);
+          x[1] += __uint_as_float(rh & 0xffff0000u) + __uint_as_float(rl & 0xffff0000u);
+        }
+        x[0] = fmaxf(x[0], relu_floor);
+        x[1] = fmaxf(x[1], relu_floor);
+        if (p.y_hi) {
+          __nv_bfloat16 h0, l0, h1, l1;
+          split_bf16(x[0], h0, l0);
+          split_bf16(x[1], h1, l1);
+          *reinterpret_cast<uint32_t*>(p.y_hi + off + c) = pack_bf16x2(h0, h1);
+          *reinterpret_cast<uint32_t*>(p.y_lo + off + c) = pack_bf16x2(l0, l1);
+        }
+        if (p.y_f32) *reinterpret_cast<float2*>(p.y_f32 + off + c) = make_float2(x[0], x[1]);
+        if (p.y2_hi) {
+          const float u0 = fmaxf(fmaf(x[0], __ldg(p.scale2 + c), __ldg(p.shift2 + c)), 0.f);
+          const float u1 = fmaxf(fmaf(x[1], __ldg(p.scale2 + c + 1), __ldg(p.shift2 + c + 1)), 0.f);
+          __nv_bfloat16 h0, l0, h1, l1;
+          split_bf16(u0, h0, l0);
+          split_bf16(u1, h1, l1);
+          *reinterpret_cast<uint32_t*>(p.y2_hi + off + c) = pack_bf16x2(h0, h1);
+          *reinterpret_cast<uint32_t*>(p.y2_lo + off + c) = pack_bf16x2(l0, l1);
+        }
+      }
+    }
+  }
+}
+
+// Head conv (Cin = 1, 3x3, stride 1, padding 1) on CUDA cores, fp32: its input rows (one value per position) break
+// TMA's 16-byte rule and it is ~0.1 % of the MACs.  One thread per (position, 8 output channels); fused BN + ReLU,
+// the split to planes and the optional second output relu(y * scale2 + shift2).
+__global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int F, const float* __restrict__ w, int Cout,
+                                 const float* __restrict__ scale, const float* __restrict__ shift,
+                                 __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl,
+                                 const float* __restrict__ scale2, const float* __restrict__ shift2,
+                                 __nv_bfloat16* __restrict__ y2h, __nv_bfloat16* __restrict__ y2l) {
+  const int groups = Cout / 8;
+  const long long total = (long long)B * T * F * groups;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c0 = (int)(i % groups) * 8;
+    const long long pos = i / groups;
+    const int f = (int)(pos % F);
+    const long long bt = pos / F;
+    const int t = (int)(bt % T);
+    const long long b = bt / T;
+    float in[9];
+#pragma unroll
+    for (int kf = 0; kf < 3; ++kf)
+#pragma unroll
+      for (int kt = 0; kt < 3; ++kt) {
+        const int ff = f + kf - 1, tt = t + kt - 1;
+        in[kf * 3 + kt] = (ff >= 0 && ff < F && tt >= 0 && tt < T) ? __ldg(x + (b * T + tt) * F + ff) : 0.f;
+      }
+    float y[8], y2[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const float* wc = w + (c0 + k) * 9;
+      float s = 0.f;
+#pragma unroll
+      for (int j = 0; j < 9; ++j) s = fmaf(__ldg(wc + j), in[j], s);
+      y[k] = fmaxf(fmaf(s, __ldg(scale + c0 + k), __ldg(shift + c0 + k)), 0.f);
+      if (y2h) y2[k] = fmaxf(fmaf(y[k], __ldg(scale2 + c0 + k), __ldg(shift2 + c0 + k)), 0.f);
+    }
+    uint4 h, l;
+    pack8(y, h, l);
+    *reinterpret_cast<uint4*>(yh + pos * Cout + c0) = h;
+    *reinterpret_cast<uint4*>(yl + pos * Cout + c0) = l;
+    if (y2h) {
+      pack8(y2, h, l);
+      *reinterpret_cast<uint4*>(y2h + pos * Cout + c0) = h;
+      *reinterpret_cast<uint4*>(y2l + pos * Cout + c0) = l;
+    }
+  }
+}
+
+// y = [relu]( z * gate[b, c] + identity ) over (B, P, C) planes -> planes and/or fp32 [, relu(y * scale2 + shift2) planes]:
+// SEBlock_2D's scaling (components.py:630-639) with the residual add of BasicBlock (resnet.py:70-104).
+__global__ void se_residual_kernel(const __nv_bfloat16* __restrict__ zh, const __nv_bfloat16* __restrict__ zl,
+                                   const float* __restrict__ gate, const __nv_bfloat16* __restrict__ ih,
+                                   const __nv_bfloat16* __restrict__ il, long long P, int C, int relu,
+                                   __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, float* __restrict__ yf,
+                                   const float* __restrict__ scale2, const float* __restrict__ shift2,
+                                   __nv_bfloat16* __restrict__ y2h, __nv_bfloat16* __restrict__ y2l, long long total) {
+  const int groups = C / 8;
+  const float floor_v = relu ? 0.f : -INFINITY;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long pos = i / groups;
+    const int c = (int)(i % groups) * 8;
+    const long long b = pos / P;
+    const long long e = pos * C + c;
+    float z[8], x[8], y[8];
+    unpack8(*reinterpret_cast<const uint4*>(zh + e), *reinterpret_cast<const uint4*>(zl + e), z);
+    unpack8(*reinterpret_cast<const uint4*>(ih + e), *reinterpret_cast<const uint4*>(il + e), x);
+    const float4 g0 = *reinterpret_cast<const float4*>(gate + b * C + c);
+    const float4 g1 = *reinterpret_cast<const float4*>(gate + b * C + c + 4);
+    const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) y[k] = fmaxf(__fadd_rn(__fmul_rn(z[k], g[k]), x[k]), floor_v);   // the reference's two roundings
+    uint4 h, l;
+    if (yh) {
+      pack8(y, h, l);
+      *reinterpret_cast<uint4*>(yh + e) = h;
+      *reinterpret_cast<uint4*>(yl + e) = l;
+    }
+    if (yf) {
+      *reinterpret_cast<float4*>(yf + e) = make_float4(y[0], y[1], y[2], y[3]);
+      *reinterpret_cast<float4*>(yf + e + 4) = make_float4(y[4], y[5], y[6], y[7]);
+    }
+    if (y2h) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) y[k] = fmaxf(fmaf(y[k], __ldg(scale2 + c + k), __ldg(shift2 + c + k)), 0.f);
+      pack8(y, h, l);
+      *reinterpret_cast<uint4*>(y2h + e) = h;
+      *reinterpret_cast<uint4*>(y2l + e) = l;
+    }
+  }
+}
+
+int grid_for(long long total, int block) {
+  long long g = (total + block - 1) / block;
+  const long long cap = (long long)sm_count() * 16;
+  return (int)(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+// (Fb, Tb, Bb) powers of two with Fb*Tb*Bb = 128 and the fewest padded output rows; ties go to the fewest utterances
+// per tile, then the widest Fb (spatially compact tiles: the 9 taps of one tile overlap in L2).
+void choose_conv_tile(int B, int To, int Fo, int stride, int* Fb, int* Tb, int* Bb) {
+  long long best = -1;
+  for (int lb = 0; lb <= 7; ++lb) {
+    for (int lf = 7 - lb; lf >= 0; --lf) {
+      const int bb = 1 << lb, fb = 1 << lf, tb = 128 / (bb * fb);
+      if (fb * stride > 256 || tb * stride > 256) continue;   // TMA box dimensions <= 256
+      const long long rows = (long long)((Fo + fb - 1) / fb) * fb * ((To + tb - 1) / tb) * tb * ((B + bb - 1) / bb) * bb;
+      if (best < 0 || rows < best) { best = rows; *Fb = fb; *Tb = tb; *Bb = bb; }
+    }
+  }
+}
+
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+// 4-D bf16 map of a (B, T, F, C) position tensor with element strides (the strided traversal of stride-2 convs, which
+// make_tensor_map does not expose)
+int make_position_map(CUtensorMap* m, const void* base, const cuuint64_t* dims, const cuuint64_t* strides,
+                      const cuuint32_t* box, const cuuint32_t* estr) {
+  static PFN_encodeTiled enc = [] {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    return (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
+            q == cudaDriverEntryPointSuccess) ? reinterpret_cast<PFN_encodeTiled>(f) : nullptr;
+  }();
+  if (!enc) { set_error("cuTensorMapEncodeTiled entry point not available"); return XVB_ECUDA; }
+  const CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), dims, strides, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("cuTensorMapEncodeTiled(position map C=%llu F=%llu T=%llu B=%llu) failed: %d", (unsigned long long)dims[0],
+              (unsigned long long)dims[1], (unsigned long long)dims[2], (unsigned long long)dims[3], (int)r);
+    return XVB_ECUDA;
+  }
+  return XVB_OK;
+}
+
+template <int BLOCK_N>
+int launch_conv(const CUtensorMap* mx, Conv2dParams& p, const void* w_hi, const void* w_lo, cudaStream_t stream) {
+  using Cfg = ConvCfg<BLOCK_N>;
+  CUtensorMap mw_hi, mw_lo;   // packed (Cout, k*k*Cin) weight, K contiguous; box 64 x BLOCK_N
+  const unsigned long long K = (unsigned long long)p.ks * p.ks * p.cin_p16;
+  const unsigned long long wd[2] = {K, (unsigned long long)p.Cout};
+  const unsigned long long ws[1] = {K * 2};
+  const unsigned wb[2] = {(unsigned)kBlockK, (unsigned)BLOCK_N};
+  int rc;
+  if ((rc = make_tensor_map(&mw_hi, w_hi, 2, 2, wd, ws, wb, 128))) return rc;
+  if ((rc = make_tensor_map(&mw_lo, w_lo, 2, 2, wd, ws, wb, 128))) return rc;
+  p.num_n_blk = (p.Cout + BLOCK_N - 1) / BLOCK_N;
+  const long long tiles = (long long)p.num_f_blk * p.num_t_blk * ((p.B + p.Bb - 1) / p.Bb) * p.num_n_blk;
+  XVB_CHECK_ARG(tiles < (1ll << 31), "xvb_conv2d: too many tiles for one launch");
+  p.num_tiles = (int)tiles;
+  const int sms = sm_count();
+  XVB_ENSURE_DYN_SMEM(conv2d_bf16x3_kernel<BLOCK_N>, Cfg::kSmemBytes);
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(p.num_tiles < sms ? p.num_tiles : sms);
+  cfg.blockDim = dim3(kNumThreads);
+  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  XVB_CUDA(cudaLaunchKernelEx(&cfg, conv2d_bf16x3_kernel<BLOCK_N>, mx[0], mx[1], mw_hi, mw_lo, p));
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}
+
+}  // namespace
+}  // namespace xvb
+
+using namespace xvb;
+
+extern "C" int xvb_conv2d(const xvb_conv2d_args_t* a, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(a, "xvb_conv2d: null args");
+  XVB_CHECK_ARG(a->x_hi && a->x_lo && a->w_hi && a->w_lo, "xvb_conv2d: null operand pointer");
+  XVB_CHECK_ARG(a->B > 0 && a->T > 0 && a->F > 0 && a->Cin > 0 && a->Cout > 0,
+                "xvb_conv2d: bad shape B=%d T=%d F=%d Cin=%d Cout=%d", a->B, a->T, a->F, a->Cin, a->Cout);
+  XVB_CHECK_ARG(a->Cin % 16 == 0 && a->Cout % 16 == 0, "xvb_conv2d: Cin=%d and Cout=%d must be multiples of 16", a->Cin, a->Cout);
+  XVB_CHECK_ARG((a->ksize == 3 || a->ksize == 1) && (a->stride == 1 || a->stride == 2),
+                "xvb_conv2d: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
+  XVB_CHECK_ARG((a->y_hi != nullptr) == (a->y_lo != nullptr) && (a->res_hi != nullptr) == (a->res_lo != nullptr) &&
+                    (a->y2_hi != nullptr) == (a->y2_lo != nullptr),
+                "xvb_conv2d: hi/lo plane pointers must both be set or both NULL");
+  XVB_CHECK_ARG(a->y_hi || a->y_f32 || a->y2_hi, "xvb_conv2d: no output requested");
+  XVB_CHECK_ARG((a->scale != nullptr) == (a->shift != nullptr), "xvb_conv2d: scale and shift must both be set or both NULL");
+  XVB_CHECK_ARG(!a->y2_hi || (a->scale2 && a->shift2), "xvb_conv2d: the second output needs scale2 and shift2");
+  XVB_CHECK_ARG(((uintptr_t)a->x_hi | (uintptr_t)a->x_lo | (uintptr_t)a->w_hi | (uintptr_t)a->w_lo | (uintptr_t)a->res_hi |
+                 (uintptr_t)a->res_lo | (uintptr_t)a->y_hi | (uintptr_t)a->y_lo | (uintptr_t)a->y_f32 | (uintptr_t)a->y2_hi |
+                 (uintptr_t)a->y2_lo) % 16 == 0,
+                "xvb_conv2d: pointers must be 16-byte aligned");
+  Conv2dParams p{};
+  p.B = a->B; p.T = a->T; p.F = a->F; p.Cin = a->Cin; p.Cout = a->Cout;
+  p.ks = a->ksize; p.stride = a->stride; p.pad = a->ksize / 2;
+  p.To = (a->T - 1) / a->stride + 1;   // (T + 2p - k) / s + 1 with p = k / 2: ceil(T / s) for k = 1 and k = 3
+  p.Fo = (a->F - 1) / a->stride + 1;
+  choose_conv_tile(p.B, p.To, p.Fo, p.stride, &p.Fb, &p.Tb, &p.Bb);
+  p.log2_fb = 0;
+  while ((1 << p.log2_fb) < p.Fb) ++p.log2_fb;
+  p.log2_tb = 0;
+  while ((1 << p.log2_tb) < p.Tb) ++p.log2_tb;
+  p.num_f_blk = (p.Fo + p.Fb - 1) / p.Fb;
+  p.num_t_blk = (p.To + p.Tb - 1) / p.Tb;
+  p.cin_p16 = p.Cin;
+  p.num_cblk = (p.Cin + kBlockK - 1) / kBlockK;
+  p.relu = a->relu ? 1 : 0;
+  p.scale = a->scale; p.shift = a->shift;
+  p.res_hi = reinterpret_cast<const __nv_bfloat16*>(a->res_hi);
+  p.res_lo = reinterpret_cast<const __nv_bfloat16*>(a->res_lo);
+  p.y_hi = reinterpret_cast<__nv_bfloat16*>(a->y_hi);
+  p.y_lo = reinterpret_cast<__nv_bfloat16*>(a->y_lo);
+  p.y_f32 = a->y_f32;
+  p.scale2 = a->scale2; p.shift2 = a->shift2;
+  p.y2_hi = reinterpret_cast<__nv_bfloat16*>(a->y2_hi);
+  p.y2_lo = reinterpret_cast<__nv_bfloat16*>(a->y2_lo);
+
+  // input (B, T, F, Cin) planes as a 4-D tensor map (C, F, T, B); box 64 channels x Fb x Tb x Bb output positions
+  CUtensorMap mx[2];
+  const cuuint64_t C = (cuuint64_t)p.Cin;
+  const cuuint64_t dims[4] = {C, (cuuint64_t)p.F, (cuuint64_t)p.T, (cuuint64_t)p.B};
+  const cuuint64_t strides[3] = {C * 2, C * 2 * p.F, C * 2 * p.F * p.T};
+  const cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)(p.Fb * p.stride), (cuuint32_t)(p.Tb * p.stride), (cuuint32_t)p.Bb};
+  const cuuint32_t estr[4] = {1u, (cuuint32_t)p.stride, (cuuint32_t)p.stride, 1u};
+  if ((rc = make_position_map(&mx[0], a->x_hi, dims, strides, box, estr))) return rc;
+  if ((rc = make_position_map(&mx[1], a->x_lo, dims, strides, box, estr))) return rc;
+
+  const long long m_tiles = (long long)p.num_f_blk * p.num_t_blk * ((p.B + p.Bb - 1) / p.Bb);
+  const int sms = sm_count();
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  if (p.Cout >= 128 && m_tiles * ((p.Cout + 127) / 128) >= sms) return launch_conv<128>(mx, p, a->w_hi, a->w_lo, s);
+  if (p.Cout >= 64 && m_tiles * ((p.Cout + 63) / 64) >= sms / 2) return launch_conv<64>(mx, p, a->w_hi, a->w_lo, s);
+  return launch_conv<32>(mx, p, a->w_hi, a->w_lo, s);
+}
+
+extern "C" int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,
+                               const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2,
+                               const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(x && w && bn_scale && bn_shift && y_hi && y_lo, "xvb_conv2d_head: null pointer");
+  XVB_CHECK_ARG(B > 0 && T > 0 && F > 0 && Cout > 0 && Cout % 8 == 0, "xvb_conv2d_head: bad shape B=%d T=%d F=%d Cout=%d", B, T, F, Cout);
+  XVB_CHECK_ARG((y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
+                "xvb_conv2d_head: the second output needs both planes, scale2 and shift2");
+  XVB_CHECK_ARG(((uintptr_t)y_hi | (uintptr_t)y_lo | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
+                "xvb_conv2d_head: planes must be 16-byte aligned");
+  const long long total = (long long)B * T * F * (Cout / 8);
+  head_conv_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      x, B, T, F, w, Cout, bn_scale, bn_shift, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
+      scale2, shift2, reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo));
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}
+
+extern "C" int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
+                               const uint16_t* id_lo, int B, int64_t P, int C, int relu, uint16_t* y_hi, uint16_t* y_lo,
+                               float* y_f32, const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo,
+                               void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(z_hi && z_lo && gate && id_hi && id_lo, "xvb_se_residual: null pointer");
+  XVB_CHECK_ARG(B > 0 && P > 0 && C > 0 && C % 8 == 0, "xvb_se_residual: bad shape B=%d P=%lld C=%d", B, (long long)P, C);
+  XVB_CHECK_ARG((y_hi != nullptr) == (y_lo != nullptr) && (y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
+                "xvb_se_residual: hi/lo planes must both be set or both NULL; the second output needs scale2 and shift2");
+  XVB_CHECK_ARG(y_hi || y_f32 || y2_hi, "xvb_se_residual: no output requested");
+  XVB_CHECK_ARG(((uintptr_t)z_hi | (uintptr_t)z_lo | (uintptr_t)gate | (uintptr_t)id_hi | (uintptr_t)id_lo | (uintptr_t)y_hi |
+                 (uintptr_t)y_lo | (uintptr_t)y_f32 | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
+                "xvb_se_residual: pointers must be 16-byte aligned");
+  const long long total = (long long)B * P * (C / 8);
+  se_residual_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(z_hi), reinterpret_cast<const __nv_bfloat16*>(z_lo), gate,
+      reinterpret_cast<const __nv_bfloat16*>(id_hi), reinterpret_cast<const __nv_bfloat16*>(id_lo), (long long)P, C, relu ? 1 : 0,
+      reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo), y_f32, scale2, shift2,
+      reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo), total);
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}

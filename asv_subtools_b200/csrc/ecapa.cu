@@ -12,28 +12,6 @@
 
 namespace xvb {
 
-__device__ __forceinline__ void unpack8(const uint4& h, const uint4& l, float (&f)[8]) {
-  const uint32_t hw[4] = {h.x, h.y, h.z, h.w}, lw[4] = {l.x, l.y, l.z, l.w};
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    f[2 * k] = __uint_as_float(hw[k] << 16) + __uint_as_float(lw[k] << 16);
-    f[2 * k + 1] = __uint_as_float(hw[k] & 0xffff0000u) + __uint_as_float(lw[k] & 0xffff0000u);
-  }
-}
-__device__ __forceinline__ void pack8(const float (&f)[8], uint4& h, uint4& l) {
-  uint32_t hw[4], lw[4];
-#pragma unroll
-  for (int k = 0; k < 4; ++k) {
-    __nv_bfloat16 h0, l0, h1, l1;
-    split_bf16(f[2 * k], h0, l0);
-    split_bf16(f[2 * k + 1], h1, l1);
-    hw[k] = pack_bf16x2(h0, h1);
-    lw[k] = pack_bf16x2(l0, l1);
-  }
-  h = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-  l = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-}
-
 // ---------------------------------------------------------------- mean over T of planes
 constexpr int kPmWarps = 8;
 __global__ void __launch_bounds__(kPmWarps * 32)

@@ -189,6 +189,62 @@ def se_apply(z, xin, gate, out, nxt=None):
                            nxt.ld if nxt else 0, b, t, c, _stream()), "xvb_se_apply")
 
 
+def _planes_ptrs(p):
+    return (p.hi.data_ptr(), p.lo.data_ptr()) if p is not None else (None, None)
+
+
+def pack_conv2d_weight(weight):
+    """Reference Conv2d weight (Cout, Cin, k, k) fp32 CUDA -> packed K-major SplitPlanes (tap = kf*k + kt)."""
+    weight = _req(weight, torch.float32, "weight")
+    cout, cin, kf, kt = weight.shape
+    if kf != kt:
+        raise ValueError("square kernels only, got {}x{}".format(kf, kt))
+    return pack_tdnn_weight(weight.reshape(cout, cin, kf * kt).contiguous(), list(range(kf * kt)))
+
+
+def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=False, y=None, y_f32=None,
+           scale2=None, shift2=None, y2=None):
+    """One 2-D convolution (xvb_conv2d): x SplitPlanes (B, T, F, Cin); w from pack_conv2d_weight; res / y / y2
+    SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride)."""
+    b, t, f, cin = x.hi.shape
+    a = _lib.Conv2dArgs()
+    a.x_hi, a.x_lo = _planes_ptrs(x)
+    a.w_hi, a.w_lo = w.hi.data_ptr(), w.lo.data_ptr()
+    a.B, a.T, a.F, a.Cin, a.Cout, a.ksize, a.stride = b, t, f, cin, cout, ksize, stride
+    for name, v in (("scale", scale), ("shift", shift), ("scale2", scale2), ("shift2", shift2)):
+        if v is not None:
+            setattr(a, name, _req(v, torch.float32, name).data_ptr())
+    a.res_hi, a.res_lo = _planes_ptrs(res)
+    a.relu = 1 if relu else 0
+    a.y_hi, a.y_lo = _planes_ptrs(y)
+    a.y2_hi, a.y2_lo = _planes_ptrs(y2)
+    if y_f32 is not None:
+        a.y_f32 = _req(y_f32, torch.float32, "y_f32").data_ptr()
+    check(lib.xvb_conv2d(C.byref(a), _stream()), "xvb_conv2d")
+
+
+def conv2d_head(feats, weight, scale, shift, y, scale2=None, shift2=None, y2=None):
+    """Head conv (xvb_conv2d_head): feats (B, T, F) fp32, weight (Cout, 1, 3, 3) fp32 -> y = relu(bn(conv)) SplitPlanes
+    (B, T, F, Cout) [, y2 = relu(y * scale2 + shift2)]."""
+    feats = _req(feats, torch.float32, "feats")
+    weight = _req(weight, torch.float32, "weight")
+    b, t, f = feats.shape
+    y2h, y2l = _planes_ptrs(y2)
+    check(lib.xvb_conv2d_head(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], _ptr(scale), _ptr(shift), y.hi.data_ptr(),
+                              y.lo.data_ptr(), _ptr(scale2), _ptr(shift2), y2h, y2l, _stream()), "xvb_conv2d_head")
+
+
+def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, shift2=None, y2=None):
+    """y = [relu](z * gate[b] + identity) over SplitPlanes (B, ..., C) (xvb_se_residual); gate (B, C) fp32."""
+    b, c = z.hi.shape[0], z.hi.shape[-1]
+    gate = _req(gate, torch.float32, "gate")
+    yh, yl = _planes_ptrs(y)
+    y2h, y2l = _planes_ptrs(y2)
+    check(lib.xvb_se_residual(z.hi.data_ptr(), z.lo.data_ptr(), _ptr(gate), identity.hi.data_ptr(), identity.lo.data_ptr(), b,
+                              z.hi.numel() // (b * c), c, 1 if relu else 0, yh, yl, _ptr(y_f32), _ptr(scale2), _ptr(shift2),
+                              y2h, y2l, _stream()), "xvb_se_residual")
+
+
 def stats_pool_ex(x, eps, mode, planes=False):
     """mode 0: StatisticsPooling; mode 1: ECAPA global context (unbiased var + eps)."""
     x = _req(x, torch.float32, "x")

@@ -232,6 +232,51 @@ int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, int G, cons
                                    int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * ResNet x-vector, 2-D (pytorch/model/resnet_xvector.py over pytorch/libs/nnet/resnet.py, BasicBlock)
+ *
+ * The reference convolves (B, 1, F, T): the conv "H" axis is the feature axis, "W" is time.  Position
+ * tensors here are channel-contiguous (B, T, F, C) with row pitch C (dense); every conv pads by k/2
+ * with zeros outside [0,F) x [0,T) of its own utterance and outputs ceil(F/s) x ceil(T/s) positions.
+ * ------------------------------------------------------------------------------------------- */
+
+/* Conv2d(Cin, Cout, k, stride s, padding k/2, bias=False) (resnet.py:12-20) on the wgmma kernel, split-plane
+ * numerics as xvb_tdnn_affine_ex, with the block epilogues of BasicBlock (resnet.py:70-104):
+ *   y  = [relu]( acc * scale[n] + shift[n]  [+ res] )      scale/shift: eval BatchNorm2d (NULL: none)
+ *   y2 = relu( y * scale2[n] + shift2[n] )                 the next pre-activation block's bn1 + relu1
+ * x: (B, T, F, Cin) planes; w: xvb_pack_tdnn_weight of the weight (Cout, Cin, k, k) viewed as (Cout, Cin, k*k)
+ * with context 0..k*k-1 (tap = kf*k + kt); res, y, y2: (B, T', F', Cout) planes; y_f32 the same in fp32.
+ * k in {1, 3}, s in {1, 2}, Cin % 16 == 0, Cout % 16 == 0, pointers 16-byte aligned.  Zero-initialise the struct;
+ * unused pointers stay NULL; at least one of y, y_f32, y2 is required. */
+typedef struct xvb_conv2d_args {
+  const uint16_t* x_hi; const uint16_t* x_lo;
+  const uint16_t* w_hi; const uint16_t* w_lo;
+  int B, T, F, Cin, Cout, ksize, stride;
+  const float* scale; const float* shift;
+  const uint16_t* res_hi; const uint16_t* res_lo;
+  int relu;
+  uint16_t* y_hi; uint16_t* y_lo;
+  float* y_f32;
+  const float* scale2; const float* shift2;
+  uint16_t* y2_hi; uint16_t* y2_lo;
+} xvb_conv2d_args_t;
+int xvb_conv2d(const xvb_conv2d_args_t* args, void* stream);
+
+/* The head of ResNet._forward_impl (resnet.py:353-358): Conv2d(1, Cout, 3, 1, 1, bias=False) -> BatchNorm2d ->
+ * ReLU on fp32 CUDA cores, straight from the (B, T, F) fp32 features (the unsqueeze of resnet_xvector.py:191 is
+ * only a view).  w: (Cout, 1, 3, 3) fp32 as stored; y: (B, T, F, Cout) planes; y2 (optional) = relu(y * scale2 +
+ * shift2), the first pre-activation block's bn1 + relu1.  Cout % 8 == 0. */
+int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,
+                    const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2, const float* shift2,
+                    uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+
+/* y = [relu]( z * gate[b, c] + id ) over (B, P, C) planes (P positions per utterance): SEBlock_2D's scaling
+ * (components.py:630-639) followed by BasicBlock's residual add (resnet.py:80-85 with relu, :100-104 without).
+ * gate: (B, C) fp32 (the sigmoid output of the SE block); y planes and/or y_f32; y2 as in xvb_conv2d.  C % 8 == 0. */
+int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
+                    const uint16_t* id_lo, int B, int64_t P, int C, int relu, uint16_t* y_hi, uint16_t* y_lo, float* y_f32,
+                    const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Feature-side front-end (SURVEY 8f rank 1) on a ragged batch: utterance u owns rows
  * offsets[u] .. offsets[u+1] of the (sum_T, F) fp32 matrix x.
  * ------------------------------------------------------------------------------------------- */
