@@ -150,6 +150,19 @@ SIGNATURES = {
     "xvb_ecapa_save": (_i, [_p, C.c_char_p]),
     "xvb_ecapa_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_ecapa_destroy": (None, [_p]),
+    "xvb_resnet_create": (_i, [C.POINTER(_p), _i, _ip, _ip, _i, _f]),
+    "xvb_resnet_set_layer": (_i, [_p, C.c_char_p, _i, _i, _i, _p, _p, _p, _p, _i]),
+    "xvb_resnet_finalize": (_i, [_p]),
+    "xvb_resnet_feat_dim": (_i, [_p]),
+    "xvb_resnet_embed_dim": (_i, [_p]),
+    "xvb_resnet_last_launches": (_i, [_p]),
+    "xvb_resnet_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_resnet_extract_host": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_resnet_extract_shard": (_i, [_p, _p, C.c_int64, _i, _i, _p, _p]),
+    "xvb_resnet_extract_shard_host": (_i, [_p, _p, C.c_int64, _i, _i, _p, _p]),
+    "xvb_resnet_save": (_i, [_p, C.c_char_p]),
+    "xvb_resnet_load": (_i, [C.POINTER(_p), C.c_char_p]),
+    "xvb_resnet_destroy": (None, [_p]),
     "xvb_extractor_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_extractor_feat_dim": (_i, [C.c_char_p]),
     "xvb_ark_reader_open": (_i, [C.POINTER(_p), C.c_char_p]),

@@ -14,7 +14,9 @@
 // :17-45: <model-path> <feats-rspecifier> <vectors-wspecifier>); the role is that of the reference's
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
-// the input side.  What it adds: utterances of equal length are batched (the reference runs batch 1).
+// the input side.  The model file is any of the three families, told apart by its magic: TDNN x-vector
+// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001) or 2-D ResNet x-vector (XVBR0001, the extractors'
+// save()).  What it adds: utterances of equal length are batched (the reference runs batch 1).
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32;
 //   * one "FV" vector per input key (order follows batch completion, which the wspecifier allows);
@@ -57,7 +59,8 @@ struct Utt {
 
 struct Runner {
   xvb_extractor_t* ex = nullptr;   // TDNN x-vector family (XVBM0001) ...
-  xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001)
+  xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001) ...
+  xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001)
   xvb_ark_writer_t* out = nullptr;
   int F = 0, D = 0, batch = 256, cmn = 0, cmn_window = 300;
   float *d_feats = nullptr, *d_tmp = nullptr, *d_emb = nullptr, *h_feats = nullptr, *h_emb = nullptr;
@@ -88,7 +91,8 @@ struct Runner {
     for (int i = 0; i < B; ++i) memcpy(h_feats + (size_t)i * T * F, items[i].feats.data(), (size_t)T * F * sizeof(float));
     CU(cudaMemcpy(d_feats, h_feats, (size_t)B * T * F * sizeof(float), cudaMemcpyHostToDevice));
     if (ex) CK(xvb_extractor_extract(ex, d_feats, B, T, d_emb, nullptr), "xvb_extractor_extract");
-    else CK(xvb_ecapa_extract(ec, d_feats, B, T, d_emb, nullptr), "xvb_ecapa_extract");
+    else if (ec) CK(xvb_ecapa_extract(ec, d_feats, B, T, d_emb, nullptr), "xvb_ecapa_extract");
+    else CK(xvb_resnet_extract(rn, d_feats, B, T, d_emb, nullptr), "xvb_resnet_extract");
     CU(cudaMemcpy(h_emb, d_emb, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToHost));
     for (int i = 0; i < B; ++i) {
       Utt& u = utts[items[i].utt];
@@ -183,7 +187,9 @@ int main(int argc, char** argv) {
       printf("usage: xvb-extract [--batch N] [--max-chunk N] [--cmn none|utt|sliding] [--cmn-window W] [--gpu-id ID]\n"
              "                   [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
-             "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n");
+             "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001) or 2-D ResNet x-vector (XVBR0001) model,\n"
+             "recognised by its magic.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -208,6 +214,10 @@ int main(int argc, char** argv) {
       CK(xvb_ecapa_load(&r.ec, pos[0]), "loading the ECAPA model");
       r.F = xvb_ecapa_feat_dim(r.ec);
       r.D = xvb_ecapa_embed_dim(r.ec);
+    } else if (memcmp(magic, "XVBR0001", 8) == 0) {
+      CK(xvb_resnet_load(&r.rn, pos[0]), "loading the ResNet model");
+      r.F = xvb_resnet_feat_dim(r.rn);
+      r.D = xvb_resnet_embed_dim(r.rn);
     } else {
       CK(xvb_extractor_load(&r.ex, pos[0]), "loading the model");
       r.F = xvb_extractor_feat_dim(pos[0]);
@@ -326,6 +336,7 @@ int main(int argc, char** argv) {
   CK(xvb_ark_writer_close(r.out), "closing the vector wspecifier");
   if (r.ex) xvb_extractor_destroy(r.ex);
   if (r.ec) xvb_ecapa_destroy(r.ec);
+  if (r.rn) xvb_resnet_destroy(r.rn);
   fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
   return 0;
 }

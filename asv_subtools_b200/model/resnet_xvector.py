@@ -12,7 +12,11 @@ Every convolution runs on the 2-D wgmma kernel (csrc/conv2d.cu, xvb_conv2d) with
 add and the next pre-activation block's BN-ReLU in its epilogue; the head conv and the SE scaling have kernels of their
 own; pooling and fc1 / fc2 reuse the TDNN path's kernels.  Activations stay channel-contiguous (B, T, F, C) split planes
 throughout, so the reshape before pooling (:193, pooled channel c*F' + f) becomes a permutation of the input columns of
-the first segment layer, made once when the weights are handed over."""
+the first segment layer, made once when the weights are handed over.
+
+The launch sequence runs in the native handle (NativeResNetExtractor over xvb_resnet_*, csrc/resnet_extractor.cu), which
+also writes XVBR0001 model files for bin/xvb-extract.  XVB_RESNET_NATIVE=0 selects ResNetExtractor, the Python driver of
+the same kernels in the same order, whose embeddings are bit-identical."""
 import copy
 import os
 import sys
@@ -162,7 +166,10 @@ class ResNetXvector(TopVirtualNnet):
             raise ValueError("extracted_embedding='far' needs fc1=True (resnet_xvector.py:196-198 asserts it)")
         if self.extracted_embedding not in ("far", "near_affine", "near"):
             raise TypeError("Expected far or near position, but got {}".format(self.extracted_embedding))
-        return ResNetExtractor(self, self.device_for_extraction())
+        dev = self.device_for_extraction()
+        if os.environ.get("XVB_RESNET_NATIVE", "1") == "0":
+            return ResNetExtractor(self, dev)       # op-by-op twin of the native handle
+        return NativeResNetExtractor(self, dev)
 
 
 def _stats_column_order(c, f):
@@ -170,6 +177,64 @@ def _stats_column_order(c, f):
     reshape (B, C*F', T') (:193, column c*F' + f): out[:, j] = ref[:, perm[j]]."""
     half = np.arange(c * f).reshape(c, f).T.reshape(-1)
     return np.concatenate([half, half + c * f])
+
+
+def _segment_chain(m):
+    """The segment layers the extracted position uses (:194-206) as (name, layer, w, b, scale, shift, relu): "far" =
+    fc1.affine alone, otherwise [fc1 whole ->] fc2 whole ("near") or fc2.affine ("near_affine"); whole layers through
+    export() (BatchNorm folded to scale / shift, or into the weight for "bn-relu"), the first layer's input columns
+    permuted to the pooling order of (B, T', F', C) frames.  Shared by ResNetExtractor and the native handle."""
+    r = m.resnet
+    perm = torch.from_numpy(_stats_column_order(r.blocks()[-1].conv2.out_channels, m.out_freq))
+    pos = m.extracted_embedding
+    chain = ([("fc1", m.fc1, pos != "far")] if m.fc1 is not None else []) + \
+            ([("fc2", m.fc2, pos == "near")] if pos != "far" else [])
+    out = []
+    for i, (name, layer, full) in enumerate(chain):
+        if full:
+            w, b, scale, shift, relu = layer.export()
+        else:
+            w, b, scale, shift, relu = layer.affine.dense_weight(), layer.affine.bias.detach().float(), None, None, False
+        if i == 0:
+            w = w[:, perm]
+        out.append((name, layer, w.contiguous(), b, scale, shift, relu))
+    return out
+
+
+def _named_records(m):
+    """(name, w, bias, scale, shift, relu) records for xvb_resnet_set_layer, named by state_dict module path:
+    convolution weights as stored (Cout, Cin, k, k), BatchNorm folded to (scale, shift) with no weight, the SE linears
+    as stored, and the segment layers of _segment_chain with their (Cout, Cin, 1) weight as (Cout, Cin).  The library
+    only packs and pads these."""
+    f = lambda t: t.detach().float().cpu().numpy()  # noqa: E731
+    r = m.resnet
+    out = []
+
+    def conv(name, c):
+        out.append((name, f(c.weight), None, None, None, False))
+
+    def bn(name, b):
+        scale, shift = fold_batchnorm(b)
+        out.append((name, None, None, scale, shift, False))
+
+    conv("resnet.conv1", r.conv1)
+    bn("resnet.bn1", r.bn1)
+    for li in range(1, 5):
+        for i, blk in enumerate(getattr(r, "layer{}".format(li))):
+            p = "resnet.layer{}.{}.".format(li, i)
+            conv(p + "conv1", blk.conv1)
+            bn(p + "bn1", blk.bn1)
+            conv(p + "conv2", blk.conv2)
+            bn(p + "bn2", blk.bn2)
+            if blk.downsample is not None:
+                conv(p + "downsample.0", blk.downsample[0])
+                bn(p + "downsample.1", blk.downsample[1])
+            if blk.se is not None:
+                out.append((p + "se.fc_1", f(blk.se.fc_1.weight), f(blk.se.fc_1.bias), None, None, False))
+                out.append((p + "se.fc_2", f(blk.se.fc_2.weight), f(blk.se.fc_2.bias), None, None, False))
+    for name, _, w, b, scale, shift, relu in _segment_chain(m):
+        out.append((name, f(w)[:, :, 0], f(b) if b is not None else None, scale, shift, relu))
+    return out
 
 
 def _se_rows(se, device):
@@ -217,19 +282,8 @@ class ResNetExtractor:
                 "ds": None if ds is None else (ops.pack_conv2d_weight(ds[0].weight.detach().float().to(device).contiguous()),
                                                bn(ds[1])),
                 "se": None if blk.se is None else _se_rows(blk.se, device)})
-        c, f = r.blocks()[-1].conv2.out_channels, m.out_freq
-        perm = torch.from_numpy(_stats_column_order(c, f))
-        pos = m.extracted_embedding
-        chain = ([(m.fc1, pos != "far")] if m.fc1 is not None else []) + ([(m.fc2, pos == "near")] if pos != "far" else [])
-        self.segment = []
-        for i, (layer, full) in enumerate(chain):
-            if full:
-                w, b, scale, shift, relu = layer.export()
-            else:
-                w, b, scale, shift, relu = layer.affine.dense_weight(), layer.affine.bias.detach().float(), None, None, False
-            if i == 0:
-                w = w[:, perm]
-            self.segment.append(_PackedAffine(layer.affine, device, relu=relu, arrays=(w.contiguous(), b, scale, shift)))
+        self.segment = [_PackedAffine(layer.affine, device, relu=relu, arrays=(w, b, scale, shift))
+                        for _, layer, w, b, scale, shift, relu in _segment_chain(m)]
         self.eps = m.stats.eps
         self.embed_dim = self.segment[-1].cout_real
 
@@ -302,6 +356,105 @@ class ResNetExtractor:
 
     def close(self):
         pass
+
+
+def _cuda_f32(feats, feat_dim):
+    if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
+        raise TypeError("feats must be a contiguous CUDA float32 tensor")
+    if feats.shape[2] != feat_dim:
+        raise ValueError("expected feature dim {}, got {}".format(feat_dim, feats.shape[2]))
+    return feats
+
+
+class NativeResNetExtractor:
+    """xvb_resnet_t: packed weights, workspace and the whole launch sequence of ResNetExtractor in the C library, on the
+    device that is current when it is built (or loaded from an XVBR0001 file)."""
+
+    def __init__(self, m=None, device=None, path=None):
+        import ctypes as C
+        from asv_subtools_b200._lib import check, int_array, lib
+        self._C, self._lib, self._check = C, lib, check
+        self._h = C.c_void_p()
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            if path is not None:
+                check(lib.xvb_resnet_load(C.byref(self._h), str(path).encode()), "xvb_resnet_load")
+            else:
+                r = m.resnet
+                stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
+                check(lib.xvb_resnet_create(C.byref(self._h), m.inputs_dim, int_array([len(s) for s in stages]),
+                                            int_array([s[0].conv1.out_channels for s in stages]),
+                                            1 if r.full_pre_activation else 0, float(m.stats.eps)), "xvb_resnet_create")
+                for name, w, b, scale, shift, relu in _named_records(m):
+                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
+                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
+                    cout = (w if w is not None else scale).shape[0]
+                    cin, k = (w.shape[1], w.shape[2] if w.ndim == 4 else 1) if w is not None else (0, 0)
+                    flags = (1 if relu else 0) | (2 if scale is not None else 0)
+                    check(lib.xvb_resnet_set_layer(self._h, name.encode(), cout, cin, k, *ptr, flags), "xvb_resnet_set_layer")
+                check(lib.xvb_resnet_finalize(self._h), "xvb_resnet_finalize")
+        self.feat_dim = lib.xvb_resnet_feat_dim(self._h)
+        self.embed_dim = lib.xvb_resnet_embed_dim(self._h)
+
+    @classmethod
+    def load(cls, path):
+        return cls(path=path)
+
+    def save(self, path):
+        self._check(self._lib.xvb_resnet_save(self._h, str(path).encode()), "xvb_resnet_save")
+
+    @property
+    def last_launches(self):
+        return self._lib.xvb_resnet_last_launches(self._h)
+
+    def _stream(self):
+        return self._C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA -> (B, embed_dim) fp32 CUDA, asynchronous on the current stream."""
+        B, T, _ = _cuda_f32(feats, self.feat_dim).shape
+        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
+        C = self._C
+        self._check(self._lib.xvb_resnet_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
+                                                 self._stream()), "xvb_resnet_extract")
+        return emb
+
+    def extract_host(self, feats_np):
+        """feats (B, T, F) float32 host array -> (B, D) float32 host array (H2D + D2H + one sync inside the call)."""
+        feats_np = np.ascontiguousarray(feats_np, dtype=np.float32)
+        b, t, f = feats_np.shape
+        if f != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
+        emb = np.empty((b, self.embed_dim), dtype=np.float32)
+        C = self._C
+        self._check(self._lib.xvb_resnet_extract_host(self._h, feats_np.ctypes.data_as(C.c_void_p), b, t,
+                                                      emb.ctypes.data_as(C.c_void_p), self._stream()), "xvb_resnet_extract_host")
+        return emb
+
+    def extract_shard(self, feats, batch=128, out=None):
+        """feats (N, T, F) fp32 CUDA -> (N, D): the whole shard in `batch`-utterance batches, one C call."""
+        n, t, _ = _cuda_f32(feats, self.feat_dim).shape
+        emb = out if out is not None else torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
+        C = self._C
+        self._check(self._lib.xvb_resnet_extract_shard(self._h, C.c_void_p(feats.data_ptr()), n, t, int(batch),
+                                                       C.c_void_p(emb.data_ptr()), self._stream()), "xvb_resnet_extract_shard")
+        return emb
+
+    def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=128):
+        """Pinned host feats (n, t, F) in, host embeddings (n, D) out; copies overlap the stack."""
+        C = self._C
+        self._check(self._lib.xvb_resnet_extract_shard_host(self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch),
+                                                            C.c_void_p(emb_ptr), self._stream()), "xvb_resnet_extract_shard_host")
+
+    def close(self):
+        h, self._h = self._h, None
+        if h:
+            self._lib.xvb_resnet_destroy(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 if __name__ == "__main__":

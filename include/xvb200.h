@@ -569,6 +569,55 @@ int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path);
 int xvb_ecapa_load(xvb_ecapa_t** out, const char* path);
 void xvb_ecapa_destroy(xvb_ecapa_t* h);
 
+/* ---------------------------------------------------------------------------------------------
+ * Whole-model extractor for the 2-D ResNet x-vector (pytorch/model/resnet_xvector.py, extract_embedding :183-208,
+ * BasicBlocks in either block order, optional SE, statistics pooling): the launch sequence of xvb_conv2d_head,
+ * xvb_conv2d, xvb_plane_mean / xvb_small_affine / xvb_se_residual, xvb_stats_pool_ex and xvb_tdnn_affine_ex in
+ * C++, with weights and workspace owned by the handle.  Bit-identical to the op-by-op Python driver of the same
+ * kernels (ResNetExtractor, XVB_RESNET_NATIVE=0).
+ *
+ * Records are named by their state_dict module path: "resnet.conv1", "resnet.bn1", "resnet.layerL.i.{conv1,bn1,
+ * conv2,bn2}", "resnet.layerL.0.downsample.{0,1}", "resnet.layerL.i.se.fc_{1,2}", "fc1", "fc2".  Convolutions:
+ * w_host (Cout, Cin, k, k) as stored, ksize k in {1, 3}, no bias; BatchNorm: ksize 0, Cin 0, w_host NULL, the eval
+ * BatchNorm folded to scale / shift; SE linears: ksize 1, w (Cout, Cin) with bias; segment layers "fc1" / "fc2": the
+ * ones the extracted position uses, ksize 1, weight (Cout, Cin) with bias, scale / shift (XVB_BN) and XVB_RELU as
+ * the layer applies them, the first one's input columns in the pooling order of (B, T', F', C) frames (column
+ * f*C + c of each [mean | std] half).  The library pads the SE hidden width to a multiple of 4 and the segment rows
+ * to a multiple of 8, and packs the convolutions itself.
+ *
+ * Workspace: grown to the largest (B, T) seen, then reused.  A call whose B*T*feat_dim exceeds 256*200*80
+ * positions runs as consecutive groups of max(1, floor(256*200*80 / (T*feat_dim))) utterances, so the workspace of
+ * one call stays within that budget (a single utterance longer than the budget is one group of its own).  At
+ * B = 128, T = 200, feat_dim = 80 with planes 32..256 it is about 1.9 GB: seven (B, T', F', C) plane pairs of
+ * 262 MB each, plus the last layer's fp32 output; the shard calls' second lane holds a second workspace.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct xvb_resnet xvb_resnet_t;
+/* layers, planes: four entries each (planes multiples of 16); pre_activation != 0: full_pre_activation blocks. */
+int xvb_resnet_create(xvb_resnet_t** out, int feat_dim, const int* layers, const int* planes, int pre_activation,
+                      float pooling_eps);
+int xvb_resnet_set_layer(xvb_resnet_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
+                         const float* bias_host, const float* scale_host, const float* shift_host, int flags);
+/* Checks that every record the configuration needs is present with its shape (and nothing else), names the one
+ * that is not, then packs the weights on the current device. */
+int xvb_resnet_finalize(xvb_resnet_t* h);
+int xvb_resnet_feat_dim(const xvb_resnet_t* h);
+int xvb_resnet_embed_dim(const xvb_resnet_t* h);
+/* Kernels launched by the last extract / shard call. */
+int xvb_resnet_last_launches(const xvb_resnet_t* h);
+/* feats (B, T, feat_dim) fp32 on the device -> emb (B, embed_dim) fp32 on the device; asynchronous. */
+int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* Same through host buffers (H2D of feats, D2H of emb inside; synchronises the stream). */
+int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream);
+/* Whole shard of N equal-length utterances in `batch`-utterance batches, as xvb_ecapa_extract_shard[_host]: batches
+ * alternate between two lanes (XVB_LANES=0: one), pinned host buffers are copied on a copy stream. */
+int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream);
+int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int64_t N, int T, int batch,
+                                  float* emb_host, void* stream);
+/* "XVBR0001" model files: the create arguments, then the records as handed to xvb_resnet_set_layer. */
+int xvb_resnet_save(const xvb_resnet_t* h, const char* path);
+int xvb_resnet_load(xvb_resnet_t** out, const char* path);
+void xvb_resnet_destroy(xvb_resnet_t* h);
+
 /* Load a finalized extractor from an .xvbm model file (written by asv_subtools_b200.ops.Extractor.save:
  * the layers exactly as the reference's state_dict stores them, eval BatchNorm folded) -- what
  * torch::jit::load does for the reference's runtime (runtime/extractor/torch_asv_model.cc:8-17). */
