@@ -114,6 +114,8 @@ SIGNATURES = {
     "xvb_trial_histogram": (_i, [_p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i, _i, _i, _f, _f, _i, _p, _p]),
     "xvb_conv2d": (_i, [_p, _p]),
     "xvb_conv2d_head": (_i, [_p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "xvb_conv2d_taps": (_i, [_p, _ip, _i, _p]),
+    "xvb_conv2d_head_k": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),

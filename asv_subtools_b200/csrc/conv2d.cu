@@ -5,8 +5,10 @@
 //
 // The reference feeds (1, 1, F, T) to Conv2d: "H" is the feature axis, "W" is time.  Here a frame tensor is a
 // channel-contiguous (B, T, F, C) split-plane pair, and the kernel reads it through a 4-D tensor map (C, F, T, B):
-//   * M = output positions, N = Cout, K = k*k taps x Cin, tap-major (the xvb_pack_tdnn_weight layout of the weight
-//     viewed as (Cout, Cin, k*k));
+//   * M = output positions, N = Cout, K = taps x Cin, tap-major (the xvb_pack_tdnn_weight layout of the weight
+//     viewed as (Cout, Cin, k*k) with the kept taps as context); the taps are a list of (kf, kt) offsets, all k*k of a
+//     dense window (xvb_conv2d) or any increasing subset of a k <= 5 window (xvb_conv2d_taps: a re-parameterised RepSPK
+//     block is a 5x5 kernel with 8 taps that are always zero, which then cost nothing);
 //   * an M tile is 128 positions = Bb utterances x Tb frames x Fb feature bins (powers of two, chosen on the host for
 //     the fewest padded rows); tap (kf, kt) is only a coordinate offset, so TMA's out-of-bounds zero fill is exactly
 //     the convolution's zero padding and never reads a neighbouring utterance;
@@ -35,10 +37,13 @@ constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB per plane per stage
 constexpr int kNumConsumers = 256;
 constexpr int kProducerWarp = kNumConsumers / 32;
 constexpr int kNumThreads = kNumConsumers + 32;
+constexpr int kMaxConvTaps = 25;                 // a 5x5 window
 
 struct Conv2dParams {
   int B, T, F, Cin, To, Fo, Cout;
   int ks, stride, pad;
+  int ntaps;
+  int8_t tap_f[kMaxConvTaps], tap_t[kMaxConvTaps];   // (kf, kt) of packed tap j
   int Fb, Tb, Bb, log2_fb, log2_tb;
   int num_f_blk, num_t_blk, num_n_blk, num_tiles;
   int cin_p16, num_cblk;
@@ -110,7 +115,7 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
   asm volatile("griddepcontrol.wait;" ::: "memory");
   asm volatile("fence.proxy.async;" ::: "memory");   // operands may come from generic-proxy stores of the previous kernel
 
-  const int num_kblk = p.ks * p.ks * p.num_cblk;
+  const int num_kblk = p.ntaps * p.num_cblk;
 
   if (warp == kProducerWarp) {
     if (lane == 0) {
@@ -120,21 +125,18 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
         int b0, t0, f0, n_blk;
         decode_conv_tile(p, tile, b0, t0, f0, n_blk);
         const int n0 = n_blk * BLOCK_N;
-        for (int kf = 0; kf < p.ks; ++kf) {
-          const int fi = f0 * p.stride + kf - p.pad;
-          for (int kt = 0; kt < p.ks; ++kt) {
-            const int ti = t0 * p.stride + kt - p.pad;
-            const int tap = kf * p.ks + kt;
-            for (int cb = 0; cb < p.num_cblk; ++cb) {
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              uint8_t* s = smem + stage * kStageBytes;
-              mbar_expect_tx(&full_bar[stage], kStageBytes);
-              tma_load_4d(s, &map_x_hi, &full_bar[stage], cb * kBlockK, fi, ti, b0);
-              tma_load_4d(s + kABytes, &map_x_lo, &full_bar[stage], cb * kBlockK, fi, ti, b0);
-              tma_load_2d(s + 2 * kABytes, &map_w_hi, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
-              tma_load_2d(s + 2 * kABytes + kBBytes, &map_w_lo, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
-              if (++stage == kStages) { stage = 0; phase ^= 1; }
-            }
+        for (int tap = 0; tap < p.ntaps; ++tap) {
+          const int fi = f0 * p.stride + p.tap_f[tap] - p.pad;
+          const int ti = t0 * p.stride + p.tap_t[tap] - p.pad;
+          for (int cb = 0; cb < p.num_cblk; ++cb) {
+            mbar_wait(&empty_bar[stage], phase ^ 1);
+            uint8_t* s = smem + stage * kStageBytes;
+            mbar_expect_tx(&full_bar[stage], kStageBytes);
+            tma_load_4d(s, &map_x_hi, &full_bar[stage], cb * kBlockK, fi, ti, b0);
+            tma_load_4d(s + kABytes, &map_x_lo, &full_bar[stage], cb * kBlockK, fi, ti, b0);
+            tma_load_2d(s + 2 * kABytes, &map_w_hi, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
+            tma_load_2d(s + 2 * kABytes + kBBytes, &map_w_lo, &full_bar[stage], tap * p.cin_p16 + cb * kBlockK, n0);
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
           }
         }
       }
@@ -234,9 +236,10 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
   }
 }
 
-// Head conv (Cin = 1, 3x3, stride 1, padding 1) on CUDA cores, fp32: its input rows (one value per position) break
-// TMA's 16-byte rule and it is ~0.1 % of the MACs.  One thread per (position, 8 output channels); fused BN + ReLU,
-// the split to planes and the optional second output relu(y * scale2 + shift2).
+// Head conv (Cin = 1, KxK with K = 3 or 5, stride 1, padding K/2) on CUDA cores, fp32: its input rows (one value per
+// position) break TMA's 16-byte rule and it is ~0.1 % of the MACs.  One thread per (position, 8 output channels);
+// fused BN + ReLU, the split to planes and the optional second output relu(y * scale2 + shift2).
+template <int K>
 __global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int F, const float* __restrict__ w, int Cout,
                                  const float* __restrict__ scale, const float* __restrict__ shift,
                                  __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl,
@@ -251,21 +254,21 @@ __global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int 
     const long long bt = pos / F;
     const int t = (int)(bt % T);
     const long long b = bt / T;
-    float in[9];
+    float in[K * K];
 #pragma unroll
-    for (int kf = 0; kf < 3; ++kf)
+    for (int kf = 0; kf < K; ++kf)
 #pragma unroll
-      for (int kt = 0; kt < 3; ++kt) {
-        const int ff = f + kf - 1, tt = t + kt - 1;
-        in[kf * 3 + kt] = (ff >= 0 && ff < F && tt >= 0 && tt < T) ? __ldg(x + (b * T + tt) * F + ff) : 0.f;
+      for (int kt = 0; kt < K; ++kt) {
+        const int ff = f + kf - K / 2, tt = t + kt - K / 2;
+        in[kf * K + kt] = (ff >= 0 && ff < F && tt >= 0 && tt < T) ? __ldg(x + (b * T + tt) * F + ff) : 0.f;
       }
     float y[8], y2[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
-      const float* wc = w + (c0 + k) * 9;
+      const float* wc = w + (c0 + k) * (K * K);
       float s = 0.f;
 #pragma unroll
-      for (int j = 0; j < 9; ++j) s = fmaf(__ldg(wc + j), in[j], s);
+      for (int j = 0; j < K * K; ++j) s = fmaf(__ldg(wc + j), in[j], s);
       y[k] = fmaxf(fmaf(s, __ldg(scale + c0 + k), __ldg(shift + c0 + k)), 0.f);
       if (y2h) y2[k] = fmaxf(fmaf(y[k], __ldg(scale2 + c0 + k), __ldg(shift2 + c0 + k)), 0.f);
     }
@@ -374,7 +377,7 @@ template <int BLOCK_N>
 int launch_conv(const CUtensorMap* mx, Conv2dParams& p, const void* w_hi, const void* w_lo, cudaStream_t stream) {
   using Cfg = ConvCfg<BLOCK_N>;
   CUtensorMap mw_hi, mw_lo;   // packed (Cout, k*k*Cin) weight, K contiguous; box 64 x BLOCK_N
-  const unsigned long long K = (unsigned long long)p.ks * p.ks * p.cin_p16;
+  const unsigned long long K = (unsigned long long)p.ntaps * p.cin_p16;
   const unsigned long long wd[2] = {K, (unsigned long long)p.Cout};
   const unsigned long long ws[1] = {K * 2};
   const unsigned wb[2] = {(unsigned)kBlockK, (unsigned)BLOCK_N};
@@ -402,35 +405,33 @@ int launch_conv(const CUtensorMap* mx, Conv2dParams& p, const void* w_hi, const 
   return XVB_OK;
 }
 
-}  // namespace
-}  // namespace xvb
-
-using namespace xvb;
-
-extern "C" int xvb_conv2d(const xvb_conv2d_args_t* a, void* stream) {
-  int rc = require_sm90();
-  if (rc) return rc;
-  XVB_CHECK_ARG(a, "xvb_conv2d: null args");
-  XVB_CHECK_ARG(a->x_hi && a->x_lo && a->w_hi && a->w_lo, "xvb_conv2d: null operand pointer");
+// Checks shared by xvb_conv2d and xvb_conv2d_taps (the window size and the tap list are checked by each), then the
+// launch.  taps: strictly increasing kf * ksize + kt, in the packed weight's order.
+int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int ntaps, void* stream) {
+  XVB_CHECK_ARG(a->x_hi && a->x_lo && a->w_hi && a->w_lo, "%s: null operand pointer", fn);
   XVB_CHECK_ARG(a->B > 0 && a->T > 0 && a->F > 0 && a->Cin > 0 && a->Cout > 0,
-                "xvb_conv2d: bad shape B=%d T=%d F=%d Cin=%d Cout=%d", a->B, a->T, a->F, a->Cin, a->Cout);
-  XVB_CHECK_ARG(a->Cin % 16 == 0 && a->Cout % 16 == 0, "xvb_conv2d: Cin=%d and Cout=%d must be multiples of 16", a->Cin, a->Cout);
-  XVB_CHECK_ARG((a->ksize == 3 || a->ksize == 1) && (a->stride == 1 || a->stride == 2),
-                "xvb_conv2d: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
+                "%s: bad shape B=%d T=%d F=%d Cin=%d Cout=%d", fn, a->B, a->T, a->F, a->Cin, a->Cout);
+  XVB_CHECK_ARG(a->Cin % 16 == 0 && a->Cout % 16 == 0, "%s: Cin=%d and Cout=%d must be multiples of 16", fn, a->Cin, a->Cout);
   XVB_CHECK_ARG((a->y_hi != nullptr) == (a->y_lo != nullptr) && (a->res_hi != nullptr) == (a->res_lo != nullptr) &&
                     (a->y2_hi != nullptr) == (a->y2_lo != nullptr),
-                "xvb_conv2d: hi/lo plane pointers must both be set or both NULL");
-  XVB_CHECK_ARG(a->y_hi || a->y_f32 || a->y2_hi, "xvb_conv2d: no output requested");
-  XVB_CHECK_ARG((a->scale != nullptr) == (a->shift != nullptr), "xvb_conv2d: scale and shift must both be set or both NULL");
-  XVB_CHECK_ARG(!a->y2_hi || (a->scale2 && a->shift2), "xvb_conv2d: the second output needs scale2 and shift2");
+                "%s: hi/lo plane pointers must both be set or both NULL", fn);
+  XVB_CHECK_ARG(a->y_hi || a->y_f32 || a->y2_hi, "%s: no output requested", fn);
+  XVB_CHECK_ARG((a->scale != nullptr) == (a->shift != nullptr), "%s: scale and shift must both be set or both NULL", fn);
+  XVB_CHECK_ARG(!a->y2_hi || (a->scale2 && a->shift2), "%s: the second output needs scale2 and shift2", fn);
   XVB_CHECK_ARG(((uintptr_t)a->x_hi | (uintptr_t)a->x_lo | (uintptr_t)a->w_hi | (uintptr_t)a->w_lo | (uintptr_t)a->res_hi |
                  (uintptr_t)a->res_lo | (uintptr_t)a->y_hi | (uintptr_t)a->y_lo | (uintptr_t)a->y_f32 | (uintptr_t)a->y2_hi |
                  (uintptr_t)a->y2_lo) % 16 == 0,
-                "xvb_conv2d: pointers must be 16-byte aligned");
+                "%s: pointers must be 16-byte aligned", fn);
+  int rc;
   Conv2dParams p{};
   p.B = a->B; p.T = a->T; p.F = a->F; p.Cin = a->Cin; p.Cout = a->Cout;
   p.ks = a->ksize; p.stride = a->stride; p.pad = a->ksize / 2;
-  p.To = (a->T - 1) / a->stride + 1;   // (T + 2p - k) / s + 1 with p = k / 2: ceil(T / s) for k = 1 and k = 3
+  p.ntaps = ntaps;
+  for (int j = 0; j < ntaps; ++j) {
+    p.tap_f[j] = (int8_t)(taps[j] / a->ksize);
+    p.tap_t[j] = (int8_t)(taps[j] % a->ksize);
+  }
+  p.To = (a->T - 1) / a->stride + 1;   // (T + 2p - k) / s + 1 with p = k / 2: ceil(T / s) for odd k
   p.Fo = (a->F - 1) / a->stride + 1;
   choose_conv_tile(p.B, p.To, p.Fo, p.stride, &p.Fb, &p.Tb, &p.Bb);
   p.log2_fb = 0;
@@ -470,23 +471,75 @@ extern "C" int xvb_conv2d(const xvb_conv2d_args_t* a, void* stream) {
   return launch_conv<32>(mx, p, a->w_hi, a->w_lo, s);
 }
 
+int conv2d_head_run(const char* fn, const float* x, int B, int T, int F, const float* w, int Cout, int ksize,
+                    const float* bn_scale, const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2,
+                    const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
+  XVB_CHECK_ARG(x && w && bn_scale && bn_shift && y_hi && y_lo, "%s: null pointer", fn);
+  XVB_CHECK_ARG(B > 0 && T > 0 && F > 0 && Cout > 0 && Cout % 8 == 0, "%s: bad shape B=%d T=%d F=%d Cout=%d", fn, B, T, F, Cout);
+  XVB_CHECK_ARG(ksize == 3 || ksize == 5, "%s: ksize must be 3 or 5 (got %d)", fn, ksize);
+  XVB_CHECK_ARG((y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
+                "%s: the second output needs both planes, scale2 and shift2", fn);
+  XVB_CHECK_ARG(((uintptr_t)y_hi | (uintptr_t)y_lo | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
+                "%s: planes must be 16-byte aligned", fn);
+  const long long total = (long long)B * T * F * (Cout / 8);
+  auto kernel = ksize == 5 ? head_conv_kernel<5> : head_conv_kernel<3>;
+  kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      x, B, T, F, w, Cout, bn_scale, bn_shift, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
+      scale2, shift2, reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo));
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}
+
+}  // namespace
+}  // namespace xvb
+
+using namespace xvb;
+
+extern "C" int xvb_conv2d(const xvb_conv2d_args_t* a, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(a, "xvb_conv2d: null args");
+  XVB_CHECK_ARG((a->ksize == 3 || a->ksize == 1) && (a->stride == 1 || a->stride == 2),
+                "xvb_conv2d: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
+  int dense[9];
+  for (int j = 0; j < a->ksize * a->ksize; ++j) dense[j] = j;
+  return conv2d_run("xvb_conv2d", a, dense, a->ksize * a->ksize, stream);
+}
+
+extern "C" int xvb_conv2d_taps(const xvb_conv2d_args_t* a, const int* taps, int ntaps, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(a, "xvb_conv2d_taps: null args");
+  XVB_CHECK_ARG((a->ksize == 1 || a->ksize == 3 || a->ksize == 5) && (a->stride == 1 || a->stride == 2),
+                "xvb_conv2d_taps: ksize must be 1, 3 or 5 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
+  XVB_CHECK_ARG(taps, "xvb_conv2d_taps: null tap list");
+  XVB_CHECK_ARG(ntaps >= 1 && ntaps <= a->ksize * a->ksize, "xvb_conv2d_taps: ntaps=%d outside [1, %d] for ksize %d", ntaps,
+                a->ksize * a->ksize, a->ksize);
+  for (int j = 0; j < ntaps; ++j) {
+    XVB_CHECK_ARG(taps[j] >= 0 && taps[j] < a->ksize * a->ksize, "xvb_conv2d_taps: tap %d = %d outside [0, %d)", j, taps[j],
+                  a->ksize * a->ksize);
+    XVB_CHECK_ARG(j == 0 || taps[j] > taps[j - 1], "xvb_conv2d_taps: taps must be strictly increasing (tap %d = %d after %d)",
+                  j, taps[j], taps[j - 1]);
+  }
+  return conv2d_run("xvb_conv2d_taps", a, taps, ntaps, stream);
+}
+
 extern "C" int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,
                                const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2,
                                const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
-  XVB_CHECK_ARG(x && w && bn_scale && bn_shift && y_hi && y_lo, "xvb_conv2d_head: null pointer");
-  XVB_CHECK_ARG(B > 0 && T > 0 && F > 0 && Cout > 0 && Cout % 8 == 0, "xvb_conv2d_head: bad shape B=%d T=%d F=%d Cout=%d", B, T, F, Cout);
-  XVB_CHECK_ARG((y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
-                "xvb_conv2d_head: the second output needs both planes, scale2 and shift2");
-  XVB_CHECK_ARG(((uintptr_t)y_hi | (uintptr_t)y_lo | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
-                "xvb_conv2d_head: planes must be 16-byte aligned");
-  const long long total = (long long)B * T * F * (Cout / 8);
-  head_conv_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      x, B, T, F, w, Cout, bn_scale, bn_shift, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
-      scale2, shift2, reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo));
-  XVB_LAUNCH_CHECK();
-  return XVB_OK;
+  return conv2d_head_run("xvb_conv2d_head", x, B, T, F, w, Cout, 3, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2, y2_hi,
+                         y2_lo, stream);
+}
+
+extern "C" int xvb_conv2d_head_k(const float* x, int B, int T, int F, const float* w, int Cout, int ksize,
+                                 const float* bn_scale, const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo,
+                                 const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  return conv2d_head_run("xvb_conv2d_head_k", x, B, T, F, w, Cout, ksize, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2,
+                         y2_hi, y2_lo, stream);
 }
 
 extern "C" int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,

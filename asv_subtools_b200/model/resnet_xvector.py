@@ -179,13 +179,15 @@ def _stats_column_order(c, f):
     return np.concatenate([half, half + c * f])
 
 
-def _segment_chain(m):
+def _segment_chain(m, channels=None):
     """The segment layers the extracted position uses (:194-206) as (name, layer, w, b, scale, shift, relu): "far" =
     fc1.affine alone, otherwise [fc1 whole ->] fc2 whole ("near") or fc2.affine ("near_affine"); whole layers through
     export() (BatchNorm folded to scale / shift, or into the weight for "bn-relu"), the first layer's input columns
-    permuted to the pooling order of (B, T', F', C) frames.  Shared by ResNetExtractor and the native handle."""
-    r = m.resnet
-    perm = torch.from_numpy(_stats_column_order(r.blocks()[-1].conv2.out_channels, m.out_freq))
+    permuted to the pooling order of (B, T', F', C) frames.  Shared by ResNetExtractor, the native handle and the
+    RepVGG blueprint, which passes the channel count of its last stage (default: the ResNet's last conv2)."""
+    if channels is None:
+        channels = m.resnet.blocks()[-1].conv2.out_channels
+    perm = torch.from_numpy(_stats_column_order(channels, m.out_freq))
     pos = m.extracted_embedding
     chain = ([("fc1", m.fc1, pos != "far")] if m.fc1 is not None else []) + \
             ([("fc2", m.fc2, pos == "near")] if pos != "far" else [])

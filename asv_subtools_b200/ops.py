@@ -193,19 +193,34 @@ def _planes_ptrs(p):
     return (p.hi.data_ptr(), p.lo.data_ptr()) if p is not None else (None, None)
 
 
-def pack_conv2d_weight(weight):
-    """Reference Conv2d weight (Cout, Cin, k, k) fp32 CUDA -> packed K-major SplitPlanes (tap = kf*k + kt)."""
+def pack_conv2d_weight(weight, taps=None):
+    """Reference Conv2d weight (Cout, Cin, k, k) fp32 CUDA -> packed K-major SplitPlanes (tap = kf*k + kt).  taps: the
+    strictly increasing tap list of conv2d(taps=...), packed in that order (None: all k*k taps)."""
     weight = _req(weight, torch.float32, "weight")
     cout, cin, kf, kt = weight.shape
     if kf != kt:
         raise ValueError("square kernels only, got {}x{}".format(kf, kt))
-    return pack_tdnn_weight(weight.reshape(cout, cin, kf * kt).contiguous(), list(range(kf * kt)))
+    if taps is None:
+        return pack_tdnn_weight(weight.reshape(cout, cin, kf * kt).contiguous(), list(range(kf * kt)))
+    taps = [int(j) for j in taps]
+    if not taps or any(j < 0 or j >= kf * kt for j in taps) or any(b <= a for a, b in zip(taps, taps[1:])):
+        raise ValueError("taps must be a strictly increasing list in [0, {}), got {}".format(kf * kt, taps))
+    # xvb_pack_tdnn_weight takes at most XVB_MAX_TAPS (16) taps per call; the packed rows are tap-major, so packing
+    # the list in pieces and concatenating the pieces along K gives the same layout
+    sel = weight.reshape(cout, cin, kf * kt)[:, :, taps]
+    pieces = [pack_tdnn_weight(sel[:, :, i:i + _lib.MAX_TAPS].contiguous(), list(range(min(_lib.MAX_TAPS, len(taps) - i))))
+              for i in range(0, len(taps), _lib.MAX_TAPS)]
+    if len(pieces) == 1:
+        return pieces[0]
+    return SplitPlanes(torch.cat([p.hi for p in pieces], 1).contiguous(), torch.cat([p.lo for p in pieces], 1).contiguous(), cin)
 
 
 def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=False, y=None, y_f32=None,
-           scale2=None, shift2=None, y2=None):
+           scale2=None, shift2=None, y2=None, taps=None):
     """One 2-D convolution (xvb_conv2d): x SplitPlanes (B, T, F, Cin); w from pack_conv2d_weight; res / y / y2
-    SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride)."""
+    SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride).
+    taps: only these taps (kf*ksize + kt, strictly increasing, ksize 1, 3 or 5) are computed, with w packed by
+    pack_conv2d_weight(weight, taps) (xvb_conv2d_taps)."""
     b, t, f, cin = x.hi.shape
     a = _lib.Conv2dArgs()
     a.x_hi, a.x_lo = _planes_ptrs(x)
@@ -220,18 +235,25 @@ def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=F
     a.y2_hi, a.y2_lo = _planes_ptrs(y2)
     if y_f32 is not None:
         a.y_f32 = _req(y_f32, torch.float32, "y_f32").data_ptr()
-    check(lib.xvb_conv2d(C.byref(a), _stream()), "xvb_conv2d")
+    if taps is None:
+        check(lib.xvb_conv2d(C.byref(a), _stream()), "xvb_conv2d")
+    else:
+        check(lib.xvb_conv2d_taps(C.byref(a), int_array(taps), len(taps), _stream()), "xvb_conv2d_taps")
 
 
 def conv2d_head(feats, weight, scale, shift, y, scale2=None, shift2=None, y2=None):
-    """Head conv (xvb_conv2d_head): feats (B, T, F) fp32, weight (Cout, 1, 3, 3) fp32 -> y = relu(bn(conv)) SplitPlanes
-    (B, T, F, Cout) [, y2 = relu(y * scale2 + shift2)]."""
+    """Head conv (xvb_conv2d_head_k): feats (B, T, F) fp32, weight (Cout, 1, k, k) fp32 with k = 3 or 5 -> y =
+    relu(bn(conv)) SplitPlanes (B, T, F, Cout) [, y2 = relu(y * scale2 + shift2)]."""
     feats = _req(feats, torch.float32, "feats")
     weight = _req(weight, torch.float32, "weight")
     b, t, f = feats.shape
+    k = weight.shape[-1]
     y2h, y2l = _planes_ptrs(y2)
-    check(lib.xvb_conv2d_head(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], _ptr(scale), _ptr(shift), y.hi.data_ptr(),
-                              y.lo.data_ptr(), _ptr(scale2), _ptr(shift2), y2h, y2l, _stream()), "xvb_conv2d_head")
+    args = (_ptr(scale), _ptr(shift), y.hi.data_ptr(), y.lo.data_ptr(), _ptr(scale2), _ptr(shift2), y2h, y2l, _stream())
+    if k == 3:
+        check(lib.xvb_conv2d_head(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], *args), "xvb_conv2d_head")
+    else:
+        check(lib.xvb_conv2d_head_k(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], k, *args), "xvb_conv2d_head_k")
 
 
 def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, shift2=None, y2=None):

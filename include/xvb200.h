@@ -261,6 +261,14 @@ typedef struct xvb_conv2d_args {
 } xvb_conv2d_args_t;
 int xvb_conv2d(const xvb_conv2d_args_t* args, void* stream);
 
+/* xvb_conv2d over a list of taps: only the taps in `taps` (host array, tap = kf*ksize + kt, strictly increasing,
+ * 1 <= ntaps <= ksize*ksize) are computed; the others count as zero weights.  ksize in {1, 3, 5}, padding ksize/2,
+ * output ceil(T/s) x ceil(F/s) as in xvb_conv2d.  w: xvb_pack_tdnn_weight of the weight viewed as (Cout, Cin, k*k)
+ * with the tap list as context (packed tap j = taps[j]).  A re-parameterised RepSPK block (pytorch/libs/nnet/repvgg.py
+ * RepSPKBlock) is a 5x5 kernel whose 8 off-pattern taps are zero: it runs with the other 17.  The dense list
+ * 0..k*k-1 with ksize 1 or 3 gives xvb_conv2d's output bit for bit. */
+int xvb_conv2d_taps(const xvb_conv2d_args_t* args, const int* taps, int ntaps, void* stream);
+
 /* The head of ResNet._forward_impl (resnet.py:353-358): Conv2d(1, Cout, 3, 1, 1, bias=False) -> BatchNorm2d ->
  * ReLU on fp32 CUDA cores, straight from the (B, T, F) fp32 features (the unsqueeze of resnet_xvector.py:191 is
  * only a view).  w: (Cout, 1, 3, 3) fp32 as stored; y: (B, T, F, Cout) planes; y2 (optional) = relu(y * scale2 +
@@ -268,6 +276,13 @@ int xvb_conv2d(const xvb_conv2d_args_t* args, void* stream);
 int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,
                     const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2, const float* shift2,
                     uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+
+/* xvb_conv2d_head with a KxK window, ksize in {3, 5}, padding ksize/2: w is (Cout, 1, k, k) fp32.  ksize 3 is
+ * xvb_conv2d_head.  A RepVGG / RepSPK stage0 block (Cin = 1) folds into this with bn_scale = 1 and bn_shift = its
+ * bias. */
+int xvb_conv2d_head_k(const float* x, int B, int T, int F, const float* w, int Cout, int ksize, const float* bn_scale,
+                      const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2, const float* shift2,
+                      uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
 
 /* y = [relu]( z * gate[b, c] + id ) over (B, P, C) planes (P positions per utterance): SEBlock_2D's scaling
  * (components.py:630-639) followed by BasicBlock's residual add (resnet.py:80-85 with relu, :100-104 without).
