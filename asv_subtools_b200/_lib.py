@@ -6,7 +6,8 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libxvb200.so")
 
-RELU, BN, SIGMOID, TANH = 1, 2, 4, 8
+RELU, BN, SIGMOID, TANH, SWISH = 1, 2, 4, 8, 16
+ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH = 0, 1, 2, 3
 
 
 class TdnnArgs(C.Structure):
@@ -32,6 +33,21 @@ class Conv2dArgs(C.Structure):
                 ("scale", C.c_void_p), ("shift", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
                 ("relu", C.c_int), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("y_f32", C.c_void_p),
                 ("scale2", C.c_void_p), ("shift2", C.c_void_p), ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p)]
+
+
+class LayerNormArgs(C.Structure):
+    """xvb_layer_norm_args_t (include/xvb200.h)."""
+    _fields_ = [("rows", C.c_int64), ("C", C.c_int), ("eps", C.c_float),
+                ("x", C.c_void_p), ("ldx", C.c_int64),
+                ("delta", C.c_void_p), ("ld_delta", C.c_int64), ("delta_scale", C.c_float),
+                ("table", C.c_void_p), ("table_rows", C.c_int),
+                ("x_out", C.c_void_p), ("ld_x_out", C.c_int64),
+                ("gamma", C.c_void_p), ("beta", C.c_void_p),
+                ("second", C.c_int),
+                ("gamma2", C.c_void_p), ("beta2", C.c_void_p),
+                ("act", C.c_int),
+                ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("ldy", C.c_int64),
+                ("y_f32", C.c_void_p), ("ldyf", C.c_int64)]
 
 
 class XvbError(RuntimeError):
@@ -116,6 +132,11 @@ SIGNATURES = {
     "xvb_conv2d_head": (_i, [_p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_taps": (_i, [_p, _ip, _i, _p]),
     "xvb_conv2d_head_k": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "xvb_conv2d_valid": (_i, [_p, _p]),
+    "xvb_subsample_head": (_i, [_p, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
+    "xvb_layer_norm": (_i, [_p, _p]),
+    "xvb_rope_attention": (_i, [_p, _i64, _i, _i, _i, _i, _p, _i, _f, _p, _p, _i64, _p]),
+    "xvb_conv_module": (_i, [_p, _i64, _i, _i, _i, _p, _p, _i, _p, _p, _i, _f, _i, _p, _p, _i64, _p]),
     "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),

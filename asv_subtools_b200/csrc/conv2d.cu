@@ -405,9 +405,10 @@ int launch_conv(const CUtensorMap* mx, Conv2dParams& p, const void* w_hi, const 
   return XVB_OK;
 }
 
-// Checks shared by xvb_conv2d and xvb_conv2d_taps (the window size and the tap list are checked by each), then the
-// launch.  taps: strictly increasing kf * ksize + kt, in the packed weight's order.
-int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int ntaps, void* stream) {
+// Checks shared by xvb_conv2d, xvb_conv2d_taps and xvb_conv2d_valid (the window size and the tap list are checked by
+// each), then the launch.  taps: strictly increasing kf * ksize + kt, in the packed weight's order.  pad: zero padding
+// on each side (ksize / 2, or 0 for xvb_conv2d_valid); the output is (T + 2 pad - k) / s + 1 x (F + 2 pad - k) / s + 1.
+int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int ntaps, int pad, void* stream) {
   XVB_CHECK_ARG(a->x_hi && a->x_lo && a->w_hi && a->w_lo, "%s: null operand pointer", fn);
   XVB_CHECK_ARG(a->B > 0 && a->T > 0 && a->F > 0 && a->Cin > 0 && a->Cout > 0,
                 "%s: bad shape B=%d T=%d F=%d Cin=%d Cout=%d", fn, a->B, a->T, a->F, a->Cin, a->Cout);
@@ -425,14 +426,16 @@ int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int 
   int rc;
   Conv2dParams p{};
   p.B = a->B; p.T = a->T; p.F = a->F; p.Cin = a->Cin; p.Cout = a->Cout;
-  p.ks = a->ksize; p.stride = a->stride; p.pad = a->ksize / 2;
+  XVB_CHECK_ARG(a->T + 2 * pad >= a->ksize && a->F + 2 * pad >= a->ksize, "%s: T=%d, F=%d shorter than the %dx%d window", fn,
+                a->T, a->F, a->ksize, a->ksize);
+  p.ks = a->ksize; p.stride = a->stride; p.pad = pad;
   p.ntaps = ntaps;
   for (int j = 0; j < ntaps; ++j) {
     p.tap_f[j] = (int8_t)(taps[j] / a->ksize);
     p.tap_t[j] = (int8_t)(taps[j] % a->ksize);
   }
-  p.To = (a->T - 1) / a->stride + 1;   // (T + 2p - k) / s + 1 with p = k / 2: ceil(T / s) for odd k
-  p.Fo = (a->F - 1) / a->stride + 1;
+  p.To = (a->T + 2 * pad - a->ksize) / a->stride + 1;   // with pad = k / 2: ceil(T / s) for odd k
+  p.Fo = (a->F + 2 * pad - a->ksize) / a->stride + 1;
   choose_conv_tile(p.B, p.To, p.Fo, p.stride, &p.Fb, &p.Tb, &p.Bb);
   p.log2_fb = 0;
   while ((1 << p.log2_fb) < p.Fb) ++p.log2_fb;
@@ -503,7 +506,7 @@ extern "C" int xvb_conv2d(const xvb_conv2d_args_t* a, void* stream) {
                 "xvb_conv2d: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
   int dense[9];
   for (int j = 0; j < a->ksize * a->ksize; ++j) dense[j] = j;
-  return conv2d_run("xvb_conv2d", a, dense, a->ksize * a->ksize, stream);
+  return conv2d_run("xvb_conv2d", a, dense, a->ksize * a->ksize, a->ksize / 2, stream);
 }
 
 extern "C" int xvb_conv2d_taps(const xvb_conv2d_args_t* a, const int* taps, int ntaps, void* stream) {
@@ -521,7 +524,20 @@ extern "C" int xvb_conv2d_taps(const xvb_conv2d_args_t* a, const int* taps, int 
     XVB_CHECK_ARG(j == 0 || taps[j] > taps[j - 1], "xvb_conv2d_taps: taps must be strictly increasing (tap %d = %d after %d)",
                   j, taps[j], taps[j - 1]);
   }
-  return conv2d_run("xvb_conv2d_taps", a, taps, ntaps, stream);
+  return conv2d_run("xvb_conv2d_taps", a, taps, ntaps, a->ksize / 2, stream);
+}
+
+// No padding: every tap of every written output lies inside the input, and the outputs a padded conv would add at the
+// far edges are neither computed into the output nor written (the epilogue clips at To x Fo).  The kernel is xvb_conv2d's.
+extern "C" int xvb_conv2d_valid(const xvb_conv2d_args_t* a, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(a, "xvb_conv2d_valid: null args");
+  XVB_CHECK_ARG((a->ksize == 3 || a->ksize == 1) && (a->stride == 1 || a->stride == 2),
+                "xvb_conv2d_valid: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
+  int dense[9];
+  for (int j = 0; j < a->ksize * a->ksize; ++j) dense[j] = j;
+  return conv2d_run("xvb_conv2d_valid", a, dense, a->ksize * a->ksize, 0, stream);
 }
 
 extern "C" int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,

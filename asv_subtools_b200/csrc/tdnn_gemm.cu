@@ -132,7 +132,9 @@ __device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, flo
   n = tot;
 }
 
-template <int BLOCK_N, bool kPool, bool kHist>
+// kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
+// one, so that the instantiations without it compile to the same code as before the flag existed.
+template <int BLOCK_N, bool kPool, bool kHist, bool kSwish = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                         const __grid_constant__ CUtensorMap map_a2_hi, const __grid_constant__ CUtensorMap map_a2_lo,
@@ -386,7 +388,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       continue;
     }
 
-    // ---- layer epilogue: +bias (+ row / utterance terms) -> ReLU -> BN -> tanh / sigmoid -> fp32 and/or split planes
+    // ---- layer epilogue: +bias (+ row / utterance terms) -> ReLU -> swish -> BN -> tanh / sigmoid -> fp32 and/or split
+    // planes
     if constexpr (!kPool && !kHist) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -409,6 +412,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
           float v = x[e] + (p.bias ? __ldg(p.bias + c + e) : 0.f) + rbias;
           if (ub) v += __ldg(ub + c + e);
           v = fmaxf(v, relu_floor);
+          if constexpr (kSwish) v = v / (1.f + expf(-v));
           if (bn) v = fmaf(v, __ldg(p.scale + c + e), __ldg(p.shift + c + e));
           if (act_tanh) v = tanhf(v);
           if (act_sigmoid) v = 1.f / (1.f + expf(-v));
@@ -441,7 +445,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 }
 
 // Split-K tail: y[b,c] = epi(sum_s part[b,s,c]) with the slices added in index order (deterministic),
-// same epilogue order as the GEMM's: +bias -> ReLU -> BN -> tanh/sigmoid -> fp32 and/or split planes.
+// same epilogue order as the GEMM's: +bias -> ReLU -> BN -> tanh/sigmoid -> fp32 and/or split planes (a layer with
+// XVB_SWISH never takes the split-K path).
 __global__ void segment_reduce_kernel(const float* __restrict__ part, int S, int B, int Cout, const float* __restrict__ bias,
                                       const float* __restrict__ scale, const float* __restrict__ shift, int flags,
                                       float* __restrict__ y_f32, long long ldyf, __nv_bfloat16* __restrict__ y_hi,
@@ -574,10 +579,10 @@ struct GemmPlan {
   __nv_bfloat16* r_y_hi = nullptr; __nv_bfloat16* r_y_lo = nullptr; long long r_ldy = 0;
 };
 
-template <int BLOCK_N, bool kPool, bool kHist>
+template <int BLOCK_N, bool kPool, bool kHist, bool kSwish>
 static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t stream) {
   using Cfg = GemmCfg<BLOCK_N>;
-  XVB_ENSURE_DYN_SMEM((tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist>), Cfg::kSmemBytes);
+  XVB_ENSURE_DYN_SMEM((tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>), Cfg::kSmemBytes);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(pl.grid);
   cfg.blockDim = dim3(kNumThreads);
@@ -588,13 +593,13 @@ static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = pl.pdl ? 1 : 0;
-  XVB_CUDA(cudaLaunchKernelEx(&cfg, tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist>, pl.ma_hi, pl.ma_lo, pl.ma2_hi,
+  XVB_CUDA(cudaLaunchKernelEx(&cfg, tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>, pl.ma_hi, pl.ma_lo, pl.ma2_hi,
                               pl.ma2_lo, pl.mw_hi, pl.mw_lo, p));
   XVB_LAUNCH_CHECK();
   return XVB_OK;
 }
 
-template <int BLOCK_N, bool kPool = false, bool kHist = false>
+template <int BLOCK_N, bool kPool = false, bool kHist = false, bool kSwish = false>
 static int prepare_gemm(GemmPlan& pl, const void* w_hi, const void* w_lo) {
   TdnnGemmParams& p = pl.p;
   const long long K = (long long)p.ntaps * p.cin_p16;
@@ -617,7 +622,7 @@ static int prepare_gemm(GemmPlan& pl, const void* w_hi, const void* w_lo) {
   pl.grid = p.num_tiles < sms ? p.num_tiles : sms;
   static const int pdl = getenv("XVB_PDL") ? atoi(getenv("XVB_PDL")) : 1;
   pl.pdl = pdl;
-  pl.launch = &launch_inst<BLOCK_N, kPool, kHist>;
+  pl.launch = &launch_inst<BLOCK_N, kPool, kHist, kSwish>;
   return XVB_OK;
 }
 
@@ -628,6 +633,7 @@ static int splitk_slices(const xvb_tdnn_args_t& a, bool has_hist, int* kb_per_sl
   *kb_per_slice = num_cblk;
   const int splitk = getenv("XVB_SPLITK") ? atoi(getenv("XVB_SPLITK")) : 1;   // read per plan: tests flip it
   if (!(splitk && a.T == 1 && a.ntaps == 1 && !a.x2_hi && !a.pool_partial && !has_hist && !a.row_bias && !a.utt_bias &&
+        !(a.flags & XVB_SWISH) &&
         a.B <= 1024 && num_cblk >= 24 && a.Cout % 4 == 0))
     return 1;
   int S = num_cblk / 6;
@@ -665,6 +671,7 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
   if (a.x2_hi) XVB_CHECK_ARG(a.ldx2 % 8 == 0 && a.ldx2 >= Cin, "xvb_tdnn_affine: ldx2=%lld must be a multiple of 8 and >= Cin", (long long)a.ldx2);
   XVB_CHECK_ARG((a.y_hi != nullptr) == (a.y_lo != nullptr), "xvb_tdnn_affine: y_hi/y_lo must both be set or both NULL");
   XVB_CHECK_ARG(a.y_hi || a.y_f32 || a.pool_partial || th, "xvb_tdnn_affine: no output requested");
+  XVB_CHECK_ARG(!(a.flags & XVB_SWISH) || !(a.pool_partial || th), "xvb_tdnn_affine: XVB_SWISH is a layer-epilogue flag only");
   if (a.pool_partial) XVB_CHECK_ARG(!a.y_hi && !a.y_f32 && Cout % 4 == 0 && (uintptr_t)a.pool_partial % 16 == 0,
                                     "xvb_tdnn_affine: pool_partial excludes other outputs and needs Cout%%4==0");
   if (a.y_hi) XVB_CHECK_ARG(a.ldy % 8 == 0 && a.ldy >= Cout, "xvb_tdnn_affine: plane output needs ldy%%8==0 and ldy>=Cout");
@@ -740,6 +747,11 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
       return prepare_gemm<128, true>(pl, w_hi, w_lo);
     if (th)              // the diagonal test of the symmetric mode assumes 128-row blocks x 128-column tiles
       return prepare_gemm<128, false, true>(pl, w_hi, w_lo);
+    if (a.flags & XVB_SWISH) {
+      if (Cout >= 128 && m_tiles * ((Cout + 127) / 128) >= sms) return prepare_gemm<128, false, false, true>(pl, w_hi, w_lo);
+      if (Cout >= 64 && m_tiles * ((Cout + 63) / 64) >= sms / 2) return prepare_gemm<64, false, false, true>(pl, w_hi, w_lo);
+      return prepare_gemm<32, false, false, true>(pl, w_hi, w_lo);
+    }
     if (Cout >= 128 && m_tiles * ((Cout + 127) / 128) >= sms) return prepare_gemm<128>(pl, w_hi, w_lo);
     if (Cout >= 64 && m_tiles * ((Cout + 63) / 64) >= sms / 2) return prepare_gemm<64>(pl, w_hi, w_lo);
     return prepare_gemm<32>(pl, w_hi, w_lo);

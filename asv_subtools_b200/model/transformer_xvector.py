@@ -1,0 +1,589 @@
+# -*- coding:utf-8 -*-
+"""Conformer x-vector blueprint for the native path -- drop-in for pytorch/model/transformer_xvector.py
+(TransformerXvector.init :93-244, extract_embedding :321-346) with the Conformer encoder of
+pytorch/libs/nnet/transformer/ (ConformerEncoder encoder.py:536-682, ConformerEncoderLayer encoder_layer.py:159-335).
+
+Same file name, class name, constructor signature and defaults (transformer_params merged with unknown keys kept, as
+assign_params_dict(support_unknow=True) does), creation string and state_dict keys for training=False; like the other
+blueprints, the training-only loss is not built, so its keys are left to load_state_dict(strict=False).
+
+Supported: transformer_type 'conformer' with input_layer 'conv2d'; pos_enc_type 'rot_pos' (rotary_value either way),
+'abs_pos' or 'no_pos'; attention norm 'softmax' or 'softmax_plus'; the convolution module with 'layer_norm' or
+'batch_norm'; activation 'swish' or 'relu'; transform_out with a LayerNorm (ln_replace) or a BatchNorm; the
+ecpa-attentive pooling with stddev; fc1 on or off (LayerNorm with or without affine); positions far / near_affine / near.
+Every other option raises NotImplementedError naming it.
+
+At extraction (ConformerExtractor) every contraction runs on the wgmma layer kernel with split-plane numerics: Q/K/V as
+one GEMM over the concatenated weights, linear_out, the feed-forward linears (swish / ReLU in the epilogue), the
+pointwise convs, the subsampling Linear (its input columns permuted from the reference's c * F'' + f to the f * C + c
+order of the conv output, x * sqrt(d) applied after the bias as the epilogue's scale), transform_out, the pooling convs
+and fc1 / fc2.  The second subsampling conv runs on the 2-D conv kernel without padding (xvb_conv2d_valid); the first
+one, the residual + LayerNorm steps, the attention and the convolution module's middle run on the kernels of
+csrc/conformer.cu.  The residual stream stays fp32.
+
+extract_embedding keeps the reference's maxChunk = 300 chunk rule (for_extract_embedding, framework.py:12-55): an
+utterance is cut into num_split = ceil(T / 300) chunks, each chunk is extracted on its own and the embeddings are
+averaged weighted by chunk length.  extract_embedding_batch applies the same rule to a batch of equal-length
+utterances with two stack runs (all full chunks, then all last chunks)."""
+import copy
+import math
+import os
+import sys
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+
+from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200._lib import ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH  # noqa: E402
+from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
+from asv_subtools_b200.nnet.components import TdnnAffine, fold_batchnorm  # noqa: E402
+from asv_subtools_b200.nnet.framework import for_extract_embedding  # noqa: E402
+
+MAX_CHUNK = 300     # @for_extract_embedding(maxChunk=300) of transformer_xvector.py:321
+MIN_FRAMES = 7      # the shortest input Conv2dSubsampling4 accepts
+
+
+def _assign(defaults, given, support_unknow=False):
+    """utils.assign_params_dict: known keys override the defaults (recursively for sub-dicts); unknown keys are kept
+    with support_unknow=True and dropped otherwise."""
+    out = copy.deepcopy(defaults)
+    for k, v in (given or {}).items():
+        if k in out:
+            out[k] = _assign(out[k], v, support_unknow) if isinstance(out[k], dict) and isinstance(v, dict) else v
+        elif support_unknow:
+            out[k] = v
+    return out
+
+
+def _unsupported(name, value):
+    raise NotImplementedError("{}={!r} is not on the native Conformer path".format(name, value))
+
+
+# ConformerEncoder's own defaults (encoder.py:538-581) under TransformerXvector's (transformer_xvector.py:98-127)
+_ENCODER_DEFAULTS = {
+    "attention_dim": 256, "attention_heads": 4, "linear_units": 2048, "mlp_head": False, "num_blocks": 6,
+    "aux_layer_period": 3, "aux_layer_start": 1, "dropout_rate": 0.1, "layer_dropout": 0., "positional_dropout_rate": 0.1,
+    "attention_dropout_rate": 0.0, "attention_conv_out": False, "attention_norm_args": {}, "input_layer": "conv2d",
+    "pos_enc_type": "rel_pos", "rotary_value": True, "rope_abs_plus": False, "add_t5rel_bias": False, "att_type": "multi",
+    "gau_units": 512, "gau_key": 64, "normalize_before": True, "norm_type": "layer_norm", "concat_after": False,
+    "positionwise_layer_type": "linear", "positionwise_conv_kernel_size": 3, "activation_type": "swish",
+    "activation_balancer": False, "static_chunk_size": 0, "left_chunk_size": -1, "use_dynamic_chunk": False,
+    "use_dynamic_left_chunk": False, "macaron_style": True, "use_cnn_module": True, "cnn_module_kernel": 15,
+    "causal": False, "cnn_module_norm": "batch_norm", "combiner_type": "norm", "re_scale": False, "convfnn_blocks": 0,
+}
+_ATT_NORM_DEFAULTS = {"scale_adapt": False, "norm_method": "softmax", "diag_mask": False, "g_sa": False, "train_len": 512}
+
+
+def _check_encoder(p):
+    """Raise for every encoder option the native path does not build."""
+    a = p["attention_norm_args"]
+    for name, ok in (("att_type", p["att_type"] == "multi"), ("input_layer", p["input_layer"] == "conv2d"),
+                     ("pos_enc_type", p["pos_enc_type"] in ("rot_pos", "abs_pos", "no_pos")),
+                     ("rope_abs_plus", not p["rope_abs_plus"]), ("add_t5rel_bias", not p["add_t5rel_bias"]),
+                     ("attention_conv_out", not p["attention_conv_out"]), ("mlp_head", not p["mlp_head"]),
+                     ("combiner_type", p["combiner_type"] == "norm"), ("convfnn_blocks", p["convfnn_blocks"] == 0),
+                     ("macaron_style", p["macaron_style"]), ("use_cnn_module", p["use_cnn_module"]),
+                     ("causal", not p["causal"]), ("normalize_before", p["normalize_before"]),
+                     ("concat_after", not p["concat_after"]), ("norm_type", p["norm_type"] == "layer_norm"),
+                     ("static_chunk_size", p["static_chunk_size"] == 0), ("use_dynamic_chunk", not p["use_dynamic_chunk"]),
+                     ("use_dynamic_left_chunk", not p["use_dynamic_left_chunk"]),
+                     ("activation_balancer", not p["activation_balancer"]), ("re_scale", not p["re_scale"]),
+                     ("positionwise_layer_type", p["positionwise_layer_type"] == "linear"),
+                     ("activation_type", p["activation_type"] in ("swish", "relu")),
+                     ("cnn_module_norm", p["cnn_module_norm"] in ("layer_norm", "batch_norm")),
+                     ("norm_method", a["norm_method"] in ("softmax", "softmax_plus")),
+                     ("scale_adapt", not a["scale_adapt"]), ("g_sa", not a["g_sa"]), ("diag_mask", not a["diag_mask"])):
+        if not ok:
+            _unsupported(name, a.get(name, p.get(name)))
+    d, h = p["attention_dim"], p["attention_heads"]
+    if d % h or d // h not in (32, 64, 128):
+        raise NotImplementedError("attention_dim / attention_heads = d_k must be 32, 64 or 128 on the native path (got {} / {})"
+                                  .format(d, h))
+    if d % 16 or p["linear_units"] % 8 or p["cnn_module_kernel"] % 2 == 0:
+        raise ValueError("attention_dim must be a multiple of 16, linear_units of 8 and cnn_module_kernel odd")
+
+
+class _Conv2dSubsampling4(nn.Module):
+    """Parameter container of subsampling.py:100-116 (conv.0, conv.2, out.0; the positional encodings hold none)."""
+
+    def __init__(self, idim, odim):
+        super().__init__()
+        self.conv = nn.Sequential(nn.Conv2d(1, odim, 3, 2), nn.ReLU(), nn.Conv2d(odim, odim, 3, 2), nn.ReLU())
+        self.out = nn.Sequential(nn.Linear(odim * (((idim - 1) // 2 - 1) // 2), odim))
+
+
+class _AttentionNormalize(nn.Module):
+    """attention.py:640-672: train_len = ln(train_len) is a parameter for softmax_plus only."""
+
+    def __init__(self, norm_method, train_len):
+        super().__init__()
+        self.method = norm_method
+        if norm_method == "softmax_plus":
+            self.train_len = nn.Parameter(torch.tensor(math.log(train_len)))
+
+
+class _SelfAttention(nn.Module):
+    """MultiHeadedAttention / RoPESelfAttention parameters (attention.py:26-53, :255-267)."""
+
+    def __init__(self, heads, dim, norm_args):
+        super().__init__()
+        self.d_k, self.h = dim // heads, heads
+        self.att_norm = _AttentionNormalize(norm_args["norm_method"], norm_args["train_len"])
+        self.linear_q = nn.Linear(dim, dim)
+        self.linear_k = nn.Linear(dim, dim)
+        self.linear_v = nn.Linear(dim, dim)
+        self.linear_out = nn.Linear(dim, dim)
+
+
+class _FeedForward(nn.Module):
+    """PositionwiseFeedForward (positionwise_feed_forward.py:19-34)."""
+
+    def __init__(self, dim, units):
+        super().__init__()
+        self.w_1 = nn.Linear(dim, units)
+        self.w_2 = nn.Linear(units, dim)
+
+
+class _ConvolutionModule(nn.Module):
+    """ConvolutionModule (convolution.py:21-76)."""
+
+    def __init__(self, channels, kernel_size, norm):
+        super().__init__()
+        self.pointwise_conv1 = nn.Conv1d(channels, 2 * channels, 1)
+        self.depthwise_conv = nn.Conv1d(channels, channels, kernel_size, padding=kernel_size // 2, groups=channels)
+        self.norm = nn.BatchNorm1d(channels) if norm == "batch_norm" else nn.LayerNorm(channels)
+        self.pointwise_conv2 = nn.Conv1d(channels, channels, 1)
+
+
+class _ConformerLayer(nn.Module):
+    """ConformerEncoderLayer parameters in the reference's registration order (encoder_layer.py:173-197)."""
+
+    def __init__(self, p):
+        super().__init__()
+        d = p["attention_dim"]
+        self.self_attn = _SelfAttention(p["attention_heads"], d, p["attention_norm_args"])
+        self.feed_forward = _FeedForward(d, p["linear_units"])
+        self.feed_forward_macaron = _FeedForward(d, p["linear_units"])
+        self.conv_module = _ConvolutionModule(d, p["cnn_module_kernel"], p["cnn_module_norm"])
+        for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
+            setattr(self, name, nn.LayerNorm(d, eps=1e-5))
+
+
+class _ConformerEncoder(nn.Module):
+    """ConformerEncoder parameters: embed, after_norm (BaseEncoder.__init__), encoders."""
+
+    def __init__(self, idim, p):
+        super().__init__()
+        self.p = p
+        self.embed = _Conv2dSubsampling4(idim, p["attention_dim"])
+        self.after_norm = nn.LayerNorm(p["attention_dim"], eps=1e-5)
+        self.encoders = nn.ModuleList([_ConformerLayer(p) for _ in range(p["num_blocks"])])
+
+
+class _TdnnLayer(nn.Module):
+    """ReluBatchNormTdnnLayer with a context-[0] TdnnAffine (components.py:337-461): affine -> activation -> LayerNorm
+    (ln_replace, affine per bn_params) or BatchNorm1d.  Only the relu-bn order is built."""
+
+    def __init__(self, input_dim, output_dim, **options):
+        super().__init__()
+        if options.get("bn-relu", False):
+            _unsupported("bn-relu", True)
+        nonlin = options.get("nonlinearity", "relu")
+        if nonlin not in ("relu", "swish", "", None, False):
+            _unsupported("nonlinearity", nonlin)
+        self.act = {"relu": ACT_RELU, "swish": ACT_SWISH}.get(nonlin, ACT_NONE)
+        self.affine = TdnnAffine(input_dim, output_dim, context=[0], bias=options.get("bias", True))
+        self.batchnorm, self.ln = None, False
+        if options.get("bn", True):
+            bn_params = {"momentum": 0.1, "affine": True, "track_running_stats": True}
+            bn_params.update(options.get("bn_params", {}))
+            if options.get("ln_replace", False):
+                self.ln = True
+                self.batchnorm = nn.LayerNorm(output_dim, eps=1e-5, elementwise_affine=bn_params["affine"])
+            else:
+                self.batchnorm = nn.BatchNorm1d(output_dim, **bn_params)
+
+
+class _AttentiveStatsPool(nn.Module):
+    """transformer_xvector.py:27-51: attention = conv -> ReLU -> LayerNorm -> tanh -> conv; norm_stats LayerNorm."""
+
+    def __init__(self, in_dim, hidden_size=128, time_attention=False, stddev=True):
+        super().__init__()
+        if time_attention:
+            _unsupported("time_attention", True)
+        if not stddev:
+            _unsupported("stddev", False)
+        self.output_dim = in_dim * 2
+        self.attention = nn.Sequential(nn.Conv1d(in_dim, hidden_size, 1), nn.ReLU(), nn.LayerNorm(hidden_size, eps=1e-5),
+                                       nn.Tanh(), nn.Conv1d(hidden_size, in_dim, 1))
+        self.norm_stats = nn.LayerNorm(self.output_dim, eps=1e-5)
+
+    def get_output_dim(self):
+        return self.output_dim
+
+
+class TransformerXvector(TopVirtualNnet):
+    """A Conformer x-vector framework."""
+
+    def init(self, inputs_dim, num_targets, embd_dim=256, training=True,
+             extracted_embedding="near", mixup=False, mixup_alpha=1.0, pooling="ecpa-attentive", pooling_params={},
+             transformer_type="conformer", transformer_params={}, tansformer_out={}, fc1=False, fc1_params={}, fc2_params={},
+             margin_loss=True, margin_loss_params={}, lsm_weight=0.0, use_step=False, step_params={},
+             transfer_from="softmax_loss", wenet_transfer=False):
+        default_transformer_params = {                                                          # :98-127
+            "attention_dim": 256, "att_type": 'multi', "attention_heads": 4, "gau_key": 64, "gau_units": 512,
+            "num_blocks": 6, "dropout_rate": 0.1, "layer_dropout": 0., "positionwise_layer_type": 'linear',
+            "positional_dropout_rate": 0.1, "linear_units": 2048, "positionwise_conv_kernel_size": 3,
+            "attention_dropout_rate": 0.0, "attention_norm_args": {"norm_method": "softmax", "train_len": 300.},
+            "input_layer": "conv2d", "pos_enc_type": "abs_pos", "cnn_module_kernel": 15, "use_cnn_module": True,
+            "cnn_module_norm": 'layer_norm', "static_chunk_size": 0, "left_chunk_size": -1, "use_dynamic_chunk": False,
+            "use_dynamic_left_chunk": False, "combiner_type": "norm", "convfnn_blocks": 0}
+        default_tansformer_out = {"out_dim": 1536, "nonlinearity": 'swish', "nonlinearity_params": {"inplace": True},
+                                  "bn-relu": False, "bn": True, "ln_replace": True,
+                                  "bn_params": {"momentum": 0.5, "affine": True, "track_running_stats": True}}
+        default_pooling_params = {"hidden_size": 128, "time_attention": False, "stddev": True}
+        default_fc_params = {"nonlinearity": 'relu', "nonlinearity_params": {"inplace": True}, "bn-relu": False,
+                             "bn": True, "ln_replace": True,
+                             "bn_params": {"momentum": 0.5, "affine": True, "track_running_stats": True}}
+        if transformer_type in ("transformer", "re_conformer"):
+            _unsupported("transformer_type", transformer_type)
+        if transformer_type != "conformer":
+            raise ValueError("unknown transformer_type: " + transformer_type)
+        if pooling != "ecpa-attentive":
+            raise ValueError("Only supoort asp for conformer now.")
+        tp = _assign(default_transformer_params, transformer_params, support_unknow=True)
+        enc = _assign(_ENCODER_DEFAULTS, tp, support_unknow=True)
+        enc["attention_norm_args"] = _assign(_ATT_NORM_DEFAULTS, enc["attention_norm_args"], support_unknow=True)
+        _check_encoder(enc)
+        to = _assign(default_tansformer_out, tansformer_out)
+        pp = _assign(default_pooling_params, pooling_params)
+        fc1_params = _assign(default_fc_params, fc1_params)
+        fc2_params = _assign(default_fc_params, fc2_params)
+        self.inputs_dim = inputs_dim
+        self.extracted_embedding = extracted_embedding
+        self.use_step, self.step_params = use_step, step_params
+        self.embd_dim = embd_dim
+        self.transformer = _ConformerEncoder(inputs_dim, enc)
+        self.transform_out = _TdnnLayer(enc["attention_dim"], to["out_dim"], **to)
+        self.stats = _AttentiveStatsPool(to["out_dim"], **pp)
+        self.fc1 = _TdnnLayer(self.stats.get_output_dim(), embd_dim, **fc1_params) if fc1 else None
+        self.fc2 = _TdnnLayer(embd_dim if fc1 else self.stats.get_output_dim(), embd_dim, **fc2_params)
+        for name, d in (("transform_out.out_dim", to["out_dim"]), ("pooling_params.hidden_size", pp["hidden_size"]),
+                        ("embd_dim", embd_dim)):
+            if d % 8:
+                raise ValueError("{}={} must be a multiple of 8 on the native Conformer path".format(name, d))
+        self.transform_keys = ["transformer", "transform_out", "stats", "fc1", "fc2", "loss"]
+        if margin_loss and transfer_from == "softmax_loss":
+            self.rename_transform_keys = {"loss.affine.weight": "loss.weight"}
+        self.wenet_transfer = wenet_transfer
+
+    def build_extractor(self):
+        if self.extracted_embedding == "far" and self.fc1 is None:
+            raise ValueError("extracted_embedding='far' needs fc1=True (transformer_xvector.py:334-336 asserts it)")
+        if self.extracted_embedding not in ("far", "near_affine", "near"):
+            raise TypeError("Expected far or near position, but got {}".format(self.extracted_embedding))
+        return ConformerExtractor(self, self.device_for_extraction())
+
+    @for_extract_embedding(maxChunk=MAX_CHUNK, isMatrix=True)
+    def _extract_embedding_chunked(self, inputs):
+        """inputs (1, frames, feat_dim) CUDA float32 -> (1, D)."""
+        return self.extractor().extract(inputs)
+
+    def extract_embedding(self, feats):
+        """feats (T, F) float32 -> 1-D CPU float32 tensor, with the reference's maxChunk = 300 chunk rule (the
+        framework's single-chunk host fast path does not apply: this model cuts every utterance above 300 frames)."""
+        if int(feats.shape[0]) < MIN_FRAMES:
+            raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, int(feats.shape[0])))
+        return self._extract_embedding_chunked(feats)
+
+    def extract_embedding_batch(self, feats):
+        """Equal-length utterances (B, T, F) float32 -> (B, D) CUDA tensor, the same arithmetic as B calls of
+        extract_embedding(): the B * (num_split - 1) full chunks run as one batch, the B last chunks as another, and the
+        chunk embeddings are recombined with the reference's length-weighted average."""
+        with torch.no_grad():
+            x = torch.as_tensor(feats)
+            if x.dtype != torch.float32:
+                raise TypeError("extract_embedding_batch expects float32 features")
+            B, T, Fd = x.shape
+            if T < MIN_FRAMES:
+                raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, T))
+            x = x.to(self.device_for_extraction(), non_blocking=True).contiguous()
+            lengths, offsets = chunk_plan(T)
+            ex = self.extractor()
+            last = ex.extract(x[:, offsets[-1]:].contiguous())
+            if len(lengths) == 1:
+                return (lengths[-1] * last) / T
+            split, ns = lengths[0], len(lengths) - 1
+            full = ex.extract(x[:, :split * ns].reshape(B * ns, split, Fd)).view(B, ns, -1)
+            acc = split * full[:, 0]
+            for i in range(1, ns):
+                acc = acc + split * full[:, i]
+            return (acc + lengths[-1] * last) / T
+
+
+def chunk_plan(num_frames, max_chunk=MAX_CHUNK):
+    """for_extract_embedding's split (framework.py:34-47): (chunk lengths, chunk offsets)."""
+    num_split = (num_frames + max_chunk - 1) // max_chunk
+    split = num_frames // num_split
+    lengths = [split] * (num_split - 1) + [num_frames - split * (num_split - 1)]
+    return lengths, [i * split for i in range(num_split)]
+
+
+def sinusoid_table(dim, max_len=5000):
+    """PositionalEncoding.pe (embedding.py:49-56), (max_len, dim)."""
+    pe = torch.zeros(max_len, dim)
+    position = torch.arange(0, max_len, dtype=torch.float32).unsqueeze(1)
+    div_term = torch.exp(torch.arange(0, dim, 2, dtype=torch.float32) * -(math.log(10000.0) / dim))
+    pe[:, 0::2] = torch.sin(position * div_term)
+    pe[:, 1::2] = torch.cos(position * div_term)
+    return pe
+
+
+def rotary_table(dk, max_len=5000):
+    """RoPositionalEncoding.pe (embedding.py:162-176), (max_len, dk) = [sin | cos]: computed on the CPU exactly as the
+    reference builds it."""
+    abs_rope = sinusoid_table(dk, max_len)
+    freq = torch.zeros_like(abs_rope)
+    freq[:, 0:dk // 2] = abs_rope[:, 0::2]
+    freq[:, dk // 2:] = abs_rope[:, 1::2]
+    return freq
+
+
+def subsampling_column_order(channels, freq):
+    """Input column of the subsampling Linear for each column of the (B, T', F'', C) conv output flattened as f * C + c:
+    the reference flattens (c, f) as c * F'' + f (subsampling.py:134-135)."""
+    f, c = np.meshgrid(np.arange(freq), np.arange(channels), indexing="ij")
+    return (c * freq + f).reshape(-1)
+
+
+def softmax_plus_multiplier(frames, train_len):
+    """AttentionNormalize.attention_normalize's factor (attention.py:719-726) with every score unmasked, in fp32:
+    (ln(l) / train_len * 1 + 1) - 1 with l = frames."""
+    mask = torch.ones((), dtype=torch.float32)
+    l = torch.tensor(float(frames), dtype=torch.float32)
+    return float(torch.log(l) / train_len.detach().float().cpu() * mask + 1 - mask)
+
+
+class _Lin:
+    """A Linear / kernel-size-1 conv packed for the wgmma layer kernel: y = epi(W x + b) with ReLU or swish, and an eval
+    BatchNorm (or a constant scale) as the epilogue's scale / shift."""
+
+    def __init__(self, weight, bias, device, act=ACT_NONE, scale=None, shift=None):
+        w = weight.detach().float().reshape(weight.shape[0], -1)
+        self.cout, self.cin = w.shape
+        self.w = ops.pack_tdnn_weight(w.to(device).unsqueeze(-1).contiguous(), [0])
+        self.bias = bias.detach().float().to(device).contiguous() if bias is not None else None
+        self.scale = torch.as_tensor(scale, dtype=torch.float32).to(device).contiguous() if scale is not None else None
+        self.shift = torch.as_tensor(shift, dtype=torch.float32).to(device).contiguous() if shift is not None else None
+        self.relu, self.swish = act == ACT_RELU, act == ACT_SWISH
+
+    def run(self, x, y=None, y_f32=None):
+        ops.tdnn_affine_ex(x, self.w, self.cout, [0], bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
+                           relu=self.relu, swish=self.swish, y=y, y_f32=y_f32)
+
+
+def _vec(t, device):
+    return t.detach().float().to(device).contiguous() if t is not None else None
+
+
+def _ln_params(ln, device):
+    return _vec(ln.weight, device), _vec(ln.bias, device)
+
+
+class ConformerExtractor:
+    """Folded weights on one device + the launch sequence of TransformerXvector.extract_embedding for one chunk per
+    utterance (all utterances of a call have the same length), driven from Python."""
+
+    def __init__(self, m, device):
+        enc = m.transformer
+        p = enc.p
+        self.device, self.feat_dim = device, m.inputs_dim
+        self.D, self.H = p["attention_dim"], p["attention_heads"]
+        self.dk = self.D // self.H
+        self.pos = p["pos_enc_type"]
+        self.rotary_value = self.pos == "rot_pos" and bool(p["rotary_value"])
+        self.softmax_plus = p["attention_norm_args"]["norm_method"] == "softmax_plus"
+        self.act = ACT_SWISH if p["activation_type"] == "swish" else ACT_RELU
+        emb = enc.embed
+        self.head_w = _vec(emb.conv[0].weight, device)
+        self.head_b = _vec(emb.conv[0].bias, device)
+        w2 = emb.conv[2].weight.detach().float().transpose(2, 3).contiguous()   # (C, C, kt, kf) -> (C, C, kf, kt)
+        self.conv2_w = ops.pack_conv2d_weight(w2.to(device))
+        self.conv2_scale = torch.ones(self.D, dtype=torch.float32, device=device)
+        self.conv2_shift = _vec(emb.conv[2].bias, device)
+        self.f2 = ((self.feat_dim - 1) // 2 - 1) // 2
+        lw = emb.out[0].weight.detach().float()[:, torch.from_numpy(subsampling_column_order(self.D, self.f2))]
+        xscale = None if self.pos == "no_pos" else np.full(self.D, math.sqrt(self.D), np.float32)
+        self.embed_out = _Lin(lw, emb.out[0].bias, device, scale=xscale,
+                              shift=None if xscale is None else np.zeros(self.D, np.float32))
+        self.layers = []
+        for layer in enc.encoders:
+            a, cm = layer.self_attn, layer.conv_module
+            L = {"ff_mac": (_Lin(layer.feed_forward_macaron.w_1.weight, layer.feed_forward_macaron.w_1.bias, device, self.act),
+                            _Lin(layer.feed_forward_macaron.w_2.weight, layer.feed_forward_macaron.w_2.bias, device)),
+                 "ff": (_Lin(layer.feed_forward.w_1.weight, layer.feed_forward.w_1.bias, device, self.act),
+                        _Lin(layer.feed_forward.w_2.weight, layer.feed_forward.w_2.bias, device)),
+                 "qkv": _Lin(torch.cat([a.linear_q.weight, a.linear_k.weight, a.linear_v.weight], 0),
+                             torch.cat([a.linear_q.bias, a.linear_k.bias, a.linear_v.bias], 0), device),
+                 "out": _Lin(a.linear_out.weight, a.linear_out.bias, device),
+                 "pw1": _Lin(cm.pointwise_conv1.weight, cm.pointwise_conv1.bias, device),
+                 "pw2": _Lin(cm.pointwise_conv2.weight, cm.pointwise_conv2.bias, device),
+                 "dw_w": _vec(cm.depthwise_conv.weight.reshape(self.D, -1), device),
+                 "dw_b": _vec(cm.depthwise_conv.bias, device),
+                 "train_len": a.att_norm.train_len if self.softmax_plus else None}
+            if isinstance(cm.norm, nn.BatchNorm1d):
+                s, t = fold_batchnorm(cm.norm)
+                L["cm_norm"] = (torch.from_numpy(s).to(device), torch.from_numpy(t).to(device), True)
+            else:
+                L["cm_norm"] = _ln_params(cm.norm, device) + (False,)
+            for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
+                L[name] = _ln_params(getattr(layer, name), device)
+            self.layers.append(L)
+        self.after_norm = _ln_params(enc.after_norm, device)
+        # transform_out: affine -> activation -> LayerNorm (its own kernel) or BatchNorm (the epilogue)
+        self.transform = self._tdnn(m.transform_out, device)
+        att = m.stats.attention
+        self.att1 = _Lin(att[0].weight, att[0].bias, device, ACT_RELU)
+        self.att_ln = _ln_params(att[2], device)
+        self.att2 = _Lin(att[4].weight, att[4].bias, device)
+        self.norm_stats = _ln_params(m.stats.norm_stats, device)
+        pos = m.extracted_embedding
+        if pos == "far":
+            self.segment = [(_Lin(m.fc1.affine.weight, m.fc1.affine.bias, device), None)]
+        else:
+            self.segment = ([self._tdnn(m.fc1, device)] if m.fc1 is not None else []) + \
+                ([self._tdnn(m.fc2, device)] if pos == "near" else [(_Lin(m.fc2.affine.weight, m.fc2.affine.bias, device), None)])
+        self.embed_dim = m.embd_dim
+        self._rope = rotary_table(self.dk) if self.pos == "rot_pos" else None
+        self._abs = sinusoid_table(self.D) if self.pos == "abs_pos" else None
+        self._tables = {}
+        self.last_launches = 0
+
+    @staticmethod
+    def _tdnn(layer, device):
+        """(_Lin with the activation [and the folded BatchNorm], LayerNorm (gamma, beta) or None)."""
+        w, b = layer.affine.weight, layer.affine.bias
+        if layer.batchnorm is not None and not layer.ln:
+            s, t = fold_batchnorm(layer.batchnorm)
+            return _Lin(w, b, device, layer.act, s, t), None
+        lin = _Lin(w, b, device, layer.act)
+        if layer.batchnorm is None:
+            return lin, None
+        return lin, (_vec(layer.batchnorm.weight, device), _vec(layer.batchnorm.bias, device))
+
+    def _tables_for(self, t):
+        if t not in self._tables:
+            if t >= 5000:
+                raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' 5000".format(t))
+            rope = self._rope[:t].to(self.device).contiguous() if self._rope is not None else None
+            absp = self._abs[:t].to(self.device).contiguous() if self._abs is not None else None
+            mults = [softmax_plus_multiplier(t, L["train_len"]) if self.softmax_plus else 1.0 for L in self.layers]
+            self._tables[t] = (rope, absp, mults)
+        return self._tables[t]
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embd_dim) fp32 CUDA, asynchronous on the current
+        stream."""
+        if feats.shape[2] != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
+        feats = feats.contiguous()
+        B, T, Fd = feats.shape
+        if T < MIN_FRAMES:
+            raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, T))
+        dev, P, D = feats.device, ops.SplitPlanes, self.D
+        T1, F1 = (T - 1) // 2, (Fd - 1) // 2
+        T2, F2 = (T1 - 1) // 2, (F1 - 1) // 2
+        rope, absp, mults = self._tables_for(T2)
+        n = 0
+        x1 = P.empty((B, T1, F1, D), dev)
+        ops.subsample_head(feats, self.head_w, self.head_b, x1)
+        x2 = P.empty((B, T2, F2, D), dev)
+        ops.conv2d(x1, self.conv2_w, D, 3, 2, self.conv2_scale, self.conv2_shift, relu=True, y=x2, valid=True)
+        del x1
+        r = torch.empty(B, T2, D, dtype=torch.float32, device=dev)
+        self.embed_out.run(P(x2.hi.view(B, T2, F2 * D), x2.lo.view(B, T2, F2 * D), F2 * D), y_f32=r)
+        n += 3
+        units = self.layers[0]["ff"][0].cout if self.layers else 0
+        h = P.empty((B, T2, D), dev)
+        hid = P.empty((B, T2, max(units, D)), dev)
+        delta = torch.empty(B, T2, 2 * D, dtype=torch.float32, device=dev)
+        qkv = torch.empty(B, T2, 3 * D, dtype=torch.float32, device=dev)
+        d1 = delta[..., :D]
+        hid_u = hid if units == hid.channels else hid.slice(0, units)
+        hid_d = hid if D == hid.channels else hid.slice(0, D)
+
+        def ffn(pair, out):
+            pair[0].run(h, y=hid_u)
+            pair[1].run(hid_u, y_f32=out)
+
+        first = self.layers[0] if self.layers else None
+        if first is not None:   # r [+ pe] -> r, norm_ff_macaron
+            ops.layer_norm(r, *first["norm_ff_macaron"], table=absp, x_out=r, y=h)
+            n += 1
+        for i, L in enumerate(self.layers):
+            ffn(L["ff_mac"], d1)
+            ops.layer_norm(r, *L["norm_mha"], delta=d1, delta_scale=0.5, x_out=r, y=h)
+            L["qkv"].run(h, y_f32=qkv)
+            ops.rope_attention(qkv, self.H, self.dk, hid_d, rope=rope, rope_v=self.rotary_value, score_mult=mults[i])
+            L["out"].run(hid_d, y_f32=d1)
+            ops.layer_norm(r, *L["norm_conv"], delta=d1, x_out=r, y=h)
+            L["pw1"].run(h, y_f32=delta)
+            g, b, bn = L["cm_norm"]
+            ops.conv_module(delta, L["dw_w"], L["dw_b"], g, b, hid_d, batch_norm=bn, act=self.act)
+            L["pw2"].run(hid_d, y_f32=d1)
+            ops.layer_norm(r, *L["norm_ff"], delta=d1, x_out=r, y=h)
+            ffn(L["ff"], d1)
+            nxt = self.layers[i + 1]["norm_ff_macaron"] if i + 1 < len(self.layers) else self.after_norm
+            ops.layer_norm(r, *L["norm_final"], delta=d1, delta_scale=0.5, x_out=r, second=nxt, y=h)
+            n += 16
+        del hid, delta, qkv
+        # transform_out (+ its LayerNorm): x fp32 for the pooling sums, planes for the attention conv
+        lin, ln = self.transform
+        od = lin.cout
+        xo = torch.empty(B, T2, od, dtype=torch.float32, device=dev)
+        xp = P.empty((B, T2, od), dev)
+        if ln is None:
+            lin.run(h, y=xp, y_f32=xo)
+            n += 1
+        else:
+            lin.run(h, y_f32=xo)
+            ops.layer_norm(xo, *ln, x_out=None, y=xp, y_f32=xo)
+            n += 2
+        # AttentiveStatsPool
+        a1 = torch.empty(B, T2, self.att1.cout, dtype=torch.float32, device=dev)
+        self.att1.run(xp, y_f32=a1)
+        ap = P.empty((B, T2, self.att1.cout), dev)
+        ops.layer_norm(a1, *self.att_ln, act=ACT_TANH, y=ap)
+        logits = torch.empty(B, T2, od, dtype=torch.float32, device=dev)
+        self.att2.run(ap, y_f32=logits)
+        stats = ops.attn_stats_pool(logits, xo, floor=1e-5)
+        z = P.empty((B, 1, 2 * od), dev)
+        zf = torch.empty(B, 1, 2 * od, dtype=torch.float32, device=dev)
+        ops.layer_norm(stats, *self.norm_stats, y=z, y_f32=zf)
+        n += 5
+        for j, (lin, ln) in enumerate(self.segment):
+            last = j + 1 == len(self.segment)
+            y = torch.empty(B, 1, lin.cout, dtype=torch.float32, device=dev)
+            lin.run(z, y_f32=y)
+            n += 1
+            yp = None
+            if ln is not None:
+                yp = None if last else P.empty((B, 1, lin.cout), dev)
+                ops.layer_norm(y, *ln, y=yp, y_f32=y)
+                n += 1
+            elif not last:
+                yp = ops.split_f32(y)
+                n += 1
+            z, zf = yp, y
+        self.last_launches = n
+        return zf.view(B, -1)[:, :self.embed_dim]
+
+    def close(self):
+        pass
+
+
+if __name__ == "__main__":
+    print(TransformerXvector(80, 10, training=False))

@@ -6,7 +6,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import BN, RELU, SIGMOID, TANH, TdnnArgs, check, int_array, lib  # noqa: F401
+from ._lib import BN, RELU, SIGMOID, SWISH, TANH, TdnnArgs, check, int_array, lib  # noqa: F401
 
 
 def _stream():
@@ -120,9 +120,10 @@ def fused_pool_layer(x, w, cout, context, bias=None, bn_scale=None, bn_shift=Non
 
 
 def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_shift=None, utt_bias=None, row_bias=None,
-                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None):
+                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False):
     """Full form of the wgmma layer (xvb_tdnn_affine_ex).  x / x2: SplitPlanes (B,T,*) (views
-    allowed); y: SplitPlanes to write (view allowed) and/or y_f32: fp32 (B,T,>=cout) tensor."""
+    allowed); y: SplitPlanes to write (view allowed) and/or y_f32: fp32 (B,T,>=cout) tensor.  swish: x * sigmoid(x)
+    after the bias (and ReLU), before the BatchNorm (XVB_SWISH)."""
     b, t = x.hi.shape[0], x.hi.shape[1]
     a = TdnnArgs()
     a.x_hi, a.x_lo, a.ldx = x.hi.data_ptr(), x.lo.data_ptr(), x.ld
@@ -136,7 +137,7 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
     if utt_bias is not None:
         a.utt_bias, a.ld_utt_bias = _req(utt_bias, torch.float32, "utt_bias").data_ptr(), utt_bias.shape[-1]
     a.flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0) | (TANH if tanh else 0) | \
-        (SIGMOID if sigmoid else 0)
+        (SIGMOID if sigmoid else 0) | (SWISH if swish else 0)
     ctx = int_array(context)
     keep.append(ctx)
     a.context_host, a.ntaps = ctx, len(context)
@@ -216,11 +217,12 @@ def pack_conv2d_weight(weight, taps=None):
 
 
 def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=False, y=None, y_f32=None,
-           scale2=None, shift2=None, y2=None, taps=None):
+           scale2=None, shift2=None, y2=None, taps=None, valid=False):
     """One 2-D convolution (xvb_conv2d): x SplitPlanes (B, T, F, Cin); w from pack_conv2d_weight; res / y / y2
     SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride).
     taps: only these taps (kf*ksize + kt, strictly increasing, ksize 1, 3 or 5) are computed, with w packed by
-    pack_conv2d_weight(weight, taps) (xvb_conv2d_taps)."""
+    pack_conv2d_weight(weight, taps) (xvb_conv2d_taps).  valid: no padding, T' = (T - k) // stride + 1 and F' likewise
+    (xvb_conv2d_valid; dense taps only)."""
     b, t, f, cin = x.hi.shape
     a = _lib.Conv2dArgs()
     a.x_hi, a.x_lo = _planes_ptrs(x)
@@ -235,7 +237,11 @@ def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=F
     a.y2_hi, a.y2_lo = _planes_ptrs(y2)
     if y_f32 is not None:
         a.y_f32 = _req(y_f32, torch.float32, "y_f32").data_ptr()
-    if taps is None:
+    if valid:
+        if taps is not None:
+            raise ValueError("conv2d(valid=True) takes the dense window only")
+        check(lib.xvb_conv2d_valid(C.byref(a), _stream()), "xvb_conv2d_valid")
+    elif taps is None:
         check(lib.xvb_conv2d(C.byref(a), _stream()), "xvb_conv2d")
     else:
         check(lib.xvb_conv2d_taps(C.byref(a), int_array(taps), len(taps), _stream()), "xvb_conv2d_taps")
@@ -265,6 +271,78 @@ def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, 
     check(lib.xvb_se_residual(z.hi.data_ptr(), z.lo.data_ptr(), _ptr(gate), identity.hi.data_ptr(), identity.lo.data_ptr(), b,
                               z.hi.numel() // (b * c), c, 1 if relu else 0, yh, yl, _ptr(y_f32), _ptr(scale2), _ptr(shift2),
                               y2h, y2l, _stream()), "xvb_se_residual")
+
+
+def subsample_head(feats, weight, bias, y):
+    """Conv2dSubsampling4's first conv + ReLU (xvb_subsample_head): feats (B, T, F) fp32, weight (C, 1, 3, 3) fp32 as
+    stored, bias (C,) -> y SplitPlanes (B, (T - 1) // 2, (F - 1) // 2, C)."""
+    feats = _req(feats, torch.float32, "feats")
+    b, t, f = feats.shape
+    check(lib.xvb_subsample_head(_ptr(feats), b, t, f, _ptr(_req(weight, torch.float32, "weight")),
+                                 _ptr(_req(bias, torch.float32, "bias")), weight.shape[0], y.hi.data_ptr(), y.lo.data_ptr(),
+                                 _stream()), "xvb_subsample_head")
+
+
+def _rows(t, name):
+    """(rows, pitch) of a fp32 CUDA tensor whose last dim is contiguous and whose leading dims collapse."""
+    if t.dtype != torch.float32 or not t.is_cuda or t.stride(-1) != 1:
+        raise TypeError("{} must be a CUDA float32 tensor with contiguous rows".format(name))
+    ld = t.stride(-2) if t.dim() >= 2 else t.shape[-1]
+    return t.numel() // t.shape[-1], ld
+
+
+def layer_norm(x, gamma=None, beta=None, eps=1e-5, delta=None, delta_scale=1.0, table=None, x_out=None, second=None,
+               act=_lib.ACT_NONE, y=None, y_f32=None, channels=None):
+    """Residual update + LayerNorm (xvb_layer_norm) over fp32 rows (..., C): v = x [+ table[row % len(table)]]
+    [+ delta_scale * delta]; n1 = LN(v) [* gamma + beta]; x_out (may be x) receives v, or n1 when `second` = (gamma2,
+    beta2) (either may be None: no affine) asks for y = act(LN(n1)); otherwise y = act(n1).  y: SplitPlanes and/or
+    y_f32: fp32 rows."""
+    rows, ldx = _rows(x, "x")
+    c = channels or x.shape[-1]
+    a = _lib.LayerNormArgs()
+    a.rows, a.C, a.eps, a.x, a.ldx = rows, c, eps, x.data_ptr(), ldx
+    if delta is not None:
+        a.delta, a.ld_delta = delta.data_ptr(), _rows(delta, "delta")[1]
+        a.delta_scale = delta_scale
+    if table is not None:
+        a.table, a.table_rows = _req(table, torch.float32, "table").data_ptr(), table.shape[0]
+    if x_out is not None:
+        a.x_out, a.ld_x_out = x_out.data_ptr(), _rows(x_out, "x_out")[1]
+    if gamma is not None:
+        a.gamma, a.beta = _req(gamma, torch.float32, "gamma").data_ptr(), _req(beta, torch.float32, "beta").data_ptr()
+    if second is not None:
+        a.second = 1
+        if second[0] is not None:
+            a.gamma2, a.beta2 = _req(second[0], torch.float32, "gamma2").data_ptr(), _req(second[1], torch.float32, "beta2").data_ptr()
+    a.act = act
+    if y is not None:
+        a.y_hi, a.y_lo, a.ldy = y.hi.data_ptr(), y.lo.data_ptr(), y.ld
+    if y_f32 is not None:
+        a.y_f32, a.ldyf = y_f32.data_ptr(), _rows(y_f32, "y_f32")[1]
+    check(lib.xvb_layer_norm(C.byref(a), _stream()), "xvb_layer_norm")
+
+
+def rope_attention(qkv, heads, dk, y, rope=None, rope_v=False, score_mult=1.0):
+    """Self-attention over the fused projection (xvb_rope_attention): qkv (B, T, >= 3 * heads * dk) fp32 rows, rope (T, dk)
+    fp32 [sin | cos] or None -> y SplitPlanes (B, T, heads * dk)."""
+    _, ldq = _rows(qkv, "qkv")
+    b, t = qkv.shape[0], qkv.shape[1]
+    check(lib.xvb_rope_attention(qkv.data_ptr(), ldq, b, t, heads, dk,
+                                 _ptr(_req(rope, torch.float32, "rope")) if rope is not None else None, 1 if rope_v else 0,
+                                 float(score_mult), y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_rope_attention")
+
+
+def conv_module(x, dw_weight, dw_bias, norm_a, norm_b, y, batch_norm=False, eps=1e-5, act=_lib.ACT_SWISH):
+    """ConvolutionModule middle (xvb_conv_module): x (B, T, >= 2C) fp32 rows (pointwise_conv1's output), dw_weight (C, K)
+    fp32, dw_bias (C,) -> GLU, depthwise conv, LayerNorm(gamma=norm_a, beta=norm_b) or y * norm_a + norm_b (folded eval
+    BatchNorm), act -> y SplitPlanes (B, T, C)."""
+    _, ldx = _rows(x, "x")
+    b, t = x.shape[0], x.shape[1]
+    c, k = dw_weight.shape
+    check(lib.xvb_conv_module(x.data_ptr(), ldx, b, t, c, _ptr(_req(dw_weight, torch.float32, "dw_weight")),
+                              _ptr(_req(dw_bias, torch.float32, "dw_bias")), k, _ptr(_req(norm_a, torch.float32, "norm_a")),
+                              _ptr(_req(norm_b, torch.float32, "norm_b")), 1 if batch_norm else 0, eps, act, y.hi.data_ptr(),
+                              y.lo.data_ptr(), y.ld, _stream()), "xvb_conv_module")
 
 
 def stats_pool_ex(x, eps, mode, planes=False):

@@ -43,11 +43,15 @@ extern "C" {
 #define XVB_ENODEVICE (-3) /* no sm_90 GPU visible */
 #define XVB_ESTATE (-4)    /* object used in the wrong state (e.g. extract before finalize) */
 
-/* epilogue flags for xvb_tdnn_affine* (order is fixed: +bias -> ReLU -> BN affine) */
+/* epilogue flags for xvb_tdnn_affine* (order is fixed: +bias -> ReLU -> swish -> BN affine -> tanh / sigmoid) */
 #define XVB_RELU 1 /* components.py:410-416 (_relu_bn_forward): ReLU first ... */
 #define XVB_BN 2   /* ... then eval-mode BatchNorm folded to y*scale[c] + shift[c] */
 #define XVB_SIGMOID 4 /* ... then sigmoid (SE gate, ecapa_tdnn_xvector.py:97-106) */
 #define XVB_TANH 8    /* ... then tanh (attention bottleneck, ecapa_tdnn_xvector.py:164-168) */
+/* swish x * sigmoid(x), between ReLU and BN: the Conformer's feed-forward activation (transformer/
+ * positionwise_feed_forward.py:31-34) and transform_out's swish before its norm (transformer_xvector.py:199).
+ * xvb_tdnn_affine / xvb_tdnn_affine_ex layer epilogues only (not the fused pooling or histogram variants). */
+#define XVB_SWISH 16
 
 #define XVB_MAX_TAPS 16
 
@@ -283,6 +287,71 @@ int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cou
 int xvb_conv2d_head_k(const float* x, int B, int T, int F, const float* w, int Cout, int ksize, const float* bn_scale,
                       const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2, const float* shift2,
                       uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+
+/* xvb_conv2d without padding: output (T - k) / s + 1 x (F - k) / s + 1, every tap inside the input (T, F >= k).
+ * ksize in {1, 3}, stride in {1, 2}, everything else as xvb_conv2d (same kernel, same epilogue).  The second conv of
+ * the Conformer's Conv2dSubsampling4 (pytorch/libs/nnet/transformer/subsampling.py:104-109: Conv2d(C, C, 3, 2) + ReLU)
+ * with scale = 1, shift = its bias, relu = 1. */
+int xvb_conv2d_valid(const xvb_conv2d_args_t* args, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * Conformer x-vector (pytorch/model/transformer_xvector.py over pytorch/libs/nnet/transformer/): the pieces that are
+ * not contractions.  Rows are channel-contiguous (B, T', C) frames of the subsampled sequence.
+ * ------------------------------------------------------------------------------------------- */
+#define XVB_ACT_NONE 0
+#define XVB_ACT_RELU 1
+#define XVB_ACT_SWISH 2 /* x * sigmoid(x) */
+#define XVB_ACT_TANH 3
+
+/* Conv2dSubsampling4's first conv (subsampling.py:104-106): Conv2d(1, C, 3, stride 2, no padding) + bias + ReLU in fp32
+ * on CUDA cores.  The reference convolves (B, 1, T, F): x (B, T, F) fp32, w (C, 1, 3, 3) fp32 as stored (kt, kf);
+ * y (B, T1, F1, C) planes with T1 = (T - 1) / 2, F1 = (F - 1) / 2.  T, F >= 3, C % 8 == 0. */
+int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, const float* bias, int C, uint16_t* y_hi,
+                       uint16_t* y_lo, void* stream);
+
+/* Residual update + LayerNorm over `rows` rows of C channels (C <= 8192), one pass:
+ *   v     = x [+ table[row % table_rows]] [+ delta_scale * delta]     the residual adds of ConformerEncoderLayer
+ *                                                                       (encoder_layer.py:248, :272, :293, :315) and
+ *                                                                       PositionalEncoding's + pe (embedding.py:75)
+ *   n1    = LN(v) [* gamma + beta]                                     eps as given (1e-5 everywhere in the model)
+ *   x_out = second ? n1 : v                                            the new residual stream (may alias x)
+ *   y     = act( second ? LN(n1) [* gamma2 + beta2] : n1 )             planes and/or fp32
+ * second = 1 is norm_final followed by the next block's norm_ff_macaron (or after_norm).  gamma / beta NULL: a
+ * LayerNorm without affine.  Zero-initialise the struct; unused pointers stay NULL. */
+typedef struct xvb_layer_norm_args {
+  int64_t rows; int C; float eps;
+  const float* x; int64_t ldx;
+  const float* delta; int64_t ld_delta; float delta_scale;
+  const float* table; int table_rows;
+  float* x_out; int64_t ld_x_out;
+  const float* gamma; const float* beta;
+  int second;
+  const float* gamma2; const float* beta2;
+  int act;
+  uint16_t* y_hi; uint16_t* y_lo; int64_t ldy;
+  float* y_f32; int64_t ldyf;
+} xvb_layer_norm_args_t;
+int xvb_layer_norm(const xvb_layer_norm_args_t* args, void* stream);
+
+/* Multi-head self-attention over the fused Q/K/V projection, RoPESelfAttention / MultiHeadedAttention
+ * (attention.py:120-154, :269-304) with AttentionNormalize (:640-728) at extraction (no mask):
+ *   qkv (B, T, >= 3 H dk) fp32, row pitch ldq: [q | k | v], head h at columns h*dk of each;
+ *   rope (T, dk) fp32 [sin | cos] (RoPositionalEncoding.pe[:T], embedding.py:162-192) or NULL: no rotation; when set,
+ *     q and k are rotated as apply_rotary (:298-304), v too if rope_v;
+ *   scores = (q . k / sqrt(dk)) * score_mult, softmax over keys: score_mult = 1 for softmax, (ln(T) / train_len + 1) - 1
+ *     in fp32 for softmax_plus;
+ *   y (B, T, H dk) planes = softmax . v, heads side by side (the input of linear_out).
+ * dk in {32, 64, 128}; any T >= 1 (keys are tiled with an online softmax). */
+int xvb_rope_attention(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
+                       float score_mult, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream);
+
+/* ConvolutionModule.forward between its pointwise convs (convolution.py:110-125): x (B, T, >= 2C) fp32 = pointwise_conv1's
+ * output; GLU a * sigmoid(b) over the two halves; depthwise Conv1d(C, C, K, padding K/2, groups C) with dw_w (C, K) and
+ * dw_b (C), zero padding at the utterance's ends; norm 0: LayerNorm(C) with gamma norm_a, beta norm_b and eps; norm 1:
+ * eval BatchNorm1d folded to y * norm_a + norm_b; then act; y (B, T, C) planes for pointwise_conv2.  K odd. */
+int xvb_conv_module(const float* x, int64_t ldx, int B, int T, int C, const float* dw_w, const float* dw_b, int K,
+                    const float* norm_a, const float* norm_b, int norm, float eps, int act, uint16_t* y_hi, uint16_t* y_lo,
+                    int64_t ldy, void* stream);
 
 /* y = [relu]( z * gate[b, c] + id ) over (B, P, C) planes (P positions per utterance): SEBlock_2D's scaling
  * (components.py:630-639) followed by BasicBlock's residual add (resnet.py:80-85 with relu, :100-104 without).
