@@ -132,6 +132,12 @@ __device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, flo
   n = tot;
 }
 
+// The layer epilogue is unrolled over all of a thread's accumulators, so whatever it inlines is repeated 64 times
+// (BLOCK_N = 128).  tanh and sigmoid, which the x-vector layers never use, stay out of line: inlined, their bodies
+// made the epilogue code larger than the instruction cache, and every tile's epilogue fetched its code from L2.
+__device__ __noinline__ float epi_tanh(float v) { return tanhf(v); }
+__device__ __noinline__ float epi_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
+
 // kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
 // one, so that the instantiations without it compile to the same code as before the flag existed.
 template <int BLOCK_N, bool kPool, bool kHist, bool kSwish = false>
@@ -414,8 +420,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
           v = fmaxf(v, relu_floor);
           if constexpr (kSwish) v = v / (1.f + expf(-v));
           if (bn) v = fmaf(v, __ldg(p.scale + c + e), __ldg(p.shift + c + e));
-          if (act_tanh) v = tanhf(v);
-          if (act_sigmoid) v = 1.f / (1.f + expf(-v));
+          if (act_tanh) v = epi_tanh(v);
+          if (act_sigmoid) v = epi_sigmoid(v);
           x[e] = v;
         }
         if (p.y_hi) {

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Seeded outputs of the 2-D conv entry points (xvb_conv2d, xvb_conv2d_taps) and the layer kernel (xvb_tdnn_affine_ex,
-every existing epilogue flag, the split-K segment path and the fused pooling) written to one .npz, so that two builds of
-the library can be compared bit for bit:
+every existing epilogue flag, the split-K segment path and the fused pooling; the five frame layers of bench.py at
+256 x 200, with the im2col first layer and tdnn5's fused pooling; an ECAPA-sized and a Conformer-sized layer) written to
+one .npz, so that two builds of the library can be compared bit for bit:
 
     python tools/dump_kernel_outputs.py <repository root> <out.npz>
 
@@ -11,6 +12,23 @@ import os
 import sys
 
 import numpy as np
+
+
+def im2col_layer(x, w, cin, cout, B, T, bias, scale, shift, y):
+    """The extractor's first layer: frame t reads rows t .. t + window - 1 of the time-padded planes x as one K = cin
+    row (xvb_tdnn_affine_ex with x_batch_stride), + bias -> ReLU -> BN."""
+    import ctypes as C
+    import torch
+    from asv_subtools_b200._lib import BN, RELU, TdnnArgs, check, int_array, lib
+    a = TdnnArgs()
+    a.x_hi, a.x_lo, a.ldx, a.x_batch_stride = x.hi.data_ptr(), x.lo.data_ptr(), x.ld, x.hi.stride(0)
+    a.w_hi, a.w_lo = w.hi.data_ptr(), w.lo.data_ptr()
+    a.bias, a.bn_scale, a.bn_shift, a.flags = bias.data_ptr(), scale.data_ptr(), shift.data_ptr(), RELU | BN
+    ctx = int_array([0])
+    a.context_host, a.ntaps = ctx, 1
+    a.y_hi, a.y_lo, a.ldy = y.hi.data_ptr(), y.lo.data_ptr(), y.ld
+    a.B, a.T, a.Cin, a.Cout = B, T, cin, cout
+    check(lib.xvb_tdnn_affine_ex(C.byref(a), C.c_void_p(torch.cuda.current_stream().cuda_stream)), "im2col layer")
 
 
 def main():
@@ -66,6 +84,34 @@ def main():
     x = ops.split_f32(rnd(4, 150, 512))
     w = rnd(1500, 512, 1, scale=1.0 / np.sqrt(512))
     res["pool"] = ops.fused_pool_layer(x, ops.pack_tdnn_weight(w, [0]), 1500, [0], bias=0.1 * rnd(1500)).cpu().numpy()
+    # the layer shapes bench.py runs (256 x 200, x-vector spec: the im2col first layer, tdnn2-4, tdnn5 with fused
+    # pooling), an ECAPA-sized and a Conformer-sized layer
+    B, T = 256, 200
+    xin = ops.split_f32(torch.nn.functional.pad(rnd(B, T, 80), (0, 0, 2, 2)).contiguous())   # time-padded planes
+    w = rnd(512, 400, 1, scale=1.0 / np.sqrt(400))
+    y = ops.SplitPlanes.empty((B, T, 512), "cuda")
+    im2col_layer(xin, ops.pack_tdnn_weight(w, [0]), 400, 512, B, T, 0.1 * rnd(512), 1 + 0.1 * rnd(512), 0.1 * rnd(512), y)
+    res["bench_tdnn1_y_hi"] = y.hi.view(torch.int16).cpu().numpy()
+    res["bench_tdnn1_y_lo"] = y.lo.view(torch.int16).cpu().numpy()
+    x = y
+    for i, ctx in ((2, [-2, 0, 2]), (3, [-3, 0, 3]), (4, [0])):
+        span = ctx[-1] - min(ctx[0], 0) + 1
+        w = rnd(512, 512, span, scale=1.0 / np.sqrt(512 * len(ctx)))
+        y = ops.SplitPlanes.empty((B, T, 512), "cuda")
+        ops.tdnn_affine_ex(x, ops.pack_tdnn_weight(w, ctx), 512, ctx, bias=0.1 * rnd(512), bn_scale=1 + 0.1 * rnd(512),
+                           bn_shift=0.1 * rnd(512), relu=True, y=y)
+        res["bench_tdnn{}_y_hi".format(i)] = y.hi.view(torch.int16).cpu().numpy()
+        res["bench_tdnn{}_y_lo".format(i)] = y.lo.view(torch.int16).cpu().numpy()
+        x = y
+    w = rnd(1500, 512, 1, scale=1.0 / np.sqrt(512))
+    res["bench_tdnn5_pool"] = ops.fused_pool_layer(x, ops.pack_tdnn_weight(w, [0]), 1500, [0], bias=0.1 * rnd(1500),
+                                                   bn_scale=1 + 0.1 * rnd(1500), bn_shift=0.1 * rnd(1500)).cpu().numpy()
+    for name, (B, T, cin, cout, ctx) in (("ecapa", (64, 200, 1024, 1024, [0])), ("conformer", (128, 74, 256, 2048, [0]))):
+        x = ops.split_f32(rnd(B, T, cin))
+        w = rnd(cout, cin, 1, scale=1.0 / np.sqrt(cin))
+        yf = torch.empty(B, T, cout, device="cuda")
+        ops.tdnn_affine_ex(x, ops.pack_tdnn_weight(w, ctx), cout, ctx, bias=0.1 * rnd(cout), relu=True, y_f32=yf)
+        res[name + "_f32"] = yf.cpu().numpy()
     np.savez(out, **res)
     print(out, len(res), "arrays")
 
