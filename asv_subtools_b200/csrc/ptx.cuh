@@ -8,8 +8,14 @@
 
 namespace xvb {
 
+// What mbar_wait does when a barrier has not completed after seconds of waiting (a protocol bug, not a slow kernel):
+//   0 -- nothing, it waits forever;
+//   1 -- (default) traps, so the launch fails instead of hanging;
+//   2 -- prints the block, thread, barrier and parity, then traps.  For debugging builds only
+//        (make EXTRA=-DXVB_WATCHDOG=2): printf is a function call, and a call anywhere in a kernel makes ptxas
+//        serialise every wgmma of that kernel (C7510, "wgmma pipeline crossing function boundary").
 #ifndef XVB_WATCHDOG
-#define XVB_WATCHDOG 1   // trap instead of hanging forever if a barrier never completes
+#define XVB_WATCHDOG 1
 #endif
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -86,9 +92,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #if XVB_WATCHDOG
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > 4000u) {  // ~ seconds: a protocol bug, not a slow kernel
+    if (++spins > 4000u) {  // ~ seconds
+#if XVB_WATCHDOG >= 2
       printf("xvb: mbarrier watchdog: block %d thread %d bar@%u parity %u\n", (int)blockIdx.x, (int)threadIdx.x,
              smem_u32(bar), parity);
+#endif
       __trap();
     }
   }

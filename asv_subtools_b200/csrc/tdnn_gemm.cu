@@ -277,9 +277,6 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     int prev_stage = -1;
     uint32_t scale_d = 0;                            // the tile's first MMA overwrites the accumulators
     for (int kb = kb_begin; kb < kb_end; ++kb) {
-      const int cb = kb % p.num_cblk;
-      int nsteps = (p.Cin - cb * kBlockK + 15) >> 4;
-      nsteps = nsteps > 4 ? 4 : nsteps;
       mbar_wait(&full_bar[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * kStageBytes);
       const uint64_t dx_hi = make_sw128_desc(sa), dx_lo = make_sw128_desc(sa + kABytes);
@@ -288,8 +285,14 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       const uint64_t m_off = (uint64_t)((wg * 64 * 128) >> 4);
       const uint64_t da_hi = (kPool ? dw_hi : dx_hi) + m_off, da_lo = (kPool ? dw_lo : dx_lo) + m_off;
       const uint64_t db_hi = kPool ? dx_hi : dw_hi, db_lo = kPool ? dx_lo : dw_lo;
+      // Every stage issues all four K steps, also the last channel block of a Cin that is not a multiple of 64: the
+      // frame maps' channel extent is Cin (the im2col view's too), so TMA fills the channels past it with zeros and the
+      // extra products add exact zeros.  The trip count has to be a compile-time constant: with a runtime one (or a
+      // branch between the fence and the commit) ptxas serialises every wgmma of the kernel (C7520), each one waiting
+      // for the previous one to finish.
       wgmma_fence();
-      for (int s = 0; s < nsteps; ++s) {
+#pragma unroll
+      for (int s = 0; s < kBlockK / 16; ++s) {
         const uint64_t koff = (uint64_t)(s * 32 >> 4);   // 16 bf16 = 32 bytes along K inside the swizzle row
         wgmma_bf16<BLOCK_N>(acc, da_lo + koff, db_hi + koff, scale_d);
         wgmma_bf16<BLOCK_N>(acc, da_hi + koff, db_lo + koff, 1);
