@@ -21,7 +21,7 @@ class TdnnArgs(C.Structure):
                 ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("ldy", C.c_int64),
                 ("y_f32", C.c_void_p), ("ldyf", C.c_int64),
                 ("B", C.c_int), ("T", C.c_int), ("Cin", C.c_int), ("Cout", C.c_int),
-                ("pool_partial", C.c_void_p), ("x_batch_stride", C.c_int64)]
+                ("pool_partial", C.c_void_p), ("x_batch_stride", C.c_int64), ("groups", C.c_int)]
 MAX_TAPS = 16
 
 
@@ -112,6 +112,8 @@ SIGNATURES = {
     "xvb_small_affine": (_i, [_p, _i64, _p, _i, _i, _i, _p, _p, _p, _i, _p, _i64, _p, _p, _i64, _p]),
     "xvb_attn_head_stats_pool": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
     "xvb_attn_head_stats_pool_prior": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _f, _i, _p, _p, _i, _p, _p, _p, _i64, _p]),
+    "xvb_attn_head_stats_pool_mq": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
+    "xvb_tdnn_grouped_fits": (_i, [_i, _i, _i]),
     "xvb_topn_mean_std": (_i, [_p, _i64, _i64, _i, _i, _p, _p, _p]),
     "xvb_topn_mean_std_ddof": (_i, [_p, _i64, _i64, _i, _i, _i, _p, _p, _p]),
     "xvb_snorm_trials": (_i, [_p, _p, _p, _i64, _p, _p, _p, _p, _p, _p]),
@@ -161,6 +163,7 @@ SIGNATURES = {
     "xvb_fbank_compute": (_i, [_p, _p, _p, _p, _i, _i64, _p, _p]),
     "xvb_fbank_destroy": (None, [_p]),
     "xvb_ecapa_create": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i]),
+    "xvb_ecapa_set_mqmha": (_i, [_p, _i, _i, _i, _i, _i, _i, _i]),
     "xvb_ecapa_set_layer": (_i, [_p, C.c_char_p, _i, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_ecapa_finalize": (_i, [_p]),
     "xvb_ecapa_embed_dim": (_i, [_p]),

@@ -431,7 +431,8 @@ small_affine_kernel(const float* __restrict__ x, long long ldx, const float* __r
 // gdiv = C / num_head, share=False: gdiv = 1; Global / MultiResolution multi-head: O = num_head * C, gdiv = C
 // (share) or 1.  One streaming pass, online softmax; per-frame loads of x are 16-byte, logits are scalar
 // (broadcast within the warp when heads are wide).  unweighted_var = 1: std of `stddev_attention=False`
-// (:357-359): mean_T((x - mean)^2) around the attention-weighted mean.
+// (:357-359): mean_T((x - mean)^2) around the attention-weighted mean.  MQMHASP (:589-698) splits C into heads of
+// head_width channels and pools each head `rep` (= num_q) times: c = (o / (rep*head_width))*head_width + o % head_width.
 struct OnlineU {
   float m, s0, s1, s2, u1, u2;
 };
@@ -442,7 +443,8 @@ struct OnlineU {
 template <int kRows>
 __global__ void __launch_bounds__(kApWarps * 32)
 attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, const float* __restrict__ x, long long ldx,
-                            int T, int C, int O, int gdiv, float floor_, int unweighted_var, const float* __restrict__ prior_logit,
+                            int T, int C, int O, int gdiv, int head_width, int rep, float floor_, int unweighted_var,
+                            const float* __restrict__ prior_logit,
                             const float* __restrict__ prior_x, int softplus2log, float* __restrict__ out,
                             __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol, long long ldo) {
   const int b = blockIdx.y;
@@ -453,7 +455,7 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
 #pragma unroll
   for (int k = 0; k < 4; ++k) st[k] = {-INFINITY, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (active) {
-    const int c = o % C;
+    const int c = (o / (rep * head_width)) * head_width + o % head_width;   // head_width = C, rep = O / C: o % C
     int g[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) g[k] = (o + k) / gdiv;
@@ -548,6 +550,22 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
   }
 }
 
+static int launch_attn_head_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C, int O,
+                                      int gdiv, int head_width, int rep, float floor_, int unweighted_var, const float* prior_logit,
+                                      const float* prior_x, int softplus2log, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                                      int64_t ldo, void* stream) {
+  dim3 grid((O + 127) / 128, B);
+  // frames in flight per thread (XVB_ATTN_ROWS = 1, 2 or 4): 1 by default, since the extra registers of the unrolled
+  // forms can cost more occupancy than they hide latency
+  static const int rows_knob = getenv("XVB_ATTN_ROWS") ? atoi(getenv("XVB_ATTN_ROWS")) : 1;
+  auto* kern = rows_knob == 1 ? attn_head_stats_pool_kernel<1> : rows_knob == 2 ? attn_head_stats_pool_kernel<2> : attn_head_stats_pool_kernel<4>;
+  kern<<<grid, kApWarps * 32, 0, (cudaStream_t)stream>>>(
+      logits, ldl, x, ldx, T, C, O, gdiv, head_width, rep, floor_, unweighted_var, prior_logit, prior_x, softplus2log, out,
+      reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}
+
 }  // namespace xvb
 
 using namespace xvb;
@@ -614,16 +632,25 @@ extern "C" int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, 
                 "xvb_attn_head_stats_pool: the head map o / gdiv must stay inside the %d logits", G);
   XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "xvb_attn_head_stats_pool: out_hi/out_lo must both be set or both NULL");
   if (out_hi) XVB_CHECK_ARG(ldo % 4 == 0 && ldo >= 2 * (int64_t)O, "xvb_attn_head_stats_pool: ldo too small / unaligned");
-  dim3 grid((O + 127) / 128, B);
-  // frames in flight per thread (XVB_ATTN_ROWS = 1, 2 or 4): 1 by default, since the extra registers of the unrolled
-  // forms can cost more occupancy than they hide latency
-  static const int rows_knob = getenv("XVB_ATTN_ROWS") ? atoi(getenv("XVB_ATTN_ROWS")) : 1;
-  auto* kern = rows_knob == 1 ? attn_head_stats_pool_kernel<1> : rows_knob == 2 ? attn_head_stats_pool_kernel<2> : attn_head_stats_pool_kernel<4>;
-  kern<<<grid, kApWarps * 32, 0, (cudaStream_t)stream>>>(
-      logits, ldl, x, ldx, T, C, O, gdiv, floor_, unweighted_var, prior_logit, prior_x, softplus2log, out,
-      reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
-  XVB_LAUNCH_CHECK();
-  return XVB_OK;
+  return launch_attn_head_stats_pool(logits, ldl, x, ldx, B, T, C, O, gdiv, C, O / C, floor_, unweighted_var, prior_logit,
+                                     prior_x, softplus2log, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_attn_head_stats_pool_mq(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
+                                           int C, int O, int gdiv, int head_width, int rep, float floor_, int unweighted_var,
+                                           float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(logits && x && out, "xvb_attn_head_stats_pool_mq: null pointer");
+  XVB_CHECK_ARG(B > 0 && T > 0 && C > 0 && ldx % 4 == 0 && ldx >= C && B <= 65535 && head_width > 0 && head_width % 4 == 0 &&
+                C % head_width == 0 && rep > 0 && O == rep * C,
+                "xvb_attn_head_stats_pool_mq: need head_width %% 4 == 0 dividing C, O == rep * C, ldx %% 4 == 0");
+  XVB_CHECK_ARG(gdiv > 0 && G > 0 && ldl >= G && (O - 1) / gdiv < G,
+                "xvb_attn_head_stats_pool_mq: the logit map o / gdiv must stay inside the %d logits", G);
+  XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "xvb_attn_head_stats_pool_mq: out_hi/out_lo must both be set or both NULL");
+  if (out_hi) XVB_CHECK_ARG(ldo % 4 == 0 && ldo >= 2 * (int64_t)O, "xvb_attn_head_stats_pool_mq: ldo too small / unaligned");
+  return launch_attn_head_stats_pool(logits, ldl, x, ldx, B, T, C, O, gdiv, head_width, rep, floor_, unweighted_var, nullptr,
+                                     nullptr, 0, out, out_hi, out_lo, ldo, stream);
 }
 
 extern "C" int xvb_plane_mean(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C, float* out,

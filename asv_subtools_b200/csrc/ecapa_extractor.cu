@@ -37,6 +37,10 @@ struct ELayer {
   float* scale = nullptr;
   float* shift = nullptr;
   float* w_f32 = nullptr;   // (Cout, Cin) fp32 as stored, kept for one-tap layers: the segment-level ones run on CUDA cores
+  // grouped 1x1 conv (the MQMHA attention convs): Cin is the per-group width; packed compactly for the layer kernel's
+  // grouped mode, or as the block-diagonal expansion (expanded) when the shape does not fit that mode
+  int groups = 1;
+  bool expanded = false;
   // host copies for save()
   std::vector<float> hw, hb, hs, ht;
 };
@@ -79,6 +83,11 @@ struct xvb_ecapa {
   float* s1f = nullptr;   // (B, se_dim) fp32: hidden vector of the SE gate
   float* f1 = nullptr;    // (B, fc1_dim) fp32: output of fc1 when the model has one
   int fc1_dim = 0;
+  // multi-query multi-head attention pooling (xvb_ecapa_set_mqmha); mq == 0: ECAPA's own attentive pooling
+  int mq = 0, mq_heads = 1, mq_q = 1, mq_hidden = 0, mq_share = 0, mq_layers = 2, mq_tatt = 1, mq_stddev = 1;
+  // widths derived from the pooling: att_x outputs AX, the logits NL (row pitch ldlog), the pooled statistics P of the
+  // P2-wide [mean | std] buffer (default model: AX = H, NL = D, P = P2 = 2D)
+  int AX = 0, NL = 0, ldlog = 0, P = 0, P2 = 0;
   int last_launches = 0;
   float* h_feats = nullptr; float* h_emb = nullptr;   // device staging of xvb_ecapa_extract_host
   size_t h_feats_cap = 0, h_emb_cap = 0;
@@ -135,8 +144,37 @@ extern "C" int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, i
   xvb_ecapa* h = new xvb_ecapa();
   h->feat_dim = feat_dim; h->ldf = (int)round_up(feat_dim, 8);
   h->C = channels; h->D = mfa_dim; h->H = att_hidden; h->E = embed_dim;
+  h->AX = att_hidden; h->NL = mfa_dim; h->ldlog = mfa_dim; h->P = 2 * mfa_dim; h->P2 = 2 * mfa_dim;
   *out = h;
   return XVB_OK;
+}
+
+extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int share, int affine_layers,
+                                   int time_attention, int stddev) {
+  XVB_CHECK_ARG(h && !h->finalized && h->layers.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
+  XVB_CHECK_ARG(num_head >= 1 && num_q >= 1 && hidden >= 1 && (affine_layers == 1 || affine_layers == 2) && h->D % num_head == 0 &&
+                (h->D / num_head) % 4 == 0 && hidden * num_head * num_q == h->H,
+                "xvb_ecapa_set_mqmha: need %d channels in heads of a multiple of 4, 1 or 2 affine layers and att_hidden = "
+                "hidden * num_head * num_q (= %d)", h->D, h->H);
+  const int cg = h->D / num_head, hq = num_head * num_q;
+  h->mq = 1; h->mq_heads = num_head; h->mq_q = num_q; h->mq_hidden = hidden; h->mq_share = share ? 1 : 0;
+  h->mq_layers = affine_layers; h->mq_tatt = time_attention ? 1 : 0; h->mq_stddev = stddev ? 1 : 0;
+  h->NL = hq * (share ? 1 : cg);
+  h->ldlog = (int)round_up(h->NL, 4);
+  h->AX = affine_layers == 2 ? h->H : h->NL;
+  XVB_CHECK_ARG(!time_attention || h->AX % 4 == 0, "xvb_ecapa_set_mqmha: the time-constant columns of the first attention conv "
+                "become a per-utterance bias, which needs a multiple of 4 outputs (got %d)", h->AX);
+  h->P2 = 2 * num_q * h->D;
+  h->P = stddev ? h->P2 : num_q * h->D;
+  return XVB_OK;
+}
+
+// Groups of a layer as the state_dict stores it: the MQMHA attention convs are grouped (pooling.py:665-698)
+static int layer_groups(const xvb_ecapa* h, const std::string& n) {
+  if (!h->mq) return 1;
+  if (n == "att_x") return h->mq_heads;
+  if (n == "att2") return h->mq_heads * h->mq_q;
+  return 1;
 }
 
 extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
@@ -155,16 +193,33 @@ extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, i
   L.hw.assign(w_host, w_host + wn);
   if (bias_host) L.hb.assign(bias_host, bias_host + Cout);
   if (flags & XVB_BN) { L.hs.assign(bn_scale_host, bn_scale_host + Cout); L.ht.assign(bn_shift_host, bn_shift_host + Cout); }
+  L.groups = layer_groups(h, name);
+  XVB_CHECK_ARG(L.groups == 1 || (ntaps == 1 && L.tot == 1 && Cout % L.groups == 0),
+                "xvb_ecapa_set_layer(%s): a grouped layer is a 1x1 conv with Cout divisible by its %d groups", name, L.groups);
+  // a grouped shape the layer kernel's grouped mode does not take runs as its block-diagonal expansion
+  L.expanded = L.groups > 1 && !xvb_tdnn_grouped_fits(Cin * L.groups, Cout, L.groups);
+  std::vector<float> dense;
+  const float* w_pack = w_host;
+  int cin_pack = Cin;
+  if (L.expanded) {
+    const int G = L.groups, co = Cout / G;
+    cin_pack = Cin * G;
+    dense.assign((size_t)Cout * cin_pack, 0.f);
+    for (int n = 0; n < Cout; ++n)
+      memcpy(&dense[(size_t)n * cin_pack + (size_t)(n / co) * Cin], w_host + (size_t)n * Cin, Cin * sizeof(float));
+    w_pack = dense.data();
+  }
+  const size_t wpn = (size_t)Cout * cin_pack * L.tot;
   float* w_dev = nullptr;
-  int rc = ealloc(&w_dev, wn);
+  int rc = ealloc(&w_dev, wpn);
   if (rc) return rc;
-  XVB_CUDA(cudaMemcpy(w_dev, w_host, wn * sizeof(float), cudaMemcpyHostToDevice));
-  const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, ntaps);
+  XVB_CUDA(cudaMemcpy(w_dev, w_pack, wpn * sizeof(float), cudaMemcpyHostToDevice));
+  const size_t pn = (size_t)xvb_packed_weight_elems(Cout, cin_pack, ntaps);
   if ((rc = ealloc(&L.w_hi, pn)) || (rc = ealloc(&L.w_lo, pn))) return rc;
-  rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, L.tot, left, L.ctx, ntaps, L.w_hi, L.w_lo, nullptr);
+  rc = xvb_pack_tdnn_weight(w_dev, Cout, cin_pack, L.tot, left, L.ctx, ntaps, L.w_hi, L.w_lo, nullptr);
   if (rc) return rc;
   XVB_CUDA(cudaDeviceSynchronize());
-  if (L.tot == 1 && Cin % 4 == 0) L.w_f32 = w_dev;   // one tap: (Cout, Cin, 1) is the (N, K) matrix xvb_small_affine takes
+  if (L.tot == 1 && Cin % 4 == 0 && L.groups == 1) L.w_f32 = w_dev;   // one tap: (Cout, Cin, 1) is the (N, K) matrix xvb_small_affine takes
   else cudaFree(w_dev);
   auto up = [&](float** d, const std::vector<float>& v) -> int {
     if (v.empty()) return XVB_OK;
@@ -227,12 +282,22 @@ extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
       XVB_CUDA(cudaMemcpy(h->res_shift[b] + (size_t)W * i, L->shift, W * sizeof(float), cudaMemcpyDeviceToDevice));
     }
   }
-  if ((rc = need("mfa", 3 * C, h->D, 1)) || (rc = need("att_x", h->D, h->H, 1)) || (rc = need("att_gs", 2 * h->D, h->H, 1)) ||
-      (rc = need("att2", h->H, h->D, 1)))
-    return rc;
+  rc = need("mfa", 3 * C, h->D, 1);
+  if (rc) return rc;
+  if (!h->mq) {
+    if ((rc = need("att_x", h->D, h->H, 1)) || (rc = need("att_gs", 2 * h->D, h->H, 1)) || (rc = need("att2", h->H, h->D, 1)))
+      return rc;
+  } else {   // per-group input widths: att_x reads a head's Cg channels of x, att2 one query's hidden units
+    rc = need("att_x", h->D / h->mq_heads, h->AX, 1);
+    if (rc) return rc;
+    if (h->mq_layers == 2 && (rc = need("att2", h->mq_hidden, h->NL, 1))) return rc;
+    XVB_CHECK_ARG(h->mq_layers == 2 || !find(h, "att2"), "xvb_ecapa_finalize: one-layer attention has no 'att2'");
+    if (h->mq_tatt && (rc = need("att_gs", (h->mq_stddev ? 2 : 1) * h->D, h->AX, 1))) return rc;
+    XVB_CHECK_ARG(h->mq_tatt || !find(h, "att_gs"), "xvb_ecapa_finalize: 'att_gs' without time attention");
+  }
   // segment level (ecapa_tdnn_xvector.py:412-422): [fc1 ->] [fc2]; "far" hands over fc1 alone, fc1=False fc2 alone
   if (const ELayer* fc1 = find(h, "fc1")) {
-    XVB_CHECK_ARG(fc1->Cin == 2 * h->D && fc1->ntaps == 1 && fc1->w_f32, "xvb_ecapa_finalize: 'fc1' must be a one-tap layer over the %d pooled statistics", 2 * h->D);
+    XVB_CHECK_ARG(fc1->Cin == h->P && fc1->ntaps == 1 && fc1->w_f32, "xvb_ecapa_finalize: 'fc1' must be a one-tap layer over the %d pooled statistics", h->P);
     if (find(h, "fc2")) {
       rc = need("fc2", fc1->Cout, h->E, 1);
       if (rc) return rc;
@@ -241,7 +306,7 @@ extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
     }
     h->fc1_dim = fc1->Cout;
   } else {
-    rc = need("fc2", 2 * h->D, h->E, 1);
+    rc = need("fc2", h->P, h->E, 1);
     if (rc) return rc;
   }
   {
@@ -273,9 +338,9 @@ static int reserve(xvb_ecapa* h, int B, int T) {
       (rc = h->planes(&h->R, nf, C)) || (rc = h->planes(&h->Z, nf, C)) || (rc = h->planes(&h->N, nf, C)) ||
       (rc = h->planes(&h->CAT, nf, 3 * C)) || (rc = h->planes(&h->M, nf, D)) || (rc = h->planes(&h->A1, nf, h->H)) ||
       (rc = h->planes(&h->gp, nb, 2 * D)) || (rc = h->planes(&h->s1, nb, h->se_dim)) || (rc = h->planes(&h->zm, nb, C)) ||
-      (rc = h->planes(&h->pp, nb, 2 * D)) || (rc = h->f32(&h->MF, nf * D)) || (rc = h->f32(&h->LOG, nf * D)) ||
-      (rc = h->f32(&h->gate, nb * C)) || (rc = h->f32(&h->ub, nb * h->H)) || (rc = h->f32(&h->zmean, nb * C)) ||
-      (rc = h->f32(&h->gstat, nb * 2 * D)) || (rc = h->f32(&h->pstat, nb * 2 * D)) || (rc = h->f32(&h->s1f, nb * (size_t)h->se_dim)) ||
+      (rc = h->planes(&h->pp, nb, h->P2)) || (rc = h->f32(&h->MF, nf * D)) || (rc = h->f32(&h->LOG, nf * h->ldlog)) ||
+      (rc = h->f32(&h->gate, nb * C)) || (rc = h->f32(&h->ub, nb * h->AX)) || (rc = h->f32(&h->zmean, nb * C)) ||
+      (rc = h->f32(&h->gstat, nb * 2 * D)) || (rc = h->f32(&h->pstat, nb * h->P2)) || (rc = h->f32(&h->s1f, nb * (size_t)h->se_dim)) ||
       (h->fc1_dim && (rc = h->f32(&h->f1, nb * (size_t)h->fc1_dim))))
     return rc;
   h->cap_frames = (long long)nf;
@@ -317,10 +382,43 @@ int launch(const Run& r, void* stream) {
   if (r.im2col_taps > 0) { a.context_host = &ctx0; a.ntaps = 1; a.x_batch_stride = r.x_batch_stride; }
   a.y_hi = r.y.hi; a.y_lo = r.y.lo; a.ldy = r.y.ld;
   a.y_f32 = r.y_f32; a.ldyf = r.ldyf;
-  a.B = r.B; a.T = r.T; a.Cin = r.im2col_taps > 0 ? r.im2col_taps * r.L->Cin : r.L->Cin; a.Cout = r.L->Cout;
+  a.B = r.B; a.T = r.T; a.Cin = r.im2col_taps > 0 ? r.im2col_taps * r.L->Cin : r.L->Cin * r.L->groups; a.Cout = r.L->Cout;
+  a.groups = r.L->expanded ? 1 : r.L->groups;
   return xvb_tdnn_affine_ex(&a, stream);
 }
 }  // namespace
+
+// MQMHASP.forward (libs/nnet/pooling.py:627-663) over the mfa output (M planes, MF fp32) into pstat / pp:
+// time attention: biased mean | sqrt(clamp(var, 1e-5)) of every channel (egrecho's compute_statistics) -> the
+// per-utterance bias of the first attention conv (its [mean_h | std_h] columns, block-diagonal over the heads) ->
+// grouped conv over x (ReLU -> BN -> tanh) -> grouped conv to the logits -> softmax over T and weighted moments with
+// the head-width map: pooled channel (h*Q + q)*Cg + c is x channel h*Cg + c under the alpha of logit (h*Q + q)[*Cg + c].
+static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
+  const int D = h->D, cg = D / h->mq_heads;
+  const ELayer* ax = find(h, "att_x");
+  int rc;
+  if (h->mq_tatt) {
+    if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 0, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
+    const ELayer* gs = find(h, "att_gs");
+    if (small_ok(gs)) {
+      if ((rc = small_layer(gs, h->gstat, 2 * D, B, h->ub, h->AX, 0, stream))) return rc;
+    } else {
+      Run r{}; r.B = B; r.T = 1; r.L = gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = h->AX;
+      if ((rc = launch(r, stream))) return rc;
+    }
+  }
+  Run r{}; r.B = B; r.T = T; r.L = ax; r.x = h->M;
+  if (h->mq_tatt) { r.utt_bias = h->ub; r.ld_utt = h->AX; }
+  if (h->mq_layers == 2) { r.y = h->A1; r.extra_flags = XVB_TANH; }
+  else { r.y_f32 = h->LOG; r.ldyf = h->ldlog; }
+  if ((rc = launch(r, stream))) return rc;
+  if (h->mq_layers == 2) {
+    r = Run{}; r.B = B; r.T = T; r.L = find(h, "att2"); r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = h->ldlog;
+    if ((rc = launch(r, stream))) return rc;
+  }
+  return xvb_attn_head_stats_pool_mq(h->LOG, h->ldlog, h->NL, h->MF, D, B, T, D, h->mq_q * D, h->mq_share ? cg : 1, cg, h->mq_q,
+                                     1e-5f, 0, h->pstat, h->pp.hi, h->pp.lo, h->P2, stream);
+}
 
 extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int T, float* emb, void* stream) {
   XVB_CHECK_ARG(h && h->finalized, "xvb_ecapa_extract: model not finalized");
@@ -377,6 +475,9 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   }
   r = Run{}; r.B = B; r.T = T; r.L = L("mfa"); r.x = h->CAT; r.y = h->M; r.y_f32 = h->MF; r.ldyf = D;
   if ((rc = launch(r, stream))) return rc;
+  if (h->mq) {
+    if ((rc = mqmha_pool(h, B, T, stream))) return rc;
+  } else {
   if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
   if (small_ok(L("att_gs"))) {
     rc = small_layer(L("att_gs"), h->gstat, 2 * D, B, h->ub, h->H, 0, stream);
@@ -390,9 +491,10 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   r = Run{}; r.B = B; r.T = T; r.L = L("att2"); r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = D;
   if ((rc = launch(r, stream))) return rc;
   if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, h->pp.hi, h->pp.lo, 2 * D, stream))) return rc;
+  }
   if (const ELayer* fc1 = L("fc1")) {              // fc1 [-> fc2] on CUDA cores (fp32)
     const ELayer* fc2 = L("fc2");
-    rc = small_layer(fc1, h->pstat, 2 * D, B, fc2 ? h->f1 : emb, fc1->Cout, 0, stream);
+    rc = small_layer(fc1, h->pstat, h->P2, B, fc2 ? h->f1 : emb, fc1->Cout, 0, stream);
     if (rc) return rc;
     if (fc2) {
       XVB_CHECK_ARG(fc2->w_f32, "xvb_ecapa_extract: 'fc2' after 'fc1' needs an input width that is a multiple of 4");
@@ -400,10 +502,10 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
       if (rc) return rc;
     }
   } else if (small_ok(L("fc2"))) {
-    rc = small_layer(L("fc2"), h->pstat, 2 * D, B, emb, h->E, 0, stream);
+    rc = small_layer(L("fc2"), h->pstat, h->P2, B, emb, h->E, 0, stream);
       if (rc) return rc;
   } else {
-    r = Run{}; r.B = B; r.T = 1; r.L = L("fc2"); r.x = h->pp; r.y_f32 = emb; r.ldyf = h->E;
+    r = Run{}; r.B = B; r.T = 1; r.L = L("fc2"); r.x = h->pp; r.y_f32 = emb; r.ldyf = h->E;   // reads the first P of P2 columns
     if ((rc = launch(r, stream))) return rc;
   }
   h->last_launches = (int)(g_launches - before);
@@ -461,6 +563,9 @@ static int ecapa_ensure_lanes(xvb_ecapa* h) {
   xvb_ecapa* c = new xvb_ecapa();
   c->feat_dim = h->feat_dim; c->ldf = h->ldf; c->C = h->C; c->D = h->D; c->H = h->H; c->E = h->E; c->scale = h->scale;
   c->se_dim = h->se_dim; c->fc1_dim = h->fc1_dim; c->finalized = true;
+  c->mq = h->mq; c->mq_heads = h->mq_heads; c->mq_q = h->mq_q; c->mq_hidden = h->mq_hidden; c->mq_share = h->mq_share;
+  c->mq_layers = h->mq_layers; c->mq_tatt = h->mq_tatt; c->mq_stddev = h->mq_stddev;
+  c->AX = h->AX; c->NL = h->NL; c->ldlog = h->ldlog; c->P = h->P; c->P2 = h->P2;
   for (int b = 0; b < 3; ++b) {
     c->dilation[b] = h->dilation[b];
     c->res_w_hi[b] = h->res_w_hi[b]; c->res_w_lo[b] = h->res_w_lo[b]; c->res_bias[b] = h->res_bias[b];
@@ -472,6 +577,7 @@ static int ecapa_ensure_lanes(xvb_ecapa* h) {
     for (int i = 0; i < XVB_MAX_TAPS; ++i) L.ctx[i] = kv.second.ctx[i];
     L.w_hi = kv.second.w_hi; L.w_lo = kv.second.w_lo; L.bias = kv.second.bias; L.scale = kv.second.scale; L.shift = kv.second.shift;
     L.w_f32 = kv.second.w_f32;
+    L.groups = kv.second.groups; L.expanded = kv.second.expanded;
     c->layers[kv.first] = L;
   }
   c->im2col_first = h->im2col_first; c->pad_front = h->pad_front; c->pad_back = h->pad_back;
@@ -581,13 +687,19 @@ extern "C" int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_h
 }
 
 // ---- .xvbm files for ECAPA ("XVBE0001"): dims, then named layer records -------------------------------------
+// "XVBE0002" (MQMHA pooling): the same with the pooling record {num_head, num_q, hidden, share, affine_layers,
+// time_attention, stddev} after the dims; layers of grouped convs are stored as the state_dict holds them.
 extern "C" int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path) {
   XVB_CHECK_ARG(h && h->finalized && path, "xvb_ecapa_save: model not finalized");
   FILE* f = fopen(path, "wb");
   XVB_CHECK_ARG(f, "xvb_ecapa_save: cannot open '%s'", path);
-  bool ok = fwrite("XVBE0001", 1, 8, f) == 8;
+  bool ok = fwrite(h->mq ? "XVBE0002" : "XVBE0001", 1, 8, f) == 8;
   const int32_t hd[6] = {h->feat_dim, h->C, h->D, h->H, h->E, (int32_t)h->order.size()};
   ok = ok && fwrite(hd, 4, 6, f) == 6;
+  if (h->mq) {
+    const int32_t pr[7] = {h->mq_heads, h->mq_q, h->mq_hidden, h->mq_share, h->mq_layers, h->mq_tatt, h->mq_stddev};
+    ok = ok && fwrite(pr, 4, 7, f) == 7;
+  }
   for (const std::string& n : h->order) {
     const ELayer& L = h->layers.at(n);
     const int32_t nl = (int32_t)n.size();
@@ -612,11 +724,15 @@ extern "C" int xvb_ecapa_load(xvb_ecapa_t** out, const char* path) {
   xvb_ecapa_t* h = nullptr;
   int rc = XVB_EINVAL;
   do {
-    if (!rd(magic, 8) || memcmp(magic, "XVBE0001", 8) != 0 || !rd(hd, sizeof hd) || hd[5] < 1 || hd[5] > 256) {
-      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 file", path);
+    int32_t pr[7];
+    const bool ok_magic = rd(magic, 8) && (memcmp(magic, "XVBE0001", 8) == 0 || memcmp(magic, "XVBE0002", 8) == 0);
+    const bool mq = ok_magic && magic[7] == '2';
+    if (!ok_magic || !rd(hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(pr, sizeof pr))) {
+      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 file", path);
       break;
     }
     if ((rc = xvb_ecapa_create(&h, hd[0], hd[1], hd[2], hd[3], hd[4]))) break;
+    if (mq && (rc = xvb_ecapa_set_mqmha(h, pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]))) break;
     std::vector<float> w, b, s, t;
     for (int i = 0; i < hd[5] && rc == XVB_OK; ++i) {
       int32_t nl = 0, rec[7], ctx[XVB_MAX_TAPS];

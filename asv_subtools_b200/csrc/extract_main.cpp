@@ -15,8 +15,8 @@
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
 // the input side.  The model file is any of the three families, told apart by its magic: TDNN x-vector
-// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001) or 2-D ResNet x-vector (XVBR0001, the extractors'
-// save()).  What it adds: utterances of equal length are batched (the reference runs batch 1).
+// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling)
+// or 2-D ResNet x-vector (XVBR0001, the extractors' save()).  What it adds: utterances of equal length are batched (the reference runs batch 1).
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32;
 //   * one "FV" vector per input key (order follows batch completion, which the wspecifier allows);
@@ -59,7 +59,7 @@ struct Utt {
 
 struct Runner {
   xvb_extractor_t* ex = nullptr;   // TDNN x-vector family (XVBM0001) ...
-  xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001) ...
+  xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001 / XVBE0002) ...
   xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001)
   xvb_ark_writer_t* out = nullptr;
   int F = 0, D = 0, batch = 256, cmn = 0, cmn_window = 300;
@@ -188,7 +188,7 @@ int main(int argc, char** argv) {
              "                   [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001) or 2-D ResNet x-vector (XVBR0001) model,\n"
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002) or 2-D ResNet x-vector (XVBR0001) model,\n"
              "recognised by its magic.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
@@ -210,7 +210,7 @@ int main(int argc, char** argv) {
     FILE* mf = fopen(pos[0], "rb");
     if (!mf || fread(magic, 1, 8, mf) != 8) { fprintf(stderr, "ERROR: xvb-extract: cannot read model file '%s'\n", pos[0]); return 1; }
     fclose(mf);
-    if (memcmp(magic, "XVBE0001", 8) == 0) {
+    if (memcmp(magic, "XVBE0001", 8) == 0 || memcmp(magic, "XVBE0002", 8) == 0) {
       CK(xvb_ecapa_load(&r.ec, pos[0]), "loading the ECAPA model");
       r.F = xvb_ecapa_feat_dim(r.ec);
       r.D = xvb_ecapa_embed_dim(r.ec);

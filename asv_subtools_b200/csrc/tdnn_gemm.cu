@@ -74,6 +74,9 @@ struct TdnnGemmParams {
   // and stores its fp32 partial at "time" s of a (B, k_slices, Cout) buffer; segment_reduce_kernel sums
   // the slices in order (deterministic) and applies the epilogue.  ntaps == 1, one source only.
   int k_slices, kb_per_slice;
+  // grouped convolution (groups > 1): N block n0 belongs to group n0 / group_ng and streams only that group's
+  // group_kg input channels, starting at frame channel (n0 / group_ng) * group_kg; 0 = dense
+  int group_ng, group_kg;
   int out_T;              // time extent of the fp32 output (k_slices for split-K partials, else T)
   __nv_bfloat16* y_hi;
   __nv_bfloat16* y_lo;
@@ -196,6 +199,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         const int cb_end = p.k_slices > 1 ? min(p.num_cblk, cb_begin + p.kb_per_slice) : p.num_cblk;
         const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;  // may be fully out of
         const int n0 = n_blk * BLOCK_N;                                                    // range: TMA zero-fills
+        const int a_c0 = p.group_ng ? (n0 / p.group_ng) * p.group_kg : 0;                  // grouped: this group's K slice
         for (int src = 0; src < p.num_src; ++src) {
           const CUtensorMap* ma_hi = src == 0 ? &map_a_hi : &map_a2_hi;
           const CUtensorMap* ma_lo = src == 0 ? &map_a_lo : &map_a2_lo;
@@ -206,8 +210,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
               uint8_t* s = smem + stage * kStageBytes;
               const int kw = tap * p.cin_p16 + cb * kBlockK;
               mbar_expect_tx(&full_bar[stage], kStageBytes);
-              tma_load_3d(s, ma_hi, &full_bar[stage], cb * kBlockK, tt, b0);
-              tma_load_3d(s + kABytes, ma_lo, &full_bar[stage], cb * kBlockK, tt, b0);
+              tma_load_3d(s, ma_hi, &full_bar[stage], a_c0 + cb * kBlockK, tt, b0);
+              tma_load_3d(s + kABytes, ma_lo, &full_bar[stage], a_c0 + cb * kBlockK, tt, b0);
               tma_load_2d(s + 2 * kABytes, &map_w_hi, &full_bar[stage], kw, n0);
               tma_load_2d(s + 2 * kABytes + kBBytes, &map_w_lo, &full_bar[stage], kw, n0);
               if (++stage == kStages) { stage = 0; phase ^= 1; }
@@ -642,7 +646,7 @@ static int splitk_slices(const xvb_tdnn_args_t& a, bool has_hist, int* kb_per_sl
   *kb_per_slice = num_cblk;
   const int splitk = getenv("XVB_SPLITK") ? atoi(getenv("XVB_SPLITK")) : 1;   // read per plan: tests flip it
   if (!(splitk && a.T == 1 && a.ntaps == 1 && !a.x2_hi && !a.pool_partial && !has_hist && !a.row_bias && !a.utt_bias &&
-        !(a.flags & XVB_SWISH) &&
+        !(a.flags & XVB_SWISH) && a.groups <= 1 &&
         a.B <= 1024 && num_cblk >= 24 && a.Cout % 4 == 0))
     return 1;
   int S = num_cblk / 6;
@@ -693,6 +697,12 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
                 "xvb_tdnn_affine: pointers must be 16-byte aligned");
   for (int i = 1; i < ntaps; ++i)
     XVB_CHECK_ARG(a.context_host[i] > a.context_host[i - 1], "xvb_tdnn_affine: context must be strictly increasing (components.py:34-36)");
+  const int G = a.groups > 1 ? a.groups : 1;
+  if (G > 1)
+    XVB_CHECK_ARG(xvb_tdnn_grouped_fits(Cin, Cout, G) && ntaps == 1 && !a.x2_hi && !a.pool_partial && !th && !a.x_batch_stride &&
+                  !(a.flags & XVB_SWISH),
+                  "xvb_tdnn_affine: groups=%d needs Cin/groups %% 64 == 0, Cout/groups %% 32 == 0, one tap and no second source, "
+                  "fused pooling, histogram, im2col view or XVB_SWISH (Cin=%d Cout=%d ntaps=%d)", G, Cin, Cout, ntaps);
 
   GemmPlan* plp = new GemmPlan();
   struct Guard { GemmPlan* p; ~Guard() { delete p; } } guard{plp};
@@ -704,8 +714,9 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
   p.num_t_blk = (T + p.Tb - 1) / p.Tb;
   p.num_b_blk = (B + p.Bb - 1) / p.Bb;
   p.ntaps = ntaps;
-  p.cin_p16 = (int)round_up(Cin, 16);
-  p.num_cblk = (Cin + kBlockK - 1) / kBlockK;
+  p.cin_p16 = (int)round_up(Cin / G, 16);        // weight K per tap: the group's slice (compact packing) when grouped
+  p.num_cblk = (Cin / G + kBlockK - 1) / kBlockK;
+  if (G > 1) { p.group_ng = Cout / G; p.group_kg = Cin / G; }
   for (int i = 0; i < ntaps; ++i) p.ctx[i] = a.context_host[i];
   p.flags = a.flags;
   p.bias = a.bias; p.scale = a.bn_scale; p.shift = a.bn_shift; p.row_bias = a.row_bias;
@@ -756,6 +767,12 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
       return prepare_gemm<128, true>(pl, w_hi, w_lo);
     if (th)              // the diagonal test of the symmetric mode assumes 128-row blocks x 128-column tiles
       return prepare_gemm<128, false, true>(pl, w_hi, w_lo);
+    if (G > 1) {         // an N tile must not straddle two groups: the widest tile that divides the group's outputs
+      const int ng = Cout / G;
+      if (ng % 128 == 0) return prepare_gemm<128>(pl, w_hi, w_lo);
+      if (ng % 64 == 0) return prepare_gemm<64>(pl, w_hi, w_lo);
+      return prepare_gemm<32>(pl, w_hi, w_lo);
+    }
     if (a.flags & XVB_SWISH) {
       if (Cout >= 128 && m_tiles * ((Cout + 127) / 128) >= sms) return prepare_gemm<128, false, false, true>(pl, w_hi, w_lo);
       if (Cout >= 64 && m_tiles * ((Cout + 63) / 64) >= sms / 2) return prepare_gemm<64, false, false, true>(pl, w_hi, w_lo);
@@ -819,6 +836,11 @@ int xvb::tdnn_affine_impl(const xvb_tdnn_args_t& a, void* stream, const TrialHis
   rc = gemm_plan_launch(pl, stream, nullptr);
   gemm_plan_destroy(pl);
   return rc;
+}
+
+extern "C" int xvb_tdnn_grouped_fits(int Cin, int Cout, int groups) {
+  return groups > 1 && Cin > 0 && Cout > 0 && Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kBlockK == 0 &&
+         (Cout / groups) % 32 == 0;
 }
 
 extern "C" int xvb_pool_partial_blocks(int B, int T, int* frames_per_block) {

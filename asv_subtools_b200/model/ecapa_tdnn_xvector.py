@@ -19,6 +19,11 @@ chunk/cat/expand copies is expressed through channel-slice views instead:
     [mean,std] part of the first conv becomes a per-utterance bias (a (B,3072)x(3072,128) GEMM),
     the softmax over T and the weighted moments are one streaming online-softmax pass;
   * bn_stats (:412) is folded into fc2's weights at build time.
+
+pooling="mqmha" (MQMHASP, libs/nnet/pooling.py:589-698, the roadmap launcher's pooling) runs its two grouped attention
+convs on the layer kernel's grouped mode (compact weights, each N tile streaming only its group's K slice), the
+time-constant [mean_h | std_h] columns of the first as a per-utterance bias, and the pooling on the head-width map of
+xvb_attn_head_stats_pool_mq.
 """
 import math
 import os
@@ -33,6 +38,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
+from asv_subtools_b200.nnet.pooling import MQMHASP  # noqa: E402
 
 
 def _merge(defaults, given):
@@ -102,8 +108,9 @@ class ECAPA_TDNN(TopVirtualNnet):
         default_pool = {"hidden_size": 128, "time_attention": True, "stddev": True}
         default_fc = {"nonlinearity": "relu", "nonlinearity_params": {"inplace": True}, "bn-relu": False, "bn": True,
                       "bn_params": {"momentum": 0.5, "affine": True, "track_running_stats": True}}
-        if pooling != "ecpa-attentive":
-            raise NotImplementedError("B200 ECAPA implements pooling='ecpa-attentive' (the reference default)")
+        if pooling not in ("ecpa-attentive", "mqmha"):
+            raise NotImplementedError("B200 ECAPA implements pooling='ecpa-attentive' (the reference default) and 'mqmha', "
+                                      "not pooling={!r}".format(pooling))
         ecapa_params = _merge(default_ecapa, ecapa_params)
         pooling_params = _merge(default_pool, pooling_params)
         fc1_params = _merge(default_fc, fc1_params)
@@ -118,10 +125,15 @@ class ECAPA_TDNN(TopVirtualNnet):
         self.layer3 = SE_Res2Block(channels, channels, kernel_size=3, dilation=3, scale=8, bn_params=ecapa_params)
         self.layer4 = SE_Res2Block(channels, channels, kernel_size=3, dilation=4, scale=8, bn_params=ecapa_params)
         self.mfa = ReluBatchNormTdnnLayer(channels * 3, mfa_conv, **ecapa_params)
-        self.stats = AttentiveStatsPool(mfa_conv, pooling_params["hidden_size"], pooling_params["time_attention"])
-        self.bn_stats = nn.BatchNorm1d(mfa_conv * 2, **ecapa_params["bn_params"])
-        self.fc1 = ReluBatchNormTdnnLayer(mfa_conv * 2, self.embd_dim, **fc1_params) if fc1 else None      # :286-287
-        self.fc2 = ReluBatchNormTdnnLayer(self.embd_dim if fc1 else mfa_conv * 2, self.embd_dim, **fc2_params)   # :326-333
+        if pooling == "mqmha":          # :289-295; `stddev` was popped from pooling_params (:274), so MQMHASP keeps its default
+            self.stats = MQMHASP(mfa_conv, **{k: v for k, v in pooling_params.items() if k != "stddev"})
+            pooled = self.stats.get_output_dim()
+        else:
+            self.stats = AttentiveStatsPool(mfa_conv, pooling_params["hidden_size"], pooling_params["time_attention"])
+            pooled = mfa_conv * 2
+        self.bn_stats = nn.BatchNorm1d(pooled, **ecapa_params["bn_params"])
+        self.fc1 = ReluBatchNormTdnnLayer(pooled, self.embd_dim, **fc1_params) if fc1 else None      # :286-287
+        self.fc2 = ReluBatchNormTdnnLayer(self.embd_dim if fc1 else pooled, self.embd_dim, **fc2_params)   # :326-333
         self.transform_keys = ["layer1", "layer2", "layer3", "layer4", "stats", "mfa", "bn_stats", "fc1", "fc2", "loss"]
         if margin_loss and transfer_from == "softmax_loss":
             self.rename_transform_keys = {"loss.affine.weight": "loss.weight"}
@@ -138,11 +150,19 @@ class ECAPA_TDNN(TopVirtualNnet):
 
 
 class _Layer:
-    """Device-side packed parameters of one TDNN / 1x1-conv layer."""
+    """Device-side packed parameters of one TDNN / 1x1-conv layer.  groups > 1: a grouped 1x1 conv with its weight as
+    stored, (Cout, Cin/groups, 1), packed compactly for the layer kernel's grouped mode, or as its block-diagonal
+    expansion when the shape does not fit that mode (ops.tdnn_grouped_fits)."""
 
-    def __init__(self, weight, bias, context, bn=None, relu=False, device=None, scale_shift=None):
+    def __init__(self, weight, bias, context, bn=None, relu=False, device=None, scale_shift=None, groups=1):
         w = weight.detach().float().to(device).contiguous()
         self.context = list(context)
+        self.groups = 1
+        if groups > 1:
+            if ops.tdnn_grouped_fits(w.shape[1] * groups, w.shape[0], groups):
+                self.groups = groups
+            else:
+                w = _block_diagonal(w, groups)
         self.w = ops.pack_tdnn_weight(w, self.context)
         self.cout = w.shape[0]
         # one-tap layers keep the (N, K) fp32 matrix too: the segment-level ones run on CUDA cores (ops.small_affine)
@@ -155,7 +175,7 @@ class _Layer:
 
     def run(self, x, **kw):
         ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
-                           relu=self.relu, **kw)
+                           relu=self.relu, groups=self.groups, **kw)
         _mark("gemm K={}x{} N={}".format(len(self.context), x.channels, self.cout))
 
     def run_rows(self, x, sigmoid=False):
@@ -163,6 +183,42 @@ class _Layer:
         y = ops.small_affine(x, self.w_f32, self.bias, self.scale, self.shift, relu=self.relu, sigmoid=sigmoid)
         _mark("rows K={} N={}".format(x.shape[1], self.cout))
         return y
+
+
+def _block_diagonal(w, groups):
+    """(Cout, Cin/G, k) grouped weight -> (Cout, Cin, k) with group g's block at rows g*Cout/G, columns g*Cin/G (conv1d's rule)."""
+    co, ci = w.shape[0] // groups, w.shape[1]
+    dense = w.new_zeros(w.shape[0], ci * groups, w.shape[2])
+    for g in range(groups):
+        dense[g * co:(g + 1) * co, g * ci:(g + 1) * ci] = w[g * co:(g + 1) * co]
+    return dense
+
+
+def _mqmha_attention(st):
+    """The MQMHASP attention as extractor records (name, weight, bias, bn (scale, shift) | None, relu, groups):
+    "att_x" = the first conv's x columns as stored (per head [x_h | mean_h | std_h], pooling.py:636-648), "att_gs" = its
+    [mean_h | std_h] columns as ONE block-diagonal (Cout, 2C) matrix over the utterance's [mean | std] plus the conv's bias
+    (time attention only: the time-constant part becomes a per-utterance bias), "att2" = the second conv."""
+    f = lambda t: t.detach().float().cpu().numpy()  # noqa: E731
+    att, H, cg = st.attention, st.num_head, st.head_width()
+    w0, b0 = f(att[0].weight), f(att[0].bias)
+    cout = w0.shape[0]
+    xcols = np.ascontiguousarray(w0[:, :cg])
+    two = st.affine_layers == 2
+    bn = fold_batchnorm(att[2]) if two else None
+    out = [("att_x", xcols, None if st.time_attention else b0, bn, two, H)]
+    if st.time_attention:
+        ns = 2 if st.stddev else 1
+        gs = np.zeros((cout, ns * st.in_dim, 1), dtype=np.float32)
+        rows = cout // H
+        for h in range(H):
+            r = slice(h * rows, (h + 1) * rows)
+            for k in range(ns):        # k = 0: mean columns, 1: std columns
+                gs[r, k * st.in_dim + h * cg:k * st.in_dim + (h + 1) * cg] = w0[r, (k + 1) * cg:(k + 2) * cg]
+        out.append(("att_gs", gs, b0, None, False, 1))
+    if two:
+        out.append(("att2", f(att[4].weight), f(att[4].bias), None, False, H * st.num_q))
+    return out
 
 
 _PROFILE = None  # list of (label, cuda event) when profiling (tools/bench_ecapa.py --profile)
@@ -196,6 +252,11 @@ def _named_layers(m):
         out.append((p + "se1", f(blk.se.se[1].weight), f(blk.se.se[1].bias), [0], None, None, True))
         out.append((p + "se2", f(blk.se.se[3].weight), f(blk.se.se[3].bias), [0], None, None, False))
     out.append(tdnn("mfa", m.mfa))
+    if isinstance(m.stats, MQMHASP):
+        for name, w, b, bn, relu, _ in _mqmha_attention(m.stats):
+            s, t = bn if bn is not None else (None, None)
+            out.append((name, w, b, [0], s, t, relu))
+        return out + _segment_layers(m)
     att, c = m.stats.attention, m.stats.in_dim
     w0 = f(att[0].weight)
     s, t = fold_batchnorm(att[2])
@@ -240,8 +301,14 @@ class NativeEcapaExtractor:
         if path is not None:
             check(lib.xvb_ecapa_load(C.byref(self._h), str(path).encode()), "xvb_ecapa_load")
         else:
-            check(lib.xvb_ecapa_create(C.byref(self._h), m.inputs_dim, m.layer1.affine.output_dim, m.stats.in_dim,
-                                       m.stats.attention[0].out_channels, m.embd_dim), "xvb_ecapa_create")
+            st = m.stats
+            mq = isinstance(st, MQMHASP)
+            check(lib.xvb_ecapa_create(C.byref(self._h), m.inputs_dim, m.layer1.affine.output_dim, st.in_dim,
+                                       st.hidden_size * st.num_head * st.num_q if mq else st.attention[0].out_channels,
+                                       m.embd_dim), "xvb_ecapa_create")
+            if mq:
+                check(lib.xvb_ecapa_set_mqmha(self._h, st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers,
+                                              int(st.time_attention), int(st.stddev)), "xvb_ecapa_set_mqmha")
             for name, w, b, ctx, scale, shift, relu in _named_layers(m):
                 w = np.ascontiguousarray(w, dtype=np.float32)
                 w3 = w.reshape(w.shape[0], w.shape[1], -1)
@@ -365,17 +432,22 @@ class EcapaExtractor:
             })
         self.channels = m.layer1.affine.output_dim
         self.mfa = tdnn(m.mfa)
+        self.mfa_dim = m.stats.in_dim
+        self.segment = [_Layer(torch.from_numpy(w), torch.from_numpy(b), ctx, relu=relu, device=device, scale_shift=(scale, shift))
+                        for _, w, b, ctx, scale, shift, relu in _segment_layers(m)]
+        self.embed_dim = m.embd_dim
+        self.mq = m.stats if isinstance(m.stats, MQMHASP) else None
+        if self.mq is not None:
+            self.att = {name: _Layer(torch.from_numpy(w), None if b is None else torch.from_numpy(b), [0], relu=relu, device=device,
+                                     scale_shift=bn if bn is not None else (None, None), groups=g)
+                        for name, w, b, bn, relu, g in _mqmha_attention(self.mq)}
+            return
         att = m.stats.attention
         c = m.stats.in_dim
         w0 = att[0].weight.detach().float()
         self.att_x = _Layer(w0[:, :c].contiguous(), None, [0], bn=att[2], relu=True, device=device)
         self.att_gs = _Layer(w0[:, c:].contiguous(), att[0].bias, [0], device=device)  # [mean | std] columns
         self.att2 = _Layer(att[4].weight, att[4].bias, [0], device=device)
-        self.mfa_dim = c
-        # segment level: [fc1 ->] [fc2], bn_stats folded into the first (same records as the native extractor gets)
-        self.segment = [_Layer(torch.from_numpy(w), torch.from_numpy(b), ctx, relu=relu, device=device, scale_shift=(scale, shift))
-                        for _, w, b, ctx, scale, shift, relu in _segment_layers(m)]
-        self.embed_dim = m.embd_dim
 
     def extract(self, feats):
         """feats (B,T,F) fp32 CUDA -> (B, embd_dim) fp32 CUDA (asynchronous on the current stream)."""
@@ -424,6 +496,8 @@ class EcapaExtractor:
         M = P.empty((B, T, D), dev)
         MF = torch.empty(B, T, D, dtype=torch.float32, device=dev)
         self.mfa.run(CAT, y=M, y_f32=MF)
+        if self.mq is not None:
+            return self._mqmha_tail(M, MF)
         gstat, gp = ops.stats_pool_ex(MF, 1e-5, 1, planes=True)      # global mean | sqrt(var_unbiased + 1e-5)
         _mark("stats_pool(global)")
         if SMALL_ROWS:
@@ -444,6 +518,44 @@ class EcapaExtractor:
             return x
         emb = torch.empty(B, 1, self.embed_dim, dtype=torch.float32, device=dev)
         self.segment[0].run(pp, y_f32=emb)
+        return emb.view(B, self.embed_dim)
+
+    def _mqmha_tail(self, M, MF):
+        """MQMHASP.forward (pooling.py:627-663) + the segment layers, in the native extractor's launch order."""
+        st, att = self.mq, self.att
+        B, T, D = MF.shape
+        dev = MF.device
+        P = ops.SplitPlanes
+        ub = None
+        if st.time_attention:        # egrecho's compute_statistics: biased variance clamped at 1e-5
+            gstat, gp = ops.stats_pool_ex(MF, 1e-5, 0, planes=True)
+            _mark("stats_pool(global)")
+            if SMALL_ROWS:
+                ub = att["att_gs"].run_rows(gstat[:, :att["att_gs"].w_f32.shape[1]].contiguous())
+            else:
+                ub = torch.empty(B, 1, att["att_gs"].cout, dtype=torch.float32, device=dev)
+                att["att_gs"].run(gp.slice(0, att["att_gs"].w_f32.shape[1]), y_f32=ub)
+            ub = ub.view(B, -1)
+        nl = st.num_logits()
+        LOG = torch.empty(B, T, (nl + 3) // 4 * 4, dtype=torch.float32, device=dev)
+        if st.affine_layers == 2:
+            A1 = P.empty((B, T, att["att_x"].cout), dev)
+            att["att_x"].run(M, utt_bias=ub, tanh=True, y=A1)
+            att["att2"].run(A1, y_f32=LOG)
+        else:
+            att["att_x"].run(M, utt_bias=ub, y_f32=LOG)
+        cg = st.head_width()
+        pstat, pp = ops.attn_head_stats_pool_mq(LOG[..., :nl], MF, st.num_q * D, cg if st.share else 1, cg, st.num_q, floor=1e-5,
+                                                planes=True)
+        _mark("attn_head_stats_pool_mq")
+        width = st.get_output_dim()
+        if SMALL_ROWS or len(self.segment) > 1:
+            x = pstat[:, :width].contiguous()
+            for layer in self.segment:
+                x = layer.run_rows(x)
+            return x
+        emb = torch.empty(B, 1, self.embed_dim, dtype=torch.float32, device=dev)
+        self.segment[0].run(pp.slice(0, width), y_f32=emb)
         return emb.view(B, self.embed_dim)
 
     def close(self):

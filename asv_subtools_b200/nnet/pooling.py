@@ -1,6 +1,6 @@
 """Pooling layers mirroring pytorch/libs/nnet/pooling.py: StatisticsPooling (:15-76), LDEPooling (:130-162) and the attention poolings built
 on AttentionAlphaComponent (:214-319) -- AttentiveStatisticsPooling (:322-368), MultiHeadAttentionPooling (:371-440),
-GlobalMultiHeadAttentionPooling (:443-515), MultiResolutionMultiHeadAttentionPooling (:518-587).  Parameter containers
+GlobalMultiHeadAttentionPooling (:443-515), MultiResolutionMultiHeadAttentionPooling (:518-587) and MQMHASP (:589-698).  Parameter containers
 under the reference's state_dict keys; the arithmetic lives in csrc/pooling.cu / csrc/ecapa.cu
 (`xvb_attn_head_stats_pool`) and the wgmma layer kernel, driven by the owning model."""
 import torch
@@ -180,3 +180,45 @@ class MultiResolutionMultiHeadAttentionPooling(_AttentionPooling):
             raise ValueError("temperature==False is not valid for MultiResolutionMultiHeadAttentionPooling.")
         self.attention = AttentionAlphaComponent(input_dim, num_head=num_head, split_input=False, temperature=True,
                                                  share=share, affine_layers=affine_layers, bias=True, **options)
+
+
+class MQMHASP(torch.nn.Module):
+    """Multi-query multi-head attention pooling (pooling.py:589-698): the input's C channels form num_head heads of
+    Cg = C / num_head channels; the attention (grouped convs, groups = num_head then num_head * num_q) gives num_q alphas
+    per head (one per channel of the head, or one shared with `share`); pooled channel (h*num_q + q)*Cg + c is channel
+    h*Cg + c weighted by alpha (h, q[, c]), out = [mean | std] (stddev) or mean.  With `time_attention` the first conv
+    also sees each head's utterance mean and std (biased, clamped at 1e-5).  Same constructor defaults, parameter names
+    and shapes as the reference; the arithmetic runs in the owning ECAPA model's extractor."""
+
+    def __init__(self, in_dim, num_q=2, num_head=4, hidden_size=128, stddev=True, share=True, affine_layers=2,
+                 time_attention=False, norm_type="batch_norm", **kargs):
+        super().__init__()
+        if norm_type != "batch_norm":
+            raise NotImplementedError("MQMHASP norm_type={!r} (GroupNorm in the attention) is not on the B200 path".format(norm_type))
+        if affine_layers not in (1, 2):
+            raise ValueError("Expected 1 or 2 affine layers, but got {}.".format(affine_layers))
+        self.stddev, self.share, self.time_attention, self.affine_layers = stddev, share, time_attention, affine_layers
+        self.num_head, self.num_q, self.hidden_size = max(1, num_head), max(1, num_q), hidden_size
+        assert in_dim % num_head == 0
+        self.in_dim = in_dim
+        head = in_dim // num_head
+        att_idim = ((3 if stddev else 2) if time_attention else 1) * head
+        att_odim = (1 if share else head) * num_head * num_q
+        if affine_layers == 2:
+            hidden = hidden_size * num_head * num_q
+            self.attention = torch.nn.Sequential(
+                torch.nn.Conv1d(att_idim * num_head, hidden, kernel_size=1, groups=num_head), torch.nn.ReLU(),
+                torch.nn.BatchNorm1d(hidden), torch.nn.Tanh(),
+                torch.nn.Conv1d(hidden, att_odim, kernel_size=1, groups=num_head * num_q))
+        else:
+            self.attention = torch.nn.Sequential(torch.nn.Conv1d(att_idim * num_head, att_odim, kernel_size=1, groups=num_head))
+        self.out_dim = in_dim * num_q * (2 if stddev else 1)
+
+    def get_output_dim(self):
+        return self.out_dim
+
+    def head_width(self):
+        return self.in_dim // self.num_head
+
+    def num_logits(self):
+        return (1 if self.share else self.head_width()) * self.num_head * self.num_q

@@ -119,11 +119,17 @@ def fused_pool_layer(x, w, cout, context, bias=None, bn_scale=None, bn_shift=Non
     return (out, op) if planes else out
 
 
+def tdnn_grouped_fits(cin, cout, groups):
+    """True when the layer kernel's grouped mode takes a (cin -> cout, groups) 1x1 conv (xvb_tdnn_grouped_fits)."""
+    return bool(lib.xvb_tdnn_grouped_fits(int(cin), int(cout), int(groups)))
+
+
 def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_shift=None, utt_bias=None, row_bias=None,
-                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False):
+                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False, groups=1):
     """Full form of the wgmma layer (xvb_tdnn_affine_ex).  x / x2: SplitPlanes (B,T,*) (views
     allowed); y: SplitPlanes to write (view allowed) and/or y_f32: fp32 (B,T,>=cout) tensor.  swish: x * sigmoid(x)
-    after the bias (and ReLU), before the BatchNorm (XVB_SWISH)."""
+    after the bias (and ReLU), before the BatchNorm (XVB_SWISH).  groups > 1: grouped 1x1 conv, w the compact packing
+    of the (cout, Cin/groups, 1) weight."""
     b, t = x.hi.shape[0], x.hi.shape[1]
     a = TdnnArgs()
     a.x_hi, a.x_lo, a.ldx = x.hi.data_ptr(), x.lo.data_ptr(), x.ld
@@ -150,6 +156,7 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
     if pool_partial is not None:
         a.pool_partial = pool_partial.data_ptr()
     a.B, a.T, a.Cin, a.Cout = b, t, x.channels, cout
+    a.groups = groups
     check(lib.xvb_tdnn_affine_ex(C.byref(a), _stream()), "xvb_tdnn_affine_ex")
 
 
@@ -426,6 +433,23 @@ def attn_head_stats_pool(logits, x, out_channels, gdiv, floor=1e-10, unweighted_
                                              1 if softplus2log else 0, _ptr(out), op.hi.data_ptr() if op else None,
                                              op.lo.data_ptr() if op else None, 2 * out_channels, _stream()),
           "xvb_attn_head_stats_pool")
+    return (out, op) if planes else out
+
+
+def attn_head_stats_pool_mq(logits, x, out_channels, gdiv, head_width, rep, floor=1e-5, planes=False):
+    """Multi-query multi-head attention pooling (xvb_attn_head_stats_pool_mq): output channel o pools
+    x[..., (o // (rep*head_width))*head_width + o % head_width] with softmax_T(logits[..., o // gdiv]), weighted
+    variance clamped at `floor`.  -> (B, 2*out_channels) [mean | std] (, SplitPlanes)."""
+    for name, v in (("logits", logits), ("x", x)):
+        if v.dtype != torch.float32 or not v.is_cuda or v.dim() != 3 or v.stride(-1) != 1 or v.stride(0) != v.shape[1] * v.stride(1):
+            raise TypeError("{} must be a (B,T,*) CUDA float32 tensor with contiguous rows".format(name))
+    b, t, c = x.shape
+    out = torch.empty(b, 2 * out_channels, dtype=torch.float32, device=x.device)
+    op = SplitPlanes.empty((b, 1, 2 * out_channels), x.device) if planes else None
+    check(lib.xvb_attn_head_stats_pool_mq(_ptr(logits), logits.stride(-2), logits.shape[-1], _ptr(x), x.stride(-2), b, t, c,
+                                          out_channels, int(gdiv), int(head_width), int(rep), floor, 0, _ptr(out),
+                                          op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None,
+                                          2 * out_channels, _stream()), "xvb_attn_head_stats_pool_mq")
     return (out, op) if planes else out
 
 

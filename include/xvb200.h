@@ -131,8 +131,16 @@ typedef struct xvb_tdnn_args {
    * frame matrix (ntaps = 1, Cin = taps*channels), so a [-2..2] layer over 80 channels streams 7
    * channel blocks of 64 instead of 5 x (64 + 16).  Requires x2_* == NULL. */
   int64_t x_batch_stride;
+  /* 0 or 1: dense.  G > 1: grouped 1x1 convolution (Conv1d groups=G): output channels [g*Cout/G, (g+1)*Cout/G)
+   * read only input channels [g*Cin/G, (g+1)*Cin/G) of x, and w is the COMPACT packing of the (Cout, Cin/G, 1)
+   * weight (xvb_pack_tdnn_weight with Cin/G input channels), not its block-diagonal expansion.  Needs
+   * xvb_tdnn_grouped_fits(Cin, Cout, G), one tap, and no x2, pool_partial, x_batch_stride or XVB_SWISH. */
+  int groups;
 } xvb_tdnn_args_t;
 int xvb_tdnn_affine_ex(const xvb_tdnn_args_t* args, void* stream);
+/* 1 when the grouped mode takes this shape: Cin/G a multiple of 64 and Cout/G a multiple of 32 (an N tile of
+ * 128, 64 or 32 channels never straddles two groups); 0 otherwise -- such layers run as block-diagonal expansions. */
+int xvb_tdnn_grouped_fits(int Cin, int Cout, int groups);
 /* Time blocking the fused-pooling epilogue will use for a (B, T) batch. */
 int xvb_pool_partial_blocks(int B, int T, int* frames_per_block);
 /* Merge the fused-pooling partials into StatisticsPooling's output (mode as in xvb_stats_pool_ex):
@@ -234,6 +242,13 @@ int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, int G, cons
                                    int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
                                    const float* prior_x, int softplus2log, float* out, uint16_t* out_hi, uint16_t* out_lo,
                                    int64_t ldo, void* stream);
+/* The same kernel with a head-width map, for multi-query multi-head attention pooling (MQMHASP, libs/nnet/pooling.py:589-
+ * 698): x's C channels form C / head_width heads of head_width channels, each pooled `rep` times (once per query), so
+ * output channel o pools x channel (o / (rep*head_width))*head_width + o % head_width with the alpha of logit o / gdiv.
+ * head_width = C, rep = O / C is xvb_attn_head_stats_pool's map.  head_width % 4 == 0, O == rep * C. */
+int xvb_attn_head_stats_pool_mq(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T, int C,
+                                int O, int gdiv, int head_width, int rep, float floor_, int unweighted_var, float* out,
+                                uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ResNet x-vector, 2-D (pytorch/model/resnet_xvector.py over pytorch/libs/nnet/resnet.py, BasicBlock)
@@ -630,6 +645,15 @@ void xvb_fbank_destroy(xvb_fbank_t* h);
  * ------------------------------------------------------------------------------------------- */
 typedef struct xvb_ecapa xvb_ecapa_t;
 int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, int mfa_dim, int att_hidden, int embed_dim);
+/* Multi-query multi-head attention pooling (MQMHASP, libs/nnet/pooling.py:589-698) instead of the attentive one: call
+ * between create and the first set_layer, with att_hidden = hidden * num_head * num_q.  Then "att_x" is the first
+ * attention conv's x columns as stored, (Cout, mfa_dim / num_head, 1) with groups = num_head (its ReLU + BatchNorm when
+ * affine_layers = 2; the logits themselves when 1); "att_gs" (time_attention only) its [mean_h | std_h] columns as a
+ * block-diagonal (Cout, 2*mfa_dim) matrix over [mean | std] ((Cout, mfa_dim) over the mean without stddev) plus its
+ * bias; "att2" (affine_layers = 2) the second conv, (logits, hidden, 1) with groups = num_head * num_q.  fc1 / fc2 read
+ * the 2 * num_q * mfa_dim pooled statistics (num_q * mfa_dim without stddev). */
+int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int share, int affine_layers, int time_attention,
+                        int stddev);
 int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
                         const float* w_host, const float* bias_host, const float* bn_scale_host,
                         const float* bn_shift_host, int flags);
@@ -648,7 +672,8 @@ int xvb_ecapa_set_gather(xvb_ecapa_t* h, float* const* tables, int ntables, int6
 int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_host, int64_t N, int T, int batch, float* emb_host,
                                  void* stream);
 int xvb_ecapa_last_launches(const xvb_ecapa_t* h);
-/* "XVBE0001" model files: the named layers as handed to xvb_ecapa_set_layer. */
+/* "XVBE0001" model files: the named layers as handed to xvb_ecapa_set_layer; "XVBE0002" for MQMHA models adds the
+ * xvb_ecapa_set_mqmha record.  Both load. */
 int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path);
 int xvb_ecapa_load(xvb_ecapa_t** out, const char* path);
 void xvb_ecapa_destroy(xvb_ecapa_t* h);

@@ -1,6 +1,10 @@
 #!/usr/bin/env python
 """ECAPA-TDNN c1024 throughput (BASELINE configs[2]: 80-d fbank, 300-frame chunks, batch 128) --
-a side measurement, not the bench.py contract line."""
+a side measurement, not the bench.py contract line.
+
+--pooling mqmha: the roadmap launcher's model (runEcapaXvector_roadmap.py:220-250: MQMHASP 2 queries x 2 heads, hidden
+64, share=False, time attention) next to the attentive-pooling model in the same call, and CUDA-event times of its two
+attention GEMMs in the layer kernel's grouped mode against their block-diagonal expansions."""
 import json
 import os
 import sys
@@ -18,9 +22,82 @@ CANON = dict(training=False, extracted_embedding="near",
                                                                         "track_running_stats": True}})
 
 
+def _card():
+    import subprocess
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                           text=True, timeout=60).stdout.strip().splitlines()
+        return q[torch.cuda.current_device()] if q else torch.cuda.get_device_name()
+    except OSError:
+        return torch.cuda.get_device_name()
+
+
+def _rate(ex, xs, steps):
+    for i in range(3):
+        ex.extract(xs[i % len(xs)])
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for i in range(steps):
+        out = ex.extract(xs[i % len(xs)])
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps, out
+
+
+def _gemm_ms(fn, reps=20):
+    fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def main_mqmha(steps):
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import ecapa_mqmha_oracle as mo
+    from asv_subtools_b200 import ops
+    from asv_subtools_b200.model.ecapa_tdnn_xvector import _block_diagonal, _mqmha_attention
+    B, T, F = 128, 300, 80
+    xs = [torch.randn(B, T, F, device="cuda") for _ in range(4)]
+    base = ECAPA_TDNN(F, 10, **CANON)
+    base.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F), 201), strict=True)
+    kw = mo.ROADMAP_KW
+    mq = ECAPA_TDNN(F, 10, training=False, extracted_embedding="near", **kw)
+    mq.load_state_dict(onn.make_state_dict(mo.ecapa_mqmha_spec(kw), 31), strict=True)
+    res = {"card": _card(), "workload": "80-d fbank, 300-frame chunks, batch 128, native extractor"}
+    for name, m in (("ecpa-attentive", base), ("mqmha", mq)):
+        m.cuda().eval()
+        ms, out = _rate(m.extractor(), xs, steps)
+        res[name] = {"ms_per_batch": round(ms, 3), "frames_per_s": round(B * T / (ms * 1e-3)), "finite": bool(torch.isfinite(out).all())}
+    # the two attention GEMMs of the roadmap model at B x T = 128 x 300
+    st = mq.stats
+    D = st.in_dim
+    x = ops.split_f32(torch.randn(B, T, D, device="cuda"))
+    a1 = ops.split_f32(torch.randn(B, T, st.hidden_size * st.num_head * st.num_q, device="cuda"))
+    recs = {r[0]: r for r in _mqmha_attention(st)}
+    for name, src in (("att_x", x), ("att2", a1)):
+        _, w, _, _, _, g = recs[name]
+        w = torch.from_numpy(w).cuda()
+        cout = w.shape[0]
+        y = torch.empty(B, T, cout, device="cuda")
+        wg, wd = ops.pack_tdnn_weight(w, [0]), ops.pack_tdnn_weight(_block_diagonal(w, g).contiguous(), [0])
+        tg = _gemm_ms(lambda: ops.tdnn_affine_ex(src, wg, cout, [0], y_f32=y, groups=g))
+        td = _gemm_ms(lambda: ops.tdnn_affine_ex(src, wd, cout, [0], y_f32=y))
+        res[name + "_gemm_us"] = {"shape": "{}x{}->{} groups {}".format(B * T, src.channels, cout, g),
+                                  "grouped": round(tg * 1e3, 1), "block_diagonal": round(td * 1e3, 1)}
+    print(json.dumps(res))
+
+
 def main():
     B, T, F = 128, 300, 80
-    steps = int(sys.argv[1]) if len(sys.argv) > 1 else 10
+    steps = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 10
+    if "--pooling" in sys.argv and sys.argv[sys.argv.index("--pooling") + 1] == "mqmha":
+        return main_mqmha(steps)
     m = ECAPA_TDNN(F, 10, **CANON)
     m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F), 201), strict=True)
     m.cuda().eval()
