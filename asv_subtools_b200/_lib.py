@@ -32,7 +32,8 @@ class Conv2dArgs(C.Structure):
                 ("ksize", C.c_int), ("stride", C.c_int),
                 ("scale", C.c_void_p), ("shift", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
                 ("relu", C.c_int), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("y_f32", C.c_void_p),
-                ("scale2", C.c_void_p), ("shift2", C.c_void_p), ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p)]
+                ("scale2", C.c_void_p), ("shift2", C.c_void_p), ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p),
+                ("stride_t", C.c_int)]
 
 
 class LayerNormArgs(C.Structure):
@@ -139,6 +140,9 @@ SIGNATURES = {
     "xvb_layer_norm": (_i, [_p, _p]),
     "xvb_rope_attention": (_i, [_p, _i64, _i, _i, _i, _i, _p, _i, _f, _p, _p, _i64, _p]),
     "xvb_conv_module": (_i, [_p, _i64, _i, _i, _i, _p, _p, _i, _p, _p, _i, _f, _i, _p, _p, _i64, _p]),
+    "xvb_bn_relu_planes": (_i, [_p, _p, _i64, _i64, _i, _p, _p, _p, _p, _i64, _p]),
+    "xvb_cam_gate": (_i, [_p, _p, _i64, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p]),
+    "xvb_seg_gate_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),

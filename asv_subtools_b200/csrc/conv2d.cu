@@ -13,7 +13,8 @@
 //     the fewest padded rows); tap (kf, kt) is only a coordinate offset, so TMA's out-of-bounds zero fill is exactly
 //     the convolution's zero padding and never reads a neighbouring utterance;
 //   * stride 2 uses the tensor map's element strides: the box traverses 2*Fb x 2*Tb input positions and lands Fb x Tb
-//     of them, so no output is computed and thrown away;
+//     of them, so no output is computed and thrown away; the two axes take their strides separately (CAM++'s FCM head
+//     strides the feature axis only, stride (2, 1));
 //   * Cin = 32 (the first stage) loads 64-channel boxes whose upper half TMA zero-fills; the MMA loop stops after the
 //     real 32 channels, so the padding costs shared-memory traffic and no tensor-core work;
 //   * numerics and pipeline are the TDNN layer's (tdnn_gemm.cu): bf16 hi/lo planes, three wgmma per K step into fp32
@@ -41,7 +42,7 @@ constexpr int kMaxConvTaps = 25;                 // a 5x5 window
 
 struct Conv2dParams {
   int B, T, F, Cin, To, Fo, Cout;
-  int ks, stride, pad;
+  int ks, stride, stride_t, pad;   // stride: feature axis; stride_t: time axis
   int ntaps;
   int8_t tap_f[kMaxConvTaps], tap_t[kMaxConvTaps];   // (kf, kt) of packed tap j
   int Fb, Tb, Bb, log2_fb, log2_tb;
@@ -127,7 +128,7 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
         const int n0 = n_blk * BLOCK_N;
         for (int tap = 0; tap < p.ntaps; ++tap) {
           const int fi = f0 * p.stride + p.tap_f[tap] - p.pad;
-          const int ti = t0 * p.stride + p.tap_t[tap] - p.pad;
+          const int ti = t0 * p.stride_t + p.tap_t[tap] - p.pad;
           for (int cb = 0; cb < p.num_cblk; ++cb) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* s = smem + stage * kStageBytes;
@@ -334,13 +335,14 @@ int grid_for(long long total, int block) {
 }
 
 // (Fb, Tb, Bb) powers of two with Fb*Tb*Bb = 128 and the fewest padded output rows; ties go to the fewest utterances
-// per tile, then the widest Fb (spatially compact tiles: the 9 taps of one tile overlap in L2).
-void choose_conv_tile(int B, int To, int Fo, int stride, int* Fb, int* Tb, int* Bb) {
+// per tile, then the widest Fb (spatially compact tiles: the 9 taps of one tile overlap in L2).  stride_f / stride_t:
+// the feature / time strides, which scale the TMA box along their axis.
+void choose_conv_tile(int B, int To, int Fo, int stride_f, int stride_t, int* Fb, int* Tb, int* Bb) {
   long long best = -1;
   for (int lb = 0; lb <= 7; ++lb) {
     for (int lf = 7 - lb; lf >= 0; --lf) {
       const int bb = 1 << lb, fb = 1 << lf, tb = 128 / (bb * fb);
-      if (fb * stride > 256 || tb * stride > 256) continue;   // TMA box dimensions <= 256
+      if (fb * stride_f > 256 || tb * stride_t > 256) continue;   // TMA box dimensions <= 256
       const long long rows = (long long)((Fo + fb - 1) / fb) * fb * ((To + tb - 1) / tb) * tb * ((B + bb - 1) / bb) * bb;
       if (best < 0 || rows < best) { best = rows; *Fb = fb; *Tb = tb; *Bb = bb; }
     }
@@ -428,15 +430,17 @@ int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int 
   p.B = a->B; p.T = a->T; p.F = a->F; p.Cin = a->Cin; p.Cout = a->Cout;
   XVB_CHECK_ARG(a->T + 2 * pad >= a->ksize && a->F + 2 * pad >= a->ksize, "%s: T=%d, F=%d shorter than the %dx%d window", fn,
                 a->T, a->F, a->ksize, a->ksize);
-  p.ks = a->ksize; p.stride = a->stride; p.pad = pad;
+  XVB_CHECK_ARG(a->stride_t >= 0 && a->stride_t <= 2, "%s: stride_t must be 0 (same as stride), 1 or 2 (got %d)", fn,
+                a->stride_t);
+  p.ks = a->ksize; p.stride = a->stride; p.stride_t = a->stride_t ? a->stride_t : a->stride; p.pad = pad;
   p.ntaps = ntaps;
   for (int j = 0; j < ntaps; ++j) {
     p.tap_f[j] = (int8_t)(taps[j] / a->ksize);
     p.tap_t[j] = (int8_t)(taps[j] % a->ksize);
   }
-  p.To = (a->T + 2 * pad - a->ksize) / a->stride + 1;   // with pad = k / 2: ceil(T / s) for odd k
+  p.To = (a->T + 2 * pad - a->ksize) / p.stride_t + 1;   // with pad = k / 2: ceil(T / s) for odd k
   p.Fo = (a->F + 2 * pad - a->ksize) / a->stride + 1;
-  choose_conv_tile(p.B, p.To, p.Fo, p.stride, &p.Fb, &p.Tb, &p.Bb);
+  choose_conv_tile(p.B, p.To, p.Fo, p.stride, p.stride_t, &p.Fb, &p.Tb, &p.Bb);
   p.log2_fb = 0;
   while ((1 << p.log2_fb) < p.Fb) ++p.log2_fb;
   p.log2_tb = 0;
@@ -461,8 +465,8 @@ int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int 
   const cuuint64_t C = (cuuint64_t)p.Cin;
   const cuuint64_t dims[4] = {C, (cuuint64_t)p.F, (cuuint64_t)p.T, (cuuint64_t)p.B};
   const cuuint64_t strides[3] = {C * 2, C * 2 * p.F, C * 2 * p.F * p.T};
-  const cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)(p.Fb * p.stride), (cuuint32_t)(p.Tb * p.stride), (cuuint32_t)p.Bb};
-  const cuuint32_t estr[4] = {1u, (cuuint32_t)p.stride, (cuuint32_t)p.stride, 1u};
+  const cuuint32_t box[4] = {(cuuint32_t)kBlockK, (cuuint32_t)(p.Fb * p.stride), (cuuint32_t)(p.Tb * p.stride_t), (cuuint32_t)p.Bb};
+  const cuuint32_t estr[4] = {1u, (cuuint32_t)p.stride, (cuuint32_t)p.stride_t, 1u};
   if ((rc = make_position_map(&mx[0], a->x_hi, dims, strides, box, estr))) return rc;
   if ((rc = make_position_map(&mx[1], a->x_lo, dims, strides, box, estr))) return rc;
 

@@ -1,7 +1,8 @@
 // ECAPA-TDNN specific bandwidth-bound kernels (pytorch/model/ecapa_tdnn_xvector.py):
 //   * plane_mean      : mean over time of a split-plane tensor (SE_Connect's AdaptiveAvgPool1d, :100)
 //   * se_apply        : out = z * gate[b] + in  (+ next = in + out)   (SE_Connect :109-111, SE_Res2Block :149,
-//                       and the dense residual sums x+x1, x+x1+x2 of ECAPA_TDNN.extract_embedding :405-408)
+//                       and the dense residual sums x+x1, x+x1+x2 of ECAPA_TDNN.extract_embedding :405-408);
+//                       with a gate per seg_len-frame segment and no `in`, CAM++'s context-aware mask y * m
 //   * attn_stats_pool : softmax over time + weighted mean / std (AttentiveStatsPool.forward :183-188) as a
 //                       single streaming pass with an online softmax (running max + rescaled sums)
 // All the dense contractions of the model run on the wgmma layer kernel (tdnn_gemm.cu).
@@ -71,22 +72,26 @@ __global__ void copy_rows_kernel(const uint4* __restrict__ src, long long ld_src
 }
 
 // ---------------------------------------------------------------- SE gate + residual (+ running sum)
+// gate[b, t / seg_len, :] scales frame t of utterance b (gate rows: nseg = ceil(T / seg_len) per utterance); seg_len = T
+// is SE_Connect's one gate per utterance.  in NULL: out = z * gate (CAMLayer's y * m, campplus.py:157-162), no add.
 __global__ void se_apply_kernel(const __nv_bfloat16* __restrict__ zh, const __nv_bfloat16* __restrict__ zl, long long ldz,
                                 const __nv_bfloat16* __restrict__ ih, const __nv_bfloat16* __restrict__ il, long long ldi,
                                 const float* __restrict__ gate, __nv_bfloat16* __restrict__ oh,
                                 __nv_bfloat16* __restrict__ ol, long long ldo, __nv_bfloat16* __restrict__ nh,
-                                __nv_bfloat16* __restrict__ nl, long long ldn, long long frames, int T, int C) {
+                                __nv_bfloat16* __restrict__ nl, long long ldn, long long frames, int T, int C, int seg_len) {
   const int groups = C / 8;
+  const int nseg = (T + seg_len - 1) / seg_len;
   const long long total = frames * groups;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long fr = i / groups;
     const int c = (int)(i % groups) * 8;
     const long long b = fr / T;
-    float z[8], x[8], o[8];
+    const long long row = b * nseg + (int)(fr - b * T) / seg_len;
+    float z[8], x[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, o[8];
     unpack8(*reinterpret_cast<const uint4*>(zh + fr * ldz + c), *reinterpret_cast<const uint4*>(zl + fr * ldz + c), z);
-    unpack8(*reinterpret_cast<const uint4*>(ih + fr * ldi + c), *reinterpret_cast<const uint4*>(il + fr * ldi + c), x);
-    const float4 g0 = *reinterpret_cast<const float4*>(gate + b * C + c);
-    const float4 g1 = *reinterpret_cast<const float4*>(gate + b * C + c + 4);
+    if (ih) unpack8(*reinterpret_cast<const uint4*>(ih + fr * ldi + c), *reinterpret_cast<const uint4*>(il + fr * ldi + c), x);
+    const float4 g0 = *reinterpret_cast<const float4*>(gate + row * C + c);
+    const float4 g1 = *reinterpret_cast<const float4*>(gate + row * C + c + 4);
     const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
     for (int k = 0; k < 8; ++k) o[k] = z[k] * g[k] + x[k];   // mul then add: the reference's two roundings
@@ -102,6 +107,23 @@ __global__ void se_apply_kernel(const __nv_bfloat16* __restrict__ zh, const __nv
       *reinterpret_cast<uint4*>(nl + fr * ldn + c) = l;
     }
   }
+}
+
+int launch_se_apply(const uint16_t* z_hi, const uint16_t* z_lo, int64_t ldz, const uint16_t* in_hi, const uint16_t* in_lo,
+                    int64_t ldin, const float* gate, int seg_len, uint16_t* out_hi, uint16_t* out_lo, int64_t ldout,
+                    uint16_t* next_hi, uint16_t* next_lo, int64_t ldnext, int B, int T, int C, void* stream) {
+  const long long frames = (long long)B * T;
+  const long long total = frames * (C / 8);
+  long long g = (total + 255) / 256;
+  const long long cap = (long long)sm_count() * 32;
+  if (g > cap) g = cap;
+  se_apply_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(z_hi), reinterpret_cast<const __nv_bfloat16*>(z_lo), ldz,
+      reinterpret_cast<const __nv_bfloat16*>(in_hi), reinterpret_cast<const __nv_bfloat16*>(in_lo), ldin, gate,
+      reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldout,
+      reinterpret_cast<__nv_bfloat16*>(next_hi), reinterpret_cast<__nv_bfloat16*>(next_lo), ldnext, frames, T, C, seg_len);
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
 }
 
 // ---------------------------------------------------------------- attentive statistics pooling
@@ -697,18 +719,23 @@ extern "C" int xvb_se_apply(const uint16_t* z_hi, const uint16_t* z_lo, int64_t 
   XVB_CHECK_ARG((next_hi != nullptr) == (next_lo != nullptr), "xvb_se_apply: next_hi/next_lo must both be set or both NULL");
   XVB_CHECK_ARG(B > 0 && T > 0 && C > 0 && C % 8 == 0 && ldz % 8 == 0 && ldin % 8 == 0 && ldout % 8 == 0 &&
                     (!next_hi || ldnext % 8 == 0), "xvb_se_apply: C and all pitches must be multiples of 8");
-  const long long frames = (long long)B * T;
-  const long long total = frames * (C / 8);
-  long long g = (total + 255) / 256;
-  const long long cap = (long long)sm_count() * 32;
-  if (g > cap) g = cap;
-  se_apply_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(z_hi), reinterpret_cast<const __nv_bfloat16*>(z_lo), ldz,
-      reinterpret_cast<const __nv_bfloat16*>(in_hi), reinterpret_cast<const __nv_bfloat16*>(in_lo), ldin, gate,
-      reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldout,
-      reinterpret_cast<__nv_bfloat16*>(next_hi), reinterpret_cast<__nv_bfloat16*>(next_lo), ldnext, frames, T, C);
-  XVB_LAUNCH_CHECK();
-  return XVB_OK;
+  return launch_se_apply(z_hi, z_lo, ldz, in_hi, in_lo, ldin, gate, T, out_hi, out_lo, ldout, next_hi, next_lo, ldnext, B, T, C,
+                         stream);
+}
+
+extern "C" int xvb_seg_gate_apply(const uint16_t* z_hi, const uint16_t* z_lo, int64_t ldz, const uint16_t* in_hi,
+                                  const uint16_t* in_lo, int64_t ldin, const float* gate, int seg_len, uint16_t* out_hi,
+                                  uint16_t* out_lo, int64_t ldout, int B, int T, int C, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(z_hi && z_lo && gate && out_hi && out_lo, "xvb_seg_gate_apply: null pointer");
+  XVB_CHECK_ARG((in_hi != nullptr) == (in_lo != nullptr), "xvb_seg_gate_apply: in_hi/in_lo must both be set or both NULL");
+  XVB_CHECK_ARG(B > 0 && T > 0 && C > 0 && seg_len > 0 && C % 8 == 0 && ldz % 8 == 0 && ldout % 8 == 0 && (!in_hi || ldin % 8 == 0),
+                "xvb_seg_gate_apply: need seg_len > 0, C and all pitches multiples of 8");
+  XVB_CHECK_ARG(((uintptr_t)z_hi | (uintptr_t)z_lo | (uintptr_t)in_hi | (uintptr_t)in_lo | (uintptr_t)gate | (uintptr_t)out_hi |
+                 (uintptr_t)out_lo) % 16 == 0, "xvb_seg_gate_apply: pointers must be 16-byte aligned");
+  return launch_se_apply(z_hi, z_lo, ldz, in_hi, in_lo, ldin, gate, seg_len, out_hi, out_lo, ldout, nullptr, nullptr, 0, B, T, C,
+                         stream);
 }
 
 extern "C" int xvb_attn_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C,

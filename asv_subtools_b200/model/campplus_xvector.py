@@ -1,0 +1,419 @@
+# -*- coding:utf-8 -*-
+"""CAM++ x-vector blueprint for the native path -- the backbone of subtools2/egrecho/models/campplus/ (CamPP, campplus.py
+:288-359; CamPPModel.extract_embedding, model.py:73-96) with the CamPPConfig defaults (campplus_config.py:11-37).
+
+Creation string: CamPPXvector(inputs_dim, num_targets, embd_dim=512, init_channels=128, growth_rate=32, bn_size=4,
+memory_efficient=True); num_targets (the classifier's classes) and memory_efficient (gradient checkpointing) only matter in
+training.  The state_dict is CamPP's key for key (`head.*`, `xvector.*`), so a backbone state_dict loads with strict=True;
+a CamPPModel state_dict (`cam.*` + `classifier.*`, e.g. torch.load(ckpt)["state_dict"] of a trained egrecho checkpoint)
+loads too: `cam.` is stripped and `classifier.*` dropped.  A dict that carries none of the backbone keys is refused even
+with strict=False, so that an unloaded model never writes embeddings.
+
+At extraction (CamPPExtractor) the FCM head runs on the 2-D conv kernels (xvb_conv2d_head, xvb_conv2d with stride (2, 1)
+and the BasicResBlock epilogue), the stride-2 `tdnn` on the layer kernel's im2col view over a time-padded copy of the head's
+output, every dense layer as BN1 -> ReLU (xvb_bn_relu_planes) -> linear1 with BN2 folded in -> the per-segment
+context-aware mask (xvb_cam_gate) -> linear_local -> y * m written into the layer's column slice of the block's
+concatenation buffer (xvb_seg_gate_apply); transit3 carries out_nonlinear, xvb_stats_pool_ex takes [mean | unbiased std];
+dense is xvb_small_affine.  extract_embedding applies CamPPModel's 4000-frame chunk rule (XvectorMixin.split_chunks with
+even=False)."""
+import os
+import sys
+from collections import OrderedDict
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
+
+from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
+from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
+
+MAX_CHUNK = 4000      # CamPPModel.extract_embedding(max_chunk=4000)
+MIN_FRAMES = 3        # T' = ceil(T / 2) >= 2 frames: the unbiased std of one frame is NaN
+SEG_LEN = 100         # CAMLayer.seg_pooling's segment length
+BLOCKS = ((12, 1), (24, 2), (16, 2))   # (layers, dilation) of the three CAMDenseTDNNBlocks, kernel size 3
+M_CHANNELS = 32       # FCM's m_channels
+
+
+def chunk_sizes(num_frames, max_chunk=MAX_CHUNK):
+    """XvectorMixin.split_chunks(max_chunk, even=False) sizes (xvector.py:78-103 over get_chunksize): max_chunk-long
+    chunks, then the last two re-split evenly, the first of them taking the odd frame (9000 -> [4000, 2500, 2500],
+    4001 -> [2001, 2000])."""
+    q, r = divmod(int(num_frames), max_chunk)
+    n = q + (1 if r else 0)
+    sizes = [max_chunk] * (n - 1) + [int(num_frames) - max_chunk * (n - 1)]
+    if len(sizes) > 1:
+        two = sizes.pop() + sizes.pop()
+        sizes += [two - two // 2, two // 2]
+    return sizes
+
+
+def _bn_relu(channels):
+    return nn.Sequential(OrderedDict([("batchnorm", nn.BatchNorm1d(channels)), ("relu", nn.ReLU())]))
+
+
+class _BasicResBlock(nn.Module):
+    """Post-activation residual block; stride (s, 1) strides the feature axis only."""
+
+    def __init__(self, in_planes, planes, stride):
+        super().__init__()
+        self.stride = stride
+        self.conv1 = nn.Conv2d(in_planes, planes, 3, stride=(stride, 1), padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, stride=1, padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(planes)
+        self.shortcut = nn.Sequential()
+        if stride != 1 or in_planes != planes:
+            self.shortcut = nn.Sequential(nn.Conv2d(in_planes, planes, 1, stride=(stride, 1), bias=False), nn.BatchNorm2d(planes))
+
+
+class _FCM(nn.Module):
+    """The 2-D front end: conv1, layer1 / layer2 of two blocks each (first stride (2, 1)), conv2 stride (2, 1)."""
+
+    def __init__(self, feat_dim, m=M_CHANNELS):
+        super().__init__()
+        self.conv1 = nn.Conv2d(1, m, 3, stride=1, padding=1, bias=False)
+        self.bn1 = nn.BatchNorm2d(m)
+        self.layer1 = nn.Sequential(_BasicResBlock(m, m, 2), _BasicResBlock(m, m, 1))
+        self.layer2 = nn.Sequential(_BasicResBlock(m, m, 2), _BasicResBlock(m, m, 1))
+        self.conv2 = nn.Conv2d(m, m, 3, stride=(2, 1), padding=1, bias=False)
+        self.bn2 = nn.BatchNorm2d(m)
+        self.out_channels = m * (feat_dim // 8)
+
+
+class _TDNNBlock(nn.Module):
+    """Conv1d -> BatchNorm -> ReLU (pre_norm) or, for `dense`, Conv1d -> (Identity, BatchNorm without affine)."""
+
+    def __init__(self, cin, cout, kernel_size=1, stride=1, bias=True, dense=False):
+        super().__init__()
+        self.linear = nn.Conv1d(cin, cout, kernel_size, stride=stride, padding=(kernel_size - 1) // 2, bias=bias)
+        if dense:
+            self.nonlinear = nn.Sequential(nn.Identity(), nn.BatchNorm1d(cout, affine=False))
+        else:
+            self.nonlinear = nn.Sequential(nn.BatchNorm1d(cout), nn.ReLU())
+
+
+class _CAMLayer(nn.Module):
+    def __init__(self, bn_channels, out_channels, dilation):
+        super().__init__()
+        self.linear_local = nn.Conv1d(bn_channels, out_channels, 3, padding=dilation, dilation=dilation, bias=False)
+        self.linear1 = nn.Conv1d(bn_channels, bn_channels // 2, 1)
+        self.relu = nn.ReLU()
+        self.linear2 = nn.Conv1d(bn_channels // 2, out_channels, 1)
+        self.sigmoid = nn.Sigmoid()
+
+
+class _DenseLayer(nn.Module):
+    def __init__(self, cin, growth, bn_channels, dilation):
+        super().__init__()
+        self.dilation = dilation
+        self.nonlinear1 = _bn_relu(cin)
+        self.linear1 = nn.Conv1d(cin, bn_channels, 1, bias=False)
+        self.nonlinear2 = _bn_relu(bn_channels)
+        self.cam_layer = _CAMLayer(bn_channels, growth, dilation)
+
+
+class _DenseBlock(nn.ModuleList):
+    def __init__(self, layers, cin, growth, bn_channels, dilation):
+        super().__init__()
+        for i in range(layers):
+            self.add_module("tdnnd%d" % (i + 1), _DenseLayer(cin + i * growth, growth, bn_channels, dilation))
+
+
+class _TransitLayer(nn.Module):
+    def __init__(self, cin, cout):
+        super().__init__()
+        self.nonlinear = _bn_relu(cin)
+        self.linear = nn.Conv1d(cin, cout, 1, bias=False)
+
+
+def _unsupported(name, value, why):
+    raise NotImplementedError("{}={!r} is not on the native CAM++ path: {}".format(name, value, why))
+
+
+def backbone_state_dict(state_dict):
+    """CamPP's keys from a CamPP or CamPPModel state_dict: `cam.` is stripped, `classifier.*` dropped.  Raises when none of
+    the backbone keys is there."""
+    if any(k.startswith("cam.") for k in state_dict):
+        state_dict = OrderedDict((k[4:] if k.startswith("cam.") else k, v) for k, v in state_dict.items()
+                                 if not k.startswith("classifier."))
+    if not any(k.startswith("head.") or k.startswith("xvector.") for k in state_dict):
+        raise KeyError("the state_dict carries none of the CAM++ backbone keys (head.*, xvector.* or cam.head.*, "
+                       "cam.xvector.*); a Lightning checkpoint keeps them under its 'state_dict' entry")
+    return state_dict
+
+
+class CamPPXvector(TopVirtualNnet):
+    """CAM++: FCM 2-D head, densely connected TDNN blocks with context-aware masking, statistics pooling, dense."""
+
+    def init(self, inputs_dim, num_targets, embd_dim=512, init_channels=128, growth_rate=32, bn_size=4,
+             memory_efficient=True):
+        if inputs_dim % 8:
+            raise ValueError("inputs_dim={} must be a multiple of 8: the FCM head halves F three times and reshapes to "
+                             "32 * (F // 8) channels".format(inputs_dim))
+        bn_channels = bn_size * growth_rate
+        if growth_rate % 8:
+            _unsupported("growth_rate", growth_rate, "each layer's column slice must start at a multiple of 8")
+        if init_channels % 8:
+            _unsupported("init_channels", init_channels, "the first block's width must be a multiple of 8")
+        self.inputs_dim, self.embd_dim = inputs_dim, embd_dim
+        self.growth_rate, self.bn_channels = growth_rate, bn_channels
+        self.head = _FCM(inputs_dim)
+        xv = OrderedDict([("tdnn", _TDNNBlock(self.head.out_channels, init_channels, 5, stride=2))])
+        channels = init_channels
+        self.widths = []
+        for i, (layers, dilation) in enumerate(BLOCKS):
+            xv["block%d" % (i + 1)] = _DenseBlock(layers, channels, growth_rate, bn_channels, dilation)
+            channels += layers * growth_rate
+            self.widths.append(channels)
+            if i < 2 and (channels // 2) % 8:
+                _unsupported("init_channels", init_channels, "transit{} gives {} channels, not a multiple of 8"
+                             .format(i + 1, channels // 2))
+            xv["transit%d" % (i + 1)] = _TransitLayer(channels, channels // 2)
+            channels //= 2
+        xv["out_nonlinear"] = _bn_relu(channels)
+        xv["dense"] = _TDNNBlock(channels * 2, embd_dim, 1, bias=False, dense=True)
+        self.xvector = nn.Sequential(xv)
+
+    def load_state_dict(self, state_dict, strict=True, **kw):
+        return super().load_state_dict(backbone_state_dict(state_dict), strict=strict, **kw)
+
+    def build_extractor(self):
+        return CamPPExtractor(self, self.device_for_extraction())
+
+    def _check(self, frames, feat_dim):
+        if feat_dim != self.inputs_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.inputs_dim, feat_dim))
+        if frames < MIN_FRAMES:
+            raise ValueError("CAM++ needs at least {} frames (the unbiased std over ceil(T / 2) frames), got {}"
+                             .format(MIN_FRAMES, frames))
+
+    def extract_embedding(self, feats):
+        """feats (T, F) float32 -> 1-D CPU float32 tensor with CamPPModel's 4000-frame chunk rule."""
+        return self.extract_embedding_batch(torch.as_tensor(np.asarray(feats) if not isinstance(feats, torch.Tensor)
+                                                            else feats)[None])[0].cpu()
+
+    def extract_embedding_batch(self, feats):
+        """Equal-length utterances (B, T, F) float32 -> (B, embd_dim) CUDA tensor, the same arithmetic as B calls of
+        extract_embedding(): each chunk position of chunk_sizes(T) runs as one batch, and the chunk embeddings are
+        combined as sum_i size_i * emb_i / T in chunk order."""
+        with torch.no_grad():
+            x = torch.as_tensor(feats)
+            if x.dtype != torch.float32:
+                raise TypeError("extract_embedding_batch expects float32 features")
+            B, T, Fd = x.shape
+            self._check(T, Fd)
+            x = x.to(self.device_for_extraction(), non_blocking=True)
+            ex = self.extractor()
+            acc, off = None, 0
+            sizes = chunk_sizes(T)
+            for s in sizes:
+                e = ex.extract(x[:, off:off + s].contiguous())
+                acc = e * s if acc is None else acc + s * e
+                off += s
+            return acc / sum(sizes)
+
+
+def tdnn_im2col_weight(weight, channels, freq):
+    """`tdnn`'s Conv1d weight (Cout, channels * freq, 5) in the reference's input order c * freq + f -> (Cout, 5 * freq *
+    channels) with K index k * freq * channels + f * channels + c: the window of 5 consecutive frames of the (B, T, F'',
+    C) head output as the layer kernel's im2col view reads it."""
+    cout = weight.shape[0]
+    w = weight.reshape(cout, channels, freq, -1)          # (o, c, f, k)
+    return w.permute(0, 3, 2, 1).reshape(cout, -1)        # (o, k, f, c)
+
+
+def _fold(w, bn, bias=None):
+    """Weight (Cout, ...) and bias of conv -> eval BatchNorm as one affine: (scale * w, scale * bias + shift)."""
+    s, t = fold_batchnorm(bn)
+    s, t = torch.from_numpy(s).to(w.device), torch.from_numpy(t).to(w.device)
+    b = t if bias is None else s * bias.detach().float() + t
+    return w.detach().float() * s.view(-1, *([1] * (w.dim() - 1))), b
+
+
+class _Conv:
+    """A bias-free Conv2d packed for xvb_conv2d, with its eval BatchNorm as the epilogue's scale / shift."""
+
+    def __init__(self, conv, bn, device):
+        self.w = ops.pack_conv2d_weight(conv.weight.detach().float().to(device).contiguous())
+        s, t = fold_batchnorm(bn)
+        self.scale, self.shift = torch.from_numpy(s).to(device), torch.from_numpy(t).to(device)
+
+
+class _Lin:
+    """A kernel-size-1 (or dilated k = 3) Conv1d packed for the layer kernel, with its bias and ReLU."""
+
+    def __init__(self, w, bias, device, context=(0,), relu=False):
+        w = w.detach().float().to(device)
+        self.cout = w.shape[0]
+        self.context = list(context)
+        w = w.reshape(self.cout, w.shape[1], -1)
+        span = self.context[-1] - self.context[0] + 1
+        if w.shape[2] != span:              # a dilated kernel: the packer takes the whole span, the gaps as zero taps
+            full = torch.zeros(self.cout, w.shape[1], span, device=device)
+            full[:, :, [c - self.context[0] for c in self.context]] = w
+            w = full
+        self.w = ops.pack_tdnn_weight(w.contiguous(), self.context)
+        self.bias = bias.detach().float().to(device).contiguous() if bias is not None else None
+        self.relu = relu
+
+    def run(self, x, **kw):
+        ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, relu=self.relu, **kw)
+
+
+def _vec(t, device):
+    return torch.as_tensor(t).detach().float().to(device).contiguous()
+
+
+class CamPPExtractor:
+    """Folded weights on one device + the launch sequence of CamPP.forward for one chunk per utterance (all utterances of
+    a call have the same length), driven from Python over a workspace reused while the batch shape stays the same."""
+
+    def __init__(self, m, device):
+        self.device, self.feat_dim, self.embed_dim = device, m.inputs_dim, m.embd_dim
+        self.f8 = m.inputs_dim // 8
+        h = m.head
+        s1, t1 = fold_batchnorm(h.bn1)
+        self.conv1 = (_vec(h.conv1.weight, device), _vec(s1, device), _vec(t1, device))   # fp32 as stored: xvb_conv2d_head
+        self.res_blocks = []
+        for layer in (h.layer1, h.layer2):
+            for blk in layer:
+                sc = _Conv(blk.shortcut[0], blk.shortcut[1], device) if len(blk.shortcut) else None
+                self.res_blocks.append((blk.stride, _Conv(blk.conv1, blk.bn1, device), _Conv(blk.conv2, blk.bn2, device), sc))
+        self.conv2 = _Conv(h.conv2, h.bn2, device)
+        xv = m.xvector
+        w, b = _fold(tdnn_im2col_weight(xv.tdnn.linear.weight.detach().float(), M_CHANNELS, self.f8).to(device),
+                     xv.tdnn.nonlinear[0], xv.tdnn.linear.bias.to(device))
+        self.tdnn = _Lin(w, b, device, relu=True)
+        self.g, self.bn_ch = m.growth_rate, m.bn_channels
+        self.blocks, self.transits = [], []
+        for i, (layers, dilation) in enumerate(BLOCKS):
+            blk = getattr(xv, "block%d" % (i + 1))
+            L = []
+            for layer in blk:
+                s1, t1 = fold_batchnorm(layer.nonlinear1.batchnorm)
+                w1, b1 = _fold(layer.linear1.weight.to(device), layer.nonlinear2.batchnorm)
+                cam = layer.cam_layer
+                L.append({"s1": _vec(s1, device), "t1": _vec(t1, device), "lin1": _Lin(w1, b1, device, relu=True),
+                          "local": _Lin(cam.linear_local.weight, None, device, context=(-dilation, 0, dilation)),
+                          "gate": tuple(_vec(p.reshape(p.shape[0], -1), device) for p in
+                                        (cam.linear1.weight, cam.linear1.bias, cam.linear2.weight, cam.linear2.bias))})
+            self.blocks.append(L)
+            tr = getattr(xv, "transit%d" % (i + 1))
+            s, t = fold_batchnorm(tr.nonlinear.batchnorm)
+            if i < 2:
+                lin = _Lin(tr.linear.weight, None, device)
+            else:                                   # out_nonlinear's BN -> ReLU folded into transit3
+                wt, bt = _fold(tr.linear.weight.to(device), xv.out_nonlinear.batchnorm)
+                lin = _Lin(wt, bt, device, relu=True)
+            self.transits.append((_vec(s, device), _vec(t, device), lin))
+        self.widths = list(m.widths)
+        ds, dt = fold_batchnorm(xv.dense.nonlinear[1])
+        self.dense = (_vec(xv.dense.linear.weight.reshape(self.embed_dim, -1), device), _vec(ds, device), _vec(dt, device))
+        self._ws_key, self._ws = None, None
+        self.last_launches = 0
+
+    def _workspace(self, B, T):
+        if self._ws_key != (B, T):
+            self._ws = None                 # release the old shape's buffers first
+            P, dev, m = ops.SplitPlanes, self.device, M_CHANNELS
+            T2 = (T + 1) // 2
+            F, ws = self.feat_dim, {}
+            ws["x0"] = P.empty((B, T, F, m), dev)
+            for j, (stride, _, _, sc) in enumerate(self.res_blocks):
+                F = (F + 1) // 2 if stride == 2 else F
+                ws["a%d" % j], ws["o%d" % j] = P.empty((B, T, F, m), dev), P.empty((B, T, F, m), dev)
+                ws["s%d" % j] = P.empty((B, T, F, m), dev) if sc is not None else None
+            ws["c2"] = P.empty((B, T, self.f8, m), dev)
+            row = self.f8 * m
+            # 2 zero frames before and after every utterance: F.pad of the stride-2 conv, written once
+            ws["pad"] = P(torch.zeros(B, T + 4, row, dtype=torch.bfloat16, device=dev),
+                          torch.zeros(B, T + 4, row, dtype=torch.bfloat16, device=dev), row)
+            ws["bufs"] = [P.empty((B, T2, w), dev) for w in self.widths]
+            ws["pre"] = P.empty((B, T2, max(self.widths)), dev)
+            ws["h"] = P.empty((B, T2, self.bn_ch), dev)
+            ws["z"] = P.empty((B, T2, self.g), dev)
+            ws["pool_in"] = torch.empty(B, T2, self.transits[-1][2].cout, dtype=torch.float32, device=dev)
+            ws["gate"] = torch.empty(B, (T2 + SEG_LEN - 1) // SEG_LEN, self.g, dtype=torch.float32, device=dev)
+            self._ws_key, self._ws = (B, T), ws
+        return self._ws
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embd_dim) fp32 CUDA, asynchronous on the current
+        stream."""
+        B, T, Fd = feats.shape
+        if Fd != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, Fd))
+        if T < MIN_FRAMES:
+            raise ValueError("CAM++ needs at least {} frames, got {}".format(MIN_FRAMES, T))
+        feats = feats.contiguous()
+        ws = self._workspace(B, T)
+        P, m = ops.SplitPlanes, M_CHANNELS
+        ops.conv2d_head(feats, *self.conv1, ws["x0"])
+        n = 1
+        x = ws["x0"]
+        for j, (stride, c1, c2, sc) in enumerate(self.res_blocks):
+            res = x
+            if sc is not None:
+                res = ws["s%d" % j]
+                ops.conv2d(x, sc.w, m, 1, stride, sc.scale, sc.shift, y=res, stride_t=1)
+                n += 1
+            ops.conv2d(x, c1.w, m, 3, stride, c1.scale, c1.shift, relu=True, y=ws["a%d" % j], stride_t=1)
+            ops.conv2d(ws["a%d" % j], c2.w, m, 3, 1, c2.scale, c2.shift, res=res, relu=True, y=ws["o%d" % j])
+            n += 2
+            x = ws["o%d" % j]
+        c = self.conv2
+        ops.conv2d(x, c.w, m, 3, 2, c.scale, c.shift, relu=True, y=ws["c2"], stride_t=1)
+        # the head output into the time-padded copy: one row of T * F'' * C elements per utterance
+        row = self.f8 * m
+        pad, src = ws["pad"], ws["c2"]
+        ops.copy_planes(P(src.hi.view(B, 1, T * row), src.lo.view(B, 1, T * row), T * row),
+                        P(pad.hi.view(B, 1, -1)[..., 2 * row:(T + 2) * row], pad.lo.view(B, 1, -1)[..., 2 * row:(T + 2) * row],
+                          T * row))
+        n += 4
+        # tdnn: Conv1d(k = 5, stride 2, padding 2) as a 1-tap layer over 5-frame windows that start every 2 frames
+        T2 = (T + 1) // 2
+        win = P(pad.hi.as_strided((B, T2, 2 * row), ((T + 4) * row, 2 * row, 1)),
+                pad.lo.as_strided((B, T2, 2 * row), ((T + 4) * row, 2 * row, 1)), 5 * row)
+        bufs, pre = ws["bufs"], ws["pre"]
+        self.tdnn.run(win, y=bufs[0].slice(0, self.tdnn.cout), x_batch_stride=(T + 4) * row)
+        n += 1
+        c0 = self.tdnn.cout
+        h, z, gate = ws["h"], ws["z"], ws["gate"]
+        for bi, layers in enumerate(self.blocks):
+            buf = bufs[bi]
+            for li, L in enumerate(layers):
+                cin = c0 + li * self.g
+                xin = buf.slice(0, cin)
+                pv = pre.slice(0, cin)
+                ops.bn_relu_planes(xin, L["s1"], L["t1"], pv)
+                L["lin1"].run(pv, y=h)
+                ops.cam_gate(h, *L["gate"], seg_len=SEG_LEN, out=gate)
+                L["local"].run(h, y=z)
+                ops.seg_gate_apply(z, gate, SEG_LEN, buf.slice(cin, cin + self.g))
+                n += 5
+            s, t, lin = self.transits[bi]
+            width = self.widths[bi]
+            pv = pre.slice(0, width)
+            ops.bn_relu_planes(buf if buf.channels == width else buf.slice(0, width), s, t, pv)
+            n += 1
+            if bi + 1 < len(self.blocks):
+                lin.run(pv, y=bufs[bi + 1].slice(0, lin.cout))
+                n += 1
+                c0 = lin.cout
+            else:
+                # out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance.  Not the fused
+                # pooling epilogue: its time blocking follows the batch shape, so a batch would not reproduce
+                # per-utterance calls bit for bit; the fp32 round trip costs ~80 MB of traffic at 128 x 300.
+                lin.run(pv, y_f32=ws["pool_in"])
+                stats = ops.stats_pool_ex(ws["pool_in"], 0.0, 1)
+                n += 2
+        wd, sd, td = self.dense
+        emb = ops.small_affine(stats, wd, bn_scale=sd, bn_shift=td)
+        self.last_launches = n + 1
+        return emb
+
+    def close(self):
+        self._ws_key, self._ws = None, None

@@ -125,11 +125,13 @@ def tdnn_grouped_fits(cin, cout, groups):
 
 
 def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_shift=None, utt_bias=None, row_bias=None,
-                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False, groups=1):
+                   relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False, groups=1,
+                   x_batch_stride=0):
     """Full form of the wgmma layer (xvb_tdnn_affine_ex).  x / x2: SplitPlanes (B,T,*) (views
     allowed); y: SplitPlanes to write (view allowed) and/or y_f32: fp32 (B,T,>=cout) tensor.  swish: x * sigmoid(x)
     after the bias (and ReLU), before the BatchNorm (XVB_SWISH).  groups > 1: grouped 1x1 conv, w the compact packing
-    of the (cout, Cin/groups, 1) weight."""
+    of the (cout, Cin/groups, 1) weight.  x_batch_stride > 0: x is an im2col view (xvb_tdnn_args_t.x_batch_stride):
+    frame t of utterance b is the x.channels-long window at element b * x_batch_stride + t * x.ld of the planes."""
     b, t = x.hi.shape[0], x.hi.shape[1]
     a = TdnnArgs()
     a.x_hi, a.x_lo, a.ldx = x.hi.data_ptr(), x.lo.data_ptr(), x.ld
@@ -157,6 +159,7 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
         a.pool_partial = pool_partial.data_ptr()
     a.B, a.T, a.Cin, a.Cout = b, t, x.channels, cout
     a.groups = groups
+    a.x_batch_stride = x_batch_stride
     check(lib.xvb_tdnn_affine_ex(C.byref(a), _stream()), "xvb_tdnn_affine_ex")
 
 
@@ -197,6 +200,42 @@ def se_apply(z, xin, gate, out, nxt=None):
                            nxt.ld if nxt else 0, b, t, c, _stream()), "xvb_se_apply")
 
 
+def seg_gate_apply(z, gate, seg_len, out, xin=None):
+    """out = z * gate[b, t // seg_len] [+ xin] (xvb_seg_gate_apply): z, out, xin SplitPlanes (B, T, C) views; gate
+    (B, ceil(T / seg_len), C) fp32."""
+    b, t, c = z.hi.shape[0], z.hi.shape[1], z.channels
+    gate = _req(gate, torch.float32, "gate")
+    ih, il = _planes_ptrs(xin)
+    check(lib.xvb_seg_gate_apply(z.hi.data_ptr(), z.lo.data_ptr(), z.ld, ih, il, xin.ld if xin is not None else 0, _ptr(gate),
+                                 int(seg_len), out.hi.data_ptr(), out.lo.data_ptr(), out.ld, b, t, c, _stream()),
+          "xvb_seg_gate_apply")
+
+
+def bn_relu_planes(x, scale, shift, y):
+    """y = relu(x * scale + shift) (xvb_bn_relu_planes): x, y SplitPlanes (B, T, C) views (any pitch), scale / shift (C,)."""
+    rows = x.hi.numel() // x.hi.shape[-1]
+    check(lib.xvb_bn_relu_planes(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, rows, x.channels,
+                                 _ptr(_req(scale, torch.float32, "scale")), _ptr(_req(shift, torch.float32, "shift")),
+                                 y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_bn_relu_planes")
+
+
+def cam_gate(h, w1, b1, w2, b2, seg_len=100, out=None):
+    """CAMLayer's per-segment mask (xvb_cam_gate): h SplitPlanes (B, T, C); w1 (R, C), b1 (R,), w2 (G, R), b2 (G,) fp32
+    -> gate (B, ceil(T / seg_len), G) fp32 (written into `out` when given)."""
+    b, t, c = h.hi.shape[0], h.hi.shape[1], h.channels
+    w1, w2 = _req(w1, torch.float32, "w1"), _req(w2, torch.float32, "w2")
+    r, g = w1.shape[0], w2.shape[0]
+    nseg = (t + seg_len - 1) // seg_len
+    if out is None:
+        out = torch.empty(b, nseg, g, dtype=torch.float32, device=h.hi.device)
+    elif _req(out, torch.float32, "out").shape != (b, nseg, g):
+        raise ValueError("out must be ({}, {}, {})".format(b, nseg, g))
+    check(lib.xvb_cam_gate(h.hi.data_ptr(), h.lo.data_ptr(), h.ld, b, t, c, int(seg_len), _ptr(w1),
+                           _ptr(_req(b1, torch.float32, "b1")), r, _ptr(w2), _ptr(_req(b2, torch.float32, "b2")), g, _ptr(out),
+                           _stream()), "xvb_cam_gate")
+    return out
+
+
 def _planes_ptrs(p):
     return (p.hi.data_ptr(), p.lo.data_ptr()) if p is not None else (None, None)
 
@@ -224,9 +263,10 @@ def pack_conv2d_weight(weight, taps=None):
 
 
 def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=False, y=None, y_f32=None,
-           scale2=None, shift2=None, y2=None, taps=None, valid=False):
+           scale2=None, shift2=None, y2=None, taps=None, valid=False, stride_t=0):
     """One 2-D convolution (xvb_conv2d): x SplitPlanes (B, T, F, Cin); w from pack_conv2d_weight; res / y / y2
     SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride).
+    stride_t: the time axis's own stride (0: `stride`; CAM++'s FCM head uses stride=2, stride_t=1).
     taps: only these taps (kf*ksize + kt, strictly increasing, ksize 1, 3 or 5) are computed, with w packed by
     pack_conv2d_weight(weight, taps) (xvb_conv2d_taps).  valid: no padding, T' = (T - k) // stride + 1 and F' likewise
     (xvb_conv2d_valid; dense taps only)."""
@@ -234,7 +274,7 @@ def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=F
     a = _lib.Conv2dArgs()
     a.x_hi, a.x_lo = _planes_ptrs(x)
     a.w_hi, a.w_lo = w.hi.data_ptr(), w.lo.data_ptr()
-    a.B, a.T, a.F, a.Cin, a.Cout, a.ksize, a.stride = b, t, f, cin, cout, ksize, stride
+    a.B, a.T, a.F, a.Cin, a.Cout, a.ksize, a.stride, a.stride_t = b, t, f, cin, cout, ksize, stride, stride_t
     for name, v in (("scale", scale), ("shift", shift), ("scale2", scale2), ("shift2", shift2)):
         if v is not None:
             setattr(a, name, _req(v, torch.float32, name).data_ptr())

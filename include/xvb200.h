@@ -277,6 +277,10 @@ typedef struct xvb_conv2d_args {
   float* y_f32;
   const float* scale2; const float* shift2;
   uint16_t* y2_hi; uint16_t* y2_lo;
+  /* Time-axis stride: 0 means "same as stride" (every square-stride caller); 1 or 2 otherwise, with `stride` then the
+   * feature-axis stride alone.  CAM++'s FCM head (subtools2/egrecho/models/campplus/campplus.py:60-80, :104-106) uses
+   * stride (2, 1): feature 2, time 1, so T' = T and F' = ceil(F / 2). */
+  int stride_t;
 } xvb_conv2d_args_t;
 int xvb_conv2d(const xvb_conv2d_args_t* args, void* stream);
 
@@ -374,6 +378,34 @@ int xvb_conv_module(const float* x, int64_t ldx, int B, int T, int C, const floa
 int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
                     const uint16_t* id_lo, int B, int64_t P, int C, int relu, uint16_t* y_hi, uint16_t* y_lo, float* y_f32,
                     const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * CAM++ x-vector (subtools2/egrecho/models/campplus/campplus.py): the pieces of the densely connected D-TDNN layers that
+ * are not contractions.  Frames are channel-contiguous (B, T', C) rows of the stride-2 `tdnn`'s output sequence.
+ * ------------------------------------------------------------------------------------------- */
+
+/* y = relu(x * scale[c] + shift[c]) over `rows` rows of C channels, split planes in and out, fp32 in between: the eval
+ * BatchNorm1d + ReLU in front of every dense layer's linear1 (CAMDenseTDNNLayer.nonlinear1, :199, :212-213) and every
+ * transit layer's 1x1 conv (TransitLayer, :262-271), which read the whole concatenation so far.  C % 8 == 0, pitches
+ * ldx, ldy >= C and multiples of 8. */
+int xvb_bn_relu_planes(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int64_t rows, int C, const float* scale,
+                       const float* shift, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream);
+
+/* CAMLayer's mask (:157-178) per segment: h (B, T, C) planes (pitch ldh) = the layer's bottleneck after BN2 + ReLU;
+ * ctx[b, s] = mean_t h[b] + mean of h[b] over frames [s*seg_len, min(T, (s+1)*seg_len)) (avg_pool1d with ceil_mode: the
+ * last segment divides by its valid frames); gate[b, s] = sigmoid(W2 relu(W1 ctx + b1) + b2), fp32 on CUDA cores, one CTA
+ * per utterance.  w1 (R, C), w2 (G, R) fp32 as stored (linear1 / linear2 weights without the kernel axis).  gate: (B,
+ * ceil(T / seg_len), G) fp32.  C % 8 == 0, C <= 2048. */
+int xvb_cam_gate(const uint16_t* h_hi, const uint16_t* h_lo, int64_t ldh, int B, int T, int C, int seg_len, const float* w1,
+                 const float* b1, int R, const float* w2, const float* b2, int G, float* gate, void* stream);
+
+/* out = z * gate[b, t / seg_len, :] [+ in] over (B, T, C) planes: the kernel of xvb_se_apply with a gate row per
+ * seg_len-frame segment (gate (B, ceil(T / seg_len), C) fp32, e.g. from xvb_cam_gate) and an optional `in` (NULL: no
+ * add).  CAMLayer's y * m (:162) written straight into the layer's column slice of the block's concatenation buffer
+ * (CAMDenseTDNNBlock.forward, :256-259); seg_len = T is xvb_se_apply without `next`.  C % 8 == 0, pitches % 8 == 0. */
+int xvb_seg_gate_apply(const uint16_t* z_hi, const uint16_t* z_lo, int64_t ldz, const uint16_t* in_hi, const uint16_t* in_lo,
+                       int64_t ldin, const float* gate, int seg_len, uint16_t* out_hi, uint16_t* out_lo, int64_t ldout, int B,
+                       int T, int C, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Feature-side front-end (SURVEY 8f rank 1) on a ragged batch: utterance u owns rows

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Seeded outputs of the 2-D conv entry points (xvb_conv2d, xvb_conv2d_taps) and the layer kernel (xvb_tdnn_affine_ex,
-every existing epilogue flag, the split-K segment path and the fused pooling; the five frame layers of bench.py at
+"""Seeded outputs of the 2-D conv entry points (xvb_conv2d, xvb_conv2d_taps), xvb_se_apply and the layer kernel
+(xvb_tdnn_affine_ex, every existing epilogue flag, the split-K segment path and the fused pooling; the five frame layers of bench.py at
 256 x 200, with the im2col first layer and tdnn5's fused pooling; an ECAPA-sized and a Conformer-sized layer) written to
 one .npz, so that two builds of the library can be compared bit for bit:
 
@@ -112,6 +112,14 @@ def main():
         yf = torch.empty(B, T, cout, device="cuda")
         ops.tdnn_affine_ex(x, ops.pack_tdnn_weight(w, ctx), cout, ctx, bias=0.1 * rnd(cout), relu=True, y_f32=yf)
         res[name + "_f32"] = yf.cpu().numpy()
+    # xvb_se_apply (SE scaling + residual, with and without the running sum), a channel-slice view as in ECAPA
+    for i, (B, T, C, nxt) in enumerate([(4, 200, 512, True), (3, 37, 1024, False)]):
+        z, xin = ops.split_f32(rnd(B, T, 2 * C)).slice(0, C), ops.split_f32(rnd(B, T, C))
+        out_p, nxt_p = ops.SplitPlanes.empty((B, T, C), "cuda"), ops.SplitPlanes.empty((B, T, C), "cuda")
+        ops.se_apply(z, xin, torch.sigmoid(rnd(B, C)), out_p, nxt_p if nxt else None)
+        for name, p in (("out", out_p), ("next", nxt_p)) if nxt else (("out", out_p),):
+            res["se_apply{}_{}_hi".format(i, name)] = p.hi.view(torch.int16).cpu().numpy()
+            res["se_apply{}_{}_lo".format(i, name)] = p.lo.view(torch.int16).cpu().numpy()
     np.savez(out, **res)
     print(out, len(res), "arrays")
 
