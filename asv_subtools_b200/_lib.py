@@ -51,6 +51,13 @@ class LayerNormArgs(C.Structure):
                 ("y_f32", C.c_void_p), ("ldyf", C.c_int64)]
 
 
+class ConformerConfig(C.Structure):
+    """xvb_conformer_config_t (include/xvb200.h)."""
+    _fields_ = [(n, C.c_int) for n in ("feat_dim", "subsampling", "D", "H", "linear_units", "blocks", "conv_kernel", "pos",
+                                       "rotary_value", "softmax_plus", "act", "cm_norm", "out_dim", "out_norm",
+                                       "pool_hidden", "fc1", "position")]
+
+
 class XvbError(RuntimeError):
     pass
 
@@ -137,6 +144,7 @@ SIGNATURES = {
     "xvb_conv2d_head_k": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_valid": (_i, [_p, _p]),
     "xvb_subsample_head": (_i, [_p, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
+    "xvb_subsample_head_stride": (_i, [_p, _i, _i, _i, _p, _p, _i, _i, _p, _p, _p]),
     "xvb_layer_norm": (_i, [_p, _p]),
     "xvb_rope_attention": (_i, [_p, _i64, _i, _i, _i, _i, _p, _i, _f, _p, _p, _i64, _p]),
     "xvb_conv_module": (_i, [_p, _i64, _i, _i, _i, _p, _p, _i, _p, _p, _i, _f, _i, _p, _p, _i64, _p]),
@@ -193,6 +201,16 @@ SIGNATURES = {
     "xvb_resnet_save": (_i, [_p, C.c_char_p]),
     "xvb_resnet_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_resnet_destroy": (None, [_p]),
+    "xvb_conformer_create": (_i, [C.POINTER(_p), _p]),
+    "xvb_conformer_set_layer": (_i, [_p, C.c_char_p, _i, _i, _p, _p, _p, _p, _i]),
+    "xvb_conformer_finalize": (_i, [_p]),
+    "xvb_conformer_feat_dim": (_i, [_p]),
+    "xvb_conformer_embed_dim": (_i, [_p]),
+    "xvb_conformer_last_launches": (_i, [_p]),
+    "xvb_conformer_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_conformer_save": (_i, [_p, C.c_char_p]),
+    "xvb_conformer_load": (_i, [C.POINTER(_p), C.c_char_p]),
+    "xvb_conformer_destroy": (None, [_p]),
     "xvb_extractor_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_extractor_feat_dim": (_i, [C.c_char_p]),
     "xvb_ark_reader_open": (_i, [C.POINTER(_p), C.c_char_p]),

@@ -3,7 +3,8 @@
 // pointwise convolutions, the subsampling Linear, transform_out, the pooling convs, fc1 / fc2 -- runs on the wgmma layer
 // kernel (tdnn_gemm.cu) and the second subsampling conv on the 2-D conv kernel (conv2d.cu, xvb_conv2d_valid).  What is
 // left is bandwidth- or latency-bound and runs here in fp32 on CUDA cores:
-//   * the first subsampling conv, Conv2d(1, C, 3, stride 2, no padding) + ReLU (subsampling.py:104-109);
+//   * the first subsampling conv, Conv2d(1, C, 3, stride 2, no padding) + ReLU (subsampling.py:104-109), or with
+//     stride (2, 1) for SVConv2dSubsampling2 (subsampling.py:365-415);
 //   * residual update + LayerNorm in one pass over the rows, with an optional second LayerNorm and activation
 //     (encoder_layer.py:234-331, the after_norm of encoder.py:414-419, the ln_replace norms of components.py:372-376,
 //     AttentiveStatsPool's LayerNorms, transformer_xvector.py:39-50);
@@ -65,9 +66,10 @@ __device__ __forceinline__ void warp_layer_norm(float* v, int C, float eps, cons
   __syncwarp();
 }
 
-// ---- Conv2dSubsampling4's first conv: one thread per (output position, 8 channels) -----------------------------------
-// 32-bit index arithmetic (the host checks total < 2^31), so decoding the flat index takes no emulated 64-bit division.
-__global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F, const float* __restrict__ w,
+// ---- the subsampling's first conv: one thread per (output position, 8 channels) --------------------------------------
+// Time stride 2, feature stride sf (2: Conv2dSubsampling4, 1: SVConv2dSubsampling2).  32-bit index arithmetic (the host
+// checks total < 2^31), so decoding the flat index takes no emulated 64-bit division.
+__global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F, int sf, const float* __restrict__ w,
                                       const float* __restrict__ bias, int C, int T1, int F1, __nv_bfloat16* __restrict__ yh,
                                       __nv_bfloat16* __restrict__ yl, unsigned total) {
   const unsigned groups = (unsigned)C / 8;
@@ -83,7 +85,7 @@ __global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F,
 #pragma unroll
     for (int kt = 0; kt < 3; ++kt)
 #pragma unroll
-      for (int kf = 0; kf < 3; ++kf) in[kt * 3 + kf] = __ldg(x + (b * T + 2 * t + kt) * F + 2 * f + kf);
+      for (int kf = 0; kf < 3; ++kf) in[kt * 3 + kf] = __ldg(x + (b * T + 2 * t + kt) * F + sf * f + kf);
     float y[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -311,22 +313,28 @@ int grid_cap(long long want) {
 
 using namespace xvb;
 
-extern "C" int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, const float* bias, int C, uint16_t* y_hi,
-                                  uint16_t* y_lo, void* stream) {
+extern "C" int xvb_subsample_head_stride(const float* x, int B, int T, int F, const float* w, const float* bias, int C,
+                                         int stride_f, uint16_t* y_hi, uint16_t* y_lo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(x && w && bias && y_hi && y_lo, "xvb_subsample_head: null pointer");
+  XVB_CHECK_ARG(stride_f == 1 || stride_f == 2, "xvb_subsample_head: feature stride must be 1 or 2 (got %d)", stride_f);
   XVB_CHECK_ARG(B > 0 && T >= 3 && F >= 3 && C > 0 && C % 8 == 0, "xvb_subsample_head: bad shape B=%d T=%d F=%d C=%d (T, F >= 3, C %% 8 == 0)",
                 B, T, F, C);
   XVB_CHECK_ARG(((uintptr_t)y_hi | (uintptr_t)y_lo) % 16 == 0, "xvb_subsample_head: planes must be 16-byte aligned");
-  const int T1 = (T - 3) / 2 + 1, F1 = (F - 3) / 2 + 1;
+  const int T1 = (T - 3) / 2 + 1, F1 = (F - 3) / stride_f + 1;
   const long long total = (long long)B * T1 * F1 * (C / 8);
   XVB_CHECK_ARG(total < (1LL << 31), "xvb_subsample_head: %lld (position, 8-channel) items exceed one launch", total);
   subsample_head_kernel<<<grid_cap((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      x, T, F, w, bias, C, T1, F1, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
+      x, T, F, stride_f, w, bias, C, T1, F1, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
       (unsigned)total);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
+}
+
+extern "C" int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, const float* bias, int C, uint16_t* y_hi,
+                                  uint16_t* y_lo, void* stream) {
+  return xvb_subsample_head_stride(x, B, T, F, w, bias, C, 2, y_hi, y_lo, stream);
 }
 
 extern "C" int xvb_layer_norm(const xvb_layer_norm_args_t* a, void* stream) {

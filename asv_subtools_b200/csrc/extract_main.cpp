@@ -14,11 +14,13 @@
 // :17-45: <model-path> <feats-rspecifier> <vectors-wspecifier>); the role is that of the reference's
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
-// the input side.  The model file is any of the three families, told apart by its magic: TDNN x-vector
-// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling)
-// or 2-D ResNet x-vector (XVBR0001, the extractors' save()).  What it adds: utterances of equal length are batched (the reference runs batch 1).
+// the input side.  The model file is any of the four families, told apart by its magic: TDNN x-vector
+// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
+// 2-D ResNet x-vector (XVBR0001) or Conformer x-vector (XVBC0001, 4x or 2x subsampling), the last two written by the
+// native extractors' save().  What it adds: utterances of equal length are batched (the reference runs batch 1).
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
-//     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32;
+//     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
+//     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
 //   * one "FV" vector per input key (order follows batch completion, which the wspecifier allows);
 //   * errors: message with "ERROR" on stderr, exit status 1 (the reference's shell greps for it,
 //     extract_xvectors_for_pytorch.sh:144-145).  No GPU / not an H100 -> error, there is no CPU path.
@@ -60,7 +62,8 @@ struct Utt {
 struct Runner {
   xvb_extractor_t* ex = nullptr;   // TDNN x-vector family (XVBM0001) ...
   xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001 / XVBE0002) ...
-  xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001)
+  xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001) ...
+  xvb_conformer_t* cf = nullptr;   // ... or Conformer x-vector (XVBC0001)
   xvb_ark_writer_t* out = nullptr;
   int F = 0, D = 0, batch = 256, cmn = 0, cmn_window = 300;
   float *d_feats = nullptr, *d_tmp = nullptr, *d_emb = nullptr, *h_feats = nullptr, *h_emb = nullptr;
@@ -92,7 +95,8 @@ struct Runner {
     CU(cudaMemcpy(d_feats, h_feats, (size_t)B * T * F * sizeof(float), cudaMemcpyHostToDevice));
     if (ex) CK(xvb_extractor_extract(ex, d_feats, B, T, d_emb, nullptr), "xvb_extractor_extract");
     else if (ec) CK(xvb_ecapa_extract(ec, d_feats, B, T, d_emb, nullptr), "xvb_ecapa_extract");
-    else CK(xvb_resnet_extract(rn, d_feats, B, T, d_emb, nullptr), "xvb_resnet_extract");
+    else if (rn) CK(xvb_resnet_extract(rn, d_feats, B, T, d_emb, nullptr), "xvb_resnet_extract");
+    else CK(xvb_conformer_extract(cf, d_feats, B, T, d_emb, nullptr), "xvb_conformer_extract");
     CU(cudaMemcpy(h_emb, d_emb, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToHost));
     for (int i = 0; i < B; ++i) {
       Utt& u = utts[items[i].utt];
@@ -155,6 +159,7 @@ bool read_wav(const std::string& path, std::vector<float>* out, int* sample_rate
 int main(int argc, char** argv) {
   Runner r;
   int max_chunk = 10000, gpu = 0;
+  bool max_chunk_set = false;
   std::string wav_type;
   xvb_fbank_opts_t fo;
   xvb_fbank_default_opts(&fo);
@@ -167,7 +172,7 @@ int main(int argc, char** argv) {
       return argv[++i];
     };
     if (a == "--batch") r.batch = atoi(val("--batch"));
-    else if (a == "--max-chunk") max_chunk = atoi(val("--max-chunk"));
+    else if (a == "--max-chunk") { max_chunk = atoi(val("--max-chunk")); max_chunk_set = true; }
     else if (a == "--cmn-window") r.cmn_window = atoi(val("--cmn-window"));
     else if (a == "--gpu-id") gpu = atoi(val("--gpu-id"));
     else if (a == "--wav") wav_type = val("--wav");
@@ -188,8 +193,10 @@ int main(int argc, char** argv) {
              "                   [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002) or 2-D ResNet x-vector (XVBR0001) model,\n"
-             "recognised by its magic.\n");
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001)\n"
+             "or Conformer x-vector (XVBC0001) model, recognised by its magic.  --max-chunk defaults to 300 frames for a\n"
+             "Conformer (the model's own chunk rule) and to 10000 otherwise.  A Conformer chunk needs at least 7 frames and\n"
+             "fewer than 5000 subsampled frames.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -218,6 +225,11 @@ int main(int argc, char** argv) {
       CK(xvb_resnet_load(&r.rn, pos[0]), "loading the ResNet model");
       r.F = xvb_resnet_feat_dim(r.rn);
       r.D = xvb_resnet_embed_dim(r.rn);
+    } else if (memcmp(magic, "XVBC0001", 8) == 0) {
+      CK(xvb_conformer_load(&r.cf, pos[0]), "loading the Conformer model");
+      r.F = xvb_conformer_feat_dim(r.cf);
+      r.D = xvb_conformer_embed_dim(r.cf);
+      if (!max_chunk_set) max_chunk = 300;
     } else {
       CK(xvb_extractor_load(&r.ex, pos[0]), "loading the model");
       r.F = xvb_extractor_feat_dim(pos[0]);
@@ -337,6 +349,7 @@ int main(int argc, char** argv) {
   if (r.ex) xvb_extractor_destroy(r.ex);
   if (r.ec) xvb_ecapa_destroy(r.ec);
   if (r.rn) xvb_resnet_destroy(r.rn);
+  if (r.cf) xvb_conformer_destroy(r.cf);
   fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
   return 0;
 }

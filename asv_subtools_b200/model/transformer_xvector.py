@@ -7,19 +7,26 @@ Same file name, class name, constructor signature and defaults (transformer_para
 assign_params_dict(support_unknow=True) does), creation string and state_dict keys for training=False; like the other
 blueprints, the training-only loss is not built, so its keys are left to load_state_dict(strict=False).
 
-Supported: transformer_type 'conformer' with input_layer 'conv2d'; pos_enc_type 'rot_pos' (rotary_value either way),
+Supported: transformer_type 'conformer' with input_layer 'conv2d' (4x subsampling) or 'conv2d2' (2x,
+SVConv2dSubsampling2, subsampling.py:365-415); pos_enc_type 'rot_pos' (rotary_value either way),
 'abs_pos' or 'no_pos'; attention norm 'softmax' or 'softmax_plus'; the convolution module with 'layer_norm' or
 'batch_norm'; activation 'swish' or 'relu'; transform_out with a LayerNorm (ln_replace) or a BatchNorm; the
 ecpa-attentive pooling with stddev; fc1 on or off (LayerNorm with or without affine); positions far / near_affine / near.
 Every other option raises NotImplementedError naming it.
 
-At extraction (ConformerExtractor) every contraction runs on the wgmma layer kernel with split-plane numerics: Q/K/V as
+At extraction every contraction runs on the wgmma layer kernel with split-plane numerics: Q/K/V as
 one GEMM over the concatenated weights, linear_out, the feed-forward linears (swish / ReLU in the epilogue), the
 pointwise convs, the subsampling Linear (its input columns permuted from the reference's c * F'' + f to the f * C + c
 order of the conv output, x * sqrt(d) applied after the bias as the epilogue's scale), transform_out, the pooling convs
 and fc1 / fc2.  The second subsampling conv runs on the 2-D conv kernel without padding (xvb_conv2d_valid); the first
 one, the residual + LayerNorm steps, the attention and the convolution module's middle run on the kernels of
-csrc/conformer.cu.  The residual stream stays fp32.
+csrc/conformer.cu (the 2x subsampling's first conv with feature stride 1, its second conv at stride 1).  The residual
+stream stays fp32.
+
+build_extractor() hands the weights to the native handle (NativeConformerExtractor over xvb_conformer_*, csrc/
+conformer_extractor.cu), which runs the whole launch sequence in C++ and also writes XVBC0001 model files for
+bin/xvb-extract.  XVB_CONFORMER_NATIVE=0 selects ConformerExtractor, the Python driver of the same kernels with the same
+arguments in the same order, kept as the A/B and profiling twin; the two give bit-identical embeddings.
 
 extract_embedding keeps the reference's maxChunk = 300 chunk rule (for_extract_embedding, framework.py:12-55): an
 utterance is cut into num_split = ceil(T / 300) chunks, each chunk is extracted on its own and the embeddings are
@@ -43,7 +50,8 @@ from asv_subtools_b200.nnet.components import TdnnAffine, fold_batchnorm  # noqa
 from asv_subtools_b200.nnet.framework import for_extract_embedding  # noqa: E402
 
 MAX_CHUNK = 300     # @for_extract_embedding(maxChunk=300) of transformer_xvector.py:321
-MIN_FRAMES = 7      # the shortest input Conv2dSubsampling4 accepts
+MIN_FRAMES = 7      # the shortest input Conv2dSubsampling4 and SVConv2dSubsampling2 accept
+TABLE_ROWS = 5000   # PositionalEncoding / RoPositionalEncoding max_len (embedding.py:41, :162)
 
 
 def _assign(defaults, given, support_unknow=False):
@@ -80,7 +88,7 @@ _ATT_NORM_DEFAULTS = {"scale_adapt": False, "norm_method": "softmax", "diag_mask
 def _check_encoder(p):
     """Raise for every encoder option the native path does not build."""
     a = p["attention_norm_args"]
-    for name, ok in (("att_type", p["att_type"] == "multi"), ("input_layer", p["input_layer"] == "conv2d"),
+    for name, ok in (("att_type", p["att_type"] == "multi"), ("input_layer", p["input_layer"] in ("conv2d", "conv2d2")),
                      ("pos_enc_type", p["pos_enc_type"] in ("rot_pos", "abs_pos", "no_pos")),
                      ("rope_abs_plus", not p["rope_abs_plus"]), ("add_t5rel_bias", not p["add_t5rel_bias"]),
                      ("attention_conv_out", not p["attention_conv_out"]), ("mlp_head", not p["mlp_head"]),
@@ -113,6 +121,25 @@ class _Conv2dSubsampling4(nn.Module):
         super().__init__()
         self.conv = nn.Sequential(nn.Conv2d(1, odim, 3, 2), nn.ReLU(), nn.Conv2d(odim, odim, 3, 2), nn.ReLU())
         self.out = nn.Sequential(nn.Linear(odim * (((idim - 1) // 2 - 1) // 2), odim))
+
+
+class _SVConv2dSubsampling2(nn.Module):
+    """Parameter container of SVConv2dSubsampling2 (subsampling.py:365-389): Conv2d(1, C, 3, stride (2, 1)) (time 2,
+    frequency 1), Conv2d(C, C, 3, 1), Linear(C * (F - 4), C); T' = (T - 1) // 2 - 2."""
+
+    def __init__(self, idim, odim):
+        super().__init__()
+        self.conv = nn.Sequential(nn.Conv2d(1, odim, 3, (2, 1)), nn.ReLU(), nn.Conv2d(odim, odim, 3, 1), nn.ReLU())
+        self.out = nn.Sequential(nn.Linear(odim * (idim - 4), odim))
+
+
+def subsampled_shape(subsampling, frames, freq):
+    """(T', F'') of the subsampling's output for a chunk of `frames` frames of `freq` bins: 4 = Conv2dSubsampling4, 2 =
+    SVConv2dSubsampling2."""
+    t1 = (frames - 1) // 2
+    if subsampling == 4:
+        return (t1 - 1) // 2, ((freq - 1) // 2 - 1) // 2
+    return t1 - 2, freq - 4
 
 
 class _AttentionNormalize(nn.Module):
@@ -178,7 +205,8 @@ class _ConformerEncoder(nn.Module):
     def __init__(self, idim, p):
         super().__init__()
         self.p = p
-        self.embed = _Conv2dSubsampling4(idim, p["attention_dim"])
+        self.subsampling = 4 if p["input_layer"] == "conv2d" else 2
+        self.embed = (_Conv2dSubsampling4 if self.subsampling == 4 else _SVConv2dSubsampling2)(idim, p["attention_dim"])
         self.after_norm = nn.LayerNorm(p["attention_dim"], eps=1e-5)
         self.encoders = nn.ModuleList([_ConformerLayer(p) for _ in range(p["num_blocks"])])
 
@@ -285,7 +313,10 @@ class TransformerXvector(TopVirtualNnet):
             raise ValueError("extracted_embedding='far' needs fc1=True (transformer_xvector.py:334-336 asserts it)")
         if self.extracted_embedding not in ("far", "near_affine", "near"):
             raise TypeError("Expected far or near position, but got {}".format(self.extracted_embedding))
-        return ConformerExtractor(self, self.device_for_extraction())
+        dev = self.device_for_extraction()
+        if os.environ.get("XVB_CONFORMER_NATIVE", "1") == "0":
+            return ConformerExtractor(self, dev)       # op-by-op twin of the native handle
+        return NativeConformerExtractor(self, dev)
 
     @for_extract_embedding(maxChunk=MAX_CHUNK, isMatrix=True)
     def _extract_embedding_chunked(self, inputs):
@@ -407,6 +438,7 @@ class ConformerExtractor:
         self.rotary_value = self.pos == "rot_pos" and bool(p["rotary_value"])
         self.softmax_plus = p["attention_norm_args"]["norm_method"] == "softmax_plus"
         self.act = ACT_SWISH if p["activation_type"] == "swish" else ACT_RELU
+        self.subsampling = enc.subsampling
         emb = enc.embed
         self.head_w = _vec(emb.conv[0].weight, device)
         self.head_b = _vec(emb.conv[0].bias, device)
@@ -414,9 +446,8 @@ class ConformerExtractor:
         self.conv2_w = ops.pack_conv2d_weight(w2.to(device))
         self.conv2_scale = torch.ones(self.D, dtype=torch.float32, device=device)
         self.conv2_shift = _vec(emb.conv[2].bias, device)
-        self.f2 = ((self.feat_dim - 1) // 2 - 1) // 2
-        lw = emb.out[0].weight.detach().float()[:, torch.from_numpy(subsampling_column_order(self.D, self.f2))]
-        xscale = None if self.pos == "no_pos" else np.full(self.D, math.sqrt(self.D), np.float32)
+        self.f2 = subsampled_shape(self.subsampling, MIN_FRAMES, self.feat_dim)[1]
+        lw, xscale = _embed_out_weight(m)
         self.embed_out = _Lin(lw, emb.out[0].bias, device, scale=xscale,
                               shift=None if xscale is None else np.zeros(self.D, np.float32))
         self.layers = []
@@ -476,8 +507,8 @@ class ConformerExtractor:
 
     def _tables_for(self, t):
         if t not in self._tables:
-            if t >= 5000:
-                raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' 5000".format(t))
+            if t >= TABLE_ROWS:
+                raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' {}".format(t, TABLE_ROWS))
             rope = self._rope[:t].to(self.device).contiguous() if self._rope is not None else None
             absp = self._abs[:t].to(self.device).contiguous() if self._abs is not None else None
             mults = [softmax_plus_multiplier(t, L["train_len"]) if self.softmax_plus else 1.0 for L in self.layers]
@@ -494,14 +525,19 @@ class ConformerExtractor:
         if T < MIN_FRAMES:
             raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, T))
         dev, P, D = feats.device, ops.SplitPlanes, self.D
-        T1, F1 = (T - 1) // 2, (Fd - 1) // 2
-        T2, F2 = (T1 - 1) // 2, (F1 - 1) // 2
+        T1 = (T - 1) // 2
+        F1 = (Fd - 1) // 2 if self.subsampling == 4 else Fd - 2
+        T2, F2 = subsampled_shape(self.subsampling, T, Fd)
         rope, absp, mults = self._tables_for(T2)
         n = 0
         x1 = P.empty((B, T1, F1, D), dev)
-        ops.subsample_head(feats, self.head_w, self.head_b, x1)
+        if self.subsampling == 4:
+            ops.subsample_head(feats, self.head_w, self.head_b, x1)
+        else:       # SVConv2dSubsampling2: time stride 2, frequency stride 1, then a stride-1 valid conv
+            ops.subsample_head(feats, self.head_w, self.head_b, x1, stride_f=1)
         x2 = P.empty((B, T2, F2, D), dev)
-        ops.conv2d(x1, self.conv2_w, D, 3, 2, self.conv2_scale, self.conv2_shift, relu=True, y=x2, valid=True)
+        ops.conv2d(x1, self.conv2_w, D, 3, 2 if self.subsampling == 4 else 1, self.conv2_scale, self.conv2_shift, relu=True,
+                   y=x2, valid=True)
         del x1
         r = torch.empty(B, T2, D, dtype=torch.float32, device=dev)
         self.embed_out.run(P(x2.hi.view(B, T2, F2 * D), x2.lo.view(B, T2, F2 * D), F2 * D), y_f32=r)
@@ -583,6 +619,205 @@ class ConformerExtractor:
 
     def close(self):
         pass
+
+
+def _embed_out_weight(m):
+    """The subsampling Linear's weight with its input columns permuted to the f * C + c order of the conv output, and
+    the xscale sqrt(d) as the epilogue's scale (None for no_pos)."""
+    enc = m.transformer
+    d = enc.p["attention_dim"]
+    f2 = subsampled_shape(enc.subsampling, MIN_FRAMES, m.inputs_dim)[1]
+    w = enc.embed.out[0].weight.detach().float()[:, torch.from_numpy(subsampling_column_order(d, f2))]
+    xscale = None if enc.p["pos_enc_type"] == "no_pos" else np.full(d, math.sqrt(d), np.float32)
+    return w, xscale
+
+
+def native_config(m):
+    """xvb_conformer_config_t fields of a TransformerXvector."""
+    p = m.transformer.p
+    to = m.transform_out
+    return dict(feat_dim=m.inputs_dim, subsampling=m.transformer.subsampling, D=p["attention_dim"], H=p["attention_heads"],
+                linear_units=p["linear_units"], blocks=p["num_blocks"], conv_kernel=p["cnn_module_kernel"],
+                pos={"no_pos": 0, "abs_pos": 1, "rot_pos": 2}[p["pos_enc_type"]], rotary_value=int(bool(p["rotary_value"])),
+                softmax_plus=int(p["attention_norm_args"]["norm_method"] == "softmax_plus"),
+                act=ACT_SWISH if p["activation_type"] == "swish" else ACT_RELU,
+                cm_norm=int(p["cnn_module_norm"] == "batch_norm"), out_dim=to.affine.weight.shape[0],
+                out_norm=0 if to.batchnorm is None else (2 if to.ln else 1),
+                pool_hidden=m.stats.attention[0].weight.shape[0], fc1=int(m.fc1 is not None),
+                position={"far": 0, "near_affine": 1, "near": 2}[m.extracted_embedding])
+
+
+def native_records(m):
+    """(name, w, bias, scale, shift, flags, keys) records and tables for xvb_conformer_set_layer, after the hand-over
+    transforms of ConformerExtractor.__init__: the concatenated Q/K/V, the subsampling Linear's column permutation and
+    xscale, the second subsampling conv transposed to (C, C, kf, kt), folded BatchNorms.  `keys` are the state_dict
+    entries the record carries.  Tables: "pos_table" (rotary_table or sinusoid_table) and, for softmax_plus, each
+    block's "self_attn.att_norm" = softmax_plus_multiplier for T' = 1 .. 4999 (index 0 unused, 0)."""
+    from asv_subtools_b200._lib import BN, RELU, SWISH
+    f = lambda t: None if t is None else t.detach().float().cpu().numpy()  # noqa: E731
+    enc = m.transformer
+    p = enc.p
+    d, h = p["attention_dim"], p["attention_heads"]
+    act = SWISH if p["activation_type"] == "swish" else RELU
+    out = []
+
+    def keys_of(mod, name):
+        return [name + "." + k for k in mod.state_dict()]
+
+    def lin(name, mod, flags=0, scale=None, shift=None, w=None):
+        w = f(mod.weight).reshape(mod.weight.shape[0], -1) if w is None else w
+        if scale is not None:
+            flags |= BN
+        out.append((name, w, f(mod.bias), scale, shift, flags, keys_of(mod, name)))
+
+    def norm(name, mod):
+        if isinstance(mod, nn.BatchNorm1d):
+            s, t = fold_batchnorm(mod)
+            out.append((name, None, None, s, t, BN, keys_of(mod, name)))
+        else:
+            out.append((name, None, None, f(mod.weight), f(mod.bias), 0, keys_of(mod, name)))
+
+    def tdnn(name, layer, whole):
+        a = layer.affine
+        w = f(a.weight)[:, :, 0]
+        flags = 0 if not whole else {ACT_RELU: RELU, ACT_SWISH: SWISH}.get(layer.act, 0)
+        if whole and layer.batchnorm is not None and not layer.ln:
+            s, t = fold_batchnorm(layer.batchnorm)
+            out.append((name + ".affine", w, f(a.bias), s, t, flags | BN,
+                        keys_of(a, name + ".affine") + keys_of(layer.batchnorm, name + ".batchnorm")))
+            return
+        out.append((name + ".affine", w, f(a.bias), None, None, flags, keys_of(a, name + ".affine")))
+        if whole and layer.batchnorm is not None:
+            norm(name + ".batchnorm", layer.batchnorm)
+
+    e = "transformer.embed."
+    conv0, conv2 = enc.embed.conv[0], enc.embed.conv[2]
+    out.append((e + "conv.0", f(conv0.weight).reshape(d, 9), f(conv0.bias), None, None, 0, keys_of(conv0, e + "conv.0")))
+    w2 = conv2.weight.detach().float().transpose(2, 3).reshape(d, 9 * d).cpu().numpy()
+    out.append((e + "conv.2", w2, f(conv2.bias), None, None, 0, keys_of(conv2, e + "conv.2")))
+    lw, xscale = _embed_out_weight(m)
+    lin(e + "out.0", enc.embed.out[0], w=f(lw), scale=xscale, shift=None if xscale is None else np.zeros(d, np.float32))
+    if p["pos_enc_type"] != "no_pos":
+        table = rotary_table(d // h) if p["pos_enc_type"] == "rot_pos" else sinusoid_table(d)
+        out.append(("pos_table", f(table), None, None, None, 0, []))
+    softmax_plus = p["attention_norm_args"]["norm_method"] == "softmax_plus"
+    for i, layer in enumerate(enc.encoders):
+        q = "transformer.encoders.{}.".format(i)
+        for ff in ("feed_forward_macaron", "feed_forward"):
+            mod = getattr(layer, ff)
+            lin(q + ff + ".w_1", mod.w_1, act)
+            lin(q + ff + ".w_2", mod.w_2)
+        a = layer.self_attn
+        qkv = [a.linear_q, a.linear_k, a.linear_v]
+        out.append((q + "self_attn.linear_qkv", f(torch.cat([x.weight for x in qkv], 0)), f(torch.cat([x.bias for x in qkv], 0)),
+                    None, None, 0,
+                    sum([keys_of(x, q + "self_attn." + n) for x, n in zip(qkv, ("linear_q", "linear_k", "linear_v"))], [])))
+        lin(q + "self_attn.linear_out", a.linear_out)
+        if softmax_plus:
+            mult = np.zeros((1, TABLE_ROWS), np.float32)
+            for t in range(1, TABLE_ROWS):
+                mult[0, t] = softmax_plus_multiplier(t, a.att_norm.train_len)
+            out.append((q + "self_attn.att_norm", mult, None, None, None, 0, keys_of(a.att_norm, q + "self_attn.att_norm")))
+        cm = layer.conv_module
+        lin(q + "conv_module.pointwise_conv1", cm.pointwise_conv1)
+        out.append((q + "conv_module.depthwise_conv", f(cm.depthwise_conv.weight).reshape(d, -1), f(cm.depthwise_conv.bias),
+                    None, None, 0, keys_of(cm.depthwise_conv, q + "conv_module.depthwise_conv")))
+        norm(q + "conv_module.norm", cm.norm)
+        lin(q + "conv_module.pointwise_conv2", cm.pointwise_conv2)
+        for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
+            norm(q + name, getattr(layer, name))
+    norm("transformer.after_norm", enc.after_norm)
+    tdnn("transform_out", m.transform_out, True)
+    att = m.stats.attention
+    lin("stats.attention.0", att[0], RELU)
+    norm("stats.attention.2", att[2])
+    lin("stats.attention.4", att[4])
+    norm("stats.norm_stats", m.stats.norm_stats)
+    pos = m.extracted_embedding
+    if pos == "far":
+        tdnn("fc1", m.fc1, False)
+    else:
+        if m.fc1 is not None:
+            tdnn("fc1", m.fc1, True)
+        tdnn("fc2", m.fc2, pos == "near")
+    return out
+
+
+def _cuda_f32(feats, feat_dim):
+    if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
+        raise TypeError("feats must be a contiguous CUDA float32 tensor")
+    if feats.shape[2] != feat_dim:
+        raise ValueError("expected feature dim {}, got {}".format(feat_dim, feats.shape[2]))
+    return feats
+
+
+class NativeConformerExtractor:
+    """xvb_conformer_t: packed weights, tables, workspace and the whole launch sequence of ConformerExtractor in the C
+    library, on the device that is current when it is built (or loaded from an XVBC0001 file)."""
+
+    def __init__(self, m=None, device=None, path=None):
+        import ctypes as C
+        from asv_subtools_b200._lib import ConformerConfig, check, lib
+        self._C, self._lib, self._check = C, lib, check
+        self._h = C.c_void_p()
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            if path is not None:
+                check(lib.xvb_conformer_load(C.byref(self._h), str(path).encode()), "xvb_conformer_load")
+            else:
+                cfg = ConformerConfig(**native_config(m))
+                check(lib.xvb_conformer_create(C.byref(self._h), C.byref(cfg)), "xvb_conformer_create")
+                for name, w, b, scale, shift, flags, _ in native_records(m):
+                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
+                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
+                    w, scale = arrs[0], arrs[2]
+                    rows = w.shape[0] if w is not None else scale.shape[0] if scale is not None else _norm_width(m, name)
+                    cols = w.shape[1] if w is not None else 0
+                    check(lib.xvb_conformer_set_layer(self._h, name.encode(), rows, cols, *ptr, flags), "xvb_conformer_set_layer")
+                check(lib.xvb_conformer_finalize(self._h), "xvb_conformer_finalize")
+        self.feat_dim = lib.xvb_conformer_feat_dim(self._h)
+        self.embed_dim = lib.xvb_conformer_embed_dim(self._h)
+
+    @classmethod
+    def load(cls, path):
+        return cls(path=path)
+
+    def save(self, path):
+        """Write an XVBC0001 model file for bin/xvb-extract."""
+        self._check(self._lib.xvb_conformer_save(self._h, str(path).encode()), "xvb_conformer_save")
+
+    @property
+    def last_launches(self):
+        return self._lib.xvb_conformer_last_launches(self._h)
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
+        stream."""
+        B, T, _ = _cuda_f32(feats, self.feat_dim).shape
+        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
+        C = self._C
+        self._check(self._lib.xvb_conformer_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
+                                                    C.c_void_p(torch.cuda.current_stream().cuda_stream)),
+                    "xvb_conformer_extract")
+        return emb
+
+    def close(self):
+        h, self._h = self._h, None
+        if h:
+            self._lib.xvb_conformer_destroy(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _norm_width(m, name):
+    """Channel count of a LayerNorm record without affine (no array to read it from)."""
+    mod = m
+    for part in name.split("."):
+        mod = mod[int(part)] if part.isdigit() else getattr(mod, part)
+    return mod.normalized_shape[0]
 
 
 if __name__ == "__main__":

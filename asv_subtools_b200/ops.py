@@ -320,14 +320,19 @@ def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, 
                               y2h, y2l, _stream()), "xvb_se_residual")
 
 
-def subsample_head(feats, weight, bias, y):
+def subsample_head(feats, weight, bias, y, stride_f=None):
     """Conv2dSubsampling4's first conv + ReLU (xvb_subsample_head): feats (B, T, F) fp32, weight (C, 1, 3, 3) fp32 as
-    stored, bias (C,) -> y SplitPlanes (B, (T - 1) // 2, (F - 1) // 2, C)."""
+    stored, bias (C,) -> y SplitPlanes (B, (T - 1) // 2, (F - 1) // 2, C).  stride_f = 1 or 2: the feature stride of
+    xvb_subsample_head_stride (1: SVConv2dSubsampling2's stride (2, 1), y (B, (T - 1) // 2, F - 2, C))."""
     feats = _req(feats, torch.float32, "feats")
     b, t, f = feats.shape
-    check(lib.xvb_subsample_head(_ptr(feats), b, t, f, _ptr(_req(weight, torch.float32, "weight")),
-                                 _ptr(_req(bias, torch.float32, "bias")), weight.shape[0], y.hi.data_ptr(), y.lo.data_ptr(),
-                                 _stream()), "xvb_subsample_head")
+    args = (_ptr(feats), b, t, f, _ptr(_req(weight, torch.float32, "weight")), _ptr(_req(bias, torch.float32, "bias")),
+            weight.shape[0])
+    if stride_f is None:
+        check(lib.xvb_subsample_head(*args, y.hi.data_ptr(), y.lo.data_ptr(), _stream()), "xvb_subsample_head")
+    else:
+        check(lib.xvb_subsample_head_stride(*args, int(stride_f), y.hi.data_ptr(), y.lo.data_ptr(), _stream()),
+              "xvb_subsample_head_stride")
 
 
 def _rows(t, name):

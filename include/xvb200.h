@@ -327,6 +327,10 @@ int xvb_conv2d_valid(const xvb_conv2d_args_t* args, void* stream);
  * y (B, T1, F1, C) planes with T1 = (T - 1) / 2, F1 = (F - 1) / 2.  T, F >= 3, C % 8 == 0. */
 int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, const float* bias, int C, uint16_t* y_hi,
                        uint16_t* y_lo, void* stream);
+/* The same first conv with feature stride stride_f in {1, 2} (time stride 2): stride_f = 1 is SVConv2dSubsampling2's
+ * Conv2d(1, C, 3, stride (2, 1)) (subsampling.py:365-415), F1 = F - 2; stride_f = 2 is xvb_subsample_head, bit for bit. */
+int xvb_subsample_head_stride(const float* x, int B, int T, int F, const float* w, const float* bias, int C, int stride_f,
+                              uint16_t* y_hi, uint16_t* y_lo, void* stream);
 
 /* Residual update + LayerNorm over `rows` rows of C channels (C <= 8192), one pass:
  *   v     = x [+ table[row % table_rows]] [+ delta_scale * delta]     the residual adds of ConformerEncoderLayer
@@ -758,6 +762,74 @@ int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int6
 int xvb_resnet_save(const xvb_resnet_t* h, const char* path);
 int xvb_resnet_load(xvb_resnet_t** out, const char* path);
 void xvb_resnet_destroy(xvb_resnet_t* h);
+
+/* ---------------------------------------------------------------------------------------------
+ * Whole-model extractor for the Conformer x-vector (pytorch/model/transformer_xvector.py, extract_embedding :321-346,
+ * Conformer encoder with 4x (input_layer "conv2d") or 2x ("conv2d2") subsampling): the launch sequence of
+ * xvb_subsample_head[_stride], xvb_conv2d_valid, xvb_tdnn_affine_ex, xvb_layer_norm, xvb_rope_attention,
+ * xvb_conv_module, xvb_attn_stats_pool and xvb_split_f32 in C++, one chunk per utterance (the 300-frame chunk rule
+ * stays with the caller).  Bit-identical to the op-by-op Python driver of the same kernels (ConformerExtractor,
+ * XVB_CONFORMER_NATIVE=0).
+ *
+ * Records (rows x cols host fp32 w, optional bias / scale / shift of `rows` entries) are named by state_dict module path
+ * and arrive after the hand-over transforms of the Python side:
+ *   "transformer.embed.conv.0"     w (D, 9) as stored (kt, kf), bias
+ *   "transformer.embed.conv.2"     w (D, 9 D) = the (D, D, kt, kf) weight transposed to (D, D, kf, kt), bias
+ *   "transformer.embed.out.0"      w (D, D F'') with its columns in the f * D + c order of the conv output, bias;
+ *                                  scale = sqrt(D), shift = 0 with XVB_BN unless pos is no_pos (the xscale)
+ *   "transformer.encoders.i.{feed_forward_macaron,feed_forward}.{w_1,w_2}", ".self_attn.linear_qkv" (Q, K, V rows
+ *   concatenated), ".self_attn.linear_out", ".conv_module.pointwise_conv{1,2}": w (Cout, Cin), bias, w_1 with the
+ *   activation flag (XVB_RELU or XVB_SWISH)
+ *   "transformer.encoders.i.conv_module.depthwise_conv"   w (D, K), bias
+ *   LayerNorms (cols 0, scale = gamma, shift = beta, or neither without affine): "transformer.encoders.i.norm_{ff,mha,
+ *   ff_macaron,conv,final}", "transformer.after_norm", ".conv_module.norm" (a BatchNorm there: folded, with XVB_BN),
+ *   "stats.attention.2", "stats.norm_stats", and "transform_out.batchnorm" / "fc1.batchnorm" / "fc2.batchnorm" when that
+ *   layer ends in a LayerNorm
+ *   "transform_out.affine", "stats.attention.0" (XVB_RELU), "stats.attention.4", "fc1.affine", "fc2.affine":
+ *   w (Cout, Cin), bias, a folded BatchNorm as scale / shift with XVB_BN, the activation flag; the segment layers are
+ *   the ones the position uses (far: fc1.affine alone; near_affine: [fc1 ->] fc2.affine alone; near: [fc1 ->] fc2)
+ * Tables, computed by the caller so that the library derives no transcendental value:
+ *   "pos_table"                    rot_pos: (5000, D / H) rotary [sin | cos]; abs_pos: (5000, D) sinusoids
+ *   "transformer.encoders.i.self_attn.att_norm"   softmax_plus only: (1, 5000), the score multiplier for T' = 0..4999
+ *
+ * Extraction takes one chunk of T >= 7 frames per utterance with T' < 5000 subsampled frames (else XVB_EINVAL).
+ * Workspace: grown to the largest call seen, then reused.  A call whose B * T exceeds 128 * 300 frames runs as
+ * consecutive groups of max(1, floor(128 * 300 / T)) utterances with the same results as one call.  At B = 128,
+ * T = 300 it is about 1.3 GB with 4x subsampling and 3.6 GB with 2x, most of it the two subsampling conv outputs.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct xvb_conformer_config {
+  int feat_dim;
+  int subsampling;        /* 4 (conv2d) or 2 (conv2d2) */
+  int D, H, linear_units, blocks, conv_kernel;
+  int pos;                /* 0 no_pos, 1 abs_pos, 2 rot_pos */
+  int rotary_value;       /* rot_pos: rotate V too */
+  int softmax_plus;       /* 0 softmax, 1 softmax_plus */
+  int act;                /* XVB_ACT_SWISH or XVB_ACT_RELU */
+  int cm_norm;            /* convolution module: 0 LayerNorm, 1 BatchNorm */
+  int out_dim;            /* transform_out */
+  int out_norm;           /* transform_out: 0 none, 1 BatchNorm (folded), 2 LayerNorm */
+  int pool_hidden;        /* AttentiveStatsPool hidden size */
+  int fc1;                /* the model has fc1 */
+  int position;           /* 0 far, 1 near_affine, 2 near */
+} xvb_conformer_config_t;
+typedef struct xvb_conformer xvb_conformer_t;
+int xvb_conformer_create(xvb_conformer_t** out, const xvb_conformer_config_t* cfg);
+int xvb_conformer_set_layer(xvb_conformer_t* h, const char* name, int rows, int cols, const float* w_host,
+                            const float* bias_host, const float* scale_host, const float* shift_host, int flags);
+/* Checks that every record the configuration needs is present with its shape (and nothing else), names the one that
+ * is not, then packs the weights on the current device. */
+int xvb_conformer_finalize(xvb_conformer_t* h);
+int xvb_conformer_feat_dim(const xvb_conformer_t* h);
+int xvb_conformer_embed_dim(const xvb_conformer_t* h);
+/* Kernels launched by the last extract call. */
+int xvb_conformer_last_launches(const xvb_conformer_t* h);
+/* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embed_dim) fp32 on the device;
+ * asynchronous on `stream`. */
+int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* "XVBC0001" model files: the configuration, then the records and tables as handed to xvb_conformer_set_layer. */
+int xvb_conformer_save(const xvb_conformer_t* h, const char* path);
+int xvb_conformer_load(xvb_conformer_t** out, const char* path);
+void xvb_conformer_destroy(xvb_conformer_t* h);
 
 /* Load a finalized extractor from an .xvbm model file (written by asv_subtools_b200.ops.Extractor.save:
  * the layers exactly as the reference's state_dict stores them, eval BatchNorm folded) -- what
