@@ -58,6 +58,11 @@ class ConformerConfig(C.Structure):
                                        "pool_hidden", "fc1", "position")]
 
 
+class CamPPConfig(C.Structure):
+    """xvb_campp_config_t (include/xvb200.h)."""
+    _fields_ = [(n, C.c_int) for n in ("feat_dim", "embd_dim", "init_channels", "growth_rate", "bn_size")]
+
+
 class XvbError(RuntimeError):
     pass
 
@@ -211,6 +216,17 @@ SIGNATURES = {
     "xvb_conformer_save": (_i, [_p, C.c_char_p]),
     "xvb_conformer_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_conformer_destroy": (None, [_p]),
+    "xvb_campp_create": (_i, [C.POINTER(_p), _p]),
+    "xvb_campp_set_layer": (_i, [_p, C.c_char_p, _i, _i, _p, _p, _p, _p, _i]),
+    "xvb_campp_finalize": (_i, [_p]),
+    "xvb_campp_feat_dim": (_i, [_p]),
+    "xvb_campp_embed_dim": (_i, [_p]),
+    "xvb_campp_last_launches": (_i, [_p]),
+    "xvb_campp_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_campp_save": (_i, [_p, C.c_char_p]),
+    "xvb_campp_load": (_i, [C.POINTER(_p), C.c_char_p]),
+    "xvb_campp_destroy": (None, [_p]),
+    "xvb_campp_chunk_sizes": (_i, [_i, _i, _ip, _i]),
     "xvb_extractor_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_extractor_feat_dim": (_i, [C.c_char_p]),
     "xvb_ark_reader_open": (_i, [C.POINTER(_p), C.c_char_p]),

@@ -1,0 +1,604 @@
+// Whole-model extractor for the CAM++ x-vector (subtools2/egrecho/models/campplus/campplus.py, CamPP.forward :355-359,
+// one chunk of CamPPModel.extract_embedding, model.py:73-96): packed weights, workspace and the launch sequence in C++,
+// so that a CAM++ model needs no Python at run time (bin/xvb-extract).  Same kernels, same C entry points, same
+// arguments and the same order as the Python driver it replaces (CamPPExtractor in
+// asv_subtools_b200/model/campplus_xvector.py, kept as XVB_CAMPP_NATIVE=0), so the embeddings are bit-identical to it:
+//
+//   FCM head: conv1 -> 4 BasicResBlocks (shortcut, conv1, conv2 + residual) -> conv2 -> copy into the time-padded
+//   frame matrix -> stride-2 tdnn (im2col view) -> per dense layer: BN1 -> ReLU, linear1 (+ BN2, ReLU), CAM gate,
+//   linear_local, y * m into the layer's column slice -> per transit: BN -> ReLU, 1x1 conv (transit3 with
+//   out_nonlinear, fp32) -> [mean | unbiased std] -> dense.
+//
+// Records arrive by state_dict module path after the Python side's folds and permutations (see xvb200.h); this file
+// only packs them.
+#include <cuda_runtime.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <map>
+#include <set>
+#include <string>
+#include <vector>
+
+#include "common.cuh"
+
+namespace {
+
+using namespace xvb;
+
+constexpr long long kFrameBudget = 128LL * 300;   // B * T frames per group of one extract call (see xvb200.h)
+constexpr int kMinFrames = 3;
+constexpr int kM = 32;                             // FCM m_channels
+constexpr int kSegLen = 100;                       // CAMLayer's segment length
+constexpr int kBlocks = 3;
+constexpr int kLayers[kBlocks] = {12, 24, 16};
+constexpr int kDilation[kBlocks] = {1, 2, 2};
+constexpr int kResBlocks = 4;                      // layer1.0, layer1.1, layer2.0, layer2.1
+constexpr int kCfgInts = 5;                        // xvb_campp_config_t as int32s, for the model file
+
+struct Rec {   // one named record exactly as handed over (host copies, for xvb_campp_save)
+  int rows = 0, cols = 0, flags = 0;
+  std::vector<float> w, b, s, t;
+};
+
+struct Planes { uint16_t* hi = nullptr; uint16_t* lo = nullptr; };
+
+struct Conv {   // a bias-free Conv2d with its eval BatchNorm as the epilogue's scale / shift
+  Planes w;
+  float* scale = nullptr; float* shift = nullptr;
+};
+
+struct Lin {   // a Conv1d on the wgmma layer kernel: y = [relu](W x + b) over the taps of `ctx`
+  Planes w;
+  float* bias = nullptr;
+  int cin = 0, cout = 0, flags = 0;
+  std::vector<int> ctx{0};
+};
+
+struct Dense {   // one CAMDenseTDNNLayer
+  float* s1 = nullptr; float* t1 = nullptr;
+  Lin lin1, local;
+  float* gw1 = nullptr; float* gb1 = nullptr; float* gw2 = nullptr; float* gb2 = nullptr;
+};
+
+struct Transit { float* s = nullptr; float* t = nullptr; Lin lin; };
+
+struct ResBlk { int stride = 1; bool has_sc = false; Conv c1, c2, sc; };
+
+struct Model {
+  xvb_campp_config_t cfg{};
+  std::map<std::string, Rec> recs;
+  std::vector<std::string> order;
+  float* conv1_w = nullptr; float* conv1_s = nullptr; float* conv1_t = nullptr;
+  ResBlk res[kResBlocks];
+  Conv conv2;
+  Lin tdnn;
+  std::vector<Dense> layers[kBlocks];
+  Transit transit[kBlocks];
+  float* dense_w = nullptr; float* dense_s = nullptr; float* dense_t = nullptr;
+  int f8 = 0, bn = 0, widths[kBlocks] = {0}, maxw = 0, c3 = 0;
+  std::vector<void*> dev;
+
+  template <typename T>
+  int alloc(T** p, size_t n) {
+    XVB_CUDA(cudaMalloc((void**)p, (n ? n : 1) * sizeof(T)));
+    dev.push_back(*p);
+    return XVB_OK;
+  }
+  int upload(float** d, const std::vector<float>& v) {
+    if (v.empty()) { *d = nullptr; return XVB_OK; }
+    int rc = alloc(d, v.size());
+    if (rc) return rc;
+    XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
+    return XVB_OK;
+  }
+  // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx (ops.pack_tdnn_weight / pack_conv2d_weight)
+  int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int tot, const std::vector<int>& ctx) {
+    float* w_dev = nullptr;
+    XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
+    cudaError_t e = cudaMemcpy(w_dev, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice);
+    const int n = (int)ctx.size(), left = ctx[0] < 0 ? ctx[0] : 0;
+    const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, n);
+    int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
+    if (!rc) rc = alloc(&c->hi, pn);
+    if (!rc) rc = alloc(&c->lo, pn);
+    if (!rc) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx.data(), n, c->hi, c->lo, nullptr);
+    if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = XVB_ECUDA;
+    if (rc == XVB_ECUDA && e != cudaSuccess) set_error("xvb_campp_finalize: weight upload failed: %s", cudaGetErrorString(e));
+    cudaFree(w_dev);
+    return rc;
+  }
+  ~Model() { for (void* p : dev) cudaFree(p); }
+};
+
+// Feature-axis size after each residual block: layerL.0 strides it by 2 (ceil), layerL.1 keeps it.
+int res_freq(int F, int j) {
+  for (int i = 0; i <= j; ++i) F = (i % 2 == 0) ? (F + 1) / 2 : F;
+  return F;
+}
+
+}  // namespace
+
+struct xvb_campp {
+  Model* m = nullptr;
+  bool finalized = false;
+  // workspace, grown to the largest call seen: each buffer has its own capacity in elements
+  enum { kX0, kA0, kO0 = kA0 + kResBlocks, kS0 = kO0 + kResBlocks, kC2 = kS0 + kResBlocks, kPad, kBuf0, kPre = kBuf0 + kBlocks,
+         kH, kZ, kPool, kGate, kStats, kBufs };
+  size_t cap[kBufs] = {0};
+  void* buf[kBufs][2] = {{nullptr}};   // [0]: fp32 or the hi plane, [1]: the lo plane
+  int pad_B = -1, pad_T = -1;          // the (B, T) layout whose pad frames are zero
+  int last_launches = 0;
+
+  void free_ws() {
+    for (int i = 0; i < kBufs; ++i) {
+      cudaFree(buf[i][0]); cudaFree(buf[i][1]);
+      buf[i][0] = buf[i][1] = nullptr;
+      cap[i] = 0;
+    }
+    pad_B = pad_T = -1;
+  }
+};
+
+namespace {
+
+using H = xvb_campp;
+
+bool is_f32(int i) { return i == H::kPool || i == H::kGate || i == H::kStats; }
+
+int reserve(H* h, int B, int T) {
+  const Model* m = h->m;
+  const size_t b = (size_t)B, t = (size_t)T, t2 = (size_t)(T + 1) / 2, row = (size_t)m->f8 * kM;
+  const size_t nseg = (t2 + kSegLen - 1) / kSegLen;
+  size_t need[H::kBufs] = {0};
+  need[H::kX0] = b * t * m->cfg.feat_dim * kM;
+  for (int j = 0; j < kResBlocks; ++j) {
+    const size_t n = b * t * res_freq(m->cfg.feat_dim, j) * kM;
+    need[H::kA0 + j] = need[H::kO0 + j] = n;
+    need[H::kS0 + j] = m->res[j].has_sc ? n : 0;
+  }
+  need[H::kC2] = b * t * row;
+  need[H::kPad] = b * (t + 4) * row;
+  for (int i = 0; i < kBlocks; ++i) need[H::kBuf0 + i] = b * t2 * m->widths[i];
+  need[H::kPre] = b * t2 * m->maxw;
+  need[H::kH] = b * t2 * m->bn;
+  need[H::kZ] = b * t2 * m->cfg.growth_rate;
+  need[H::kPool] = b * t2 * m->c3;
+  need[H::kGate] = b * nseg * m->cfg.growth_rate;
+  need[H::kStats] = b * 2 * m->c3;
+  for (int i = 0; i < H::kBufs; ++i) {
+    if (need[i] <= h->cap[i]) continue;
+    cudaFree(h->buf[i][0]); cudaFree(h->buf[i][1]);
+    h->buf[i][0] = h->buf[i][1] = nullptr;
+    h->cap[i] = 0;
+    if (i == H::kPad) h->pad_B = h->pad_T = -1;
+    const size_t bytes = need[i] * (is_f32(i) ? sizeof(float) : sizeof(uint16_t));
+    XVB_CUDA(cudaMalloc(&h->buf[i][0], bytes));
+    if (!is_f32(i)) XVB_CUDA(cudaMalloc(&h->buf[i][1], bytes));
+    h->cap[i] = need[i];
+  }
+  return XVB_OK;
+}
+
+Planes planes(H* h, int i) { return {(uint16_t*)h->buf[i][0], (uint16_t*)h->buf[i][1]}; }
+Planes offset(Planes p, size_t n) { return {p.hi + n, p.lo + n}; }
+float* f32(H* h, int i) { return (float*)h->buf[i][0]; }
+
+// _Lin.run / ops.tdnn_affine_ex: x planes (B, T, Cin) with row pitch ldx -> y planes (pitch ldy) or y_f32 (pitch ldyf)
+int lin(const Lin& l, Planes x, int64_t ldx, int Cin, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
+        int64_t x_batch_stride, void* stream) {
+  xvb_tdnn_args_t a{};
+  a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
+  a.w_hi = l.w.hi; a.w_lo = l.w.lo;
+  a.bias = l.bias;
+  a.flags = l.flags;
+  a.context_host = l.ctx.data(); a.ntaps = (int)l.ctx.size();
+  if (y) { a.y_hi = y->hi; a.y_lo = y->lo; a.ldy = ldy; }
+  if (yf) { a.y_f32 = yf; a.ldyf = ldyf; }
+  a.B = B; a.T = T; a.Cin = Cin; a.Cout = l.cout;
+  a.groups = 1;
+  a.x_batch_stride = x_batch_stride;
+  return xvb_tdnn_affine_ex(&a, stream);
+}
+
+// ops.conv2d: x (B, T, F, 32) planes -> y (B, T, F', 32) with F' = ceil(F / stride); stride_t 0 or 1 as the driver passes it
+int conv(const Conv& c, Planes x, int B, int T, int F, int ksize, int stride, int stride_t, const Planes* res, bool relu, Planes y,
+         void* stream) {
+  xvb_conv2d_args_t a{};
+  a.x_hi = x.hi; a.x_lo = x.lo;
+  a.w_hi = c.w.hi; a.w_lo = c.w.lo;
+  a.B = B; a.T = T; a.F = F; a.Cin = kM; a.Cout = kM; a.ksize = ksize; a.stride = stride; a.stride_t = stride_t;
+  a.scale = c.scale; a.shift = c.shift;
+  if (res) { a.res_hi = res->hi; a.res_lo = res->lo; }
+  a.relu = relu ? 1 : 0;
+  a.y_hi = y.hi; a.y_lo = y.lo;
+  return xvb_conv2d(&a, stream);
+}
+
+// One group of utterances: CamPPExtractor.extract.  *n counts the launches as the driver does.
+int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, void* stream) {
+  int rc = reserve(h, B, T);
+  if (rc) return rc;
+  const Model* m = h->m;
+  const xvb_campp_config_t& c = m->cfg;
+  const int g = c.growth_rate, T2 = (T + 1) / 2, row = m->f8 * kM;
+  const long long rows = (long long)B * T2;
+  // the time-padded copy of the head output: 2 zero frames before and after every utterance.  The copy below writes
+  // only the T middle frames, so the pad frames of a layout stay zero until another layout's copy lands on them.
+  const Planes pad = planes(h, H::kPad);
+  if (h->pad_B != B || h->pad_T != T) {
+    const size_t pitch = (size_t)(T + 4) * row * sizeof(uint16_t), width = (size_t)2 * row * sizeof(uint16_t);
+    for (uint16_t* p : {pad.hi, pad.lo}) {
+      XVB_CUDA(cudaMemset2DAsync(p, pitch, 0, width, B, (cudaStream_t)stream));
+      XVB_CUDA(cudaMemset2DAsync(p + (size_t)(T + 2) * row, pitch, 0, width, B, (cudaStream_t)stream));
+    }
+    h->pad_B = B; h->pad_T = T;
+  }
+  Planes x = planes(h, H::kX0);
+  if ((rc = xvb_conv2d_head(feats, B, T, c.feat_dim, m->conv1_w, kM, m->conv1_s, m->conv1_t, x.hi, x.lo, nullptr, nullptr,
+                            nullptr, nullptr, stream)))
+    return rc;
+  *n += 1;
+  int F = c.feat_dim;
+  for (int j = 0; j < kResBlocks; ++j) {
+    const ResBlk& r = m->res[j];
+    const int Fo = res_freq(c.feat_dim, j);
+    Planes res = x;
+    if (r.has_sc) {
+      res = planes(h, H::kS0 + j);
+      if ((rc = conv(r.sc, x, B, T, F, 1, r.stride, 1, nullptr, false, res, stream))) return rc;
+      *n += 1;
+    }
+    const Planes a = planes(h, H::kA0 + j), o = planes(h, H::kO0 + j);
+    if ((rc = conv(r.c1, x, B, T, F, 3, r.stride, 1, nullptr, true, a, stream)) ||
+        (rc = conv(r.c2, a, B, T, Fo, 3, 1, 0, &res, true, o, stream)))
+      return rc;
+    *n += 2;
+    x = o;
+    F = Fo;
+  }
+  const Planes c2 = planes(h, H::kC2);
+  if ((rc = conv(m->conv2, x, B, T, F, 3, 2, 1, nullptr, true, c2, stream))) return rc;
+  // the head output into the time-padded copy: one row of T * F'' * C elements per utterance
+  const int64_t tb = (int64_t)T * row * sizeof(uint16_t), pb = (int64_t)(T + 4) * row * sizeof(uint16_t);
+  if ((rc = xvb_copy_rows(c2.hi, tb, pad.hi + 2 * row, pb, B, tb, stream)) ||
+      (rc = xvb_copy_rows(c2.lo, tb, pad.lo + 2 * row, pb, B, tb, stream)))
+    return rc;
+  *n += 4;   // conv2 and the copy, counted as CamPPExtractor counts them
+  // tdnn: Conv1d(k = 5, stride 2, padding 2) as a 1-tap layer over 5-frame windows that start every 2 frames
+  Planes bufs[kBlocks];
+  for (int i = 0; i < kBlocks; ++i) bufs[i] = planes(h, H::kBuf0 + i);
+  if ((rc = lin(m->tdnn, pad, 2 * row, 5 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, stream)))
+    return rc;
+  *n += 1;
+  const Planes pre = planes(h, H::kPre), hh = planes(h, H::kH), z = planes(h, H::kZ);
+  float* gate = f32(h, H::kGate);
+  int c0 = m->tdnn.cout;
+  float* stats = f32(h, H::kStats);
+  for (int bi = 0; bi < kBlocks; ++bi) {
+    const Planes buf = bufs[bi];
+    const int width = m->widths[bi];
+    for (int li = 0; li < kLayers[bi]; ++li) {
+      const Dense& L = m->layers[bi][li];
+      const int cin = c0 + li * g;
+      Planes out = offset(buf, cin);
+      if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, cin, L.s1, L.t1, pre.hi, pre.lo, m->maxw, stream)) ||
+          (rc = lin(L.lin1, pre, m->maxw, cin, B, T2, &hh, m->bn, nullptr, 0, 0, stream)) ||
+          (rc = xvb_cam_gate(hh.hi, hh.lo, m->bn, B, T2, m->bn, kSegLen, L.gw1, L.gb1, m->bn / 2, L.gw2, L.gb2, g, gate, stream)) ||
+          (rc = lin(L.local, hh, m->bn, m->bn, B, T2, &z, g, nullptr, 0, 0, stream)) ||
+          (rc = xvb_seg_gate_apply(z.hi, z.lo, g, nullptr, nullptr, 0, gate, kSegLen, out.hi, out.lo, width, B, T2, g, stream)))
+        return rc;
+      *n += 5;
+    }
+    const Transit& tr = m->transit[bi];
+    if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, width, tr.s, tr.t, pre.hi, pre.lo, m->maxw, stream))) return rc;
+    *n += 1;
+    if (bi + 1 < kBlocks) {
+      if ((rc = lin(tr.lin, pre, m->maxw, width, B, T2, &bufs[bi + 1], m->widths[bi + 1], nullptr, 0, 0, stream))) return rc;
+      *n += 1;
+      c0 = tr.lin.cout;
+    } else {
+      // out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance
+      float* pool = f32(h, H::kPool);
+      if ((rc = lin(tr.lin, pre, m->maxw, width, B, T2, nullptr, 0, pool, m->c3, 0, stream)) ||
+          (rc = xvb_stats_pool_ex(pool, m->c3, B, T2, m->c3, 0.0f, 1, stats, nullptr, nullptr, 2 * m->c3, stream)))
+        return rc;
+      *n += 2;
+    }
+  }
+  if ((rc = xvb_small_affine(stats, 2 * m->c3, m->dense_w, B, 2 * m->c3, c.embd_dim, nullptr, m->dense_s, m->dense_t, XVB_BN, emb,
+                             c.embd_dim, nullptr, nullptr, 0, stream)))
+    return rc;
+  *n += 1;
+  return XVB_OK;
+}
+
+const Rec* find(const Model* m, const std::string& n) {
+  auto it = m->recs.find(n);
+  return it == m->recs.end() ? nullptr : &it->second;
+}
+
+void to_ints(const xvb_campp_config_t& c, int32_t* v) {
+  const int32_t a[kCfgInts] = {c.feat_dim, c.embd_dim, c.init_channels, c.growth_rate, c.bn_size};
+  memcpy(v, a, sizeof a);
+}
+
+xvb_campp_config_t from_ints(const int32_t* v) {
+  xvb_campp_config_t c{};
+  c.feat_dim = v[0]; c.embd_dim = v[1]; c.init_channels = v[2]; c.growth_rate = v[3]; c.bn_size = v[4];
+  return c;
+}
+
+}  // namespace
+
+extern "C" int xvb_campp_create(xvb_campp_t** out, const xvb_campp_config_t* cfg) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(out && cfg, "xvb_campp_create: null argument");
+  const xvb_campp_config_t& c = *cfg;
+  XVB_CHECK_ARG(c.feat_dim >= 8 && c.feat_dim <= 4096 && c.feat_dim % 8 == 0,
+                "xvb_campp_create: feat_dim %d must be a multiple of 8 in [8, 4096]", c.feat_dim);
+  XVB_CHECK_ARG(c.growth_rate > 0 && c.growth_rate % 8 == 0 && c.growth_rate <= 1024 && c.bn_size >= 1 &&
+                    c.bn_size * c.growth_rate <= 2048,
+                "xvb_campp_create: growth_rate %d (a multiple of 8), bn_size %d (bn_size * growth_rate <= 2048)", c.growth_rate,
+                c.bn_size);
+  XVB_CHECK_ARG(c.init_channels > 0 && c.init_channels % 8 == 0 && c.init_channels <= 8192 && c.embd_dim > 0 && c.embd_dim <= 8192,
+                "xvb_campp_create: init_channels %d (a multiple of 8), embd_dim %d", c.init_channels, c.embd_dim);
+  int ch = c.init_channels;
+  for (int i = 0; i < kBlocks; ++i) {
+    ch += kLayers[i] * c.growth_rate;
+    XVB_CHECK_ARG(i == kBlocks - 1 || (ch / 2) % 8 == 0, "xvb_campp_create: transit%d gives %d channels, not a multiple of 8",
+                  i + 1, ch / 2);
+    ch /= 2;
+  }
+  xvb_campp* h = new xvb_campp();
+  h->m = new Model();
+  h->m->cfg = c;
+  *out = h;
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_set_layer(xvb_campp_t* h, const char* name, int rows, int cols, const float* w_host,
+                                   const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
+  XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127,
+                "xvb_campp_set_layer: bad arguments or finalized model");
+  XVB_CHECK_ARG(rows > 0 && rows <= 65536 && cols >= 0 && cols <= (1 << 20) && (int64_t)rows * cols <= (int64_t)1 << 28,
+                "xvb_campp_set_layer(%s): bad shape %d x %d", name, rows, cols);
+  XVB_CHECK_ARG((cols > 0) == (w_host != nullptr), "xvb_campp_set_layer(%s): a weight needs cols > 0, a norm record cols 0", name);
+  XVB_CHECK_ARG((scale_host == nullptr) == (shift_host == nullptr), "xvb_campp_set_layer(%s): scale and shift go together", name);
+  XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN)) == 0, "xvb_campp_set_layer(%s): flags %d", name, flags);
+  XVB_CHECK_ARG(h->m->recs.find(name) == h->m->recs.end(), "xvb_campp_set_layer: record '%s' set twice", name);
+  Rec r;
+  r.rows = rows; r.cols = cols; r.flags = flags;
+  if (w_host) r.w.assign(w_host, w_host + (size_t)rows * cols);
+  if (bias_host) r.b.assign(bias_host, bias_host + rows);
+  if (scale_host) { r.s.assign(scale_host, scale_host + rows); r.t.assign(shift_host, shift_host + rows); }
+  h->m->recs[name] = std::move(r);
+  h->m->order.push_back(name);
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
+  XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_campp_finalize: null or finalized model");
+  Model* m = h->m;
+  const xvb_campp_config_t& c = m->cfg;
+  const int g = c.growth_rate;
+  m->f8 = c.feat_dim / 8;
+  m->bn = c.bn_size * g;
+  std::set<std::string> used;
+  // a record with its shape, whether it carries a bias and scale / shift, and its flags
+  auto need = [&](const std::string& n, int rows, int cols, bool bias, bool bn, int flags, const Rec** out) -> int {
+    const Rec* r = find(m, n);
+    XVB_CHECK_ARG(r, "xvb_campp_finalize: record '%s' is missing", n.c_str());
+    XVB_CHECK_ARG(r->rows == rows && r->cols == cols, "xvb_campp_finalize: record '%s' is %d x %d, expected %d x %d", n.c_str(),
+                  r->rows, r->cols, rows, cols);
+    XVB_CHECK_ARG(r->b.empty() != bias && r->s.empty() != bn && r->flags == flags,
+                  "xvb_campp_finalize: record '%s' needs %s bias, %s scale / shift and flags %d (has flags %d)", n.c_str(),
+                  bias ? "a" : "no", bn ? "a" : "no", flags, r->flags);
+    used.insert(n);
+    *out = r;
+    return XVB_OK;
+  };
+  auto conv = [&](const std::string& n, int cin, int ksize, int flags, Conv* cv) -> int {
+    const Rec* r;
+    int rc = need(n, kM, cin * ksize * ksize, false, true, flags, &r);
+    if (rc) return rc;
+    std::vector<int> ctx(ksize * ksize);
+    for (int i = 0; i < ksize * ksize; ++i) ctx[i] = i;
+    if ((rc = m->pack(&cv->w, r->w, kM, cin, ksize * ksize, ctx)) || (rc = m->upload(&cv->scale, r->s)) ||
+        (rc = m->upload(&cv->shift, r->t)))
+      return rc;
+    return XVB_OK;
+  };
+  auto linear = [&](const std::string& n, int cout, int cin, bool bias, int flags, Lin* l) -> int {
+    const Rec* r;
+    int rc = need(n, cout, cin, bias, false, flags, &r);
+    if (rc) return rc;
+    l->cin = cin; l->cout = cout; l->flags = flags;
+    if ((rc = m->pack(&l->w, r->w, cout, cin, 1, l->ctx)) || (rc = m->upload(&l->bias, r->b))) return rc;
+    return XVB_OK;
+  };
+  auto norm = [&](const std::string& n, int C, float** s, float** t) -> int {
+    const Rec* r;
+    int rc = need(n, C, 0, false, true, XVB_BN | XVB_RELU, &r);
+    if (rc) return rc;
+    if ((rc = m->upload(s, r->s)) || (rc = m->upload(t, r->t))) return rc;
+    return XVB_OK;
+  };
+  auto plain = [&](const std::string& n, int rows, int cols, float** w, float** b) -> int {
+    const Rec* r;
+    int rc = need(n, rows, cols, true, false, 0, &r);
+    if (rc) return rc;
+    if ((rc = m->upload(w, r->w)) || (rc = m->upload(b, r->b))) return rc;
+    return XVB_OK;
+  };
+  int rc;
+  const Rec* r;
+  if ((rc = need("head.conv1", kM, 9, false, true, XVB_BN | XVB_RELU, &r)) || (rc = m->upload(&m->conv1_w, r->w)) ||
+      (rc = m->upload(&m->conv1_s, r->s)) || (rc = m->upload(&m->conv1_t, r->t)))
+    return rc;
+  for (int j = 0; j < kResBlocks; ++j) {
+    ResBlk& b = m->res[j];
+    const std::string p = "head.layer" + std::to_string(j / 2 + 1) + "." + std::to_string(j % 2) + ".";
+    b.stride = j % 2 == 0 ? 2 : 1;
+    b.has_sc = b.stride != 1;
+    if ((rc = conv(p + "conv1", kM, 3, XVB_BN | XVB_RELU, &b.c1)) || (rc = conv(p + "conv2", kM, 3, XVB_BN | XVB_RELU, &b.c2)))
+      return rc;
+    if (b.has_sc && (rc = conv(p + "shortcut.0", kM, 1, XVB_BN, &b.sc))) return rc;
+  }
+  if ((rc = conv("head.conv2", kM, 3, XVB_BN | XVB_RELU, &m->conv2)) != XVB_OK) return rc;
+  int ch = c.init_channels;
+  if ((rc = linear("xvector.tdnn.linear", ch, 5 * m->f8 * kM, true, XVB_RELU, &m->tdnn)) != XVB_OK) return rc;
+  for (int bi = 0; bi < kBlocks; ++bi) {
+    const std::string p = "xvector.block" + std::to_string(bi + 1) + ".tdnnd";
+    const int d = kDilation[bi];
+    for (int li = 0; li < kLayers[bi]; ++li) {
+      const std::string q = p + std::to_string(li + 1) + ".";
+      const int cin = ch + li * g;
+      Dense L;
+      if ((rc = norm(q + "nonlinear1", cin, &L.s1, &L.t1)) || (rc = linear(q + "linear1", m->bn, cin, true, XVB_RELU, &L.lin1)))
+        return rc;
+      // linear_local: the dilated k = 3 kernel packed over its whole span, the gap taps as zeros (as _Lin packs it)
+      const std::string ln = q + "cam_layer.linear_local";
+      if ((rc = need(ln, g, m->bn * 3, false, false, 0, &r))) return rc;
+      const int span = 2 * d + 1;
+      std::vector<float> full((size_t)g * m->bn * span, 0.f);
+      for (size_t oc = 0; oc < (size_t)g * m->bn; ++oc)
+        for (int k = 0; k < 3; ++k) full[oc * span + k * d] = r->w[oc * 3 + k];
+      L.local.cin = m->bn; L.local.cout = g; L.local.flags = 0;
+      L.local.ctx = {-d, 0, d};
+      if ((rc = m->pack(&L.local.w, full, g, m->bn, span, L.local.ctx))) return rc;
+      if ((rc = plain(q + "cam_layer.linear1", m->bn / 2, m->bn, &L.gw1, &L.gb1)) ||
+          (rc = plain(q + "cam_layer.linear2", g, m->bn / 2, &L.gw2, &L.gb2)))
+        return rc;
+      m->layers[bi].push_back(std::move(L));
+    }
+    ch += kLayers[bi] * g;
+    m->widths[bi] = ch;
+    m->maxw = ch > m->maxw ? ch : m->maxw;
+    const std::string t = "xvector.transit" + std::to_string(bi + 1) + ".";
+    Transit& tr = m->transit[bi];
+    const bool last = bi + 1 == kBlocks;
+    if ((rc = norm(t + "nonlinear", ch, &tr.s, &tr.t)) ||
+        (rc = linear(t + "linear", ch / 2, ch, last, last ? XVB_RELU : 0, &tr.lin)))
+      return rc;
+    ch /= 2;
+  }
+  m->c3 = ch;
+  if ((rc = need("xvector.dense.linear", c.embd_dim, 2 * ch, false, true, XVB_BN, &r)) || (rc = m->upload(&m->dense_w, r->w)) ||
+      (rc = m->upload(&m->dense_s, r->s)) || (rc = m->upload(&m->dense_t, r->t)))
+    return rc;
+  for (const std::string& n : m->order)
+    XVB_CHECK_ARG(used.count(n), "xvb_campp_finalize: record '%s' is not part of this configuration", n.c_str());
+  h->finalized = true;
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_feat_dim(const xvb_campp_t* h) { return h && h->m ? h->m->cfg.feat_dim : XVB_EINVAL; }
+extern "C" int xvb_campp_embed_dim(const xvb_campp_t* h) { return h && h->m ? h->m->cfg.embd_dim : XVB_EINVAL; }
+extern "C" int xvb_campp_last_launches(const xvb_campp_t* h) { return h ? h->last_launches : 0; }
+
+extern "C" int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int T, float* emb, void* stream) {
+  XVB_CHECK_ARG(h && h->finalized, "xvb_campp_extract: model not finalized");
+  XVB_CHECK_ARG(feats && emb && B > 0, "xvb_campp_extract: bad arguments");
+  XVB_CHECK_ARG(T >= kMinFrames, "xvb_campp_extract: CAM++ needs at least %d frames per chunk, got %d", kMinFrames, T);
+  const long long per_utt = (long long)T * h->m->cfg.feat_dim;
+  int g = (int)(kFrameBudget / T);
+  if (g < 1) g = 1;
+  int n = 0;
+  for (int i = 0; i < B; i += g) {
+    const int b = B - i < g ? B - i : g;
+    int rc = extract_group(h, feats + (size_t)i * per_utt, b, T, emb + (size_t)i * h->m->cfg.embd_dim, &n, stream);
+    if (rc) return rc;
+  }
+  h->last_launches = n;
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_chunk_sizes(int T, int max_chunk, int* sizes, int cap) {
+  XVB_CHECK_ARG(T >= 1 && max_chunk >= 1, "xvb_campp_chunk_sizes: T %d and max_chunk %d must be >= 1", T, max_chunk);
+  // XvectorMixin.split_chunks(even=False): max_chunk-long chunks and a shorter last one, then the last two re-split
+  // evenly, the first of them taking the odd frame
+  const int num = T / max_chunk + (T % max_chunk ? 1 : 0);
+  XVB_CHECK_ARG(sizes && cap >= num, "xvb_campp_chunk_sizes: %d chunks do not fit in %d entries", num, cap);
+  for (int i = 0; i + 1 < num; ++i) sizes[i] = max_chunk;
+  sizes[num - 1] = T - max_chunk * (num - 1);
+  if (num > 1) {
+    const int two = sizes[num - 2] + sizes[num - 1];
+    sizes[num - 2] = two - two / 2;
+    sizes[num - 1] = two / 2;
+  }
+  return num;
+}
+
+// ---- "XVBP0001" model files: the configuration, then the records as handed over ----------------------------------
+extern "C" int xvb_campp_save(const xvb_campp_t* h, const char* path) {
+  XVB_CHECK_ARG(h && h->finalized && path, "xvb_campp_save: model not finalized");
+  const Model* m = h->m;
+  FILE* f = fopen(path, "wb");
+  XVB_CHECK_ARG(f, "xvb_campp_save: cannot open '%s'", path);
+  int32_t cfg[kCfgInts];
+  to_ints(m->cfg, cfg);
+  const int32_t nrec = (int32_t)m->order.size();
+  bool ok = fwrite("XVBP0001", 1, 8, f) == 8 && fwrite(cfg, 4, kCfgInts, f) == kCfgInts && fwrite(&nrec, 4, 1, f) == 1;
+  for (const std::string& n : m->order) {
+    const Rec& r = m->recs.at(n);
+    const int32_t nl = (int32_t)n.size();
+    const int32_t rec[6] = {r.rows, r.cols, r.flags, (int32_t)!r.w.empty(), (int32_t)!r.b.empty(), (int32_t)!r.s.empty()};
+    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(rec, 4, 6, f) == 6 &&
+         fwrite(r.w.data(), 4, r.w.size(), f) == r.w.size() && fwrite(r.b.data(), 4, r.b.size(), f) == r.b.size() &&
+         fwrite(r.s.data(), 4, r.s.size(), f) == r.s.size() && fwrite(r.t.data(), 4, r.t.size(), f) == r.t.size();
+  }
+  ok = fclose(f) == 0 && ok;
+  XVB_CHECK_ARG(ok, "xvb_campp_save: write to '%s' failed", path);
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_load(xvb_campp_t** out, const char* path) {
+  XVB_CHECK_ARG(out && path, "xvb_campp_load: null argument");
+  FILE* f = fopen(path, "rb");
+  XVB_CHECK_ARG(f, "xvb_campp_load: cannot open '%s'", path);
+  auto rd = [&](void* p, size_t n) { return fread(p, 1, n, f) == n; };
+  char magic[8];
+  int32_t cfg[kCfgInts], nrec = 0;
+  xvb_campp_t* h = nullptr;
+  int rc = XVB_EINVAL;
+  do {
+    if (!rd(magic, 8) || memcmp(magic, "XVBP0001", 8) != 0 || !rd(cfg, sizeof cfg) || !rd(&nrec, 4) || nrec < 1 || nrec > 65536) {
+      set_error("xvb_campp_load: '%s' is not an XVBP0001 file", path);
+      break;
+    }
+    const xvb_campp_config_t c = from_ints(cfg);
+    if ((rc = xvb_campp_create(&h, &c))) break;
+    std::vector<float> w, b, s, t;
+    for (int i = 0; i < nrec && rc == XVB_OK; ++i) {
+      int32_t nl = 0, rec[6];
+      char name[128];
+      bool ok = rd(&nl, 4) && nl > 0 && nl < 127 && rd(name, (size_t)nl) && rd(rec, sizeof rec) && rec[0] > 0 && rec[0] <= 65536 &&
+                rec[1] >= 0 && rec[1] <= (1 << 20) && (int64_t)rec[0] * rec[1] <= (int64_t)1 << 28 && rec[3] == (rec[1] > 0);
+      if (ok) {
+        name[nl] = 0;
+        w.resize(rec[3] ? (size_t)rec[0] * rec[1] : 0);
+        ok = rd(w.data(), w.size() * 4);
+        if (ok && rec[4]) { b.resize(rec[0]); ok = rd(b.data(), b.size() * 4); }
+        if (ok && rec[5]) { s.resize(rec[0]); t.resize(rec[0]); ok = rd(s.data(), s.size() * 4) && rd(t.data(), t.size() * 4); }
+      }
+      if (!ok) { set_error("xvb_campp_load: '%s' is truncated or corrupt at record %d", path, i); rc = XVB_EINVAL; break; }
+      rc = xvb_campp_set_layer(h, name, rec[0], rec[1], rec[3] ? w.data() : nullptr, rec[4] ? b.data() : nullptr,
+                               rec[5] ? s.data() : nullptr, rec[5] ? t.data() : nullptr, rec[2]);
+    }
+    if (rc == XVB_OK) rc = xvb_campp_finalize(h);
+  } while (0);
+  fclose(f);
+  if (rc != XVB_OK) { if (h) xvb_campp_destroy(h); return rc; }
+  *out = h;
+  return XVB_OK;
+}
+
+extern "C" void xvb_campp_destroy(xvb_campp_t* h) {
+  if (!h) return;
+  h->free_ws();
+  delete h->m;
+  delete h;
+}

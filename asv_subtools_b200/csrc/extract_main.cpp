@@ -14,13 +14,17 @@
 // :17-45: <model-path> <feats-rspecifier> <vectors-wspecifier>); the role is that of the reference's
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
-// the input side.  The model file is any of the four families, told apart by its magic: TDNN x-vector
+// the input side.  The model file is any of the five families, told apart by its magic: TDNN x-vector
 // (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
-// 2-D ResNet x-vector (XVBR0001) or Conformer x-vector (XVBC0001, 4x or 2x subsampling), the last two written by the
-// native extractors' save().  What it adds: utterances of equal length are batched (the reference runs batch 1).
+// 2-D ResNet x-vector (XVBR0001), Conformer x-vector (XVBC0001, 4x or 2x subsampling) or CAM++ x-vector (XVBP0001), the
+// last three written by the native extractors' save().  What it adds: utterances of equal length are batched (the
+// reference runs batch 1).
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
+//   * a CAM++ model keeps egrecho's rule instead (CamPPModel.extract_embedding, XvectorMixin.split_chunks with
+//     even=False, xvb_campp_chunk_sizes): max-chunk-long chunks, the last two re-split evenly (9000 -> 4000, 2500,
+//     2500); its default max-chunk is 4000;
 //   * one "FV" vector per input key (order follows batch completion, which the wspecifier allows);
 //   * errors: message with "ERROR" on stderr, exit status 1 (the reference's shell greps for it,
 //     extract_xvectors_for_pytorch.sh:144-145).  No GPU / not an H100 -> error, there is no CPU path.
@@ -63,7 +67,8 @@ struct Runner {
   xvb_extractor_t* ex = nullptr;   // TDNN x-vector family (XVBM0001) ...
   xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001 / XVBE0002) ...
   xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001) ...
-  xvb_conformer_t* cf = nullptr;   // ... or Conformer x-vector (XVBC0001)
+  xvb_conformer_t* cf = nullptr;   // ... or Conformer x-vector (XVBC0001) ...
+  xvb_campp_t* cp = nullptr;       // ... or CAM++ x-vector (XVBP0001)
   xvb_ark_writer_t* out = nullptr;
   int F = 0, D = 0, batch = 256, cmn = 0, cmn_window = 300;
   float *d_feats = nullptr, *d_tmp = nullptr, *d_emb = nullptr, *h_feats = nullptr, *h_emb = nullptr;
@@ -96,7 +101,8 @@ struct Runner {
     if (ex) CK(xvb_extractor_extract(ex, d_feats, B, T, d_emb, nullptr), "xvb_extractor_extract");
     else if (ec) CK(xvb_ecapa_extract(ec, d_feats, B, T, d_emb, nullptr), "xvb_ecapa_extract");
     else if (rn) CK(xvb_resnet_extract(rn, d_feats, B, T, d_emb, nullptr), "xvb_resnet_extract");
-    else CK(xvb_conformer_extract(cf, d_feats, B, T, d_emb, nullptr), "xvb_conformer_extract");
+    else if (cf) CK(xvb_conformer_extract(cf, d_feats, B, T, d_emb, nullptr), "xvb_conformer_extract");
+    else CK(xvb_campp_extract(cp, d_feats, B, T, d_emb, nullptr), "xvb_campp_extract");
     CU(cudaMemcpy(h_emb, d_emb, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToHost));
     for (int i = 0; i < B; ++i) {
       Utt& u = utts[items[i].utt];
@@ -193,10 +199,12 @@ int main(int argc, char** argv) {
              "                   [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001)\n"
-             "or Conformer x-vector (XVBC0001) model, recognised by its magic.  --max-chunk defaults to 300 frames for a\n"
-             "Conformer (the model's own chunk rule) and to 10000 otherwise.  A Conformer chunk needs at least 7 frames and\n"
-             "fewer than 5000 subsampled frames.\n");
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001),\n"
+             "Conformer x-vector (XVBC0001) or CAM++ x-vector (XVBP0001) model, recognised by its magic.  --max-chunk defaults\n"
+             "to 300 frames for a Conformer (the model's own chunk rule), 4000 for CAM++ and 10000 otherwise.  A Conformer\n"
+             "chunk needs at least 7 frames and fewer than 5000 subsampled frames.  CAM++ cuts an utterance with egrecho's\n"
+             "rule (max-chunk-long chunks, the last two re-split evenly: 9000 -> 4000, 2500, 2500); a chunk needs at least\n"
+             "3 frames.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -230,6 +238,11 @@ int main(int argc, char** argv) {
       r.F = xvb_conformer_feat_dim(r.cf);
       r.D = xvb_conformer_embed_dim(r.cf);
       if (!max_chunk_set) max_chunk = 300;
+    } else if (memcmp(magic, "XVBP0001", 8) == 0) {
+      CK(xvb_campp_load(&r.cp, pos[0]), "loading the CAM++ model");
+      r.F = xvb_campp_feat_dim(r.cp);
+      r.D = xvb_campp_embed_dim(r.cp);
+      if (!max_chunk_set) max_chunk = 4000;
     } else {
       CK(xvb_extractor_load(&r.ex, pos[0]), "loading the model");
       r.F = xvb_extractor_feat_dim(pos[0]);
@@ -316,12 +329,22 @@ int main(int argc, char** argv) {
     Utt u;
     u.key = key;
     u.frames = rows;
-    const int num_split = (rows + max_chunk - 1) / max_chunk, split = rows / num_split;
+    std::vector<int> lens;
+    if (r.cp) {   // egrecho's split_chunks(even=False)
+      lens.resize((size_t)rows / max_chunk + 1);
+      const int n = xvb_campp_chunk_sizes(rows, max_chunk, lens.data(), (int)lens.size());
+      if (n < 1) die("planning the CAM++ chunks");
+      lens.resize(n);
+    } else {
+      const int num_split = (rows + max_chunk - 1) / max_chunk, split = rows / num_split;
+      for (int c = 0, off = 0; c < num_split; ++c, off += split) lens.push_back(c + 1 < num_split ? split : rows - off);
+    }
+    const int num_split = (int)lens.size();
     u.pending = num_split;
     const int ui = (int)r.utts.size();
     r.utts.push_back(u);
     for (int c = 0, off = 0; c < num_split; ++c) {
-      const int len = c + 1 < num_split ? split : rows - off;
+      const int len = lens[c];
       Item it;
       it.utt = ui;
       it.frames = len;
@@ -350,6 +373,7 @@ int main(int argc, char** argv) {
   if (r.ec) xvb_ecapa_destroy(r.ec);
   if (r.rn) xvb_resnet_destroy(r.rn);
   if (r.cf) xvb_conformer_destroy(r.cf);
+  if (r.cp) xvb_campp_destroy(r.cp);
   fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
   return 0;
 }

@@ -15,7 +15,11 @@ output, every dense layer as BN1 -> ReLU (xvb_bn_relu_planes) -> linear1 with BN
 context-aware mask (xvb_cam_gate) -> linear_local -> y * m written into the layer's column slice of the block's
 concatenation buffer (xvb_seg_gate_apply); transit3 carries out_nonlinear, xvb_stats_pool_ex takes [mean | unbiased std];
 dense is xvb_small_affine.  extract_embedding applies CamPPModel's 4000-frame chunk rule (XvectorMixin.split_chunks with
-even=False)."""
+even=False).
+
+build_extractor() returns NativeCamPPExtractor: the same launch sequence in the C library (csrc/campplus_extractor.cu),
+which also writes XVBP0001 model files for bin/xvb-extract.  XVB_CAMPP_NATIVE=0 selects CamPPExtractor, the Python driver
+of the same kernels with the same embeddings bit for bit."""
 import os
 import sys
 from collections import OrderedDict
@@ -181,7 +185,10 @@ class CamPPXvector(TopVirtualNnet):
         return super().load_state_dict(backbone_state_dict(state_dict), strict=strict, **kw)
 
     def build_extractor(self):
-        return CamPPExtractor(self, self.device_for_extraction())
+        dev = self.device_for_extraction()
+        if os.environ.get("XVB_CAMPP_NATIVE", "1") == "0":
+            return CamPPExtractor(self, dev)          # op-by-op twin of the native handle
+        return NativeCamPPExtractor(self, dev)
 
     def _check(self, frames, feat_dim):
         if feat_dim != self.inputs_dim:
@@ -417,3 +424,140 @@ class CamPPExtractor:
 
     def close(self):
         self._ws_key, self._ws = None, None
+
+
+def native_config(m):
+    """xvb_campp_config_t fields of a CamPPXvector."""
+    return dict(feat_dim=m.inputs_dim, embd_dim=m.embd_dim, init_channels=m.xvector.tdnn.linear.weight.shape[0],
+                growth_rate=m.growth_rate, bn_size=m.bn_channels // m.growth_rate)
+
+
+def native_records(m):
+    """(name, w, bias, scale, shift, flags, keys) records for xvb_campp_set_layer, after the hand-over folds of
+    CamPPExtractor.__init__: every BatchNorm folded to scale / shift or into the preceding conv, the `tdnn` weight in the
+    im2col column order, out_nonlinear folded into transit3.  `keys` are the state_dict entries the record carries."""
+    from asv_subtools_b200._lib import BN, RELU
+    f = lambda t: None if t is None else (t.detach().float().cpu().numpy() if isinstance(t, torch.Tensor) else t)  # noqa: E731
+    out = []
+
+    def keys_of(mod, name):
+        return [name + "." + k for k in mod.state_dict()]
+
+    def conv(name, c, bn, bn_name, flags):
+        s, t = fold_batchnorm(bn)
+        out.append((name, f(c.weight).reshape(c.weight.shape[0], -1), None, s, t, flags,
+                    keys_of(c, name) + keys_of(bn, bn_name)))
+
+    def bn_relu(name, bn):
+        s, t = fold_batchnorm(bn)
+        out.append((name, None, None, s, t, BN | RELU, keys_of(bn, name + ".batchnorm")))
+
+    def folded(name, c, bn, bn_name, bias=None, extra=()):
+        w, b = _fold(c.weight.detach().float().cpu(), bn, bias)
+        out.append((name, f(w).reshape(w.shape[0], -1), f(b), None, None, RELU,
+                    keys_of(c, name) + keys_of(bn, bn_name) + list(extra)))
+
+    h = m.head
+    conv("head.conv1", h.conv1, h.bn1, "head.bn1", BN | RELU)
+    for li, layer in enumerate((h.layer1, h.layer2)):
+        for i, blk in enumerate(layer):
+            p = "head.layer{}.{}.".format(li + 1, i)
+            conv(p + "conv1", blk.conv1, blk.bn1, p + "bn1", BN | RELU)
+            conv(p + "conv2", blk.conv2, blk.bn2, p + "bn2", BN | RELU)
+            if len(blk.shortcut):
+                conv(p + "shortcut.0", blk.shortcut[0], blk.shortcut[1], p + "shortcut.1", BN)
+    conv("head.conv2", h.conv2, h.bn2, "head.bn2", BN | RELU)
+    xv = m.xvector
+    lin = xv.tdnn.linear
+    w, b = _fold(tdnn_im2col_weight(lin.weight.detach().float().cpu(), M_CHANNELS, m.inputs_dim // 8), xv.tdnn.nonlinear[0],
+                 lin.bias.detach().float().cpu())
+    out.append(("xvector.tdnn.linear", f(w), f(b), None, None, RELU,
+                keys_of(lin, "xvector.tdnn.linear") + keys_of(xv.tdnn.nonlinear[0], "xvector.tdnn.nonlinear.0")))
+    for bi in range(len(BLOCKS)):
+        for li, layer in enumerate(getattr(xv, "block%d" % (bi + 1))):
+            p = "xvector.block{}.tdnnd{}.".format(bi + 1, li + 1)
+            bn_relu(p + "nonlinear1", layer.nonlinear1.batchnorm)
+            folded(p + "linear1", layer.linear1, layer.nonlinear2.batchnorm, p + "nonlinear2.batchnorm")
+            cam = layer.cam_layer
+            q = p + "cam_layer."
+            out.append((q + "linear_local", f(cam.linear_local.weight).reshape(cam.linear_local.weight.shape[0], -1), None, None,
+                        None, 0, keys_of(cam.linear_local, q + "linear_local")))
+            for name in ("linear1", "linear2"):
+                c = getattr(cam, name)
+                out.append((q + name, f(c.weight).reshape(c.weight.shape[0], -1), f(c.bias), None, None, 0, keys_of(c, q + name)))
+        tr = getattr(xv, "transit%d" % (bi + 1))
+        p = "xvector.transit{}.".format(bi + 1)
+        bn_relu(p + "nonlinear", tr.nonlinear.batchnorm)
+        if bi + 1 < len(BLOCKS):
+            out.append((p + "linear", f(tr.linear.weight).reshape(tr.linear.weight.shape[0], -1), None, None, None, 0,
+                        keys_of(tr.linear, p + "linear")))
+        else:
+            folded(p + "linear", tr.linear, xv.out_nonlinear.batchnorm, "xvector.out_nonlinear.batchnorm")
+    ds, dt = fold_batchnorm(xv.dense.nonlinear[1])
+    out.append(("xvector.dense.linear", f(xv.dense.linear.weight).reshape(m.embd_dim, -1), None, ds, dt, BN,
+                keys_of(xv.dense.linear, "xvector.dense.linear") + keys_of(xv.dense.nonlinear[1], "xvector.dense.nonlinear.1")))
+    return out
+
+
+class NativeCamPPExtractor:
+    """xvb_campp_t: packed weights, workspace and the whole launch sequence of CamPPExtractor in the C library, on the
+    device that is current when it is built (or loaded from an XVBP0001 file)."""
+
+    def __init__(self, m=None, device=None, path=None):
+        import ctypes as C
+        from asv_subtools_b200._lib import CamPPConfig, check, lib
+        self._C, self._lib, self._check = C, lib, check
+        self._h = C.c_void_p()
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            if path is not None:
+                check(lib.xvb_campp_load(C.byref(self._h), str(path).encode()), "xvb_campp_load")
+            else:
+                cfg = CamPPConfig(**native_config(m))
+                check(lib.xvb_campp_create(C.byref(self._h), C.byref(cfg)), "xvb_campp_create")
+                for name, w, b, scale, shift, flags, _ in native_records(m):
+                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
+                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
+                    rows = arrs[0].shape[0] if arrs[0] is not None else arrs[2].shape[0]
+                    cols = arrs[0].shape[1] if arrs[0] is not None else 0
+                    check(lib.xvb_campp_set_layer(self._h, name.encode(), rows, cols, *ptr, flags), "xvb_campp_set_layer")
+                check(lib.xvb_campp_finalize(self._h), "xvb_campp_finalize")
+        self.feat_dim = lib.xvb_campp_feat_dim(self._h)
+        self.embed_dim = lib.xvb_campp_embed_dim(self._h)
+
+    @classmethod
+    def load(cls, path):
+        return cls(path=path)
+
+    def save(self, path):
+        """Write an XVBP0001 model file for bin/xvb-extract."""
+        self._check(self._lib.xvb_campp_save(self._h, str(path).encode()), "xvb_campp_save")
+
+    @property
+    def last_launches(self):
+        return self._lib.xvb_campp_last_launches(self._h)
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
+        stream."""
+        if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.dim() == 3):
+            raise TypeError("feats must be a (B, T, F) CUDA float32 tensor")
+        B, T, Fd = feats.shape
+        if Fd != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, Fd))
+        feats = feats.contiguous()
+        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
+        C = self._C
+        self._check(self._lib.xvb_campp_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
+                                                C.c_void_p(torch.cuda.current_stream().cuda_stream)), "xvb_campp_extract")
+        return emb
+
+    def close(self):
+        h, self._h = self._h, None
+        if h:
+            self._lib.xvb_campp_destroy(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

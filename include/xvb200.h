@@ -831,6 +831,69 @@ int xvb_conformer_save(const xvb_conformer_t* h, const char* path);
 int xvb_conformer_load(xvb_conformer_t** out, const char* path);
 void xvb_conformer_destroy(xvb_conformer_t* h);
 
+/* ---------------------------------------------------------------------------------------------
+ * Whole-model extractor for the CAM++ x-vector (subtools2/egrecho/models/campplus/campplus.py, CamPP.forward :355-359,
+ * one chunk of CamPPModel.extract_embedding, model.py:73-96): the launch sequence of xvb_conv2d_head, xvb_conv2d,
+ * xvb_copy_rows, xvb_tdnn_affine_ex, xvb_bn_relu_planes, xvb_cam_gate, xvb_seg_gate_apply, xvb_stats_pool_ex and
+ * xvb_small_affine in C++, one chunk per utterance (the chunk rule stays with the caller, see xvb_campp_chunk_sizes).
+ * Bit-identical to the op-by-op Python driver of the same kernels (CamPPExtractor, XVB_CAMPP_NATIVE=0).
+ *
+ * The block structure is fixed as in CamPP: an FCM head with 32 channels (conv1, layer1 and layer2 of two BasicResBlocks
+ * each, the first striding the feature axis by 2, conv2 with stride (2, 1)); the stride-2 `tdnn` (k = 5); three
+ * densely connected blocks of 12, 24 and 16 layers with dilations 1, 2 and 2, each followed by a transit layer that
+ * halves the width; the context-aware mask over 100-frame segments.  bn = bn_size * growth_rate, c = the width after
+ * transit3.
+ *
+ * Records (rows x cols host fp32 w, optional bias / scale / shift of `rows` entries) are named by state_dict module path
+ * and arrive after the hand-over folds of the Python side; flags are exactly the ones listed:
+ *   "head.conv1"                      w (32, 9) as stored; head.bn1 folded to scale / shift; XVB_BN | XVB_RELU
+ *   "head.layerL.i.conv1", ".conv2"   w (32, 32 * 9) as stored; bn1 / bn2 as scale / shift; XVB_BN | XVB_RELU
+ *   "head.layerL.0.shortcut.0"        w (32, 32); shortcut.1 as scale / shift; XVB_BN
+ *   "head.conv2"                      w (32, 32 * 9); head.bn2 as scale / shift; XVB_BN | XVB_RELU
+ *   "xvector.tdnn.linear"             w (init_channels, 5 * F'' * 32), F'' = feat_dim / 8, in the im2col order k * F'' * 32
+ *                                     + f * 32 + c, with tdnn.nonlinear.0 folded into w and bias; XVB_RELU
+ *   "xvector.blockB.tdnndL.nonlinear1"            cols 0, scale / shift; XVB_BN | XVB_RELU
+ *   "xvector.blockB.tdnndL.linear1"               w (bn, cin) with nonlinear2 folded into w and bias; XVB_RELU
+ *   "xvector.blockB.tdnndL.cam_layer.linear_local"  w (growth_rate, bn * 3) as stored (packed over the dilated span)
+ *   "xvector.blockB.tdnndL.cam_layer.linear1", ".linear2"   w (bn / 2, bn) and (growth_rate, bn / 2), bias each
+ *   "xvector.transitB.nonlinear"      cols 0, scale / shift; XVB_BN | XVB_RELU
+ *   "xvector.transitB.linear"         w (width / 2, width); for transit3 out_nonlinear folded into w and bias, XVB_RELU
+ *   "xvector.dense.linear"            w (embd_dim, 2 c); the affine-free BatchNorm as scale / shift; XVB_BN
+ *
+ * Extraction takes one chunk of T >= 3 frames per utterance (else XVB_EINVAL: the unbiased std over ceil(T / 2) frames
+ * needs two).  Workspace: grown to the largest call seen, then reused; the pad frames of the time-padded head copy are
+ * zeroed again whenever the (B, T) layout changes.  A call whose B * T exceeds 128 * 300 frames runs as consecutive
+ * groups of max(1, floor(128 * 300 / T)) utterances with the same results as separate calls.  The workspace is about
+ * 60 KB per input frame at feat_dim 80 with the default widths, most of it the FCM head's planes: about 2.3 GB at
+ * B = 128, T = 300.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct xvb_campp_config {
+  int feat_dim;        /* inputs_dim, a multiple of 8 */
+  int embd_dim, init_channels, growth_rate, bn_size;
+} xvb_campp_config_t;
+typedef struct xvb_campp xvb_campp_t;
+int xvb_campp_create(xvb_campp_t** out, const xvb_campp_config_t* cfg);
+int xvb_campp_set_layer(xvb_campp_t* h, const char* name, int rows, int cols, const float* w_host,
+                        const float* bias_host, const float* scale_host, const float* shift_host, int flags);
+/* Checks that every record the configuration needs is present with its shape and flags (and nothing else), names the
+ * one that is not, then packs the weights on the current device. */
+int xvb_campp_finalize(xvb_campp_t* h);
+int xvb_campp_feat_dim(const xvb_campp_t* h);
+int xvb_campp_embed_dim(const xvb_campp_t* h);
+/* Kernels launched by the last extract call. */
+int xvb_campp_last_launches(const xvb_campp_t* h);
+/* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embd_dim) fp32 on the device;
+ * asynchronous on `stream`. */
+int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* "XVBP0001" model files: the configuration, then the records as handed to xvb_campp_set_layer. */
+int xvb_campp_save(const xvb_campp_t* h, const char* path);
+int xvb_campp_load(xvb_campp_t** out, const char* path);
+void xvb_campp_destroy(xvb_campp_t* h);
+/* Host only, no GPU: the chunk sizes of egrecho's XvectorMixin.split_chunks(max_chunk, even=False) for a T-frame
+ * utterance (max_chunk-long chunks, then the last two re-split evenly, the first taking the odd frame: 9000 at 4000 ->
+ * 4000, 2500, 2500).  Writes them to sizes[0..n) and returns n, or XVB_EINVAL when T < 1, max_chunk < 1 or cap < n. */
+int xvb_campp_chunk_sizes(int T, int max_chunk, int* sizes, int cap);
+
 /* Load a finalized extractor from an .xvbm model file (written by asv_subtools_b200.ops.Extractor.save:
  * the layers exactly as the reference's state_dict stores them, eval BatchNorm folded) -- what
  * torch::jit::load does for the reference's runtime (runtime/extractor/torch_asv_model.cc:8-17). */

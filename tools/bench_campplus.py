@@ -9,7 +9,12 @@ Alternates the native extractor with the torch restatement of tests/campplus_ora
 `steps_per_round` batches per round, and reports the median over rounds of the ms per batch of each, frames/s,
 algorithmic TFLOP/s (2 x the MACs counted from the shapes), the native path's launches per batch, the largest relative
 difference between the two paths' embeddings, and the card's name and power limit, read in the same run.  Prints one
-JSON line.  --profile prints a torch.profiler kernel table of the native path and the share of its GPU time spent in
+JSON line.
+
+It also times the native handle (NativeCamPPExtractor, the launch sequence in C++) against the Python driver of the same
+kernels (CamPPExtractor, one ctypes call per launch) in the same run, alternating them, at 128 x 300 and at 8 x 300
+frames, where the per-launch host cost weighs most: ms per batch (median over rounds), frames/s, launches per batch,
+and whether the two paths' embeddings are torch.equal.  --profile prints a torch.profiler kernel table of the native path and the share of its GPU time spent in
 the BN1 -> ReLU pre-activation kernel (bn_relu_planes_kernel)."""
 import json
 import os
@@ -23,7 +28,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-from asv_subtools_b200.model.campplus_xvector import BLOCKS, CamPPXvector  # noqa: E402
+from asv_subtools_b200.model.campplus_xvector import (BLOCKS, CamPPExtractor, CamPPXvector,  # noqa: E402
+                                                      NativeCamPPExtractor)
 import campplus_oracle as co  # noqa: E402
 
 
@@ -46,6 +52,38 @@ def macs_per_chunk(T, F, m=32, init=128, growth=32, bn_size=4, embd=512):
         macs += T2 * c * (c // 2)                     # transit
         c //= 2
     return macs + 2 * c * embd
+
+
+def handle_vs_driver(m, F, rounds, steps):
+    """Native handle against the Python driver, alternating, at 128 x 300 and 8 x 300 frames."""
+    dev = torch.device("cuda")
+    paths = {"native_handle": NativeCamPPExtractor(m, dev), "python_driver": CamPPExtractor(m, dev)}
+    out = {}
+    for B, T in ((128, 300), (8, 300)):
+        xs = [co.utterances(B, T, F, 950 + i).cuda() for i in range(4)]
+        for ex in paths.values():
+            for i in range(3):
+                ex.extract(xs[i % 4])
+        torch.cuda.synchronize()
+        equal = all(torch.equal(paths["native_handle"].extract(x), paths["python_driver"].extract(x)) for x in xs)
+        times = {k: [] for k in paths}
+        for _ in range(rounds):
+            for name, ex in paths.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for i in range(steps):
+                    ex.extract(xs[i % 4])
+                e1.record()
+                torch.cuda.synchronize()
+                times[name].append(e0.elapsed_time(e1) / steps)
+        r = {"torch_equal": equal}
+        for name, ex in paths.items():
+            ms = statistics.median(times[name])
+            r[name] = {"ms_per_batch": round(ms, 3), "frames_per_s": round(B * T / ms * 1e3), "launches": ex.last_launches,
+                       "rounds_ms": [round(v, 3) for v in times[name]]}
+        out["{}x{}".format(B, T)] = r
+    paths["native_handle"].close()
+    return out
 
 
 def main():
@@ -102,6 +140,7 @@ def main():
                 e1.record()
                 torch.cuda.synchronize()
                 times[name].append(e0.elapsed_time(e1) / steps)
+        hvd = handle_vs_driver(m, F, rounds, steps)
     ms = {k: statistics.median(v) for k, v in times.items()}
     macs = macs_per_chunk(T, F)
     print(json.dumps({
@@ -114,6 +153,7 @@ def main():
         "oracle_over_native": round(ms["oracle_fp32"] / ms["native"], 3),
         "rounds_ms": {k: [round(v, 3) for v in vs] for k, vs in times.items()},
         "embedding_rel_diff_vs_oracle": diff,
+        "native_handle_vs_python_driver": hvd,
         "gpu": smi[0] if smi else "unknown"}))
 
 
