@@ -16,12 +16,10 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
-#include <set>
 #include <string>
 #include <vector>
 
-#include "common.cuh"
+#include "records.cuh"
 
 namespace {
 
@@ -35,14 +33,9 @@ constexpr int kBlocks = 3;
 constexpr int kLayers[kBlocks] = {12, 24, 16};
 constexpr int kDilation[kBlocks] = {1, 2, 2};
 constexpr int kResBlocks = 4;                      // layer1.0, layer1.1, layer2.0, layer2.1
-constexpr int kCfgInts = 5;                        // xvb_campp_config_t as int32s, for the model file
-
-struct Rec {   // one named record exactly as handed over (host copies, for xvb_campp_save)
-  int rows = 0, cols = 0, flags = 0;
-  std::vector<float> w, b, s, t;
-};
-
-struct Planes { uint16_t* hi = nullptr; uint16_t* lo = nullptr; };
+// the configuration block of a model file is the config struct, 5 int32s in declaration order
+static_assert(sizeof(xvb_campp_config_t) == 5 * sizeof(int32_t), "the XVBP0001 configuration block");
+const RecordFormat kFile = {"XVBP0001", sizeof(xvb_campp_config_t), 2, 65536};
 
 struct Conv {   // a bias-free Conv2d with its eval BatchNorm as the epilogue's scale / shift
   Planes w;
@@ -68,8 +61,7 @@ struct ResBlk { int stride = 1; bool has_sc = false; Conv c1, c2, sc; };
 
 struct Model {
   xvb_campp_config_t cfg{};
-  std::map<std::string, Rec> recs;
-  std::vector<std::string> order;
+  RecordStore recs{kFile.nshape};
   float* conv1_w = nullptr; float* conv1_s = nullptr; float* conv1_t = nullptr;
   ResBlk res[kResBlocks];
   Conv conv2;
@@ -78,38 +70,7 @@ struct Model {
   Transit transit[kBlocks];
   float* dense_w = nullptr; float* dense_s = nullptr; float* dense_t = nullptr;
   int f8 = 0, bn = 0, widths[kBlocks] = {0}, maxw = 0, c3 = 0;
-  std::vector<void*> dev;
-
-  template <typename T>
-  int alloc(T** p, size_t n) {
-    XVB_CUDA(cudaMalloc((void**)p, (n ? n : 1) * sizeof(T)));
-    dev.push_back(*p);
-    return XVB_OK;
-  }
-  int upload(float** d, const std::vector<float>& v) {
-    if (v.empty()) { *d = nullptr; return XVB_OK; }
-    int rc = alloc(d, v.size());
-    if (rc) return rc;
-    XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-    return XVB_OK;
-  }
-  // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx (ops.pack_tdnn_weight / pack_conv2d_weight)
-  int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int tot, const std::vector<int>& ctx) {
-    float* w_dev = nullptr;
-    XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
-    cudaError_t e = cudaMemcpy(w_dev, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice);
-    const int n = (int)ctx.size(), left = ctx[0] < 0 ? ctx[0] : 0;
-    const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, n);
-    int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
-    if (!rc) rc = alloc(&c->hi, pn);
-    if (!rc) rc = alloc(&c->lo, pn);
-    if (!rc) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx.data(), n, c->hi, c->lo, nullptr);
-    if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = XVB_ECUDA;
-    if (rc == XVB_ECUDA && e != cudaSuccess) set_error("xvb_campp_finalize: weight upload failed: %s", cudaGetErrorString(e));
-    cudaFree(w_dev);
-    return rc;
-  }
-  ~Model() { for (void* p : dev) cudaFree(p); }
+  Weights dev{"xvb_campp_finalize"};
 };
 
 // Feature-axis size after each residual block: layerL.0 strides it by 2 (ceil), layerL.1 keeps it.
@@ -123,29 +84,16 @@ int res_freq(int F, int j) {
 struct xvb_campp {
   Model* m = nullptr;
   bool finalized = false;
-  // workspace, grown to the largest call seen: each buffer has its own capacity in elements
   enum { kX0, kA0, kO0 = kA0 + kResBlocks, kS0 = kO0 + kResBlocks, kC2 = kS0 + kResBlocks, kPad, kBuf0, kPre = kBuf0 + kBlocks,
          kH, kZ, kPool, kGate, kStats, kBufs };
-  size_t cap[kBufs] = {0};
-  void* buf[kBufs][2] = {{nullptr}};   // [0]: fp32 or the hi plane, [1]: the lo plane
+  Workspace<kBufs> ws;
   int pad_B = -1, pad_T = -1;          // the (B, T) layout whose pad frames are zero
   int last_launches = 0;
-
-  void free_ws() {
-    for (int i = 0; i < kBufs; ++i) {
-      cudaFree(buf[i][0]); cudaFree(buf[i][1]);
-      buf[i][0] = buf[i][1] = nullptr;
-      cap[i] = 0;
-    }
-    pad_B = pad_T = -1;
-  }
 };
 
 namespace {
 
 using H = xvb_campp;
-
-bool is_f32(int i) { return i == H::kPool || i == H::kGate || i == H::kStats; }
 
 int reserve(H* h, int B, int T) {
   const Model* m = h->m;
@@ -167,23 +115,15 @@ int reserve(H* h, int B, int T) {
   need[H::kPool] = b * t2 * m->c3;
   need[H::kGate] = b * nseg * m->cfg.growth_rate;
   need[H::kStats] = b * 2 * m->c3;
-  for (int i = 0; i < H::kBufs; ++i) {
-    if (need[i] <= h->cap[i]) continue;
-    cudaFree(h->buf[i][0]); cudaFree(h->buf[i][1]);
-    h->buf[i][0] = h->buf[i][1] = nullptr;
-    h->cap[i] = 0;
-    if (i == H::kPad) h->pad_B = h->pad_T = -1;
-    const size_t bytes = need[i] * (is_f32(i) ? sizeof(float) : sizeof(uint16_t));
-    XVB_CUDA(cudaMalloc(&h->buf[i][0], bytes));
-    if (!is_f32(i)) XVB_CUDA(cudaMalloc(&h->buf[i][1], bytes));
-    h->cap[i] = need[i];
-  }
-  return XVB_OK;
+  bool planes[H::kBufs];
+  for (int i = 0; i < H::kBufs; ++i) planes[i] = i != H::kPool && i != H::kGate && i != H::kStats;
+  uint64_t grown;
+  const int rc = h->ws.reserve(need, planes, &grown);
+  if (grown >> H::kPad & 1) h->pad_B = h->pad_T = -1;
+  return rc;
 }
 
-Planes planes(H* h, int i) { return {(uint16_t*)h->buf[i][0], (uint16_t*)h->buf[i][1]}; }
 Planes offset(Planes p, size_t n) { return {p.hi + n, p.lo + n}; }
-float* f32(H* h, int i) { return (float*)h->buf[i][0]; }
 
 // _Lin.run / ops.tdnn_affine_ex: x planes (B, T, Cin) with row pitch ldx -> y planes (pitch ldy) or y_f32 (pitch ldyf)
 int lin(const Lin& l, Planes x, int64_t ldx, int Cin, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
@@ -226,7 +166,7 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
   const long long rows = (long long)B * T2;
   // the time-padded copy of the head output: 2 zero frames before and after every utterance.  The copy below writes
   // only the T middle frames, so the pad frames of a layout stay zero until another layout's copy lands on them.
-  const Planes pad = planes(h, H::kPad);
+  const Planes pad = h->ws.planes(H::kPad);
   if (h->pad_B != B || h->pad_T != T) {
     const size_t pitch = (size_t)(T + 4) * row * sizeof(uint16_t), width = (size_t)2 * row * sizeof(uint16_t);
     for (uint16_t* p : {pad.hi, pad.lo}) {
@@ -235,7 +175,7 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     }
     h->pad_B = B; h->pad_T = T;
   }
-  Planes x = planes(h, H::kX0);
+  Planes x = h->ws.planes(H::kX0);
   if ((rc = xvb_conv2d_head(feats, B, T, c.feat_dim, m->conv1_w, kM, m->conv1_s, m->conv1_t, x.hi, x.lo, nullptr, nullptr,
                             nullptr, nullptr, stream)))
     return rc;
@@ -246,11 +186,11 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     const int Fo = res_freq(c.feat_dim, j);
     Planes res = x;
     if (r.has_sc) {
-      res = planes(h, H::kS0 + j);
+      res = h->ws.planes(H::kS0 + j);
       if ((rc = conv(r.sc, x, B, T, F, 1, r.stride, 1, nullptr, false, res, stream))) return rc;
       *n += 1;
     }
-    const Planes a = planes(h, H::kA0 + j), o = planes(h, H::kO0 + j);
+    const Planes a = h->ws.planes(H::kA0 + j), o = h->ws.planes(H::kO0 + j);
     if ((rc = conv(r.c1, x, B, T, F, 3, r.stride, 1, nullptr, true, a, stream)) ||
         (rc = conv(r.c2, a, B, T, Fo, 3, 1, 0, &res, true, o, stream)))
       return rc;
@@ -258,7 +198,7 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     x = o;
     F = Fo;
   }
-  const Planes c2 = planes(h, H::kC2);
+  const Planes c2 = h->ws.planes(H::kC2);
   if ((rc = conv(m->conv2, x, B, T, F, 3, 2, 1, nullptr, true, c2, stream))) return rc;
   // the head output into the time-padded copy: one row of T * F'' * C elements per utterance
   const int64_t tb = (int64_t)T * row * sizeof(uint16_t), pb = (int64_t)(T + 4) * row * sizeof(uint16_t);
@@ -268,14 +208,14 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
   *n += 4;   // conv2 and the copy, counted as CamPPExtractor counts them
   // tdnn: Conv1d(k = 5, stride 2, padding 2) as a 1-tap layer over 5-frame windows that start every 2 frames
   Planes bufs[kBlocks];
-  for (int i = 0; i < kBlocks; ++i) bufs[i] = planes(h, H::kBuf0 + i);
+  for (int i = 0; i < kBlocks; ++i) bufs[i] = h->ws.planes(H::kBuf0 + i);
   if ((rc = lin(m->tdnn, pad, 2 * row, 5 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, stream)))
     return rc;
   *n += 1;
-  const Planes pre = planes(h, H::kPre), hh = planes(h, H::kH), z = planes(h, H::kZ);
-  float* gate = f32(h, H::kGate);
+  const Planes pre = h->ws.planes(H::kPre), hh = h->ws.planes(H::kH), z = h->ws.planes(H::kZ);
+  float* gate = h->ws.f32(H::kGate);
   int c0 = m->tdnn.cout;
-  float* stats = f32(h, H::kStats);
+  float* stats = h->ws.f32(H::kStats);
   for (int bi = 0; bi < kBlocks; ++bi) {
     const Planes buf = bufs[bi];
     const int width = m->widths[bi];
@@ -300,7 +240,7 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
       c0 = tr.lin.cout;
     } else {
       // out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance
-      float* pool = f32(h, H::kPool);
+      float* pool = h->ws.f32(H::kPool);
       if ((rc = lin(tr.lin, pre, m->maxw, width, B, T2, nullptr, 0, pool, m->c3, 0, stream)) ||
           (rc = xvb_stats_pool_ex(pool, m->c3, B, T2, m->c3, 0.0f, 1, stats, nullptr, nullptr, 2 * m->c3, stream)))
         return rc;
@@ -312,22 +252,6 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     return rc;
   *n += 1;
   return XVB_OK;
-}
-
-const Rec* find(const Model* m, const std::string& n) {
-  auto it = m->recs.find(n);
-  return it == m->recs.end() ? nullptr : &it->second;
-}
-
-void to_ints(const xvb_campp_config_t& c, int32_t* v) {
-  const int32_t a[kCfgInts] = {c.feat_dim, c.embd_dim, c.init_channels, c.growth_rate, c.bn_size};
-  memcpy(v, a, sizeof a);
-}
-
-xvb_campp_config_t from_ints(const int32_t* v) {
-  xvb_campp_config_t c{};
-  c.feat_dim = v[0]; c.embd_dim = v[1]; c.init_channels = v[2]; c.growth_rate = v[3]; c.bn_size = v[4];
-  return c;
 }
 
 }  // namespace
@@ -363,20 +287,12 @@ extern "C" int xvb_campp_set_layer(xvb_campp_t* h, const char* name, int rows, i
                                    const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
   XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127,
                 "xvb_campp_set_layer: bad arguments or finalized model");
-  XVB_CHECK_ARG(rows > 0 && rows <= 65536 && cols >= 0 && cols <= (1 << 20) && (int64_t)rows * cols <= (int64_t)1 << 28,
-                "xvb_campp_set_layer(%s): bad shape %d x %d", name, rows, cols);
-  XVB_CHECK_ARG((cols > 0) == (w_host != nullptr), "xvb_campp_set_layer(%s): a weight needs cols > 0, a norm record cols 0", name);
-  XVB_CHECK_ARG((scale_host == nullptr) == (shift_host == nullptr), "xvb_campp_set_layer(%s): scale and shift go together", name);
+  const char* fn = "xvb_campp_set_layer";
+  const int shape[2] = {rows, cols};
+  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  if (rc) return rc;
   XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN)) == 0, "xvb_campp_set_layer(%s): flags %d", name, flags);
-  XVB_CHECK_ARG(h->m->recs.find(name) == h->m->recs.end(), "xvb_campp_set_layer: record '%s' set twice", name);
-  Rec r;
-  r.rows = rows; r.cols = cols; r.flags = flags;
-  if (w_host) r.w.assign(w_host, w_host + (size_t)rows * cols);
-  if (bias_host) r.b.assign(bias_host, bias_host + rows);
-  if (scale_host) { r.s.assign(scale_host, scale_host + rows); r.t.assign(shift_host, shift_host + rows); }
-  h->m->recs[name] = std::move(r);
-  h->m->order.push_back(name);
-  return XVB_OK;
+  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
 extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
@@ -386,28 +302,23 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
   const int g = c.growth_rate;
   m->f8 = c.feat_dim / 8;
   m->bn = c.bn_size * g;
-  std::set<std::string> used;
   // a record with its shape, whether it carries a bias and scale / shift, and its flags
   auto need = [&](const std::string& n, int rows, int cols, bool bias, bool bn, int flags, const Rec** out) -> int {
-    const Rec* r = find(m, n);
-    XVB_CHECK_ARG(r, "xvb_campp_finalize: record '%s' is missing", n.c_str());
-    XVB_CHECK_ARG(r->rows == rows && r->cols == cols, "xvb_campp_finalize: record '%s' is %d x %d, expected %d x %d", n.c_str(),
-                  r->rows, r->cols, rows, cols);
+    const int shape[2] = {rows, cols};
+    int rc = m->recs.take("xvb_campp_finalize", n, shape, out);
+    if (rc) return rc;
+    const Rec* r = *out;
     XVB_CHECK_ARG(r->b.empty() != bias && r->s.empty() != bn && r->flags == flags,
                   "xvb_campp_finalize: record '%s' needs %s bias, %s scale / shift and flags %d (has flags %d)", n.c_str(),
                   bias ? "a" : "no", bn ? "a" : "no", flags, r->flags);
-    used.insert(n);
-    *out = r;
     return XVB_OK;
   };
   auto conv = [&](const std::string& n, int cin, int ksize, int flags, Conv* cv) -> int {
     const Rec* r;
     int rc = need(n, kM, cin * ksize * ksize, false, true, flags, &r);
     if (rc) return rc;
-    std::vector<int> ctx(ksize * ksize);
-    for (int i = 0; i < ksize * ksize; ++i) ctx[i] = i;
-    if ((rc = m->pack(&cv->w, r->w, kM, cin, ksize * ksize, ctx)) || (rc = m->upload(&cv->scale, r->s)) ||
-        (rc = m->upload(&cv->shift, r->t)))
+    if ((rc = m->dev.pack(&cv->w, r->w, kM, cin, ksize * ksize, kTaps, ksize * ksize)) || (rc = m->dev.upload(&cv->scale, r->s)) ||
+        (rc = m->dev.upload(&cv->shift, r->t)))
       return rc;
     return XVB_OK;
   };
@@ -416,27 +327,27 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
     int rc = need(n, cout, cin, bias, false, flags, &r);
     if (rc) return rc;
     l->cin = cin; l->cout = cout; l->flags = flags;
-    if ((rc = m->pack(&l->w, r->w, cout, cin, 1, l->ctx)) || (rc = m->upload(&l->bias, r->b))) return rc;
+    if ((rc = m->dev.pack(&l->w, r->w, cout, cin, 1, l->ctx.data(), (int)l->ctx.size())) || (rc = m->dev.upload(&l->bias, r->b))) return rc;
     return XVB_OK;
   };
   auto norm = [&](const std::string& n, int C, float** s, float** t) -> int {
     const Rec* r;
     int rc = need(n, C, 0, false, true, XVB_BN | XVB_RELU, &r);
     if (rc) return rc;
-    if ((rc = m->upload(s, r->s)) || (rc = m->upload(t, r->t))) return rc;
+    if ((rc = m->dev.upload(s, r->s)) || (rc = m->dev.upload(t, r->t))) return rc;
     return XVB_OK;
   };
   auto plain = [&](const std::string& n, int rows, int cols, float** w, float** b) -> int {
     const Rec* r;
     int rc = need(n, rows, cols, true, false, 0, &r);
     if (rc) return rc;
-    if ((rc = m->upload(w, r->w)) || (rc = m->upload(b, r->b))) return rc;
+    if ((rc = m->dev.upload(w, r->w)) || (rc = m->dev.upload(b, r->b))) return rc;
     return XVB_OK;
   };
   int rc;
   const Rec* r;
-  if ((rc = need("head.conv1", kM, 9, false, true, XVB_BN | XVB_RELU, &r)) || (rc = m->upload(&m->conv1_w, r->w)) ||
-      (rc = m->upload(&m->conv1_s, r->s)) || (rc = m->upload(&m->conv1_t, r->t)))
+  if ((rc = need("head.conv1", kM, 9, false, true, XVB_BN | XVB_RELU, &r)) || (rc = m->dev.upload(&m->conv1_w, r->w)) ||
+      (rc = m->dev.upload(&m->conv1_s, r->s)) || (rc = m->dev.upload(&m->conv1_t, r->t)))
     return rc;
   for (int j = 0; j < kResBlocks; ++j) {
     ResBlk& b = m->res[j];
@@ -468,7 +379,7 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
         for (int k = 0; k < 3; ++k) full[oc * span + k * d] = r->w[oc * 3 + k];
       L.local.cin = m->bn; L.local.cout = g; L.local.flags = 0;
       L.local.ctx = {-d, 0, d};
-      if ((rc = m->pack(&L.local.w, full, g, m->bn, span, L.local.ctx))) return rc;
+      if ((rc = m->dev.pack(&L.local.w, full, g, m->bn, span, L.local.ctx.data(), (int)L.local.ctx.size()))) return rc;
       if ((rc = plain(q + "cam_layer.linear1", m->bn / 2, m->bn, &L.gw1, &L.gb1)) ||
           (rc = plain(q + "cam_layer.linear2", g, m->bn / 2, &L.gw2, &L.gb2)))
         return rc;
@@ -486,11 +397,10 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
     ch /= 2;
   }
   m->c3 = ch;
-  if ((rc = need("xvector.dense.linear", c.embd_dim, 2 * ch, false, true, XVB_BN, &r)) || (rc = m->upload(&m->dense_w, r->w)) ||
-      (rc = m->upload(&m->dense_s, r->s)) || (rc = m->upload(&m->dense_t, r->t)))
+  if ((rc = need("xvector.dense.linear", c.embd_dim, 2 * ch, false, true, XVB_BN, &r)) || (rc = m->dev.upload(&m->dense_w, r->w)) ||
+      (rc = m->dev.upload(&m->dense_s, r->s)) || (rc = m->dev.upload(&m->dense_t, r->t)))
     return rc;
-  for (const std::string& n : m->order)
-    XVB_CHECK_ARG(used.count(n), "xvb_campp_finalize: record '%s' is not part of this configuration", n.c_str());
+  if ((rc = m->recs.check_all_used("xvb_campp_finalize"))) return rc;
   h->finalized = true;
   return XVB_OK;
 }
@@ -503,15 +413,11 @@ extern "C" int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int 
   XVB_CHECK_ARG(h && h->finalized, "xvb_campp_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0, "xvb_campp_extract: bad arguments");
   XVB_CHECK_ARG(T >= kMinFrames, "xvb_campp_extract: CAM++ needs at least %d frames per chunk, got %d", kMinFrames, T);
-  const long long per_utt = (long long)T * h->m->cfg.feat_dim;
-  int g = (int)(kFrameBudget / T);
-  if (g < 1) g = 1;
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->cfg.embd_dim;
   int n = 0;
-  for (int i = 0; i < B; i += g) {
-    const int b = B - i < g ? B - i : g;
-    int rc = extract_group(h, feats + (size_t)i * per_utt, b, T, emb + (size_t)i * h->m->cfg.embd_dim, &n, stream);
-    if (rc) return rc;
-  }
+  int rc = for_groups(B, T, kFrameBudget,
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, &n, stream); });
+  if (rc) return rc;
   h->last_launches = n;
   return XVB_OK;
 }
@@ -532,73 +438,24 @@ extern "C" int xvb_campp_chunk_sizes(int T, int max_chunk, int* sizes, int cap) 
   return num;
 }
 
-// ---- "XVBP0001" model files: the configuration, then the records as handed over ----------------------------------
+// ---- "XVBP0001" model files: the configuration, then the records as handed over (save_records) ------------------
 extern "C" int xvb_campp_save(const xvb_campp_t* h, const char* path) {
   XVB_CHECK_ARG(h && h->finalized && path, "xvb_campp_save: model not finalized");
-  const Model* m = h->m;
-  FILE* f = fopen(path, "wb");
-  XVB_CHECK_ARG(f, "xvb_campp_save: cannot open '%s'", path);
-  int32_t cfg[kCfgInts];
-  to_ints(m->cfg, cfg);
-  const int32_t nrec = (int32_t)m->order.size();
-  bool ok = fwrite("XVBP0001", 1, 8, f) == 8 && fwrite(cfg, 4, kCfgInts, f) == kCfgInts && fwrite(&nrec, 4, 1, f) == 1;
-  for (const std::string& n : m->order) {
-    const Rec& r = m->recs.at(n);
-    const int32_t nl = (int32_t)n.size();
-    const int32_t rec[6] = {r.rows, r.cols, r.flags, (int32_t)!r.w.empty(), (int32_t)!r.b.empty(), (int32_t)!r.s.empty()};
-    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(rec, 4, 6, f) == 6 &&
-         fwrite(r.w.data(), 4, r.w.size(), f) == r.w.size() && fwrite(r.b.data(), 4, r.b.size(), f) == r.b.size() &&
-         fwrite(r.s.data(), 4, r.s.size(), f) == r.s.size() && fwrite(r.t.data(), 4, r.t.size(), f) == r.t.size();
-  }
-  ok = fclose(f) == 0 && ok;
-  XVB_CHECK_ARG(ok, "xvb_campp_save: write to '%s' failed", path);
-  return XVB_OK;
+  return save_records("xvb_campp_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
 extern "C" int xvb_campp_load(xvb_campp_t** out, const char* path) {
-  XVB_CHECK_ARG(out && path, "xvb_campp_load: null argument");
-  FILE* f = fopen(path, "rb");
-  XVB_CHECK_ARG(f, "xvb_campp_load: cannot open '%s'", path);
-  auto rd = [&](void* p, size_t n) { return fread(p, 1, n, f) == n; };
-  char magic[8];
-  int32_t cfg[kCfgInts], nrec = 0;
-  xvb_campp_t* h = nullptr;
-  int rc = XVB_EINVAL;
-  do {
-    if (!rd(magic, 8) || memcmp(magic, "XVBP0001", 8) != 0 || !rd(cfg, sizeof cfg) || !rd(&nrec, 4) || nrec < 1 || nrec > 65536) {
-      set_error("xvb_campp_load: '%s' is not an XVBP0001 file", path);
-      break;
-    }
-    const xvb_campp_config_t c = from_ints(cfg);
-    if ((rc = xvb_campp_create(&h, &c))) break;
-    std::vector<float> w, b, s, t;
-    for (int i = 0; i < nrec && rc == XVB_OK; ++i) {
-      int32_t nl = 0, rec[6];
-      char name[128];
-      bool ok = rd(&nl, 4) && nl > 0 && nl < 127 && rd(name, (size_t)nl) && rd(rec, sizeof rec) && rec[0] > 0 && rec[0] <= 65536 &&
-                rec[1] >= 0 && rec[1] <= (1 << 20) && (int64_t)rec[0] * rec[1] <= (int64_t)1 << 28 && rec[3] == (rec[1] > 0);
-      if (ok) {
-        name[nl] = 0;
-        w.resize(rec[3] ? (size_t)rec[0] * rec[1] : 0);
-        ok = rd(w.data(), w.size() * 4);
-        if (ok && rec[4]) { b.resize(rec[0]); ok = rd(b.data(), b.size() * 4); }
-        if (ok && rec[5]) { s.resize(rec[0]); t.resize(rec[0]); ok = rd(s.data(), s.size() * 4) && rd(t.data(), t.size() * 4); }
-      }
-      if (!ok) { set_error("xvb_campp_load: '%s' is truncated or corrupt at record %d", path, i); rc = XVB_EINVAL; break; }
-      rc = xvb_campp_set_layer(h, name, rec[0], rec[1], rec[3] ? w.data() : nullptr, rec[4] ? b.data() : nullptr,
-                               rec[5] ? s.data() : nullptr, rec[5] ? t.data() : nullptr, rec[2]);
-    }
-    if (rc == XVB_OK) rc = xvb_campp_finalize(h);
-  } while (0);
-  fclose(f);
-  if (rc != XVB_OK) { if (h) xvb_campp_destroy(h); return rc; }
-  *out = h;
-  return XVB_OK;
+  return load_records(
+      "xvb_campp_load", path, kFile, (void**)out,
+      [](void** h, const void* cfg) { return xvb_campp_create((xvb_campp_t**)h, (const xvb_campp_config_t*)cfg); },
+      [](void* h, const char* name, const int* shape, const float* w, const float* b, const float* s, const float* t, int flags) {
+        return xvb_campp_set_layer((xvb_campp_t*)h, name, shape[0], shape[1], w, b, s, t, flags);
+      },
+      [](void* h) { return xvb_campp_finalize((xvb_campp_t*)h); }, [](void* h) { xvb_campp_destroy((xvb_campp_t*)h); });
 }
 
 extern "C" void xvb_campp_destroy(xvb_campp_t* h) {
   if (!h) return;
-  h->free_ws();
   delete h->m;
   delete h;
 }

@@ -18,12 +18,10 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
-#include <set>
 #include <string>
 #include <vector>
 
-#include "common.cuh"
+#include "records.cuh"
 
 namespace {
 
@@ -32,14 +30,9 @@ using namespace xvb;
 constexpr long long kFrameBudget = 128LL * 300;   // B * T frames per group of one extract call (see xvb200.h)
 constexpr int kTableRows = 5000;                   // PositionalEncoding max_len (embedding.py:41)
 constexpr int kMinFrames = 7;
-constexpr int kCfgInts = 17;                       // xvb_conformer_config_t as int32s, for the model file
-
-struct Rec {   // one named record exactly as handed over (host copies, for xvb_conformer_save)
-  int rows = 0, cols = 0, flags = 0;
-  std::vector<float> w, b, s, t;
-};
-
-struct Planes { uint16_t* hi = nullptr; uint16_t* lo = nullptr; };
+// the configuration block of a model file is the config struct, 17 int32s in declaration order
+static_assert(sizeof(xvb_conformer_config_t) == 17 * sizeof(int32_t), "the XVBC0001 configuration block");
+const RecordFormat kFile = {"XVBC0001", sizeof(xvb_conformer_config_t), 2, 65536};
 
 struct Lin {   // a Linear / 1x1 conv on the wgmma layer kernel: y = epi(W x + b)
   Planes w;
@@ -57,8 +50,7 @@ struct Seg { Lin lin; bool ln = false; Ln norm; };
 
 struct Model {
   xvb_conformer_config_t cfg{};
-  std::map<std::string, Rec> recs;
-  std::vector<std::string> order;
+  RecordStore recs{kFile.nshape};
   float* head_w = nullptr; float* head_b = nullptr;
   Planes conv2_w;
   float* conv2_scale = nullptr; float* conv2_shift = nullptr;
@@ -71,39 +63,7 @@ struct Model {
   Ln transform_norm, att_ln, norm_stats;
   std::vector<Seg> seg;
   int E = 0, dk = 0, F2 = 0;
-  std::vector<void*> dev;
-
-  template <typename T>
-  int alloc(T** p, size_t n) {
-    XVB_CUDA(cudaMalloc((void**)p, (n ? n : 1) * sizeof(T)));
-    dev.push_back(*p);
-    return XVB_OK;
-  }
-  int upload(float** d, const std::vector<float>& v) {
-    if (v.empty()) { *d = nullptr; return XVB_OK; }
-    int rc = alloc(d, v.size());
-    if (rc) return rc;
-    XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-    return XVB_OK;
-  }
-  // (Cout, Cin, taps) fp32 host -> packed planes, taps 0..ntaps-1 (ops.pack_tdnn_weight / pack_conv2d_weight)
-  int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int ntaps) {
-    float* w_dev = nullptr;
-    XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
-    cudaError_t e = cudaMemcpy(w_dev, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice);
-    int ctx[XVB_MAX_TAPS];
-    for (int i = 0; i < ntaps; ++i) ctx[i] = i;
-    const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, ntaps);
-    int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
-    if (!rc) rc = alloc(&c->hi, pn);
-    if (!rc) rc = alloc(&c->lo, pn);
-    if (!rc) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, ntaps, 0, ctx, ntaps, c->hi, c->lo, nullptr);
-    if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = XVB_ECUDA;
-    if (rc == XVB_ECUDA && e != cudaSuccess) set_error("xvb_conformer_finalize: weight upload failed: %s", cudaGetErrorString(e));
-    cudaFree(w_dev);
-    return rc;
-  }
-  ~Model() { for (void* p : dev) cudaFree(p); }
+  Weights dev{"xvb_conformer_finalize"};
 };
 
 // Subsampled sizes of one chunk of T frames: (T1, F1) after the head conv, (T2, F2) after the valid conv.
@@ -125,19 +85,9 @@ void sub_shape(const xvb_conformer_config_t& c, int T, int* T1, int* F1, int* T2
 struct xvb_conformer {
   Model* m = nullptr;
   bool finalized = false;
-  // workspace, grown to the largest call seen: each buffer has its own capacity in elements
   enum { kX1, kX2, kR, kH, kHid, kDelta, kQkv, kXo, kXp, kA1, kAp, kLogits, kStats, kZ, kZf, kSegY, kSegP, kBufs };
-  size_t cap[kBufs] = {0};
-  void* buf[kBufs][2] = {{nullptr}};   // [0]: fp32 or the hi plane, [1]: the lo plane
+  Workspace<kBufs> ws;
   int last_launches = 0;
-
-  void free_ws() {
-    for (int i = 0; i < kBufs; ++i) {
-      cudaFree(buf[i][0]); cudaFree(buf[i][1]);
-      buf[i][0] = buf[i][1] = nullptr;
-      cap[i] = 0;
-    }
-  }
 };
 
 namespace {
@@ -156,21 +106,9 @@ int reserve(xvb_conformer* h, int B, int T) {
   const size_t need[xvb_conformer::kBufs] = {
       b * T1 * F1 * D, b * T2 * F2 * D, r2 * D, r2 * D, r2 * units, r2 * 2 * D, r2 * 3 * D, r2 * od, r2 * od,
       r2 * c.pool_hidden, r2 * c.pool_hidden, r2 * od, b * 2 * od, b * 2 * od, b * 2 * od, b * seg, b * seg};
-  for (int i = 0; i < xvb_conformer::kBufs; ++i) {
-    if (need[i] <= h->cap[i]) continue;
-    cudaFree(h->buf[i][0]); cudaFree(h->buf[i][1]);
-    h->buf[i][0] = h->buf[i][1] = nullptr;
-    h->cap[i] = 0;
-    const size_t bytes = need[i] * (kPlanes[i] ? sizeof(uint16_t) : sizeof(float));
-    XVB_CUDA(cudaMalloc(&h->buf[i][0], bytes));
-    if (kPlanes[i]) XVB_CUDA(cudaMalloc(&h->buf[i][1], bytes));
-    h->cap[i] = need[i];
-  }
-  return XVB_OK;
+  uint64_t grown;
+  return h->ws.reserve(need, kPlanes, &grown);
 }
-
-Planes planes(xvb_conformer* h, int i) { return {(uint16_t*)h->buf[i][0], (uint16_t*)h->buf[i][1]}; }
-float* f32(xvb_conformer* h, int i) { return (float*)h->buf[i][0]; }
 
 // _Lin.run: x planes (B, T, Cin) with row pitch ldx -> y planes (pitch ldy) and / or y_f32 (pitch ldyf)
 int lin(const Lin& l, Planes x, int64_t ldx, int Cin, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
@@ -224,7 +162,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   int T1, F1, T2, F2;
   sub_shape(c, T, &T1, &F1, &T2, &F2);
   const long long rows = (long long)B * T2;
-  const Planes x1 = planes(h, xvb_conformer::kX1), x2 = planes(h, xvb_conformer::kX2);
+  const Planes x1 = h->ws.planes(xvb_conformer::kX1), x2 = h->ws.planes(xvb_conformer::kX2);
   if (c.subsampling == 4)
     rc = xvb_subsample_head(feats, B, T, c.feat_dim, m->head_w, m->head_b, D, x1.hi, x1.lo, stream);
   else
@@ -240,14 +178,14 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     a.y_hi = x2.hi; a.y_lo = x2.lo;
     if ((rc = xvb_conv2d_valid(&a, stream)) != XVB_OK) return rc;
   }
-  float* r = f32(h, xvb_conformer::kR);
+  float* r = h->ws.f32(xvb_conformer::kR);
   if ((rc = lin(m->embed_out, x2, (int64_t)F2 * D, F2 * D, B, T2, nullptr, 0, r, D, stream)) != XVB_OK) return rc;
   *n += 3;
   const int units = c.linear_units;
   const int hid_ld = units > D ? units : D;
-  const Planes hh = planes(h, xvb_conformer::kH), hid = planes(h, xvb_conformer::kHid);
-  float* delta = f32(h, xvb_conformer::kDelta);
-  float* qkv = f32(h, xvb_conformer::kQkv);
+  const Planes hh = h->ws.planes(xvb_conformer::kH), hid = h->ws.planes(xvb_conformer::kHid);
+  float* delta = h->ws.f32(xvb_conformer::kDelta);
+  float* qkv = h->ws.f32(xvb_conformer::kQkv);
   float* d1 = delta;   // delta[..., :D], pitch 2D
   const float* rope = c.pos == 2 ? m->table : nullptr;
   const float* absp = c.pos == 1 ? m->table : nullptr;
@@ -300,8 +238,8 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   }
   // transform_out (+ its LayerNorm): x fp32 for the pooling sums, planes for the attention conv
   const int od = c.out_dim, hd = c.pool_hidden;
-  float* xo = f32(h, xvb_conformer::kXo);
-  const Planes xp = planes(h, xvb_conformer::kXp);
+  float* xo = h->ws.f32(xvb_conformer::kXo);
+  const Planes xp = h->ws.planes(xvb_conformer::kXp);
   if (!m->transform_ln) {
     if ((rc = lin(m->transform, hh, D, D, B, T2, &xp, od, xo, od, stream)) != XVB_OK) return rc;
     *n += 1;
@@ -315,9 +253,9 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     *n += 2;
   }
   // AttentiveStatsPool
-  float* a1 = f32(h, xvb_conformer::kA1);
+  float* a1 = h->ws.f32(xvb_conformer::kA1);
   if ((rc = lin(m->att1, xp, od, od, B, T2, nullptr, 0, a1, hd, stream)) != XVB_OK) return rc;
-  const Planes ap = planes(h, xvb_conformer::kAp);
+  const Planes ap = h->ws.planes(xvb_conformer::kAp);
   {
     LnCall l{rows, hd, a1, hd};
     l.n = m->att_ln;
@@ -325,12 +263,12 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     l.y = &ap; l.ldy = hd;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
   }
-  float* logits = f32(h, xvb_conformer::kLogits);
+  float* logits = h->ws.f32(xvb_conformer::kLogits);
   if ((rc = lin(m->att2, ap, hd, hd, B, T2, nullptr, 0, logits, od, stream)) != XVB_OK) return rc;
-  float* stats = f32(h, xvb_conformer::kStats);
+  float* stats = h->ws.f32(xvb_conformer::kStats);
   if ((rc = xvb_attn_stats_pool(logits, od, xo, od, B, T2, od, 1e-5f, stats, nullptr, nullptr, 2 * od, stream)) != XVB_OK) return rc;
-  Planes z = planes(h, xvb_conformer::kZ);
-  float* zf = f32(h, xvb_conformer::kZf);
+  Planes z = h->ws.planes(xvb_conformer::kZ);
+  float* zf = h->ws.f32(xvb_conformer::kZf);
   {
     LnCall l{B, 2 * od, stats, 2 * od};
     l.n = m->norm_stats;
@@ -345,10 +283,10 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     const Seg& s = m->seg[j];
     const bool last = j + 1 == ns;
     const int co = s.lin.cout;
-    float* y = last ? emb : f32(h, xvb_conformer::kSegY);
+    float* y = last ? emb : h->ws.f32(xvb_conformer::kSegY);
     if ((rc = lin(s.lin, z, zc, zc, B, 1, nullptr, 0, y, co, stream)) != XVB_OK) return rc;
     *n += 1;
-    const Planes yp = planes(h, xvb_conformer::kSegP);
+    const Planes yp = h->ws.planes(xvb_conformer::kSegP);
     if (s.ln) {
       LnCall l{B, co, y, co};
       l.n = s.norm;
@@ -364,26 +302,6 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     zc = co;
   }
   return XVB_OK;
-}
-
-const Rec* find(const Model* m, const std::string& n) {
-  auto it = m->recs.find(n);
-  return it == m->recs.end() ? nullptr : &it->second;
-}
-
-void to_ints(const xvb_conformer_config_t& c, int32_t* v) {
-  const int32_t a[kCfgInts] = {c.feat_dim, c.subsampling, c.D, c.H, c.linear_units, c.blocks, c.conv_kernel, c.pos,
-                               c.rotary_value, c.softmax_plus, c.act, c.cm_norm, c.out_dim, c.out_norm, c.pool_hidden, c.fc1,
-                               c.position};
-  memcpy(v, a, sizeof a);
-}
-
-xvb_conformer_config_t from_ints(const int32_t* v) {
-  xvb_conformer_config_t c{};
-  c.feat_dim = v[0]; c.subsampling = v[1]; c.D = v[2]; c.H = v[3]; c.linear_units = v[4]; c.blocks = v[5];
-  c.conv_kernel = v[6]; c.pos = v[7]; c.rotary_value = v[8]; c.softmax_plus = v[9]; c.act = v[10]; c.cm_norm = v[11];
-  c.out_dim = v[12]; c.out_norm = v[13]; c.pool_hidden = v[14]; c.fc1 = v[15]; c.position = v[16];
-  return c;
 }
 
 }  // namespace
@@ -421,21 +339,13 @@ extern "C" int xvb_conformer_set_layer(xvb_conformer_t* h, const char* name, int
                                        const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
   XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127,
                 "xvb_conformer_set_layer: bad arguments or finalized model");
-  XVB_CHECK_ARG(rows > 0 && rows <= 65536 && cols >= 0 && cols <= (1 << 20) && (int64_t)rows * cols <= (int64_t)1 << 28,
-                "xvb_conformer_set_layer(%s): bad shape %d x %d", name, rows, cols);
-  XVB_CHECK_ARG((cols > 0) == (w_host != nullptr), "xvb_conformer_set_layer(%s): a weight needs cols > 0, a norm record cols 0", name);
-  XVB_CHECK_ARG((scale_host == nullptr) == (shift_host == nullptr), "xvb_conformer_set_layer(%s): scale and shift go together", name);
+  const char* fn = "xvb_conformer_set_layer";
+  const int shape[2] = {rows, cols};
+  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  if (rc) return rc;
   XVB_CHECK_ARG(!(flags & XVB_BN) || scale_host, "xvb_conformer_set_layer(%s): XVB_BN without scale/shift", name);
   XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN | XVB_SWISH)) == 0, "xvb_conformer_set_layer(%s): flags %d", name, flags);
-  XVB_CHECK_ARG(h->m->recs.find(name) == h->m->recs.end(), "xvb_conformer_set_layer: record '%s' set twice", name);
-  Rec r;
-  r.rows = rows; r.cols = cols; r.flags = flags;
-  if (w_host) r.w.assign(w_host, w_host + (size_t)rows * cols);
-  if (bias_host) r.b.assign(bias_host, bias_host + rows);
-  if (scale_host) { r.s.assign(scale_host, scale_host + rows); r.t.assign(shift_host, shift_host + rows); }
-  h->m->recs[name] = std::move(r);
-  h->m->order.push_back(name);
-  return XVB_OK;
+  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
 extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
@@ -443,15 +353,9 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
   Model* m = h->m;
   const xvb_conformer_config_t& c = m->cfg;
   const int D = c.D;
-  std::set<std::string> used;
   auto need = [&](const std::string& n, int rows, int cols, const Rec** out) -> int {
-    const Rec* r = find(m, n);
-    XVB_CHECK_ARG(r, "xvb_conformer_finalize: record '%s' is missing", n.c_str());
-    XVB_CHECK_ARG(r->rows == rows && r->cols == cols, "xvb_conformer_finalize: record '%s' is %d x %d, expected %d x %d", n.c_str(),
-                  r->rows, r->cols, rows, cols);
-    used.insert(n);
-    *out = r;
-    return XVB_OK;
+    const int shape[2] = {rows, cols};
+    return m->recs.take("xvb_conformer_finalize", n, shape, out);
   };
   // a Linear: weight and bias; the folded BatchNorm / xscale and the activation as flagged
   auto linear = [&](const std::string& n, int cout, int cin, Lin* l) -> int {
@@ -461,8 +365,8 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
     XVB_CHECK_ARG(!r->b.empty(), "xvb_conformer_finalize: record '%s' needs its bias", n.c_str());
     XVB_CHECK_ARG(r->s.empty() || (r->flags & XVB_BN), "xvb_conformer_finalize: record '%s' has scale/shift without XVB_BN", n.c_str());
     l->cin = cin; l->cout = cout; l->flags = r->flags;
-    if ((rc = m->pack(&l->w, r->w, cout, cin, 1)) || (rc = m->upload(&l->bias, r->b)) || (rc = m->upload(&l->scale, r->s)) ||
-        (rc = m->upload(&l->shift, r->t)))
+    if ((rc = m->dev.pack(&l->w, r->w, cout, cin, 1, kTaps, 1)) || (rc = m->dev.upload(&l->bias, r->b)) || (rc = m->dev.upload(&l->scale, r->s)) ||
+        (rc = m->dev.upload(&l->shift, r->t)))
       return rc;
     return XVB_OK;
   };
@@ -479,7 +383,7 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
     if (rc) return rc;
     XVB_CHECK_ARG(r->b.empty() && !(r->flags & ~XVB_BN) && (!affine || !r->s.empty()),
                   "xvb_conformer_finalize: record '%s' is not a LayerNorm", n.c_str());
-    if ((rc = m->upload(&l->g, r->s)) || (rc = m->upload(&l->b, r->t)) != XVB_OK) return rc;
+    if ((rc = m->dev.upload(&l->g, r->s)) || (rc = m->dev.upload(&l->b, r->t)) != XVB_OK) return rc;
     return XVB_OK;
   };
   int rc;
@@ -490,11 +394,11 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
   m->dk = D / c.H;
   if ((rc = need(e + "conv.0", D, 9, &r)) != XVB_OK) return rc;
   XVB_CHECK_ARG(!r->b.empty() && r->s.empty() && r->flags == 0, "xvb_conformer_finalize: record '%sconv.0' needs a bias only", e.c_str());
-  if ((rc = m->upload(&m->head_w, r->w)) || (rc = m->upload(&m->head_b, r->b)) != XVB_OK) return rc;
+  if ((rc = m->dev.upload(&m->head_w, r->w)) || (rc = m->dev.upload(&m->head_b, r->b)) != XVB_OK) return rc;
   if ((rc = need(e + "conv.2", D, 9 * D, &r)) != XVB_OK) return rc;
   XVB_CHECK_ARG(!r->b.empty() && r->s.empty() && r->flags == 0, "xvb_conformer_finalize: record '%sconv.2' needs a bias only", e.c_str());
-  if ((rc = m->pack(&m->conv2_w, r->w, D, D, 9)) || (rc = m->upload(&m->conv2_scale, std::vector<float>(D, 1.f))) ||
-      (rc = m->upload(&m->conv2_shift, r->b)))
+  if ((rc = m->dev.pack(&m->conv2_w, r->w, D, D, 9, kTaps, 9)) || (rc = m->dev.upload(&m->conv2_scale, std::vector<float>(D, 1.f))) ||
+      (rc = m->dev.upload(&m->conv2_shift, r->b)))
     return rc;
   if ((rc = linear(e + "out.0", D, m->F2 * D, &m->embed_out)) != XVB_OK) return rc;
   XVB_CHECK_ARG((m->embed_out.flags == XVB_BN) == (c.pos != 0) && (m->embed_out.flags & ~XVB_BN) == 0,
@@ -502,7 +406,7 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
                 e.c_str());
   if (c.pos) {
     const int width = c.pos == 2 ? m->dk : D;
-    if ((rc = need("pos_table", kTableRows, width, &r)) || (rc = m->upload(&m->table, r->w)) != XVB_OK) return rc;
+    if ((rc = need("pos_table", kTableRows, width, &r)) || (rc = m->dev.upload(&m->table, r->w)) != XVB_OK) return rc;
   }
   const int act_flag = c.act == XVB_ACT_SWISH ? XVB_SWISH : XVB_RELU;
   for (int i = 0; i < c.blocks; ++i) {
@@ -518,9 +422,9 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
                   "xvb_conformer_finalize: the feed-forward w_1 records of block %d must carry the configured activation", i);
     if ((rc = need(p + "conv_module.depthwise_conv", D, c.conv_kernel, &r)) != XVB_OK) return rc;
     XVB_CHECK_ARG(!r->b.empty(), "xvb_conformer_finalize: record '%sconv_module.depthwise_conv' needs its bias", p.c_str());
-    if ((rc = m->upload(&L.dw_w, r->w)) || (rc = m->upload(&L.dw_b, r->b)) != XVB_OK) return rc;
+    if ((rc = m->dev.upload(&L.dw_w, r->w)) || (rc = m->dev.upload(&L.dw_b, r->b)) != XVB_OK) return rc;
     if ((rc = norm(p + "conv_module.norm", D, true, &L.cm_norm)) != XVB_OK) return rc;
-    XVB_CHECK_ARG(((find(m, p + "conv_module.norm")->flags & XVB_BN) != 0) == (c.cm_norm == 1),
+    XVB_CHECK_ARG(((m->recs.find(p + "conv_module.norm")->flags & XVB_BN) != 0) == (c.cm_norm == 1),
                   "xvb_conformer_finalize: record '%sconv_module.norm' does not match the configured norm", p.c_str());
     if ((rc = norm(p + "norm_ff", D, false, &L.norm_ff)) || (rc = norm(p + "norm_mha", D, false, &L.norm_mha)) ||
         (rc = norm(p + "norm_ff_macaron", D, false, &L.norm_ff_macaron)) || (rc = norm(p + "norm_conv", D, false, &L.norm_conv)) ||
@@ -555,20 +459,19 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
   }
   for (const Want& w : chain) {
     const std::string a = std::string(w.name) + ".affine", b = std::string(w.name) + ".batchnorm";
-    const Rec* ra = find(m, a);
+    const Rec* ra = m->recs.find(a);
     XVB_CHECK_ARG(ra, "xvb_conformer_finalize: record '%s' is missing", a.c_str());
     Seg s;
-    if ((rc = w.whole ? linear(a, ra->rows, cin, &s.lin) : plain(a, ra->rows, cin, &s.lin)) != XVB_OK) return rc;
+    if ((rc = w.whole ? linear(a, ra->shape[0], cin, &s.lin) : plain(a, ra->shape[0], cin, &s.lin)) != XVB_OK) return rc;
     XVB_CHECK_ARG(s.lin.cout % 8 == 0, "xvb_conformer_finalize: record '%s' has %d rows, need a multiple of 8", a.c_str(), s.lin.cout);
-    s.ln = w.whole && find(m, b) != nullptr;
+    s.ln = w.whole && m->recs.find(b) != nullptr;
     if (s.ln && (rc = norm(b, s.lin.cout, false, &s.norm))) return rc;
     XVB_CHECK_ARG(!(s.ln && (s.lin.flags & XVB_BN)), "xvb_conformer_finalize: '%s' has both a LayerNorm and a folded BatchNorm", w.name);
     m->seg.push_back(s);
     cin = s.lin.cout;
   }
   m->E = m->seg.back().lin.cout;
-  for (const std::string& n : m->order)
-    XVB_CHECK_ARG(used.count(n), "xvb_conformer_finalize: record '%s' is not part of this configuration", n.c_str());
+  if ((rc = m->recs.check_all_used("xvb_conformer_finalize"))) return rc;
   h->finalized = true;
   return XVB_OK;
 }
@@ -585,86 +488,34 @@ extern "C" int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int
   sub_shape(h->m->cfg, T, &T1, &F1, &T2, &F2);
   XVB_CHECK_ARG(T2 < kTableRows, "xvb_conformer_extract: a chunk of %d subsampled frames exceeds the positional tables' %d", T2,
                 kTableRows);
-  const long long per_utt = (long long)T * h->m->cfg.feat_dim;
-  int g = (int)(kFrameBudget / T);
-  if (g < 1) g = 1;
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->E;
   int n = 0;
-  for (int i = 0; i < B; i += g) {
-    const int b = B - i < g ? B - i : g;
-    int rc = extract_group(h, feats + (size_t)i * per_utt, b, T, emb + (size_t)i * h->m->E, &n, stream);
-    if (rc) return rc;
-  }
+  int rc = for_groups(B, T, kFrameBudget,
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, &n, stream); });
+  if (rc) return rc;
   h->last_launches = n;
   return XVB_OK;
 }
 
-// ---- "XVBC0001" model files: the configuration, then the records and tables as handed over ----------------------
+// ---- "XVBC0001" model files: the configuration, then the records and tables as handed over (save_records) ---------
 extern "C" int xvb_conformer_save(const xvb_conformer_t* h, const char* path) {
   XVB_CHECK_ARG(h && h->finalized && path, "xvb_conformer_save: model not finalized");
-  const Model* m = h->m;
-  FILE* f = fopen(path, "wb");
-  XVB_CHECK_ARG(f, "xvb_conformer_save: cannot open '%s'", path);
-  int32_t cfg[kCfgInts];
-  to_ints(m->cfg, cfg);
-  const int32_t nrec = (int32_t)m->order.size();
-  bool ok = fwrite("XVBC0001", 1, 8, f) == 8 && fwrite(cfg, 4, kCfgInts, f) == kCfgInts && fwrite(&nrec, 4, 1, f) == 1;
-  for (const std::string& n : m->order) {
-    const Rec& r = m->recs.at(n);
-    const int32_t nl = (int32_t)n.size();
-    const int32_t rec[6] = {r.rows, r.cols, r.flags, (int32_t)!r.w.empty(), (int32_t)!r.b.empty(), (int32_t)!r.s.empty()};
-    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(rec, 4, 6, f) == 6 &&
-         fwrite(r.w.data(), 4, r.w.size(), f) == r.w.size() && fwrite(r.b.data(), 4, r.b.size(), f) == r.b.size() &&
-         fwrite(r.s.data(), 4, r.s.size(), f) == r.s.size() && fwrite(r.t.data(), 4, r.t.size(), f) == r.t.size();
-  }
-  ok = fclose(f) == 0 && ok;
-  XVB_CHECK_ARG(ok, "xvb_conformer_save: write to '%s' failed", path);
-  return XVB_OK;
+  return save_records("xvb_conformer_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
 extern "C" int xvb_conformer_load(xvb_conformer_t** out, const char* path) {
-  XVB_CHECK_ARG(out && path, "xvb_conformer_load: null argument");
-  FILE* f = fopen(path, "rb");
-  XVB_CHECK_ARG(f, "xvb_conformer_load: cannot open '%s'", path);
-  auto rd = [&](void* p, size_t n) { return fread(p, 1, n, f) == n; };
-  char magic[8];
-  int32_t cfg[kCfgInts], nrec = 0;
-  xvb_conformer_t* h = nullptr;
-  int rc = XVB_EINVAL;
-  do {
-    if (!rd(magic, 8) || memcmp(magic, "XVBC0001", 8) != 0 || !rd(cfg, sizeof cfg) || !rd(&nrec, 4) || nrec < 1 || nrec > 65536) {
-      set_error("xvb_conformer_load: '%s' is not an XVBC0001 file", path);
-      break;
-    }
-    const xvb_conformer_config_t c = from_ints(cfg);
-    if ((rc = xvb_conformer_create(&h, &c))) break;
-    std::vector<float> w, b, s, t;
-    for (int i = 0; i < nrec && rc == XVB_OK; ++i) {
-      int32_t nl = 0, rec[6];
-      char name[128];
-      bool ok = rd(&nl, 4) && nl > 0 && nl < 127 && rd(name, (size_t)nl) && rd(rec, sizeof rec) && rec[0] > 0 && rec[0] <= 65536 &&
-                rec[1] >= 0 && rec[1] <= (1 << 20) && (int64_t)rec[0] * rec[1] <= (int64_t)1 << 28 && rec[3] == (rec[1] > 0);
-      if (ok) {
-        name[nl] = 0;
-        w.resize(rec[3] ? (size_t)rec[0] * rec[1] : 0);
-        ok = rd(w.data(), w.size() * 4);
-        if (ok && rec[4]) { b.resize(rec[0]); ok = rd(b.data(), b.size() * 4); }
-        if (ok && rec[5]) { s.resize(rec[0]); t.resize(rec[0]); ok = rd(s.data(), s.size() * 4) && rd(t.data(), t.size() * 4); }
-      }
-      if (!ok) { set_error("xvb_conformer_load: '%s' is truncated or corrupt at record %d", path, i); rc = XVB_EINVAL; break; }
-      rc = xvb_conformer_set_layer(h, name, rec[0], rec[1], rec[3] ? w.data() : nullptr, rec[4] ? b.data() : nullptr,
-                                   rec[5] ? s.data() : nullptr, rec[5] ? t.data() : nullptr, rec[2]);
-    }
-    if (rc == XVB_OK) rc = xvb_conformer_finalize(h);
-  } while (0);
-  fclose(f);
-  if (rc != XVB_OK) { if (h) xvb_conformer_destroy(h); return rc; }
-  *out = h;
-  return XVB_OK;
+  return load_records(
+      "xvb_conformer_load", path, kFile, (void**)out,
+      [](void** h, const void* cfg) { return xvb_conformer_create((xvb_conformer_t**)h, (const xvb_conformer_config_t*)cfg); },
+      [](void* h, const char* name, const int* shape, const float* w, const float* b, const float* s, const float* t, int flags) {
+        return xvb_conformer_set_layer((xvb_conformer_t*)h, name, shape[0], shape[1], w, b, s, t, flags);
+      },
+      [](void* h) { return xvb_conformer_finalize((xvb_conformer_t*)h); },
+      [](void* h) { xvb_conformer_destroy((xvb_conformer_t*)h); });
 }
 
 extern "C" void xvb_conformer_destroy(xvb_conformer_t* h) {
   if (!h) return;
-  h->free_ws();
   delete h->m;
   delete h;
 }

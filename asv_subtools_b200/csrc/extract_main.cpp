@@ -63,12 +63,52 @@ struct Utt {
 #define CK(call, what) do { if ((call) != XVB_OK) die(what); } while (0)
 #define CU(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) { fprintf(stderr, "ERROR: xvb-extract: %s: %s\n", #call, cudaGetErrorString(_e)); exit(1); } } while (0)
 
+// One model family: its magic(s), its C entry points over an opaque handle, its default --max-chunk and chunk rule.
+struct Family {
+  const char* magic[2];
+  const char* loading;     // the load error's context
+  const char* extract_fn;
+  int (*load)(void** h, const char* path);
+  int (*feat_dim)(const void* h, const char* path);
+  int (*embed_dim)(const void* h);
+  int (*extract)(void* h, const float* feats, int B, int T, float* emb);
+  void (*destroy)(void* h);
+  int max_chunk;
+  bool campp_chunks;       // egrecho's split_chunks(even=False) through xvb_campp_chunk_sizes
+};
+
+// the entry points of a family whose C API is xvb_<p>_load / _feat_dim / _embed_dim / _extract / _destroy on xvb_<p>_t
+#define HANDLE_FAMILY(p)                                                                                              \
+  [](void** h, const char* path) { return xvb_##p##_load((xvb_##p##_t**)h, path); },                                  \
+  [](const void* h, const char*) { return xvb_##p##_feat_dim((const xvb_##p##_t*)h); },                               \
+  [](const void* h) { return xvb_##p##_embed_dim((const xvb_##p##_t*)h); },                                           \
+  [](void* h, const float* x, int B, int T, float* e) { return xvb_##p##_extract((xvb_##p##_t*)h, x, B, T, e, nullptr); }, \
+  [](void* h) { xvb_##p##_destroy((xvb_##p##_t*)h); }
+
+const Family kFamilies[] = {
+    {{"XVBE0001", "XVBE0002"}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false},
+    {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false},
+    {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false},
+    {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true},
+    // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
+    {{nullptr, nullptr}, "loading the model", "xvb_extractor_extract",
+     [](void** h, const char* path) { return xvb_extractor_load((xvb_extractor_t**)h, path); },
+     [](const void*, const char* path) { return xvb_extractor_feat_dim(path); },
+     [](const void* h) { return xvb_extractor_embed_dim((const xvb_extractor_t*)h); },
+     [](void* h, const float* x, int B, int T, float* e) { return xvb_extractor_extract((xvb_extractor_t*)h, x, B, T, e, nullptr); },
+     [](void* h) { xvb_extractor_destroy((xvb_extractor_t*)h); }, 10000, false},
+};
+
+const Family& family_of(const char (&magic)[8]) {
+  for (const Family& f : kFamilies)
+    for (const char* m : f.magic)
+      if (m && memcmp(magic, m, 8) == 0) return f;
+  return kFamilies[sizeof kFamilies / sizeof kFamilies[0] - 1];
+}
+
 struct Runner {
-  xvb_extractor_t* ex = nullptr;   // TDNN x-vector family (XVBM0001) ...
-  xvb_ecapa_t* ec = nullptr;       // ... or ECAPA-TDNN (XVBE0001 / XVBE0002) ...
-  xvb_resnet_t* rn = nullptr;      // ... or 2-D ResNet x-vector (XVBR0001) ...
-  xvb_conformer_t* cf = nullptr;   // ... or Conformer x-vector (XVBC0001) ...
-  xvb_campp_t* cp = nullptr;       // ... or CAM++ x-vector (XVBP0001)
+  const Family* fam = nullptr;
+  void* model = nullptr;
   xvb_ark_writer_t* out = nullptr;
   int F = 0, D = 0, batch = 256, cmn = 0, cmn_window = 300;
   float *d_feats = nullptr, *d_tmp = nullptr, *d_emb = nullptr, *h_feats = nullptr, *h_emb = nullptr;
@@ -98,11 +138,7 @@ struct Runner {
     reserve((size_t)B * T);
     for (int i = 0; i < B; ++i) memcpy(h_feats + (size_t)i * T * F, items[i].feats.data(), (size_t)T * F * sizeof(float));
     CU(cudaMemcpy(d_feats, h_feats, (size_t)B * T * F * sizeof(float), cudaMemcpyHostToDevice));
-    if (ex) CK(xvb_extractor_extract(ex, d_feats, B, T, d_emb, nullptr), "xvb_extractor_extract");
-    else if (ec) CK(xvb_ecapa_extract(ec, d_feats, B, T, d_emb, nullptr), "xvb_ecapa_extract");
-    else if (rn) CK(xvb_resnet_extract(rn, d_feats, B, T, d_emb, nullptr), "xvb_resnet_extract");
-    else if (cf) CK(xvb_conformer_extract(cf, d_feats, B, T, d_emb, nullptr), "xvb_conformer_extract");
-    else CK(xvb_campp_extract(cp, d_feats, B, T, d_emb, nullptr), "xvb_campp_extract");
+    CK(fam->extract(model, d_feats, B, T, d_emb), fam->extract_fn);
     CU(cudaMemcpy(h_emb, d_emb, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToHost));
     for (int i = 0; i < B; ++i) {
       Utt& u = utts[items[i].utt];
@@ -225,29 +261,11 @@ int main(int argc, char** argv) {
     FILE* mf = fopen(pos[0], "rb");
     if (!mf || fread(magic, 1, 8, mf) != 8) { fprintf(stderr, "ERROR: xvb-extract: cannot read model file '%s'\n", pos[0]); return 1; }
     fclose(mf);
-    if (memcmp(magic, "XVBE0001", 8) == 0 || memcmp(magic, "XVBE0002", 8) == 0) {
-      CK(xvb_ecapa_load(&r.ec, pos[0]), "loading the ECAPA model");
-      r.F = xvb_ecapa_feat_dim(r.ec);
-      r.D = xvb_ecapa_embed_dim(r.ec);
-    } else if (memcmp(magic, "XVBR0001", 8) == 0) {
-      CK(xvb_resnet_load(&r.rn, pos[0]), "loading the ResNet model");
-      r.F = xvb_resnet_feat_dim(r.rn);
-      r.D = xvb_resnet_embed_dim(r.rn);
-    } else if (memcmp(magic, "XVBC0001", 8) == 0) {
-      CK(xvb_conformer_load(&r.cf, pos[0]), "loading the Conformer model");
-      r.F = xvb_conformer_feat_dim(r.cf);
-      r.D = xvb_conformer_embed_dim(r.cf);
-      if (!max_chunk_set) max_chunk = 300;
-    } else if (memcmp(magic, "XVBP0001", 8) == 0) {
-      CK(xvb_campp_load(&r.cp, pos[0]), "loading the CAM++ model");
-      r.F = xvb_campp_feat_dim(r.cp);
-      r.D = xvb_campp_embed_dim(r.cp);
-      if (!max_chunk_set) max_chunk = 4000;
-    } else {
-      CK(xvb_extractor_load(&r.ex, pos[0]), "loading the model");
-      r.F = xvb_extractor_feat_dim(pos[0]);
-      r.D = xvb_extractor_embed_dim(r.ex);
-    }
+    r.fam = &family_of(magic);
+    CK(r.fam->load(&r.model, pos[0]), r.fam->loading);
+    r.F = r.fam->feat_dim(r.model, pos[0]);
+    r.D = r.fam->embed_dim(r.model);
+    if (!max_chunk_set) max_chunk = r.fam->max_chunk;
   }
   xvb_ark_reader_t* in = nullptr;
   FILE* wav_scp = nullptr;
@@ -330,7 +348,7 @@ int main(int argc, char** argv) {
     u.key = key;
     u.frames = rows;
     std::vector<int> lens;
-    if (r.cp) {   // egrecho's split_chunks(even=False)
+    if (r.fam->campp_chunks) {   // egrecho's split_chunks(even=False)
       lens.resize((size_t)rows / max_chunk + 1);
       const int n = xvb_campp_chunk_sizes(rows, max_chunk, lens.data(), (int)lens.size());
       if (n < 1) die("planning the CAM++ chunks");
@@ -369,11 +387,7 @@ int main(int argc, char** argv) {
   if (wav_scp) fclose(wav_scp);
   if (fb) xvb_fbank_destroy(fb);
   CK(xvb_ark_writer_close(r.out), "closing the vector wspecifier");
-  if (r.ex) xvb_extractor_destroy(r.ex);
-  if (r.ec) xvb_ecapa_destroy(r.ec);
-  if (r.rn) xvb_resnet_destroy(r.rn);
-  if (r.cf) xvb_conformer_destroy(r.cf);
-  if (r.cp) xvb_campp_destroy(r.cp);
+  r.fam->destroy(r.model);
   fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
   return 0;
 }

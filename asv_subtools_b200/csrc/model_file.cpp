@@ -7,6 +7,9 @@
 //   frame layer  : i32 Cout, Cin, ntaps, tot_context, flags, has_bias, has_bn | i32 ctx[ntaps]
 //                  | f32 w[Cout*Cin*tot_context] | f32 bias[Cout]? | f32 scale[Cout], shift[Cout]?
 //   segment layer: same header with ntaps = tot_context = 1 and ctx = {0}
+//
+// The named-record files of the native ResNet, Conformer and CAM++ extractors (save_records / load_records below) and
+// the record store behind them (records.h).
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
@@ -14,6 +17,7 @@
 #include <vector>
 
 #include "../../include/xvb200.h"
+#include "records.h"
 
 namespace xvb {
 void set_error(const char* fmt, ...);
@@ -22,7 +26,159 @@ using xvb::set_error;
 
 namespace {
 bool rd(FILE* f, void* p, size_t n) { return fread(p, 1, n, f) == n; }
+
+#define FAIL_IF(cond, ...) do { if (cond) { set_error(__VA_ARGS__); return XVB_EINVAL; } } while (0)
+
+// weight elements of a record shape; a ksize outside [0, 4096] counts as too large
+int64_t weight_elems(const int* shape, int n) {
+  const int64_t rc = (int64_t)shape[0] * shape[1];
+  if (n == 2) return rc;
+  return shape[2] < 0 || shape[2] > 4096 ? INT64_MAX : rc * shape[2] * shape[2];
 }
+
+// the bounds every record shape meets, in set_layer and in a model file
+bool shape_ok(const int* shape, int n) {
+  return shape[0] > 0 && shape[0] <= 65536 && shape[1] >= 0 && shape[1] <= (1 << 20) &&
+         weight_elems(shape, n) <= (int64_t)1 << 28;
+}
+
+const char* shape_str(const int* shape, int n, char (&buf)[48]) {
+  if (n == 2) snprintf(buf, sizeof buf, "%d x %d", shape[0], shape[1]);
+  else snprintf(buf, sizeof buf, "%d x %d x k%d", shape[0], shape[1], shape[2]);
+  return buf;
+}
+}  // namespace
+
+namespace xvb {
+
+int RecordStore::check(const char* fn, const char* name, const int* shape, const float* w, const float* s,
+                       const float* t) const {
+  char buf[48];
+  FAIL_IF(!shape_ok(shape, n), "%s(%s): bad shape %s", fn, name, shape_str(shape, n, buf));
+  FAIL_IF((shape[n - 1] > 0) != (w != nullptr) || (w && shape[1] == 0),
+          n == 2 ? "%s(%s): a weight needs cols > 0, a norm record cols 0"
+                 : "%s(%s): a weight needs ksize 1 or 3 and Cin > 0, a BatchNorm record ksize 0 and no weight",
+          fn, name);
+  FAIL_IF((s == nullptr) != (t == nullptr), "%s(%s): scale and shift go together", fn, name);
+  return XVB_OK;
+}
+
+int RecordStore::add(const char* fn, const char* name, const int* shape, const float* w, const float* b,
+                     const float* s, const float* t, int flags) {
+  FAIL_IF(recs.count(name), "%s: record '%s' set twice", fn, name);
+  Rec r;
+  for (int i = 0; i < n; ++i) r.shape[i] = shape[i];
+  r.flags = flags;
+  const size_t rows = (size_t)shape[0];
+  if (w) r.w.assign(w, w + (size_t)weight_elems(shape, n));
+  if (b) r.b.assign(b, b + rows);
+  if (s) { r.s.assign(s, s + rows); r.t.assign(t, t + rows); }
+  recs[name] = std::move(r);
+  order.push_back(name);
+  return XVB_OK;
+}
+
+const Rec* RecordStore::find(const std::string& name) const {
+  auto it = recs.find(name);
+  return it == recs.end() ? nullptr : &it->second;
+}
+
+int RecordStore::take(const char* fn, const std::string& name, const int* shape, const Rec** out) {
+  const Rec* r = find(name);
+  FAIL_IF(!r, "%s: record '%s' is missing", fn, name.c_str());
+  char have[48], want[48];
+  FAIL_IF(memcmp(r->shape, shape, n * sizeof(int)) != 0, "%s: record '%s' is %s, expected %s", fn, name.c_str(),
+          shape_str(r->shape, n, have), shape_str(shape, n, want));
+  used.insert(name);
+  *out = r;
+  return XVB_OK;
+}
+
+int RecordStore::check_all_used(const char* fn) const {
+  for (const std::string& name : order)
+    FAIL_IF(!used.count(name), "%s: record '%s' is not part of this configuration", fn, name.c_str());
+  return XVB_OK;
+}
+
+// The named-record model files ("XVBR0001" ResNet, "XVBC0001" Conformer, "XVBP0001" CAM++), little-endian:
+//
+//   magic[8] | configuration block (RecordFormat::cfg_bytes raw bytes) | i32 nrec
+//   per record, in set_layer order:
+//     i32 name_len | name (no NUL) | i32 shape[nshape] | i32 flags | i32 has_w | i32 has_b | i32 has_s
+//     | f32 w[weight elements]? | f32 b[rows]? | f32 s[rows], t[rows]?
+//
+// Loading refuses a wrong magic, nrec outside [1, max_records], a name length outside (0, 127), a shape outside the
+// set_layer bounds (rows in (0, 65536], the second int in [0, 2^20], at most 2^28 weight elements), has_w not equal to
+// (last shape int > 0) and a short read; set_layer and finalize then check the records against the configuration.
+int save_records(const char* fn, const char* path, const RecordFormat& fmt, const void* cfg, const RecordStore& store) {
+  FILE* f = fopen(path, "wb");
+  FAIL_IF(!f, "%s: cannot open '%s'", fn, path);
+  const int32_t nrec = (int32_t)store.order.size();
+  bool ok = fwrite(fmt.magic, 1, 8, f) == 8 && fwrite(cfg, 1, fmt.cfg_bytes, f) == fmt.cfg_bytes && fwrite(&nrec, 4, 1, f) == 1;
+  for (const std::string& n : store.order) {
+    const Rec& r = store.recs.at(n);
+    const int32_t nl = (int32_t)n.size();
+    int32_t hd[7];
+    int k = 0;
+    for (int i = 0; i < fmt.nshape; ++i) hd[k++] = r.shape[i];
+    hd[k++] = r.flags; hd[k++] = !r.w.empty(); hd[k++] = !r.b.empty(); hd[k++] = !r.s.empty();
+    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(hd, 4, k, f) == (size_t)k &&
+         fwrite(r.w.data(), 4, r.w.size(), f) == r.w.size() && fwrite(r.b.data(), 4, r.b.size(), f) == r.b.size() &&
+         fwrite(r.s.data(), 4, r.s.size(), f) == r.s.size() && fwrite(r.t.data(), 4, r.t.size(), f) == r.t.size();
+  }
+  ok = fclose(f) == 0 && ok;
+  FAIL_IF(!ok, "%s: write to '%s' failed", fn, path);
+  return XVB_OK;
+}
+
+int load_records(const char* fn, const char* path, const RecordFormat& fmt, void** out,
+                 int (*create)(void** h, const void* cfg),
+                 int (*set_layer)(void* h, const char* name, const int* shape, const float* w, const float* b,
+                                  const float* s, const float* t, int flags),
+                 int (*finalize)(void* h), void (*destroy)(void* h)) {
+  FAIL_IF(!out || !path, "%s: null argument", fn);
+  FILE* f = fopen(path, "rb");
+  FAIL_IF(!f, "%s: cannot open '%s'", fn, path);
+  char magic[8];
+  std::vector<char> cfg(fmt.cfg_bytes);
+  int32_t nrec = 0;
+  void* h = nullptr;
+  int rc = XVB_EINVAL;
+  do {
+    if (!rd(f, magic, 8) || memcmp(magic, fmt.magic, 8) != 0 || !rd(f, cfg.data(), cfg.size()) || !rd(f, &nrec, 4) ||
+        nrec < 1 || nrec > fmt.max_records) {
+      set_error("%s: '%s' is not an %.8s file", fn, path, fmt.magic);
+      break;
+    }
+    if ((rc = create(&h, cfg.data()))) break;
+    const int ns = fmt.nshape;
+    std::vector<float> w, b, s, t;
+    for (int i = 0; i < nrec && rc == XVB_OK; ++i) {
+      int32_t nl = 0, hd[7] = {0};   // shape[ns], flags, has_w, has_b, has_s
+      char name[128];
+      bool ok = rd(f, &nl, 4) && nl > 0 && nl < 127 && rd(f, name, (size_t)nl) && rd(f, hd, 4 * (size_t)(ns + 4)) &&
+                shape_ok(hd, ns) && hd[ns + 1] == (hd[ns - 1] > 0);
+      const int32_t flags = hd[ns], has_w = hd[ns + 1], has_b = hd[ns + 2], has_s = hd[ns + 3];
+      if (ok) {
+        name[nl] = 0;
+        w.resize(has_w ? (size_t)weight_elems(hd, ns) : 0);
+        ok = rd(f, w.data(), w.size() * 4);
+        if (ok && has_b) { b.resize(hd[0]); ok = rd(f, b.data(), b.size() * 4); }
+        if (ok && has_s) { s.resize(hd[0]); t.resize(hd[0]); ok = rd(f, s.data(), s.size() * 4) && rd(f, t.data(), t.size() * 4); }
+      }
+      if (!ok) { set_error("%s: '%s' is truncated or corrupt at record %d", fn, path, i); rc = XVB_EINVAL; break; }
+      rc = set_layer(h, name, hd, has_w ? w.data() : nullptr, has_b ? b.data() : nullptr, has_s ? s.data() : nullptr,
+                     has_s ? t.data() : nullptr, flags);
+    }
+    if (rc == XVB_OK) rc = finalize(h);
+  } while (0);
+  fclose(f);
+  if (rc != XVB_OK) { if (h) destroy(h); return rc; }
+  *out = h;
+  return XVB_OK;
+}
+
+}  // namespace xvb
 
 extern "C" int xvb_extractor_load(xvb_extractor_t** out, const char* path) {
   if (!out || !path) { set_error("xvb_extractor_load: null argument"); return XVB_EINVAL; }

@@ -1,0 +1,63 @@
+// Named-record model store and model-file codec of the ResNet, Conformer and CAM++ native extractors (host code; the
+// device-weight arena and the workspace are in records.cuh).
+//
+// A family's set_layer hands over one record per state_dict module path: a small fixed shape, flags and up to four
+// fp32 arrays.  The store keeps host copies in insertion order, so that save() writes the records exactly as they were
+// handed over, and finalize() takes each record its configuration needs and then refuses any record it did not take.
+#pragma once
+#include <stddef.h>
+#include <stdint.h>
+
+#include <map>
+#include <set>
+#include <string>
+#include <vector>
+
+namespace xvb {
+
+struct Rec {   // one named record exactly as handed over
+  int shape[3] = {0, 0, 0};        // rows, cols (CAM++, Conformer) or Cout, Cin, ksize (ResNet)
+  int flags = 0;
+  std::vector<float> w, b, s, t;   // weight, bias, scale, shift; empty when not handed over
+};
+
+// One family's records and model file (layout at save_records in model_file.cpp).
+struct RecordFormat {
+  const char* magic;   // 8 bytes
+  size_t cfg_bytes;    // the configuration block
+  int nshape;          // 2: rows x cols, weight rows * cols; 3: Cout x Cin x ksize, weight Cout * Cin * ksize^2
+  int max_records;
+};
+
+struct RecordStore {
+  explicit RecordStore(int nshape) : n(nshape) {}
+  const int n;                        // shape ints per record
+  std::map<std::string, Rec> recs;
+  std::vector<std::string> order;     // insertion order, for save
+  std::set<std::string> used;         // taken by finalize
+
+  // set_layer's shared checks (fn: the caller's name): shape bounds, a weight exactly when the last shape int is > 0,
+  // scale and shift together.  Family checks come between check and add.
+  int check(const char* fn, const char* name, const int* shape, const float* w, const float* s, const float* t) const;
+  // refuses a name set twice, then keeps host copies of the arrays
+  int add(const char* fn, const char* name, const int* shape, const float* w, const float* b, const float* s,
+          const float* t, int flags);
+  const Rec* find(const std::string& name) const;
+  // the record `name` with exactly this shape, marked used (fn: the caller's name)
+  int take(const char* fn, const std::string& name, const int* shape, const Rec** out);
+  // refuses the first record that no take marked used
+  int check_all_used(const char* fn) const;
+};
+
+// Writes magic, the configuration block and the store's records in insertion order (fn: the caller's name).
+int save_records(const char* fn, const char* path, const RecordFormat& fmt, const void* cfg, const RecordStore& store);
+
+// Reads a file written by save_records through the family's entry points: create from the configuration block,
+// set_layer per record, finalize; destroys the handle on any failure.  *out is written on success only.
+int load_records(const char* fn, const char* path, const RecordFormat& fmt, void** out,
+                 int (*create)(void** h, const void* cfg),
+                 int (*set_layer)(void* h, const char* name, const int* shape, const float* w, const float* b,
+                                  const float* s, const float* t, int flags),
+                 int (*finalize)(void* h), void (*destroy)(void* h));
+
+}  // namespace xvb

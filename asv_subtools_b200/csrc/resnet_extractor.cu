@@ -20,12 +20,10 @@
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
-#include <set>
 #include <string>
 #include <vector>
 
-#include "common.cuh"
+#include "records.cuh"
 
 namespace {
 
@@ -34,13 +32,7 @@ using namespace xvb;
 // One B*T*F position budget per extract call: larger calls run as consecutive groups of utterances (see xvb200.h).
 constexpr long long kPositionBudget = 256LL * 200 * 80;
 constexpr int kSeMaxK = 9;   // k = 1, 2, ..., 256 for the k-grouped SE mean
-
-struct Rec {   // one named record exactly as handed over (host copies, for xvb_resnet_save)
-  int Cout = 0, Cin = 0, ksize = 0, flags = 0;
-  std::vector<float> w, b, s, t;
-};
-
-struct Conv { uint16_t* hi = nullptr; uint16_t* lo = nullptr; };
+const RecordFormat kFile = {"XVBR0001", 10 * sizeof(int32_t) + sizeof(float), 3, 4096};
 struct Bn { float* s = nullptr; float* t = nullptr; };
 struct Se {
   int C = 0, Hp = 0, kmax = 1;           // hidden width padded to a multiple of 4; k = 1 .. kmax (powers of two)
@@ -49,13 +41,13 @@ struct Se {
 };
 struct Block {
   int stride = 1, cin = 0, cout = 0;
-  Conv conv1, conv2, ds;
+  Planes conv1, conv2, ds;
   Bn bn1, bn2, dsbn;
   bool has_ds = false, has_se = false;
   Se se;
 };
 struct Seg {   // one segment layer on the wgmma layer kernel (T = 1), output rows padded to a multiple of 8
-  Conv w;
+  Planes w;
   float* bias = nullptr; float* scale = nullptr; float* shift = nullptr;
   int Cin = 0, Cout = 0, Cout_real = 0, flags = 0;
 };
@@ -63,49 +55,14 @@ struct Seg {   // one segment layer on the wgmma layer kernel (T = 1), output ro
 struct Model {   // shared by a handle and its second shard lane
   int feat_dim = 0, layers[4] = {0}, planes[4] = {0}, pre = 0;
   float eps = 0.f;
-  std::map<std::string, Rec> recs;
-  std::vector<std::string> order;   // insertion order, for save()
+  RecordStore recs{kFile.nshape};
   float* head_w = nullptr;
   Bn head_bn;
   std::vector<Block> blocks;
   std::vector<Seg> seg;
   int F4 = 0, C4 = 0, E = 0, Cmax = 0, Hmax = 0, seg_mid = 0;
-  std::vector<void*> dev;           // every device allocation of the weights
-
-  template <typename T>
-  int alloc(T** p, size_t n) {
-    XVB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-    dev.push_back(*p);
-    return XVB_OK;
-  }
-  int upload(float** d, const std::vector<float>& v) {
-    if (v.empty()) { *d = nullptr; return XVB_OK; }
-    int rc = alloc(d, v.size());
-    if (rc) return rc;
-    XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
-    return XVB_OK;
-  }
-  // (Cout, Cin, taps) fp32 host -> packed planes, taps 0..ntaps-1 (what ops.pack_tdnn_weight does)
-  int pack(Conv* c, const std::vector<float>& w, int Cout, int Cin, int ntaps) {
-    float* w_dev = nullptr;
-    XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
-    cudaError_t e = cudaMemcpy(w_dev, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice);
-    int ctx[XVB_MAX_TAPS];
-    for (int i = 0; i < ntaps; ++i) ctx[i] = i;
-    const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, ntaps);
-    int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
-    if (!rc) rc = alloc(&c->hi, pn);
-    if (!rc) rc = alloc(&c->lo, pn);
-    if (!rc) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, ntaps, 0, ctx, ntaps, c->hi, c->lo, nullptr);
-    if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = XVB_ECUDA;
-    if (rc == XVB_ECUDA && e != cudaSuccess) set_error("xvb_resnet_finalize: weight upload failed: %s", cudaGetErrorString(e));
-    cudaFree(w_dev);
-    return rc;
-  }
-  ~Model() { for (void* p : dev) cudaFree(p); }
+  Weights dev{"xvb_resnet_finalize"};
 };
-
-struct Planes { uint16_t* hi = nullptr; uint16_t* lo = nullptr; };
 
 }  // namespace
 
@@ -195,7 +152,7 @@ int reserve(xvb_resnet* h, int B, int T) {
   return XVB_OK;
 }
 
-int conv(const Planes& x, const Conv& w, int B, int T, int F, int Cin, int Cout, int k, int stride, const Bn& bn,
+int conv(const Planes& x, const Planes& w, int B, int T, int F, int Cin, int Cout, int k, int stride, const Bn& bn,
          const Planes* res, int relu, const Planes* y, float* y_f32, const Bn& bn2, const Planes* y2, void* stream) {
   xvb_conv2d_args_t a{};
   a.x_hi = x.hi; a.x_lo = x.lo;
@@ -308,11 +265,6 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
   return XVB_OK;
 }
 
-const Rec* find(const Model* m, const std::string& n) {
-  auto it = m->recs.find(n);
-  return it == m->recs.end() ? nullptr : &it->second;
-}
-
 }  // namespace
 
 extern "C" int xvb_resnet_create(xvb_resnet_t** out, int feat_dim, const int* layers, const int* planes, int pre_activation,
@@ -339,55 +291,41 @@ extern "C" int xvb_resnet_create(xvb_resnet_t** out, int feat_dim, const int* la
 extern "C" int xvb_resnet_set_layer(xvb_resnet_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
                                     const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
   XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127, "xvb_resnet_set_layer: bad arguments or finalized model");
-  XVB_CHECK_ARG(Cout > 0 && Cout <= 65536 && Cin >= 0 && Cin <= (1 << 20) && (ksize == 0 || ksize == 1 || ksize == 3),
-                "xvb_resnet_set_layer(%s): bad shape %d x %d x k%d", name, Cout, Cin, ksize);
-  XVB_CHECK_ARG((ksize > 0) == (w_host != nullptr) && (ksize == 0 || Cin > 0),
-                "xvb_resnet_set_layer(%s): a weight needs ksize 1 or 3 and Cin > 0, a BatchNorm record ksize 0 and no weight", name);
-  XVB_CHECK_ARG((scale_host == nullptr) == (shift_host == nullptr), "xvb_resnet_set_layer(%s): scale and shift go together", name);
+  XVB_CHECK_ARG(ksize == 0 || ksize == 1 || ksize == 3, "xvb_resnet_set_layer(%s): bad shape %d x %d x k%d", name, Cout, Cin, ksize);
+  const char* fn = "xvb_resnet_set_layer";
+  const int shape[3] = {Cout, Cin, ksize};
+  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  if (rc) return rc;
   XVB_CHECK_ARG(!(flags & XVB_BN) || scale_host, "xvb_resnet_set_layer(%s): XVB_BN without scale/shift", name);
-  XVB_CHECK_ARG(h->m->recs.find(name) == h->m->recs.end(), "xvb_resnet_set_layer: record '%s' set twice", name);
-  Rec r;
-  r.Cout = Cout; r.Cin = Cin; r.ksize = ksize; r.flags = flags;
-  if (w_host) r.w.assign(w_host, w_host + (size_t)Cout * Cin * ksize * ksize);
-  if (bias_host) r.b.assign(bias_host, bias_host + Cout);
-  if (scale_host) { r.s.assign(scale_host, scale_host + Cout); r.t.assign(shift_host, shift_host + Cout); }
-  h->m->recs[name] = std::move(r);
-  h->m->order.push_back(name);
-  return XVB_OK;
+  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
 extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
   XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_resnet_finalize: null or finalized model");
   Model* m = h->m;
-  std::set<std::string> used;
   // a record the configuration needs: present, with the expected shape
   auto need = [&](const std::string& n, int cout, int cin, int k, const Rec** out) -> int {
-    const Rec* r = find(m, n);
-    XVB_CHECK_ARG(r, "xvb_resnet_finalize: record '%s' is missing", n.c_str());
-    XVB_CHECK_ARG(r->Cout == cout && r->Cin == cin && r->ksize == k, "xvb_resnet_finalize: record '%s' is %d x %d x k%d, expected %d x %d x k%d",
-                  n.c_str(), r->Cout, r->Cin, r->ksize, cout, cin, k);
-    used.insert(n);
-    *out = r;
-    return XVB_OK;
+    const int shape[3] = {cout, cin, k};
+    return m->recs.take("xvb_resnet_finalize", n, shape, out);
   };
   auto bn = [&](const std::string& n, int c, Bn* out) -> int {
     const Rec* r;
     int rc = need(n, c, 0, 0, &r);
     if (rc) return rc;
     XVB_CHECK_ARG(!r->s.empty(), "xvb_resnet_finalize: BatchNorm record '%s' has no scale/shift", n.c_str());
-    if ((rc = m->upload(&out->s, r->s)) || (rc = m->upload(&out->t, r->t))) return rc;
+    if ((rc = m->dev.upload(&out->s, r->s)) || (rc = m->dev.upload(&out->t, r->t))) return rc;
     return XVB_OK;
   };
-  auto conv_rec = [&](const std::string& n, int cout, int cin, int k, Conv* out) -> int {
+  auto conv_rec = [&](const std::string& n, int cout, int cin, int k, Planes* out) -> int {
     const Rec* r;
     int rc = need(n, cout, cin, k, &r);
-    return rc ? rc : m->pack(out, r->w, cout, cin, k * k);
+    return rc ? rc : m->dev.pack(out, r->w, cout, cin, k * k, kTaps, k * k);
   };
   int rc;
   const Rec* r;
-  if ((rc = need("resnet.conv1", m->planes[0], 1, 3, &r)) || (rc = m->upload(&m->head_w, r->w)) || (rc = bn("resnet.bn1", m->planes[0], &m->head_bn)))
+  if ((rc = need("resnet.conv1", m->planes[0], 1, 3, &r)) || (rc = m->dev.upload(&m->head_w, r->w)) || (rc = bn("resnet.bn1", m->planes[0], &m->head_bn)))
     return rc;
-  const bool use_se = find(m, "resnet.layer1.0.se.fc_1") != nullptr;
+  const bool use_se = m->recs.find("resnet.layer1.0.se.fc_1") != nullptr;
   int inp = m->planes[0], f = m->feat_dim;
   m->Cmax = 0; m->Hmax = 0;
   for (int li = 0; li < 4; ++li) {
@@ -406,9 +344,9 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
       if (b.has_ds && ((rc = conv_rec(pre + "downsample.0", p, inp, 1, &b.ds)) || (rc = bn(pre + "downsample.1", p, &b.dsbn)))) return rc;
       b.has_se = use_se;
       if (use_se) {
-        const Rec* r1 = find(m, pre + "se.fc_1");
+        const Rec* r1 = m->recs.find(pre + "se.fc_1");
         XVB_CHECK_ARG(r1, "xvb_resnet_finalize: record '%sse.fc_1' is missing (the first block has SE)", pre.c_str());
-        const int hid = r1->Cout;
+        const int hid = r1->shape[0];
         const Rec* r2;
         if ((rc = need(pre + "se.fc_1", hid, p, 1, &r1)) || (rc = need(pre + "se.fc_2", p, hid, 1, &r2))) return rc;
         XVB_CHECK_ARG(!r1->b.empty() && !r2->b.empty(), "xvb_resnet_finalize: the SE linears of '%s' need their biases", pre.c_str());
@@ -428,11 +366,11 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
           for (int u = 0; u < se.Hp; ++u)
             for (int j = 0; j < k; ++j)
               for (int c = 0; c < p; ++c) wk[((size_t)u * k + j) * p + c] = w1[(size_t)u * p + c] / (float)k;
-          if ((rc = m->upload(&se.w1k[l], wk))) return rc;
+          if ((rc = m->dev.upload(&se.w1k[l], wk))) return rc;
           se.kmax = k;
         }
-        if (!se.w1k[0] && (rc = m->upload(&se.w1k[0], w1))) return rc;   // C > 256: the plain mean only
-        if ((rc = m->upload(&se.b1, b1)) || (rc = m->upload(&se.w2, w2)) || (rc = m->upload(&se.b2, r2->b))) return rc;
+        if (!se.w1k[0] && (rc = m->dev.upload(&se.w1k[0], w1))) return rc;   // C > 256: the plain mean only
+        if ((rc = m->dev.upload(&se.b1, b1)) || (rc = m->dev.upload(&se.w2, w2)) || (rc = m->dev.upload(&se.b2, r2->b))) return rc;
         if (se.Hp > m->Hmax) m->Hmax = se.Hp;
       }
       if (p > m->Cmax) m->Cmax = p;
@@ -445,28 +383,27 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
   // segment level (resnet_xvector.py:194-206): [fc1 ->] [fc2], as many as the extracted position hands over
   int cin = 2 * m->F4 * m->C4;
   for (const char* n : {"fc1", "fc2"}) {
-    const Rec* s = find(m, n);
+    const Rec* s = m->recs.find(n);
     if (!s) continue;
-    rc = need(n, s->Cout, cin, 1, &s);
+    rc = need(n, s->shape[0], cin, 1, &s);
     if (rc) return rc;
     Seg g;
-    g.Cin = cin; g.Cout_real = s->Cout; g.Cout = (s->Cout + 7) / 8 * 8;
+    g.Cin = cin; g.Cout_real = s->shape[0]; g.Cout = (s->shape[0] + 7) / 8 * 8;
     g.flags = (s->flags & XVB_RELU) | (s->s.empty() ? 0 : XVB_BN);
     std::vector<float> w(s->w), b(s->b), sc(s->s), sh(s->t);
     w.resize((size_t)g.Cout * cin, 0.f);   // padded output rows come out as exact zeros
     if (!b.empty()) b.resize(g.Cout, 0.f);
     if (!sc.empty()) { sc.resize(g.Cout, 0.f); sh.resize(g.Cout, 0.f); }
-    if ((rc = m->pack(&g.w, w, g.Cout, cin, 1)) || (rc = m->upload(&g.bias, b)) || (rc = m->upload(&g.scale, sc)) ||
-        (rc = m->upload(&g.shift, sh)))
+    if ((rc = m->dev.pack(&g.w, w, g.Cout, cin, 1, kTaps, 1)) || (rc = m->dev.upload(&g.bias, b)) || (rc = m->dev.upload(&g.scale, sc)) ||
+        (rc = m->dev.upload(&g.shift, sh)))
       return rc;
     m->seg.push_back(g);
-    cin = s->Cout;
+    cin = s->shape[0];
   }
   XVB_CHECK_ARG(!m->seg.empty(), "xvb_resnet_finalize: record 'fc1' or 'fc2' is missing (no segment layer)");
   m->E = m->seg.back().Cout_real;
   m->seg_mid = m->seg.size() > 1 ? m->seg[0].Cout : 0;
-  for (const std::string& n : m->order)
-    XVB_CHECK_ARG(used.count(n), "xvb_resnet_finalize: record '%s' is not part of this configuration", n.c_str());
+  if ((rc = m->recs.check_all_used("xvb_resnet_finalize"))) return rc;
   h->finalized = true;
   return XVB_OK;
 }
@@ -479,14 +416,10 @@ extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, in
   XVB_CHECK_ARG(h && h->finalized, "xvb_resnet_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_resnet_extract: bad arguments");
   const long before = g_launches;
-  const long long per_utt = (long long)T * h->m->feat_dim;
-  int g = (int)(kPositionBudget / per_utt);
-  if (g < 1) g = 1;
-  for (int i = 0; i < B; i += g) {
-    const int b = B - i < g ? B - i : g;
-    int rc = extract_group(h, feats + (size_t)i * per_utt, b, T, emb + (size_t)i * h->m->E, stream);
-    if (rc) return rc;
-  }
+  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->E;
+  int rc = for_groups(B, (long long)per_utt, kPositionBudget,
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, stream); });
+  if (rc) return rc;
   h->last_launches = (int)(g_launches - before);
   return XVB_OK;
 }
@@ -621,71 +554,29 @@ extern "C" int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats
   return XVB_OK;
 }
 
-// ---- "XVBR0001" model files: the create arguments, then the named records as handed over -------------------------
+// ---- "XVBR0001" model files: the create arguments, then the named records as handed over (save_records) -----------
 extern "C" int xvb_resnet_save(const xvb_resnet_t* h, const char* path) {
   XVB_CHECK_ARG(h && h->finalized && path, "xvb_resnet_save: model not finalized");
   const Model* m = h->m;
-  FILE* f = fopen(path, "wb");
-  XVB_CHECK_ARG(f, "xvb_resnet_save: cannot open '%s'", path);
-  bool ok = fwrite("XVBR0001", 1, 8, f) == 8;
-  const int32_t hd[10] = {m->feat_dim, m->layers[0], m->layers[1], m->layers[2], m->layers[3],
-                          m->planes[0], m->planes[1], m->planes[2], m->planes[3], m->pre};
-  const int32_t nrec = (int32_t)m->order.size();
-  ok = ok && fwrite(hd, 4, 10, f) == 10 && fwrite(&m->eps, 4, 1, f) == 1 && fwrite(&nrec, 4, 1, f) == 1;
-  for (const std::string& n : m->order) {
-    const Rec& r = m->recs.at(n);
-    const int32_t nl = (int32_t)n.size();
-    const int32_t rec[7] = {r.Cout, r.Cin, r.ksize, r.flags, (int32_t)!r.w.empty(), (int32_t)!r.b.empty(), (int32_t)!r.s.empty()};
-    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(rec, 4, 7, f) == 7 &&
-         fwrite(r.w.data(), 4, r.w.size(), f) == r.w.size() && fwrite(r.b.data(), 4, r.b.size(), f) == r.b.size() &&
-         fwrite(r.s.data(), 4, r.s.size(), f) == r.s.size() && fwrite(r.t.data(), 4, r.t.size(), f) == r.t.size();
-  }
-  ok = fclose(f) == 0 && ok;
-  XVB_CHECK_ARG(ok, "xvb_resnet_save: write to '%s' failed", path);
-  return XVB_OK;
+  int32_t cfg[11] = {m->feat_dim, m->layers[0], m->layers[1], m->layers[2], m->layers[3],
+                     m->planes[0], m->planes[1], m->planes[2], m->planes[3], m->pre};
+  memcpy(cfg + 10, &m->eps, sizeof(float));   // pooling_eps as f32
+  return save_records("xvb_resnet_save", path, kFile, cfg, m->recs);
 }
 
 extern "C" int xvb_resnet_load(xvb_resnet_t** out, const char* path) {
-  XVB_CHECK_ARG(out && path, "xvb_resnet_load: null argument");
-  FILE* f = fopen(path, "rb");
-  XVB_CHECK_ARG(f, "xvb_resnet_load: cannot open '%s'", path);
-  auto rd = [&](void* p, size_t n) { return fread(p, 1, n, f) == n; };
-  char magic[8];
-  int32_t hd[10], nrec = 0;
-  float eps = 0.f;
-  xvb_resnet_t* h = nullptr;
-  int rc = XVB_EINVAL;
-  do {
-    if (!rd(magic, 8) || memcmp(magic, "XVBR0001", 8) != 0 || !rd(hd, sizeof hd) || !rd(&eps, 4) || !rd(&nrec, 4) || nrec < 1 ||
-        nrec > 4096) {
-      set_error("xvb_resnet_load: '%s' is not an XVBR0001 file", path);
-      break;
-    }
-    if ((rc = xvb_resnet_create(&h, hd[0], hd + 1, hd + 5, hd[9], eps))) break;
-    std::vector<float> w, b, s, t;
-    for (int i = 0; i < nrec && rc == XVB_OK; ++i) {
-      int32_t nl = 0, rec[7];
-      char name[128];
-      bool ok = rd(&nl, 4) && nl > 0 && nl < 127 && rd(name, (size_t)nl) && rd(rec, sizeof rec) && rec[0] > 0 && rec[0] <= 65536 &&
-                rec[1] >= 0 && rec[1] <= (1 << 20) && (rec[2] == 0 || rec[2] == 1 || rec[2] == 3) && rec[4] == (rec[2] > 0) &&
-                (int64_t)rec[0] * rec[1] * rec[2] * rec[2] <= (int64_t)1 << 28;
-      if (ok) {
-        name[nl] = 0;
-        w.resize(rec[4] ? (size_t)rec[0] * rec[1] * rec[2] * rec[2] : 0);
-        ok = rd(w.data(), w.size() * 4);
-        if (ok && rec[5]) { b.resize(rec[0]); ok = rd(b.data(), b.size() * 4); }
-        if (ok && rec[6]) { s.resize(rec[0]); t.resize(rec[0]); ok = rd(s.data(), s.size() * 4) && rd(t.data(), t.size() * 4); }
-      }
-      if (!ok) { set_error("xvb_resnet_load: '%s' is truncated or corrupt at record %d", path, i); rc = XVB_EINVAL; break; }
-      rc = xvb_resnet_set_layer(h, name, rec[0], rec[1], rec[2], rec[4] ? w.data() : nullptr, rec[5] ? b.data() : nullptr,
-                                rec[6] ? s.data() : nullptr, rec[6] ? t.data() : nullptr, rec[3]);
-    }
-    if (rc == XVB_OK) rc = xvb_resnet_finalize(h);
-  } while (0);
-  fclose(f);
-  if (rc != XVB_OK) { if (h) xvb_resnet_destroy(h); return rc; }
-  *out = h;
-  return XVB_OK;
+  return load_records(
+      "xvb_resnet_load", path, kFile, (void**)out,
+      [](void** h, const void* cfg) {
+        const int32_t* v = (const int32_t*)cfg;
+        float eps;
+        memcpy(&eps, v + 10, sizeof eps);
+        return xvb_resnet_create((xvb_resnet_t**)h, v[0], v + 1, v + 5, v[9], eps);
+      },
+      [](void* h, const char* name, const int* shape, const float* w, const float* b, const float* s, const float* t, int flags) {
+        return xvb_resnet_set_layer((xvb_resnet_t*)h, name, shape[0], shape[1], shape[2], w, b, s, t, flags);
+      },
+      [](void* h) { return xvb_resnet_finalize((xvb_resnet_t*)h); }, [](void* h) { xvb_resnet_destroy((xvb_resnet_t*)h); });
 }
 
 extern "C" void xvb_resnet_destroy(xvb_resnet_t* h) {

@@ -20,6 +20,7 @@ even=False).
 build_extractor() returns NativeCamPPExtractor: the same launch sequence in the C library (csrc/campplus_extractor.cu),
 which also writes XVBP0001 model files for bin/xvb-extract.  XVB_CAMPP_NATIVE=0 selects CamPPExtractor, the Python driver
 of the same kernels with the same embeddings bit for bit."""
+import ctypes as C
 import os
 import sys
 from collections import OrderedDict
@@ -31,6 +32,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor  # noqa: E402
 from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 
@@ -499,65 +501,24 @@ def native_records(m):
     return out
 
 
-class NativeCamPPExtractor:
+class NativeCamPPExtractor(NativeExtractor):
     """xvb_campp_t: packed weights, workspace and the whole launch sequence of CamPPExtractor in the C library, on the
     device that is current when it is built (or loaded from an XVBP0001 file)."""
 
-    def __init__(self, m=None, device=None, path=None):
-        import ctypes as C
-        from asv_subtools_b200._lib import CamPPConfig, check, lib
-        self._C, self._lib, self._check = C, lib, check
-        self._h = C.c_void_p()
-        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
-            if path is not None:
-                check(lib.xvb_campp_load(C.byref(self._h), str(path).encode()), "xvb_campp_load")
-            else:
-                cfg = CamPPConfig(**native_config(m))
-                check(lib.xvb_campp_create(C.byref(self._h), C.byref(cfg)), "xvb_campp_create")
-                for name, w, b, scale, shift, flags, _ in native_records(m):
-                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
-                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
-                    rows = arrs[0].shape[0] if arrs[0] is not None else arrs[2].shape[0]
-                    cols = arrs[0].shape[1] if arrs[0] is not None else 0
-                    check(lib.xvb_campp_set_layer(self._h, name.encode(), rows, cols, *ptr, flags), "xvb_campp_set_layer")
-                check(lib.xvb_campp_finalize(self._h), "xvb_campp_finalize")
-        self.feat_dim = lib.xvb_campp_feat_dim(self._h)
-        self.embed_dim = lib.xvb_campp_embed_dim(self._h)
+    PREFIX = "campp"
 
-    @classmethod
-    def load(cls, path):
-        return cls(path=path)
+    def _create_args(self, m):
+        from asv_subtools_b200._lib import CamPPConfig
+        return (C.byref(CamPPConfig(**native_config(m))),)
 
-    def save(self, path):
-        """Write an XVBP0001 model file for bin/xvb-extract."""
-        self._check(self._lib.xvb_campp_save(self._h, str(path).encode()), "xvb_campp_save")
+    def _layers(self, m):
+        for name, w, b, scale, shift, flags, _ in native_records(m):
+            rows = (w if w is not None else scale).shape[0]
+            yield name, (rows, w.shape[1] if w is not None else 0), (w, b, scale, shift), flags
 
-    @property
-    def last_launches(self):
-        return self._lib.xvb_campp_last_launches(self._h)
-
-    def extract(self, feats):
-        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
-        stream."""
+    def _input(self, feats):
         if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.dim() == 3):
             raise TypeError("feats must be a (B, T, F) CUDA float32 tensor")
-        B, T, Fd = feats.shape
-        if Fd != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, Fd))
-        feats = feats.contiguous()
-        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
-        self._check(self._lib.xvb_campp_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
-                                                C.c_void_p(torch.cuda.current_stream().cuda_stream)), "xvb_campp_extract")
-        return emb
-
-    def close(self):
-        h, self._h = self._h, None
-        if h:
-            self._lib.xvb_campp_destroy(h)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        if feats.shape[2] != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
+        return feats.contiguous()

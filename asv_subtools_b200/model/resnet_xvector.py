@@ -18,6 +18,7 @@ The launch sequence runs in the native handle (NativeResNetExtractor over xvb_re
 also writes XVBR0001 model files for bin/xvb-extract.  XVB_RESNET_NATIVE=0 selects ResNetExtractor, the Python driver of
 the same kernels in the same order, whose embeddings are bit-identical."""
 import copy
+import ctypes as C
 import os
 import sys
 
@@ -28,6 +29,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor, _cuda_f32  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
@@ -360,65 +362,24 @@ class ResNetExtractor:
         pass
 
 
-def _cuda_f32(feats, feat_dim):
-    if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
-        raise TypeError("feats must be a contiguous CUDA float32 tensor")
-    if feats.shape[2] != feat_dim:
-        raise ValueError("expected feature dim {}, got {}".format(feat_dim, feats.shape[2]))
-    return feats
-
-
-class NativeResNetExtractor:
+class NativeResNetExtractor(NativeExtractor):
     """xvb_resnet_t: packed weights, workspace and the whole launch sequence of ResNetExtractor in the C library, on the
     device that is current when it is built (or loaded from an XVBR0001 file)."""
 
-    def __init__(self, m=None, device=None, path=None):
-        import ctypes as C
-        from asv_subtools_b200._lib import check, int_array, lib
-        self._C, self._lib, self._check = C, lib, check
-        self._h = C.c_void_p()
-        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
-            if path is not None:
-                check(lib.xvb_resnet_load(C.byref(self._h), str(path).encode()), "xvb_resnet_load")
-            else:
-                r = m.resnet
-                stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
-                check(lib.xvb_resnet_create(C.byref(self._h), m.inputs_dim, int_array([len(s) for s in stages]),
-                                            int_array([s[0].conv1.out_channels for s in stages]),
-                                            1 if r.full_pre_activation else 0, float(m.stats.eps)), "xvb_resnet_create")
-                for name, w, b, scale, shift, relu in _named_records(m):
-                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
-                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
-                    cout = (w if w is not None else scale).shape[0]
-                    cin, k = (w.shape[1], w.shape[2] if w.ndim == 4 else 1) if w is not None else (0, 0)
-                    flags = (1 if relu else 0) | (2 if scale is not None else 0)
-                    check(lib.xvb_resnet_set_layer(self._h, name.encode(), cout, cin, k, *ptr, flags), "xvb_resnet_set_layer")
-                check(lib.xvb_resnet_finalize(self._h), "xvb_resnet_finalize")
-        self.feat_dim = lib.xvb_resnet_feat_dim(self._h)
-        self.embed_dim = lib.xvb_resnet_embed_dim(self._h)
+    PREFIX = "resnet"
 
-    @classmethod
-    def load(cls, path):
-        return cls(path=path)
+    def _create_args(self, m):
+        from asv_subtools_b200._lib import int_array
+        r = m.resnet
+        stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
+        return (m.inputs_dim, int_array([len(s) for s in stages]), int_array([s[0].conv1.out_channels for s in stages]),
+                1 if r.full_pre_activation else 0, float(m.stats.eps))
 
-    def save(self, path):
-        self._check(self._lib.xvb_resnet_save(self._h, str(path).encode()), "xvb_resnet_save")
-
-    @property
-    def last_launches(self):
-        return self._lib.xvb_resnet_last_launches(self._h)
-
-    def _stream(self):
-        return self._C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-    def extract(self, feats):
-        """feats (B, T, F) fp32 CUDA -> (B, embed_dim) fp32 CUDA, asynchronous on the current stream."""
-        B, T, _ = _cuda_f32(feats, self.feat_dim).shape
-        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
-        self._check(self._lib.xvb_resnet_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
-                                                 self._stream()), "xvb_resnet_extract")
-        return emb
+    def _layers(self, m):
+        for name, w, b, scale, shift, relu in _named_records(m):
+            cout = (w if w is not None else scale).shape[0]
+            cin, k = (w.shape[1], w.shape[2] if w.ndim == 4 else 1) if w is not None else (0, 0)
+            yield name, (cout, cin, k), (w, b, scale, shift), (1 if relu else 0) | (2 if scale is not None else 0)
 
     def extract_host(self, feats_np):
         """feats (B, T, F) float32 host array -> (B, D) float32 host array (H2D + D2H + one sync inside the call)."""
@@ -427,7 +388,6 @@ class NativeResNetExtractor:
         if f != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
         emb = np.empty((b, self.embed_dim), dtype=np.float32)
-        C = self._C
         self._check(self._lib.xvb_resnet_extract_host(self._h, feats_np.ctypes.data_as(C.c_void_p), b, t,
                                                       emb.ctypes.data_as(C.c_void_p), self._stream()), "xvb_resnet_extract_host")
         return emb
@@ -436,27 +396,14 @@ class NativeResNetExtractor:
         """feats (N, T, F) fp32 CUDA -> (N, D): the whole shard in `batch`-utterance batches, one C call."""
         n, t, _ = _cuda_f32(feats, self.feat_dim).shape
         emb = out if out is not None else torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
         self._check(self._lib.xvb_resnet_extract_shard(self._h, C.c_void_p(feats.data_ptr()), n, t, int(batch),
                                                        C.c_void_p(emb.data_ptr()), self._stream()), "xvb_resnet_extract_shard")
         return emb
 
     def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=128):
         """Pinned host feats (n, t, F) in, host embeddings (n, D) out; copies overlap the stack."""
-        C = self._C
         self._check(self._lib.xvb_resnet_extract_shard_host(self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch),
                                                             C.c_void_p(emb_ptr), self._stream()), "xvb_resnet_extract_shard_host")
-
-    def close(self):
-        h, self._h = self._h, None
-        if h:
-            self._lib.xvb_resnet_destroy(h)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 if __name__ == "__main__":

@@ -33,6 +33,7 @@ utterance is cut into num_split = ceil(T / 300) chunks, each chunk is extracted 
 averaged weighted by chunk length.  extract_embedding_batch applies the same rule to a batch of equal-length
 utterances with two stack runs (all full chunks, then all last chunks)."""
 import copy
+import ctypes as C
 import math
 import os
 import sys
@@ -47,6 +48,7 @@ from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200._lib import ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH  # noqa: E402
 from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import TdnnAffine, fold_batchnorm  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor  # noqa: E402
 from asv_subtools_b200.nnet.framework import for_extract_embedding  # noqa: E402
 
 MAX_CHUNK = 300     # @for_extract_embedding(maxChunk=300) of transformer_xvector.py:321
@@ -743,73 +745,20 @@ def native_records(m):
     return out
 
 
-def _cuda_f32(feats, feat_dim):
-    if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
-        raise TypeError("feats must be a contiguous CUDA float32 tensor")
-    if feats.shape[2] != feat_dim:
-        raise ValueError("expected feature dim {}, got {}".format(feat_dim, feats.shape[2]))
-    return feats
-
-
-class NativeConformerExtractor:
+class NativeConformerExtractor(NativeExtractor):
     """xvb_conformer_t: packed weights, tables, workspace and the whole launch sequence of ConformerExtractor in the C
     library, on the device that is current when it is built (or loaded from an XVBC0001 file)."""
 
-    def __init__(self, m=None, device=None, path=None):
-        import ctypes as C
-        from asv_subtools_b200._lib import ConformerConfig, check, lib
-        self._C, self._lib, self._check = C, lib, check
-        self._h = C.c_void_p()
-        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
-            if path is not None:
-                check(lib.xvb_conformer_load(C.byref(self._h), str(path).encode()), "xvb_conformer_load")
-            else:
-                cfg = ConformerConfig(**native_config(m))
-                check(lib.xvb_conformer_create(C.byref(self._h), C.byref(cfg)), "xvb_conformer_create")
-                for name, w, b, scale, shift, flags, _ in native_records(m):
-                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (w, b, scale, shift)]
-                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
-                    w, scale = arrs[0], arrs[2]
-                    rows = w.shape[0] if w is not None else scale.shape[0] if scale is not None else _norm_width(m, name)
-                    cols = w.shape[1] if w is not None else 0
-                    check(lib.xvb_conformer_set_layer(self._h, name.encode(), rows, cols, *ptr, flags), "xvb_conformer_set_layer")
-                check(lib.xvb_conformer_finalize(self._h), "xvb_conformer_finalize")
-        self.feat_dim = lib.xvb_conformer_feat_dim(self._h)
-        self.embed_dim = lib.xvb_conformer_embed_dim(self._h)
+    PREFIX = "conformer"
 
-    @classmethod
-    def load(cls, path):
-        return cls(path=path)
+    def _create_args(self, m):
+        from asv_subtools_b200._lib import ConformerConfig
+        return (C.byref(ConformerConfig(**native_config(m))),)
 
-    def save(self, path):
-        """Write an XVBC0001 model file for bin/xvb-extract."""
-        self._check(self._lib.xvb_conformer_save(self._h, str(path).encode()), "xvb_conformer_save")
-
-    @property
-    def last_launches(self):
-        return self._lib.xvb_conformer_last_launches(self._h)
-
-    def extract(self, feats):
-        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
-        stream."""
-        B, T, _ = _cuda_f32(feats, self.feat_dim).shape
-        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
-        self._check(self._lib.xvb_conformer_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
-                                                    C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                    "xvb_conformer_extract")
-        return emb
-
-    def close(self):
-        h, self._h = self._h, None
-        if h:
-            self._lib.xvb_conformer_destroy(h)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _layers(self, m):
+        for name, w, b, scale, shift, flags, _ in native_records(m):
+            rows = w.shape[0] if w is not None else scale.shape[0] if scale is not None else _norm_width(m, name)
+            yield name, (rows, w.shape[1] if w is not None else 0), (w, b, scale, shift), flags
 
 
 def _norm_width(m, name):

@@ -1,0 +1,87 @@
+"""Python handles over the native whole-model extractors of the C library that take named records: the ResNet
+(xvb_resnet_*), Conformer (xvb_conformer_*) and CAM++ (xvb_campp_*) x-vectors.  NativeExtractor holds the part they
+share: create, set_layer per record and finalize (or load a model file), save, extract and close."""
+import ctypes as C
+
+import numpy as np
+import torch
+
+
+def _cuda_f32(feats, feat_dim):
+    if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
+        raise TypeError("feats must be a contiguous CUDA float32 tensor")
+    if feats.shape[2] != feat_dim:
+        raise ValueError("expected feature dim {}, got {}".format(feat_dim, feats.shape[2]))
+    return feats
+
+
+class NativeExtractor:
+    """xvb_<PREFIX>_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
+    current when it is built from a model `m` (or loaded from a model file at `path`).
+
+    A family sets PREFIX and supplies `_create_args(m)`, the arguments of xvb_<PREFIX>_create after the handle, and
+    `_layers(m)`, which yields (name, shape, (w, b, scale, shift), flags) per record, `shape` being the set_layer
+    arguments between the name and the arrays."""
+
+    PREFIX = None
+
+    def __init__(self, m=None, device=None, path=None):
+        from asv_subtools_b200._lib import check, lib
+        self._lib, self._check = lib, check
+        self._h = C.c_void_p()
+        with torch.cuda.device(device if device is not None else torch.cuda.current_device()):
+            if path is not None:
+                self._call("load", C.byref(self._h), str(path).encode())
+            else:
+                self._call("create", C.byref(self._h), *self._create_args(m))
+                for name, shape, arrays, flags in self._layers(m):
+                    arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in arrays]
+                    ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
+                    self._call("set_layer", self._h, name.encode(), *shape, *ptr, flags)
+                self._call("finalize", self._h)
+        self.feat_dim = self._fn("feat_dim")(self._h)
+        self.embed_dim = self._fn("embed_dim")(self._h)
+
+    def _fn(self, name):
+        return getattr(self._lib, "xvb_{}_{}".format(self.PREFIX, name))
+
+    def _call(self, name, *args):
+        self._check(self._fn(name)(*args), "xvb_{}_{}".format(self.PREFIX, name))
+
+    @classmethod
+    def load(cls, path):
+        return cls(path=path)
+
+    def save(self, path):
+        """Write the model file that load() and bin/xvb-extract read."""
+        self._call("save", self._h, str(path).encode())
+
+    @property
+    def last_launches(self):
+        return self._fn("last_launches")(self._h)
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+    def _input(self, feats):
+        return _cuda_f32(feats, self.feat_dim)
+
+    def extract(self, feats):
+        """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
+        stream."""
+        feats = self._input(feats)
+        B, T, _ = feats.shape
+        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
+        self._call("extract", self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()), self._stream())
+        return emb
+
+    def close(self):
+        h, self._h = self._h, None
+        if h:
+            self._fn("destroy")(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass

@@ -758,7 +758,8 @@ int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int
 int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream);
 int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int64_t N, int T, int batch,
                                   float* emb_host, void* stream);
-/* "XVBR0001" model files: the create arguments, then the records as handed to xvb_resnet_set_layer. */
+/* "XVBR0001" model files: the create arguments, then the records as handed to xvb_resnet_set_layer (layout at
+ * save_records in csrc/model_file.cpp). */
 int xvb_resnet_save(const xvb_resnet_t* h, const char* path);
 int xvb_resnet_load(xvb_resnet_t** out, const char* path);
 void xvb_resnet_destroy(xvb_resnet_t* h);
@@ -826,7 +827,8 @@ int xvb_conformer_last_launches(const xvb_conformer_t* h);
 /* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embed_dim) fp32 on the device;
  * asynchronous on `stream`. */
 int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int B, int T, float* emb, void* stream);
-/* "XVBC0001" model files: the configuration, then the records and tables as handed to xvb_conformer_set_layer. */
+/* "XVBC0001" model files: the configuration, then the records and tables as handed to xvb_conformer_set_layer
+ * (layout at save_records in csrc/model_file.cpp). */
 int xvb_conformer_save(const xvb_conformer_t* h, const char* path);
 int xvb_conformer_load(xvb_conformer_t** out, const char* path);
 void xvb_conformer_destroy(xvb_conformer_t* h);
@@ -885,7 +887,8 @@ int xvb_campp_last_launches(const xvb_campp_t* h);
 /* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embd_dim) fp32 on the device;
  * asynchronous on `stream`. */
 int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int T, float* emb, void* stream);
-/* "XVBP0001" model files: the configuration, then the records as handed to xvb_campp_set_layer. */
+/* "XVBP0001" model files: the configuration, then the records as handed to xvb_campp_set_layer (layout at
+ * save_records in csrc/model_file.cpp). */
 int xvb_campp_save(const xvb_campp_t* h, const char* path);
 int xvb_campp_load(xvb_campp_t** out, const char* path);
 void xvb_campp_destroy(xvb_campp_t* h);

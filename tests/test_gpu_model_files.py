@@ -1,0 +1,126 @@
+"""The named-record model files of the native ResNet (XVBR0001), Conformer (XVBC0001) and CAM++ (XVBP0001) extractors on
+the H100, over every case of the three families' fixtures: save() writes exactly the bytes of a writer of the documented
+layout fed the records the handle was built from; load() then save() reproduces the file byte for byte; and corrupt files
+are refused with an error naming the magic or the damage, without a crash."""
+import struct
+
+import numpy as np
+import pytest
+
+import campplus_oracle as po
+import conformer_2sub_oracle as c2
+import conformer_oracle as co
+import resnet_oracle as ro
+from asv_subtools_b200._lib import CamPPConfig, ConformerConfig
+from asv_subtools_b200.model.campplus_xvector import CamPPXvector, NativeCamPPExtractor, native_config as campp_config
+from asv_subtools_b200.model.resnet_xvector import NativeResNetExtractor, ResNetXvector
+from asv_subtools_b200.model.transformer_xvector import (NativeConformerExtractor, TransformerXvector,
+                                                         native_config as conformer_config)
+from oracle import nnet as onn
+
+pytestmark = pytest.mark.gpu
+
+CONFORMER_CASES = dict(co.CASES, **c2.CASES)
+# family -> (magic, shape ints per record, record limit)
+FORMATS = {"resnet": (b"XVBR0001", 3, 4096), "conformer": (b"XVBC0001", 2, 65536), "campp": (b"XVBP0001", 2, 65536)}
+CASES = ([("resnet", c) for c in sorted(ro.CASES)] + [("conformer", c) for c in sorted(CONFORMER_CASES)] +
+         [("campp", c) for c in sorted(po.CASES)])
+
+
+def _build(family, case, golden):
+    """(model, native handle, configuration block) of one fixture case."""
+    if family == "resnet":
+        kwargs, fdim, _, positions, seed, _ = ro.CASES[case]
+        m = ResNetXvector(fdim, 10, training=False, extracted_embedding=positions[0], **kwargs)
+        m.load_state_dict(onn.make_state_dict(ro.resnet_spec(fdim, kwargs), seed), strict=True)
+        m = m.cuda().eval()
+        r = m.resnet
+        stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
+        ints = [m.inputs_dim] + [len(s) for s in stages] + [s[0].conv1.out_channels for s in stages]
+        cfg = np.array(ints + [1 if r.full_pre_activation else 0], "<i4").tobytes() + np.float32(m.stats.eps).tobytes()
+        return m, NativeResNetExtractor(m), cfg
+    if family == "conformer":
+        kwargs, fdim, _, positions, seed = CONFORMER_CASES[case][:5]
+        npz = "conformer" if case in co.CASES else "conformer_2sub"
+        m = TransformerXvector(fdim, 10, training=False, extracted_embedding=positions[0], **kwargs)
+        m.load_state_dict(co.seeded_state_dict(golden(npz)["keys_" + case], seed), strict=True)
+        m = m.cuda().eval()
+        return m, NativeConformerExtractor(m), bytes(ConformerConfig(**conformer_config(m)))
+    kw = dict(po.CASES[case][0])
+    m = CamPPXvector(kw.pop("inputs_dim"), 10, **kw)
+    m.load_state_dict(po.seeded_state_dict(golden("campplus")["keys_" + case], po.CASES[case][3]), strict=True)
+    m = m.cuda().eval()
+    return m, NativeCamPPExtractor(m), bytes(CamPPConfig(**campp_config(m)))
+
+
+def _write(magic, cfg, layers):
+    """The layout: magic | configuration block | i32 nrec, then per record i32 name_len | name | i32 shape[n] | i32 flags
+    | i32 has_w, has_b, has_s | f32 w? | f32 b? | f32 s, t?"""
+    out = bytearray(magic + cfg + struct.pack("<i", len(layers)))
+    for name, shape, arrays, flags in layers:
+        w, b, s, t = [None if a is None else np.ascontiguousarray(a, dtype="<f4") for a in arrays]
+        out += struct.pack("<i", len(name)) + name.encode()
+        out += np.array(list(shape) + [flags, w is not None, b is not None, s is not None], "<i4").tobytes()
+        for a in (w, b, s, t):
+            if a is not None:
+                out += a.tobytes()
+    return bytes(out)
+
+
+def _records(data, cfg_len, nshape):
+    """(start, payload start, end, has_w offset) of each record of a model file."""
+    pos = 8 + cfg_len
+    (nrec,) = struct.unpack_from("<i", data, pos)
+    pos += 4
+    out = []
+    for _ in range(nrec):
+        start = pos
+        (nl,) = struct.unpack_from("<i", data, pos)
+        hd = np.frombuffer(data, "<i4", nshape + 4, pos + 4 + nl)
+        payload = pos + 4 + nl + 4 * (nshape + 4)
+        rows = int(hd[0])
+        welems = rows * int(hd[1]) * (int(hd[2]) ** 2 if nshape == 3 else 1)
+        end = payload + 4 * (welems * int(hd[nshape + 1]) + rows * int(hd[nshape + 2]) + 2 * rows * int(hd[nshape + 3]))
+        out.append((start, payload, end, pos + 4 + nl + 4 * (nshape + 1)))
+        pos = end
+    assert pos == len(data)
+    return out
+
+
+@pytest.mark.parametrize("family, case", CASES)
+def test_model_file_bytes_roundtrip_and_rejects(tmp_path, golden, family, case):
+    magic, nshape, limit = FORMATS[family]
+    m, ex, cfg = _build(family, case, golden)
+    cls = type(ex)
+    path, again, bad = str(tmp_path / "model.xvbm"), str(tmp_path / "again.xvbm"), str(tmp_path / "bad.xvbm")
+    ex.save(path)
+    data = open(path, "rb").read()
+    assert data == _write(magic, cfg, list(ex._layers(m)))
+    loaded = cls.load(path)
+    loaded.save(again)
+    loaded.close()
+    assert open(again, "rb").read() == data
+
+    recs = _records(data, len(cfg), nshape)
+    first_w = next(r for r in recs if r[2] - r[1] > 8)
+    nrec_at = 8 + len(cfg)
+
+    def patched(offset, value):
+        b = bytearray(data)
+        b[offset:offset + 4] = struct.pack("<i", value)
+        return bytes(b)
+
+    has_w = struct.unpack_from("<i", data, recs[0][3])[0]
+    blobs = [(data[:recs[1][0]], "truncated|corrupt"),                    # cut at a record boundary
+             (data[:first_w[1] + 6], "truncated|corrupt"),                # cut inside a weight
+             (patched(nrec_at, 0), magic.decode()),
+             (patched(nrec_at, limit + 1), magic.decode()),
+             (patched(recs[0][0], 0), "truncated|corrupt"),               # name length 0
+             (patched(recs[0][0], 127), "truncated|corrupt"),             # name length 127
+             (patched(recs[0][3], 1 - has_w), "truncated|corrupt")]       # has_w contradicts the shape
+    for blob, msg in blobs:
+        with open(bad, "wb") as f:
+            f.write(blob)
+        with pytest.raises(RuntimeError, match=msg):
+            cls.load(bad)
+    ex.close()
