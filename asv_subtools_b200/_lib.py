@@ -63,6 +63,12 @@ class CamPPConfig(C.Structure):
     _fields_ = [(n, C.c_int) for n in ("feat_dim", "embd_dim", "init_channels", "growth_rate", "bn_size")]
 
 
+class RepVGGConfig(C.Structure):
+    """xvb_repvgg_config_t (include/xvb200.h)."""
+    _fields_ = [("feat_dim", C.c_int), ("ksize", C.c_int), ("num_blocks", C.c_int * 4), ("strides", C.c_int * 5),
+                ("widths", C.c_int * 5), ("pooling_eps", C.c_float)]
+
+
 class XvbError(RuntimeError):
     pass
 
@@ -206,6 +212,17 @@ SIGNATURES = {
     "xvb_resnet_save": (_i, [_p, C.c_char_p]),
     "xvb_resnet_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_resnet_destroy": (None, [_p]),
+    "xvb_repvgg_create": (_i, [C.POINTER(_p), _p]),
+    "xvb_repvgg_set_layer": (_i, [_p, C.c_char_p, _i, _i, _i, _p, _p, _p, _p, _i]),
+    "xvb_repvgg_finalize": (_i, [_p]),
+    "xvb_repvgg_feat_dim": (_i, [_p]),
+    "xvb_repvgg_embed_dim": (_i, [_p]),
+    "xvb_repvgg_last_launches": (_i, [_p]),
+    "xvb_repvgg_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_repvgg_save": (_i, [_p, C.c_char_p]),
+    "xvb_repvgg_load": (_i, [C.POINTER(_p), C.c_char_p]),
+    "xvb_repvgg_destroy": (None, [_p]),
+    "xvb_conv2d_kept_taps": (_i, [_p, _i, _i, _i, _ip, _i]),
     "xvb_conformer_create": (_i, [C.POINTER(_p), _p]),
     "xvb_conformer_set_layer": (_i, [_p, C.c_char_p, _i, _i, _p, _p, _p, _p, _i]),
     "xvb_conformer_finalize": (_i, [_p]),

@@ -14,11 +14,11 @@
 // :17-45: <model-path> <feats-rspecifier> <vectors-wspecifier>); the role is that of the reference's
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
-// the input side.  The model file is any of the five families, told apart by its magic: TDNN x-vector
+// the input side.  The model file is any of the six families, told apart by its magic: TDNN x-vector
 // (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
-// 2-D ResNet x-vector (XVBR0001), Conformer x-vector (XVBC0001, 4x or 2x subsampling) or CAM++ x-vector (XVBP0001), the
-// last three written by the native extractors' save().  What it adds: utterances of equal length are batched (the
-// reference runs batch 1).
+// 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
+// subsampling) or CAM++ x-vector (XVBP0001), the last four written by the native extractors' save().  What it adds:
+// utterances of equal length are batched (the reference runs batch 1).
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
@@ -88,6 +88,7 @@ struct Family {
 const Family kFamilies[] = {
     {{"XVBE0001", "XVBE0002"}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false},
     {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false},
+    {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false},
     {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false},
     {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true},
     // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
@@ -236,11 +237,11 @@ int main(int argc, char** argv) {
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
              "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001),\n"
-             "Conformer x-vector (XVBC0001) or CAM++ x-vector (XVBP0001) model, recognised by its magic.  --max-chunk defaults\n"
-             "to 300 frames for a Conformer (the model's own chunk rule), 4000 for CAM++ and 10000 otherwise.  A Conformer\n"
-             "chunk needs at least 7 frames and fewer than 5000 subsampled frames.  CAM++ cuts an utterance with egrecho's\n"
-             "rule (max-chunk-long chunks, the last two re-split evenly: 9000 -> 4000, 2500, 2500); a chunk needs at least\n"
-             "3 frames.\n");
+             "RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001) or CAM++ x-vector (XVBP0001) model,\n"
+             "recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the model's own chunk rule),\n"
+             "4000 for CAM++ and 10000 otherwise.  A Conformer chunk needs at least 7 frames and fewer than 5000 subsampled\n"
+             "frames.  CAM++ cuts an utterance with egrecho's rule (max-chunk-long chunks, the last two re-split evenly:\n"
+             "9000 -> 4000, 2500, 2500); a chunk needs at least 3 frames.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());

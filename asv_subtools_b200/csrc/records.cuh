@@ -1,6 +1,6 @@
-// Device side of the ResNet, Conformer and CAM++ native extractors' shared plumbing: the packed split-bf16 planes, the
-// arena that owns a model's device weights, the grow-only workspace and the group loop of an extract call.  The record
-// store and the model-file codec are host code in records.h.
+// Device side of the ResNet, RepVGG, Conformer and CAM++ native extractors' shared plumbing: the packed split-bf16
+// planes, the arena that owns a model's device weights, the grow-only workspace, the segment level of the 2-D families
+// and the group loop of an extract call.  The record store and the model-file codec are host code in records.h.
 #pragma once
 #include <vector>
 
@@ -31,7 +31,10 @@ struct Weights {
     XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
     return XVB_OK;
   }
-  // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx[0..n) (ops.pack_tdnn_weight / pack_conv2d_weight)
+  // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx[0..n) (ops.pack_tdnn_weight / pack_conv2d_weight).
+  // xvb_pack_tdnn_weight takes at most XVB_MAX_TAPS taps per call: a longer list is packed in pieces of that many taps
+  // (the last one shorter), each piece's rows then copied into its K range of every output row, as pack_conv2d_weight
+  // concatenates the pieces along K.  Up to XVB_MAX_TAPS taps it is the one call straight into the planes.
   int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int tot, const int* ctx, int n) {
     float* w_dev = nullptr;
     XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
@@ -41,9 +44,30 @@ struct Weights {
     int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
     if (!rc) rc = alloc(&c->hi, pn);
     if (!rc) rc = alloc(&c->lo, pn);
-    if (!rc) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx, n, c->hi, c->lo, nullptr);
+    if (!rc && n <= XVB_MAX_TAPS) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx, n, c->hi, c->lo, nullptr);
+    Planes piece;
+    if (!rc && n > XVB_MAX_TAPS) {
+      const size_t tap = pn / ((size_t)Cout * n);   // packed elements of one tap in one output row (Cin padded to 16)
+      const size_t bytes = (size_t)xvb_packed_weight_elems(Cout, Cin, XVB_MAX_TAPS) * sizeof(uint16_t);
+      if (cudaMalloc((void**)&piece.hi, bytes) != cudaSuccess || cudaMalloc((void**)&piece.lo, bytes) != cudaSuccess) {
+        set_error("%s: cudaMalloc of a packing piece failed", fn);
+        rc = XVB_ECUDA;
+      }
+      for (int i = 0; i < n && !rc; i += XVB_MAX_TAPS) {
+        const int m = n - i < XVB_MAX_TAPS ? n - i : XVB_MAX_TAPS;
+        rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx + i, m, piece.hi, piece.lo, nullptr);
+        const size_t dpitch = (size_t)n * tap * sizeof(uint16_t), spitch = (size_t)m * tap * sizeof(uint16_t);
+        for (int p = 0; p < 2 && !rc; ++p) {
+          uint16_t* dst = (p ? c->lo : c->hi) + (size_t)i * tap;
+          const cudaError_t ce = cudaMemcpy2D(dst, dpitch, p ? piece.lo : piece.hi, spitch, spitch, (size_t)Cout,
+                                              cudaMemcpyDeviceToDevice);
+          if (ce != cudaSuccess) { set_error("%s: joining the packed pieces failed: %s", fn, cudaGetErrorString(ce)); rc = XVB_ECUDA; }
+        }
+      }
+    }
     if (!rc && cudaDeviceSynchronize() != cudaSuccess) rc = XVB_ECUDA;
     if (rc == XVB_ECUDA && e != cudaSuccess) set_error("%s: weight upload failed: %s", fn, cudaGetErrorString(e));
+    cudaFree(piece.hi); cudaFree(piece.lo);
     cudaFree(w_dev);
     return rc;
   }
@@ -82,6 +106,81 @@ struct Workspace {
     cap[i] = 0;
   }
   void free() { for (int i = 0; i < N; ++i) release(i); }
+};
+
+// The segment level of the 2-D families (ResNet, RepVGG): statistics pooling of the last conv's fp32 (B, T', F' * C)
+// output with planes out, then [fc1 ->] fc2 on the wgmma layer kernel at T = 1, each as _PackedAffine runs it.
+struct SegLayer {   // one segment layer, output rows padded to a multiple of 8
+  Planes w;
+  float* bias = nullptr; float* scale = nullptr; float* shift = nullptr;
+  int Cin = 0, Cout = 0, Cout_real = 0, flags = 0;
+};
+
+struct SegTail {
+  std::vector<SegLayer> seg;
+  int E = 0;     // the embedding dim, the last layer's real rows
+  int mid = 0;   // the first layer's padded rows when there are two layers, else 0
+
+  // Takes "fc1" / "fc2", as many as the extracted position hands over, the first one over `cin` pooled columns: each
+  // record (Cout, Cin, 1) with a bias, scale / shift as XVB_BN and XVB_RELU as the layer applies them.  Pads the rows to
+  // a multiple of 8 with zeros (the padded outputs are exact zeros) and packs them.  fn: the caller's name.
+  int build(RecordStore& recs, Weights& dev, const char* fn, int cin) {
+    for (const char* n : {"fc1", "fc2"}) {
+      const Rec* s = recs.find(n);
+      if (!s) continue;
+      const int shape[3] = {s->shape[0], cin, 1};
+      int rc = recs.take(fn, n, shape, &s);
+      if (rc) return rc;
+      SegLayer g;
+      g.Cin = cin; g.Cout_real = s->shape[0]; g.Cout = (s->shape[0] + 7) / 8 * 8;
+      g.flags = (s->flags & XVB_RELU) | (s->s.empty() ? 0 : XVB_BN);
+      std::vector<float> w(s->w), b(s->b), sc(s->s), sh(s->t);
+      w.resize((size_t)g.Cout * cin, 0.f);
+      if (!b.empty()) b.resize(g.Cout, 0.f);
+      if (!sc.empty()) { sc.resize(g.Cout, 0.f); sh.resize(g.Cout, 0.f); }
+      if ((rc = dev.pack(&g.w, w, g.Cout, cin, 1, kTaps, 1)) || (rc = dev.upload(&g.bias, b)) || (rc = dev.upload(&g.scale, sc)) ||
+          (rc = dev.upload(&g.shift, sh)))
+        return rc;
+      seg.push_back(g);
+      cin = s->shape[0];
+    }
+    XVB_CHECK_ARG(!seg.empty(), "%s: record 'fc1' or 'fc2' is missing (no segment layer)", fn);
+    E = seg.back().Cout_real;
+    mid = seg.size() > 1 ? seg[0].Cout : 0;
+    return XVB_OK;
+  }
+  int out_rows() const { return seg.back().Cout; }
+
+  // last: the (B, T, pc) fp32 output of the last conv -> emb (B, E).  Buffers per utterance: pooled planes and
+  // pooled_f32 of 2 * pc, mid planes of `mid` and out of out_rows() (used when the last layer is padded).
+  int run(const float* last, int pc, int B, int T, float eps, Planes pooled, float* pooled_f32, Planes mid_planes,
+          float* out, float* emb, void* stream) const {
+    int rc;
+    if ((rc = xvb_stats_pool_ex(last, pc, B, T, pc, eps, 0, pooled_f32, pooled.hi, pooled.lo, 2 * pc, stream))) return rc;
+    Planes x = pooled;
+    int64_t ldx = 2 * pc;
+    const int ctx0 = 0;
+    for (size_t j = 0; j < seg.size(); ++j) {
+      const SegLayer& s = seg[j];
+      const bool fin = j + 1 == seg.size();
+      xvb_tdnn_args_t a{};
+      a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
+      a.w_hi = s.w.hi; a.w_lo = s.w.lo;
+      a.bias = s.bias; a.bn_scale = s.scale; a.bn_shift = s.shift;
+      a.flags = s.flags;
+      a.context_host = &ctx0; a.ntaps = 1;
+      if (fin) { a.y_f32 = s.Cout == E ? emb : out; a.ldyf = s.Cout; }
+      else { a.y_hi = mid_planes.hi; a.y_lo = mid_planes.lo; a.ldy = s.Cout; }
+      a.B = B; a.T = 1; a.Cin = s.Cin; a.Cout = s.Cout;
+      if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
+      x = mid_planes; ldx = s.Cout;
+    }
+    const SegLayer& s = seg.back();
+    if (s.Cout != E)
+      XVB_CUDA(cudaMemcpy2DAsync(emb, (size_t)E * sizeof(float), out, (size_t)s.Cout * sizeof(float), (size_t)E * sizeof(float),
+                                 (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    return XVB_OK;
+  }
 };
 
 // One extract call as groups of floor(budget / per_utt) utterances (at least one): run(first, count) per group.

@@ -46,12 +46,6 @@ struct Block {
   bool has_ds = false, has_se = false;
   Se se;
 };
-struct Seg {   // one segment layer on the wgmma layer kernel (T = 1), output rows padded to a multiple of 8
-  Planes w;
-  float* bias = nullptr; float* scale = nullptr; float* shift = nullptr;
-  int Cin = 0, Cout = 0, Cout_real = 0, flags = 0;
-};
-
 struct Model {   // shared by a handle and its second shard lane
   int feat_dim = 0, layers[4] = {0}, planes[4] = {0}, pre = 0;
   float eps = 0.f;
@@ -59,8 +53,8 @@ struct Model {   // shared by a handle and its second shard lane
   float* head_w = nullptr;
   Bn head_bn;
   std::vector<Block> blocks;
-  std::vector<Seg> seg;
-  int F4 = 0, C4 = 0, E = 0, Cmax = 0, Hmax = 0, seg_mid = 0;
+  SegTail tail;
+  int F4 = 0, C4 = 0, Cmax = 0, Hmax = 0;
   Weights dev{"xvb_resnet_finalize"};
 };
 
@@ -138,12 +132,12 @@ int reserve(xvb_resnet* h, int B, int T) {
   h->free_ws();
   const Model* m = h->m;
   const size_t pooled = (size_t)2 * m->F4 * m->C4, mean = m->Cmax > 256 ? m->Cmax : 256;
-  const size_t out = (size_t)m->seg.back().Cout;
+  const size_t out = (size_t)m->tail.out_rows();
   int rc = XVB_OK;
   for (int i = 0; i < xvb_resnet::kBufs && !rc; ++i) rc = h->planes(&h->buf[i], np);
   if (rc || (rc = h->alloc(&h->last, nl)) || (rc = h->planes(&h->pooled, nb * pooled)) || (rc = h->alloc(&h->pooled_f32, nb * pooled)) ||
       (rc = h->alloc(&h->se_mean, nb * mean)) || (rc = h->alloc(&h->se_hidden, nb * (size_t)(m->Hmax ? m->Hmax : 4))) ||
-      (rc = h->alloc(&h->se_gate, nb * (size_t)m->Cmax)) || (rc = h->planes(&h->seg_mid, nb * (size_t)(m->seg_mid ? m->seg_mid : 8))) ||
+      (rc = h->alloc(&h->se_gate, nb * (size_t)m->Cmax)) || (rc = h->planes(&h->seg_mid, nb * (size_t)(m->tail.mid ? m->tail.mid : 8))) ||
       (rc = h->alloc(&h->seg_out, nb * out))) {
     h->free_ws();
     return rc;
@@ -238,31 +232,7 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
     }
     xi = yi; ai = an; Tl = Tn; Fl = Fn;
   }
-  const int pc = Fl * m->C4;
-  if ((rc = xvb_stats_pool_ex(h->last, pc, B, Tl, pc, m->eps, 0, h->pooled_f32, h->pooled.hi, h->pooled.lo, 2 * pc, stream))) return rc;
-  Planes x = h->pooled;
-  int64_t ldx = 2 * pc;
-  const int ctx0 = 0;
-  for (size_t j = 0; j < m->seg.size(); ++j) {
-    const Seg& s = m->seg[j];
-    const bool fin = j + 1 == m->seg.size();
-    xvb_tdnn_args_t a{};
-    a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
-    a.w_hi = s.w.hi; a.w_lo = s.w.lo;
-    a.bias = s.bias; a.bn_scale = s.scale; a.bn_shift = s.shift;
-    a.flags = s.flags;
-    a.context_host = &ctx0; a.ntaps = 1;
-    if (fin) { a.y_f32 = s.Cout == m->E ? emb : h->seg_out; a.ldyf = s.Cout; }
-    else { a.y_hi = h->seg_mid.hi; a.y_lo = h->seg_mid.lo; a.ldy = s.Cout; }
-    a.B = B; a.T = 1; a.Cin = s.Cin; a.Cout = s.Cout;
-    if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
-    x = h->seg_mid; ldx = s.Cout;
-  }
-  const Seg& s = m->seg.back();
-  if (s.Cout != m->E)
-    XVB_CUDA(cudaMemcpy2DAsync(emb, (size_t)m->E * sizeof(float), h->seg_out, (size_t)s.Cout * sizeof(float), (size_t)m->E * sizeof(float),
-                               (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return XVB_OK;
+  return m->tail.run(h->last, Fl * m->C4, B, Tl, m->eps, h->pooled, h->pooled_f32, h->seg_mid, h->seg_out, emb, stream);
 }
 
 }  // namespace
@@ -381,42 +351,21 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
   m->F4 = f;
   m->C4 = m->planes[3];
   // segment level (resnet_xvector.py:194-206): [fc1 ->] [fc2], as many as the extracted position hands over
-  int cin = 2 * m->F4 * m->C4;
-  for (const char* n : {"fc1", "fc2"}) {
-    const Rec* s = m->recs.find(n);
-    if (!s) continue;
-    rc = need(n, s->shape[0], cin, 1, &s);
-    if (rc) return rc;
-    Seg g;
-    g.Cin = cin; g.Cout_real = s->shape[0]; g.Cout = (s->shape[0] + 7) / 8 * 8;
-    g.flags = (s->flags & XVB_RELU) | (s->s.empty() ? 0 : XVB_BN);
-    std::vector<float> w(s->w), b(s->b), sc(s->s), sh(s->t);
-    w.resize((size_t)g.Cout * cin, 0.f);   // padded output rows come out as exact zeros
-    if (!b.empty()) b.resize(g.Cout, 0.f);
-    if (!sc.empty()) { sc.resize(g.Cout, 0.f); sh.resize(g.Cout, 0.f); }
-    if ((rc = m->dev.pack(&g.w, w, g.Cout, cin, 1, kTaps, 1)) || (rc = m->dev.upload(&g.bias, b)) || (rc = m->dev.upload(&g.scale, sc)) ||
-        (rc = m->dev.upload(&g.shift, sh)))
-      return rc;
-    m->seg.push_back(g);
-    cin = s->shape[0];
-  }
-  XVB_CHECK_ARG(!m->seg.empty(), "xvb_resnet_finalize: record 'fc1' or 'fc2' is missing (no segment layer)");
-  m->E = m->seg.back().Cout_real;
-  m->seg_mid = m->seg.size() > 1 ? m->seg[0].Cout : 0;
+  if ((rc = m->tail.build(m->recs, m->dev, "xvb_resnet_finalize", 2 * m->F4 * m->C4))) return rc;
   if ((rc = m->recs.check_all_used("xvb_resnet_finalize"))) return rc;
   h->finalized = true;
   return XVB_OK;
 }
 
 extern "C" int xvb_resnet_feat_dim(const xvb_resnet_t* h) { return h && h->m ? h->m->feat_dim : XVB_EINVAL; }
-extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return h && h->finalized ? h->m->E : XVB_EINVAL; }
+extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return h && h->finalized ? h->m->tail.E : XVB_EINVAL; }
 extern "C" int xvb_resnet_last_launches(const xvb_resnet_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream) {
   XVB_CHECK_ARG(h && h->finalized, "xvb_resnet_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_resnet_extract: bad arguments");
   const long before = g_launches;
-  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->E;
+  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
   int rc = for_groups(B, (long long)per_utt, kPositionBudget,
                       [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, stream); });
   if (rc) return rc;
@@ -427,7 +376,7 @@ extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, in
 extern "C" int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream) {
   XVB_CHECK_ARG(h && h->finalized && feats_host && emb_host && B > 0 && T > 0, "xvb_resnet_extract_host: bad arguments");
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t nf = (size_t)B * T * h->m->feat_dim, ne = (size_t)B * h->m->E;
+  const size_t nf = (size_t)B * T * h->m->feat_dim, ne = (size_t)B * h->m->tail.E;
   int rc;
   if (nf > h->h_feats_cap) {
     cudaFree(h->h_feats); h->h_feats = nullptr; h->h_feats_cap = 0;
@@ -486,7 +435,7 @@ int lanes_join(xvb_resnet* h, cudaStream_t s) {
 
 extern "C" int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream) {
   XVB_CHECK_ARG(h && h->finalized && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard: bad arguments");
-  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->E;
+  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->tail.E;
   const bool lanes = lanes_enabled() && N > batch;
   int rc, launches = 0, k = 0;
   if (lanes && ((rc = ensure_lanes(h)) || (rc = lanes_fork(h, (cudaStream_t)stream)))) return rc;
@@ -514,7 +463,7 @@ extern "C" int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats
       XVB_CUDA(cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming));
     }
   }
-  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->E;
+  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->tail.E;
   const int bmax = (int)(N < batch ? N : batch);
   const size_t nf = (size_t)bmax * T * F, ne = (size_t)bmax * E;
   int rc;

@@ -15,7 +15,13 @@ and :226-275): the branches are folded at hand-over in float64 (groups expanded 
 every tap whose (Cout, Cin) slab is exactly zero is dropped -- 8 of the 25 taps of a RepSPK block's 5x5 kernel.  stage0
 (Cin = 1) runs on the head conv (xvb_conv2d_head_k), every other block on the tap-list conv (xvb_conv2d_taps) with the
 bias and ReLU in its epilogue; pooling and fc1 / fc2 are the ResNet blueprint's (the reshape before pooling, :191, is
-the same column permutation of the first segment layer)."""
+the same column permutation of the first segment layer).
+
+The launch sequence runs in the native handle (NativeRepVGGExtractor over xvb_repvgg_*, csrc/repvgg_extractor.cu),
+which also writes XVBV0001 model files for bin/xvb-extract.  Python hands it the folded blocks; the library prunes the
+taps by the same rule (xvb_conv2d_kept_taps) and packs.  XVB_REPVGG_NATIVE=0 selects RepVGGExtractor, the Python driver
+of the same kernels in the same order, whose embeddings are bit-identical."""
+import ctypes as C
 import os
 import sys
 
@@ -26,6 +32,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspa
 
 from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200.model.resnet_xvector import _assign, _segment_chain  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
 
@@ -251,7 +258,69 @@ class RepVggXvector(TopVirtualNnet):
             raise ValueError("extracted_embedding='far' needs fc1=True (repvgg_xvector.py:194-196 asserts it)")
         if self.extracted_embedding not in ("far", "near_affine", "near"):
             raise TypeError("Expected far or near position, but got {}".format(self.extracted_embedding))
-        return RepVGGExtractor(self, self.device_for_extraction())
+        dev = self.device_for_extraction()
+        if os.environ.get("XVB_REPVGG_NATIVE", "1") == "0":
+            return RepVGGExtractor(self, dev)       # op-by-op twin of the native handle
+        return NativeRepVGGExtractor(self, dev)
+
+
+def _block_names(m):
+    """The state_dict module path of every block, in m.repvgg.blocks() order."""
+    r = m.repvgg
+    return ["repvgg.stage0"] + ["repvgg.stage{}.{}".format(si, i) for si in range(1, 5)
+                                for i in range(len(getattr(r, "stage{}".format(si))))]
+
+
+def native_config(m):
+    """The fields of xvb_repvgg_config_t for model m."""
+    r = m.repvgg
+    stages = [getattr(r, "stage{}".format(si)) for si in range(1, 5)]
+    return {"feat_dim": m.inputs_dim, "ksize": r.stage0.window, "num_blocks": [len(s) for s in stages],
+            "strides": [r.stage0.stride] + [s[0].stride for s in stages],
+            "widths": [r.stage0.out_channels] + [s[0].out_channels for s in stages], "pooling_eps": float(m.stats.eps)}
+
+
+def _named_records(m):
+    """(name, w, bias, scale, shift, relu) records for xvb_repvgg_set_layer, named by block module path: every block
+    as its fold_block kernel (Cout, Cin, k, k) and bias cast to fp32 -- the arrays RepVGGExtractor packs -- with its ReLU,
+    then the segment layers of _segment_chain with their (Cout, Cin, 1) weight as (Cout, Cin), as the ResNet hands them
+    over.  The library prunes the taps and packs."""
+    f = lambda t: t.detach().float().cpu().numpy()  # noqa: E731
+    out = []
+    for name, blk in zip(_block_names(m), m.repvgg.blocks()):
+        w, b = fold_block(blk)
+        out.append((name, f(w), f(b), None, None, True))
+    for name, _, w, b, scale, shift, relu in _segment_chain(m, m.repvgg.get_output_planes()):
+        out.append((name, f(w)[:, :, 0], f(b) if b is not None else None, scale, shift, relu))
+    return out
+
+
+class NativeRepVGGExtractor(NativeExtractor):
+    """xvb_repvgg_t: folded weights, workspace and the whole launch sequence of RepVGGExtractor in the C library, on the
+    device that is current when it is built (or loaded from an XVBV0001 file)."""
+
+    PREFIX = "repvgg"
+
+    def _create_args(self, m):
+        from asv_subtools_b200._lib import RepVGGConfig
+        c = native_config(m)
+        cfg = RepVGGConfig(feat_dim=c["feat_dim"], ksize=c["ksize"], pooling_eps=c["pooling_eps"])
+        for field in ("num_blocks", "strides", "widths"):
+            getattr(cfg, field)[:] = c[field]
+        return (C.byref(cfg),)
+
+    def _layers(self, m):
+        for name, w, b, scale, shift, relu in _named_records(m):
+            yield name, (w.shape[0], w.shape[1], w.shape[2] if w.ndim == 4 else 1), (w, b, scale, shift), \
+                (1 if relu else 0) | (2 if scale is not None else 0)
+
+    def _input(self, feats):
+        """Any (B, T, F) CUDA float32 tensor, made contiguous as RepVGGExtractor.extract does."""
+        if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.dim() == 3):
+            raise TypeError("feats must be a (B, T, F) CUDA float32 tensor")
+        if feats.shape[2] != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
+        return feats.contiguous()
 
 
 class RepVGGExtractor:

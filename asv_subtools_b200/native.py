@@ -1,6 +1,7 @@
 """Python handles over the native whole-model extractors of the C library that take named records: the ResNet
-(xvb_resnet_*), Conformer (xvb_conformer_*) and CAM++ (xvb_campp_*) x-vectors.  NativeExtractor holds the part they
-share: create, set_layer per record and finalize (or load a model file), save, extract and close."""
+(xvb_resnet_*), RepVGG / RepSPK (xvb_repvgg_*), Conformer (xvb_conformer_*) and CAM++ (xvb_campp_*) x-vectors.
+NativeExtractor holds the part they share: create, set_layer per record and finalize (or load a model file), save,
+extract and close."""
 import ctypes as C
 
 import numpy as np

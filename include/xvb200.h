@@ -765,6 +765,62 @@ int xvb_resnet_load(xvb_resnet_t** out, const char* path);
 void xvb_resnet_destroy(xvb_resnet_t* h);
 
 /* ---------------------------------------------------------------------------------------------
+ * Whole-model extractor for the RepVGG / RepSPK x-vector (pytorch/model/repvgg_xvector.py, extract_embedding :181-208
+ * over pytorch/libs/nnet/repvgg.py): the launch sequence of xvb_conv2d_head[_k], xvb_conv2d_taps, xvb_stats_pool_ex and
+ * xvb_tdnn_affine_ex in C++, with weights and workspace owned by the handle.  Bit-identical to the op-by-op Python
+ * driver of the same kernels (RepVGGExtractor, XVB_REPVGG_NATIVE=0).
+ *
+ * Every block is one convolution with a bias and ReLU.  Records are named by block module path and arrive folded:
+ *   "repvgg.stage0", "repvgg.stageS.I"   Cout x Cin x k: w (Cout, Cin, k, k) the block's equivalent kernel (branches
+ *                                        folded in float64, groups expanded block-diagonally, then cast to fp32), bias
+ *                                        the folded bias, flags XVB_RELU; stage0 has Cin = 1.  Training-form and
+ *                                        deploy-form checkpoints give the same records.
+ *   "fc1", "fc2"                         as for xvb_resnet_set_layer: the ones the extracted position uses, ksize 1,
+ *                                        the first one's input columns in the pooling order of (B, T', F', C) frames.
+ * Finalize drops every tap whose (Cout, Cin) slab of a block's kernel is exactly zero (xvb_conv2d_kept_taps: 17 of the
+ * 25 taps of a RepSPK block) and packs the rest.  stage0 runs on xvb_conv2d_head (k = 3) or xvb_conv2d_head_k (k = 5)
+ * with scale 1 and shift = the bias, every other block on xvb_conv2d_taps with the same epilogue (the last block writes
+ * fp32 only).
+ *
+ * Workspace: grown to the largest (B, T) seen, then reused: two ping-pong (B, T', F', C) plane pairs, the last block's
+ * fp32 output, the pooled statistics and the segment layers.  A call whose B*T*feat_dim exceeds 256*200*80 positions
+ * runs as consecutive groups of max(1, floor(256*200*80 / (T*feat_dim))) utterances.  The launcher's model (RepSPK,
+ * base width 32) at B = 128, T = 200, feat_dim = 80 needs about 0.6 GB: 262 MB per plane pair at stage0 / stage1 widths
+ * and 82 MB of fp32 for stage4's output.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct xvb_repvgg_config {
+  int feat_dim;
+  int ksize;             /* 3: RepVGG blocks, 5: RepSPK blocks */
+  int num_blocks[4];     /* blocks of stage1 .. stage4 (stage0 is one block) */
+  int strides[5];        /* stage0 .. stage4, 1 or 2; stage0 1 (the head conv) */
+  int widths[5];         /* output channels of stage0 .. stage4, multiples of 16 */
+  float pooling_eps;
+} xvb_repvgg_config_t;
+typedef struct xvb_repvgg xvb_repvgg_t;
+/* Refuses a configuration outside the bounds above, naming the field. */
+int xvb_repvgg_create(xvb_repvgg_t** out, const xvb_repvgg_config_t* cfg);
+int xvb_repvgg_set_layer(xvb_repvgg_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
+                         const float* bias_host, const float* scale_host, const float* shift_host, int flags);
+/* Checks that every record the configuration needs is present with its shape (and nothing else), names the one that
+ * is not, then prunes the taps and packs the weights on the current device. */
+int xvb_repvgg_finalize(xvb_repvgg_t* h);
+int xvb_repvgg_feat_dim(const xvb_repvgg_t* h);
+int xvb_repvgg_embed_dim(const xvb_repvgg_t* h);
+/* Kernels launched by the last extract call. */
+int xvb_repvgg_last_launches(const xvb_repvgg_t* h);
+/* feats (B, T, feat_dim) fp32 on the device -> emb (B, embed_dim) fp32 on the device; asynchronous on `stream`. */
+int xvb_repvgg_extract(xvb_repvgg_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* "XVBV0001" model files: the configuration, then the records as handed to xvb_repvgg_set_layer (layout at
+ * save_records in csrc/model_file.cpp). */
+int xvb_repvgg_save(const xvb_repvgg_t* h, const char* path);
+int xvb_repvgg_load(xvb_repvgg_t** out, const char* path);
+void xvb_repvgg_destroy(xvb_repvgg_t* h);
+/* Host only, no GPU: the taps kf*k + kt of a (Cout, Cin, k, k) fp32 kernel whose (Cout, Cin) slab is not all zero, in
+ * increasing order, or the centre tap alone when every slab is zero.  Writes them to taps[0..n) and returns n, or
+ * XVB_EINVAL on a null pointer, a non-positive size or cap < n. */
+int xvb_conv2d_kept_taps(const float* w, int Cout, int Cin, int k, int* taps, int cap);
+
+/* ---------------------------------------------------------------------------------------------
  * Whole-model extractor for the Conformer x-vector (pytorch/model/transformer_xvector.py, extract_embedding :321-346,
  * Conformer encoder with 4x (input_layer "conv2d") or 2x ("conv2d2") subsampling): the launch sequence of
  * xvb_subsample_head[_stride], xvb_conv2d_valid, xvb_tdnn_affine_ex, xvb_layer_norm, xvb_rope_attention,
