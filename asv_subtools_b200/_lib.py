@@ -21,7 +21,8 @@ class TdnnArgs(C.Structure):
                 ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("ldy", C.c_int64),
                 ("y_f32", C.c_void_p), ("ldyf", C.c_int64),
                 ("B", C.c_int), ("T", C.c_int), ("Cin", C.c_int), ("Cout", C.c_int),
-                ("pool_partial", C.c_void_p), ("x_batch_stride", C.c_int64), ("groups", C.c_int)]
+                ("pool_partial", C.c_void_p), ("x_batch_stride", C.c_int64), ("groups", C.c_int),
+                ("lengths", C.c_void_p)]
 MAX_TAPS = 16
 
 
@@ -106,6 +107,7 @@ SIGNATURES = {
     "xvb_split_frames": (_i, [_p, _i, _i, _i, _p, _p, _i64, _i, _i, _p]),
     "xvb_pool_partial_blocks": (_i, [_i, _i, _ip]),
     "xvb_pool_finalize": (_i, [_p, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
+    "xvb_stats_pool_lengths": (_i, [_p, _i64, _i, _i, _i, _f, _i, _p, _p, _p, _p, _i64, _p]),
     "xvb_extractor_set_fused_pooling": (_i, [_p, _i]),
     "xvb_plane_mean": (_i, [_p, _p, _i64, _i, _i, _i, _p, _p, _p, _i64, _p]),
     "xvb_res2net_block": (_i, [_p, _p, _i64, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _i, _i, _p]),
@@ -169,6 +171,7 @@ SIGNATURES = {
     "xvb_extractor_finalize": (_i, [_p, _f]),
     "xvb_extractor_embed_dim": (_i, [_p]),
     "xvb_extractor_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_extractor_extract_lengths": (_i, [_p, _p, _p, _i, _i, _p, _p]),
     "xvb_extractor_extract_host": (_i, [_p, _p, _i, _i, _p, _p]),
     "xvb_extractor_submit_host": (_i, [_p, _p, _i, _i, _p, _i, _p]),
     "xvb_extractor_wait": (_i, [_p, _i]),

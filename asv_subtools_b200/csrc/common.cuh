@@ -125,6 +125,14 @@ int gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& args, const TrialHist
 int gemm_plan_launch(const GemmPlan* plan, void* stream, float* y_f32_override = nullptr);
 void gemm_plan_destroy(GemmPlan* plan);
 
+// pooling.cu: xvb_stats_pool_ex / xvb_stats_pool_lengths; `lengths` (device int32[B]) may be NULL (every utterance T
+// frames long).
+int stats_pool(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, const int* lengths, float* out,
+               uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
+// core.cu: xvb_split_frames with the frames past lengths[b] (device int32[B], may be NULL) written as zeros.
+int split_frames(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front, int pad_back,
+                 const int* lengths, void* stream);
+
 // tdnn_gemm.cu: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda).
 int make_tensor_map(CUtensorMap* m, const void* base, int esize, int rank, const unsigned long long* dims,
                     const unsigned long long* strides_bytes, const unsigned* box, int swizzle_bytes);

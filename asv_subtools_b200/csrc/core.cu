@@ -82,9 +82,11 @@ __global__ void split_f32_kernel(const float* __restrict__ x, long long rows, in
 }
 
 // (B, T, C) fp32 frames -> planes (B, pad_front + T + pad_back, ldp) with zero frames around each
-// utterance.  One thread per 8 output columns; float4 loads when the source rows allow it.
+// utterance.  One thread per 8 output columns; float4 loads when the source rows allow it.  A masked batch
+// (lengths != NULL) also writes zeros for the frames t >= lengths[b], which are never read.
 __global__ void split_frames_kernel(const float* __restrict__ x, int B, int T, int C, __nv_bfloat16* __restrict__ hi,
-                                    __nv_bfloat16* __restrict__ lo, long long ldp, int pad_front, int Tp, int vec) {
+                                    __nv_bfloat16* __restrict__ lo, long long ldp, int pad_front, int Tp, int vec,
+                                    const int* __restrict__ lengths) {
   const long long groups_per_row = ldp / 8;
   const long long total = (long long)B * Tp * groups_per_row;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -94,7 +96,7 @@ __global__ void split_frames_kernel(const float* __restrict__ x, int B, int T, i
     float v[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) v[k] = 0.f;
-    if (t >= 0 && t < T) {
+    if (t >= 0 && t < (lengths ? lengths[b] : T)) {
       const float* src = x + ((long long)b * T + t) * C + c0;
       if (vec && c0 + 8 <= C) {
         const float4 a = *reinterpret_cast<const float4*>(src), c = *reinterpret_cast<const float4*>(src + 4);
@@ -201,6 +203,11 @@ extern "C" int xvb_split_f32(const float* x, int64_t rows, int C, int64_t ldx, u
 
 extern "C" int xvb_split_frames(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front,
                                 int pad_back, void* stream) {
+  return split_frames(x, B, T, C, hi, lo, ldp, pad_front, pad_back, nullptr, stream);
+}
+
+int xvb::split_frames(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front, int pad_back,
+                      const int* lengths, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(x && hi && lo && B > 0 && T > 0 && C > 0 && ldp >= C && ldp % 8 == 0 && pad_front >= 0 && pad_back >= 0,
@@ -210,7 +217,7 @@ extern "C" int xvb_split_frames(const float* x, int B, int T, int C, uint16_t* h
   const long long total = (long long)B * Tp * (ldp / 8);
   const int vec = (C % 4 == 0 && (uintptr_t)x % 16 == 0) ? 1 : 0;
   split_frames_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      x, B, T, C, reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), ldp, pad_front, Tp, vec);
+      x, B, T, C, reinterpret_cast<__nv_bfloat16*>(hi), reinterpret_cast<__nv_bfloat16*>(lo), ldp, pad_front, Tp, vec, lengths);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
 }

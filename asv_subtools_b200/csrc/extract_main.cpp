@@ -1,7 +1,7 @@
 // xvb-extract: Python-free x-vector extraction over the C ABI (SURVEY section 8f rank 4).
 //
 //   xvb-extract [--batch N] [--max-chunk N] [--cmn none|utt|sliding] [--cmn-window W] [--gpu-id ID]
-//               [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]
+//               [--mixed-lengths] [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]
 //                [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]
 //               <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>
 //
@@ -18,7 +18,9 @@
 // (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), the last four written by the native extractors' save().  What it adds:
-// utterances of equal length are batched (the reference runs batch 1).
+// utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector files
+// only) chunks of different lengths share masked batches (plan_mixed_batches, xvb_extractor_extract_lengths), which
+// fills batches on a real corpus where most frame counts occur a few times only.
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
@@ -33,6 +35,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <string>
 #include <vector>
@@ -75,6 +78,8 @@ struct Family {
   void (*destroy)(void* h);
   int max_chunk;
   bool campp_chunks;       // egrecho's split_chunks(even=False) through xvb_campp_chunk_sizes
+  // masked batch of different lengths (host lengths), or nullptr: the family batches equal lengths only
+  int (*extract_lengths)(void* h, const float* feats, const int32_t* lengths, int B, int T, float* emb);
 };
 
 // the entry points of a family whose C API is xvb_<p>_load / _feat_dim / _embed_dim / _extract / _destroy on xvb_<p>_t
@@ -86,18 +91,21 @@ struct Family {
   [](void* h) { xvb_##p##_destroy((xvb_##p##_t*)h); }
 
 const Family kFamilies[] = {
-    {{"XVBE0001", "XVBE0002"}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false},
-    {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false},
-    {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false},
-    {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false},
-    {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true},
+    {{"XVBE0001", "XVBE0002"}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false, nullptr},
+    {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false, nullptr},
+    {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false, nullptr},
+    {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false, nullptr},
+    {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true, nullptr},
     // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
     {{nullptr, nullptr}, "loading the model", "xvb_extractor_extract",
      [](void** h, const char* path) { return xvb_extractor_load((xvb_extractor_t**)h, path); },
      [](const void*, const char* path) { return xvb_extractor_feat_dim(path); },
      [](const void* h) { return xvb_extractor_embed_dim((const xvb_extractor_t*)h); },
      [](void* h, const float* x, int B, int T, float* e) { return xvb_extractor_extract((xvb_extractor_t*)h, x, B, T, e, nullptr); },
-     [](void* h) { xvb_extractor_destroy((xvb_extractor_t*)h); }, 10000, false},
+     [](void* h) { xvb_extractor_destroy((xvb_extractor_t*)h); }, 10000, false,
+     [](void* h, const float* x, const int32_t* lens, int B, int T, float* e) {
+       return xvb_extractor_extract_lengths((xvb_extractor_t*)h, x, lens, B, T, e, nullptr);
+     }},
 };
 
 const Family& family_of(const char (&magic)[8]) {
@@ -105,6 +113,30 @@ const Family& family_of(const char (&magic)[8]) {
     for (const char* m : f.magic)
       if (m && memcmp(magic, m, 8) == 0) return f;
   return kFamilies[sizeof kFamilies / sizeof kFamilies[0] - 1];
+}
+
+// The batch rule of --mixed-lengths (pipeline/extract_embeddings.py plan_mixed_batches is the same rule): items in
+// ascending length (ties in arrival order), each batch up to `batch` consecutive items whose padded frames
+// n * max(len) - sum(len) are at most 1/8 of n * max(len).  Returns index lists into `lens`.  Equal lengths give the
+// equal-length buckets: runs of `batch` items in arrival order, then the remainder.
+std::vector<std::vector<int>> plan_mixed_batches(const std::vector<int>& lens, int batch) {
+  std::vector<int> order(lens.size());
+  for (size_t i = 0; i < order.size(); ++i) order[i] = (int)i;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return lens[a] < lens[b]; });
+  std::vector<std::vector<int>> out;
+  for (size_t i = 0; i < order.size();) {
+    size_t j = i + 1;
+    long long total = lens[order[i]];
+    while (j < order.size() && (long long)(j - i) < batch) {
+      const long long n = (long long)(j - i + 1), tmax = lens[order[j]];
+      if (8 * (n * tmax - (total + tmax)) > n * tmax) break;
+      total += tmax;
+      ++j;
+    }
+    out.emplace_back(order.begin() + i, order.begin() + j);
+    i = j;
+  }
+  return out;
 }
 
 struct Runner {
@@ -117,6 +149,8 @@ struct Runner {
   size_t cap_frames = 0;
   std::vector<Utt> utts;
   long done_utts = 0, done_frames = 0;
+  long mixed_batches = 0, padded_frames = 0, batch_frames = 0;   // --mixed-lengths summary
+  std::vector<int32_t> lens;
 
   void reserve(size_t frames) {
     if (frames <= cap_frames) return;
@@ -135,11 +169,45 @@ struct Runner {
 
   void run(std::vector<Item>& items) {
     if (items.empty()) return;
-    const int B = (int)items.size(), T = items[0].frames;
+    run_batch(items);
+    items.clear();
+  }
+
+  // --mixed-lengths: everything pending, as masked batches of the batch rule
+  void run_mixed(std::vector<Item>& items) {
+    std::vector<int> len(items.size());
+    for (size_t i = 0; i < items.size(); ++i) len[i] = items[i].frames;
+    for (const std::vector<int>& idx : plan_mixed_batches(len, batch)) {
+      std::vector<Item> b;
+      for (int i : idx) b.push_back(std::move(items[i]));
+      run_batch(b, true);
+    }
+    items.clear();
+  }
+
+  // one batch: equal lengths, or (masked) padded to the longest with the frames past each item's end zeroed
+  void run_batch(std::vector<Item>& items, bool masked = false) {
+    const int B = (int)items.size();
+    int T = 0;
+    long frames = 0;
+    for (const Item& it : items) { T = std::max(T, it.frames); frames += it.frames; }
     reserve((size_t)B * T);
-    for (int i = 0; i < B; ++i) memcpy(h_feats + (size_t)i * T * F, items[i].feats.data(), (size_t)T * F * sizeof(float));
+    lens.resize(B);
+    for (int i = 0; i < B; ++i) {
+      float* dst = h_feats + (size_t)i * T * F;
+      memcpy(dst, items[i].feats.data(), (size_t)items[i].frames * F * sizeof(float));
+      memset(dst + (size_t)items[i].frames * F, 0, (size_t)(T - items[i].frames) * F * sizeof(float));
+      lens[i] = items[i].frames;
+    }
     CU(cudaMemcpy(d_feats, h_feats, (size_t)B * T * F * sizeof(float), cudaMemcpyHostToDevice));
-    CK(fam->extract(model, d_feats, B, T, d_emb), fam->extract_fn);
+    if (masked) {
+      CK(fam->extract_lengths(model, d_feats, lens.data(), B, T, d_emb), "xvb_extractor_extract_lengths");
+      ++mixed_batches;
+      padded_frames += (long)B * T - frames;
+      batch_frames += (long)B * T;
+    } else {
+      CK(fam->extract(model, d_feats, B, T, d_emb), fam->extract_fn);
+    }
     CU(cudaMemcpy(h_emb, d_emb, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToHost));
     for (int i = 0; i < B; ++i) {
       Utt& u = utts[items[i].utt];
@@ -156,7 +224,6 @@ struct Runner {
         done_frames += u.frames;
       }
     }
-    items.clear();
   }
 };
 
@@ -202,7 +269,7 @@ bool read_wav(const std::string& path, std::vector<float>* out, int* sample_rate
 int main(int argc, char** argv) {
   Runner r;
   int max_chunk = 10000, gpu = 0;
-  bool max_chunk_set = false;
+  bool max_chunk_set = false, mixed = false;
   std::string wav_type;
   xvb_fbank_opts_t fo;
   xvb_fbank_default_opts(&fo);
@@ -227,13 +294,14 @@ int main(int argc, char** argv) {
     else if (a == "--frame-shift") fo.frame_shift_ms = (float)atof(val("--frame-shift"));
     else if (a == "--energy-floor") fo.energy_floor = (float)atof(val("--energy-floor"));
     else if (a == "--use-energy") fo.use_energy = 1;
+    else if (a == "--mixed-lengths") mixed = true;
     else if (a == "--cmn") {
       const std::string m = val("--cmn");
       r.cmn = m == "none" ? 0 : m == "utt" ? 1 : m == "sliding" ? 2 : -1;
       if (r.cmn < 0) { fprintf(stderr, "ERROR: xvb-extract: --cmn must be none, utt or sliding\n"); return 1; }
     } else if (a == "--help" || a == "-h") {
       printf("usage: xvb-extract [--batch N] [--max-chunk N] [--cmn none|utt|sliding] [--cmn-window W] [--gpu-id ID]\n"
-             "                   [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
+             "                   [--mixed-lengths] [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
              "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001),\n"
@@ -241,7 +309,10 @@ int main(int argc, char** argv) {
              "recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the model's own chunk rule),\n"
              "4000 for CAM++ and 10000 otherwise.  A Conformer chunk needs at least 7 frames and fewer than 5000 subsampled\n"
              "frames.  CAM++ cuts an utterance with egrecho's rule (max-chunk-long chunks, the last two re-split evenly:\n"
-             "9000 -> 4000, 2500, 2500); a chunk needs at least 3 frames.\n");
+             "9000 -> 4000, 2500, 2500); a chunk needs at least 3 frames.\n"
+             "--mixed-lengths (TDNN x-vector models): after the chunk rule, chunks of different lengths share batches of up\n"
+             "to --batch, taken in ascending length, with at most 1/8 of a batch's frames padding; the summary line also\n"
+             "reports the padded frames.  Vectors differ from the default mode's at the rounding level.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -267,6 +338,11 @@ int main(int argc, char** argv) {
     r.F = r.fam->feat_dim(r.model, pos[0]);
     r.D = r.fam->embed_dim(r.model);
     if (!max_chunk_set) max_chunk = r.fam->max_chunk;
+    if (mixed && !r.fam->extract_lengths) {
+      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector model (XVBM0001); '%s' is read with %s\n", pos[0],
+              r.fam->extract_fn);
+      return 1;
+    }
   }
   xvb_ark_reader_t* in = nullptr;
   FILE* wav_scp = nullptr;
@@ -326,6 +402,7 @@ int main(int argc, char** argv) {
   const std::string wspec = pos[2];
   const bool to_stdout = wspec == "-" || (wspec.size() >= 2 && wspec.compare(wspec.size() - 2, 2, ":-") == 0);   // keep the ark stream clean
   std::map<int, std::vector<Item>> buckets;   // frames -> pending chunks of that length
+  std::vector<Item> mixed_items;              // --mixed-lengths: every pending chunk
   size_t pending = 0;
   const size_t max_pending = (size_t)r.batch * 64;
   const char* key;
@@ -369,10 +446,19 @@ int main(int argc, char** argv) {
       it.frames = len;
       it.feats.assign(data + (size_t)off * cols, data + (size_t)(off + len) * cols);
       off += len;
+      if (mixed) {
+        mixed_items.push_back(std::move(it));
+        ++pending;
+        continue;
+      }
       std::vector<Item>& b = buckets[len];
       b.push_back(std::move(it));
       ++pending;
       if ((int)b.size() == r.batch) { pending -= b.size(); r.run(b); }
+    }
+    if (mixed && pending > max_pending) {   // bound host memory: run everything pending
+      r.run_mixed(mixed_items);
+      pending = 0;
     }
     if (pending > max_pending) {   // bound host memory: flush the fullest bucket
       auto best = buckets.begin();
@@ -384,11 +470,17 @@ int main(int argc, char** argv) {
   }
   if (rc < 0) die("reading features");
   for (auto& kv : buckets) r.run(kv.second);
+  r.run_mixed(mixed_items);
   if (in) xvb_ark_reader_close(in);
   if (wav_scp) fclose(wav_scp);
   if (fb) xvb_fbank_destroy(fb);
   CK(xvb_ark_writer_close(r.out), "closing the vector wspecifier");
   r.fam->destroy(r.model);
-  fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
+  if (mixed)
+    fprintf(stderr, "xvb-extract: %ld utterances, %ld frames, %ld masked batches, %ld padded frames (%.4f of %ld batch frames)\n",
+            r.done_utts, r.done_frames, r.mixed_batches, r.padded_frames,
+            r.batch_frames ? (double)r.padded_frames / (double)r.batch_frames : 0.0, r.batch_frames);
+  else
+    fprintf(stderr, "xvb-extract: %ld utterances, %ld frames\n", r.done_utts, r.done_frames);
   return 0;
 }

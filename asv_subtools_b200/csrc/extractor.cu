@@ -7,7 +7,7 @@
 #include <stdlib.h>
 
 #include <map>
-#include <utility>
+#include <tuple>
 #include <vector>
 
 #include "common.cuh"
@@ -84,8 +84,12 @@ struct xvb_extractor {
   int pad_front = 0, pad_back = 0;
   float* pool_partial = nullptr;
   size_t pool_partial_cap = 0;
-  // launch plans per batch shape; they hold pointers into the workspace, so anything that reallocates it clears them
-  std::map<std::pair<int, int>, StepPlan*> plans;
+  // per-utterance frame counts of the last masked call (xvb_extractor_extract_lengths), on the device
+  int* d_lengths = nullptr;
+  int d_lengths_cap = 0;
+  // launch plans per batch shape (B, T, masked); they hold pointers into the workspace (and, masked, into d_lengths),
+  // so anything that reallocates either clears them
+  std::map<std::tuple<int, int, bool>, StepPlan*> plans;
   void drop_plans() {
     for (auto& kv : plans) delete kv.second;
     plans.clear();
@@ -269,7 +273,11 @@ static int reserve(xvb_extractor* h, int B, int T) {
 }
 
 // Build the launch plan of one batch shape (see StepPlan).  On failure nothing is cached.
-static int build_step_plan(xvb_extractor* h, int B, int T, StepPlan** out) {
+// A masked plan (utterances of different lengths) passes the extractor's device lengths to every frame layer, whose
+// epilogue then zeroes the frames past each utterance's end, and always keeps the last layer's fp32 output for the
+// length-aware standalone pooling (the fused pooling epilogue takes equal lengths only); the segment layers see one row
+// per utterance either way.
+static int build_step_plan(xvb_extractor* h, int B, int T, bool masked, StepPlan** out) {
   StepPlan* sp = new StepPlan();
   struct Guard { StepPlan* p; ~Guard() { delete p; } } guard{sp};
   int rc;
@@ -301,12 +309,13 @@ static int build_step_plan(xvb_extractor* h, int B, int T, StepPlan** out) {
     a.context_host = L.ctx; a.ntaps = L.ntaps;
     a.y_hi = y_hi; a.y_lo = y_lo; a.ldy = L.Cout;
     a.B = B; a.T = T; a.Cin = L.Cin; a.Cout = L.Cout;
+    a.lengths = masked ? h->d_lengths : nullptr;
     const int ctx0 = 0;
     if (i == 0 && h->im2col_first) {   // window of ntaps consecutive frames = one long row of the padded planes
       a.context_host = &ctx0; a.ntaps = 1; a.Cin = L.ntaps * L.Cin;
       a.x_batch_stride = (int64_t)(T + h->pad_front + h->pad_back) * ldx;
     }
-    if (last && h->fused_pooling) {
+    if (last && h->fused_pooling && !masked) {
       a.pool_partial = h->pool_partial;
     } else if (last) {
       a.y_f32 = h->last_f32; a.ldyf = L.Cout;
@@ -338,9 +347,8 @@ static int build_step_plan(xvb_extractor* h, int B, int T, StepPlan** out) {
   return XVB_OK;
 }
 
-extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized, "xvb_extractor_extract: extractor not finalized");
-  XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_extractor_extract: bad arguments");
+// One batch through the stack.  masked: h->d_lengths already holds the B utterance lengths (stream-ordered on `stream`).
+static int extract_batch(xvb_extractor* h, const float* feats, int B, int T, bool masked, float* emb, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
   const long before = g_launches;
@@ -348,11 +356,12 @@ extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int
   if (!h->in_shard) h->events_used = 0;   // a shard call keeps the events of all its batches
   h->events_stream = cs;
   StepPlan* sp = nullptr;
-  auto it = h->plans.find(std::make_pair(B, T));
+  const auto key = std::make_tuple(B, T, masked);
+  auto it = h->plans.find(key);
   if (it != h->plans.end()) {
     sp = it->second;
   } else {
-    if (h->fused_pooling) {   // partials of the fused pooling epilogue: (time blocks, B, 2C) fp32
+    if (h->fused_pooling && !masked) {   // partials of the fused pooling epilogue: (time blocks, B, 2C) fp32
       int tb = 0;
       const size_t need = (size_t)xvb_pool_partial_blocks(B, T, &tb) * B * 2 * h->frame.back().Cout;
       if (need > h->pool_partial_cap) {
@@ -363,21 +372,23 @@ extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int
         h->pool_partial_cap = need;
       }
     }
-    rc = build_step_plan(h, B, T, &sp);
+    rc = build_step_plan(h, B, T, masked, &sp);
     if (rc == -1000) {        // the driver refused the overlapping (im2col) tensor map: plain first layer from now on
       h->im2col_first = false;
       h->pad_front = h->pad_back = 0;
       h->drop_plans();
-      return xvb_extractor_extract(h, feats, B, T, emb, stream);
+      return extract_batch(h, feats, B, T, masked, emb, stream);
     }
     if (rc) return rc;
-    h->plans[std::make_pair(B, T)] = sp;
+    h->plans[key] = sp;
   }
   if ((rc = h->mark(cs))) return rc;
   // 1. stage the frame matrix as split planes (framework.py:28-33 staging); for the im2col first layer with
-  //    the zero frames of F.pad (components.py:117) written out around every utterance
-  if (h->im2col_first)
-    rc = xvb_split_frames(feats, B, T, h->feat_dim, h->in_hi, h->in_lo, h->ldf, h->pad_front, h->pad_back, stream);
+  //    the zero frames of F.pad (components.py:117) written out around every utterance; a masked batch also writes
+  //    zeros for every frame past an utterance's end, so no layer ever reads what the caller left there
+  const int* lens = masked ? h->d_lengths : nullptr;
+  if (h->im2col_first || masked)
+    rc = split_frames(feats, B, T, h->feat_dim, h->in_hi, h->in_lo, h->ldf, h->pad_front, h->pad_back, lens, stream);
   else
     rc = xvb_split_f32(feats, (int64_t)B * T, h->feat_dim, h->feat_dim, h->in_hi, h->in_lo, h->ldf, stream);
   if (rc) return rc;
@@ -389,11 +400,11 @@ extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int
   }
   // 3. statistics pooling (xvector.py:90, pooling.py:58-67)
   const int cl = h->frame.back().Cout;
-  if (h->fused_pooling)
+  if (h->fused_pooling && !masked)
     rc = xvb_pool_finalize(h->pool_partial, sp->pool_blocks, sp->pool_tb, B, T, cl, h->pooling_eps, 0, h->stats, h->stats_hi,
                            h->stats_lo, 2 * cl, stream);
   else
-    rc = xvb_stats_pool(h->last_f32, cl, B, T, cl, h->pooling_eps, h->stats, h->stats_hi, h->stats_lo, 2 * cl, stream);
+    rc = stats_pool(h->last_f32, cl, B, T, cl, h->pooling_eps, 0, lens, h->stats, h->stats_hi, h->stats_lo, 2 * cl, stream);
   if (rc) return rc;
   if ((rc = h->mark(cs))) return rc;
   // 4. segment-level layers (xvector.py:92-96); the last one writes the caller's embedding matrix
@@ -404,6 +415,38 @@ extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int
   }
   h->last_launches = (int)(g_launches - before);
   return XVB_OK;
+}
+
+extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int B, int T, float* emb, void* stream) {
+  XVB_CHECK_ARG(h && h->finalized, "xvb_extractor_extract: extractor not finalized");
+  XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_extractor_extract: bad arguments");
+  return extract_batch(h, feats, B, T, false, emb, stream);
+}
+
+extern "C" int xvb_extractor_extract_lengths(xvb_extractor_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
+                                             float* emb, void* stream) {
+  XVB_CHECK_ARG(h && h->finalized, "xvb_extractor_extract_lengths: extractor not finalized");
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "xvb_extractor_extract_lengths: bad arguments");
+  bool all_T = true;
+  for (int b = 0; b < B; ++b) {
+    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "xvb_extractor_extract_lengths: lengths[%d]=%d outside [1, T=%d]", b,
+                  (int)lengths_host[b], T);
+    all_T = all_T && lengths_host[b] == T;
+  }
+  if (all_T) return extract_batch(h, feats, B, T, false, emb, stream);   // nothing to mask: the unmasked call itself
+  if (B > h->d_lengths_cap) {
+    h->drop_plans();          // the masked ones point at the old buffer
+    cudaFree(h->d_lengths);
+    h->d_lengths = nullptr; h->d_lengths_cap = 0;
+    const int cap = B > h->cap_B ? B : h->cap_B;
+    int rc = dev_alloc(&h->d_lengths, (size_t)cap);
+    if (rc) return rc;
+    h->d_lengths_cap = cap;
+  }
+  // stream-ordered: the previous call's kernels on `stream` have read the old lengths before these land
+  XVB_CUDA(cudaMemcpyAsync(h->d_lengths, lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice,
+                           (cudaStream_t)stream));
+  return extract_batch(h, feats, B, T, true, emb, stream);
 }
 
 extern "C" int xvb_extractor_set_gather(xvb_extractor_t* h, float* const* tables, int ntables, int64_t row0, int64_t ld) {
@@ -676,7 +719,7 @@ extern "C" void xvb_extractor_destroy(xvb_extractor_t* h) {
     if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]);
   }
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  cudaFree(h->h_feats); cudaFree(h->h_emb); cudaFree(h->pool_partial);
+  cudaFree(h->h_feats); cudaFree(h->h_emb); cudaFree(h->pool_partial); cudaFree(h->d_lengths);
   if (!h->is_lane)
     for (auto* v : {&h->frame, &h->segment})
       for (Layer& L : *v) { cudaFree(L.w_hi); cudaFree(L.w_lo); cudaFree(L.bias); cudaFree(L.scale); cudaFree(L.shift); }

@@ -25,7 +25,8 @@ constexpr int kPoolNumBars = (kPoolSlabRows + kPoolBoxRows - 1) / kPoolBoxRows;
 constexpr int kPoolSmemBytes = kPoolNumBars * kPoolBoxRows * 128 * 4 + kPoolWarps * 128 * 4 + 128 + 128 /* alignment slack */;
 
 __global__ void __launch_bounds__(kPoolWarps * 32, 2)
-stats_pool_tma_kernel(const __grid_constant__ CUtensorMap map_x, int T, int C, float eps, int mode, float* __restrict__ out,
+stats_pool_tma_kernel(const __grid_constant__ CUtensorMap map_x, int T_all, int C, float eps, int mode,
+                      const int* __restrict__ lengths, float* __restrict__ out,
                       __nv_bfloat16* __restrict__ out_hi, __nv_bfloat16* __restrict__ out_lo, long long ldo) {
   // TMA destinations need 128-byte alignment; CUDA only promises 16 for dynamic shared memory (and a tool that adds
   // its own static shared memory, e.g. compute-sanitizer, does shift the base), so align by hand
@@ -36,6 +37,7 @@ stats_pool_tma_kernel(const __grid_constant__ CUtensorMap map_x, int T, int C, f
   uint64_t* bars = reinterpret_cast<uint64_t*>(scratch + kPoolWarps * 128);           // [kPoolNumBars]
 
   const int b = blockIdx.y;
+  const int T = lengths ? lengths[b] : T_all;     // masked batch: this utterance's own frames
   const int c0 = blockIdx.x * 128;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int c = c0 + lane * 4;
@@ -215,6 +217,17 @@ extern "C" int xvb_stats_pool(const float* x, int64_t ldx, int B, int T, int C, 
 
 extern "C" int xvb_stats_pool_ex(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, float* out,
                                  uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+  return stats_pool(x, ldx, B, T, C, eps, mode, nullptr, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_stats_pool_lengths(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, const int* lengths,
+                                      float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_stats_pool_lengths: null lengths");
+  return stats_pool(x, ldx, B, T, C, eps, mode, lengths, out, out_hi, out_lo, ldo, stream);
+}
+
+int xvb::stats_pool(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, const int* lengths, float* out,
+                    uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(x && out, "xvb_stats_pool: null pointer");
@@ -233,7 +246,7 @@ extern "C" int xvb_stats_pool_ex(const float* x, int64_t ldx, int B, int T, int 
   XVB_ENSURE_DYN_SMEM((stats_pool_tma_kernel), kPoolSmemBytes);
   dim3 grid((C + 127) / 128, B);
   stats_pool_tma_kernel<<<grid, kPoolWarps * 32, kPoolSmemBytes, (cudaStream_t)stream>>>(
-      map, T, C, eps, mode, out, reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
+      map, T, C, eps, mode, lengths, out, reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
 }

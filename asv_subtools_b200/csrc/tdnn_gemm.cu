@@ -78,6 +78,9 @@ struct TdnnGemmParams {
   // group_kg input channels, starting at frame channel (n0 / group_ng) * group_kg; 0 = dense
   int group_ng, group_kg;
   int out_T;              // time extent of the fp32 output (k_slices for split-K partials, else T)
+  // masked batch of utterances of different lengths: utterance b owns frames [0, lengths[b]); the layer epilogue stores
+  // zeros for the frames past it (what the next layer's taps must read, F.pad).  NULL: every utterance is T frames long.
+  const int* lengths;
   __nv_bfloat16* y_hi;
   __nv_bfloat16* y_lo;
   long long ldy;
@@ -140,6 +143,28 @@ __device__ __forceinline__ void chan_merge(float& n, float& mean, float& m2, flo
 // made the epilogue code larger than the instruction cache, and every tile's epilogue fetched its code from L2.
 __device__ __noinline__ float epi_tanh(float v) { return tanhf(v); }
 __device__ __noinline__ float epi_sigmoid(float v) { return 1.f / (1.f + expf(-v)); }
+
+// A masked batch's rows past an utterance's end store zeros: this thread's column pairs c, c + 8, ... below c_end.  Out
+// of line for the same reason, and because unmasked layers never take it.
+__device__ __noinline__ void epi_zero_row(const TdnnGemmParams& p, long long grow, long long frow, int c_begin, int c_end) {
+  for (int c = c_begin; c < c_end; c += 8) {
+    const bool has1 = c + 1 < p.Cout;
+    if (p.y_hi) {
+      if (has1) {
+        *reinterpret_cast<uint32_t*>(p.y_hi + grow * p.ldy + c) = 0u;
+        *reinterpret_cast<uint32_t*>(p.y_lo + grow * p.ldy + c) = 0u;
+      } else {
+        p.y_hi[grow * p.ldy + c] = __float2bfloat16(0.f);
+        p.y_lo[grow * p.ldy + c] = __float2bfloat16(0.f);
+      }
+    }
+    if (p.y_f32) {
+      float* df = p.y_f32 + frow * p.ldyf + c;
+      if (has1) *reinterpret_cast<float2*>(df) = make_float2(0.f, 0.f);
+      else *df = 0.f;
+    }
+  }
+}
 
 // kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
 // one, so that the instantiations without it compile to the same code as before the flag existed.
@@ -409,6 +434,10 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       const int row = row0 + 8 * h;
       const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
       if (b >= p.B || t >= p.T) continue;
+      if (p.lengths && t >= __ldg(p.lengths + b)) {   // masked batch, frame past the utterance's end: store zeros
+        epi_zero_row(p, (long long)b * p.T + t, (long long)b * p.out_T + t + slice, n0 + 2 * q4, min(n0 + BLOCK_N, p.Cout));
+        continue;
+      }
       const float rbias = p.row_bias ? __ldg(p.row_bias + (long long)b * p.T + t) : 0.f;
       const float* ub = p.utt_bias ? p.utt_bias + (long long)b * p.ld_utt : nullptr;
       const long long grow = (long long)b * p.T + t;
@@ -685,6 +714,7 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
   XVB_CHECK_ARG((a.y_hi != nullptr) == (a.y_lo != nullptr), "xvb_tdnn_affine: y_hi/y_lo must both be set or both NULL");
   XVB_CHECK_ARG(a.y_hi || a.y_f32 || a.pool_partial || th, "xvb_tdnn_affine: no output requested");
   XVB_CHECK_ARG(!(a.flags & XVB_SWISH) || !(a.pool_partial || th), "xvb_tdnn_affine: XVB_SWISH is a layer-epilogue flag only");
+  XVB_CHECK_ARG(!(a.lengths && (th || a.pool_partial)), "xvb_tdnn_affine: lengths apply to the layer epilogue only");
   if (a.pool_partial) XVB_CHECK_ARG(!a.y_hi && !a.y_f32 && Cout % 4 == 0 && (uintptr_t)a.pool_partial % 16 == 0,
                                     "xvb_tdnn_affine: pool_partial excludes other outputs and needs Cout%%4==0");
   if (a.y_hi) XVB_CHECK_ARG(a.ldy % 8 == 0 && a.ldy >= Cout, "xvb_tdnn_affine: plane output needs ldy%%8==0 and ldy>=Cout");
@@ -722,6 +752,7 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
   p.bias = a.bias; p.scale = a.bn_scale; p.shift = a.bn_shift; p.row_bias = a.row_bias;
   p.utt_bias = a.utt_bias; p.ld_utt = a.ld_utt_bias;
   p.pool_partial = a.pool_partial;
+  p.lengths = a.lengths;
   p.num_src = a.x2_hi ? 2 : 1;
   p.unit_first = 0; p.unit_stride = 1;
   if (th) {

@@ -204,10 +204,13 @@ class CamPPXvector(TopVirtualNnet):
         return self.extract_embedding_batch(torch.as_tensor(np.asarray(feats) if not isinstance(feats, torch.Tensor)
                                                             else feats)[None])[0].cpu()
 
-    def extract_embedding_batch(self, feats):
+    def extract_embedding_batch(self, feats, lengths=None):
         """Equal-length utterances (B, T, F) float32 -> (B, embd_dim) CUDA tensor, the same arithmetic as B calls of
         extract_embedding(): each chunk position of chunk_sizes(T) runs as one batch, and the chunk embeddings are
         combined as sum_i size_i * emb_i / T in chunk order."""
+        if lengths is not None:
+            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector blueprints only"
+                                      .format(type(self).__name__))
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:

@@ -332,10 +332,13 @@ class TransformerXvector(TopVirtualNnet):
             raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, int(feats.shape[0])))
         return self._extract_embedding_chunked(feats)
 
-    def extract_embedding_batch(self, feats):
+    def extract_embedding_batch(self, feats, lengths=None):
         """Equal-length utterances (B, T, F) float32 -> (B, D) CUDA tensor, the same arithmetic as B calls of
         extract_embedding(): the B * (num_split - 1) full chunks run as one batch, the B last chunks as another, and the
         chunk embeddings are recombined with the reference's length-weighted average."""
+        if lengths is not None:
+            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector blueprints only"
+                                      .format(type(self).__name__))
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:

@@ -149,10 +149,12 @@ class TopVirtualNnet(torch.nn.Module):
                 return torch.from_numpy(emb)
         return self._extract_embedding_chunked(feats)
 
-    def extract_embedding_batch(self, feats):
+    def extract_embedding_batch(self, feats, lengths=None):
         """Equal-length utterances in one call: feats (B, T, F) float32 (CUDA tensor, CPU tensor or
         ndarray; T <= maxChunk) -> (B, D) CUDA tensor.  Same arithmetic as B calls of
-        extract_embedding()."""
+        extract_embedding().  lengths (B,) host ints, 1 <= lengths[b] <= T: utterances of different lengths padded to
+        T, row b being the embedding of feats[b, :lengths[b]] (what is past it is ignored); TDNN x-vector blueprints
+        (build_tdnn_extractor with statistics pooling) only."""
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:
@@ -160,7 +162,15 @@ class TopVirtualNnet(torch.nn.Module):
             if x.shape[1] > 10000:
                 raise ValueError("T > maxChunk: use extract_embedding() per utterance")
             x = x.to(self.device_for_extraction(), non_blocking=True).contiguous()
-            return self.extractor().extract(x)
+            if lengths is None:
+                return self.extractor().extract(x)
+            from .. import ops
+            ex = self.extractor()
+            if not isinstance(ex, ops.Extractor):
+                raise NotImplementedError("{}: extract_embedding_batch(lengths=...) needs the TDNN x-vector extractor with "
+                                          "statistics pooling; this model runs on {}".format(type(self).__name__,
+                                                                                              type(ex).__name__))
+            return ex.extract(x, lengths)
 
 
 def build_tdnn_extractor(model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, extracted_embedding):

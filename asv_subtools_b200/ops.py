@@ -126,12 +126,13 @@ def tdnn_grouped_fits(cin, cout, groups):
 
 def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_shift=None, utt_bias=None, row_bias=None,
                    relu=False, tanh=False, sigmoid=False, y=None, y_f32=None, pool_partial=None, swish=False, groups=1,
-                   x_batch_stride=0):
+                   x_batch_stride=0, lengths=None):
     """Full form of the wgmma layer (xvb_tdnn_affine_ex).  x / x2: SplitPlanes (B,T,*) (views
     allowed); y: SplitPlanes to write (view allowed) and/or y_f32: fp32 (B,T,>=cout) tensor.  swish: x * sigmoid(x)
     after the bias (and ReLU), before the BatchNorm (XVB_SWISH).  groups > 1: grouped 1x1 conv, w the compact packing
     of the (cout, Cin/groups, 1) weight.  x_batch_stride > 0: x is an im2col view (xvb_tdnn_args_t.x_batch_stride):
-    frame t of utterance b is the x.channels-long window at element b * x_batch_stride + t * x.ld of the planes."""
+    frame t of utterance b is the x.channels-long window at element b * x_batch_stride + t * x.ld of the planes.
+    lengths: int32 CUDA (B,) tensor of a masked batch (xvb_tdnn_args_t.lengths): frames t >= lengths[b] store zeros."""
     b, t = x.hi.shape[0], x.hi.shape[1]
     a = TdnnArgs()
     a.x_hi, a.x_lo, a.ldx = x.hi.data_ptr(), x.lo.data_ptr(), x.ld
@@ -160,6 +161,8 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
     a.B, a.T, a.Cin, a.Cout = b, t, x.channels, cout
     a.groups = groups
     a.x_batch_stride = x_batch_stride
+    if lengths is not None:
+        a.lengths = _req(lengths, torch.int32, "lengths").data_ptr()
     check(lib.xvb_tdnn_affine_ex(C.byref(a), _stream()), "xvb_tdnn_affine_ex")
 
 
@@ -397,14 +400,19 @@ def conv_module(x, dw_weight, dw_bias, norm_a, norm_b, y, batch_norm=False, eps=
                               y.lo.data_ptr(), y.ld, _stream()), "xvb_conv_module")
 
 
-def stats_pool_ex(x, eps, mode, planes=False):
-    """mode 0: StatisticsPooling; mode 1: ECAPA global context (unbiased var + eps)."""
+def stats_pool_ex(x, eps, mode, planes=False, lengths=None):
+    """mode 0: StatisticsPooling; mode 1: ECAPA global context (unbiased var + eps).  lengths: int32 CUDA (B,) tensor of
+    a masked batch (utterance b pools its first lengths[b] frames; xvb_stats_pool_lengths)."""
     x = _req(x, torch.float32, "x")
     b, t, c = x.shape
     out = torch.empty(b, 2 * c, dtype=torch.float32, device=x.device)
     op = SplitPlanes.empty((b, 1, 2 * c), x.device) if planes else None
-    check(lib.xvb_stats_pool_ex(_ptr(x), c, b, t, c, eps, mode, _ptr(out), op.hi.data_ptr() if op else None,
-                                op.lo.data_ptr() if op else None, 2 * c, _stream()), "xvb_stats_pool_ex")
+    tail = (_ptr(out), op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, 2 * c, _stream())
+    if lengths is None:
+        check(lib.xvb_stats_pool_ex(_ptr(x), c, b, t, c, eps, mode, *tail), "xvb_stats_pool_ex")
+    else:
+        check(lib.xvb_stats_pool_lengths(_ptr(x), c, b, t, c, eps, mode, _ptr(_req(lengths, torch.int32, "lengths")), *tail),
+              "xvb_stats_pool_lengths")
     return (out, op) if planes else out
 
 
@@ -801,14 +809,26 @@ class Extractor:
         self._keep, self._layers, self._eps = [], [], None
         return self
 
-    def extract(self, feats):
-        """feats (B,T,F) fp32 CUDA -> (B,D) fp32 CUDA, asynchronous on the current stream."""
+    def extract(self, feats, lengths=None):
+        """feats (B,T,F) fp32 CUDA -> (B,D) fp32 CUDA, asynchronous on the current stream.  lengths (B,) host ints
+        (sequence, ndarray or CPU tensor), 1 <= lengths[b] <= T: a batch of utterances of different lengths, row b being
+        feats[b, :lengths[b]] extracted alone (xvb_extractor_extract_lengths); the frames past them are never read."""
         feats = _req(feats, torch.float32, "feats")
         b, t, f = feats.shape
         if f != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
         emb = torch.empty(b, self.embed_dim, dtype=torch.float32, device=feats.device)
-        check(lib.xvb_extractor_extract(self._h, _ptr(feats), b, t, _ptr(emb), _stream()), "xvb_extractor_extract")
+        if lengths is None:
+            check(lib.xvb_extractor_extract(self._h, _ptr(feats), b, t, _ptr(emb), _stream()), "xvb_extractor_extract")
+            return emb
+        if isinstance(lengths, torch.Tensor):
+            lengths = lengths.cpu().numpy()
+        lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
+        if lens.shape[0] != b:
+            raise ValueError("lengths has {} entries for a batch of {}".format(lens.shape[0], b))
+        lens = np.clip(lens, -2 ** 31, 2 ** 31 - 1).astype(np.int32)    # out-of-range values stay out of range for the C check
+        check(lib.xvb_extractor_extract_lengths(self._h, _ptr(feats), lens.ctypes.data_as(C.c_void_p), b, t, _ptr(emb),
+                                                _stream()), "xvb_extractor_extract_lengths")
         return emb
 
     def extract_host(self, feats_np):

@@ -13,6 +13,12 @@ splitDataByLength.sh-balanced jobs); utterances longer than maxChunk fall back t
 per-utterance `extract_embedding()` with the reference's chunk rule.  One `FV` vector is written per
 input key (bucket order).  `--shard i/n` keeps every n-th utterance (one process per GPU without
 pre-splitting the scp).
+
+`--mixed-lengths` (TDNN x-vector models with statistics pooling): the maxChunk rule cuts every utterance first, and the
+chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
+call, `extract_embedding_batch(x, lengths)`, and each utterance's embedding is sum(len_i * emb_i) / frames over its
+chunks, as `bin/xvb-extract --mixed-lengths` does.  The pooling merge order depends on the batch shape, so the vectors
+differ from the default mode's at the rounding level.
 """
 import argparse
 import os
@@ -77,6 +83,83 @@ class Batcher:
         self.buckets, self.pending = {}, 0
 
 
+def plan_mixed_batches(lengths, batch_size):
+    """The batch rule of --mixed-lengths (the same as xvb-extract's): items in ascending length (ties in arrival order),
+    each batch up to `batch_size` consecutive items whose padded frames n * max(len) - sum(len) are at most 1/8 of
+    n * max(len).  Returns lists of indices into `lengths`.  Equal lengths give the equal-length buckets: runs of
+    batch_size items in arrival order, then the remainder."""
+    order = sorted(range(len(lengths)), key=lambda i: lengths[i])
+    batches, i = [], 0
+    while i < len(order):
+        j, total = i + 1, lengths[order[i]]
+        while j < len(order) and j - i < batch_size:
+            n, tmax = j - i + 1, lengths[order[j]]
+            if 8 * (n * tmax - (total + tmax)) > n * tmax:
+                break
+            total += tmax
+            j += 1
+        batches.append(order[i:j])
+        i = j
+    return batches
+
+
+def chunk_lengths(frames, max_chunk=MAX_CHUNK):
+    """The maxChunk rule of framework.py:29-39: ceil(frames / max_chunk) chunks of frames // num_split frames, the last
+    one taking the remainder."""
+    num_split = (frames + max_chunk - 1) // max_chunk
+    split = frames // num_split
+    return [split] * (num_split - 1) + [frames - split * (num_split - 1)]
+
+
+def extract_stream_mixed(model, reader, writer, batch_size=256, shard=(0, 1), log=print, max_pending_frames=4_000_000):
+    """--mixed-lengths form of extract_stream.  Returns (utterances, batches, padded frames, batch frames)."""
+    utts, items = [], []              # utts: [key, frames, chunks pending, sum(len_i * emb_i)]; items: (utt, chunk)
+    stats = [0, 0, 0]
+    pending = [0]
+
+    def run():
+        lens = [c.shape[0] for _, c in items]
+        for idx in plan_mixed_batches(lens, batch_size):
+            tmax = max(lens[i] for i in idx)
+            x = np.zeros((len(idx), tmax, items[idx[0]][1].shape[1]), dtype=np.float32)
+            for r, i in enumerate(idx):
+                x[r, :lens[i]] = items[i][1]
+            emb = model.extract_embedding_batch(x, lengths=[lens[i] for i in idx]).cpu().numpy()
+            stats[0] += 1
+            stats[1] += len(idx) * tmax - sum(lens[i] for i in idx)
+            stats[2] += len(idx) * tmax
+            for r, i in enumerate(idx):
+                u = utts[items[i][0]]
+                u[3] = u[3] + np.float32(lens[i]) * emb[r]
+                u[2] -= 1
+                if u[2] == 0:
+                    writer(u[0], u[3] / np.float32(u[1]))
+                    u[3] = None
+        items.clear()
+        pending[0] = 0
+
+    count = 0
+    for i, (key, feats) in enumerate(reader):
+        if i % shard[1] != shard[0]:
+            continue
+        log("Process utterance for key {0}".format(key))
+        feats = np.ascontiguousarray(feats)
+        if feats.dtype != np.float32:
+            raise TypeError("features of {} are {}, the extractor takes float32 (FM/CM) matrices".format(key, feats.dtype))
+        count += 1
+        lens = chunk_lengths(feats.shape[0])
+        utts.append([key, feats.shape[0], len(lens), np.float32(0)])
+        off = 0
+        for n in lens:
+            items.append((len(utts) - 1, feats[off:off + n]))
+            off += n
+        pending[0] += feats.shape[0]
+        if pending[0] > max_pending_frames:
+            run()
+    run()
+    return count, stats[0], stats[1], stats[2]
+
+
 def extract_stream(model, reader, writer, batch_size=256, shard=(0, 1), log=print):
     """reader yields (key, (T,F) float32 ndarray); writer(key, 1-D float32 ndarray)."""
     batcher = Batcher(batch_size)
@@ -117,6 +200,9 @@ def main(argv=None):
     ap.add_argument("--gpu-id", type=str, default="")
     ap.add_argument("--batch-size", type=int, default=256)
     ap.add_argument("--shard", type=str, default="0/1", help="i/n: keep utterances with index %% n == i")
+    ap.add_argument("--mixed-lengths", action="store_true",
+                    help="batch utterances of different lengths (padding at most 1/8 of a batch); TDNN x-vector models with "
+                         "statistics pooling only")
     ap.add_argument("--blueprint-dir", type=str, default="",
                     help="take the blueprint of the same file name from this directory (asv_subtools_b200/model) instead of "
                          "the path stored in nnet.config, so a reference model dir is used as it is")
@@ -144,10 +230,26 @@ def main(argv=None):
         torch.cuda.set_device(int(args.gpu_id.split(",")[0]) if args.gpu_id != "" else 0)
         model.cuda().eval()
         i, n = (int(v) for v in args.shard.split("/"))
+        if args.mixed_lengths:
+            from asv_subtools_b200 import ops
+            ex = model.extractor()
+            if not isinstance(ex, ops.Extractor):
+                print("ERROR: --mixed-lengths needs a TDNN x-vector model with statistics pooling; {} runs on {}".format(
+                    type(model).__name__, type(ex).__name__), file=sys.stderr)
+                sys.exit(1)
         # native ark reader (csrc/ark_io.cpp): the reference's byte-at-a-time key loop is the wall at GPU rates
         with kaldi_io.open_or_fd(args.vectors_wspecifier, "wb") as w:
-            extract_stream(model, kaldi_io.read_mat_ark_native(args.feats_rspecifier),
-                           lambda k, v: kaldi_io.write_vec_flt(w, v, key=k), batch_size=args.batch_size, shard=(i, n))
+            reader = kaldi_io.read_mat_ark_native(args.feats_rspecifier)
+            write = lambda k, v: kaldi_io.write_vec_flt(w, v, key=k)  # noqa: E731
+            if args.mixed_lengths:
+                utts, batches, padded, total = extract_stream_mixed(model, reader, write, batch_size=args.batch_size,
+                                                                    shard=(i, n))
+                print("extract_embeddings: {} utterances, {} masked batches, {} padded frames ({:.4f} of {} batch frames)"
+                      .format(utts, batches, padded, padded / max(total, 1), total), file=sys.stderr)
+            else:
+                extract_stream(model, reader, write, batch_size=args.batch_size, shard=(i, n))
+    except SystemExit:
+        raise
     except BaseException as err:
         if not isinstance(err, KeyboardInterrupt):
             traceback.print_exc()

@@ -136,6 +136,12 @@ typedef struct xvb_tdnn_args {
    * weight (xvb_pack_tdnn_weight with Cin/G input channels), not its block-diagonal expansion.  Needs
    * xvb_tdnn_grouped_fits(Cin, Cout, G), one tap, and no x2, pool_partial, x_batch_stride or XVB_SWISH. */
   int groups;
+  /* NULL, or a DEVICE int32[B] with 1 <= lengths[b] <= T: a masked batch of utterances of different lengths, utterance b
+   * owning frames [0, lengths[b]).  The layer epilogue stores exact zeros (planes and fp32) for the frames past it, so
+   * the next layer's context taps read the zero padding of F.pad (components.py:117).  The x planes must already hold
+   * zeros past each utterance's end.  Not with pool_partial (pool a masked batch with xvb_stats_pool_lengths) or the
+   * trial histogram. */
+  const int* lengths;
 } xvb_tdnn_args_t;
 int xvb_tdnn_affine_ex(const xvb_tdnn_args_t* args, void* stream);
 /* 1 when the grouped mode takes this shape: Cin/G a multiple of 64 and Cout/G a multiple of 32 (an N tile of
@@ -171,6 +177,10 @@ int xvb_stats_pool(const float* x, int64_t ldx, int B, int T, int C, float eps, 
  * (pytorch/model/ecapa_tdnn_xvector.py:175-178): std = sqrt(unbiased_var + eps). */
 int xvb_stats_pool_ex(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, float* out,
                       uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
+/* xvb_stats_pool_ex over a masked batch: utterance b pools its first lengths[b] frames (DEVICE int32[B],
+ * 1 <= lengths[b] <= T); the frames past them are never read. */
+int xvb_stats_pool_lengths(const float* x, int64_t ldx, int B, int T, int C, float eps, int mode, const int* lengths,
+                           float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * ECAPA-TDNN pieces that are not contractions (pytorch/model/ecapa_tdnn_xvector.py)
@@ -576,6 +586,15 @@ int xvb_extractor_finalize(xvb_extractor_t* h, float pooling_eps);
 int xvb_extractor_embed_dim(const xvb_extractor_t* h);
 /* feats (B, T, feat_dim) fp32 on the device -> emb (B, embed_dim) fp32 on the device. */
 int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* A batch of utterances of different lengths: feats (B, T, feat_dim) fp32 on the device, utterance b in its first
+ * lengths_host[b] frames (HOST int32[B], 1 <= lengths_host[b] <= T; the frames past them are never read, whatever they
+ * hold).  Row b of emb is the embedding of feats[b, :lengths_host[b]] extracted alone, up to the rounding of the
+ * pooling merge order.  A batch with lengths below T pools with xvb_stats_pool_lengths after an fp32 last frame layer,
+ * whatever xvb_extractor_set_fused_pooling says (the fused pooling epilogue takes equal lengths only).  The lengths are checked (XVB_EINVAL naming the first bad one) and copied into a device buffer
+ * of the extractor on `stream`; the host array may be reused when the call returns.  With every length equal to T the
+ * result equals xvb_extractor_extract bit for bit. */
+int xvb_extractor_extract_lengths(xvb_extractor_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
+                                  float* emb, void* stream);
 /* Same through host buffers (H2D of feats, D2H of emb inside; synchronises the stream). */
 int xvb_extractor_extract_host(xvb_extractor_t* h, const float* feats_host, int B, int T, float* emb_host,
                                void* stream);

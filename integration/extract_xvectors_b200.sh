@@ -19,17 +19,21 @@
 #   XVB200_ROOT    repo root (default: the directory above this file)      XVB200_PYTHON  interpreter (default: python3)
 #   XVB200_BATCH   utterances per batch (default 256)                      XVB200_REF     the reference script to wrap
 #   XVB200_DRYRUN  non-empty: print the rewritten command lines and exit
+#   XVB200_MIXED_LENGTHS  1: add --mixed-lengths (batches of utterances of different lengths, at most 1/8 padding;
+#                  TDNN x-vector models with statistics pooling only)
 
 set -e
 XVB200_ROOT=${XVB200_ROOT:-$(cd "$(dirname "${BASH_SOURCE[0]}")/.." && pwd)}
 XVB200_PYTHON=${XVB200_PYTHON:-python3}
 XVB200_BATCH=${XVB200_BATCH:-256}
+mixed=""
+[ "${XVB200_MIXED_LENGTHS:-}" = "1" ] && mixed=" --mixed-lengths"
 XVB200_REF=${XVB200_REF:-subtools/pytorch/pipeline/extract_xvectors_for_pytorch.sh}
 
 [ ! -f "$XVB200_REF" ] && echo "[exit] $XVB200_REF not found: run from the recipe directory (or set XVB200_REF)" && exit 1
 
 old="python3 subtools/pytorch/pipeline/onestep/extract_embeddings.py"
-new="env PYTHONPATH=$XVB200_ROOT\${PYTHONPATH:+:\$PYTHONPATH} $XVB200_PYTHON -m asv_subtools_b200.pipeline.extract_embeddings --batch-size $XVB200_BATCH --blueprint-dir $XVB200_ROOT/asv_subtools_b200/model"
+new="env PYTHONPATH=$XVB200_ROOT\${PYTHONPATH:+:\$PYTHONPATH} $XVB200_PYTHON -m asv_subtools_b200.pipeline.extract_embeddings --batch-size $XVB200_BATCH$mixed --blueprint-dir $XVB200_ROOT/asv_subtools_b200/model"
 grep -q "$old" "$XVB200_REF" || { echo "[exit] $XVB200_REF does not call '$old' any more: nothing to swap"; exit 1; }
 
 tmp=$(mktemp /tmp/extract_xvectors_b200.XXXXXX.sh)

@@ -1,0 +1,105 @@
+#!/usr/bin/env python
+"""Throughput of the TDNN x-vector handle on a corpus of utterances of different lengths -- a side measurement, not the
+bench.py line.
+
+    python tools/bench_mixed_lengths.py [rounds] [--utts N] [--min-frames A] [--max-frames B] [--batch N] [--dim F]
+
+The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
+numpy.random.RandomState(2026), run through one Xvector(F, far) handle (default F = 23) under two batch policies:
+
+  * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
+    up to `batch` utterances of exactly the same frame count, one xvb_extractor_extract call each;
+  * masked: --mixed-lengths' rule (plan_mixed_batches: ascending length, up to `batch` per batch, padding at most 1/8),
+    one xvb_extractor_extract_lengths call each.
+
+Features come from one resident random buffer (no host copies in the timed region).  Each round times the whole corpus
+under each policy with CUDA events, the policies alternating; every launch plan is built in an untimed warm-up pass
+first.  Reports per policy the median frames/s over rounds (real frames only: padding does not count), the batch
+count and the padded share of the frames computed, with the card's name and power limit read in the same run.
+Prints one JSON line."""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+
+import numpy as np
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from asv_subtools_b200.model.xvector import Xvector  # noqa: E402
+from asv_subtools_b200.pipeline.extract_embeddings import plan_mixed_batches  # noqa: E402
+from oracle import nnet as onn  # noqa: E402
+
+
+def equal_length_batches(lengths, batch):
+    """Exact-length buckets in batches of up to `batch` (the default mode of both CLIs)."""
+    buckets = {}
+    for i, n in enumerate(lengths):
+        buckets.setdefault(n, []).append(i)
+    return [idx[k:k + batch] for n in sorted(buckets) for idx in [buckets[n]] for k in range(0, len(idx), batch)]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("rounds", nargs="?", type=int, default=5)
+    ap.add_argument("--utts", type=int, default=4000)
+    ap.add_argument("--min-frames", type=int, default=200)
+    ap.add_argument("--max-frames", type=int, default=2000)
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--dim", type=int, default=23)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_mixed_lengths.py needs a GPU")
+    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                          str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
+    F = args.dim
+    lengths = [int(v) for v in np.random.RandomState(2026).randint(args.min_frames, args.max_frames + 1, args.utts)]
+    m = Xvector(F, 10, training=False, extracted_embedding="far")
+    m.load_state_dict(onn.make_state_dict(onn.xvector_spec(F), 7), strict=True)
+    m.cuda().eval()
+    ex = m.extractor()
+    base = torch.randn(args.batch * args.max_frames * F, device="cuda")
+
+    policies = {}
+    for name, plan in (("equal_length", equal_length_batches(lengths, args.batch)),
+                       ("masked", plan_mixed_batches(lengths, args.batch))):
+        jobs = []
+        for idx in plan:
+            lens = [lengths[i] for i in idx]
+            B, T = len(lens), max(lens)
+            jobs.append((B, T, np.asarray(lens, np.int32) if name == "masked" else None))
+        computed = sum(B * T for B, T, _ in jobs)
+        policies[name] = {"jobs": jobs, "batches": len(jobs), "padded_share": 1.0 - sum(lengths) / computed, "fps": []}
+
+    def run(jobs):
+        for B, T, lens in jobs:
+            x = base[:B * T * F].view(B, T, F)
+            ex.extract(x) if lens is None else ex.extract(x, lens)
+
+    with torch.no_grad():
+        for p in policies.values():          # warm-up: every plan built, every buffer grown
+            run(p["jobs"])
+        torch.cuda.synchronize()
+        for _ in range(args.rounds):
+            for p in policies.values():
+                start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                start.record()
+                run(p["jobs"])
+                stop.record()
+                stop.synchronize()
+                p["fps"].append(sum(lengths) / (start.elapsed_time(stop) / 1e3))
+    out = {"workload": "Xvector({}) far, {} utterances uniform over {}..{} frames (RandomState(2026)), batch {}".format(
+               F, args.utts, args.min_frames, args.max_frames, args.batch),
+           "frames": sum(lengths), "card": smi, "rounds": args.rounds}
+    for name, p in policies.items():
+        out[name] = {"frames_per_s": statistics.median(p["fps"]), "frames_per_s_min": min(p["fps"]),
+                     "frames_per_s_max": max(p["fps"]), "batches": p["batches"], "padded_share": round(p["padded_share"], 5)}
+    out["speedup"] = out["masked"]["frames_per_s"] / out["equal_length"]["frames_per_s"]
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()
