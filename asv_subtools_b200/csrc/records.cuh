@@ -1,6 +1,6 @@
-// Device side of the ResNet, RepVGG, Conformer and CAM++ native extractors' shared plumbing: the packed split-bf16
-// planes, the arena that owns a model's device weights, the grow-only workspace, the segment level of the 2-D families
-// and the group loop of an extract call.  The record store and the model-file codec are host code in records.h.
+// Device side of the native extractors' shared plumbing: the packed split-bf16 planes and the arena that owns a model's
+// device weights (every family), the grow-only workspace, the segment level of the 2-D families and the group loop of
+// an extract call.  The record store and the model-file codec are host code in records.h.
 #pragma once
 #include <vector>
 
@@ -24,13 +24,15 @@ struct Weights {
     dev.push_back(*p);
     return XVB_OK;
   }
-  int upload(float** d, const std::vector<float>& v) {
-    if (v.empty()) { *d = nullptr; return XVB_OK; }
-    int rc = alloc(d, v.size());
+  // n host floats, or nothing (*d = NULL) when v is NULL or n is 0
+  int upload(float** d, const float* v, size_t n) {
+    if (!v || !n) { *d = nullptr; return XVB_OK; }
+    int rc = alloc(d, n);
     if (rc) return rc;
-    XVB_CUDA(cudaMemcpy(*d, v.data(), v.size() * sizeof(float), cudaMemcpyHostToDevice));
+    XVB_CUDA(cudaMemcpy(*d, v, n * sizeof(float), cudaMemcpyHostToDevice));
     return XVB_OK;
   }
+  int upload(float** d, const std::vector<float>& v) { return upload(d, v.data(), v.size()); }
   // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx[0..n) (ops.pack_tdnn_weight / pack_conv2d_weight).
   // xvb_pack_tdnn_weight takes at most XVB_MAX_TAPS taps per call: a longer list is packed in pieces of that many taps
   // (the last one shorter), each piece's rows then copied into its K range of every output row, as pack_conv2d_weight

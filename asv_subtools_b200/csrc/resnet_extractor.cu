@@ -20,10 +20,12 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "records.cuh"
+#include "shard.cuh"
 
 namespace {
 
@@ -46,7 +48,8 @@ struct Block {
   bool has_ds = false, has_se = false;
   Se se;
 };
-struct Model {   // shared by a handle and its second shard lane
+// Shared read-only by a handle and its second shard lane once finalized.
+struct Model {
   int feat_dim = 0, layers[4] = {0}, planes[4] = {0}, pre = 0;
   float eps = 0.f;
   RecordStore recs{kFile.nshape};
@@ -61,8 +64,8 @@ struct Model {   // shared by a handle and its second shard lane
 }  // namespace
 
 struct xvb_resnet {
-  Model* m = nullptr;
-  bool owns_model = true, finalized = false;
+  std::shared_ptr<const Model> m;
+  Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
   // workspace, grown to the largest (B, T) seen: seven rotating (B, T', F', C) plane buffers for the roles block
   // input / activated input / h / identity / z / output / next activated input, the fp32 last-layer output, then the
   // per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers)
@@ -73,18 +76,10 @@ struct xvb_resnet {
   Planes buf[kBufs], pooled, seg_mid;
   float *last = nullptr, *pooled_f32 = nullptr, *se_mean = nullptr, *se_hidden = nullptr, *se_gate = nullptr, *seg_out = nullptr;
   int last_launches = 0;
-  float* h_feats = nullptr; float* h_emb = nullptr;   // device staging of xvb_resnet_extract_host
-  size_t h_feats_cap = 0, h_emb_cap = 0;
-  // pipeline of xvb_resnet_extract_shard_host: two device slots per lane, the copy engine runs ahead of both lanes
-  static constexpr int kSlots = 4;
-  float* p_feats[kSlots] = {nullptr, nullptr, nullptr, nullptr}; float* p_emb[kSlots] = {nullptr, nullptr, nullptr, nullptr};
-  size_t p_feats_cap[kSlots] = {0, 0, 0, 0}, p_emb_cap[kSlots] = {0, 0, 0, 0};
-  cudaStream_t copy_stream = nullptr;
-  cudaEvent_t ev_h2d[kSlots] = {nullptr, nullptr, nullptr, nullptr}, ev_done[kSlots] = {nullptr, nullptr, nullptr, nullptr};
-  // two-lane shard pipeline: `lane1` shares the weights and owns its workspace; batches alternate between two streams
-  xvb_resnet* lane1 = nullptr;
-  cudaStream_t lane_stream[2] = {nullptr, nullptr};
-  cudaEvent_t ev_lane_start = nullptr, ev_lane_done[2] = {nullptr, nullptr};
+  Shard<xvb_resnet> shard;
+
+  explicit xvb_resnet(std::shared_ptr<const Model> model) : m(std::move(model)) {}
+  ~xvb_resnet() { free_ws(); }
 
   void free_ws() {
     for (void* p : ws) cudaFree(p);
@@ -102,6 +97,16 @@ struct xvb_resnet {
     int rc = alloc(&p->hi, n);
     return rc ? rc : alloc(&p->lo, n);
   }
+};
+
+template <>
+struct xvb::ShardFamily<xvb_resnet> {
+  static int extract(xvb_resnet* h, const float* feats, int B, int T, float* emb, void* stream) {
+    return xvb_resnet_extract(h, feats, B, T, emb, stream);
+  }
+  static xvb_resnet* twin(const xvb_resnet* h) { return new xvb_resnet(h->m); }
+  static int feat_dim(const xvb_resnet* h) { return h->m->feat_dim; }
+  static int embed_dim(const xvb_resnet* h) { return h->m->tail.E; }
 };
 
 namespace {
@@ -124,13 +129,13 @@ void shapes(const Model* m, int B, int T, size_t* planes, size_t* last) {
 
 int reserve(xvb_resnet* h, int B, int T) {
   size_t np, nl;
-  shapes(h->m, B, T, &np, &nl);
+  shapes(h->m.get(), B, T, &np, &nl);
   if (np <= h->cap_planes && nl <= h->cap_last && B <= h->cap_B) return XVB_OK;
   np = np > h->cap_planes ? np : h->cap_planes;
   nl = nl > h->cap_last ? nl : h->cap_last;
   const size_t nb = (size_t)(B > h->cap_B ? B : h->cap_B);
   h->free_ws();
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const size_t pooled = (size_t)2 * m->F4 * m->C4, mean = m->Cmax > 256 ? m->Cmax : 256;
   const size_t out = (size_t)m->tail.out_rows();
   int rc = XVB_OK;
@@ -180,7 +185,7 @@ int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, long long P, vo
 int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const bool pre = m->pre != 0;
   int Tl = T, Fl = m->feat_dim;
   int xi = 0, ai = pre ? 1 : -1;
@@ -248,31 +253,32 @@ extern "C" int xvb_resnet_create(xvb_resnet_t** out, int feat_dim, const int* la
     XVB_CHECK_ARG(planes[i] >= 16 && planes[i] <= 4096 && planes[i] % 16 == 0,
                   "xvb_resnet_create: planes[%d] = %d, need a multiple of 16 for the 2-D conv kernel", i, planes[i]);
   }
-  xvb_resnet* h = new xvb_resnet();
-  h->m = new Model();
-  h->m->feat_dim = feat_dim;
-  for (int i = 0; i < 4; ++i) { h->m->layers[i] = layers[i]; h->m->planes[i] = planes[i]; }
-  h->m->pre = pre_activation ? 1 : 0;
-  h->m->eps = pooling_eps;
+  auto m = std::make_shared<Model>();
+  m->feat_dim = feat_dim;
+  for (int i = 0; i < 4; ++i) { m->layers[i] = layers[i]; m->planes[i] = planes[i]; }
+  m->pre = pre_activation ? 1 : 0;
+  m->eps = pooling_eps;
+  xvb_resnet* h = new xvb_resnet(m);
+  h->draft = m.get();
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_resnet_set_layer(xvb_resnet_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
                                     const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
-  XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127, "xvb_resnet_set_layer: bad arguments or finalized model");
+  XVB_CHECK_ARG(h && h->draft && name && strlen(name) > 0 && strlen(name) < 127, "xvb_resnet_set_layer: bad arguments or finalized model");
   XVB_CHECK_ARG(ksize == 0 || ksize == 1 || ksize == 3, "xvb_resnet_set_layer(%s): bad shape %d x %d x k%d", name, Cout, Cin, ksize);
   const char* fn = "xvb_resnet_set_layer";
   const int shape[3] = {Cout, Cin, ksize};
-  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  int rc = h->draft->recs.check(fn, name, shape, w_host, scale_host, shift_host);
   if (rc) return rc;
   XVB_CHECK_ARG(!(flags & XVB_BN) || scale_host, "xvb_resnet_set_layer(%s): XVB_BN without scale/shift", name);
-  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
+  return h->draft->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
 extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
-  XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_resnet_finalize: null or finalized model");
-  Model* m = h->m;
+  XVB_CHECK_ARG(h && h->draft, "xvb_resnet_finalize: null or finalized model");
+  Model* m = h->draft;
   // a record the configuration needs: present, with the expected shape
   auto need = [&](const std::string& n, int cout, int cin, int k, const Rec** out) -> int {
     const int shape[3] = {cout, cin, k};
@@ -353,16 +359,16 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
   // segment level (resnet_xvector.py:194-206): [fc1 ->] [fc2], as many as the extracted position hands over
   if ((rc = m->tail.build(m->recs, m->dev, "xvb_resnet_finalize", 2 * m->F4 * m->C4))) return rc;
   if ((rc = m->recs.check_all_used("xvb_resnet_finalize"))) return rc;
-  h->finalized = true;
+  h->draft = nullptr;
   return XVB_OK;
 }
 
-extern "C" int xvb_resnet_feat_dim(const xvb_resnet_t* h) { return h && h->m ? h->m->feat_dim : XVB_EINVAL; }
-extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return h && h->finalized ? h->m->tail.E : XVB_EINVAL; }
+extern "C" int xvb_resnet_feat_dim(const xvb_resnet_t* h) { return h ? h->m->feat_dim : XVB_EINVAL; }
+extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return h && !h->draft ? h->m->tail.E : XVB_EINVAL; }
 extern "C" int xvb_resnet_last_launches(const xvb_resnet_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized, "xvb_resnet_extract: model not finalized");
+  XVB_CHECK_ARG(h && !h->draft, "xvb_resnet_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_resnet_extract: bad arguments");
   const long before = g_launches;
   const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
@@ -374,139 +380,26 @@ extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, in
 }
 
 extern "C" int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized && feats_host && emb_host && B > 0 && T > 0, "xvb_resnet_extract_host: bad arguments");
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t nf = (size_t)B * T * h->m->feat_dim, ne = (size_t)B * h->m->tail.E;
-  int rc;
-  if (nf > h->h_feats_cap) {
-    cudaFree(h->h_feats); h->h_feats = nullptr; h->h_feats_cap = 0;
-    XVB_CUDA(cudaMalloc((void**)&h->h_feats, nf * sizeof(float)));
-    h->h_feats_cap = nf;
-  }
-  if (ne > h->h_emb_cap) {
-    cudaFree(h->h_emb); h->h_emb = nullptr; h->h_emb_cap = 0;
-    XVB_CUDA(cudaMalloc((void**)&h->h_emb, ne * sizeof(float)));
-    h->h_emb_cap = ne;
-  }
-  XVB_CUDA(cudaMemcpyAsync(h->h_feats, feats_host, nf * sizeof(float), cudaMemcpyHostToDevice, s));
-  if ((rc = xvb_resnet_extract(h, h->h_feats, B, T, h->h_emb, stream))) return rc;
-  XVB_CUDA(cudaMemcpyAsync(emb_host, h->h_emb, ne * sizeof(float), cudaMemcpyDeviceToHost, s));
-  XVB_CUDA(cudaStreamSynchronize(s));
-  return XVB_OK;
+  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && B > 0 && T > 0, "xvb_resnet_extract_host: bad arguments");
+  return h->shard.extract_host(h, feats_host, B, T, emb_host, stream);
 }
 
-// ---- whole shards: the protocol of xvb_ecapa_extract_shard[_host] ------------------------------------------------
-namespace {
-
-// Two lanes unless XVB_LANES=0 (read per call, so one process can compare both).
-bool lanes_enabled() {
-  const char* v = getenv("XVB_LANES");
-  return v ? atoi(v) != 0 : true;
-}
-
-int ensure_lanes(xvb_resnet* h) {
-  if (h->lane1) return XVB_OK;
-  for (int i = 0; i < 2; ++i) {
-    XVB_CUDA(cudaStreamCreateWithFlags(&h->lane_stream[i], cudaStreamNonBlocking));
-    XVB_CUDA(cudaEventCreateWithFlags(&h->ev_lane_done[i], cudaEventDisableTiming));
-  }
-  XVB_CUDA(cudaEventCreateWithFlags(&h->ev_lane_start, cudaEventDisableTiming));
-  xvb_resnet* c = new xvb_resnet();
-  c->m = h->m;
-  c->owns_model = false;
-  c->finalized = true;
-  h->lane1 = c;
-  return XVB_OK;
-}
-int lanes_fork(xvb_resnet* h, cudaStream_t s) {
-  XVB_CUDA(cudaEventRecord(h->ev_lane_start, s));
-  for (int i = 0; i < 2; ++i) XVB_CUDA(cudaStreamWaitEvent(h->lane_stream[i], h->ev_lane_start, 0));
-  return XVB_OK;
-}
-int lanes_join(xvb_resnet* h, cudaStream_t s) {
-  for (int i = 0; i < 2; ++i) {
-    XVB_CUDA(cudaEventRecord(h->ev_lane_done[i], h->lane_stream[i]));
-    XVB_CUDA(cudaStreamWaitEvent(s, h->ev_lane_done[i], 0));
-  }
-  return XVB_OK;
-}
-
-}  // namespace
-
+// ---- whole shards: the protocol of shard.cuh ---------------------------------------------------------------------
 extern "C" int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard: bad arguments");
-  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->tail.E;
-  const bool lanes = lanes_enabled() && N > batch;
-  int rc, launches = 0, k = 0;
-  if (lanes && ((rc = ensure_lanes(h)) || (rc = lanes_fork(h, (cudaStream_t)stream)))) return rc;
-  for (int64_t i = 0; i < N; i += batch, ++k) {
-    const int b = (int)(N - i < batch ? N - i : batch);
-    xvb_resnet* lane = (lanes && (k & 1)) ? h->lane1 : h;
-    void* ls = lanes ? (void*)h->lane_stream[k & 1] : stream;
-    if ((rc = xvb_resnet_extract(lane, feats + (size_t)i * T * F, b, T, emb + (size_t)i * E, ls))) return rc;
-    launches += lane->last_launches;
-  }
-  if (lanes && (rc = lanes_join(h, (cudaStream_t)stream))) return rc;
-  h->last_launches = launches;
-  return XVB_OK;
+  XVB_CHECK_ARG(h && !h->draft && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard: bad arguments");
+  return h->shard.device(h, feats, N, T, batch, emb, stream, false);
 }
 
 extern "C" int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int64_t N, int T, int batch,
                                              float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized && feats_host && emb_host && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard_host: bad arguments");
-  cudaStream_t s = (cudaStream_t)stream;
-  constexpr int S = xvb_resnet::kSlots;
-  if (!h->copy_stream) {
-    XVB_CUDA(cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking));
-    for (int i = 0; i < S; ++i) {
-      XVB_CUDA(cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming));
-      XVB_CUDA(cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming));
-    }
-  }
-  const size_t F = (size_t)h->m->feat_dim, E = (size_t)h->m->tail.E;
-  const int bmax = (int)(N < batch ? N : batch);
-  const size_t nf = (size_t)bmax * T * F, ne = (size_t)bmax * E;
-  int rc;
-  for (int slot = 0; slot < S; ++slot) {
-    if (nf > h->p_feats_cap[slot]) {
-      cudaFree(h->p_feats[slot]); h->p_feats[slot] = nullptr; h->p_feats_cap[slot] = 0;
-      XVB_CUDA(cudaMalloc((void**)&h->p_feats[slot], nf * sizeof(float)));
-      h->p_feats_cap[slot] = nf;
-    }
-    if (ne > h->p_emb_cap[slot]) {
-      cudaFree(h->p_emb[slot]); h->p_emb[slot] = nullptr; h->p_emb_cap[slot] = 0;
-      XVB_CUDA(cudaMalloc((void**)&h->p_emb[slot], ne * sizeof(float)));
-      h->p_emb_cap[slot] = ne;
-    }
-  }
-  const bool lanes = lanes_enabled() && N > batch;
-  if (lanes && ((rc = ensure_lanes(h)) || (rc = lanes_fork(h, s)))) return rc;
-  int launches = 0, k = 0;
-  for (int64_t i = 0; i < N; i += batch, ++k) {
-    const int b = (int)(N - i < batch ? N - i : batch);
-    const int slot = k % S;
-    xvb_resnet* lane = (lanes && (k & 1)) ? h->lane1 : h;
-    cudaStream_t ls = lanes ? h->lane_stream[k & 1] : s;
-    if (k >= S) XVB_CUDA(cudaStreamWaitEvent(h->copy_stream, h->ev_done[slot], 0));
-    XVB_CUDA(cudaMemcpyAsync(h->p_feats[slot], feats_host + (size_t)i * T * F, (size_t)b * T * F * sizeof(float),
-                             cudaMemcpyHostToDevice, h->copy_stream));
-    XVB_CUDA(cudaEventRecord(h->ev_h2d[slot], h->copy_stream));
-    XVB_CUDA(cudaStreamWaitEvent(ls, h->ev_h2d[slot], 0));
-    if ((rc = xvb_resnet_extract(lane, h->p_feats[slot], b, T, h->p_emb[slot], ls))) return rc;
-    XVB_CUDA(cudaMemcpyAsync(emb_host + (size_t)i * E, h->p_emb[slot], (size_t)b * E * sizeof(float), cudaMemcpyDeviceToHost, ls));
-    XVB_CUDA(cudaEventRecord(h->ev_done[slot], ls));
-    launches += lane->last_launches;
-  }
-  if (lanes && (rc = lanes_join(h, s))) return rc;
-  XVB_CUDA(cudaStreamSynchronize(s));
-  h->last_launches = launches;
-  return XVB_OK;
+  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard_host: bad arguments");
+  return h->shard.host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_resnet_extract_shard_host");
 }
 
 // ---- "XVBR0001" model files: the create arguments, then the named records as handed over (save_records) -----------
 extern "C" int xvb_resnet_save(const xvb_resnet_t* h, const char* path) {
-  XVB_CHECK_ARG(h && h->finalized && path, "xvb_resnet_save: model not finalized");
-  const Model* m = h->m;
+  XVB_CHECK_ARG(h && !h->draft && path, "xvb_resnet_save: model not finalized");
+  const Model* m = h->m.get();
   int32_t cfg[11] = {m->feat_dim, m->layers[0], m->layers[1], m->layers[2], m->layers[3],
                      m->planes[0], m->planes[1], m->planes[2], m->planes[3], m->pre};
   memcpy(cfg + 10, &m->eps, sizeof(float));   // pooling_eps as f32
@@ -528,22 +421,4 @@ extern "C" int xvb_resnet_load(xvb_resnet_t** out, const char* path) {
       [](void* h) { return xvb_resnet_finalize((xvb_resnet_t*)h); }, [](void* h) { xvb_resnet_destroy((xvb_resnet_t*)h); });
 }
 
-extern "C" void xvb_resnet_destroy(xvb_resnet_t* h) {
-  if (!h) return;
-  if (h->lane1) xvb_resnet_destroy(h->lane1);
-  for (int i = 0; i < 2; ++i) {
-    if (h->lane_stream[i]) cudaStreamDestroy(h->lane_stream[i]);
-    if (h->ev_lane_done[i]) cudaEventDestroy(h->ev_lane_done[i]);
-  }
-  if (h->ev_lane_start) cudaEventDestroy(h->ev_lane_start);
-  h->free_ws();
-  cudaFree(h->h_feats); cudaFree(h->h_emb);
-  for (int i = 0; i < xvb_resnet::kSlots; ++i) {
-    cudaFree(h->p_feats[i]); cudaFree(h->p_emb[i]);
-    if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]);
-    if (h->ev_done[i]) cudaEventDestroy(h->ev_done[i]);
-  }
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  if (h->owns_model) delete h->m;
-  delete h;
-}
+extern "C" void xvb_resnet_destroy(xvb_resnet_t* h) { delete h; }

@@ -36,6 +36,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200.native import ShardExtractor  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 from asv_subtools_b200.nnet.pooling import MQMHASP  # noqa: E402
@@ -290,109 +291,30 @@ def _segment_layers(m):
     return out
 
 
-class NativeEcapaExtractor:
-    """xvb_ecapa_t: packed weights, workspace and the whole launch sequence in the C library."""
+class NativeEcapaExtractor(ShardExtractor):
+    """xvb_ecapa_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
+    current when it is built (or loaded from an XVBE0001 / XVBE0002 file)."""
 
-    def __init__(self, m=None, device=None, path=None):
-        import ctypes as C
-        from asv_subtools_b200._lib import check, int_array, lib
-        self._C, self._lib, self._check = C, lib, check
-        self._h = C.c_void_p()
-        if path is not None:
-            check(lib.xvb_ecapa_load(C.byref(self._h), str(path).encode()), "xvb_ecapa_load")
-        else:
-            st = m.stats
-            mq = isinstance(st, MQMHASP)
-            check(lib.xvb_ecapa_create(C.byref(self._h), m.inputs_dim, m.layer1.affine.output_dim, st.in_dim,
-                                       st.hidden_size * st.num_head * st.num_q if mq else st.attention[0].out_channels,
-                                       m.embd_dim), "xvb_ecapa_create")
-            if mq:
-                check(lib.xvb_ecapa_set_mqmha(self._h, st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers,
-                                              int(st.time_attention), int(st.stddev)), "xvb_ecapa_set_mqmha")
-            for name, w, b, ctx, scale, shift, relu in _named_layers(m):
-                w = np.ascontiguousarray(w, dtype=np.float32)
-                w3 = w.reshape(w.shape[0], w.shape[1], -1)
-                arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in (b, scale, shift)]
-                ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
-                flags = (1 if relu else 0) | (2 if scale is not None else 0)
-                check(lib.xvb_ecapa_set_layer(self._h, name.encode(), w3.shape[0], w3.shape[1], int_array(ctx), len(ctx),
-                                              w3.ctypes.data_as(C.c_void_p), ptr[0], ptr[1], ptr[2], flags), "xvb_ecapa_set_layer")
-            check(lib.xvb_ecapa_finalize(self._h), "xvb_ecapa_finalize")
-        self.feat_dim = lib.xvb_ecapa_feat_dim(self._h)
-        self.embed_dim = lib.xvb_ecapa_embed_dim(self._h)
+    PREFIX = "ecapa"
 
-    @classmethod
-    def load(cls, path):
-        return cls(path=path)
+    def _create_args(self, m):
+        st = m.stats
+        hidden = st.hidden_size * st.num_head * st.num_q if isinstance(st, MQMHASP) else st.attention[0].out_channels
+        return m.inputs_dim, m.layer1.affine.output_dim, st.in_dim, hidden, m.embd_dim
 
-    def save(self, path):
-        self._check(self._lib.xvb_ecapa_save(self._h, str(path).encode()), "xvb_ecapa_save")
+    def _configure(self, m):
+        st = m.stats
+        if isinstance(st, MQMHASP):
+            self._call("set_mqmha", self._h, st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers,
+                       int(st.time_attention), int(st.stddev))
 
-    @property
-    def last_launches(self):
-        return self._lib.xvb_ecapa_last_launches(self._h)
-
-    def extract(self, feats):
-        if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
-            raise TypeError("feats must be a contiguous CUDA float32 tensor")
-        if feats.shape[2] != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
-        B, T, _ = feats.shape
-        emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
-        self._check(self._lib.xvb_ecapa_extract(self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()),
-                                                C.c_void_p(torch.cuda.current_stream().cuda_stream)), "xvb_ecapa_extract")
-        return emb
-
-    def extract_shard(self, feats, batch=128, out=None):
-        """feats (N,T,F) fp32 CUDA -> (N,D): the whole shard in `batch`-utterance batches, one C call."""
-        if not (isinstance(feats, torch.Tensor) and feats.is_cuda and feats.dtype == torch.float32 and feats.is_contiguous()):
-            raise TypeError("feats must be a contiguous CUDA float32 tensor")
-        n, t, f = feats.shape
-        if f != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
-        emb = out if out is not None else torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
-        C = self._C
-        self._check(self._lib.xvb_ecapa_extract_shard(self._h, C.c_void_p(feats.data_ptr()), n, t, int(batch),
-                                                      C.c_void_p(emb.data_ptr()),
-                                                      C.c_void_p(torch.cuda.current_stream().cuda_stream)), "xvb_ecapa_extract_shard")
-        return emb
-
-    def set_gather(self, pointers, ntables, row0, ld):
-        """Replicated-table form of the shard calls (parallel.PeerTable.attach)."""
-        self._check(self._lib.xvb_ecapa_set_gather(self._h, pointers, int(ntables), int(row0), int(ld)), "xvb_ecapa_set_gather")
-
-    def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=128):
-        """Pinned host feats (n,t,F) in, host embeddings (n,D) out; copies overlap the stack."""
-        C = self._C
-        self._check(self._lib.xvb_ecapa_extract_shard_host(self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch),
-                                                           C.c_void_p(emb_ptr),
-                                                           C.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                    "xvb_ecapa_extract_shard_host")
-
-    def extract_host(self, feats_np):
-        """feats (B,T,F) float32 host array -> (B,D) float32 host array (H2D + D2H + one sync inside the call)."""
-        feats_np = np.ascontiguousarray(feats_np, dtype=np.float32)
-        b, t, f = feats_np.shape
-        if f != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
-        emb = np.empty((b, self.embed_dim), dtype=np.float32)
-        C = self._C
-        self._check(self._lib.xvb_ecapa_extract_host(self._h, feats_np.ctypes.data_as(C.c_void_p), b, t,
-                                                     emb.ctypes.data_as(C.c_void_p),
-                                                     C.c_void_p(torch.cuda.current_stream().cuda_stream)), "xvb_ecapa_extract_host")
-        return emb
-
-    def close(self):
-        h, self._h = self._h, None
-        if h:
-            self._lib.xvb_ecapa_destroy(h)
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+    def _layers(self, m):
+        from asv_subtools_b200._lib import int_array
+        for name, w, b, ctx, scale, shift, relu in _named_layers(m):
+            w = np.asarray(w, dtype=np.float32)
+            w3 = w.reshape(w.shape[0], w.shape[1], -1)
+            yield name, (w3.shape[0], w3.shape[1], int_array(ctx), len(ctx)), (w3, b, scale, shift), \
+                (1 if relu else 0) | (2 if scale is not None else 0)
 
 
 class EcapaExtractor:

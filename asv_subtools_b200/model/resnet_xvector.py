@@ -18,7 +18,6 @@ The launch sequence runs in the native handle (NativeResNetExtractor over xvb_re
 also writes XVBR0001 model files for bin/xvb-extract.  XVB_RESNET_NATIVE=0 selects ResNetExtractor, the Python driver of
 the same kernels in the same order, whose embeddings are bit-identical."""
 import copy
-import ctypes as C
 import os
 import sys
 
@@ -29,7 +28,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
-from asv_subtools_b200.native import NativeExtractor, _cuda_f32  # noqa: E402
+from asv_subtools_b200.native import ShardExtractor  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
@@ -362,7 +361,7 @@ class ResNetExtractor:
         pass
 
 
-class NativeResNetExtractor(NativeExtractor):
+class NativeResNetExtractor(ShardExtractor):
     """xvb_resnet_t: packed weights, workspace and the whole launch sequence of ResNetExtractor in the C library, on the
     device that is current when it is built (or loaded from an XVBR0001 file)."""
 
@@ -380,30 +379,6 @@ class NativeResNetExtractor(NativeExtractor):
             cout = (w if w is not None else scale).shape[0]
             cin, k = (w.shape[1], w.shape[2] if w.ndim == 4 else 1) if w is not None else (0, 0)
             yield name, (cout, cin, k), (w, b, scale, shift), (1 if relu else 0) | (2 if scale is not None else 0)
-
-    def extract_host(self, feats_np):
-        """feats (B, T, F) float32 host array -> (B, D) float32 host array (H2D + D2H + one sync inside the call)."""
-        feats_np = np.ascontiguousarray(feats_np, dtype=np.float32)
-        b, t, f = feats_np.shape
-        if f != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
-        emb = np.empty((b, self.embed_dim), dtype=np.float32)
-        self._check(self._lib.xvb_resnet_extract_host(self._h, feats_np.ctypes.data_as(C.c_void_p), b, t,
-                                                      emb.ctypes.data_as(C.c_void_p), self._stream()), "xvb_resnet_extract_host")
-        return emb
-
-    def extract_shard(self, feats, batch=128, out=None):
-        """feats (N, T, F) fp32 CUDA -> (N, D): the whole shard in `batch`-utterance batches, one C call."""
-        n, t, _ = _cuda_f32(feats, self.feat_dim).shape
-        emb = out if out is not None else torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
-        self._check(self._lib.xvb_resnet_extract_shard(self._h, C.c_void_p(feats.data_ptr()), n, t, int(batch),
-                                                       C.c_void_p(emb.data_ptr()), self._stream()), "xvb_resnet_extract_shard")
-        return emb
-
-    def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=128):
-        """Pinned host feats (n, t, F) in, host embeddings (n, D) out; copies overlap the stack."""
-        self._check(self._lib.xvb_resnet_extract_shard_host(self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch),
-                                                            C.c_void_p(emb_ptr), self._stream()), "xvb_resnet_extract_shard_host")
 
 
 if __name__ == "__main__":

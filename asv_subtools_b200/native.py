@@ -1,7 +1,8 @@
-"""Python handles over the native whole-model extractors of the C library that take named records: the ResNet
-(xvb_resnet_*), RepVGG / RepSPK (xvb_repvgg_*), Conformer (xvb_conformer_*) and CAM++ (xvb_campp_*) x-vectors.
-NativeExtractor holds the part they share: create, set_layer per record and finalize (or load a model file), save,
-extract and close."""
+"""Python handles over the native whole-model extractors of the C library: the TDNN (xvb_extractor_*, ops.Extractor),
+ECAPA-TDNN (xvb_ecapa_*), ResNet (xvb_resnet_*), RepVGG / RepSPK (xvb_repvgg_*), Conformer (xvb_conformer_*) and CAM++
+(xvb_campp_*) x-vectors.  NativeExtractor holds the part they share: create, set_layer per record and finalize (or load
+a model file), save, extract and close; ShardExtractor adds the host-buffer and whole-shard calls of the TDNN, ECAPA-TDNN
+and ResNet handles."""
 import ctypes as C
 
 import numpy as np
@@ -20,9 +21,10 @@ class NativeExtractor:
     """xvb_<PREFIX>_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
     current when it is built from a model `m` (or loaded from a model file at `path`).
 
-    A family sets PREFIX and supplies `_create_args(m)`, the arguments of xvb_<PREFIX>_create after the handle, and
-    `_layers(m)`, which yields (name, shape, (w, b, scale, shift), flags) per record, `shape` being the set_layer
-    arguments between the name and the arrays."""
+    A family sets PREFIX and supplies `_create_args(m)`, the arguments of xvb_<PREFIX>_create after the handle,
+    `_configure(m)`, any call between create and the first set_layer, and `_layers(m)`, which yields
+    (name, shape, (w, b, scale, shift), flags) per record, `shape` being the set_layer arguments between the name and
+    the arrays."""
 
     PREFIX = None
 
@@ -35,6 +37,7 @@ class NativeExtractor:
                 self._call("load", C.byref(self._h), str(path).encode())
             else:
                 self._call("create", C.byref(self._h), *self._create_args(m))
+                self._configure(m)
                 for name, shape, arrays, flags in self._layers(m):
                     arrs = [None if a is None else np.ascontiguousarray(a, dtype=np.float32) for a in arrays]
                     ptr = [None if a is None else a.ctypes.data_as(C.c_void_p) for a in arrs]
@@ -42,6 +45,9 @@ class NativeExtractor:
                 self._call("finalize", self._h)
         self.feat_dim = self._fn("feat_dim")(self._h)
         self.embed_dim = self._fn("embed_dim")(self._h)
+
+    def _configure(self, m):
+        pass
 
     def _fn(self, name):
         return getattr(self._lib, "xvb_{}_{}".format(self.PREFIX, name))
@@ -86,3 +92,45 @@ class NativeExtractor:
             self.close()
         except Exception:
             pass
+
+
+class ShardExtractor(NativeExtractor):
+    """A handle with xvb_<PREFIX>_extract_host, _extract_shard, _extract_shard_host and (where the family has it)
+    _set_gather; `batch` is the default batch of the shard calls."""
+
+    batch = 128
+
+    def extract_host(self, feats_np):
+        """feats (B, T, F) float32 host array -> (B, D) float32 host array (H2D + D2H + one sync inside the call)."""
+        feats_np = np.ascontiguousarray(feats_np, dtype=np.float32)
+        b, t, f = feats_np.shape
+        if f != self.feat_dim:
+            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
+        emb = np.empty((b, self.embed_dim), dtype=np.float32)
+        self._call("extract_host", self._h, feats_np.ctypes.data_as(C.c_void_p), b, t, emb.ctypes.data_as(C.c_void_p),
+                   self._stream())
+        return emb
+
+    def extract_shard(self, feats, batch=None, out=None):
+        """feats (N, T, F) fp32 CUDA -> (N, D) fp32 CUDA (`out` if given): the whole shard in `batch`-utterance batches,
+        one C call (extract_embeddings.py:73-83's loop), asynchronous on the current stream."""
+        n, t, _ = self._input(feats).shape
+        if out is None:
+            out = torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
+        elif not (isinstance(out, torch.Tensor) and out.is_cuda and out.dtype == torch.float32 and out.is_contiguous()):
+            raise TypeError("out must be a contiguous CUDA float32 tensor")
+        elif tuple(out.shape) != (n, self.embed_dim):
+            raise ValueError("out must be ({}, {})".format(n, self.embed_dim))
+        self._call("extract_shard", self._h, C.c_void_p(feats.data_ptr()), n, t, int(batch or self.batch),
+                   C.c_void_p(out.data_ptr()), self._stream())
+        return out
+
+    def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=None):
+        """Pinned host feats (n, t, F) in, host embeddings (n, D) out; the copies overlap the stack."""
+        self._call("extract_shard_host", self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch or self.batch),
+                   C.c_void_p(emb_ptr), self._stream())
+
+    def set_gather(self, pointers, ntables, row0, ld):
+        """Replicated-table form of the shard calls (parallel.PeerTable.attach): every batch's embeddings also go to
+        `ntables` table copies at row0 + row; ntables = 0 turns it off."""
+        self._call("set_gather", self._h, pointers, int(ntables), int(row0), int(ld))

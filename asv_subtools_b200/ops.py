@@ -7,6 +7,7 @@ import torch
 
 from . import _lib
 from ._lib import BN, RELU, SIGMOID, SWISH, TANH, TdnnArgs, check, int_array, lib  # noqa: F401
+from .native import ShardExtractor
 
 
 def _stream():
@@ -734,15 +735,20 @@ def trial_histogram(enroll, enroll_spk, test, test_spk, lo, hi, nbins=2048, row_
 
 
 # ------------------------------------------------------------------ whole-model extractor
-class Extractor:
-    """Owner of a native xvb_extractor_t (packed weights + workspace on the current device)."""
+class Extractor(ShardExtractor):
+    """Owner of a native xvb_extractor_t (packed weights + workspace on the current device), built layer by layer with
+    add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file."""
+
+    PREFIX = "extractor"
+    batch = 256
 
     def __init__(self, feat_dim):
+        self._lib, self._check = lib, check
         self._h = C.c_void_p()
         check(lib.xvb_extractor_create(C.byref(self._h), int(feat_dim)), "xvb_extractor_create")
         self.feat_dim = int(feat_dim)
         self._keep = []
-        self._layers = []      # (kind, context, w, b, scale, shift, flags): what save() writes
+        self._saved = []      # (kind, context, w, b, scale, shift, flags): what save() writes
         self._eps = None
 
     @staticmethod
@@ -760,7 +766,7 @@ class Extractor:
         flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0)
         check(lib.xvb_extractor_add_frame_layer(self._h, w.shape[0], int_array(context), len(context), wp, bp, sp, tp,
                                                 flags), "xvb_extractor_add_frame_layer")
-        self._layers.append(("frame", [int(c) for c in context], w, b, s, t, flags))
+        self._saved.append(("frame", [int(c) for c in context], w, b, s, t, flags))
 
     def add_segment_layer(self, weight, bias, bn_scale=None, bn_shift=None, relu=False):
         w, wp = self._np(weight)
@@ -770,7 +776,7 @@ class Extractor:
         flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0)
         check(lib.xvb_extractor_add_segment_layer(self._h, w.shape[0], wp, bp, sp, tp, flags),
               "xvb_extractor_add_segment_layer")
-        self._layers.append(("segment", [0], w, b, s, t, flags))
+        self._saved.append(("segment", [0], w, b, s, t, flags))
 
     def finalize(self, pooling_eps=1e-10):
         check(lib.xvb_extractor_finalize(self._h, pooling_eps), "xvb_extractor_finalize")
@@ -783,8 +789,8 @@ class Extractor:
         import struct
         if self._eps is None:
             raise RuntimeError("Extractor.save: finalize() first")
-        frames = [l for l in self._layers if l[0] == "frame"]
-        segs = [l for l in self._layers if l[0] == "segment"]
+        frames = [l for l in self._saved if l[0] == "frame"]
+        segs = [l for l in self._saved if l[0] == "segment"]
         with open(path, "wb") as f:
             f.write(b"XVBM0001" + struct.pack("<ifii", self.feat_dim, self._eps, len(frames), len(segs)))
             for _, ctx, w, b, s, t, flags in frames + segs:
@@ -802,11 +808,12 @@ class Extractor:
     def load(cls, path):
         """An extractor straight from an .xvbm file (no Python-side layer objects)."""
         self = cls.__new__(cls)
+        self._lib, self._check = lib, check
         self._h = C.c_void_p()
         check(lib.xvb_extractor_load(C.byref(self._h), str(path).encode()), "xvb_extractor_load")
         self.feat_dim = lib.xvb_extractor_feat_dim(str(path).encode())
         self.embed_dim = lib.xvb_extractor_embed_dim(self._h)
-        self._keep, self._layers, self._eps = [], [], None
+        self._keep, self._saved, self._eps = [], [], None
         return self
 
     def extract(self, feats, lengths=None):
@@ -831,17 +838,6 @@ class Extractor:
                                                 _stream()), "xvb_extractor_extract_lengths")
         return emb
 
-    def extract_host(self, feats_np):
-        """feats (B,T,F) float32 host array -> (B,D) float32 host array (H2D + D2H inside the call)."""
-        feats_np = np.ascontiguousarray(feats_np, dtype=np.float32)
-        b, t, f = feats_np.shape
-        if f != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
-        emb = np.empty((b, self.embed_dim), dtype=np.float32)
-        check(lib.xvb_extractor_extract_host(self._h, feats_np.ctypes.data_as(C.c_void_p), b, t,
-                                             emb.ctypes.data_as(C.c_void_p), _stream()), "xvb_extractor_extract_host")
-        return emb
-
     def submit_host(self, feats_ptr, b, t, emb_ptr, slot):
         """Pipelined host path: queue batch `slot` (0/1); pair with wait(slot)."""
         check(lib.xvb_extractor_submit_host(self._h, C.c_void_p(feats_ptr), b, t, C.c_void_p(emb_ptr), slot, _stream()),
@@ -849,32 +845,6 @@ class Extractor:
 
     def wait(self, slot):
         check(lib.xvb_extractor_wait(self._h, slot), "xvb_extractor_wait")
-
-    def extract_shard(self, feats, batch=256, out=None):
-        """feats (N,T,F) fp32 CUDA -> (N,D) fp32 CUDA: the whole shard in `batch`-utterance batches, one C call
-        (extract_embeddings.py:73-83's loop), asynchronous on the current stream."""
-        feats = _req(feats, torch.float32, "feats")
-        n, t, f = feats.shape
-        if f != self.feat_dim:
-            raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, f))
-        emb = out if out is not None else torch.empty(n, self.embed_dim, dtype=torch.float32, device=feats.device)
-        if out is not None:
-            _req(out, torch.float32, "out")
-            if tuple(out.shape) != (n, self.embed_dim):
-                raise ValueError("out must be ({}, {})".format(n, self.embed_dim))
-        check(lib.xvb_extractor_extract_shard(self._h, _ptr(feats), n, t, int(batch), _ptr(emb), _stream()),
-              "xvb_extractor_extract_shard")
-        return emb
-
-    def extract_shard_host(self, feats_ptr, n, t, emb_ptr, batch=256):
-        """Host-buffer shard call (pinned feats in, embeddings out, copies overlapped with the stack)."""
-        check(lib.xvb_extractor_extract_shard_host(self._h, C.c_void_p(feats_ptr), int(n), int(t), int(batch),
-                                                   C.c_void_p(emb_ptr), _stream()), "xvb_extractor_extract_shard_host")
-
-    def set_gather(self, pointers, ntables, row0, ld):
-        """Replicated-table form of the shard calls (parallel.PeerTable.attach): every batch's embeddings also go to
-        `ntables` table copies at row0 + row; ntables = 0 turns it off."""
-        check(lib.xvb_extractor_set_gather(self._h, pointers, int(ntables), int(row0), int(ld)), "xvb_extractor_set_gather")
 
     def extract_host_into(self, feats_ptr, b, t, emb_ptr):
         check(lib.xvb_extractor_extract_host(self._h, C.c_void_p(feats_ptr), b, t, C.c_void_p(emb_ptr), _stream()),
@@ -896,10 +866,6 @@ class Extractor:
             check(n, "xvb_extractor_kernel_times")
         return [float(buf[i]) for i in range(n)]
 
-    @property
-    def last_launches(self):
-        return lib.xvb_extractor_last_launches(self._h)
-
     def debug_f32(self, which, shape):
         """View of an internal fp32 buffer of the last call (which=-1: pooled stats, 0: last frame layer)."""
         ptr = lib.xvb_extractor_debug_f32(self._h, which)
@@ -912,14 +878,3 @@ class Extractor:
 
         torch.cuda.synchronize()
         return torch.as_tensor(_DevPtr(), device="cuda").clone()
-
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h:
-            lib.xvb_extractor_destroy(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass

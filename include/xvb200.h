@@ -608,11 +608,17 @@ int xvb_extractor_submit_host(xvb_extractor_t* h, const float* feats_host, int B
 int xvb_extractor_wait(xvb_extractor_t* h, int slot);
 /* A whole shard of N equal-length utterances -- the caller loop of the reference
  * (pytorch/pipeline/onestep/extract_embeddings.py:73-83, one utterance per iteration; sharded over `nj` jobs by
- * extract_xvectors_for_pytorch.sh:125-136) as ONE call: ceil(N / batch) batches through the stack back to back.
+ * extract_xvectors_for_pytorch.sh:125-136) as ONE call: ceil(N / batch) batches through the stack.  One protocol for
+ * the TDNN, ECAPA-TDNN and ResNet handles:
  *   _shard      : feats (N, T, feat_dim) and emb (N, embed_dim) on the device; asynchronous on `stream`;
- *   _shard_host : the same through host buffers (pinned, so that the copies overlap): batch i+1 crosses the link
- *                 while batch i runs (the submit/wait protocol above); returns when emb_host is complete.
- * Launch plans (tensor maps, tile geometry) are cached per batch shape, so a batch costs its launches only. */
+ *   _shard_host : the same through host buffers (pinned, so that the copies overlap): batch k crosses the link on a
+ *                 copy stream into device slot k % 4 while earlier batches run; returns when emb_host is complete.
+ *                 Refused while a submit_host slot is in flight.
+ * Batch k runs on lane k & 1: the handle itself and a twin on the same weights with its own workspace (made on first
+ * use, kept until destroy), each on its own stream forked from `stream` and joined back into it.  There are two lanes
+ * only when N > batch; XVB_LANES=0 in the environment (read on every call) and per-kernel profiling keep one lane,
+ * on `stream`.  Launch plans (tensor maps, tile geometry) are cached per batch shape, so a batch costs its launches
+ * only; last_launches after a shard call is the sum over its batches, xvb_scatter_rows launches included. */
 int xvb_extractor_extract_shard(xvb_extractor_t* h, const float* feats, int64_t N, int T, int batch, float* emb,
                                 void* stream);
 int xvb_extractor_extract_shard_host(xvb_extractor_t* h, const float* feats_host, int64_t N, int T, int batch,
@@ -626,7 +632,8 @@ int xvb_extractor_extract_shard_host(xvb_extractor_t* h, const float* feats_host
  * store every batch's embeddings into ALL copies at row0 + (row inside the shard) as soon as the batch's last layer
  * has produced them (xvb_scatter_rows on the batch's stream), overlapped with the following batches; the caller ends
  * the step with a barrier.  tables[k], k < ntables: base pointers valid in THIS process (own copy included);
- * ntables = 0 turns it off.  `emb` of the shard call still receives the rank's own rows.
+ * ntables = 0 turns it off.  `emb` of the shard call still receives the rank's own rows.  Every batch of every shard
+ * call stores, on one lane or two, with profiling on or off; each store is one launch in last_launches.
  * ------------------------------------------------------------------------------------------- */
 #define XVB_MAX_PEERS 16
 #define XVB_IPC_HANDLE_BYTES 64
@@ -720,7 +727,8 @@ int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int T, float* e
 /* Same through host buffers (H2D of feats, D2H of emb inside; synchronises the stream). */
 int xvb_ecapa_extract_host(xvb_ecapa_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream);
 /* Whole shard of N equal-length utterances in `batch`-utterance batches (extract_embeddings.py:73-83's loop as one
- * call): device-resident and asynchronous, or through pinned host buffers with the copies overlapped. */
+ * call): device-resident and asynchronous, or through pinned host buffers with the copies overlapped; the protocol of
+ * xvb_extractor_extract_shard[_host]. */
 int xvb_ecapa_extract_shard(xvb_ecapa_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream);
 /* the replicated-table form of the shard calls, see xvb_extractor_set_gather */
 int xvb_ecapa_set_gather(xvb_ecapa_t* h, float* const* tables, int ntables, int64_t row0, int64_t ld);
@@ -772,8 +780,8 @@ int xvb_resnet_last_launches(const xvb_resnet_t* h);
 int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream);
 /* Same through host buffers (H2D of feats, D2H of emb inside; synchronises the stream). */
 int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream);
-/* Whole shard of N equal-length utterances in `batch`-utterance batches, as xvb_ecapa_extract_shard[_host]: batches
- * alternate between two lanes (XVB_LANES=0: one), pinned host buffers are copied on a copy stream. */
+/* Whole shard of N equal-length utterances in `batch`-utterance batches: the protocol of
+ * xvb_extractor_extract_shard[_host]. */
 int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream);
 int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int64_t N, int T, int batch,
                                   float* emb_host, void* stream);

@@ -238,17 +238,29 @@ def test_ecapa_vs_oracle_batch():
         assert rel(got[i], ref[i]) < EMB_TOL
 
 
-def test_ecapa_shard_calls_on_two_lanes_equal_per_batch_extraction():
-    """xvb_ecapa_extract_shard[_host]: batches alternate between the two lanes (twin workspaces, two streams) and must
-    reproduce independent per-batch calls bit for bit, ragged tail batch included; C3's full batch size (128 x 300) is
-    checked against sub-batches of itself (batch invariance at the BASELINE shape)."""
+def test_ecapa_shard_calls_on_two_lanes_equal_per_batch_extraction(monkeypatch):
+    """xvb_ecapa_extract_shard[_host]: batches alternate between the two lanes (twin workspaces, two streams; one lane
+    with XVB_LANES=0) and must reproduce independent per-batch calls bit for bit, ragged tail batch, a single batch and
+    whole batches included, as must xvb_ecapa_extract_host; C3's full batch size (128 x 300) is checked against
+    sub-batches of itself (batch invariance at the BASELINE shape).  One handle serves both settings: XVB_LANES is read
+    on every shard call."""
     m, _ = _model("near")
     ex = m.extractor()
     n, t = 11, 47
     feats = torch.from_numpy(onn.synthetic_feats(n, t, 80, 777)).cuda()
     want = torch.cat([ex.extract(feats[i:i + 4]).clone() for i in range(0, n, 4)])         # batches of 4, 4, 3
+    for lanes in ("0", "1"):
+        monkeypatch.setenv("XVB_LANES", lanes)
+        _check_ecapa_shard(ex, feats, want)
+
+
+def _check_ecapa_shard(ex, feats, want):
+    n, t, _ = feats.shape
     assert torch.equal(ex.extract_shard(feats, 4), want)
     assert torch.equal(ex.extract_shard(feats, 4), want)                                    # lanes reused
+    assert torch.equal(ex.extract_shard(feats[:3], 4), ex.extract(feats[:3]))               # N <= batch
+    assert torch.equal(ex.extract_shard(feats[:8], 4), want[:8])                            # N a multiple of batch
+    assert np.array_equal(ex.extract_host(feats[:4].cpu().numpy()), want[:4].cpu().numpy())
     host = torch.empty(n, t, 80, dtype=torch.float32, pin_memory=True)
     host.copy_(feats)
     out = torch.empty(n, ex.embed_dim, dtype=torch.float32, pin_memory=True)

@@ -359,18 +359,41 @@ def test_snowdar_xvector_matches_reference_golden(golden, cname, extend, seed):
         Xvector(40, 10, SE=True)
 
 
-def test_replicated_table_hooks_store_every_batch_into_every_copy():
-    """xvb_extractor_set_gather + xvb_scatter_rows on ONE GPU (csrc/peer.cu; the multi-process NVLink form is
-    tools/peer_table_check.py under torchrun): two table copies allocated with xvb_ipc_alloc, the shard call (device
-    and host-buffer forms, two lanes, ragged tail batch) fills both at the rank's row offset and still returns its own
-    rows; turning the hook off stops the stores."""
+def _ecapa_model():
+    from asv_subtools_b200.model.ecapa_tdnn_xvector import ECAPA_TDNN
+    m = ECAPA_TDNN(80, 10, training=False)
+    m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(80, fc2_bn_affine=True), 201), strict=True)
+    return m.cuda().eval()
+
+
+def test_replicated_table_hooks_store_every_batch_into_every_copy(monkeypatch):
+    """xvb_extractor_set_gather / xvb_ecapa_set_gather + xvb_scatter_rows on ONE GPU (csrc/peer.cu; the multi-process
+    NVLink form is tools/peer_table_check.py under torchrun): two table copies allocated with xvb_ipc_alloc, the shard
+    call (device and host-buffer forms, one or two lanes, ragged tail batch, TDNN with per-kernel profiling on too) fills
+    both at the rank's row offset, still returns its own rows and counts one scatter launch per batch; turning the hook
+    off stops the stores."""
+    for family, lanes, profiling in [("tdnn", "0", False), ("tdnn", "1", False), ("tdnn", "1", True), ("ecapa", "0", False),
+                                     ("ecapa", "1", False)]:
+        _check_replicated_table(monkeypatch, family, lanes, profiling)
+
+
+def _check_replicated_table(monkeypatch, family, lanes, profiling):
     import ctypes as C
     from asv_subtools_b200._lib import check, lib
-    m, _ = _model(80, 102, "far")
-    ex = m.extractor()
-    n, t, d, row0, rows = 150, 61, 512, 40, 256
+    monkeypatch.setenv("XVB_LANES", lanes)
+    ex = _model(80, 102, "far")[0].extractor() if family == "tdnn" else _ecapa_model().extractor()
+    n, t, row0, rows, batch = 150, 61, 40, 256, 64
+    d = ex.embed_dim
     feats = torch.from_numpy(onn.synthetic_feats(n, t, 80, 919)).cuda()
-    want = ex.extract_shard(feats, 64).clone()
+    want, per_batch = [], 0
+    for i in range(0, n, batch):
+        want.append(ex.extract(feats[i:i + batch]).clone())
+        per_batch += ex.last_launches
+    want = torch.cat(want)
+    assert torch.equal(ex.extract_shard(feats, batch), want)
+    assert ex.last_launches == per_batch
+    if profiling:
+        ex.set_profiling(True)
     ptrs = (C.c_void_p * 2)()
     for k in range(2):
         p = C.c_void_p()
@@ -388,24 +411,27 @@ def test_replicated_table_hooks_store_every_batch_into_every_copy():
         ex.set_gather(ptrs, 2, row0, d)
         for tb in tabs:
             tb.fill_(-7.0)
-        got = ex.extract_shard(feats, 64)
+        got = ex.extract_shard(feats, batch)
         torch.cuda.synchronize()
-        assert torch.equal(got, want)
+        assert torch.equal(got, want) and ex.last_launches == per_batch + 3
         for tb in tabs:
             assert torch.equal(tb[row0:row0 + n], want) and bool((tb[:row0] == -7.0).all()) and bool((tb[row0 + n:] == -7.0).all())
         host = torch.empty(n, t, 80, dtype=torch.float32, pin_memory=True)
         host.copy_(feats)
         out = torch.empty(n, d, dtype=torch.float32, pin_memory=True)
         tabs[1].fill_(-7.0)
-        ex.extract_shard_host(host.data_ptr(), n, t, out.data_ptr(), 64)
+        ex.extract_shard_host(host.data_ptr(), n, t, out.data_ptr(), batch)
         assert torch.equal(out, want.cpu()) and torch.equal(tabs[1][row0:row0 + n], want)
+        assert ex.last_launches == per_batch + 3
         ex.set_gather(None, 0, 0, 0)
         tabs[0].fill_(-7.0)
-        ex.extract_shard(feats, 64)
+        ex.extract_shard(feats, batch)
         torch.cuda.synchronize()
         assert bool((tabs[0] == -7.0).all())
     finally:
         ex.set_gather(None, 0, 0, 0)
+        if profiling:
+            ex.set_profiling(False)
         torch.cuda.synchronize()
         del tabs
         for k in range(2):
@@ -555,12 +581,15 @@ def test_factored_xvector_matches_reference_golden(golden, pos):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("lanes", ["0", "1"])
 @pytest.mark.parametrize("pos", ["far", "near"])
-def test_shard_calls_and_cached_launch_plans_equal_per_batch_extraction(pos):
+def test_shard_calls_and_cached_launch_plans_equal_per_batch_extraction(monkeypatch, pos, lanes):
     """xvb_extractor_extract_shard[_host] (the reference's caller loop, extract_embeddings.py:73-83, as one call) and
-    the per-(B, T) launch-plan cache: a shard in ragged batches, the same shard through pinned host buffers, and batch
-    shapes revisited in a different order all reproduce independent per-batch calls bit for bit ("far": split-K last
-    layer, reduce kernel redirected; "near": the last layer's output map re-encoded per destination)."""
+    the per-(B, T) launch-plan cache: a shard in ragged batches, one of a single batch and one of whole batches, the same
+    shard through pinned host buffers, and batch shapes revisited in a different order all reproduce independent
+    per-batch calls bit for bit, on one lane or two ("far": split-K last layer, reduce kernel redirected; "near": the
+    last layer's output map re-encoded per destination)."""
+    monkeypatch.setenv("XVB_LANES", lanes)
     m, _ = _model(80, 102, pos)
     ex = m.extractor()
     n, t = 150, 61
@@ -569,6 +598,9 @@ def test_shard_calls_and_cached_launch_plans_equal_per_batch_extraction(pos):
     got = ex.extract_shard(feats, 64)
     assert torch.equal(got, want)
     assert ex.last_launches >= 3 * 8
+    assert torch.equal(ex.extract_shard(feats[:50], 64), ex.extract(feats[:50]))          # N <= batch
+    assert torch.equal(ex.extract_shard(feats[:128], 64), want[:128])                     # N a multiple of batch
+    assert np.array_equal(ex.extract_host(feats[:64].cpu().numpy()), want[:64].cpu().numpy())
     other = torch.from_numpy(onn.synthetic_feats(5, 33, 80, 910)).cuda()                  # another shape in between
     w_other = ex.extract(other).clone()
     assert torch.equal(ex.extract_shard(feats, 64), want) and torch.equal(ex.extract(other), w_other)

@@ -1,7 +1,8 @@
 """The named-record model files of the native ResNet (XVBR0001), Conformer (XVBC0001) and CAM++ (XVBP0001) extractors on
 the H100, over every case of the three families' fixtures: save() writes exactly the bytes of a writer of the documented
 layout fed the records the handle was built from; load() then save() reproduces the file byte for byte; and corrupt files
-are refused with an error naming the magic or the damage, without a crash."""
+are refused with an error naming the magic or the damage, without a crash.  The ECAPA-TDNN files (XVBE0001, XVBE0002
+with MQMHA pooling) are checked the same way against a writer of their own layout."""
 import struct
 
 import numpy as np
@@ -10,12 +11,15 @@ import pytest
 import campplus_oracle as po
 import conformer_2sub_oracle as c2
 import conformer_oracle as co
+import ecapa_mqmha_oracle as mo
 import resnet_oracle as ro
 from asv_subtools_b200._lib import CamPPConfig, ConformerConfig
 from asv_subtools_b200.model.campplus_xvector import CamPPXvector, NativeCamPPExtractor, native_config as campp_config
+from asv_subtools_b200.model.ecapa_tdnn_xvector import ECAPA_TDNN, NativeEcapaExtractor
 from asv_subtools_b200.model.resnet_xvector import NativeResNetExtractor, ResNetXvector
 from asv_subtools_b200.model.transformer_xvector import (NativeConformerExtractor, TransformerXvector,
                                                          native_config as conformer_config)
+from asv_subtools_b200.nnet.pooling import MQMHASP
 from oracle import nnet as onn
 
 pytestmark = pytest.mark.gpu
@@ -123,4 +127,47 @@ def test_model_file_bytes_roundtrip_and_rejects(tmp_path, golden, family, case):
             f.write(blob)
         with pytest.raises(RuntimeError, match=msg):
             cls.load(bad)
+    ex.close()
+
+
+def _ecapa_write(ex, m):
+    """xvb_ecapa_save's layout: magic | i32 feat_dim, channels, mfa_dim, att_hidden, embed_dim, nlayers | (XVBE0002) i32
+    num_head, num_q, hidden, share, affine_layers, time_attention, stddev | per layer i32 name_len | name | i32 Cout, Cin,
+    ntaps, tot, flags, has_b, has_s | i32 ctx[ntaps] | f32 w (Cout, Cin, tot) | f32 b? | f32 s, t?"""
+    layers = list(ex._layers(m))
+    st = m.stats
+    mq = isinstance(st, MQMHASP)
+    out = bytearray((b"XVBE0002" if mq else b"XVBE0001") + struct.pack("<6i", *ex._create_args(m), len(layers)))
+    if mq:
+        out += struct.pack("<7i", st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers,
+                           int(st.time_attention), int(st.stddev))
+    for name, (cout, cin, ctx, ntaps), (w, b, s, t), flags in layers:
+        out += struct.pack("<i", len(name)) + name.encode()
+        out += struct.pack("<7i", cout, cin, ntaps, w.shape[2], flags, b is not None, s is not None)
+        out += struct.pack("<%di" % ntaps, *ctx[:ntaps])
+        for a in (w, b, s, t):
+            if a is not None:
+                out += np.ascontiguousarray(a, dtype="<f4").tobytes()
+    return bytes(out)
+
+
+@pytest.mark.parametrize("magic", ["XVBE0001", "XVBE0002"])
+def test_ecapa_model_file_bytes_and_roundtrip(tmp_path, magic):
+    if magic == "XVBE0001":
+        m = ECAPA_TDNN(80, 10, training=False)
+        m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(80, fc2_bn_affine=True), 201), strict=True)
+    else:
+        kwargs, _, _, seed, _ = mo.CASES["fc1"]
+        m = ECAPA_TDNN(80, 10, training=False, extracted_embedding="near", **kwargs)
+        m.load_state_dict(onn.make_state_dict(mo.ecapa_mqmha_spec(kwargs), seed), strict=True)
+    m = m.cuda().eval()
+    ex = NativeEcapaExtractor(m)
+    path, again = str(tmp_path / "model.xvbm"), str(tmp_path / "again.xvbm")
+    ex.save(path)
+    data = open(path, "rb").read()
+    assert data[:8] == magic.encode() and data == _ecapa_write(ex, m)
+    loaded = NativeEcapaExtractor.load(path)
+    loaded.save(again)
+    loaded.close()
+    assert open(again, "rb").read() == data
     ex.close()
