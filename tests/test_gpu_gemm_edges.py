@@ -18,11 +18,10 @@ import pytest
 import torch
 
 import gemm_exact as gx
+from gpu_checks import Fenced as _Fenced, equal as _equal, profiled, within as _within
 
 pytestmark = pytest.mark.gpu
 
-SENT16 = 0x7FA5          # a NaN payload no kernel writes
-SENT32 = 0x7FA5A5A5
 SMS_FOR_IDS = 132        # case names do not depend on the SM count; shapes do (built from multi_processor_count)
 
 
@@ -53,25 +52,6 @@ def _tb(B, T):
     return tb.value
 
 
-def _equal(got, want, what):
-    got = np.asarray(got)
-    if np.array_equal(got, want):
-        return
-    bad = ~(got == want)
-    i = tuple(np.argwhere(bad)[0])
-    raise AssertionError("{}: {} of {} elements differ; first at {}: got {!r}, want {!r}".format(
-        what, int(bad.sum()), bad.size, i, got[i], want[i]))
-
-
-def _within(got, want, bound, what):
-    err = np.abs(np.asarray(got, dtype=np.float64) - want)
-    bad = ~(err <= bound)
-    if bad.any():
-        i = tuple(np.argwhere(bad)[0])
-        raise AssertionError("{}: {} elements outside the bound; first at {}: got {!r}, want {!r}, bound {!r}".format(
-            what, int(bad.sum()), i, got[i], want[i], bound[i]))
-
-
 def _poisoned(ops, hi, lo, c0, ld):
     """(B, ..., C) planes as the channel slice [c0, c0 + C) of (B + 1, ..., ld) buffers that hold NaN everywhere else."""
     B, Cn = hi.shape[0], hi.shape[-1]
@@ -81,26 +61,6 @@ def _poisoned(ops, hi, lo, c0, ld):
         buf[:B, ..., c0:c0 + Cn] = _dev(a).to(torch.bfloat16)
         bufs.append(buf)
     return ops.SplitPlanes(bufs[0][:B, ..., c0:c0 + Cn], bufs[1][:B, ..., c0:c0 + Cn], Cn)
-
-
-class _Fenced:
-    """A view inside a larger buffer that starts out as a sentinel bit pattern."""
-
-    def __init__(self, shape, dtype, index):
-        self.buf = torch.empty(shape, dtype=dtype, device="cuda")
-        self.sent = SENT16 if dtype == torch.bfloat16 else SENT32
-        self.bits = self.buf.view(torch.int16 if dtype == torch.bfloat16 else torch.int32)
-        self.bits.fill_(self.sent)
-        self.view = self.buf[index]
-        self.outside = torch.ones(shape, dtype=torch.bool, device="cuda")
-        self.outside[index] = False
-
-    def check(self, what):
-        n = int((self.bits[self.outside] != self.sent).sum())
-        assert n == 0, "{}: {} elements outside the output were written".format(what, n)
-
-    def numpy(self):
-        return self.view.float().cpu().numpy()
 
 
 def _fenced_planes(ops, shape, index, channels):
@@ -132,22 +92,8 @@ _KERNEL = re.compile(r"(tdnn_gemm_bf16x3_kernel|conv2d_bf16x3_kernel)<([^>]*)>")
 
 
 def _profiled(run):
-    """Calls run() under torch.profiler and returns the 'tdnn_gemm_bf16x3_kernel<128,false,false,false>'-style names of
-    the GEMM kernels it launched.  A short profiler session now and then returns no kernel records at all (seen on the
-    H100: 2 of about 120 sessions); every caller launches a GEMM kernel, so an empty capture is the profiler's miss and
-    is taken again, up to three times.  run() only rewrites the same outputs and checks them again."""
-    seen = set()
-    for _ in range(3):
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            run()
-            torch.cuda.synchronize()
-        for e in prof.events():
-            m = _KERNEL.search(e.name)
-            if m:
-                seen.add("{}<{}>".format(m.group(1), m.group(2).replace(" ", "")))
-        if seen:
-            break
-    return seen
+    """The 'tdnn_gemm_bf16x3_kernel<128,false,false,false>'-style names of the GEMM kernels run() launched."""
+    return profiled(run, _KERNEL)
 
 
 def _layer_name(block_n, pool=False, hist=False, swish=False):
