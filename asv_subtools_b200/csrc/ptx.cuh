@@ -147,6 +147,12 @@ template <int kPending>
 __device__ __forceinline__ void wgmma_wait() {
   asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory");
 }
+// Hand registers between warpgroups: every thread of the calling warpgroup must execute it.  dec frees registers to the
+// CTA's pool, inc waits until the pool has them.
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
 // keeps the compiler from moving accesses of the accumulators across wgmma_fence / wgmma_wait
 template <int R>
 __device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {

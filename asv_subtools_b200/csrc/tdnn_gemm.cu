@@ -12,9 +12,12 @@
 //   * fp32-grade accuracy at bf16 tensor rate: operands are bf16 "split planes" (hi, lo) and each
 //     K step issues hi*hi + lo*hi + hi*lo into the same fp32 accumulator;
 //   * warp-specialised persistent CTAs: one producer warp drives TMA through an mbarrier ring of
-//     operand stages, two consumer warpgroups (64 accumulator rows each) issue wgmma with the
-//     accumulators in registers and run the epilogue (+bias -> ReLU -> BN -> split -> st.global)
-//     while the producer already loads the next tile's operands.
+//     operand stages, two consumer warpgroups issue wgmma with the accumulators in registers and run
+//     the epilogue (+bias -> ReLU -> BN -> split -> st.global) while the producer already loads the
+//     next tile's operands.  The 128-wide layer and fused-pooling instances run the two warpgroups
+//     ping-pong: each one owns every other tile of the CTA whole (128 accumulator rows), so one
+//     warpgroup's epilogue runs under the other's MMAs.  The other instances split each tile
+//     between the two warpgroups (64 accumulator rows each).
 // Variants of the same kernel (template flags): kPool -- swapped operands, the epilogue pools over time
 // instead of storing (fused statistics pooling); kHist -- the epilogue bins scores into a trial histogram
 // (scoring.cu); runtime: a second A source (W.(a+b)), split-K slices for the segment layers, an im2col
@@ -38,10 +41,19 @@ namespace xvb {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;                      // bf16 elements = one 128-byte swizzle row
 constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB per plane per stage
-constexpr int kNumConsumers = 256;               // two warpgroups, 64 accumulator rows each
+constexpr int kNumConsumers = 256;               // two consumer warpgroups
 constexpr int kProducerWarp = kNumConsumers / 32;
-constexpr int kNumThreads = kNumConsumers + 32;  // + the TMA producer warp
 constexpr int kSlabBytes = 16384;                // trial histogram: 2 x hist_bins u32 counters
+
+// The instances whose two consumer warpgroups run ping-pong (see the kernel).  Each of their consumer threads holds a
+// whole 128 x 128 tile's share of accumulators (128 registers), more than fits in the 168 registers a thread of a
+// 288-thread CTA may use.  So they run a whole producer warpgroup (384 threads) that gives its registers to the consumers
+// with setmaxnreg: 40 for the producer, 232 for each consumer, 64512 in all as at launch (168 x 384).
+template <int BLOCK_N, bool kHist, bool kSwish>
+__host__ __device__ constexpr bool ping_pong() { return BLOCK_N == 128 && !kHist && !kSwish; }
+template <int BLOCK_N, bool kHist, bool kSwish>
+__host__ __device__ constexpr int gemm_threads() { return kNumConsumers + (ping_pong<BLOCK_N, kHist, kSwish>() ? 128 : 32); }
+constexpr uint32_t kProducerRegs = 40, kConsumerRegs = 232;
 
 struct TdnnGemmParams {
   int B, T, Cin, Cout;
@@ -168,8 +180,17 @@ __device__ __noinline__ void epi_zero_row(const TdnnGemmParams& p, long long gro
 
 // kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
 // one, so that the instantiations without it compile to the same code as before the flag existed.
+//
+// Ping-pong (the 128-wide layer and fused-pooling instances): tile j of the CTA's list (blockIdx.x + j * gridDim.x)
+// belongs to warpgroup j & 1, which computes all 128 of its rows as two m64 halves.  Each warpgroup finds its place in
+// the operand ring from a running count of the K blocks of all the CTA's tiles, the other warpgroup's included.  Both
+// wait on the ring's full barriers by phase parity, which only tells the phase being waited for from the one before it:
+// a warpgroup that started waiting on its next tile's first stage while the producer was still more than one lap of
+// the ring behind would take an older load of that stage for its own.  So the main loops take turns on named barriers
+// 2 + wg ("warpgroup wg may start its main loop"): a warpgroup starts one only after the other has issued the previous
+// tile's MMAs, and the epilogue of that tile then runs under the other's main loop.
 template <int BLOCK_N, bool kPool, bool kHist, bool kSwish = false>
-__global__ void __launch_bounds__(kNumThreads, 1)
+__global__ void __launch_bounds__(gemm_threads<BLOCK_N, kHist, kSwish>(), 1)
 tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                         const __grid_constant__ CUtensorMap map_a2_hi, const __grid_constant__ CUtensorMap map_a2_lo,
                         const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
@@ -179,6 +200,9 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
   constexpr int kBBytes = Cfg::kBBytes;
   constexpr int kStageBytes = Cfg::kStageBytes;
   static_assert(!kPool || BLOCK_N == kBlockM, "fused pooling: 128 channels x 128 frames per tile");
+  constexpr bool kPingPong = ping_pong<BLOCK_N, kHist, kSwish>();
+  constexpr int kHalves = kPingPong ? 2 : 1;                  // 64-row accumulator halves per consumer thread
+  constexpr int kReleaseWarps = kPingPong ? 4 : kNumConsumers / 32;   // warps that consume (and release) one stage
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment
@@ -197,7 +221,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     tma_prefetch_desc(&map_w_lo);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);                   // producer arrival + all TMA bytes
-      mbar_init(&empty_bar[i], kNumConsumers / 32); // one arrival per consumer warp
+      mbar_init(&empty_bar[i], kReleaseWarps);      // one arrival per consumer warp of the stage's warpgroup(s)
     }
     fence_barrier_init();
   }
@@ -212,9 +236,10 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 
   const int num_kblk = p.num_src * p.ntaps * p.num_cblk;
 
-  if (warp == kProducerWarp) {
+  if (warp >= kProducerWarp) {
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if constexpr (kPingPong) setmaxnreg_dec<kProducerRegs>();   // the whole producer warpgroup
+    if (warp == kProducerWarp && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
@@ -249,18 +274,29 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
   }
 
   // ================================ consumers: wgmma + epilogue ================================
-  const int wg = warp >> 2;                          // accumulator rows 64*wg .. 64*wg+63
+  if constexpr (kPingPong) setmaxnreg_inc<kConsumerRegs>();
+  const int wg = warp >> 2;                         // split tiles: accumulator rows 64*wg .. 64*wg+63
   const int q4 = lane & 3;
-  const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+  const int row_base = kPingPong ? 0 : 64 * wg;      // first accumulator row of this warpgroup's (first) half
+  // this thread's rows: row0 + 64 * hh + 8 * h for half hh < kHalves and h < 2
+  const int row0 = row_base + 16 * (warp & 3) + (lane >> 2);
   const int etid = threadIdx.x;                      // 0..255
   const bool relu = (p.flags & XVB_RELU) != 0;
   const bool bn = (p.flags & XVB_BN) != 0;
   const bool act_sigmoid = (p.flags & XVB_SIGMOID) != 0;
   const bool act_tanh = (p.flags & XVB_TANH) != 0;
   const float relu_floor = relu ? 0.f : -INFINITY;   // branch-free ReLU switch
-  float acc[Cfg::kAccRegs];
+  float acc[kHalves][Cfg::kAccRegs];
 #pragma unroll
-  for (int i = 0; i < Cfg::kAccRegs; ++i) acc[i] = 0.f;
+  for (int hh = 0; hh < kHalves; ++hh)
+#pragma unroll
+    for (int i = 0; i < Cfg::kAccRegs; ++i) acc[hh][i] = 0.f;
+  // The epilogues take the halves one after the other through the same code on acc[0] (a rolled loop): unrolled over
+  // both, the ping-pong instances' code was twice as large, more than the instruction cache holds.
+  auto half_down = [&]() {
+#pragma unroll
+    for (int i = 0; i < Cfg::kAccRegs; ++i) acc[0][i] = acc[kHalves - 1][i];
+  };
   int stage = 0;
   uint32_t phase = 0;
   uint32_t it = 0;
@@ -293,15 +329,25 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     asm volatile("bar.sync 1, 256;" ::: "memory");
   }
 
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+  int tj = 0;                                        // index of the tile in the CTA's list
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tj) {
     int m_unit, n_blk, slice;
     if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;
-    ++it;
     int kb_begin = 0, kb_end = num_kblk;
     if (p.k_slices > 1) {
       kb_begin = slice * p.kb_per_slice;
       kb_end = min(num_kblk, kb_begin + p.kb_per_slice);
     }
+    if constexpr (kPingPong) {
+      if ((tj & 1) != wg) {                          // the other warpgroup's tile: skip its stages in the ring
+        stage += kb_end - kb_begin;
+        phase ^= (uint32_t)(stage / kStages) & 1u;
+        stage %= kStages;
+        continue;
+      }
+      if (tj > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
+    }
+    ++it;
     // ---- main loop: one k block (64 channels of one tap and source) per operand stage
     int prev_stage = -1;
     uint32_t scale_d = 0;                            // the tile's first MMA overwrites the accumulators
@@ -310,9 +356,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       const uint32_t sa = smem_u32(smem + stage * kStageBytes);
       const uint64_t dx_hi = make_sw128_desc(sa), dx_lo = make_sw128_desc(sa + kABytes);
       const uint64_t dw_hi = make_sw128_desc(sa + 2 * kABytes), dw_lo = make_sw128_desc(sa + 2 * kABytes + kBBytes);
-      // M side: this warpgroup's 64 rows (8 KB into the 128-row tile); N side: the whole other tile
-      const uint64_t m_off = (uint64_t)((wg * 64 * 128) >> 4);
-      const uint64_t da_hi = (kPool ? dw_hi : dx_hi) + m_off, da_lo = (kPool ? dw_lo : dx_lo) + m_off;
+      // M side: 64 rows per half (8 KB each into the 128-row tile); N side: the whole other tile
+      const uint64_t da_hi = kPool ? dw_hi : dx_hi, da_lo = kPool ? dw_lo : dx_lo;
       const uint64_t db_hi = kPool ? dx_hi : dw_hi, db_lo = kPool ? dx_lo : dw_lo;
       // Every stage issues all four K steps, also the last channel block of a Cin that is not a multiple of 64: the
       // frame maps' channel extent is Cin (the im2col view's too), so TMA fills the channels past it with zeros and the
@@ -323,9 +368,13 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
       for (int s = 0; s < kBlockK / 16; ++s) {
         const uint64_t koff = (uint64_t)(s * 32 >> 4);   // 16 bf16 = 32 bytes along K inside the swizzle row
-        wgmma_bf16<BLOCK_N>(acc, da_lo + koff, db_hi + koff, scale_d);
-        wgmma_bf16<BLOCK_N>(acc, da_hi + koff, db_lo + koff, 1);
-        wgmma_bf16<BLOCK_N>(acc, da_hi + koff, db_hi + koff, 1);
+#pragma unroll
+        for (int hh = 0; hh < kHalves; ++hh) {
+          const uint64_t m_off = (uint64_t)((row_base + 64 * hh) * 128 >> 4);
+          wgmma_bf16<BLOCK_N>(acc[hh], da_lo + m_off + koff, db_hi + koff, scale_d);
+          wgmma_bf16<BLOCK_N>(acc[hh], da_hi + m_off + koff, db_lo + koff, 1);
+          wgmma_bf16<BLOCK_N>(acc[hh], da_hi + m_off + koff, db_hi + koff, 1);
+        }
         scale_d = 1;
       }
       wgmma_commit();
@@ -334,8 +383,11 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       prev_stage = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
+    // the next tile's warpgroup may start its main loop
+    if (kPingPong && tile + gridDim.x < p.num_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(3 - wg) : "memory");
     wgmma_wait<0>();
-    wgmma_fence_operands(acc);
+#pragma unroll
+    for (int hh = 0; hh < kHalves; ++hh) wgmma_fence_operands(acc[hh]);
     if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
     const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;
@@ -348,15 +400,22 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       nv = nv < 0 ? 0 : (nv > p.Tb ? p.Tb : nv);
       const int tblk = m_unit % p.num_t_blk;
       const int gl = p.Tb < 8 ? p.Tb : 8;              // columns of one group inside one 8-column chunk
+#pragma unroll 1
+      for (int hh = 0; hh < kHalves; ++hh) {
+      if (hh > 0) half_down();
+      // opaque per half: hoisted out of the rolled loop, the store addresses and validity masks derived from them
+      // stayed live through both halves and spilled
+      int b0h = b0, nvh = nv;
+      asm volatile("" : "+r"(b0h), "+r"(nvh));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int cch = n0 + row0 + 8 * h;             // this thread's output channel
+        const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
         const bool cvalid = cch < p.Cout;
         const float bias_c = (cvalid && p.bias) ? __ldg(p.bias + cch) : 0.f;
         const float scale_c = (cvalid && bn) ? __ldg(p.scale + cch) : 1.f;
         const float shift_c = (cvalid && bn) ? __ldg(p.shift + cch) : 0.f;
         auto emit = [&](int col, float mean, float m2) {
-          const int bb = b0 + (col >> p.log2_tb);
+          const int bb = b0h + (col >> p.log2_tb);
           if (cvalid && bb < p.B) {
             float* dst = p.pool_partial + ((long long)tblk * p.B + bb) * (2LL * p.Cout) + cch;
             dst[0] = mean;
@@ -367,14 +426,14 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 8; ++i) {
           const int col = 8 * i + 2 * q4;
-          const float x0 = fmaf(fmaxf(acc[4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
-          const float x1 = fmaf(fmaxf(acc[4 * i + 2 * h + 1] + bias_c, relu_floor), scale_c, shift_c);
+          const float x0 = fmaf(fmaxf(acc[0][4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
+          const float x1 = fmaf(fmaxf(acc[0][4 * i + 2 * h + 1] + bias_c, relu_floor), scale_c, shift_c);
           if (p.Tb == 1) {
-            if (nv > 0) { emit(col, x0, 0.f); emit(col + 1, x1, 0.f); }
+            if (nvh > 0) { emit(col, x0, 0.f); emit(col + 1, x1, 0.f); }
             continue;
           }
           const int j = col & (p.Tb - 1);              // frame offset of x0 inside its time block
-          const bool v0 = j < nv, v1 = j + 1 < nv;
+          const bool v0 = j < nvh, v1 = j + 1 < nvh;
           const float pn = (float)v0 + (float)v1;
           const float pm = v1 ? 0.5f * (x0 + x1) : (v0 ? x0 : 0.f);
           const float pm2 = v1 ? 0.5f * (x0 - x1) * (x0 - x1) : 0.f;
@@ -388,6 +447,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             rn = 0.f; rmean = 0.f; rm2 = 0.f;
           }
         }
+      }
       }
       continue;
     }
@@ -410,7 +470,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             const int c = n0 + 8 * i + 2 * q4 + e;
             const bool in = c < p.Cout;
             const uint32_t ok = (valid && in && (!p.hist_sym || c > b)) ? 1u : 0u;
-            const float sc = acc[4 * i + 2 * h + e] + ((in && p.bias) ? __ldg(p.bias + c) : 0.f) + rbias;
+            const float sc = acc[0][4 * i + 2 * h + e] + ((in && p.bias) ? __ldg(p.bias + c) : 0.f) + rbias;
             const float x = (sc - p.hist_lo) * p.hist_inv_w;
             const uint32_t cls = (in && __ldg(p.col_label + c) == lab_r) ? 1u : 0u;
             const uint32_t bl = x < 0.f ? ok : 0u;
@@ -428,59 +488,82 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 
     // ---- layer epilogue: +bias (+ row / utterance terms) -> ReLU -> swish -> BN -> tanh / sigmoid -> fp32 and/or split
     // planes
+    // Column pairs outer, rows inner: a thread's two rows of a half share its columns, so bias, scale and shift are
+    // loaded once per column and half.
     if constexpr (!kPool && !kHist) {
+#pragma unroll 1
+      for (int hh = 0; hh < kHalves; ++hh) {
+      if (hh > 0) half_down();
+      constexpr int kRows = 2;
+      bool live[kRows];                               // row exists and is not masked
+      float rbias[kRows];
+      const float* ub[kRows];
+      long long grow[kRows], frow[kRows];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = row0 + 8 * h;
-      const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
-      if (b >= p.B || t >= p.T) continue;
-      if (p.lengths && t >= __ldg(p.lengths + b)) {   // masked batch, frame past the utterance's end: store zeros
-        epi_zero_row(p, (long long)b * p.T + t, (long long)b * p.out_T + t + slice, n0 + 2 * q4, min(n0 + BLOCK_N, p.Cout));
-        continue;
+      for (int r = 0; r < kRows; ++r) {
+        const int row = row0 + 64 * hh + 8 * r;
+        const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
+        live[r] = b < p.B && t < p.T;
+        grow[r] = (long long)b * p.T + t;
+        frow[r] = (long long)b * p.out_T + t + slice;   // split-K: partial of slice s at "time" s
+        if (live[r] && p.lengths && t >= __ldg(p.lengths + b)) {   // masked batch, frame past the utterance's end: zeros
+          epi_zero_row(p, grow[r], frow[r], n0 + 2 * q4, min(n0 + BLOCK_N, p.Cout));
+          live[r] = false;
+        }
+        rbias[r] = (live[r] && p.row_bias) ? __ldg(p.row_bias + grow[r]) : 0.f;
+        ub[r] = (live[r] && p.utt_bias) ? p.utt_bias + (long long)b * p.ld_utt : nullptr;
       }
-      const float rbias = p.row_bias ? __ldg(p.row_bias + (long long)b * p.T + t) : 0.f;
-      const float* ub = p.utt_bias ? p.utt_bias + (long long)b * p.ld_utt : nullptr;
-      const long long grow = (long long)b * p.T + t;
-      const long long frow = (long long)b * p.out_T + t + slice;   // split-K: partial of slice s at "time" s
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 8; ++i) {
         const int c = n0 + 8 * i + 2 * q4;
         if (c >= p.Cout) break;
         const bool has1 = c + 1 < p.Cout;
-        float x[2] = {acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]};
+        float bias_c[2], scale_c[2], shift_c[2];
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          if (e == 1 && !has1) break;
-          float v = x[e] + (p.bias ? __ldg(p.bias + c + e) : 0.f) + rbias;
-          if (ub) v += __ldg(ub + c + e);
-          v = fmaxf(v, relu_floor);
-          if constexpr (kSwish) v = v / (1.f + expf(-v));
-          if (bn) v = fmaf(v, __ldg(p.scale + c + e), __ldg(p.shift + c + e));
-          if (act_tanh) v = epi_tanh(v);
-          if (act_sigmoid) v = epi_sigmoid(v);
-          x[e] = v;
+          const bool in = e == 0 || has1;
+          bias_c[e] = (in && p.bias) ? __ldg(p.bias + c + e) : 0.f;
+          scale_c[e] = (in && bn) ? __ldg(p.scale + c + e) : 1.f;
+          shift_c[e] = (in && bn) ? __ldg(p.shift + c + e) : 0.f;
         }
-        if (p.y_hi) {
-          __nv_bfloat16 h0, l0, h1, l1;
-          split_bf16(x[0], h0, l0);
-          split_bf16(x[1], h1, l1);
-          __nv_bfloat16* dh = p.y_hi + grow * p.ldy + c;
-          __nv_bfloat16* dl = p.y_lo + grow * p.ldy + c;
-          if (has1) {
-            *reinterpret_cast<uint32_t*>(dh) = pack_bf16x2(h0, h1);
-            *reinterpret_cast<uint32_t*>(dl) = pack_bf16x2(l0, l1);
-          } else {
-            *dh = h0;
-            *dl = l0;
+#pragma unroll
+        for (int r = 0; r < kRows; ++r) {
+          if (!live[r]) continue;
+          float x[2] = {acc[0][4 * i + 2 * r], acc[0][4 * i + 2 * r + 1]};
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            if (e == 1 && !has1) break;
+            float v = x[e] + bias_c[e] + rbias[r];
+            if (ub[r]) v += __ldg(ub[r] + c + e);
+            v = fmaxf(v, relu_floor);
+            if constexpr (kSwish) v = v / (1.f + expf(-v));
+            if (bn) v = fmaf(v, scale_c[e], shift_c[e]);
+            if (act_tanh) v = epi_tanh(v);
+            if (act_sigmoid) v = epi_sigmoid(v);
+            x[e] = v;
+          }
+          if (p.y_hi) {
+            __nv_bfloat16 h0, l0, h1, l1;
+            split_bf16(x[0], h0, l0);
+            split_bf16(x[1], h1, l1);
+            __nv_bfloat16* dh = p.y_hi + grow[r] * p.ldy + c;
+            __nv_bfloat16* dl = p.y_lo + grow[r] * p.ldy + c;
+            if (has1) {
+              *reinterpret_cast<uint32_t*>(dh) = pack_bf16x2(h0, h1);
+              *reinterpret_cast<uint32_t*>(dl) = pack_bf16x2(l0, l1);
+            } else {
+              *dh = h0;
+              *dl = l0;
+            }
+          }
+          if (p.y_f32) {
+            float* df = p.y_f32 + frow[r] * p.ldyf + c;
+            if (has1) *reinterpret_cast<float2*>(df) = make_float2(x[0], x[1]);
+            else *df = x[0];
           }
         }
-        if (p.y_f32) {
-          float* df = p.y_f32 + frow * p.ldyf + c;
-          if (has1) *reinterpret_cast<float2*>(df) = make_float2(x[0], x[1]);
-          else *df = x[0];
-        }
       }
-    }
+      }
     }
   }
   if constexpr (kHist) hist_flush();
@@ -627,7 +710,7 @@ static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t
   XVB_ENSURE_DYN_SMEM((tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>), Cfg::kSmemBytes);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(pl.grid);
-  cfg.blockDim = dim3(kNumThreads);
+  cfg.blockDim = dim3(gemm_threads<BLOCK_N, kHist, kSwish>());
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
