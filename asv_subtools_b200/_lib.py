@@ -4,7 +4,8 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "libxvb200.so")
+# XVB_LIB names another build of the same library (tools/tile_timeline.py loads the timeline build through it)
+LIB_PATH = os.environ.get("XVB_LIB") or os.path.join(_HERE, "libxvb200.so")
 
 RELU, BN, SIGMOID, TANH, SWISH = 1, 2, 4, 8, 16
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH = 0, 1, 2, 3

@@ -131,11 +131,30 @@ __device__ __forceinline__ void tma_load_4d(void* smem, const CUtensorMap* m, ui
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t smem_addr, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
+               "r"(smem_addr), "r"(c0), "r"(c1), "r"(c2)
                : "memory");
+}
+// TMA stores complete in bulk groups of the issuing thread.  wait_read: the stores of all but the newest kPending groups
+// have read their shared memory (it may be written again); wait_done: they have also reached global memory.
+__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void tma_store_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(kPending) : "memory");
+}
+template <int kPending>
+__device__ __forceinline__ void tma_store_wait_done() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kPending) : "memory");
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_f2(uint32_t addr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr));
+  return v;
 }
 // ---------------------------------------------------------------- wgmma
 // A warpgroup (4 consecutive warps, the first one's index a multiple of 4) computes a 64 x N fp32 tile in

@@ -13,8 +13,8 @@
 //     K step issues hi*hi + lo*hi + hi*lo into the same fp32 accumulator;
 //   * warp-specialised persistent CTAs: one producer warp drives TMA through an mbarrier ring of
 //     operand stages, two consumer warpgroups issue wgmma with the accumulators in registers and run
-//     the epilogue (+bias -> ReLU -> BN -> split -> st.global) while the producer already loads the
-//     next tile's operands.  The 128-wide layer and fused-pooling instances run the two warpgroups
+//     the epilogue (+bias -> ReLU -> BN -> split -> shared memory -> TMA store for plane-only layers, st.global
+//     otherwise) while the producer already loads the next tile's operands.  The 128-wide layer and fused-pooling instances run the two warpgroups
 //     ping-pong: each one owns every other tile of the CTA whole (128 accumulator rows), so one
 //     warpgroup's epilogue runs under the other's MMAs.  The other instances split each tile
 //     between the two warpgroups (64 accumulator rows each).
@@ -44,6 +44,15 @@ constexpr int kABytes = kBlockM * kBlockK * 2;   // 16 KB per plane per stage
 constexpr int kNumConsumers = 256;               // two consumer warpgroups
 constexpr int kProducerWarp = kNumConsumers / 32;
 constexpr int kSlabBytes = 16384;                // trial histogram: 2 x hist_bins u32 counters
+// Staged layer epilogue (outputs leave through shared memory and TMA stores): each consumer warpgroup owns one piece of
+// 64 rows x 64 channels x both planes, swizzled like the operand tiles, and the bias, scale and shift of its 64 columns.
+// The two ping-pong warpgroups can be in their epilogues at once, so they share nothing.  The histogram's slab is the
+// first 16 KB of the same region: no instance has both.
+constexpr int kStagePlaneBytes = 64 * kBlockK * 2;
+constexpr int kStageOutBytes = 2 * kStagePlaneBytes;
+constexpr int kCoefBytes = 3 * kBlockK * 4;
+constexpr int kEpiBytes = 2 * (kStageOutBytes + kCoefBytes);
+static_assert(kEpiBytes >= kSlabBytes, "the histogram slab lives in the epilogue region");
 
 // The instances whose two consumer warpgroups run ping-pong (see the kernel).  Each of their consumer threads holds a
 // whole 128 x 128 tile's share of accumulators (128 registers), more than fits in the 168 registers a thread of a
@@ -93,6 +102,14 @@ struct TdnnGemmParams {
   // masked batch of utterances of different lengths: utterance b owns frames [0, lengths[b]); the layer epilogue stores
   // zeros for the frames past it (what the next layer's taps must read, F.pad).  NULL: every utterance is T frames long.
   const int* lengths;
+  // the layer epilogue stages its output tiles in shared memory and stores them with TMA (map_y_hi / map_y_lo): planes
+  // only, no fp32 output, split-K, row or utterance term
+  int tma_store;
+#ifdef XVB_TILE_TIMELINE
+  unsigned long long* timeline;   // per CTA: kTimelineHead words, then kTimelineRec per tile of its list
+  int timeline_tiles;             // tiles per CTA the buffer has room for
+  int timeline_general;           // keep the fused pooling epilogue on its general path
+#endif
   __nv_bfloat16* y_hi;
   __nv_bfloat16* y_lo;
   long long ldy;
@@ -100,14 +117,21 @@ struct TdnnGemmParams {
   long long ldyf;
 };
 
-// One CTA per 128 x BLOCK_N tile; operand stages as deep as 192 KB of shared memory allows.
-template <int BLOCK_N>
+// The instances with the staged layer epilogue: it moves 64-channel boxes, so the 32-wide ones keep the direct stores.
+template <int BLOCK_N, bool kPool, bool kHist>
+__host__ __device__ constexpr bool staged_epilogue() { return !kPool && !kHist && BLOCK_N % kBlockK == 0; }
+
+// One CTA per 128 x BLOCK_N tile; operand stages as deep as 192 KB of shared memory allows.  Behind them the staged
+// instances have the epilogue region; the others keep the 16 KB slab alone, and with it the shared memory they leave
+// to a kernel of another stream.
+template <int BLOCK_N, bool kStagedEpi>
 struct GemmCfg {
+  static constexpr int kTailBytes = kStagedEpi ? kEpiBytes : kSlabBytes;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;          // one plane of the weight tile
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
   static constexpr int kStages = (192 * 1024) / kStageBytes > 6 ? 6 : (192 * 1024) / kStageBytes;
   static constexpr int kAccRegs = BLOCK_N / 2;                   // per consumer thread
-  static constexpr int kSmemBytes = kStages * kStageBytes + kSlabBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kSmemBytes = kStages * kStageBytes + kTailBytes + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared memory of an sm_90 CTA");
   static_assert(kStages >= 2, "need at least a double-buffered operand pipeline");
 };
@@ -178,6 +202,27 @@ __device__ __noinline__ void epi_zero_row(const TdnnGemmParams& p, long long gro
   }
 }
 
+// Per-tile timeline of the consumer warpgroups, for tools/tile_timeline.py.  Compiled in only with -DXVB_TILE_TIMELINE
+// (`make timeline` builds libxvb200_timeline.so next to the library the package loads); the default build contains none
+// of it.  One thread per warpgroup writes clock64 stamps per tile into the buffer given to xvb_tile_timeline_set: main
+// loop start, first operands there, last MMA issued, MMAs retired, epilogue end, and the clocks spent waiting on the full
+// barriers.  The CTA's head holds %globaltimer and clock64 at its start and at each warpgroup's end, which gives the
+// clock's rate.  Plain stores: a printf or any other call would serialise the MMAs (C7510).
+#ifdef XVB_TILE_TIMELINE
+#define XVB_TL(...) __VA_ARGS__
+constexpr int kTimelineHead = 8, kTimelineRec = 8;
+static unsigned long long* g_timeline = nullptr;
+static int g_timeline_tiles = 0;
+static bool g_timeline_direct = false;
+__device__ __forceinline__ unsigned long long global_timer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+#else
+#define XVB_TL(...)
+#endif
+
 // kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
 // one, so that the instantiations without it compile to the same code as before the flag existed.
 //
@@ -194,8 +239,11 @@ __global__ void __launch_bounds__(gemm_threads<BLOCK_N, kHist, kSwish>(), 1)
 tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
                         const __grid_constant__ CUtensorMap map_a2_hi, const __grid_constant__ CUtensorMap map_a2_lo,
                         const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                        const __grid_constant__ CUtensorMap map_y_hi, const __grid_constant__ CUtensorMap map_y_lo,
                         const __grid_constant__ TdnnGemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N>;
+  // the staged epilogue moves 64-channel boxes; the 32-wide instances keep the direct stores
+  constexpr bool kStaged = staged_epilogue<BLOCK_N, kPool, kHist>();
+  using Cfg = GemmCfg<BLOCK_N, kStaged>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBBytes = Cfg::kBBytes;
   constexpr int kStageBytes = Cfg::kStageBytes;
@@ -208,7 +256,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
   // SWIZZLE_128B tiles need 1024-byte alignment
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* slab_base = smem + kStages * kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slab_base + kSlabBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slab_base + Cfg::kTailBytes);
   uint64_t* empty_bar = full_bar + kStages;
 
   const int warp = threadIdx.x >> 5;
@@ -219,6 +267,10 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     tma_prefetch_desc(&map_a_lo);
     tma_prefetch_desc(&map_w_hi);
     tma_prefetch_desc(&map_w_lo);
+    if (kStaged && p.tma_store) {
+      tma_prefetch_desc(&map_y_hi);
+      tma_prefetch_desc(&map_y_lo);
+    }
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);                   // producer arrival + all TMA bytes
       mbar_init(&empty_bar[i], kReleaseWarps);      // one arrival per consumer warp of the stage's warpgroup(s)
@@ -329,7 +381,20 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     asm volatile("bar.sync 1, 256;" ::: "memory");
   }
 
+  XVB_TL(
+    long long tl_start = 0, tl_first = 0, tl_issued = 0, tl_retired = 0, tl_wait = 0;
+    unsigned long long* tl_cta = p.timeline ? p.timeline + (size_t)blockIdx.x * (kTimelineHead + (size_t)kTimelineRec * p.timeline_tiles) : nullptr;
+    if (tl_cta && threadIdx.x == 0) { tl_cta[0] = global_timer(); tl_cta[1] = (unsigned long long)clock64(); }
+  )
   int tj = 0;                                        // index of the tile in the CTA's list
+  XVB_TL(auto tl_flush = [&]() {
+    if (tl_cta && (threadIdx.x & 127) == 0 && tj < p.timeline_tiles) {
+      unsigned long long* r = tl_cta + kTimelineHead + (size_t)kTimelineRec * tj;
+      r[0] = (unsigned long long)tl_start; r[1] = (unsigned long long)tl_first; r[2] = (unsigned long long)tl_issued;
+      r[3] = (unsigned long long)tl_retired; r[4] = (unsigned long long)clock64(); r[5] = (unsigned long long)tl_wait;
+      r[6] = (unsigned long long)wg; r[7] = 1ull;
+    }
+  };)
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tj) {
     int m_unit, n_blk, slice;
     if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;
@@ -348,11 +413,15 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       if (tj > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
     }
     ++it;
+    XVB_TL(tl_start = clock64(); tl_wait = 0;)
     // ---- main loop: one k block (64 channels of one tap and source) per operand stage
-    int prev_stage = -1;
-    uint32_t scale_d = 0;                            // the tile's first MMA overwrites the accumulators
+    // The stage before `stage` in the ring is the one whose MMAs retire next.  It is derived, and so is the tile's
+    // first MMA (which overwrites the accumulators), rather than carried: the ping-pong main loop has no register to spare.
+    auto stage_before = [&]() { return stage == 0 ? kStages - 1 : stage - 1; };
     for (int kb = kb_begin; kb < kb_end; ++kb) {
+      XVB_TL(const long long tl_w0 = clock64();)
       mbar_wait(&full_bar[stage], phase);
+      XVB_TL(const long long tl_w1 = clock64(); tl_wait += tl_w1 - tl_w0; tl_first = kb == kb_begin ? tl_w1 : tl_first;)
       const uint32_t sa = smem_u32(smem + stage * kStageBytes);
       const uint64_t dx_hi = make_sw128_desc(sa), dx_lo = make_sw128_desc(sa + kABytes);
       const uint64_t dw_hi = make_sw128_desc(sa + 2 * kABytes), dw_lo = make_sw128_desc(sa + 2 * kABytes + kBBytes);
@@ -371,24 +440,24 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 #pragma unroll
         for (int hh = 0; hh < kHalves; ++hh) {
           const uint64_t m_off = (uint64_t)((row_base + 64 * hh) * 128 >> 4);
-          wgmma_bf16<BLOCK_N>(acc[hh], da_lo + m_off + koff, db_hi + koff, scale_d);
+          wgmma_bf16<BLOCK_N>(acc[hh], da_lo + m_off + koff, db_hi + koff, s == 0 ? (uint32_t)(kb != kb_begin) : 1u);
           wgmma_bf16<BLOCK_N>(acc[hh], da_hi + m_off + koff, db_lo + koff, 1);
           wgmma_bf16<BLOCK_N>(acc[hh], da_hi + m_off + koff, db_hi + koff, 1);
         }
-        scale_d = 1;
       }
       wgmma_commit();
       wgmma_wait<1>();                               // the previous stage's MMAs have retired: release it
-      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-      prev_stage = stage;
+      if (kb != kb_begin && lane == 0) mbar_arrive(&empty_bar[stage_before()]);
       if (++stage == kStages) { stage = 0; phase ^= 1; }
     }
     // the next tile's warpgroup may start its main loop
     if (kPingPong && tile + gridDim.x < p.num_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(3 - wg) : "memory");
+    XVB_TL(tl_issued = clock64();)
     wgmma_wait<0>();
+    XVB_TL(tl_retired = clock64();)
 #pragma unroll
     for (int hh = 0; hh < kHalves; ++hh) wgmma_fence_operands(acc[hh]);
-    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    if (kb_end > kb_begin && lane == 0) mbar_arrive(&empty_bar[stage_before()]);
 
     const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;
     const int n0 = n_blk * BLOCK_N;
@@ -407,6 +476,49 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       // stayed live through both halves and spilled
       int b0h = b0, nvh = nv;
       asm volatile("" : "+r"(b0h), "+r"(nvh));
+      // Full 8-frame time blocks (Tb == 8 and all 8 frames exist; uniform per tile): block i of the tile is exactly the
+      // 8-column chunk i, and every Chan merge in it has known counts, so the divisions fold.  With chan_merge's names:
+      //   pair into the empty summary: n = 0, nb = tot = 2, wb = 1: d = pm - 0 = pm, mean = fmaf(pm, 1, 0) = pm + 0 (a -0
+      //     becomes +0), m2 = 0 + (pm2 + pm * pm * 0 * 1) = pm2, since pm2 >= 0 and the product is +0 on finite data;
+      //   lanes q4 ^ 1: n = nb = 2, tot = 4, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 2 * 0.5;
+      //   lanes q4 ^ 2: n = nb = 4, tot = 8, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 4 * 0.5.
+      // Every operation that rounds is kept, in chan_merge's order (the two multiplications by powers of two as well:
+      // they are exact except where d * d * n overflows, and there they give what chan_merge gives), so the partials
+      // are bit-identical to the general path's on finite data.  No summary carries from one chunk to the next, so
+      // the 16 chunks of a row are independent chains that the compiler interleaves.
+      if (p.Tb == 8 && nvh == 8 XVB_TL(&& !p.timeline_general)) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
+          const bool cvalid = cch < p.Cout;
+          const float bias_c = (cvalid && p.bias) ? __ldg(p.bias + cch) : 0.f;
+          const float scale_c = (cvalid && bn) ? __ldg(p.scale + cch) : 1.f;
+          const float shift_c = (cvalid && bn) ? __ldg(p.shift + cch) : 0.f;
+          float* dst0 = p.pool_partial + ((long long)tblk * p.B + b0h) * (2LL * p.Cout) + cch;
+          const bool writer = cvalid && q4 == 0;
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 8; ++i) {
+            const float x0 = fmaf(fmaxf(acc[0][4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
+            const float x1 = fmaf(fmaxf(acc[0][4 * i + 2 * h + 1] + bias_c, relu_floor), scale_c, shift_c);
+            float mean = 0.5f * (x0 + x1) + 0.f;
+            float m2 = 0.5f * (x0 - x1) * (x0 - x1);
+            float d = __shfl_xor_sync(0xffffffffu, mean, 1) - mean;
+            float m2b = __shfl_xor_sync(0xffffffffu, m2, 1);
+            mean = fmaf(d, 0.5f, mean);
+            m2 += m2b + d * d * 2.f * 0.5f;
+            d = __shfl_xor_sync(0xffffffffu, mean, 2) - mean;
+            m2b = __shfl_xor_sync(0xffffffffu, m2, 2);
+            mean = fmaf(d, 0.5f, mean);
+            m2 += m2b + d * d * 4.f * 0.5f;
+            if (writer && b0h + i < p.B) {
+              float* dst = dst0 + (long long)i * (2LL * p.Cout);
+              dst[0] = mean;
+              dst[p.Cout] = m2;
+            }
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
@@ -449,6 +561,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         }
       }
       }
+      XVB_TL(tl_flush();)
       continue;
     }
 
@@ -490,6 +603,94 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     // planes
     // Column pairs outer, rows inner: a thread's two rows of a half share its columns, so bias, scale and shift are
     // loaded once per column and half.
+    // Staged path (p.tma_store, one uniform branch per tile): a 64-row half leaves in pieces of 64 channels.  Per piece
+    // the warpgroup puts the 64 columns' bias, scale and shift into shared memory once, every thread applies the same
+    // arithmetic in the same order as the direct path below and writes its packed hi and lo pairs into the warpgroup's
+    // staging buffer, and one thread stores the two planes with TMA.  The buffer has the 128-byte swizzle of the store
+    // maps (16-byte chunk index ^ row & 7): a warp's eight rows fall into eight different chunks, so its stores do not
+    // conflict.  The maps' extents (Cout, T, B) clip the rows past T or B and the channels past Cout, so there are no
+    // tail branches; rows past an utterance's length are staged as zeros.
+    if constexpr (kStaged) {
+      if (p.tma_store) {
+        // Everything below derives from an opaque copy of the thread index, per tile: hoisted out of the tile loop, these
+        // addresses stayed live through the main loop, which has no register to spare, and spilled more.
+        int tid = threadIdx.x;
+        asm volatile("" : "+r"(tid));
+        const int wgo = tid >> 7, wtid = tid & 127, q4o = tid & 3;
+        const int prow = 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2);   // this thread's first row of a 64-row piece
+        const uint32_t stg = smem_u32(slab_base) + wgo * kStageOutBytes;
+        const uint32_t coefs = smem_u32(slab_base) + 2 * kStageOutBytes + wgo * kCoefBytes;
+        const int ebar = 4 + wgo;                         // named barrier of this warpgroup's epilogue
+        const uint32_t coef = coefs + 8 * q4o;            // this thread's column pair of the first 8 columns
+        // this thread's 4 bytes of 16-byte chunk 0 of its first row (the second is 8 rows on, with the same row & 7):
+        // chunk i of the row is at my ^ (i << 4), the swizzle being an XOR on those three address bits
+        const uint32_t my = stg + (uint32_t)prow * 128u + ((uint32_t)(prow & 7) << 4) + 4u * q4o;
+#pragma unroll 1
+        for (int hh = 0; hh < kHalves; ++hh) {
+          if (hh > 0) half_down();
+          const int hrow = (kPingPong ? 0 : 64 * wgo) + 64 * hh;   // the half's first row of the tile: a box of the store maps
+          uint32_t keep[2];                               // 0 for a masked batch's rows past the utterance's end
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const int row = hrow + prow + 8 * r;
+            const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
+            keep[r] = (p.lengths && b < p.B && t >= __ldg(p.lengths + b)) ? 0u : 0xffffffffu;
+          }
+#pragma unroll
+          for (int cr = 0; cr < BLOCK_N / kBlockK; ++cr) {
+            const int c0 = n0 + kBlockK * cr;
+            if (c0 >= p.Cout) break;
+            if (wtid == 0) tma_store_wait_read<0>();      // the previous piece has left the staging buffer
+            if (wtid < kBlockK) {
+              const int c = c0 + wtid;
+              const bool in = c < p.Cout;
+              st_shared_f32(coefs + 4 * wtid, (in && p.bias) ? __ldg(p.bias + c) : 0.f);
+              st_shared_f32(coefs + 4 * (kBlockK + wtid), (in && bn) ? __ldg(p.scale + c) : 1.f);
+              st_shared_f32(coefs + 4 * (2 * kBlockK + wtid), (in && bn) ? __ldg(p.shift + c) : 0.f);
+            }
+            asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
+#pragma unroll
+            for (int i = 0; i < kBlockK / 8; ++i) {
+              const float2 bias_c = ld_shared_f2(coef + 32 * i), scale_c = ld_shared_f2(coef + 32 * i + 4 * kBlockK),
+                           shift_c = ld_shared_f2(coef + 32 * i + 8 * kBlockK);
+              const float bias_e[2] = {bias_c.x, bias_c.y}, scale_e[2] = {scale_c.x, scale_c.y},
+                          shift_e[2] = {shift_c.x, shift_c.y};
+#pragma unroll
+              for (int r = 0; r < 2; ++r) {
+                float x[2] = {acc[0][4 * (8 * cr + i) + 2 * r], acc[0][4 * (8 * cr + i) + 2 * r + 1]};
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  // + 0.f: the direct path adds its (absent) row term here, which turns a -0 sum into +0
+                  float v = x[e] + bias_e[e] + 0.f;
+                  v = fmaxf(v, relu_floor);
+                  if constexpr (kSwish) v = v / (1.f + expf(-v));
+                  if (bn) v = fmaf(v, scale_e[e], shift_e[e]);
+                  if (act_tanh) v = epi_tanh(v);
+                  if (act_sigmoid) v = epi_sigmoid(v);
+                  x[e] = v;
+                }
+                __nv_bfloat16 h0, l0, h1, l1;
+                split_bf16(x[0], h0, l0);
+                split_bf16(x[1], h1, l1);
+                const uint32_t at = (my ^ ((uint32_t)i << 4)) + 1024u * r;
+                st_shared_u32(at, pack_bf16x2(h0, h1) & keep[r]);
+                st_shared_u32(at + kStagePlaneBytes, pack_bf16x2(l0, l1) & keep[r]);
+              }
+            }
+            fence_proxy_async();                          // the staged piece becomes visible to the TMA unit
+            asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
+            if (wtid == 0) {
+              const int hb = b0 + (hrow >> p.log2_tb), ht = t0 + (hrow & (p.Tb - 1));
+              tma_store_3d(&map_y_hi, stg, c0, ht, hb);
+              tma_store_3d(&map_y_lo, stg + kStagePlaneBytes, c0, ht, hb);
+              tma_store_commit();
+            }
+          }
+        }
+        XVB_TL(tl_flush();)
+        continue;
+      }
+    }
     if constexpr (!kPool && !kHist) {
 #pragma unroll 1
       for (int hh = 0; hh < kHalves; ++hh) {
@@ -564,9 +765,14 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         }
       }
       }
+      XVB_TL(tl_flush();)
     }
   }
   if constexpr (kHist) hist_flush();
+  if constexpr (kStaged) {
+    if (p.tma_store && (threadIdx.x & 127) == 0) tma_store_wait_done<0>();   // this thread's stores have landed
+  }
+  XVB_TL(if (tl_cta && (threadIdx.x & 127) == 0) { tl_cta[2 + 2 * wg] = global_timer(); tl_cta[3 + 2 * wg] = (unsigned long long)clock64(); })
 }
 
 // Split-K tail: y[b,c] = epi(sum_s part[b,s,c]) with the slices added in index order (deterministic),
@@ -651,6 +857,16 @@ static int make_frame_map(CUtensorMap* m, const void* base, int C, int T, int B,
   return XVB_OK;
 }
 
+// Store map of the staged layer epilogue: the (Cout, T, B) bf16 output plane with row pitch ld; box = 64 channels x the 64
+// rows of one accumulator half (Tb frames x 64 / Tb utterances, or 64 frames of one utterance).  The extents clip the box.
+static int make_store_map(CUtensorMap* m, const void* base, int Cout, int T, int B, long long ld, int Tb) {
+  const int box_t = Tb < 64 ? Tb : 64;
+  const unsigned long long dims[3] = {(unsigned long long)Cout, (unsigned long long)T, (unsigned long long)B};
+  const unsigned long long strides[2] = {(unsigned long long)ld * 2, (unsigned long long)ld * 2 * (unsigned long long)T};
+  const unsigned box[3] = {(unsigned)kBlockK, (unsigned)box_t, (unsigned)(64 / box_t)};
+  return make_tensor_map(m, base, 2, 3, dims, strides, box, 128);
+}
+
 // (K, Cout) bf16 packed weight, K contiguous; box = 64 x block_n.
 static int make_weight_map(CUtensorMap* m, const void* base, long long K, int Cout, int block_n) {
   PFN_encodeTiled enc = get_encode();
@@ -691,7 +907,7 @@ static void choose_m_tile(int B, int T, int* Tb_out, int* Bb_out, int max_tb = 1
 // extractor objects keep their plans per (B, T), so a batch costs launches only.
 // ------------------------------------------------------------------------------------------------
 struct GemmPlan {
-  CUtensorMap ma_hi, ma_lo, ma2_hi, ma2_lo, mw_hi, mw_lo;
+  CUtensorMap ma_hi, ma_lo, ma2_hi, ma2_lo, mw_hi, mw_lo, my_hi, my_lo;
   TdnnGemmParams p;
   int (*launch)(const GemmPlan&, const TdnnGemmParams&, cudaStream_t) = nullptr;   // nullptr: this shard owns no rows
   int grid = 0;
@@ -706,7 +922,7 @@ struct GemmPlan {
 
 template <int BLOCK_N, bool kPool, bool kHist, bool kSwish>
 static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N>;
+  using Cfg = GemmCfg<BLOCK_N, staged_epilogue<BLOCK_N, kPool, kHist>()>;
   XVB_ENSURE_DYN_SMEM((tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>), Cfg::kSmemBytes);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(pl.grid);
@@ -719,7 +935,7 @@ static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t
   cfg.attrs = attr;
   cfg.numAttrs = pl.pdl ? 1 : 0;
   XVB_CUDA(cudaLaunchKernelEx(&cfg, tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>, pl.ma_hi, pl.ma_lo, pl.ma2_hi,
-                              pl.ma2_lo, pl.mw_hi, pl.mw_lo, p));
+                              pl.ma2_lo, pl.mw_hi, pl.mw_lo, pl.my_hi, pl.my_lo, p));
   XVB_LAUNCH_CHECK();
   return XVB_OK;
 }
@@ -733,6 +949,16 @@ static int prepare_gemm(GemmPlan& pl, const void* w_hi, const void* w_lo) {
   rc = make_weight_map(&pl.mw_lo, w_lo, K, p.Cout, BLOCK_N);
   if (rc) return rc;
   p.num_n_blk = (p.Cout + BLOCK_N - 1) / BLOCK_N;
+  // Plane-only layers (every frame layer of the extractors) take the staged epilogue.  The direct stores stay for fp32
+  // outputs, split-K partials, row and utterance terms, and for the 32-wide instances.
+  p.tma_store = staged_epilogue<BLOCK_N, kPool, kHist>() && p.y_hi && !p.y_f32 && p.k_slices == 1 && !p.row_bias && !p.utt_bias;
+  XVB_TL(if (g_timeline_direct) p.tma_store = 0;)
+  if (p.tma_store) {
+    if ((rc = make_store_map(&pl.my_hi, p.y_hi, p.Cout, p.T, p.B, p.ldy, p.Tb))) return rc;
+    if ((rc = make_store_map(&pl.my_lo, p.y_lo, p.Cout, p.T, p.B, p.ldy, p.Tb))) return rc;
+  } else {
+    pl.my_hi = pl.mw_hi; pl.my_lo = pl.mw_lo;  // unused
+  }
   const int all_m_units = kHist ? (p.num_t_blk * p.num_b_blk + 1) / 2 : p.num_t_blk * p.num_b_blk;  // see unit_first
   if (p.unit_first >= all_m_units) { pl.launch = nullptr; return XVB_OK; }  // this shard owns no rows
   const int num_m_units = (all_m_units - p.unit_first + p.unit_stride - 1) / p.unit_stride;
@@ -849,6 +1075,7 @@ int xvb::gemm_plan_build(GemmPlan** out, const xvb_tdnn_args_t& a, const TrialHi
   p.y_lo = reinterpret_cast<__nv_bfloat16*>(a.y_lo);
   p.ldy = a.ldy; p.y_f32 = a.y_f32; p.ldyf = a.ldyf;
 
+  XVB_TL(p.timeline = g_timeline; p.timeline_tiles = g_timeline_tiles; p.timeline_general = g_timeline_direct;)
   p.k_slices = splitk_slices(a, th != nullptr, &p.kb_per_slice);
   if (p.k_slices > 1) {
     XVB_CHECK_ARG(scratch, "xvb_tdnn_affine: split-K plan needs %zu bytes of scratch", gemm_plan_scratch_bytes(a, th));
@@ -951,6 +1178,17 @@ int xvb::tdnn_affine_impl(const xvb_tdnn_args_t& a, void* stream, const TrialHis
   gemm_plan_destroy(pl);
   return rc;
 }
+
+#ifdef XVB_TILE_TIMELINE
+// Timeline build only: plans built from now on stamp into `buf` (device memory, gridDim x (8 + 8 x tiles_per_cta) u64,
+// zeroed by the caller; NULL switches it off).  direct_stores != 0 keeps such plans on the direct-store layer epilogue
+// and on the general path of the fused pooling epilogue, so that the old and new epilogues can be set side by side.
+extern "C" void xvb_tile_timeline_set(unsigned long long* buf, int tiles_per_cta, int direct_stores) {
+  g_timeline = buf;
+  g_timeline_tiles = tiles_per_cta;
+  g_timeline_direct = direct_stores != 0;
+}
+#endif
 
 extern "C" int xvb_tdnn_grouped_fits(int Cin, int Cout, int groups) {
   return groups > 1 && Cin > 0 && Cout > 0 && Cin % groups == 0 && Cout % groups == 0 && (Cin / groups) % kBlockK == 0 &&
