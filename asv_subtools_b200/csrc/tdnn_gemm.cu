@@ -950,8 +950,11 @@ static int prepare_gemm(GemmPlan& pl, const void* w_hi, const void* w_lo) {
   if (rc) return rc;
   p.num_n_blk = (p.Cout + BLOCK_N - 1) / BLOCK_N;
   // Plane-only layers (every frame layer of the extractors) take the staged epilogue.  The direct stores stay for fp32
-  // outputs, split-K partials, row and utterance terms, and for the 32-wide instances.
-  p.tma_store = staged_epilogue<BLOCK_N, kPool, kHist>() && p.y_hi && !p.y_f32 && p.k_slices == 1 && !p.row_bias && !p.utt_bias;
+  // outputs, split-K partials, row and utterance terms, and for the 32-wide instances.  They also stay when Cout % 8 != 0:
+  // the store maps' Cout extent does not clip inside a 16-byte chunk, so the last chunk of every row would be written
+  // whole, up to 7 channels past Cout (in a channel slice of a wider buffer, another tensor's channels).
+  p.tma_store = staged_epilogue<BLOCK_N, kPool, kHist>() && p.y_hi && !p.y_f32 && p.k_slices == 1 && !p.row_bias && !p.utt_bias &&
+                p.Cout % 8 == 0;
   XVB_TL(if (g_timeline_direct) p.tma_store = 0;)
   if (p.tma_store) {
     if ((rc = make_store_map(&pl.my_hi, p.y_hi, p.Cout, p.T, p.B, p.ldy, p.Tb))) return rc;

@@ -215,10 +215,11 @@ def layer_acc(d, context):
     return acc.reshape(B, T, -1)
 
 
-def layer_reference(case, d):
+def layer_reference(case, d, acc=None):
     """-> (want, bound): the float64 output of the layer epilogue (+bias, row / utterance terms -> ReLU -> swish -> BN ->
-    tanh / sigmoid), and None when it is exact (float32 array then) or the per-element bound of a transcendental one."""
-    v = layer_acc(d, case["ctx"]) + d["bias"][None, None, :].astype(np.float64)
+    tanh / sigmoid), and None when it is exact (float32 array then) or the per-element bound of a transcendental one.
+    acc: the (B, T, Cout) float64 contraction when it is not layer_acc's (grouped layers)."""
+    v = (layer_acc(d, case["ctx"]) if acc is None else acc) + d["bias"][None, None, :].astype(np.float64)
     B, T = case["B"], case["T"]
     if "row" in d:
         v = v + d["row"].reshape(B, T)[:, :, None]
