@@ -94,7 +94,8 @@ __global__ void se_apply_kernel(const __nv_bfloat16* __restrict__ zh, const __nv
     const float4 g1 = *reinterpret_cast<const float4*>(gate + row * C + c + 4);
     const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
-    for (int k = 0; k < 8; ++k) o[k] = z[k] * g[k] + x[k];   // mul then add: the reference's two roundings
+    // mul then add: the reference's two roundings (spelled out: the compiler would otherwise contract them into one FFMA)
+    for (int k = 0; k < 8; ++k) o[k] = __fadd_rn(__fmul_rn(z[k], g[k]), x[k]);
     uint4 h, l;
     pack8(o, h, l);
     *reinterpret_cast<uint4*>(oh + fr * ldo + c) = h;
