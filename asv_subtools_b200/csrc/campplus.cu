@@ -152,7 +152,8 @@ extern "C" int xvb_cam_gate(const uint16_t* h_hi, const uint16_t* h_lo, int64_t 
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(h_hi && h_lo && w1 && b1 && w2 && b2 && gate, "xvb_cam_gate: null pointer");
-  XVB_CHECK_ARG(B > 0 && T > 0 && seg_len > 0 && R > 0 && G > 0 && C % 8 == 0 && C / 8 <= kGateThreads && ldh % 8 == 0 && ldh >= C,
+  XVB_CHECK_ARG(B > 0 && T > 0 && seg_len > 0 && R > 0 && G > 0 && C > 0 && C % 8 == 0 && C / 8 <= kGateThreads && ldh % 8 == 0 &&
+                    ldh >= C,
                 "xvb_cam_gate: need C %% 8 == 0, 8 <= C <= %d, ldh %% 8 == 0 (C=%d ldh=%lld)", 8 * kGateThreads, C,
                 (long long)ldh);
   XVB_CHECK_ARG(((uintptr_t)h_hi | (uintptr_t)h_lo) % 16 == 0, "xvb_cam_gate: planes must be 16-byte aligned");

@@ -344,6 +344,13 @@ def _rows(t, name):
     if t.dtype != torch.float32 or not t.is_cuda or t.stride(-1) != 1:
         raise TypeError("{} must be a CUDA float32 tensor with contiguous rows".format(name))
     ld = t.stride(-2) if t.dim() >= 2 else t.shape[-1]
+    # the kernels address row r at r * ld: a view such as buf[:, :T] of a longer buffer does not collapse that way
+    want = ld
+    for i in range(t.dim() - 2, -1, -1):
+        if t.shape[i] > 1 and t.stride(i) != want:
+            raise ValueError("{}: leading dimensions {} do not collapse into rows of pitch {} (strides {})".format(
+                name, tuple(t.shape[:-1]), ld, t.stride()))
+        want *= t.shape[i]
     return t.numel() // t.shape[-1], ld
 
 
@@ -361,7 +368,9 @@ def layer_norm(x, gamma=None, beta=None, eps=1e-5, delta=None, delta_scale=1.0, 
         a.delta, a.ld_delta = delta.data_ptr(), _rows(delta, "delta")[1]
         a.delta_scale = delta_scale
     if table is not None:
-        a.table, a.table_rows = _req(table, torch.float32, "table").data_ptr(), table.shape[0]
+        if _req(table, torch.float32, "table").dim() != 2 or table.shape[1] != c:
+            raise ValueError("table must be (rows, {}), got {}".format(c, tuple(table.shape)))
+        a.table, a.table_rows = table.data_ptr(), table.shape[0]
     if x_out is not None:
         a.x_out, a.ld_x_out = x_out.data_ptr(), _rows(x_out, "x_out")[1]
     if gamma is not None:
@@ -383,6 +392,8 @@ def rope_attention(qkv, heads, dk, y, rope=None, rope_v=False, score_mult=1.0):
     fp32 [sin | cos] or None -> y SplitPlanes (B, T, heads * dk)."""
     _, ldq = _rows(qkv, "qkv")
     b, t = qkv.shape[0], qkv.shape[1]
+    if rope is not None and (_req(rope, torch.float32, "rope").dim() != 2 or rope.shape[0] < t or rope.shape[1] != dk):
+        raise ValueError("rope must be (>= {}, {}), got {}".format(t, dk, tuple(rope.shape)))
     check(lib.xvb_rope_attention(qkv.data_ptr(), ldq, b, t, heads, dk,
                                  _ptr(_req(rope, torch.float32, "rope")) if rope is not None else None, 1 if rope_v else 0,
                                  float(score_mult), y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_rope_attention")

@@ -356,11 +356,20 @@ def conv_cases(sms):
                                          y=True, yf=True),
         "k1s1_cin128_cout16_odd": D(B=2, T=7, F=5, Cin=128, Cout=16, k=1, s=1, yf=True, y2=True),
         "k3s1_cin32_cout64_res": D(B=2, T=10, F=9, Cin=32, Cout=64, k=3, s=1, scale=True, res=True, relu=True, y=True),
+        # CAM++'s FCM front end: feature stride 2, time stride 1 (st), over T > 256 (several time blocks), odd and even F
+        "fcm_k3_s2t1_F11_T300": D(B=2, T=300, F=11, Cin=32, Cout=32, k=3, s=2, st=1, scale=True, relu=True, y=True, yf=True),
+        "fcm_k3_s2t1_F10_T257": D(B=2, T=257, F=10, Cin=32, Cout=32, k=3, s=2, st=1, scale=True, res=True, relu=True,
+                                  y=True),
+        "fcm_k1_s2t1_F11_T300": D(B=2, T=300, F=11, Cin=32, Cout=32, k=1, s=2, st=1, scale=True, y=True, yf=True),
+        "fcm_k1_s2t1_F10_T270": D(B=3, T=270, F=10, Cin=32, Cout=32, k=1, s=2, st=1, scale=True, y=True),
+        # the other mixed stride the API takes: feature stride 1, time stride 2
+        "k3_s1t2_F9_T41": D(B=2, T=41, F=9, Cin=32, Cout=48, k=3, s=1, st=2, scale=True, relu=True, y=True, yf=True),
     }
     for c in cases.values():
         c.setdefault("taps", None)
+        c.setdefault("st", c["s"])
         pad = 0 if c.get("valid") else c["k"] // 2
-        c["To"] = (c["T"] + 2 * pad - c["k"]) // c["s"] + 1
+        c["To"] = (c["T"] + 2 * pad - c["k"]) // c["st"] + 1
         c["Fo"] = (c["F"] + 2 * pad - c["k"]) // c["s"] + 1
     return cases
 
@@ -387,7 +396,7 @@ def make_conv(case, seed):
 
 def conv_reference(case, d):
     """-> (y, y2): float32 outputs of the conv epilogue (BN -> + residual -> ReLU; y2 = relu(y * scale2 + shift2))."""
-    k, s = case["k"], case["s"]
+    k, s, st = case["k"], case["s"], case.get("st", case["s"])      # st: the time stride
     pad = 0 if case.get("valid") else k // 2
     taps = case["taps"] if case["taps"] is not None else list(range(k * k))
     hx, lx = d["x"]
@@ -401,8 +410,8 @@ def conv_reference(case, d):
     acc = np.zeros((B * To * Fo, wh.shape[0]))
     for j in taps:
         kf, kt = divmod(j, k)   # tap = kf * k + kt; "H" is the feature axis, "W" is time
-        sh = ph[:, kt:kt + s * (To - 1) + 1:s, kf:kf + s * (Fo - 1) + 1:s].reshape(-1, Cin)
-        sl = pl[:, kt:kt + s * (To - 1) + 1:s, kf:kf + s * (Fo - 1) + 1:s].reshape(-1, Cin)
+        sh = ph[:, kt:kt + st * (To - 1) + 1:st, kf:kf + s * (Fo - 1) + 1:s].reshape(-1, Cin)
+        sl = pl[:, kt:kt + st * (To - 1) + 1:st, kf:kf + s * (Fo - 1) + 1:s].reshape(-1, Cin)
         acc += (sh + sl) @ wh[:, :, j].T.astype(np.float64) + sh @ wl[:, :, j].T.astype(np.float64)
     v = acc.reshape(B, To, Fo, -1)
     if "scale" in d:

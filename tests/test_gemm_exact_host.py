@@ -118,6 +118,10 @@ def test_conv_cases_are_exact():
         assert {16, 32, 48, 64, 80, 96, 112, 128, 144} <= {c["Cin"] for c in cases.values()}
         assert {16, 48, 80, 144, 272} <= {c["Cout"] for c in cases.values()}
         assert {c.get("inst") for c in cases.values()} >= {32, 64, 128}
+        # CAM++'s (2, 1) stride with k = 1 and 3, odd and even F, T > 256; and one (1, 2)
+        fcm = [c for c in cases.values() if (c["s"], c["st"]) == (2, 1) and c["Cin"] == c["Cout"] == 32 and c["T"] > 256]
+        assert {c["k"] for c in fcm} == {1, 3} and {c["F"] % 2 for c in fcm} == {0, 1}
+        assert any((c["s"], c["st"]) == (1, 2) for c in cases.values())
         for name, case in cases.items():
             y, y2 = gx.conv_reference(case, gx.make_conv(case, 5))
             assert y.shape == (case["B"], case["To"], case["Fo"], case["Cout"]), name
@@ -127,7 +131,8 @@ def test_conv_cases_are_exact():
 def test_conv_reference_matches_torch():
     """The im2col reference against F.conv2d (float64) on one strided, one tap-list and one valid case."""
     cases = gx.conv_cases(132)
-    for name in ("w32_k3s2_cin80_cout48_res_y2", "taps_k5s2_cin96_cout16", "valid_k3s2_cin96_cout16_odd"):
+    for name in ("w32_k3s2_cin80_cout48_res_y2", "taps_k5s2_cin96_cout16", "valid_k3s2_cin96_cout16_odd",
+                 "fcm_k3_s2t1_F11_T300", "fcm_k1_s2t1_F10_T270", "k3_s1t2_F9_T41"):
         case = dict(cases[name], relu=False)
         d = gx.make_conv(case, 3)
         for k in ("scale", "res", "scale2"):
@@ -137,7 +142,8 @@ def test_conv_reference_matches_torch():
         wh, wl = torch.from_numpy(d["w_int"]).double(), torch.from_numpy(d["w_frac"]).double()
         pad = 0 if case.get("valid") else case["k"] // 2
         conv = torch.nn.functional.conv2d
-        ref = conv(hx + lx, wh, stride=case["s"], padding=pad) + conv(hx, wl, stride=case["s"], padding=pad)
+        stride = (case["s"], case["st"])                                               # (F, T)
+        ref = conv(hx + lx, wh, stride=stride, padding=pad) + conv(hx, wl, stride=stride, padding=pad)
         assert np.array_equal(y, ref.permute(0, 3, 2, 1).numpy()), name
 
 

@@ -311,7 +311,7 @@ def _conv_case(ops, sms, name):
         ops.conv2d(x, w, Cout, k, stride=case["s"], scale=_dev(d["scale"]) if "scale" in d else None,
                    shift=_dev(d["shift"]) if "shift" in d else None, res=res, relu=bool(case.get("relu")), y=y, y_f32=yf,
                    scale2=_dev(d["scale2"]) if "scale2" in d else None, shift2=_dev(d["shift2"]) if "shift2" in d else None,
-                   y2=y2, taps=taps, valid=bool(case.get("valid")))
+                   y2=y2, taps=taps, valid=bool(case.get("valid")), stride_t=case["st"] if case["st"] != case["s"] else 0)
 
     seen = _profiled(run)
     if y is not None:
