@@ -74,9 +74,7 @@ struct Model {
   // widths derived from the pooling: att_x outputs AX, the logits NL (row pitch ldlog), the pooled statistics P of the
   // P2-wide [mean | std] buffer (default model: AX = H, NL = D, P = P2 = 2D)
   int AX = 0, NL = 0, ldlog = 0, P = 0, P2 = 0;
-  // layer1 as an im2col view over time-padded planes (see extractor.cu): consecutive taps, feat_dim % 16 == 0
-  bool im2col_first = false;
-  int pad_front = 0, pad_back = 0;
+  Im2col im2col;   // layer1 as an im2col view (records.cuh)
   Weights dev{"xvb_ecapa_set_layer"};
 };
 
@@ -87,42 +85,20 @@ using namespace xvb;
 struct xvb_ecapa {
   std::shared_ptr<const Model> m;
   Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
-  // workspace
-  long long cap_frames = 0;
-  int cap_B = 0;
-  std::vector<void*> ws;
+  // workspace, each buffer grown to the largest call seen: the plane buffers up to kPp, then the fp32 ones
+  enum { kIn, kX, kH, kR, kZ, kN, kCat, kM, kA1, kGp, kS1, kZm, kPp, kMF, kLog, kGate, kUb, kZmean, kGstat, kPstat, kS1f,
+         kF1, kBufs };
+  Workspace<kBufs> ws;
+  // the workspace's buffers as reserve last left them: planes with their row pitch, and fp32
   View in, X, Hh, R, Z, N, CAT, M, A1, gp, s1, zm, pp;
   float *MF = nullptr, *LOG = nullptr, *gate = nullptr, *ub = nullptr, *zmean = nullptr, *gstat = nullptr, *pstat = nullptr;
   float* s1f = nullptr;   // (B, se_dim) fp32: hidden vector of the SE gate
   float* f1 = nullptr;    // (B, fc1_dim) fp32: output of fc1 when the model has one
   int last_launches = 0;
-  bool im2col_first = false;   // this lane's copy of the model's decision, cleared if the driver refuses the view
-  int pad_front = 0, pad_back = 0;
+  Im2col im2col;   // this lane's copy of the model's choice
   Shard<xvb_ecapa> shard;
 
-  explicit xvb_ecapa(std::shared_ptr<const Model> model) : m(std::move(model)) {
-    im2col_first = m->im2col_first; pad_front = m->pad_front; pad_back = m->pad_back;
-  }
-  ~xvb_ecapa() { free_ws(); }
-
-  void free_ws() {
-    for (void* p : ws) cudaFree(p);
-    ws.clear();
-    cap_frames = 0; cap_B = 0;
-  }
-  template <typename T>
-  int alloc(T** p, size_t n) {
-    XVB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-    ws.push_back(*p);
-    return XVB_OK;
-  }
-  int planes(View* p, size_t rows, int64_t ld) {
-    int rc = alloc(&p->hi, rows * ld);
-    if (!rc) rc = alloc(&p->lo, rows * ld);
-    p->ld = ld;
-    return rc;
-  }
-  int f32(float** p, size_t n) { return alloc(p, n); }
+  explicit xvb_ecapa(std::shared_ptr<const Model> model) : m(std::move(model)), im2col(m->im2col) {}
 };
 
 template <>
@@ -297,16 +273,8 @@ extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
     rc = need("fc2", m->P, m->E, 1);
     if (rc) return rc;
   }
-  {
-    const ELayer* L0 = find(m, "layer1");
-    bool consecutive = L0->ntaps > 1 && L0->ctx[0] <= 0 && L0->ctx[L0->ntaps - 1] >= 0;
-    for (int i = 1; i < L0->ntaps; ++i) consecutive = consecutive && L0->ctx[i] == L0->ctx[i - 1] + 1;
-    const int knob = getenv("XVB_IM2COL") ? atoi(getenv("XVB_IM2COL")) : 1;
-    m->im2col_first = knob && consecutive && m->feat_dim % 16 == 0;
-    m->pad_front = m->im2col_first ? -L0->ctx[0] : 0;
-    m->pad_back = m->im2col_first ? L0->ctx[L0->ntaps - 1] : 0;
-  }
-  h->im2col_first = m->im2col_first; h->pad_front = m->pad_front; h->pad_back = m->pad_back;
+  const ELayer* L0 = find(m, "layer1");
+  m->im2col = h->im2col = im2col_choice(L0->ctx, L0->ntaps, m->feat_dim);
   h->draft = nullptr;
   return XVB_OK;
 }
@@ -316,25 +284,26 @@ extern "C" int xvb_ecapa_feat_dim(const xvb_ecapa_t* h) { return h ? h->m->feat_
 extern "C" int xvb_ecapa_last_launches(const xvb_ecapa_t* h) { return h ? h->last_launches : 0; }
 
 static int reserve(xvb_ecapa* h, int B, int T) {
-  const long long frames = (long long)B * T;
-  if (frames <= h->cap_frames && B <= h->cap_B) return XVB_OK;
-  const size_t nf = (size_t)(frames > h->cap_frames ? frames : h->cap_frames);
-  const size_t nb = (size_t)(B > h->cap_B ? B : h->cap_B);
-  h->free_ws();
+  using H = xvb_ecapa;
   const Model* m = h->m.get();
-  const int C = m->C, D = m->D;
-  int rc;
-  if ((rc = h->planes(&h->in, nf + nb * (size_t)(h->pad_front + h->pad_back), m->ldf)) || (rc = h->planes(&h->X, nf, C)) || (rc = h->planes(&h->Hh, nf, C)) ||
-      (rc = h->planes(&h->R, nf, C)) || (rc = h->planes(&h->Z, nf, C)) || (rc = h->planes(&h->N, nf, C)) ||
-      (rc = h->planes(&h->CAT, nf, 3 * C)) || (rc = h->planes(&h->M, nf, D)) || (rc = h->planes(&h->A1, nf, m->H)) ||
-      (rc = h->planes(&h->gp, nb, 2 * D)) || (rc = h->planes(&h->s1, nb, m->se_dim)) || (rc = h->planes(&h->zm, nb, C)) ||
-      (rc = h->planes(&h->pp, nb, m->P2)) || (rc = h->f32(&h->MF, nf * D)) || (rc = h->f32(&h->LOG, nf * m->ldlog)) ||
-      (rc = h->f32(&h->gate, nb * C)) || (rc = h->f32(&h->ub, nb * m->AX)) || (rc = h->f32(&h->zmean, nb * C)) ||
-      (rc = h->f32(&h->gstat, nb * 2 * D)) || (rc = h->f32(&h->pstat, nb * m->P2)) || (rc = h->f32(&h->s1f, nb * (size_t)m->se_dim)) ||
-      (m->fc1_dim && (rc = h->f32(&h->f1, nb * (size_t)m->fc1_dim))))
-    return rc;
-  h->cap_frames = (long long)nf;
-  h->cap_B = (int)nb;
+  const size_t b = (size_t)B, f = (size_t)B * T, C = (size_t)m->C, D = (size_t)m->D;
+  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->ldf, f * C, f * C, f * C, f * C,
+                                 f * C, f * 3 * C, f * D, f * m->H, b * 2 * D, b * m->se_dim, b * C, b * m->P2,
+                                 f * D, f * m->ldlog, b * C, b * m->AX, b * C, b * 2 * D, b * m->P2, b * m->se_dim,
+                                 b * m->fc1_dim};
+  bool planes[H::kBufs];
+  for (int i = 0; i < H::kBufs; ++i) planes[i] = i <= H::kPp;
+  uint64_t grown;
+  const int rc = h->ws.reserve(need, planes, &grown);
+  if (rc) return rc;
+  auto view = [&](int i, int64_t ld) { const Planes p = h->ws.planes(i); return View{p.hi, p.lo, ld}; };
+  h->in = view(H::kIn, m->ldf); h->X = view(H::kX, C); h->Hh = view(H::kH, C); h->R = view(H::kR, C);
+  h->Z = view(H::kZ, C); h->N = view(H::kN, C); h->CAT = view(H::kCat, 3 * C); h->M = view(H::kM, D);
+  h->A1 = view(H::kA1, m->H); h->gp = view(H::kGp, 2 * D); h->s1 = view(H::kS1, m->se_dim); h->zm = view(H::kZm, C);
+  h->pp = view(H::kPp, m->P2);
+  h->MF = h->ws.f32(H::kMF); h->LOG = h->ws.f32(H::kLog); h->gate = h->ws.f32(H::kGate); h->ub = h->ws.f32(H::kUb);
+  h->zmean = h->ws.f32(H::kZmean); h->gstat = h->ws.f32(H::kGstat); h->pstat = h->ws.f32(H::kPstat);
+  h->s1f = h->ws.f32(H::kS1f); h->f1 = h->ws.f32(H::kF1);
   return XVB_OK;
 }
 
@@ -420,19 +389,19 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   const long before = g_launches;
   const int C = m->C, D = m->D;
   auto L = [&](const std::string& n) { return find(m, n); };
-  if (h->im2col_first)
-    rc = xvb_split_frames(feats, B, T, m->feat_dim, h->in.hi, h->in.lo, m->ldf, h->pad_front, h->pad_back, stream);
+  const Im2col& im = h->im2col;
+  if (im.on)
+    rc = xvb_split_frames(feats, B, T, m->feat_dim, h->in.hi, h->in.lo, m->ldf, im.pad_front, im.pad_back, stream);
   else
     rc = xvb_split_f32(feats, (int64_t)B * T, m->feat_dim, m->feat_dim, h->in.hi, h->in.lo, m->ldf, stream);
   if (rc) return rc;
   Run r{};
   r.B = B; r.T = T;
   r.L = L("layer1"); r.x = h->in; r.y = h->X;
-  if (h->im2col_first) { r.im2col_taps = r.L->ntaps; r.x_batch_stride = (int64_t)(T + h->pad_front + h->pad_back) * m->ldf; }
+  if (im.on) { r.im2col_taps = r.L->ntaps; r.x_batch_stride = (int64_t)(T + im.pad_front + im.pad_back) * m->ldf; }
   rc = launch(r, stream);
-  if (rc && h->im2col_first) {   // overlapping tensor map refused by the driver: plain path from now on
-    h->im2col_first = false;
-    h->pad_front = h->pad_back = 0;
+  if (rc && im.on) {   // overlapping tensor map refused by the driver: plain path from now on
+    h->im2col = Im2col{};
     return xvb_ecapa_extract(h, feats, B, T, emb, stream);
   }
   if (rc) return rc;

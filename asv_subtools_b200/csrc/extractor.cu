@@ -4,7 +4,6 @@
 // equal-length utterances and for the "load weights, run extraction without Python" role of the
 // reference's C++ runtime (runtime/bin/extractor_main.cc, runtime/speaker/torch_asv_model.cc).
 #include <cuda_runtime.h>
-#include <stdlib.h>
 
 #include <map>
 #include <memory>
@@ -34,18 +33,9 @@ struct Model {
   float pooling_eps = 1e-10f;
   std::vector<Layer> frame, segment;
   int max_c = 0, max_seg_c = 0;
-  // first layer as an im2col view (consecutive context taps over a time-padded frame matrix): 7 channel blocks instead
-  // of 10 for [-2..2] x 80.  Each lane turns it off for good if the driver rejects the overlapping tensor map.
-  bool im2col_first = false;
-  int pad_front = 0, pad_back = 0;
+  Im2col im2col;   // the first layer as an im2col view (records.cuh)
   Weights dev{"xvb_extractor_add_layer"};
 };
-
-template <typename T>
-static int dev_alloc(T** p, size_t n) {
-  XVB_CUDA(cudaMalloc((void**)p, n * sizeof(T)));
-  return XVB_OK;
-}
 
 // Everything one (B, T) batch shape needs besides launches: a GemmPlan per layer (tensor maps over the
 // extractor's own workspace, tile geometry, kernel instantiation) and the split-K scratch those plans own.
@@ -67,28 +57,17 @@ using namespace xvb;
 struct xvb_extractor {
   std::shared_ptr<const Model> m;
   Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
-  // workspace
-  long long cap_frames = 0;
-  int cap_B = 0;
-  uint16_t* in_hi = nullptr; uint16_t* in_lo = nullptr;        // (B,T,ldf)
-  uint16_t* act_hi[2] = {nullptr, nullptr};                    // ping-pong (B,T,max_c)
-  uint16_t* act_lo[2] = {nullptr, nullptr};
-  float* last_f32 = nullptr;                                   // (B,T,C_last)
-  float* stats = nullptr;                                      // (B,2*C_last)
-  float* emb_ws = nullptr;                                     // (B,D): nominal target of the last layer's plan
-  uint16_t* stats_hi = nullptr; uint16_t* stats_lo = nullptr;
-  uint16_t* seg_hi[2] = {nullptr, nullptr}; uint16_t* seg_lo[2] = {nullptr, nullptr};  // (B,max_seg_c)
+  // workspace, each buffer grown to the largest call seen: the input planes (B, pad_front + T + pad_back, ldf), the
+  // ping-pong activations (B, T, max_c), the last frame layer's fp32 output (B, T, C_last), the pooled statistics
+  // (B, 2 C_last) in fp32, the nominal target of the last segment layer's plan (B, D), the pooled statistics as planes,
+  // the segment ping-pong (B, max_seg_c), the partials of the fused pooling epilogue (time blocks, B, 2 C_last) and the
+  // per-utterance frame counts of a masked call (xvb_extractor_extract_lengths)
+  enum { kIn, kAct0, kAct1, kLast, kStats, kEmb, kStatsPlanes, kSeg0, kSeg1, kPoolPartial, kLengths, kBufs };
+  Workspace<kBufs> ws;
   int last_launches = 0;
   bool fused_pooling = true;
-  bool im2col_first = false;   // this lane's copy of the model's decision (see Model)
-  int pad_front = 0, pad_back = 0;
-  float* pool_partial = nullptr;
-  size_t pool_partial_cap = 0;
-  // per-utterance frame counts of the last masked call (xvb_extractor_extract_lengths), on the device
-  int* d_lengths = nullptr;
-  int d_lengths_cap = 0;
-  // launch plans per batch shape (B, T, masked); they hold pointers into the workspace (and, masked, into d_lengths),
-  // so anything that reallocates either clears them
+  Im2col im2col;   // this lane's copy of the model's choice
+  // launch plans per batch shape (B, T, masked); they hold workspace addresses, so a reserve that reallocates clears them
   std::map<std::tuple<int, int, bool>, StepPlan*> plans;
   // optional per-kernel CUDA-event timing on the launching stream (bench.py roofline)
   bool profiling = false;
@@ -98,13 +77,10 @@ struct xvb_extractor {
   cudaStream_t events_stream = nullptr;
   Shard<xvb_extractor> shard;
 
-  explicit xvb_extractor(std::shared_ptr<const Model> model) : m(std::move(model)) {
-    im2col_first = m->im2col_first; pad_front = m->pad_front; pad_back = m->pad_back;
-  }
+  explicit xvb_extractor(std::shared_ptr<const Model> model) : m(std::move(model)), im2col(m->im2col) {}
   ~xvb_extractor() {
-    free_ws();
+    drop_plans();
     for (cudaEvent_t e : events) cudaEventDestroy(e);
-    cudaFree(pool_partial); cudaFree(d_lengths);
   }
 
   void drop_plans() {
@@ -122,17 +98,9 @@ struct xvb_extractor {
     XVB_CUDA(cudaEventRecord(events[events_used++], s));
     return XVB_OK;
   }
-
-  void free_ws() {
-    drop_plans();
-    cudaFree(in_hi); cudaFree(in_lo);
-    for (int i = 0; i < 2; ++i) { cudaFree(act_hi[i]); cudaFree(act_lo[i]); cudaFree(seg_hi[i]); cudaFree(seg_lo[i]); }
-    cudaFree(last_f32); cudaFree(stats); cudaFree(stats_hi); cudaFree(stats_lo); cudaFree(emb_ws);
-    in_hi = in_lo = nullptr; last_f32 = stats = emb_ws = nullptr; stats_hi = stats_lo = nullptr;
-    for (int i = 0; i < 2; ++i) act_hi[i] = act_lo[i] = seg_hi[i] = seg_lo[i] = nullptr;
-    cap_frames = 0; cap_B = 0;
-  }
 };
+
+using H = xvb_extractor;
 
 template <>
 struct xvb::ShardFamily<xvb_extractor> {
@@ -219,16 +187,7 @@ extern "C" int xvb_extractor_finalize(xvb_extractor_t* h, float pooling_eps) {
   }
   XVB_CHECK_ARG(m->segment.back().Cout % 4 == 0, "last segment layer: Cout must be a multiple of 4");
   m->pooling_eps = pooling_eps;
-  {
-    const Layer& L0 = m->frame[0];
-    bool consecutive = L0.ntaps > 1 && L0.ctx[0] <= 0 && L0.ctx[L0.ntaps - 1] >= 0;
-    for (int i = 1; i < L0.ntaps; ++i) consecutive = consecutive && L0.ctx[i] == L0.ctx[i - 1] + 1;
-    const int knob = getenv("XVB_IM2COL") ? atoi(getenv("XVB_IM2COL")) : 1;   // read per extractor: tests flip it
-    m->im2col_first = knob && consecutive && m->feat_dim % 16 == 0;   // plane pitch == packed tap pitch
-    m->pad_front = m->im2col_first ? -L0.ctx[0] : 0;
-    m->pad_back = m->im2col_first ? L0.ctx[L0.ntaps - 1] : 0;
-  }
-  h->im2col_first = m->im2col_first; h->pad_front = m->pad_front; h->pad_back = m->pad_back;
+  m->im2col = h->im2col = im2col_choice(m->frame[0].ctx, m->frame[0].ntaps, m->feat_dim);
   h->draft = nullptr;
   return XVB_OK;
 }
@@ -237,36 +196,20 @@ extern "C" int xvb_extractor_embed_dim(const xvb_extractor_t* h) {
   return (h && !h->m->segment.empty()) ? h->m->segment.back().Cout : XVB_ESTATE;
 }
 
-static int reserve(xvb_extractor* h, int B, int T) {
-  const long long frames = (long long)B * T;
-  if (frames <= h->cap_frames && B <= h->cap_B) return XVB_OK;
-  const long long nf = frames > h->cap_frames ? frames : h->cap_frames;
-  const int nb = B > h->cap_B ? B : h->cap_B;
-  h->free_ws();
-  int rc;
+// Grows the workspace to what one (B, T, masked) call needs.  Any reallocation drops the launch plans, which hold the
+// old addresses.  Without growth this is host arithmetic only.
+static int reserve(H* h, int B, int T, bool masked) {
   const Model* m = h->m.get();
-  const size_t in_rows = (size_t)nf + (size_t)nb * (h->pad_front + h->pad_back);
-  if ((rc = dev_alloc(&h->in_hi, in_rows * m->ldf))) return rc;
-  if ((rc = dev_alloc(&h->in_lo, in_rows * m->ldf))) return rc;
-  if (m->max_c > 0)
-    for (int i = 0; i < 2; ++i) {
-      if ((rc = dev_alloc(&h->act_hi[i], (size_t)nf * m->max_c))) return rc;
-      if ((rc = dev_alloc(&h->act_lo[i], (size_t)nf * m->max_c))) return rc;
-    }
-  const int cl = m->frame.back().Cout;
-  if ((rc = dev_alloc(&h->last_f32, (size_t)nf * cl))) return rc;
-  if ((rc = dev_alloc(&h->stats, (size_t)nb * 2 * cl))) return rc;
-  if ((rc = dev_alloc(&h->emb_ws, (size_t)nb * m->segment.back().Cout))) return rc;
-  if ((rc = dev_alloc(&h->stats_hi, (size_t)nb * 2 * cl))) return rc;
-  if ((rc = dev_alloc(&h->stats_lo, (size_t)nb * 2 * cl))) return rc;
-  if (m->max_seg_c > 0)
-    for (int i = 0; i < 2; ++i) {
-      if ((rc = dev_alloc(&h->seg_hi[i], (size_t)nb * m->max_seg_c))) return rc;
-      if ((rc = dev_alloc(&h->seg_lo[i], (size_t)nb * m->max_seg_c))) return rc;
-    }
-  h->cap_frames = nf;
-  h->cap_B = nb;
-  return XVB_OK;
+  const size_t b = (size_t)B, f = (size_t)B * T, cl = (size_t)m->frame.back().Cout;
+  const size_t pool = h->fused_pooling && !masked ? (size_t)xvb_pool_partial_blocks(B, T, nullptr) * b * 2 * cl : 0;
+  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->ldf,
+                                 f * m->max_c, f * m->max_c, f * cl, b * 2 * cl, b * m->segment.back().Cout, b * 2 * cl,
+                                 b * m->max_seg_c, b * m->max_seg_c, pool, masked ? b : 0};
+  const bool planes[H::kBufs] = {true, true, true, false, false, false, true, true, true, false, false};
+  uint64_t grown;
+  const int rc = h->ws.reserve(need, planes, &grown);
+  if (grown) h->drop_plans();
+  return rc;
 }
 
 // Build the launch plan of one batch shape (see StepPlan).  On failure nothing is cached.
@@ -274,14 +217,13 @@ static int reserve(xvb_extractor* h, int B, int T) {
 // epilogue then zeroes the frames past each utterance's end, and always keeps the last layer's fp32 output for the
 // length-aware standalone pooling (the fused pooling epilogue takes equal lengths only); the segment layers see one row
 // per utterance either way.
-static int build_step_plan(xvb_extractor* h, int B, int T, bool masked, StepPlan** out) {
+static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
   const Model* m = h->m.get();
   StepPlan* sp = new StepPlan();
   struct Guard { StepPlan* p; ~Guard() { delete p; } } guard{sp};
   int rc;
   sp->pool_blocks = xvb_pool_partial_blocks(B, T, &sp->pool_tb);
-  const uint16_t* x_hi = h->in_hi;
-  const uint16_t* x_lo = h->in_lo;
+  Planes x = h->ws.planes(H::kIn);
   int64_t ldx = m->ldf;
   auto add = [&](std::vector<GemmPlan*>& dst, const xvb_tdnn_args_t& a) -> int {
     void* scratch = nullptr;
@@ -299,55 +241,54 @@ static int build_step_plan(xvb_extractor* h, int B, int T, bool masked, StepPlan
   for (size_t i = 0; i < m->frame.size(); ++i) {
     const Layer& L = m->frame[i];
     const bool last = i + 1 == m->frame.size();
-    uint16_t* y_hi = last ? nullptr : h->act_hi[i & 1];
-    uint16_t* y_lo = last ? nullptr : h->act_lo[i & 1];
+    const Planes y = last ? Planes{} : h->ws.planes(H::kAct0 + (i & 1));
     xvb_tdnn_args_t a{};
-    a.x_hi = x_hi; a.x_lo = x_lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
+    a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
     a.bias = L.bias; a.bn_scale = L.scale; a.bn_shift = L.shift; a.flags = L.flags;
     a.context_host = L.ctx; a.ntaps = L.ntaps;
-    a.y_hi = y_hi; a.y_lo = y_lo; a.ldy = L.Cout;
+    a.y_hi = y.hi; a.y_lo = y.lo; a.ldy = L.Cout;
     a.B = B; a.T = T; a.Cin = L.Cin; a.Cout = L.Cout;
-    a.lengths = masked ? h->d_lengths : nullptr;
+    a.lengths = masked ? h->ws.i32(H::kLengths) : nullptr;
     const int ctx0 = 0;
-    if (i == 0 && h->im2col_first) {   // window of ntaps consecutive frames = one long row of the padded planes
+    if (i == 0 && h->im2col.on) {   // window of ntaps consecutive frames = one long row of the padded planes
       a.context_host = &ctx0; a.ntaps = 1; a.Cin = L.ntaps * L.Cin;
-      a.x_batch_stride = (int64_t)(T + h->pad_front + h->pad_back) * ldx;
+      a.x_batch_stride = (int64_t)(T + h->im2col.pad_front + h->im2col.pad_back) * ldx;
     }
     if (last && h->fused_pooling && !masked) {
-      a.pool_partial = h->pool_partial;
+      a.pool_partial = h->ws.f32(H::kPoolPartial);
     } else if (last) {
-      a.y_f32 = h->last_f32; a.ldyf = L.Cout;
+      a.y_f32 = h->ws.f32(H::kLast); a.ldyf = L.Cout;
     }
     rc = add(sp->frame, a);
-    if (rc && i == 0 && h->im2col_first) return -1000;   // overlapping tensor map refused: caller falls back for good
+    if (rc && i == 0 && h->im2col.on) return -1000;   // overlapping tensor map refused: caller falls back for good
     if (rc) return rc;
-    x_hi = y_hi; x_lo = y_lo; ldx = L.Cout;
+    x = y; ldx = L.Cout;
   }
   const int cl = m->frame.back().Cout;
-  x_hi = h->stats_hi; x_lo = h->stats_lo; ldx = 2 * cl;
+  x = h->ws.planes(H::kStatsPlanes); ldx = 2 * cl;
   for (size_t i = 0; i < m->segment.size(); ++i) {
     const Layer& L = m->segment[i];
     const bool last = i + 1 == m->segment.size();
-    uint16_t* y_hi = last ? nullptr : h->seg_hi[i & 1];
-    uint16_t* y_lo = last ? nullptr : h->seg_lo[i & 1];
+    const Planes y = last ? Planes{} : h->ws.planes(H::kSeg0 + (i & 1));
     xvb_tdnn_args_t a{};
-    a.x_hi = x_hi; a.x_lo = x_lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
+    a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
     a.bias = L.bias; a.bn_scale = L.scale; a.bn_shift = L.shift; a.flags = L.flags;
     a.context_host = L.ctx; a.ntaps = 1;
-    a.y_hi = y_hi; a.y_lo = y_lo; a.ldy = L.Cout;
-    if (last) { a.y_f32 = h->emb_ws; a.ldyf = L.Cout; }   // redirected to the caller's matrix at launch
+    a.y_hi = y.hi; a.y_lo = y.lo; a.ldy = L.Cout;
+    if (last) { a.y_f32 = h->ws.f32(H::kEmb); a.ldyf = L.Cout; }   // redirected to the caller's matrix at launch
     a.B = B; a.T = 1; a.Cin = L.Cin; a.Cout = L.Cout;
     if ((rc = add(sp->segment, a))) return rc;
-    x_hi = y_hi; x_lo = y_lo; ldx = L.Cout;
+    x = y; ldx = L.Cout;
   }
   guard.p = nullptr;
   *out = sp;
   return XVB_OK;
 }
 
-// One batch through the stack.  masked: h->d_lengths already holds the B utterance lengths (stream-ordered on `stream`).
-static int extract_batch(xvb_extractor* h, const float* feats, int B, int T, bool masked, float* emb, void* stream) {
-  int rc = reserve(h, B, T);
+// One batch through the stack.  masked: the workspace's lengths already hold the B utterance lengths (stream-ordered on
+// `stream`).
+static int extract_batch(H* h, const float* feats, int B, int T, bool masked, float* emb, void* stream) {
+  int rc = reserve(h, B, T, masked);
   if (rc) return rc;
   const Model* m = h->m.get();
   const long before = g_launches;
@@ -360,21 +301,9 @@ static int extract_batch(xvb_extractor* h, const float* feats, int B, int T, boo
   if (it != h->plans.end()) {
     sp = it->second;
   } else {
-    if (h->fused_pooling && !masked) {   // partials of the fused pooling epilogue: (time blocks, B, 2C) fp32
-      int tb = 0;
-      const size_t need = (size_t)xvb_pool_partial_blocks(B, T, &tb) * B * 2 * m->frame.back().Cout;
-      if (need > h->pool_partial_cap) {
-        h->drop_plans();      // they point into the old buffer
-        cudaFree(h->pool_partial);
-        h->pool_partial = nullptr; h->pool_partial_cap = 0;
-        if ((rc = dev_alloc(&h->pool_partial, need))) return rc;
-        h->pool_partial_cap = need;
-      }
-    }
     rc = build_step_plan(h, B, T, masked, &sp);
     if (rc == -1000) {        // the driver refused the overlapping (im2col) tensor map: plain first layer from now on
-      h->im2col_first = false;
-      h->pad_front = h->pad_back = 0;
+      h->im2col = Im2col{};
       h->drop_plans();
       return extract_batch(h, feats, B, T, masked, emb, stream);
     }
@@ -385,11 +314,12 @@ static int extract_batch(xvb_extractor* h, const float* feats, int B, int T, boo
   // 1. stage the frame matrix as split planes (framework.py:28-33 staging); for the im2col first layer with
   //    the zero frames of F.pad (components.py:117) written out around every utterance; a masked batch also writes
   //    zeros for every frame past an utterance's end, so no layer ever reads what the caller left there
-  const int* lens = masked ? h->d_lengths : nullptr;
-  if (h->im2col_first || masked)
-    rc = split_frames(feats, B, T, m->feat_dim, h->in_hi, h->in_lo, m->ldf, h->pad_front, h->pad_back, lens, stream);
+  const int* lens = masked ? h->ws.i32(H::kLengths) : nullptr;
+  const Planes in = h->ws.planes(H::kIn);
+  if (h->im2col.on || masked)
+    rc = split_frames(feats, B, T, m->feat_dim, in.hi, in.lo, m->ldf, h->im2col.pad_front, h->im2col.pad_back, lens, stream);
   else
-    rc = xvb_split_f32(feats, (int64_t)B * T, m->feat_dim, m->feat_dim, h->in_hi, h->in_lo, m->ldf, stream);
+    rc = xvb_split_f32(feats, (int64_t)B * T, m->feat_dim, m->feat_dim, in.hi, in.lo, m->ldf, stream);
   if (rc) return rc;
   if ((rc = h->mark(cs))) return rc;
   // 2. frame-level TDNN stack (xvector.py:85-89)
@@ -399,11 +329,13 @@ static int extract_batch(xvb_extractor* h, const float* feats, int B, int T, boo
   }
   // 3. statistics pooling (xvector.py:90, pooling.py:58-67)
   const int cl = m->frame.back().Cout;
+  float* stats = h->ws.f32(H::kStats);
+  const Planes pooled = h->ws.planes(H::kStatsPlanes);
   if (h->fused_pooling && !masked)
-    rc = xvb_pool_finalize(h->pool_partial, sp->pool_blocks, sp->pool_tb, B, T, cl, m->pooling_eps, 0, h->stats, h->stats_hi,
-                           h->stats_lo, 2 * cl, stream);
+    rc = xvb_pool_finalize(h->ws.f32(H::kPoolPartial), sp->pool_blocks, sp->pool_tb, B, T, cl, m->pooling_eps, 0, stats,
+                           pooled.hi, pooled.lo, 2 * cl, stream);
   else
-    rc = stats_pool(h->last_f32, cl, B, T, cl, m->pooling_eps, 0, lens, h->stats, h->stats_hi, h->stats_lo, 2 * cl, stream);
+    rc = stats_pool(h->ws.f32(H::kLast), cl, B, T, cl, m->pooling_eps, 0, lens, stats, pooled.hi, pooled.lo, 2 * cl, stream);
   if (rc) return rc;
   if ((rc = h->mark(cs))) return rc;
   // 4. segment-level layers (xvector.py:92-96); the last one writes the caller's embedding matrix
@@ -433,17 +365,10 @@ extern "C" int xvb_extractor_extract_lengths(xvb_extractor_t* h, const float* fe
     all_T = all_T && lengths_host[b] == T;
   }
   if (all_T) return extract_batch(h, feats, B, T, false, emb, stream);   // nothing to mask: the unmasked call itself
-  if (B > h->d_lengths_cap) {
-    h->drop_plans();          // the masked ones point at the old buffer
-    cudaFree(h->d_lengths);
-    h->d_lengths = nullptr; h->d_lengths_cap = 0;
-    const int cap = B > h->cap_B ? B : h->cap_B;
-    int rc = dev_alloc(&h->d_lengths, (size_t)cap);
-    if (rc) return rc;
-    h->d_lengths_cap = cap;
-  }
+  const int rc = reserve(h, B, T, true);   // first, so that the lengths land in the buffer the plans read
+  if (rc) return rc;
   // stream-ordered: the previous call's kernels on `stream` have read the old lengths before these land
-  XVB_CUDA(cudaMemcpyAsync(h->d_lengths, lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice,
+  XVB_CUDA(cudaMemcpyAsync(h->ws.i32(H::kLengths), lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice,
                            (cudaStream_t)stream));
   return extract_batch(h, feats, B, T, true, emb, stream);
 }
@@ -520,7 +445,7 @@ extern "C" int xvb_extractor_last_launches(const xvb_extractor_t* h) { return h 
 
 extern "C" const float* xvb_extractor_debug_f32(const xvb_extractor_t* h, int which) {
   if (!h) return nullptr;
-  return which < 0 ? h->stats : h->last_f32;
+  return h->ws.f32(which < 0 ? H::kStats : H::kLast);
 }
 
 extern "C" void xvb_extractor_destroy(xvb_extractor_t* h) { delete h; }

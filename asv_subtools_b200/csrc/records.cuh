@@ -2,6 +2,8 @@
 // device weights (every family), the grow-only workspace, the segment level of the 2-D families and the group loop of
 // an extract call.  The record store and the model-file codec are host code in records.h.
 #pragma once
+#include <stdlib.h>
+
 #include <vector>
 
 #include "common.cuh"
@@ -102,6 +104,7 @@ struct Workspace {
   }
   Planes planes(int i) const { return {(uint16_t*)buf[i][0], (uint16_t*)buf[i][1]}; }
   float* f32(int i) const { return (float*)buf[i][0]; }
+  int* i32(int i) const { return (int*)buf[i][0]; }
   void release(int i) {
     cudaFree(buf[i][0]); cudaFree(buf[i][1]);
     buf[i][0] = buf[i][1] = nullptr;
@@ -109,6 +112,25 @@ struct Workspace {
   }
   void free() { for (int i = 0; i < N; ++i) release(i); }
 };
+
+// The first layer of the TDNN and ECAPA-TDNN as an im2col view: a window of ntaps consecutive frames is one long row
+// of planes padded with pad_front / pad_back zero frames around every utterance (7 channel blocks instead of 10 for
+// [-2..2] x 80).  A model fixes it at finalize; each lane keeps a copy and turns it off for good if the driver refuses
+// the overlapping tensor map.
+struct Im2col {
+  bool on = false;
+  int pad_front = 0, pad_back = 0;
+};
+
+// Consecutive taps around 0, and feat_dim % 16 == 0 so that the plane pitch is the packed tap pitch.  XVB_IM2COL=0
+// turns the view off; it is read for every model, not once per process, since tests flip it between models.
+inline Im2col im2col_choice(const int* ctx, int ntaps, int feat_dim) {
+  bool consecutive = ntaps > 1 && ctx[0] <= 0 && ctx[ntaps - 1] >= 0;
+  for (int i = 1; i < ntaps; ++i) consecutive = consecutive && ctx[i] == ctx[i - 1] + 1;
+  const int knob = getenv("XVB_IM2COL") ? atoi(getenv("XVB_IM2COL")) : 1;
+  if (!knob || !consecutive || feat_dim % 16 != 0) return Im2col{};
+  return Im2col{true, -ctx[0], ctx[ntaps - 1]};
+}
 
 // The segment level of the 2-D families (ResNet, RepVGG): statistics pooling of the last conv's fp32 (B, T', F' * C)
 // output with planes out, then [fc1 ->] fc2 on the wgmma layer kernel at T = 1, each as _PackedAffine runs it.

@@ -66,38 +66,19 @@ struct Model {
 struct xvb_resnet {
   std::shared_ptr<const Model> m;
   Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
-  // workspace, grown to the largest (B, T) seen: seven rotating (B, T', F', C) plane buffers for the roles block
-  // input / activated input / h / identity / z / output / next activated input, the fp32 last-layer output, then the
-  // per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers)
-  static constexpr int kBufs = 7;
-  size_t cap_planes = 0, cap_last = 0;
-  int cap_B = 0;
-  std::vector<void*> ws;
-  Planes buf[kBufs], pooled, seg_mid;
-  float *last = nullptr, *pooled_f32 = nullptr, *se_mean = nullptr, *se_hidden = nullptr, *se_gate = nullptr, *seg_out = nullptr;
+  // workspace, each buffer grown to the largest call seen: seven rotating (B, T', F', C) plane buffers for the roles
+  // block input / activated input / h / identity / z / output / next activated input, picked by index, the fp32
+  // last-layer output, then the per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers)
+  static constexpr int kRotating = 7;
+  enum { kRot0, kLast = kRot0 + kRotating, kPooled, kPooledF32, kSeMean, kSeHidden, kSeGate, kSegMid, kSegOut, kBufs };
+  Workspace<kBufs> ws;
   int last_launches = 0;
   Shard<xvb_resnet> shard;
 
   explicit xvb_resnet(std::shared_ptr<const Model> model) : m(std::move(model)) {}
-  ~xvb_resnet() { free_ws(); }
-
-  void free_ws() {
-    for (void* p : ws) cudaFree(p);
-    ws.clear();
-    cap_planes = cap_last = 0;
-    cap_B = 0;
-  }
-  template <typename T>
-  int alloc(T** p, size_t n) {
-    XVB_CUDA(cudaMalloc((void**)p, (n ? n : 1) * sizeof(T)));
-    ws.push_back(*p);
-    return XVB_OK;
-  }
-  int planes(Planes* p, size_t n) {
-    int rc = alloc(&p->hi, n);
-    return rc ? rc : alloc(&p->lo, n);
-  }
 };
+
+using H = xvb_resnet;
 
 template <>
 struct xvb::ShardFamily<xvb_resnet> {
@@ -127,28 +108,22 @@ void shapes(const Model* m, int B, int T, size_t* planes, size_t* last) {
   *last = (size_t)B * t * f * m->C4;
 }
 
-int reserve(xvb_resnet* h, int B, int T) {
-  size_t np, nl;
-  shapes(h->m.get(), B, T, &np, &nl);
-  if (np <= h->cap_planes && nl <= h->cap_last && B <= h->cap_B) return XVB_OK;
-  np = np > h->cap_planes ? np : h->cap_planes;
-  nl = nl > h->cap_last ? nl : h->cap_last;
-  const size_t nb = (size_t)(B > h->cap_B ? B : h->cap_B);
-  h->free_ws();
+int reserve(H* h, int B, int T) {
   const Model* m = h->m.get();
-  const size_t pooled = (size_t)2 * m->F4 * m->C4, mean = m->Cmax > 256 ? m->Cmax : 256;
-  const size_t out = (size_t)m->tail.out_rows();
-  int rc = XVB_OK;
-  for (int i = 0; i < xvb_resnet::kBufs && !rc; ++i) rc = h->planes(&h->buf[i], np);
-  if (rc || (rc = h->alloc(&h->last, nl)) || (rc = h->planes(&h->pooled, nb * pooled)) || (rc = h->alloc(&h->pooled_f32, nb * pooled)) ||
-      (rc = h->alloc(&h->se_mean, nb * mean)) || (rc = h->alloc(&h->se_hidden, nb * (size_t)(m->Hmax ? m->Hmax : 4))) ||
-      (rc = h->alloc(&h->se_gate, nb * (size_t)m->Cmax)) || (rc = h->planes(&h->seg_mid, nb * (size_t)(m->tail.mid ? m->tail.mid : 8))) ||
-      (rc = h->alloc(&h->seg_out, nb * out))) {
-    h->free_ws();
-    return rc;
-  }
-  h->cap_planes = np; h->cap_last = nl; h->cap_B = (int)nb;
-  return XVB_OK;
+  size_t need[H::kBufs], np;
+  shapes(m, B, T, &np, &need[H::kLast]);
+  for (int i = 0; i < H::kRotating; ++i) need[H::kRot0 + i] = np;
+  const size_t b = (size_t)B;
+  need[H::kPooled] = need[H::kPooledF32] = b * 2 * m->F4 * m->C4;
+  need[H::kSeMean] = b * (m->Cmax > 256 ? m->Cmax : 256);
+  need[H::kSeHidden] = b * (m->Hmax ? m->Hmax : 4);
+  need[H::kSeGate] = b * m->Cmax;
+  need[H::kSegMid] = b * (m->tail.mid ? m->tail.mid : 8);
+  need[H::kSegOut] = b * m->tail.out_rows();
+  bool planes[H::kBufs];
+  for (int i = 0; i < H::kBufs; ++i) planes[i] = i < H::kLast || i == H::kPooled || i == H::kSegMid;
+  uint64_t grown;
+  return h->ws.reserve(need, planes, &grown);
 }
 
 int conv(const Planes& x, const Planes& w, int B, int T, int F, int Cin, int Cout, int k, int stride, const Bn& bn,
@@ -173,11 +148,13 @@ int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, long long P, vo
   int k = 1;
   while (2 * k <= se.kmax && P % (2 * k) == 0) k *= 2;
   const int kc = k * se.C;
-  int rc = xvb_plane_mean(z.hi, z.lo, kc, B, (int)(P / k), kc, h->se_mean, nullptr, nullptr, kc, stream);
-  if (!rc) rc = xvb_small_affine(h->se_mean, kc, se.w1k[log2i(k)], B, kc, se.Hp, se.b1, nullptr, nullptr, XVB_RELU,
-                                 h->se_hidden, se.Hp, nullptr, nullptr, 0, stream);
-  if (!rc) rc = xvb_small_affine(h->se_hidden, se.Hp, se.w2, B, se.Hp, se.C, se.b2, nullptr, nullptr, XVB_SIGMOID,
-                                 h->se_gate, se.C, nullptr, nullptr, 0, stream);
+  float* mean = h->ws.f32(H::kSeMean);
+  float* hidden = h->ws.f32(H::kSeHidden);
+  int rc = xvb_plane_mean(z.hi, z.lo, kc, B, (int)(P / k), kc, mean, nullptr, nullptr, kc, stream);
+  if (!rc) rc = xvb_small_affine(mean, kc, se.w1k[log2i(k)], B, kc, se.Hp, se.b1, nullptr, nullptr, XVB_RELU,
+                                 hidden, se.Hp, nullptr, nullptr, 0, stream);
+  if (!rc) rc = xvb_small_affine(hidden, se.Hp, se.w2, B, se.Hp, se.C, se.b2, nullptr, nullptr, XVB_SIGMOID,
+                                 h->ws.f32(H::kSeGate), se.C, nullptr, nullptr, 0, stream);
   return rc;
 }
 
@@ -185,6 +162,8 @@ int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, long long P, vo
 int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
+  Planes buf[H::kRotating];
+  for (int i = 0; i < H::kRotating; ++i) buf[i] = h->ws.planes(H::kRot0 + i);
   const Model* m = h->m.get();
   const bool pre = m->pre != 0;
   int Tl = T, Fl = m->feat_dim;
@@ -192,8 +171,8 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
   const Bn none;
   {
     const Bn first = pre ? m->blocks[0].bn1 : none;
-    const Planes* a = pre ? &h->buf[ai] : nullptr;
-    rc = xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, h->buf[xi].hi, h->buf[xi].lo,
+    const Planes* a = pre ? &buf[ai] : nullptr;
+    rc = xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi, buf[xi].lo,
                          first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream);
     if (rc) return rc;
   }
@@ -206,38 +185,39 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
     auto take = [&]() { int j = 0; while (used & (1u << j)) ++j; used |= 1u << j; return j; };
     const int hh = take();
     // pre-activation: h = relu(bn2(conv1(relu(bn1(x))))); post-activation: h = relu(bn1(conv1(x)))
-    if ((rc = conv(pre ? h->buf[ai] : h->buf[xi], blk.conv1, B, Tl, Fl, blk.cin, co, 3, st, pre ? blk.bn2 : blk.bn1, nullptr, 1,
-                   &h->buf[hh], nullptr, none, nullptr, stream)))
+    if ((rc = conv(pre ? buf[ai] : buf[xi], blk.conv1, B, Tl, Fl, blk.cin, co, 3, st, pre ? blk.bn2 : blk.bn1, nullptr, 1,
+                   &buf[hh], nullptr, none, nullptr, stream)))
       return rc;
     int id = xi;
     if (blk.has_ds) {   // conv1x1 (stride) + BN of the un-activated block input
       id = take();
-      if ((rc = conv(h->buf[xi], blk.ds, B, Tl, Fl, blk.cin, co, 1, st, blk.dsbn, nullptr, 0, &h->buf[id], nullptr, none, nullptr, stream)))
+      if ((rc = conv(buf[xi], blk.ds, B, Tl, Fl, blk.cin, co, 1, st, blk.dsbn, nullptr, 0, &buf[id], nullptr, none, nullptr, stream)))
         return rc;
     }
     const Bn nxt = (!last && pre) ? m->blocks[i + 1].bn1 : none;
     const int yi = last ? -1 : take();
     const int an = nxt.s ? take() : -1;
-    const Planes* y = yi >= 0 ? &h->buf[yi] : nullptr;
-    const Planes* y2 = an >= 0 ? &h->buf[an] : nullptr;
-    float* yf = last ? h->last : nullptr;
+    const Planes* y = yi >= 0 ? &buf[yi] : nullptr;
+    const Planes* y2 = an >= 0 ? &buf[an] : nullptr;
+    float* yf = last ? h->ws.f32(H::kLast) : nullptr;
     const Bn bn2 = pre ? none : blk.bn2;
     if (!blk.has_se) {   // conv2 [+ bn2] + identity [-> relu] in one epilogue
-      if ((rc = conv(h->buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, &h->buf[id], pre ? 0 : 1, y, yf, nxt, y2, stream))) return rc;
+      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, &buf[id], pre ? 0 : 1, y, yf, nxt, y2, stream))) return rc;
     } else {
       const int zi = take();
-      if ((rc = conv(h->buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, nullptr, 0, &h->buf[zi], nullptr, none, nullptr, stream)))
+      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, nullptr, 0, &buf[zi], nullptr, none, nullptr, stream)))
         return rc;
       const long long P = (long long)Tn * Fn;
-      if ((rc = se_gate(h, blk.se, h->buf[zi], B, P, stream))) return rc;
-      if ((rc = xvb_se_residual(h->buf[zi].hi, h->buf[zi].lo, h->se_gate, h->buf[id].hi, h->buf[id].lo, B, P, co, pre ? 0 : 1,
+      if ((rc = se_gate(h, blk.se, buf[zi], B, P, stream))) return rc;
+      if ((rc = xvb_se_residual(buf[zi].hi, buf[zi].lo, h->ws.f32(H::kSeGate), buf[id].hi, buf[id].lo, B, P, co, pre ? 0 : 1,
                                 y ? y->hi : nullptr, y ? y->lo : nullptr, yf, nxt.s, nxt.t, y2 ? y2->hi : nullptr,
                                 y2 ? y2->lo : nullptr, stream)))
         return rc;
     }
     xi = yi; ai = an; Tl = Tn; Fl = Fn;
   }
-  return m->tail.run(h->last, Fl * m->C4, B, Tl, m->eps, h->pooled, h->pooled_f32, h->seg_mid, h->seg_out, emb, stream);
+  return m->tail.run(h->ws.f32(H::kLast), Fl * m->C4, B, Tl, m->eps, h->ws.planes(H::kPooled), h->ws.f32(H::kPooledF32),
+                     h->ws.planes(H::kSegMid), h->ws.f32(H::kSegOut), emb, stream);
 }
 
 }  // namespace

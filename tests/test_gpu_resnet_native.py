@@ -73,8 +73,9 @@ def test_native_matches_reference_golden(monkeypatch, golden, case, pos):
 def test_workspace_reuse_across_shapes(monkeypatch):
     ex = _extractor(monkeypatch, "online", "near", True)
     big, small = _feats(64, 200, 80, 1), _feats(3, 37, 80, 2)
-    results = [ex.extract(big).clone(), ex.extract(small).clone(), ex.extract(big).clone()]
-    for x, got in zip((big, small, big), results):
+    wide = _feats(96, 20, 80, 5)   # the batch grows, the positions shrink: only the per-utterance buffers grow
+    results = [ex.extract(big).clone(), ex.extract(small).clone(), ex.extract(big).clone(), ex.extract(wide).clone()]
+    for x, got in zip((big, small, big, wide), results):
         fresh = NativeResNetExtractor(_model("online", "near"))
         assert torch.equal(got, fresh.extract(x))
         fresh.close()
