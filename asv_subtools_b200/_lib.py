@@ -35,7 +35,7 @@ class Conv2dArgs(C.Structure):
                 ("scale", C.c_void_p), ("shift", C.c_void_p), ("res_hi", C.c_void_p), ("res_lo", C.c_void_p),
                 ("relu", C.c_int), ("y_hi", C.c_void_p), ("y_lo", C.c_void_p), ("y_f32", C.c_void_p),
                 ("scale2", C.c_void_p), ("shift2", C.c_void_p), ("y2_hi", C.c_void_p), ("y2_lo", C.c_void_p),
-                ("stride_t", C.c_int)]
+                ("stride_t", C.c_int), ("lengths", C.c_void_p)]
 
 
 class LayerNormArgs(C.Structure):
@@ -111,6 +111,7 @@ SIGNATURES = {
     "xvb_stats_pool_lengths": (_i, [_p, _i64, _i, _i, _i, _f, _i, _p, _p, _p, _p, _i64, _p]),
     "xvb_extractor_set_fused_pooling": (_i, [_p, _i]),
     "xvb_plane_mean": (_i, [_p, _p, _i64, _i, _i, _i, _p, _p, _p, _i64, _p]),
+    "xvb_plane_mean_lengths": (_i, [_p, _p, _i64, _i, _i, _i, _p, _i, _p, _p, _p, _i64, _p]),
     "xvb_res2net_block": (_i, [_p, _p, _i64, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _i, _i, _p]),
     "xvb_copy_rows": (_i, [_p, _i64, _p, _i64, _i64, _i64, _p]),
     "xvb_se_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i64, _i, _i, _i, _p]),
@@ -155,6 +156,7 @@ SIGNATURES = {
     "xvb_conv2d": (_i, [_p, _p]),
     "xvb_conv2d_head": (_i, [_p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_taps": (_i, [_p, _ip, _i, _p]),
+    "xvb_conv2d_head_lengths": (_i, [_p, _i, _i, _i, _p, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_head_k": (_i, [_p, _i, _i, _i, _p, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_valid": (_i, [_p, _p]),
     "xvb_subsample_head": (_i, [_p, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
@@ -166,6 +168,7 @@ SIGNATURES = {
     "xvb_cam_gate": (_i, [_p, _p, _i64, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p]),
     "xvb_seg_gate_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
+    "xvb_se_residual_lengths": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_extractor_add_segment_layer": (_i, [_p, _i, _p, _p, _p, _p, _i]),
@@ -210,6 +213,7 @@ SIGNATURES = {
     "xvb_resnet_embed_dim": (_i, [_p]),
     "xvb_resnet_last_launches": (_i, [_p]),
     "xvb_resnet_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_resnet_extract_lengths": (_i, [_p, _p, _p, _i, _i, _p, _p]),
     "xvb_resnet_extract_host": (_i, [_p, _p, _i, _i, _p, _p]),
     "xvb_resnet_extract_shard": (_i, [_p, _p, C.c_int64, _i, _i, _p, _p]),
     "xvb_resnet_extract_shard_host": (_i, [_p, _p, C.c_int64, _i, _i, _p, _p]),

@@ -21,7 +21,9 @@
 //     register accumulators, one TMA producer warp feeding an mbarrier operand ring, two consumer warpgroups;
 //   * epilogue: y = acc * scale[n] + shift[n] (eval BatchNorm after the bias-free conv) [+ residual] [ReLU] -> planes
 //     and/or fp32, and optionally a second output relu(y * scale2[n] + shift2[n]) (the next pre-activation block's
-//     BN-ReLU, which cannot be folded into that block's conv because the zero padding comes after it).
+//     BN-ReLU, which cannot be folded into that block's conv because the zero padding comes after it);
+//   * a masked batch (lengths: each utterance's input length) stores exact zeros at the frames past each utterance's
+//     output length, so the next conv's taps read that utterance's own zero padding; the tiles are computed in full.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -60,6 +62,7 @@ struct Conv2dParams {
   const float* shift2;
   __nv_bfloat16* y2_hi;
   __nv_bfloat16* y2_lo;
+  const int* lengths;   // NULL, or the input length of each utterance (xvb_conv2d_args_t.lengths)
 };
 
 template <int BLOCK_N>
@@ -81,6 +84,27 @@ __device__ __forceinline__ void decode_conv_tile(const Conv2dParams& p, int tile
   m /= p.num_f_blk;
   t0 = (m % p.num_t_blk) * p.Tb;
   b0 = (m / p.num_t_blk) * p.Bb;
+}
+
+// A masked batch's output frames past an utterance's end: zeros in every output (y, y_f32, y2), this thread's column
+// pairs c, c + 8, ... below c_end.  Out of line, so that the unmasked epilogue keeps its code and registers.
+__device__ __noinline__ void conv_zero_row(const Conv2dParams& p, long long off, int c_begin, int c_end) {
+  for (int c = c_begin; c < c_end; c += 8) {
+    if (p.y_hi) {
+      *reinterpret_cast<uint32_t*>(p.y_hi + off + c) = 0u;
+      *reinterpret_cast<uint32_t*>(p.y_lo + off + c) = 0u;
+    }
+    if (p.y_f32) *reinterpret_cast<float2*>(p.y_f32 + off + c) = make_float2(0.f, 0.f);
+    if (p.y2_hi) {
+      *reinterpret_cast<uint32_t*>(p.y2_hi + off + c) = 0u;
+      *reinterpret_cast<uint32_t*>(p.y2_lo + off + c) = 0u;
+    }
+  }
+}
+
+// Output frames of utterance b in a masked batch: the conv's own rule (conv2d_run's To) applied to its input length.
+__device__ __noinline__ int conv_out_length(const Conv2dParams& p, int b) {
+  return (__ldg(p.lengths + b) + 2 * p.pad - p.ks) / p.stride_t + 1;
 }
 
 template <int BLOCK_N>
@@ -198,6 +222,10 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
       const int b = b0 + (row >> (p.log2_fb + p.log2_tb));
       if (f >= p.Fo || t >= p.To || b >= p.B) continue;
       const long long off = (((long long)b * p.To + t) * p.Fo + f) * p.Cout;
+      if (p.lengths && t >= conv_out_length(p, b)) {   // masked batch, frame past the utterance's end
+        conv_zero_row(p, off, n0 + 2 * q4, min(n0 + BLOCK_N, p.Cout));
+        continue;
+      }
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 8; ++i) {
         const int c = n0 + 8 * i + 2 * q4;   // Cout % 16 == 0: c and c + 1 both exist or neither
@@ -239,9 +267,11 @@ conv2d_bf16x3_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_
 
 // Head conv (Cin = 1, KxK with K = 3 or 5, stride 1, padding K/2) on CUDA cores, fp32: its input rows (one value per
 // position) break TMA's 16-byte rule and it is ~0.1 % of the MACs.  One thread per (position, 8 output channels);
-// fused BN + ReLU, the split to planes and the optional second output relu(y * scale2 + shift2).
+// fused BN + ReLU, the split to planes and the optional second output relu(y * scale2 + shift2).  A masked batch
+// (lengths != NULL) reads the frames t >= lengths[b] as zeros and stores zeros there.
 template <int K>
-__global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int F, const float* __restrict__ w, int Cout,
+__global__ void head_conv_kernel(const float* __restrict__ x, const int* __restrict__ lengths, int B, int T, int F,
+                                 const float* __restrict__ w, int Cout,
                                  const float* __restrict__ scale, const float* __restrict__ shift,
                                  __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl,
                                  const float* __restrict__ scale2, const float* __restrict__ shift2,
@@ -255,13 +285,25 @@ __global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int 
     const long long bt = pos / F;
     const int t = (int)(bt % T);
     const long long b = bt / T;
+    const int L = lengths ? __ldg(lengths + b) : T;
+    uint4 h, l;
+    if (t >= L) {
+      h = l = make_uint4(0u, 0u, 0u, 0u);
+      *reinterpret_cast<uint4*>(yh + pos * Cout + c0) = h;
+      *reinterpret_cast<uint4*>(yl + pos * Cout + c0) = l;
+      if (y2h) {
+        *reinterpret_cast<uint4*>(y2h + pos * Cout + c0) = h;
+        *reinterpret_cast<uint4*>(y2l + pos * Cout + c0) = l;
+      }
+      continue;
+    }
     float in[K * K];
 #pragma unroll
     for (int kf = 0; kf < K; ++kf)
 #pragma unroll
       for (int kt = 0; kt < K; ++kt) {
         const int ff = f + kf - K / 2, tt = t + kt - K / 2;
-        in[kf * K + kt] = (ff >= 0 && ff < F && tt >= 0 && tt < T) ? __ldg(x + (b * T + tt) * F + ff) : 0.f;
+        in[kf * K + kt] = (ff >= 0 && ff < F && tt >= 0 && tt < L) ? __ldg(x + (b * T + tt) * F + ff) : 0.f;
       }
     float y[8], y2[8];
 #pragma unroll
@@ -273,7 +315,6 @@ __global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int 
       y[k] = fmaxf(fmaf(s, __ldg(scale + c0 + k), __ldg(shift + c0 + k)), 0.f);
       if (y2h) y2[k] = fmaxf(fmaf(y[k], __ldg(scale2 + c0 + k), __ldg(shift2 + c0 + k)), 0.f);
     }
-    uint4 h, l;
     pack8(y, h, l);
     *reinterpret_cast<uint4*>(yh + pos * Cout + c0) = h;
     *reinterpret_cast<uint4*>(yl + pos * Cout + c0) = l;
@@ -286,10 +327,12 @@ __global__ void head_conv_kernel(const float* __restrict__ x, int B, int T, int 
 }
 
 // y = [relu]( z * gate[b, c] + identity ) over (B, P, C) planes -> planes and/or fp32 [, relu(y * scale2 + shift2) planes]:
-// SEBlock_2D's scaling (components.py:630-639) with the residual add of BasicBlock (resnet.py:70-104).
+// SEBlock_2D's scaling (components.py:630-639) with the residual add of BasicBlock (resnet.py:70-104).  A masked batch
+// (lengths != NULL, P = T * F positions per utterance) stores zeros at the positions of frames t >= lengths[b].
 __global__ void se_residual_kernel(const __nv_bfloat16* __restrict__ zh, const __nv_bfloat16* __restrict__ zl,
                                    const float* __restrict__ gate, const __nv_bfloat16* __restrict__ ih,
-                                   const __nv_bfloat16* __restrict__ il, long long P, int C, int relu,
+                                   const __nv_bfloat16* __restrict__ il, long long P, int C, const int* __restrict__ lengths,
+                                   int F, int relu,
                                    __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, float* __restrict__ yf,
                                    const float* __restrict__ scale2, const float* __restrict__ shift2,
                                    __nv_bfloat16* __restrict__ y2h, __nv_bfloat16* __restrict__ y2l, long long total) {
@@ -300,6 +343,23 @@ __global__ void se_residual_kernel(const __nv_bfloat16* __restrict__ zh, const _
     const int c = (int)(i % groups) * 8;
     const long long b = pos / P;
     const long long e = pos * C + c;
+    uint4 h, l;
+    if (lengths && pos - b * P >= (long long)__ldg(lengths + b) * F) {
+      h = l = make_uint4(0u, 0u, 0u, 0u);
+      if (yh) {
+        *reinterpret_cast<uint4*>(yh + e) = h;
+        *reinterpret_cast<uint4*>(yl + e) = l;
+      }
+      if (yf) {
+        *reinterpret_cast<float4*>(yf + e) = make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4*>(yf + e + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+      if (y2h) {
+        *reinterpret_cast<uint4*>(y2h + e) = h;
+        *reinterpret_cast<uint4*>(y2l + e) = l;
+      }
+      continue;
+    }
     float z[8], x[8], y[8];
     unpack8(*reinterpret_cast<const uint4*>(zh + e), *reinterpret_cast<const uint4*>(zl + e), z);
     unpack8(*reinterpret_cast<const uint4*>(ih + e), *reinterpret_cast<const uint4*>(il + e), x);
@@ -308,7 +368,6 @@ __global__ void se_residual_kernel(const __nv_bfloat16* __restrict__ zh, const _
     const float g[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
 #pragma unroll
     for (int k = 0; k < 8; ++k) y[k] = fmaxf(__fadd_rn(__fmul_rn(z[k], g[k]), x[k]), floor_v);   // the reference's two roundings
-    uint4 h, l;
     if (yh) {
       pack8(y, h, l);
       *reinterpret_cast<uint4*>(yh + e) = h;
@@ -459,6 +518,7 @@ int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int 
   p.scale2 = a->scale2; p.shift2 = a->shift2;
   p.y2_hi = reinterpret_cast<__nv_bfloat16*>(a->y2_hi);
   p.y2_lo = reinterpret_cast<__nv_bfloat16*>(a->y2_lo);
+  p.lengths = a->lengths;
 
   // input (B, T, F, Cin) planes as a 4-D tensor map (C, F, T, B); box 64 channels x Fb x Tb x Bb output positions
   CUtensorMap mx[2];
@@ -478,7 +538,7 @@ int conv2d_run(const char* fn, const xvb_conv2d_args_t* a, const int* taps, int 
   return launch_conv<32>(mx, p, a->w_hi, a->w_lo, s);
 }
 
-int conv2d_head_run(const char* fn, const float* x, int B, int T, int F, const float* w, int Cout, int ksize,
+int conv2d_head_run(const char* fn, const float* x, const int* lengths, int B, int T, int F, const float* w, int Cout, int ksize,
                     const float* bn_scale, const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2,
                     const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
   XVB_CHECK_ARG(x && w && bn_scale && bn_shift && y_hi && y_lo, "%s: null pointer", fn);
@@ -491,7 +551,7 @@ int conv2d_head_run(const char* fn, const float* x, int B, int T, int F, const f
   const long long total = (long long)B * T * F * (Cout / 8);
   auto kernel = ksize == 5 ? head_conv_kernel<5> : head_conv_kernel<3>;
   kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      x, B, T, F, w, Cout, bn_scale, bn_shift, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
+      x, lengths, B, T, F, w, Cout, bn_scale, bn_shift, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
       scale2, shift2, reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo));
   XVB_LAUNCH_CHECK();
   return XVB_OK;
@@ -537,6 +597,7 @@ extern "C" int xvb_conv2d_valid(const xvb_conv2d_args_t* a, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(a, "xvb_conv2d_valid: null args");
+  XVB_CHECK_ARG(!a->lengths, "xvb_conv2d_valid: lengths are not supported (a masked batch needs the padded convs)");
   XVB_CHECK_ARG((a->ksize == 3 || a->ksize == 1) && (a->stride == 1 || a->stride == 2),
                 "xvb_conv2d_valid: ksize must be 1 or 3 and stride 1 or 2 (got %d, %d)", a->ksize, a->stride);
   int dense[9];
@@ -549,7 +610,7 @@ extern "C" int xvb_conv2d_head(const float* x, int B, int T, int F, const float*
                                const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
-  return conv2d_head_run("xvb_conv2d_head", x, B, T, F, w, Cout, 3, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2, y2_hi,
+  return conv2d_head_run("xvb_conv2d_head", x, nullptr, B, T, F, w, Cout, 3, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2, y2_hi,
                          y2_lo, stream);
 }
 
@@ -558,30 +619,63 @@ extern "C" int xvb_conv2d_head_k(const float* x, int B, int T, int F, const floa
                                  const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
-  return conv2d_head_run("xvb_conv2d_head_k", x, B, T, F, w, Cout, ksize, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2,
+  return conv2d_head_run("xvb_conv2d_head_k", x, nullptr, B, T, F, w, Cout, ksize, bn_scale, bn_shift, y_hi, y_lo, scale2, shift2,
                          y2_hi, y2_lo, stream);
+}
+
+namespace xvb {
+namespace {
+
+int se_residual_run(const char* fn, const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
+                    const uint16_t* id_lo, int B, int64_t P, int C, const int* lengths, int F, int relu, uint16_t* y_hi,
+                    uint16_t* y_lo, float* y_f32, const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo,
+                    void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(z_hi && z_lo && gate && id_hi && id_lo, "%s: null pointer", fn);
+  XVB_CHECK_ARG(B > 0 && P > 0 && C > 0 && C % 8 == 0, "%s: bad shape B=%d P=%lld C=%d", fn, B, (long long)P, C);
+  XVB_CHECK_ARG((y_hi != nullptr) == (y_lo != nullptr) && (y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
+                "%s: hi/lo planes must both be set or both NULL; the second output needs scale2 and shift2", fn);
+  XVB_CHECK_ARG(y_hi || y_f32 || y2_hi, "%s: no output requested", fn);
+  XVB_CHECK_ARG(((uintptr_t)z_hi | (uintptr_t)z_lo | (uintptr_t)gate | (uintptr_t)id_hi | (uintptr_t)id_lo | (uintptr_t)y_hi |
+                 (uintptr_t)y_lo | (uintptr_t)y_f32 | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
+                "%s: pointers must be 16-byte aligned", fn);
+  const long long total = (long long)B * P * (C / 8);
+  se_residual_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+      reinterpret_cast<const __nv_bfloat16*>(z_hi), reinterpret_cast<const __nv_bfloat16*>(z_lo), gate,
+      reinterpret_cast<const __nv_bfloat16*>(id_hi), reinterpret_cast<const __nv_bfloat16*>(id_lo), (long long)P, C, lengths, F,
+      relu ? 1 : 0, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo), y_f32, scale2, shift2,
+      reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo), total);
+  XVB_LAUNCH_CHECK();
+  return XVB_OK;
+}
+
+}  // namespace
+}  // namespace xvb
+
+extern "C" int xvb_conv2d_head_lengths(const float* x, int B, int T, int F, const int* lengths, const float* w, int Cout,
+                                       const float* bn_scale, const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo,
+                                       const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
+  int rc = require_sm90();
+  if (rc) return rc;
+  XVB_CHECK_ARG(lengths, "xvb_conv2d_head_lengths: null lengths");
+  return conv2d_head_run("xvb_conv2d_head_lengths", x, lengths, B, T, F, w, Cout, 3, bn_scale, bn_shift, y_hi, y_lo, scale2,
+                         shift2, y2_hi, y2_lo, stream);
 }
 
 extern "C" int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
                                const uint16_t* id_lo, int B, int64_t P, int C, int relu, uint16_t* y_hi, uint16_t* y_lo,
                                float* y_f32, const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo,
                                void* stream) {
-  int rc = require_sm90();
-  if (rc) return rc;
-  XVB_CHECK_ARG(z_hi && z_lo && gate && id_hi && id_lo, "xvb_se_residual: null pointer");
-  XVB_CHECK_ARG(B > 0 && P > 0 && C > 0 && C % 8 == 0, "xvb_se_residual: bad shape B=%d P=%lld C=%d", B, (long long)P, C);
-  XVB_CHECK_ARG((y_hi != nullptr) == (y_lo != nullptr) && (y2_hi != nullptr) == (y2_lo != nullptr) && (!y2_hi || (scale2 && shift2)),
-                "xvb_se_residual: hi/lo planes must both be set or both NULL; the second output needs scale2 and shift2");
-  XVB_CHECK_ARG(y_hi || y_f32 || y2_hi, "xvb_se_residual: no output requested");
-  XVB_CHECK_ARG(((uintptr_t)z_hi | (uintptr_t)z_lo | (uintptr_t)gate | (uintptr_t)id_hi | (uintptr_t)id_lo | (uintptr_t)y_hi |
-                 (uintptr_t)y_lo | (uintptr_t)y_f32 | (uintptr_t)y2_hi | (uintptr_t)y2_lo) % 16 == 0,
-                "xvb_se_residual: pointers must be 16-byte aligned");
-  const long long total = (long long)B * P * (C / 8);
-  se_residual_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(z_hi), reinterpret_cast<const __nv_bfloat16*>(z_lo), gate,
-      reinterpret_cast<const __nv_bfloat16*>(id_hi), reinterpret_cast<const __nv_bfloat16*>(id_lo), (long long)P, C, relu ? 1 : 0,
-      reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo), y_f32, scale2, shift2,
-      reinterpret_cast<__nv_bfloat16*>(y2_hi), reinterpret_cast<__nv_bfloat16*>(y2_lo), total);
-  XVB_LAUNCH_CHECK();
-  return XVB_OK;
+  return se_residual_run("xvb_se_residual", z_hi, z_lo, gate, id_hi, id_lo, B, P, C, nullptr, 1, relu, y_hi, y_lo, y_f32,
+                         scale2, shift2, y2_hi, y2_lo, stream);
+}
+
+extern "C" int xvb_se_residual_lengths(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
+                                       const uint16_t* id_lo, int B, int T, int F, int C, const int* lengths, int relu,
+                                       uint16_t* y_hi, uint16_t* y_lo, float* y_f32, const float* scale2, const float* shift2,
+                                       uint16_t* y2_hi, uint16_t* y2_lo, void* stream) {
+  XVB_CHECK_ARG(lengths && T > 0 && F > 0, "xvb_se_residual_lengths: null lengths or bad shape T=%d F=%d", T, F);
+  return se_residual_run("xvb_se_residual_lengths", z_hi, z_lo, gate, id_hi, id_lo, B, (int64_t)T * F, C, lengths, F, relu,
+                         y_hi, y_lo, y_f32, scale2, shift2, y2_hi, y2_lo, stream);
 }

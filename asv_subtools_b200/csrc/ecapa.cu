@@ -14,17 +14,20 @@
 namespace xvb {
 
 // ---------------------------------------------------------------- mean over T of planes
+// lengths != NULL: utterance b averages its first lengths[b] * rows_per_length rows (a masked batch).
 constexpr int kPmWarps = 8;
 __global__ void __launch_bounds__(kPmWarps * 32)
-plane_mean_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl, long long ldx, int T, int C,
-                  float* __restrict__ out, __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol, long long ldo) {
+plane_mean_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl, long long ldx, int T_all, int C,
+                  const int* __restrict__ lengths, int rows_per_length, float* __restrict__ out, __nv_bfloat16* __restrict__ oh,
+                  __nv_bfloat16* __restrict__ ol, long long ldo) {
   const int b = blockIdx.y;
+  const int T = lengths ? min(__ldg(lengths + b) * rows_per_length, T_all) : T_all;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int c = blockIdx.x * 256 + lane * 8;
   const bool active = c < C;  // C % 8 == 0
   float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (active) {
-    const long long base = (long long)b * T * ldx + c;
+    const long long base = (long long)b * T_all * ldx + c;
     for (int t = warp; t < T; t += kPmWarps) {
       const uint4 h = *reinterpret_cast<const uint4*>(xh + base + (long long)t * ldx);
       const uint4 l = *reinterpret_cast<const uint4*>(xl + base + (long long)t * ldx);
@@ -676,20 +679,39 @@ extern "C" int xvb_attn_head_stats_pool_mq(const float* logits, int64_t ldl, int
                                      nullptr, 0, out, out_hi, out_lo, ldo, stream);
 }
 
-extern "C" int xvb_plane_mean(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C, float* out,
-                              uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+namespace {
+
+int plane_mean_run(const char* fn, const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C,
+                   const int* lengths, int rows_per_length, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo,
+                   void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
-  XVB_CHECK_ARG(x_hi && x_lo && (out || out_hi), "xvb_plane_mean: null pointer");
-  XVB_CHECK_ARG(B > 0 && T > 0 && C > 0 && C % 8 == 0 && ldx % 8 == 0 && ldx >= C && B <= 65535, "xvb_plane_mean: need C%%8==0, ldx%%8==0");
-  XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "xvb_plane_mean: out_hi/out_lo must both be set or both NULL");
-  if (out_hi) XVB_CHECK_ARG(ldo % 8 == 0 && ldo >= C, "xvb_plane_mean: ldo must be a multiple of 8 and >= C");
+  XVB_CHECK_ARG(x_hi && x_lo && (out || out_hi), "%s: null pointer", fn);
+  XVB_CHECK_ARG(B > 0 && T > 0 && C > 0 && C % 8 == 0 && ldx % 8 == 0 && ldx >= C && B <= 65535, "%s: need C%%8==0, ldx%%8==0", fn);
+  XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "%s: out_hi/out_lo must both be set or both NULL", fn);
+  if (out_hi) XVB_CHECK_ARG(ldo % 8 == 0 && ldo >= C, "%s: ldo must be a multiple of 8 and >= C", fn);
   dim3 grid((C + 255) / 256, B);
   plane_mean_kernel<<<grid, kPmWarps * 32, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const __nv_bfloat16*>(x_hi), reinterpret_cast<const __nv_bfloat16*>(x_lo), ldx, T, C, out,
-      reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
+      reinterpret_cast<const __nv_bfloat16*>(x_hi), reinterpret_cast<const __nv_bfloat16*>(x_lo), ldx, T, C, lengths,
+      rows_per_length, out, reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
+}
+
+}  // namespace
+
+extern "C" int xvb_plane_mean(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C, float* out,
+                              uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+  return plane_mean_run("xvb_plane_mean", x_hi, x_lo, ldx, B, T, C, nullptr, 1, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_plane_mean_lengths(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C,
+                                      const int* lengths, int rows_per_length, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                                      int64_t ldo, void* stream) {
+  XVB_CHECK_ARG(lengths && rows_per_length > 0, "xvb_plane_mean_lengths: null lengths or rows_per_length=%d < 1",
+                rows_per_length);
+  return plane_mean_run("xvb_plane_mean_lengths", x_hi, x_lo, ldx, B, T, C, lengths, rows_per_length, out, out_hi, out_lo,
+                        ldo, stream);
 }
 
 extern "C" int xvb_copy_rows(const void* src, int64_t src_pitch_bytes, void* dst, int64_t dst_pitch_bytes, int64_t rows,

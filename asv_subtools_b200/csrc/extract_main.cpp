@@ -18,9 +18,9 @@
 // (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), the last four written by the native extractors' save().  What it adds:
-// utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector files
-// only) chunks of different lengths share masked batches (plan_mixed_batches, xvb_extractor_extract_lengths), which
-// fills batches on a real corpus where most frame counts occur a few times only.
+// utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector and ResNet
+// x-vector files) chunks of different lengths share masked batches (plan_mixed_batches, xvb_extractor_extract_lengths /
+// xvb_resnet_extract_lengths), which fills batches on a real corpus where most frame counts occur a few times only.
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
@@ -92,7 +92,10 @@ struct Family {
 
 const Family kFamilies[] = {
     {{"XVBE0001", "XVBE0002"}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false, nullptr},
-    {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false, nullptr},
+    {{"XVBR0001", nullptr}, "loading the ResNet model", "xvb_resnet_extract", HANDLE_FAMILY(resnet), 10000, false,
+     [](void* h, const float* x, const int32_t* lens, int B, int T, float* e) {
+       return xvb_resnet_extract_lengths((xvb_resnet_t*)h, x, lens, B, T, e, nullptr);
+     }},
     {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false, nullptr},
     {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false, nullptr},
     {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true, nullptr},
@@ -201,7 +204,7 @@ struct Runner {
     }
     CU(cudaMemcpy(d_feats, h_feats, (size_t)B * T * F * sizeof(float), cudaMemcpyHostToDevice));
     if (masked) {
-      CK(fam->extract_lengths(model, d_feats, lens.data(), B, T, d_emb), "xvb_extractor_extract_lengths");
+      CK(fam->extract_lengths(model, d_feats, lens.data(), B, T, d_emb), (std::string(fam->extract_fn) + "_lengths").c_str());
       ++mixed_batches;
       padded_frames += (long)B * T - frames;
       batch_frames += (long)B * T;
@@ -310,9 +313,10 @@ int main(int argc, char** argv) {
              "4000 for CAM++ and 10000 otherwise.  A Conformer chunk needs at least 7 frames and fewer than 5000 subsampled\n"
              "frames.  CAM++ cuts an utterance with egrecho's rule (max-chunk-long chunks, the last two re-split evenly:\n"
              "9000 -> 4000, 2500, 2500); a chunk needs at least 3 frames.\n"
-             "--mixed-lengths (TDNN x-vector models): after the chunk rule, chunks of different lengths share batches of up\n"
-             "to --batch, taken in ascending length, with at most 1/8 of a batch's frames padding; the summary line also\n"
-             "reports the padded frames.  Vectors differ from the default mode's at the rounding level.\n");
+             "--mixed-lengths (TDNN x-vector and ResNet x-vector models): after the chunk rule, chunks of different\n"
+             "lengths share batches of up to --batch, taken in ascending length, with at most 1/8 of a batch's frames\n"
+             "padding; the summary line also reports the padded frames.  Vectors differ from the default mode's at the\n"
+             "rounding level.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -339,7 +343,8 @@ int main(int argc, char** argv) {
     r.D = r.fam->embed_dim(r.model);
     if (!max_chunk_set) max_chunk = r.fam->max_chunk;
     if (mixed && !r.fam->extract_lengths) {
-      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector model (XVBM0001); '%s' is read with %s\n", pos[0],
+      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector (XVBM0001) or ResNet x-vector (XVBR0001) model; "
+                      "'%s' is read with %s\n", pos[0],
               r.fam->extract_fn);
       return 1;
     }

@@ -176,11 +176,12 @@ struct SegTail {
   int out_rows() const { return seg.back().Cout; }
 
   // last: the (B, T, pc) fp32 output of the last conv -> emb (B, E).  Buffers per utterance: pooled planes and
-  // pooled_f32 of 2 * pc, mid planes of `mid` and out of out_rows() (used when the last layer is padded).
+  // pooled_f32 of 2 * pc, mid planes of `mid` and out of out_rows() (used when the last layer is padded).  lengths:
+  // NULL, or a masked batch's frame counts at the last conv's resolution (device int32[B]), each pooling its own.
   int run(const float* last, int pc, int B, int T, float eps, Planes pooled, float* pooled_f32, Planes mid_planes,
-          float* out, float* emb, void* stream) const {
+          float* out, float* emb, void* stream, const int* lengths = nullptr) const {
     int rc;
-    if ((rc = xvb_stats_pool_ex(last, pc, B, T, pc, eps, 0, pooled_f32, pooled.hi, pooled.lo, 2 * pc, stream))) return rc;
+    if ((rc = stats_pool(last, pc, B, T, pc, eps, 0, lengths, pooled_f32, pooled.hi, pooled.lo, 2 * pc, stream))) return rc;
     Planes x = pooled;
     int64_t ldx = 2 * pc;
     const int ctx0 = 0;

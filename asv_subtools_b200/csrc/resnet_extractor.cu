@@ -68,9 +68,11 @@ struct xvb_resnet {
   Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
   // workspace, each buffer grown to the largest call seen: seven rotating (B, T', F', C) plane buffers for the roles
   // block input / activated input / h / identity / z / output / next activated input, picked by index, the fp32
-  // last-layer output, then the per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers)
+  // last-layer output, then the per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers) and
+  // a masked call's lengths at the four time resolutions (int32 (kLevels, B), level l = after l stride-2 stages)
   static constexpr int kRotating = 7;
-  enum { kRot0, kLast = kRot0 + kRotating, kPooled, kPooledF32, kSeMean, kSeHidden, kSeGate, kSegMid, kSegOut, kBufs };
+  static constexpr int kLevels = 4;
+  enum { kRot0, kLast = kRot0 + kRotating, kPooled, kPooledF32, kSeMean, kSeHidden, kSeGate, kSegMid, kSegOut, kLengths, kBufs };
   Workspace<kBufs> ws;
   int last_launches = 0;
   Shard<xvb_resnet> shard;
@@ -120,6 +122,7 @@ int reserve(H* h, int B, int T) {
   need[H::kSeGate] = b * m->Cmax;
   need[H::kSegMid] = b * (m->tail.mid ? m->tail.mid : 8);
   need[H::kSegOut] = b * m->tail.out_rows();
+  need[H::kLengths] = 0;   // sized by xvb_resnet_extract_lengths for the whole call, before its groups run
   bool planes[H::kBufs];
   for (int i = 0; i < H::kBufs; ++i) planes[i] = i < H::kLast || i == H::kPooled || i == H::kSegMid;
   uint64_t grown;
@@ -127,8 +130,10 @@ int reserve(H* h, int B, int T) {
 }
 
 int conv(const Planes& x, const Planes& w, int B, int T, int F, int Cin, int Cout, int k, int stride, const Bn& bn,
-         const Planes* res, int relu, const Planes* y, float* y_f32, const Bn& bn2, const Planes* y2, void* stream) {
+         const Planes* res, int relu, const Planes* y, float* y_f32, const Bn& bn2, const Planes* y2, const int* lens,
+         void* stream) {
   xvb_conv2d_args_t a{};
+  a.lengths = lens;
   a.x_hi = x.hi; a.x_lo = x.lo;
   a.w_hi = w.hi; a.w_lo = w.lo;
   a.B = B; a.T = T; a.F = F; a.Cin = Cin; a.Cout = Cout; a.ksize = k; a.stride = stride;
@@ -142,15 +147,18 @@ int conv(const Planes& x, const Planes& w, int B, int T, int F, int Cin, int Cou
   return xvb_conv2d(&a, stream);
 }
 
-// sigmoid(fc_2(relu(fc_1(mean over the P positions of z)))) as ResNetExtractor._se_gate: the (B, P, C) planes read as
-// (B, P/k, k*C) with the largest k in the table (2k too) that divides P.
-int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, long long P, void* stream) {
+// sigmoid(fc_2(relu(fc_1(mean over the T * F positions of z)))) as ResNetExtractor._se_gate: the (B, T*F, C) planes
+// read as (B, T*F/k, k*C) with the largest k in the table (2k too) that divides T * F.  A masked batch (lens: frames
+// per utterance) takes the largest such k dividing F, so that k divides every utterance's own positions.
+int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, int T, int F, const int* lens, void* stream) {
+  const long long P = (long long)T * F;
   int k = 1;
-  while (2 * k <= se.kmax && P % (2 * k) == 0) k *= 2;
+  while (2 * k <= se.kmax && (lens ? F : P) % (2 * k) == 0) k *= 2;
   const int kc = k * se.C;
   float* mean = h->ws.f32(H::kSeMean);
   float* hidden = h->ws.f32(H::kSeHidden);
-  int rc = xvb_plane_mean(z.hi, z.lo, kc, B, (int)(P / k), kc, mean, nullptr, nullptr, kc, stream);
+  int rc = lens ? xvb_plane_mean_lengths(z.hi, z.lo, kc, B, (int)(P / k), kc, lens, F / k, mean, nullptr, nullptr, kc, stream)
+                : xvb_plane_mean(z.hi, z.lo, kc, B, (int)(P / k), kc, mean, nullptr, nullptr, kc, stream);
   if (!rc) rc = xvb_small_affine(mean, kc, se.w1k[log2i(k)], B, kc, se.Hp, se.b1, nullptr, nullptr, XVB_RELU,
                                  hidden, se.Hp, nullptr, nullptr, 0, stream);
   if (!rc) rc = xvb_small_affine(hidden, se.Hp, se.w2, B, se.Hp, se.C, se.b2, nullptr, nullptr, XVB_SIGMOID,
@@ -158,8 +166,9 @@ int se_gate(xvb_resnet* h, const Se& se, const Planes& z, int B, long long P, vo
   return rc;
 }
 
-// One group of utterances (B * T * F within the budget, or a single utterance): ResNetExtractor.extract.
-int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, void* stream) {
+// One group of utterances (B * T * F within the budget, or a single utterance): ResNetExtractor.extract.  A masked
+// group passes lens, its lengths at level 0 of the workspace's (kLevels, ld) table; NULL otherwise.
+int extract_group(xvb_resnet* h, const float* feats, int B, int T, const int* lens, int ld, float* emb, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
   Planes buf[H::kRotating];
@@ -169,11 +178,15 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
   int Tl = T, Fl = m->feat_dim;
   int xi = 0, ai = pre ? 1 : -1;
   const Bn none;
+  int level = 0;
+  auto at = [&](int l) { return lens ? lens + (size_t)l * ld : nullptr; };
   {
     const Bn first = pre ? m->blocks[0].bn1 : none;
     const Planes* a = pre ? &buf[ai] : nullptr;
-    rc = xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi, buf[xi].lo,
-                         first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream);
+    rc = lens ? xvb_conv2d_head_lengths(feats, B, T, Fl, lens, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi,
+                                        buf[xi].lo, first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream)
+              : xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi, buf[xi].lo,
+                                first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream);
     if (rc) return rc;
   }
   const int nb = (int)m->blocks.size();
@@ -181,17 +194,20 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
     const Block& blk = m->blocks[i];
     const bool last = i + 1 == nb;
     const int st = blk.stride, co = blk.cout, Tn = (Tl - 1) / st + 1, Fn = (Fl - 1) / st + 1;
+    const int* lin = at(level);   // lengths of the block input and of its output
+    const int* lout = at(st == 2 ? level + 1 : level);
     unsigned used = (1u << xi) | (ai >= 0 ? 1u << ai : 0u);
     auto take = [&]() { int j = 0; while (used & (1u << j)) ++j; used |= 1u << j; return j; };
     const int hh = take();
     // pre-activation: h = relu(bn2(conv1(relu(bn1(x))))); post-activation: h = relu(bn1(conv1(x)))
     if ((rc = conv(pre ? buf[ai] : buf[xi], blk.conv1, B, Tl, Fl, blk.cin, co, 3, st, pre ? blk.bn2 : blk.bn1, nullptr, 1,
-                   &buf[hh], nullptr, none, nullptr, stream)))
+                   &buf[hh], nullptr, none, nullptr, lin, stream)))
       return rc;
     int id = xi;
     if (blk.has_ds) {   // conv1x1 (stride) + BN of the un-activated block input
       id = take();
-      if ((rc = conv(buf[xi], blk.ds, B, Tl, Fl, blk.cin, co, 1, st, blk.dsbn, nullptr, 0, &buf[id], nullptr, none, nullptr, stream)))
+      if ((rc = conv(buf[xi], blk.ds, B, Tl, Fl, blk.cin, co, 1, st, blk.dsbn, nullptr, 0, &buf[id], nullptr, none, nullptr, lin,
+                     stream)))
         return rc;
     }
     const Bn nxt = (!last && pre) ? m->blocks[i + 1].bn1 : none;
@@ -202,22 +218,29 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, float* emb, v
     float* yf = last ? h->ws.f32(H::kLast) : nullptr;
     const Bn bn2 = pre ? none : blk.bn2;
     if (!blk.has_se) {   // conv2 [+ bn2] + identity [-> relu] in one epilogue
-      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, &buf[id], pre ? 0 : 1, y, yf, nxt, y2, stream))) return rc;
+      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, &buf[id], pre ? 0 : 1, y, yf, nxt, y2, lout, stream)))
+        return rc;
     } else {
       const int zi = take();
-      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, nullptr, 0, &buf[zi], nullptr, none, nullptr, stream)))
+      if ((rc = conv(buf[hh], blk.conv2, B, Tn, Fn, co, co, 3, 1, bn2, nullptr, 0, &buf[zi], nullptr, none, nullptr, lout,
+                     stream)))
         return rc;
-      const long long P = (long long)Tn * Fn;
-      if ((rc = se_gate(h, blk.se, buf[zi], B, P, stream))) return rc;
-      if ((rc = xvb_se_residual(buf[zi].hi, buf[zi].lo, h->ws.f32(H::kSeGate), buf[id].hi, buf[id].lo, B, P, co, pre ? 0 : 1,
-                                y ? y->hi : nullptr, y ? y->lo : nullptr, yf, nxt.s, nxt.t, y2 ? y2->hi : nullptr,
-                                y2 ? y2->lo : nullptr, stream)))
-        return rc;
+      if ((rc = se_gate(h, blk.se, buf[zi], B, Tn, Fn, lout, stream))) return rc;
+      const float* gate = h->ws.f32(H::kSeGate);
+      Planes yp, y2p;
+      if (y) yp = *y;
+      if (y2) y2p = *y2;
+      rc = lout ? xvb_se_residual_lengths(buf[zi].hi, buf[zi].lo, gate, buf[id].hi, buf[id].lo, B, Tn, Fn, co, lout, pre ? 0 : 1,
+                                          yp.hi, yp.lo, yf, nxt.s, nxt.t, y2p.hi, y2p.lo, stream)
+                : xvb_se_residual(buf[zi].hi, buf[zi].lo, gate, buf[id].hi, buf[id].lo, B, (long long)Tn * Fn, co, pre ? 0 : 1,
+                                  yp.hi, yp.lo, yf, nxt.s, nxt.t, y2p.hi, y2p.lo, stream);
+      if (rc) return rc;
     }
     xi = yi; ai = an; Tl = Tn; Fl = Fn;
+    if (st == 2) ++level;
   }
   return m->tail.run(h->ws.f32(H::kLast), Fl * m->C4, B, Tl, m->eps, h->ws.planes(H::kPooled), h->ws.f32(H::kPooledF32),
-                     h->ws.planes(H::kSegMid), h->ws.f32(H::kSegOut), emb, stream);
+                     h->ws.planes(H::kSegMid), h->ws.f32(H::kSegOut), emb, stream, at(level));
 }
 
 }  // namespace
@@ -353,7 +376,42 @@ extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, in
   const long before = g_launches;
   const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
   int rc = for_groups(B, (long long)per_utt, kPositionBudget,
-                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, stream); });
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, nullptr, 0, emb + i * E, stream); });
+  if (rc) return rc;
+  h->last_launches = (int)(g_launches - before);
+  return XVB_OK;
+}
+
+extern "C" int xvb_resnet_extract_lengths(xvb_resnet_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
+                                          float* emb, void* stream) {
+  XVB_CHECK_ARG(h && !h->draft, "xvb_resnet_extract_lengths: model not finalized");
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "xvb_resnet_extract_lengths: bad arguments");
+  bool all_T = true;
+  for (int b = 0; b < B; ++b) {
+    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "xvb_resnet_extract_lengths: lengths[%d]=%d outside [1, T=%d]", b,
+                  (int)lengths_host[b], T);
+    all_T = all_T && lengths_host[b] == T;
+  }
+  if (all_T) return xvb_resnet_extract(h, feats, B, T, emb, stream);   // nothing to mask: the unmasked call itself
+  // level l + 1 = ceil(level l / 2): every stride-2 conv's output length, (L + 2 * pad - k) / 2 + 1 for k = 3 and 1
+  std::vector<int32_t> table((size_t)H::kLevels * B);
+  for (int b = 0; b < B; ++b) {
+    table[b] = lengths_host[b];
+    for (int l = 1; l < H::kLevels; ++l) table[(size_t)l * B + b] = (table[(size_t)(l - 1) * B + b] - 1) / 2 + 1;
+  }
+  size_t need[H::kBufs] = {0};
+  bool planes[H::kBufs] = {false};
+  need[H::kLengths] = table.size();
+  uint64_t grown;
+  int rc = h->ws.reserve(need, planes, &grown);
+  if (rc) return rc;
+  int* lens = h->ws.i32(H::kLengths);
+  // stream-ordered: the previous call's kernels on `stream` have read the old table before this one lands
+  XVB_CUDA(cudaMemcpyAsync(lens, table.data(), table.size() * sizeof(int32_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  const long before = g_launches;
+  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
+  rc = for_groups(B, (long long)per_utt, kPositionBudget,
+                  [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, lens + i, B, emb + i * E, stream); });
   if (rc) return rc;
   h->last_launches = (int)(g_launches - before);
   return XVB_OK;

@@ -209,7 +209,8 @@ class CamPPXvector(TopVirtualNnet):
         extract_embedding(): each chunk position of chunk_sizes(T) runs as one batch, and the chunk embeddings are
         combined as sum_i size_i * emb_i / T in chunk order."""
         if lengths is not None:
-            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector blueprints only"
+            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN and ResNet x-vector "
+                                      "blueprints only"
                                       .format(type(self).__name__))
         with torch.no_grad():
             x = torch.as_tensor(feats)

@@ -16,7 +16,9 @@ the first segment layer, made once when the weights are handed over.
 
 The launch sequence runs in the native handle (NativeResNetExtractor over xvb_resnet_*, csrc/resnet_extractor.cu), which
 also writes XVBR0001 model files for bin/xvb-extract.  XVB_RESNET_NATIVE=0 selects ResNetExtractor, the Python driver of
-the same kernels in the same order, whose embeddings are bit-identical."""
+the same kernels in the same order, whose embeddings are bit-identical.  Both take a masked batch of utterances of
+different lengths (extract(feats, lengths)): every position tensor then holds exact zeros past each utterance's length at
+its own time resolution, which is what the next conv's taps must read."""
 import copy
 import os
 import sys
@@ -28,7 +30,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
-from asv_subtools_b200.native import ShardExtractor  # noqa: E402
+from asv_subtools_b200.native import ShardExtractor, host_lengths  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
@@ -264,6 +266,8 @@ class ResNetExtractor:
     like AttentionPoolingExtractor: per block two convs (+ a 1x1 stride-2 downsample in the first block of layers 2-4)
     [+ plane mean, two small affines and the SE scaling], then statistics pooling and the segment layers."""
 
+    TAKES_LENGTHS = True
+
     def __init__(self, m, device):
         def bn(b):
             s, t = fold_batchnorm(b)
@@ -290,47 +294,64 @@ class ResNetExtractor:
         self.eps = m.stats.eps
         self.embed_dim = self.segment[-1].cout_real
 
-    def _se_gate(self, z, se):
+    def _se_gate(self, z, se, lengths=None):
         """sigmoid(fc_2(relu(fc_1(mean over positions of z)))).  xvb_plane_mean puts one thread on 8 channels and spreads
         the positions over 8 warps, so a 32-channel layer would keep 4 lanes of a warp busy: the (B, P, C) planes are
         read as (B, P/k, k*C) instead, k consecutive positions side by side, and fc_1's copies of its weight (w1k) sum the
-        k group means."""
-        b, c = z.hi.shape[0], z.channels
+        k group means.  A masked batch (lengths: frames per utterance) takes k from F alone, so that k divides every
+        utterance's own L * F positions, and averages each utterance's own rows."""
+        b, _, f, c = z.hi.shape
         w1k, b1, w2, b2 = se
         p = z.hi.numel() // (b * c)
         k = 1
-        while 2 * k in w1k and p % (2 * k) == 0:
+        while 2 * k in w1k and (p if lengths is None else f) % (2 * k) == 0:
             k *= 2
         zmean, _ = ops.plane_mean(ops.SplitPlanes(z.hi.view(b, p // k, k * c), z.lo.view(b, p // k, k * c), k * c),
-                                  planes=False)
+                                  planes=False, lengths=lengths, rows_per_length=f // k)
         return ops.small_affine(ops.small_affine(zmean, w1k[k], b1, relu=True), w2, b2, sigmoid=True)
 
-    def extract(self, feats):
-        """feats (B, T, F) fp32 CUDA -> (B, embd_dim) fp32 CUDA, asynchronous on the current stream."""
+    def extract(self, feats, lengths=None):
+        """feats (B, T, F) fp32 CUDA -> (B, embd_dim) fp32 CUDA, asynchronous on the current stream.  lengths (B,) host
+        ints, 1 <= lengths[b] <= T: a masked batch as xvb_resnet_extract_lengths runs it (every length equal to T: the
+        unmasked sequence)."""
         if feats.shape[2] != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
         feats = feats.contiguous()
         B, T, F = feats.shape
         dev, P = feats.device, ops.SplitPlanes
+        levels = None    # (4, B) int32: the lengths after 0..3 stride-2 stages, ceil(L / 2) each
+        if lengths is not None:
+            lens = host_lengths(lengths, B)
+            bad = np.flatnonzero((lens < 1) | (lens > T))
+            if bad.size:
+                raise ValueError("lengths[{}]={} outside [1, T={}]".format(bad[0], lens[bad[0]], T))
+            if (lens != T).any():
+                table = [lens]
+                for _ in range(3):
+                    table.append((table[-1] - 1) // 2 + 1)
+                levels = torch.from_numpy(np.stack(table)).to(dev)
+        at = lambda lv: None if levels is None else levels[lv]  # noqa: E731
+        level = 0
         c0 = self.head_w.shape[0]
         x = P.empty((B, T, F, c0), dev)
         a = P.empty((B, T, F, c0), dev) if self.pre else None   # relu(bn1(x)) of the first pre-activation block
         s2, t2 = self.blocks[0]["bn1"] if self.pre else (None, None)
-        ops.conv2d_head(feats, self.head_w, self.head_bn[0], self.head_bn[1], x, s2, t2, a)
+        ops.conv2d_head(feats, self.head_w, self.head_bn[0], self.head_bn[1], x, s2, t2, a, lengths=at(0))
         out = None
         for i, blk in enumerate(self.blocks):
             last = i + 1 == len(self.blocks)
             st, co = blk["stride"], blk["cout"]
             T, F = (T - 1) // st + 1, (F - 1) // st + 1
+            lin, lout = at(level), at(level + 1 if st == 2 else level)
             h = P.empty((B, T, F, co), dev)
             if self.pre:     # h = relu(bn2(conv1(relu(bn1(x)))))  (resnet.py:87-98)
-                ops.conv2d(a, blk["conv1"], co, 3, st, *blk["bn2"], relu=True, y=h)
+                ops.conv2d(a, blk["conv1"], co, 3, st, *blk["bn2"], relu=True, y=h, lengths=lin)
             else:            # h = relu(bn1(conv1(x)))  (resnet.py:70-75)
-                ops.conv2d(x, blk["conv1"], co, 3, st, *blk["bn1"], relu=True, y=h)
+                ops.conv2d(x, blk["conv1"], co, 3, st, *blk["bn1"], relu=True, y=h, lengths=lin)
             ident = x
             if blk["ds"] is not None:   # downsample = conv1x1 (stride) + BN of the un-activated block input
                 ident = P.empty((B, T, F, co), dev)
-                ops.conv2d(x, blk["ds"][0], co, 1, st, *blk["ds"][1], y=ident)
+                ops.conv2d(x, blk["ds"][0], co, 1, st, *blk["ds"][1], y=ident, lengths=lin)
             nxt = None if last or not self.pre else self.blocks[i + 1]["bn1"]
             y = None if last else P.empty((B, T, F, co), dev)
             yf = torch.empty(B, T, F, co, dtype=torch.float32, device=dev) if last else None
@@ -339,14 +360,15 @@ class ResNetExtractor:
             bn2 = (None, None) if self.pre else blk["bn2"]
             if blk["se"] is None:       # conv2 [+ bn2] + identity [-> relu] in one epilogue
                 ops.conv2d(h, blk["conv2"], co, 3, 1, *bn2, res=ident, relu=not self.pre, y=y, y_f32=yf,
-                           scale2=s2, shift2=t2, y2=a)
+                           scale2=s2, shift2=t2, y2=a, lengths=lout)
             else:
                 z = P.empty((B, T, F, co), dev)
-                ops.conv2d(h, blk["conv2"], co, 3, 1, *bn2, y=z)
-                gate = self._se_gate(z, blk["se"])
-                ops.se_residual(z, gate, ident, relu=not self.pre, y=y, y_f32=yf, scale2=s2, shift2=t2, y2=a)
+                ops.conv2d(h, blk["conv2"], co, 3, 1, *bn2, y=z, lengths=lout)
+                gate = self._se_gate(z, blk["se"], lout)
+                ops.se_residual(z, gate, ident, relu=not self.pre, y=y, y_f32=yf, scale2=s2, shift2=t2, y2=a, lengths=lout)
             x, out = y, yf
-        _, xp = ops.stats_pool_ex(out.view(B, T, F * out.shape[-1]), self.eps, 0, planes=True)
+            level += st == 2
+        _, xp = ops.stats_pool_ex(out.view(B, T, F * out.shape[-1]), self.eps, 0, planes=True, lengths=at(level))
         for i, layer in enumerate(self.segment):
             if i + 1 == len(self.segment):
                 emb = torch.empty(B, 1, layer.cout, dtype=torch.float32, device=dev)
@@ -366,6 +388,7 @@ class NativeResNetExtractor(ShardExtractor):
     device that is current when it is built (or loaded from an XVBR0001 file)."""
 
     PREFIX = "resnet"
+    TAKES_LENGTHS = True
 
     def _create_args(self, m):
         from asv_subtools_b200._lib import int_array

@@ -337,7 +337,8 @@ class TransformerXvector(TopVirtualNnet):
         extract_embedding(): the B * (num_split - 1) full chunks run as one batch, the B last chunks as another, and the
         chunk embeddings are recombined with the reference's length-weighted average."""
         if lengths is not None:
-            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector blueprints only"
+            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN and ResNet x-vector "
+                                      "blueprints only"
                                       .format(type(self).__name__))
         with torch.no_grad():
             x = torch.as_tensor(feats)

@@ -17,6 +17,17 @@ def _cuda_f32(feats, feat_dim):
     return feats
 
 
+def host_lengths(lengths, b):
+    """The lengths argument of a masked extract call ((B,) sequence, ndarray or tensor) as a contiguous host int32 array
+    of B entries; out-of-range values stay out of range (clipped to int32) for the library's check to name them."""
+    if isinstance(lengths, torch.Tensor):
+        lengths = lengths.cpu().numpy()
+    lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
+    if lens.shape[0] != b:
+        raise ValueError("lengths has {} entries for a batch of {}".format(lens.shape[0], b))
+    return np.clip(lens, -2 ** 31, 2 ** 31 - 1).astype(np.int32)
+
+
 class NativeExtractor:
     """xvb_<PREFIX>_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
     current when it is built from a model `m` (or loaded from a model file at `path`).
@@ -24,9 +35,13 @@ class NativeExtractor:
     A family sets PREFIX and supplies `_create_args(m)`, the arguments of xvb_<PREFIX>_create after the handle,
     `_configure(m)`, any call between create and the first set_layer, and `_layers(m)`, which yields
     (name, shape, (w, b, scale, shift), flags) per record, `shape` being the set_layer arguments between the name and
-    the arrays."""
+    the arrays.
+
+    TAKES_LENGTHS: the handle has xvb_<PREFIX>_extract_lengths, and extract() takes `lengths` (a masked batch of
+    utterances of different lengths).  extract_embedding_batch and the --mixed-lengths CLIs ask this of any extractor."""
 
     PREFIX = None
+    TAKES_LENGTHS = False
 
     def __init__(self, m=None, device=None, path=None):
         from asv_subtools_b200._lib import check, lib
@@ -73,13 +88,21 @@ class NativeExtractor:
     def _input(self, feats):
         return _cuda_f32(feats, self.feat_dim)
 
-    def extract(self, feats):
+    def extract(self, feats, lengths=None):
         """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embed_dim) fp32 CUDA, asynchronous on the current
-        stream."""
+        stream.  lengths (B,) host ints, 1 <= lengths[b] <= T (TAKES_LENGTHS families): a batch of utterances of
+        different lengths, row b being feats[b, :lengths[b]] extracted alone; the frames past them are never read."""
         feats = self._input(feats)
         B, T, _ = feats.shape
         emb = torch.empty(B, self.embed_dim, dtype=torch.float32, device=feats.device)
-        self._call("extract", self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()), self._stream())
+        if lengths is None:
+            self._call("extract", self._h, C.c_void_p(feats.data_ptr()), B, T, C.c_void_p(emb.data_ptr()), self._stream())
+            return emb
+        if not self.TAKES_LENGTHS:
+            raise NotImplementedError("{}: extract(lengths=...) is not supported by this family".format(type(self).__name__))
+        lens = host_lengths(lengths, B)
+        self._call("extract_lengths", self._h, C.c_void_p(feats.data_ptr()), lens.ctypes.data_as(C.c_void_p), B, T,
+                   C.c_void_p(emb.data_ptr()), self._stream())
         return emb
 
     def close(self):

@@ -153,8 +153,8 @@ class TopVirtualNnet(torch.nn.Module):
         """Equal-length utterances in one call: feats (B, T, F) float32 (CUDA tensor, CPU tensor or
         ndarray; T <= maxChunk) -> (B, D) CUDA tensor.  Same arithmetic as B calls of
         extract_embedding().  lengths (B,) host ints, 1 <= lengths[b] <= T: utterances of different lengths padded to
-        T, row b being the embedding of feats[b, :lengths[b]] (what is past it is ignored); TDNN x-vector blueprints
-        (build_tdnn_extractor with statistics pooling) only."""
+        T, row b being the embedding of feats[b, :lengths[b]] (what is past it is ignored); models whose extractor
+        declares TAKES_LENGTHS (the TDNN x-vector with statistics pooling, the ResNet x-vector) only."""
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:
@@ -164,12 +164,11 @@ class TopVirtualNnet(torch.nn.Module):
             x = x.to(self.device_for_extraction(), non_blocking=True).contiguous()
             if lengths is None:
                 return self.extractor().extract(x)
-            from .. import ops
             ex = self.extractor()
-            if not isinstance(ex, ops.Extractor):
-                raise NotImplementedError("{}: extract_embedding_batch(lengths=...) needs the TDNN x-vector extractor with "
-                                          "statistics pooling; this model runs on {}".format(type(self).__name__,
-                                                                                              type(ex).__name__))
+            if not getattr(ex, "TAKES_LENGTHS", False):
+                raise NotImplementedError("{}: extract_embedding_batch(lengths=...) needs an extractor that takes lengths (the "
+                                          "TDNN x-vector with statistics pooling or the ResNet x-vector); this model runs on "
+                                          "{}".format(type(self).__name__, type(ex).__name__))
             return ex.extract(x, lengths)
 
 

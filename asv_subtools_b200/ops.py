@@ -7,7 +7,7 @@ import torch
 
 from . import _lib
 from ._lib import BN, RELU, SIGMOID, SWISH, TANH, TdnnArgs, check, int_array, lib  # noqa: F401
-from .native import ShardExtractor
+from .native import ShardExtractor, host_lengths
 
 
 def _stream():
@@ -167,14 +167,19 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
     check(lib.xvb_tdnn_affine_ex(C.byref(a), _stream()), "xvb_tdnn_affine_ex")
 
 
-def plane_mean(x, planes=True):
-    """Mean over T of SplitPlanes (B,T,C) -> (fp32 (B,C), SplitPlanes (B,1,C) | None)."""
+def plane_mean(x, planes=True, lengths=None, rows_per_length=1):
+    """Mean over T of SplitPlanes (B,T,C) -> (fp32 (B,C), SplitPlanes (B,1,C) | None).  lengths: int32 CUDA (B,) tensor
+    of a masked batch: utterance b averages its first lengths[b] * rows_per_length rows (xvb_plane_mean_lengths)."""
     b, t, c = x.hi.shape[0], x.hi.shape[1], x.channels
     out = torch.empty(b, c, dtype=torch.float32, device=x.hi.device)
     op = SplitPlanes.empty((b, 1, c), x.hi.device) if planes else None
-    check(lib.xvb_plane_mean(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, b, t, c, _ptr(out),
-                             op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, c, _stream()),
-          "xvb_plane_mean")
+    tail = (_ptr(out), op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, c, _stream())
+    if lengths is None:
+        check(lib.xvb_plane_mean(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, b, t, c, *tail), "xvb_plane_mean")
+    else:
+        check(lib.xvb_plane_mean_lengths(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, b, t, c,
+                                         _ptr(_req(lengths, torch.int32, "lengths")), int(rows_per_length), *tail),
+              "xvb_plane_mean_lengths")
     return out, op
 
 
@@ -267,13 +272,14 @@ def pack_conv2d_weight(weight, taps=None):
 
 
 def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=False, y=None, y_f32=None,
-           scale2=None, shift2=None, y2=None, taps=None, valid=False, stride_t=0):
+           scale2=None, shift2=None, y2=None, taps=None, valid=False, stride_t=0, lengths=None):
     """One 2-D convolution (xvb_conv2d): x SplitPlanes (B, T, F, Cin); w from pack_conv2d_weight; res / y / y2
     SplitPlanes (B, T', F', cout), y_f32 fp32 of the same shape, with T' = ceil(T / stride), F' = ceil(F / stride).
     stride_t: the time axis's own stride (0: `stride`; CAM++'s FCM head uses stride=2, stride_t=1).
     taps: only these taps (kf*ksize + kt, strictly increasing, ksize 1, 3 or 5) are computed, with w packed by
     pack_conv2d_weight(weight, taps) (xvb_conv2d_taps).  valid: no padding, T' = (T - k) // stride + 1 and F' likewise
-    (xvb_conv2d_valid; dense taps only)."""
+    (xvb_conv2d_valid; dense taps only).  lengths: int32 CUDA (B,) tensor of a masked batch, the input length of each
+    utterance (xvb_conv2d_args_t.lengths): the outputs past each utterance's own output length store zeros."""
     b, t, f, cin = x.hi.shape
     a = _lib.Conv2dArgs()
     a.x_hi, a.x_lo = _planes_ptrs(x)
@@ -288,6 +294,8 @@ def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=F
     a.y2_hi, a.y2_lo = _planes_ptrs(y2)
     if y_f32 is not None:
         a.y_f32 = _req(y_f32, torch.float32, "y_f32").data_ptr()
+    if lengths is not None:
+        a.lengths = _req(lengths, torch.int32, "lengths").data_ptr()
     if valid:
         if taps is not None:
             raise ValueError("conv2d(valid=True) takes the dense window only")
@@ -298,27 +306,42 @@ def conv2d(x, w, cout, ksize, stride=1, scale=None, shift=None, res=None, relu=F
         check(lib.xvb_conv2d_taps(C.byref(a), int_array(taps), len(taps), _stream()), "xvb_conv2d_taps")
 
 
-def conv2d_head(feats, weight, scale, shift, y, scale2=None, shift2=None, y2=None):
+def conv2d_head(feats, weight, scale, shift, y, scale2=None, shift2=None, y2=None, lengths=None):
     """Head conv (xvb_conv2d_head_k): feats (B, T, F) fp32, weight (Cout, 1, k, k) fp32 with k = 3 or 5 -> y =
-    relu(bn(conv)) SplitPlanes (B, T, F, Cout) [, y2 = relu(y * scale2 + shift2)]."""
+    relu(bn(conv)) SplitPlanes (B, T, F, Cout) [, y2 = relu(y * scale2 + shift2)].  lengths: int32 CUDA (B,) tensor of a
+    masked batch (k = 3, xvb_conv2d_head_lengths): the frames t >= lengths[b] read as zeros and store zeros."""
     feats = _req(feats, torch.float32, "feats")
     weight = _req(weight, torch.float32, "weight")
     b, t, f = feats.shape
     k = weight.shape[-1]
     y2h, y2l = _planes_ptrs(y2)
     args = (_ptr(scale), _ptr(shift), y.hi.data_ptr(), y.lo.data_ptr(), _ptr(scale2), _ptr(shift2), y2h, y2l, _stream())
-    if k == 3:
+    if lengths is not None:
+        if k != 3:
+            raise ValueError("conv2d_head(lengths=...) takes the 3x3 head only, got k={}".format(k))
+        check(lib.xvb_conv2d_head_lengths(_ptr(feats), b, t, f, _ptr(_req(lengths, torch.int32, "lengths")), _ptr(weight),
+                                          weight.shape[0], *args), "xvb_conv2d_head_lengths")
+    elif k == 3:
         check(lib.xvb_conv2d_head(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], *args), "xvb_conv2d_head")
     else:
         check(lib.xvb_conv2d_head_k(_ptr(feats), b, t, f, _ptr(weight), weight.shape[0], k, *args), "xvb_conv2d_head_k")
 
 
-def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, shift2=None, y2=None):
-    """y = [relu](z * gate[b] + identity) over SplitPlanes (B, ..., C) (xvb_se_residual); gate (B, C) fp32."""
+def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, shift2=None, y2=None, lengths=None):
+    """y = [relu](z * gate[b] + identity) over SplitPlanes (B, ..., C) (xvb_se_residual); gate (B, C) fp32.  lengths:
+    int32 CUDA (B,) tensor of a masked batch of (B, T, F, C) planes (xvb_se_residual_lengths): the positions of frames
+    t >= lengths[b] store zeros."""
     b, c = z.hi.shape[0], z.hi.shape[-1]
     gate = _req(gate, torch.float32, "gate")
     yh, yl = _planes_ptrs(y)
     y2h, y2l = _planes_ptrs(y2)
+    if lengths is not None:
+        _, t, f, _ = z.hi.shape
+        check(lib.xvb_se_residual_lengths(z.hi.data_ptr(), z.lo.data_ptr(), _ptr(gate), identity.hi.data_ptr(),
+                                          identity.lo.data_ptr(), b, t, f, c, _ptr(_req(lengths, torch.int32, "lengths")),
+                                          1 if relu else 0, yh, yl, _ptr(y_f32), _ptr(scale2), _ptr(shift2), y2h, y2l,
+                                          _stream()), "xvb_se_residual_lengths")
+        return
     check(lib.xvb_se_residual(z.hi.data_ptr(), z.lo.data_ptr(), _ptr(gate), identity.hi.data_ptr(), identity.lo.data_ptr(), b,
                               z.hi.numel() // (b * c), c, 1 if relu else 0, yh, yl, _ptr(y_f32), _ptr(scale2), _ptr(shift2),
                               y2h, y2l, _stream()), "xvb_se_residual")
@@ -750,6 +773,8 @@ class Extractor(ShardExtractor):
     """Owner of a native xvb_extractor_t (packed weights + workspace on the current device), built layer by layer with
     add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file."""
 
+    TAKES_LENGTHS = True
+
     PREFIX = "extractor"
     batch = 256
 
@@ -839,12 +864,7 @@ class Extractor(ShardExtractor):
         if lengths is None:
             check(lib.xvb_extractor_extract(self._h, _ptr(feats), b, t, _ptr(emb), _stream()), "xvb_extractor_extract")
             return emb
-        if isinstance(lengths, torch.Tensor):
-            lengths = lengths.cpu().numpy()
-        lens = np.ascontiguousarray(np.asarray(lengths, dtype=np.int64).reshape(-1))
-        if lens.shape[0] != b:
-            raise ValueError("lengths has {} entries for a batch of {}".format(lens.shape[0], b))
-        lens = np.clip(lens, -2 ** 31, 2 ** 31 - 1).astype(np.int32)    # out-of-range values stay out of range for the C check
+        lens = host_lengths(lengths, b)
         check(lib.xvb_extractor_extract_lengths(self._h, _ptr(feats), lens.ctypes.data_as(C.c_void_p), b, t, _ptr(emb),
                                                 _stream()), "xvb_extractor_extract_lengths")
         return emb

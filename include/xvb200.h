@@ -190,6 +190,11 @@ int xvb_stats_pool_lengths(const float* x, int64_t ldx, int B, int T, int C, flo
  * AdaptiveAvgPool1d(1) of SE_Connect (:100).  C % 8 == 0. */
 int xvb_plane_mean(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C, float* out,
                    uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
+/* xvb_plane_mean over a masked batch: utterance b averages its first lengths[b] * rows_per_length rows (DEVICE
+ * int32[B], 1 <= lengths[b] * rows_per_length <= T); the rows past them are never read.  A (B, T, F, C) position tensor
+ * read as (B, T * F / k, k * C) rows takes rows_per_length = F / k (k dividing F). */
+int xvb_plane_mean_lengths(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, int B, int T, int C, const int* lengths,
+                           int rows_per_length, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
 
 /* Res2NetBlock.forward (pytorch/model/ecapa_tdnn_xvector.py:61-75) as ONE persistent kernel: chunk 0
  * of x passes through; step i = TDNN 128->128, context [-d,0,d], ReLU, BN on (x chunk i+1 [+ y chunk i]),
@@ -291,6 +296,12 @@ typedef struct xvb_conv2d_args {
    * feature-axis stride alone.  CAM++'s FCM head (subtools2/egrecho/models/campplus/campplus.py:60-80, :104-106) uses
    * stride (2, 1): feature 2, time 1, so T' = T and F' = ceil(F / 2). */
   int stride_t;
+  /* NULL, or a DEVICE int32[B] with 1 <= lengths[b] <= T: a masked batch of utterances of different lengths, utterance b
+   * owning input frames [0, lengths[b]).  Its output length follows the conv's own rule, L' = (L + 2 pad - k) / s_t + 1
+   * (ceil(L / s_t) with pad = k / 2), and the epilogue stores exact zeros in y, y_f32 and y2 at every output frame
+   * t >= L', so the next conv's taps read the utterance's own zero padding.  The x planes must already hold zeros at
+   * the input frames t >= L.  Tiles are computed in full; only the stores differ.  Not with xvb_conv2d_valid. */
+  const int* lengths;
 } xvb_conv2d_args_t;
 int xvb_conv2d(const xvb_conv2d_args_t* args, void* stream);
 
@@ -309,6 +320,11 @@ int xvb_conv2d_taps(const xvb_conv2d_args_t* args, const int* taps, int ntaps, v
 int xvb_conv2d_head(const float* x, int B, int T, int F, const float* w, int Cout, const float* bn_scale,
                     const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo, const float* scale2, const float* shift2,
                     uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+/* xvb_conv2d_head over a masked batch (lengths: DEVICE int32[B], 1 <= lengths[b] <= T): the feature frames
+ * t >= lengths[b] are read as zeros (never loaded), and y and y2 hold exact zeros there. */
+int xvb_conv2d_head_lengths(const float* x, int B, int T, int F, const int* lengths, const float* w, int Cout,
+                            const float* bn_scale, const float* bn_shift, uint16_t* y_hi, uint16_t* y_lo,
+                            const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
 
 /* xvb_conv2d_head with a KxK window, ksize in {3, 5}, padding ksize/2: w is (Cout, 1, k, k) fp32.  ksize 3 is
  * xvb_conv2d_head.  A RepVGG / RepSPK stage0 block (Cin = 1) folds into this with bn_scale = 1 and bn_shift = its
@@ -392,6 +408,12 @@ int xvb_conv_module(const float* x, int64_t ldx, int B, int T, int C, const floa
 int xvb_se_residual(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
                     const uint16_t* id_lo, int B, int64_t P, int C, int relu, uint16_t* y_hi, uint16_t* y_lo, float* y_f32,
                     const float* scale2, const float* shift2, uint16_t* y2_hi, uint16_t* y2_lo, void* stream);
+/* xvb_se_residual over a masked batch of (B, T, F, C) planes (P = T * F): y, y_f32 and y2 hold exact zeros at the
+ * positions of frames t >= lengths[b] (DEVICE int32[B], 1 <= lengths[b] <= T), whose z and identity are not read. */
+int xvb_se_residual_lengths(const uint16_t* z_hi, const uint16_t* z_lo, const float* gate, const uint16_t* id_hi,
+                            const uint16_t* id_lo, int B, int T, int F, int C, const int* lengths, int relu, uint16_t* y_hi,
+                            uint16_t* y_lo, float* y_f32, const float* scale2, const float* shift2, uint16_t* y2_hi,
+                            uint16_t* y2_lo, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * CAM++ x-vector (subtools2/egrecho/models/campplus/campplus.py): the pieces of the densely connected D-TDNN layers that
@@ -778,6 +800,17 @@ int xvb_resnet_embed_dim(const xvb_resnet_t* h);
 int xvb_resnet_last_launches(const xvb_resnet_t* h);
 /* feats (B, T, feat_dim) fp32 on the device -> emb (B, embed_dim) fp32 on the device; asynchronous. */
 int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* A batch of utterances of different lengths: feats (B, T, feat_dim) fp32 on the device, utterance b in its first
+ * lengths_host[b] frames (HOST int32[B], 1 <= lengths_host[b] <= T; the frames past them are never read, whatever they
+ * hold).  Row b of emb is the embedding of feats[b, :lengths_host[b]] extracted alone, up to the rounding of the
+ * pooling merge order and of the SE mean's position grouping (chosen from F' alone in a masked batch).  Every conv,
+ * SE scaling and the head conv store zeros past each utterance's length at their resolution (ceil(L / 2) per
+ * stride-2 stage), and each utterance pools its own frames.  The lengths are checked (XVB_EINVAL naming the first bad
+ * one) and copied, with the per-stage lengths, into the workspace on `stream`; the host array may be reused when the
+ * call returns.  The position budget splits the call into groups as xvb_resnet_extract does.  With every length equal
+ * to T the result equals xvb_resnet_extract bit for bit. */
+int xvb_resnet_extract_lengths(xvb_resnet_t* h, const float* feats, const int32_t* lengths_host, int B, int T, float* emb,
+                               void* stream);
 /* Same through host buffers (H2D of feats, D2H of emb inside; synchronises the stream). */
 int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream);
 /* Whole shard of N equal-length utterances in `batch`-utterance batches: the protocol of

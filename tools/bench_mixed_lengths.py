@@ -1,16 +1,20 @@
 #!/usr/bin/env python
-"""Throughput of the TDNN x-vector handle on a corpus of utterances of different lengths -- a side measurement, not the
-bench.py line.
+"""Throughput of the TDNN or ResNet x-vector handle on a corpus of utterances of different lengths -- a side
+measurement, not the bench.py line.
 
-    python tools/bench_mixed_lengths.py [rounds] [--utts N] [--min-frames A] [--max-frames B] [--batch N] [--dim F]
+    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet] [--utts N] [--min-frames A] [--max-frames B]
+                                        [--batch N] [--dim F]
 
 The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
-numpy.random.RandomState(2026), run through one Xvector(F, far) handle (default F = 23) under two batch policies:
+numpy.random.RandomState(2026), run through one handle under two batch policies.  --model xvector (the default): an
+Xvector(F, far) handle (default F = 23, batch 256).  --model resnet: the online launcher's SE ResNet34 of
+tools/bench_resnet.py (post-activation blocks with SE, fc1=False, position near) on 80-d features (--dim is ignored),
+batch 128 by default, as bench_resnet.py times it.
 
   * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
-    up to `batch` utterances of exactly the same frame count, one xvb_extractor_extract call each;
+    up to `batch` utterances of exactly the same frame count, one xvb_<handle>_extract call each;
   * masked: --mixed-lengths' rule (plan_mixed_batches: ascending length, up to `batch` per batch, padding at most 1/8),
-    one xvb_extractor_extract_lengths call each.
+    one xvb_<handle>_extract_lengths call each.
 
 Features come from one resident random buffer (no host copies in the timed region).  Each round times the whole corpus
 under each policy with CUDA events, the policies alternating; every launch plan is built in an untimed warm-up pass
@@ -33,6 +37,9 @@ from asv_subtools_b200.model.xvector import Xvector  # noqa: E402
 from asv_subtools_b200.pipeline.extract_embeddings import plan_mixed_batches  # noqa: E402
 from oracle import nnet as onn  # noqa: E402
 
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import resnet_oracle as ro  # noqa: E402
+
 
 def equal_length_batches(lengths, batch):
     """Exact-length buckets in batches of up to `batch` (the default mode of both CLIs)."""
@@ -48,17 +55,28 @@ def main():
     ap.add_argument("--utts", type=int, default=4000)
     ap.add_argument("--min-frames", type=int, default=200)
     ap.add_argument("--max-frames", type=int, default=2000)
-    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--batch", type=int, default=None, help="default 256 (xvector) or 128 (resnet)")
     ap.add_argument("--dim", type=int, default=23)
+    ap.add_argument("--model", choices=["xvector", "resnet"], default="xvector")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_mixed_lengths.py needs a GPU")
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
                           str(torch.cuda.current_device())], capture_output=True, text=True).stdout.strip()
-    F = args.dim
     lengths = [int(v) for v in np.random.RandomState(2026).randint(args.min_frames, args.max_frames + 1, args.utts)]
-    m = Xvector(F, 10, training=False, extracted_embedding="far")
-    m.load_state_dict(onn.make_state_dict(onn.xvector_spec(F), 7), strict=True)
+    if args.model == "resnet":
+        from asv_subtools_b200.model.resnet_xvector import ResNetXvector
+        F = 80
+        args.batch = args.batch or 128
+        m = ResNetXvector(F, 10, training=False, extracted_embedding="near", **ro.ONLINE)
+        m.load_state_dict(onn.make_state_dict(ro.resnet_spec(F, ro.ONLINE), 301), strict=True)
+        workload = "online SE ResNet34 (80-d, near)"
+    else:
+        F = args.dim
+        args.batch = args.batch or 256
+        m = Xvector(F, 10, training=False, extracted_embedding="far")
+        m.load_state_dict(onn.make_state_dict(onn.xvector_spec(F), 7), strict=True)
+        workload = "Xvector({}) far".format(F)
     m.cuda().eval()
     ex = m.extractor()
     base = torch.randn(args.batch * args.max_frames * F, device="cuda")
@@ -91,8 +109,8 @@ def main():
                 stop.record()
                 stop.synchronize()
                 p["fps"].append(sum(lengths) / (start.elapsed_time(stop) / 1e3))
-    out = {"workload": "Xvector({}) far, {} utterances uniform over {}..{} frames (RandomState(2026)), batch {}".format(
-               F, args.utts, args.min_frames, args.max_frames, args.batch),
+    out = {"workload": "{}, {} utterances uniform over {}..{} frames (RandomState(2026)), batch {}".format(
+               workload, args.utts, args.min_frames, args.max_frames, args.batch),
            "frames": sum(lengths), "card": smi, "rounds": args.rounds}
     for name, p in policies.items():
         out[name] = {"frames_per_s": statistics.median(p["fps"]), "frames_per_s_min": min(p["fps"]),
