@@ -81,14 +81,11 @@ int res_freq(int F, int j) {
 
 }  // namespace
 
-struct xvb_campp {
-  Model* m = nullptr;
-  bool finalized = false;
+struct xvb_campp : Handle<Model> {
   enum { kX0, kA0, kO0 = kA0 + kResBlocks, kS0 = kO0 + kResBlocks, kC2 = kS0 + kResBlocks, kPad, kBuf0, kPre = kBuf0 + kBlocks,
          kH, kZ, kPool, kGate, kStats, kBufs };
   Workspace<kBufs> ws;
   int pad_B = -1, pad_T = -1;          // the (B, T) layout whose pad frames are zero
-  int last_launches = 0;
 };
 
 namespace {
@@ -96,7 +93,7 @@ namespace {
 using H = xvb_campp;
 
 int reserve(H* h, int B, int T) {
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const size_t b = (size_t)B, t = (size_t)T, t2 = (size_t)(T + 1) / 2, row = (size_t)m->f8 * kM;
   const size_t nseg = (t2 + kSegLen - 1) / kSegLen;
   size_t need[H::kBufs] = {0};
@@ -160,7 +157,7 @@ int conv(const Conv& c, Planes x, int B, int T, int F, int ksize, int stride, in
 int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const xvb_campp_config_t& c = m->cfg;
   const int g = c.growth_rate, T2 = (T + 1) / 2, row = m->f8 * kM;
   const long long rows = (long long)B * T2;
@@ -277,27 +274,24 @@ extern "C" int xvb_campp_create(xvb_campp_t** out, const xvb_campp_config_t* cfg
     ch /= 2;
   }
   xvb_campp* h = new xvb_campp();
-  h->m = new Model();
-  h->m->cfg = c;
+  h->draft->cfg = c;
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_campp_set_layer(xvb_campp_t* h, const char* name, int rows, int cols, const float* w_host,
                                    const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
-  XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127,
+  XVB_CHECK_ARG(is_draft(h) && name && strlen(name) > 0 && strlen(name) < 127,
                 "xvb_campp_set_layer: bad arguments or finalized model");
   const char* fn = "xvb_campp_set_layer";
   const int shape[2] = {rows, cols};
-  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  int rc = h->draft->recs.check(fn, name, shape, w_host, scale_host, shift_host);
   if (rc) return rc;
   XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN)) == 0, "xvb_campp_set_layer(%s): flags %d", name, flags);
-  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
+  return h->draft->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
-extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
-  XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_campp_finalize: null or finalized model");
-  Model* m = h->m;
+static int build(Model* m, RecordStore& recs) {
   const xvb_campp_config_t& c = m->cfg;
   const int g = c.growth_rate;
   m->f8 = c.feat_dim / 8;
@@ -305,7 +299,7 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
   // a record with its shape, whether it carries a bias and scale / shift, and its flags
   auto need = [&](const std::string& n, int rows, int cols, bool bias, bool bn, int flags, const Rec** out) -> int {
     const int shape[2] = {rows, cols};
-    int rc = m->recs.take("xvb_campp_finalize", n, shape, out);
+    int rc = recs.take("xvb_campp_finalize", n, shape, out);
     if (rc) return rc;
     const Rec* r = *out;
     XVB_CHECK_ARG(r->b.empty() != bias && r->s.empty() != bn && r->flags == flags,
@@ -400,17 +394,17 @@ extern "C" int xvb_campp_finalize(xvb_campp_t* h) {
   if ((rc = need("xvector.dense.linear", c.embd_dim, 2 * ch, false, true, XVB_BN, &r)) || (rc = m->dev.upload(&m->dense_w, r->w)) ||
       (rc = m->dev.upload(&m->dense_s, r->s)) || (rc = m->dev.upload(&m->dense_t, r->t)))
     return rc;
-  if ((rc = m->recs.check_all_used("xvb_campp_finalize"))) return rc;
-  h->finalized = true;
-  return XVB_OK;
+  return recs.check_all_used("xvb_campp_finalize");
 }
 
-extern "C" int xvb_campp_feat_dim(const xvb_campp_t* h) { return h && h->m ? h->m->cfg.feat_dim : XVB_EINVAL; }
-extern "C" int xvb_campp_embed_dim(const xvb_campp_t* h) { return h && h->m ? h->m->cfg.embd_dim : XVB_EINVAL; }
+extern "C" int xvb_campp_finalize(xvb_campp_t* h) { return publish_built(h, build, "xvb_campp_finalize"); }
+
+extern "C" int xvb_campp_feat_dim(const xvb_campp_t* h) { return h ? h->m->cfg.feat_dim : XVB_EINVAL; }
+extern "C" int xvb_campp_embed_dim(const xvb_campp_t* h) { return h ? h->m->cfg.embd_dim : XVB_EINVAL; }
 extern "C" int xvb_campp_last_launches(const xvb_campp_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized, "xvb_campp_extract: model not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_campp_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0, "xvb_campp_extract: bad arguments");
   XVB_CHECK_ARG(T >= kMinFrames, "xvb_campp_extract: CAM++ needs at least %d frames per chunk, got %d", kMinFrames, T);
   const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->cfg.embd_dim;
@@ -440,7 +434,7 @@ extern "C" int xvb_campp_chunk_sizes(int T, int max_chunk, int* sizes, int cap) 
 
 // ---- "XVBP0001" model files: the configuration, then the records as handed over (save_records) ------------------
 extern "C" int xvb_campp_save(const xvb_campp_t* h, const char* path) {
-  XVB_CHECK_ARG(h && h->finalized && path, "xvb_campp_save: model not finalized");
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_campp_save: model not finalized");
   return save_records("xvb_campp_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
@@ -454,8 +448,4 @@ extern "C" int xvb_campp_load(xvb_campp_t** out, const char* path) {
       [](void* h) { return xvb_campp_finalize((xvb_campp_t*)h); }, [](void* h) { xvb_campp_destroy((xvb_campp_t*)h); });
 }
 
-extern "C" void xvb_campp_destroy(xvb_campp_t* h) {
-  if (!h) return;
-  delete h->m;
-  delete h;
-}
+extern "C" void xvb_campp_destroy(xvb_campp_t* h) { delete h; }

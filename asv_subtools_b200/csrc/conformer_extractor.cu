@@ -82,12 +82,9 @@ void sub_shape(const xvb_conformer_config_t& c, int T, int* T1, int* F1, int* T2
 
 }  // namespace
 
-struct xvb_conformer {
-  Model* m = nullptr;
-  bool finalized = false;
+struct xvb_conformer : Handle<Model> {
   enum { kX1, kX2, kR, kH, kHid, kDelta, kQkv, kXo, kXp, kA1, kAp, kLogits, kStats, kZ, kZf, kSegY, kSegP, kBufs };
   Workspace<kBufs> ws;
-  int last_launches = 0;
 };
 
 namespace {
@@ -156,7 +153,7 @@ int layer_norm(const LnCall& c, void* stream) {
 int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb, int* n, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const xvb_conformer_config_t& c = m->cfg;
   const int D = c.D;
   int T1, F1, T2, F2;
@@ -329,33 +326,30 @@ extern "C" int xvb_conformer_create(xvb_conformer_t** out, const xvb_conformer_c
                     (c.position != 0 || c.fc1),
                 "xvb_conformer_create: bad transform_out / pooling / fc1 / position (far needs fc1)");
   xvb_conformer* h = new xvb_conformer();
-  h->m = new Model();
-  h->m->cfg = c;
+  h->draft->cfg = c;
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_conformer_set_layer(xvb_conformer_t* h, const char* name, int rows, int cols, const float* w_host,
                                        const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
-  XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127,
+  XVB_CHECK_ARG(is_draft(h) && name && strlen(name) > 0 && strlen(name) < 127,
                 "xvb_conformer_set_layer: bad arguments or finalized model");
   const char* fn = "xvb_conformer_set_layer";
   const int shape[2] = {rows, cols};
-  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  int rc = h->draft->recs.check(fn, name, shape, w_host, scale_host, shift_host);
   if (rc) return rc;
   XVB_CHECK_ARG(!(flags & XVB_BN) || scale_host, "xvb_conformer_set_layer(%s): XVB_BN without scale/shift", name);
   XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN | XVB_SWISH)) == 0, "xvb_conformer_set_layer(%s): flags %d", name, flags);
-  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
+  return h->draft->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
-extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
-  XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_conformer_finalize: null or finalized model");
-  Model* m = h->m;
+static int build(Model* m, RecordStore& recs) {
   const xvb_conformer_config_t& c = m->cfg;
   const int D = c.D;
   auto need = [&](const std::string& n, int rows, int cols, const Rec** out) -> int {
     const int shape[2] = {rows, cols};
-    return m->recs.take("xvb_conformer_finalize", n, shape, out);
+    return recs.take("xvb_conformer_finalize", n, shape, out);
   };
   // a Linear: weight and bias; the folded BatchNorm / xscale and the activation as flagged
   auto linear = [&](const std::string& n, int cout, int cin, Lin* l) -> int {
@@ -424,7 +418,7 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
     XVB_CHECK_ARG(!r->b.empty(), "xvb_conformer_finalize: record '%sconv_module.depthwise_conv' needs its bias", p.c_str());
     if ((rc = m->dev.upload(&L.dw_w, r->w)) || (rc = m->dev.upload(&L.dw_b, r->b)) != XVB_OK) return rc;
     if ((rc = norm(p + "conv_module.norm", D, true, &L.cm_norm)) != XVB_OK) return rc;
-    XVB_CHECK_ARG(((m->recs.find(p + "conv_module.norm")->flags & XVB_BN) != 0) == (c.cm_norm == 1),
+    XVB_CHECK_ARG(((recs.find(p + "conv_module.norm")->flags & XVB_BN) != 0) == (c.cm_norm == 1),
                   "xvb_conformer_finalize: record '%sconv_module.norm' does not match the configured norm", p.c_str());
     if ((rc = norm(p + "norm_ff", D, false, &L.norm_ff)) || (rc = norm(p + "norm_mha", D, false, &L.norm_mha)) ||
         (rc = norm(p + "norm_ff_macaron", D, false, &L.norm_ff_macaron)) || (rc = norm(p + "norm_conv", D, false, &L.norm_conv)) ||
@@ -459,29 +453,29 @@ extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) {
   }
   for (const Want& w : chain) {
     const std::string a = std::string(w.name) + ".affine", b = std::string(w.name) + ".batchnorm";
-    const Rec* ra = m->recs.find(a);
+    const Rec* ra = recs.find(a);
     XVB_CHECK_ARG(ra, "xvb_conformer_finalize: record '%s' is missing", a.c_str());
     Seg s;
     if ((rc = w.whole ? linear(a, ra->shape[0], cin, &s.lin) : plain(a, ra->shape[0], cin, &s.lin)) != XVB_OK) return rc;
     XVB_CHECK_ARG(s.lin.cout % 8 == 0, "xvb_conformer_finalize: record '%s' has %d rows, need a multiple of 8", a.c_str(), s.lin.cout);
-    s.ln = w.whole && m->recs.find(b) != nullptr;
+    s.ln = w.whole && recs.find(b) != nullptr;
     if (s.ln && (rc = norm(b, s.lin.cout, false, &s.norm))) return rc;
     XVB_CHECK_ARG(!(s.ln && (s.lin.flags & XVB_BN)), "xvb_conformer_finalize: '%s' has both a LayerNorm and a folded BatchNorm", w.name);
     m->seg.push_back(s);
     cin = s.lin.cout;
   }
   m->E = m->seg.back().lin.cout;
-  if ((rc = m->recs.check_all_used("xvb_conformer_finalize"))) return rc;
-  h->finalized = true;
-  return XVB_OK;
+  return recs.check_all_used("xvb_conformer_finalize");
 }
 
-extern "C" int xvb_conformer_feat_dim(const xvb_conformer_t* h) { return h && h->m ? h->m->cfg.feat_dim : XVB_EINVAL; }
-extern "C" int xvb_conformer_embed_dim(const xvb_conformer_t* h) { return h && h->finalized ? h->m->E : XVB_EINVAL; }
+extern "C" int xvb_conformer_finalize(xvb_conformer_t* h) { return publish_built(h, build, "xvb_conformer_finalize"); }
+
+extern "C" int xvb_conformer_feat_dim(const xvb_conformer_t* h) { return h ? h->m->cfg.feat_dim : XVB_EINVAL; }
+extern "C" int xvb_conformer_embed_dim(const xvb_conformer_t* h) { return finalized(h) ? h->m->E : XVB_EINVAL; }
 extern "C" int xvb_conformer_last_launches(const xvb_conformer_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized, "xvb_conformer_extract: model not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_conformer_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0, "xvb_conformer_extract: bad arguments");
   XVB_CHECK_ARG(T >= kMinFrames, "xvb_conformer_extract: the Conformer needs at least %d frames, got %d", kMinFrames, T);
   int T1, F1, T2, F2;
@@ -499,7 +493,7 @@ extern "C" int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int
 
 // ---- "XVBC0001" model files: the configuration, then the records and tables as handed over (save_records) ---------
 extern "C" int xvb_conformer_save(const xvb_conformer_t* h, const char* path) {
-  XVB_CHECK_ARG(h && h->finalized && path, "xvb_conformer_save: model not finalized");
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_conformer_save: model not finalized");
   return save_records("xvb_conformer_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
@@ -514,8 +508,4 @@ extern "C" int xvb_conformer_load(xvb_conformer_t** out, const char* path) {
       [](void* h) { xvb_conformer_destroy((xvb_conformer_t*)h); });
 }
 
-extern "C" void xvb_conformer_destroy(xvb_conformer_t* h) {
-  if (!h) return;
-  delete h->m;
-  delete h;
-}
+extern "C" void xvb_conformer_destroy(xvb_conformer_t* h) { delete h; }

@@ -82,9 +82,7 @@ struct Model {
 
 using namespace xvb;
 
-struct xvb_ecapa {
-  std::shared_ptr<const Model> m;
-  Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
+struct xvb_ecapa : Handle<Model> {
   // workspace, each buffer grown to the largest call seen: the plane buffers up to kPp, then the fp32 ones
   enum { kIn, kX, kH, kR, kZ, kN, kCat, kM, kA1, kGp, kS1, kZm, kPp, kMF, kLog, kGate, kUb, kZmean, kGstat, kPstat, kS1f,
          kF1, kBufs };
@@ -94,11 +92,11 @@ struct xvb_ecapa {
   float *MF = nullptr, *LOG = nullptr, *gate = nullptr, *ub = nullptr, *zmean = nullptr, *gstat = nullptr, *pstat = nullptr;
   float* s1f = nullptr;   // (B, se_dim) fp32: hidden vector of the SE gate
   float* f1 = nullptr;    // (B, fc1_dim) fp32: output of fc1 when the model has one
-  int last_launches = 0;
   Im2col im2col;   // this lane's copy of the model's choice
   Shard<xvb_ecapa> shard;
 
-  explicit xvb_ecapa(std::shared_ptr<const Model> model) : m(std::move(model)), im2col(m->im2col) {}
+  xvb_ecapa() = default;
+  explicit xvb_ecapa(std::shared_ptr<const Model> model) : Handle(std::move(model)), im2col(m->im2col) {}
 };
 
 template <>
@@ -117,19 +115,18 @@ extern "C" int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, i
   XVB_CHECK_ARG(out && feat_dim > 0 && channels > 0 && mfa_dim > 0 && att_hidden > 0 && embed_dim > 0, "xvb_ecapa_create: bad arguments");
   XVB_CHECK_ARG(channels % 64 == 0 && channels / 8 == 128, "xvb_ecapa_create: the Res2Net chain kernel is built for scale 8 x width 128 (channels = 1024), got %d", channels);
   XVB_CHECK_ARG(mfa_dim % 8 == 0 && att_hidden % 8 == 0 && embed_dim % 4 == 0, "xvb_ecapa_create: mfa_dim/att_hidden must be multiples of 8, embed_dim of 4");
-  auto m = std::make_shared<Model>();
+  xvb_ecapa* h = new xvb_ecapa();
+  Model* m = h->draft;
   m->feat_dim = feat_dim; m->ldf = (int)round_up(feat_dim, 8);
   m->C = channels; m->D = mfa_dim; m->H = att_hidden; m->E = embed_dim;
   m->AX = att_hidden; m->NL = mfa_dim; m->ldlog = mfa_dim; m->P = 2 * mfa_dim; m->P2 = 2 * mfa_dim;
-  xvb_ecapa* h = new xvb_ecapa(m);
-  h->draft = m.get();
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int share, int affine_layers,
                                    int time_attention, int stddev) {
-  XVB_CHECK_ARG(h && h->draft && h->draft->layers.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
+  XVB_CHECK_ARG(is_draft(h) && h->draft->layers.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
   Model* m = h->draft;
   XVB_CHECK_ARG(num_head >= 1 && num_q >= 1 && hidden >= 1 && (affine_layers == 1 || affine_layers == 2) && m->D % num_head == 0 &&
                 (m->D / num_head) % 4 == 0 && hidden * num_head * num_q == m->H,
@@ -159,7 +156,7 @@ static int layer_groups(const Model* m, const std::string& n) {
 extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
                                    const float* w_host, const float* bias_host, const float* bn_scale_host,
                                    const float* bn_shift_host, int flags) {
-  XVB_CHECK_ARG(h && h->draft && name && w_host && context_host, "xvb_ecapa_set_layer: bad arguments or finalized model");
+  XVB_CHECK_ARG(is_draft(h) && name && w_host && context_host, "xvb_ecapa_set_layer: bad arguments or finalized model");
   Model* m = h->draft;
   XVB_CHECK_ARG(Cout > 0 && Cin > 0 && ntaps >= 1 && ntaps <= XVB_MAX_TAPS, "xvb_ecapa_set_layer(%s): bad shape", name);
   XVB_CHECK_ARG(!(flags & XVB_BN) || (bn_scale_host && bn_shift_host), "xvb_ecapa_set_layer(%s): XVB_BN without scale/shift", name);
@@ -203,7 +200,7 @@ static const ELayer* find(const Model* m, const std::string& n) {
 }
 
 extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
-  XVB_CHECK_ARG(h && h->draft, "xvb_ecapa_finalize: null or finalized model");
+  XVB_CHECK_ARG(is_draft(h), "xvb_ecapa_finalize: null or finalized model");
   Model* m = h->draft;
   const int C = m->C, W = C / m->scale;
   auto need = [&](const std::string& n, int cin, int cout, int ntaps) -> int {
@@ -381,7 +378,7 @@ static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
 }
 
 extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_ecapa_extract: model not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_ecapa_extract: model not finalized");
   const Model* m = h->m.get();
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_ecapa_extract: bad arguments");
   int rc = reserve(h, B, T);
@@ -474,33 +471,30 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
 }
 
 extern "C" int xvb_ecapa_extract_host(xvb_ecapa_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && B > 0 && T > 0, "xvb_ecapa_extract_host: bad arguments");
-  return h->shard.extract_host(h, feats_host, B, T, emb_host, stream);
+  return Shard<xvb_ecapa>::extract_host(h, feats_host, B, T, emb_host, stream, "xvb_ecapa_extract_host");
 }
 
 // A whole shard of N equal-length utterances in `batch`-utterance batches (the reference's caller loop,
 // extract_embeddings.py:73-83), device-resident / through pinned host buffers with the copies overlapped (shard.cuh).
 extern "C" int xvb_ecapa_set_gather(xvb_ecapa_t* h, float* const* tables, int ntables, int64_t row0, int64_t ld) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_ecapa_set_gather: bad arguments");
+  XVB_CHECK_ARG(finalized(h), "xvb_ecapa_set_gather: bad arguments");
   return h->shard.set_gather(tables, ntables, row0, ld, h->m->E, "xvb_ecapa_set_gather");
 }
 
 extern "C" int xvb_ecapa_extract_shard(xvb_ecapa_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_ecapa_extract_shard: bad arguments");
-  return h->shard.device(h, feats, N, T, batch, emb, stream, false);
+  return Shard<xvb_ecapa>::device(h, feats, N, T, batch, emb, stream, false, "xvb_ecapa_extract_shard");
 }
 
 extern "C" int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_host, int64_t N, int T, int batch, float* emb_host,
                                             void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && N > 0 && T > 0 && batch > 0, "xvb_ecapa_extract_shard_host: bad arguments");
-  return h->shard.host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_ecapa_extract_shard_host");
+  return Shard<xvb_ecapa>::host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_ecapa_extract_shard_host");
 }
 
 // ---- .xvbm files for ECAPA ("XVBE0001"): dims, then named layer records -------------------------------------
 // "XVBE0002" (MQMHA pooling): the same with the pooling record {num_head, num_q, hidden, share, affine_layers,
 // time_attention, stddev} after the dims; layers of grouped convs are stored as the state_dict holds them.
 extern "C" int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path) {
-  XVB_CHECK_ARG(h && !h->draft && path, "xvb_ecapa_save: model not finalized");
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_ecapa_save: model not finalized");
   const Model* m = h->m.get();
   FILE* f = fopen(path, "wb");
   XVB_CHECK_ARG(f, "xvb_ecapa_save: cannot open '%s'", path);

@@ -54,9 +54,7 @@ struct StepPlan {
 
 using namespace xvb;
 
-struct xvb_extractor {
-  std::shared_ptr<const Model> m;
-  Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
+struct xvb_extractor : Handle<Model> {
   // workspace, each buffer grown to the largest call seen: the input planes (B, pad_front + T + pad_back, ldf), the
   // ping-pong activations (B, T, max_c), the last frame layer's fp32 output (B, T, C_last), the pooled statistics
   // (B, 2 C_last) in fp32, the nominal target of the last segment layer's plan (B, D), the pooled statistics as planes,
@@ -64,7 +62,6 @@ struct xvb_extractor {
   // per-utterance frame counts of a masked call (xvb_extractor_extract_lengths)
   enum { kIn, kAct0, kAct1, kLast, kStats, kEmb, kStatsPlanes, kSeg0, kSeg1, kPoolPartial, kLengths, kBufs };
   Workspace<kBufs> ws;
-  int last_launches = 0;
   bool fused_pooling = true;
   Im2col im2col;   // this lane's copy of the model's choice
   // launch plans per batch shape (B, T, masked); they hold workspace addresses, so a reserve that reallocates clears them
@@ -77,7 +74,8 @@ struct xvb_extractor {
   cudaStream_t events_stream = nullptr;
   Shard<xvb_extractor> shard;
 
-  explicit xvb_extractor(std::shared_ptr<const Model> model) : m(std::move(model)), im2col(m->im2col) {}
+  xvb_extractor() = default;
+  explicit xvb_extractor(std::shared_ptr<const Model> model) : Handle(std::move(model)), im2col(m->im2col) {}
   ~xvb_extractor() {
     drop_plans();
     for (cudaEvent_t e : events) cudaEventDestroy(e);
@@ -142,11 +140,9 @@ extern "C" int xvb_extractor_create(xvb_extractor_t** out, int feat_dim) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(out && feat_dim > 0, "xvb_extractor_create: bad arguments");
-  auto m = std::make_shared<Model>();
-  m->feat_dim = feat_dim;
-  m->ldf = (int)round_up(feat_dim, 8);
-  xvb_extractor* h = new xvb_extractor(m);
-  h->draft = m.get();
+  xvb_extractor* h = new xvb_extractor();
+  h->draft->feat_dim = feat_dim;
+  h->draft->ldf = (int)round_up(feat_dim, 8);
   *out = h;
   return XVB_OK;
 }
@@ -154,7 +150,7 @@ extern "C" int xvb_extractor_create(xvb_extractor_t** out, int feat_dim) {
 extern "C" int xvb_extractor_add_frame_layer(xvb_extractor_t* h, int Cout, const int* context_host, int ntaps,
                                              const float* w_host, const float* bias_host, const float* bn_scale_host,
                                              const float* bn_shift_host, int flags) {
-  XVB_CHECK_ARG(h && h->draft, "xvb_extractor_add_frame_layer: null or finalized extractor");
+  XVB_CHECK_ARG(is_draft(h), "xvb_extractor_add_frame_layer: null or finalized extractor");
   Model* m = h->draft;
   XVB_CHECK_ARG(m->segment.empty(), "xvb_extractor_add_frame_layer: frame layers must precede segment layers");
   const int Cin = m->frame.empty() ? m->feat_dim : m->frame.back().Cout;
@@ -163,7 +159,7 @@ extern "C" int xvb_extractor_add_frame_layer(xvb_extractor_t* h, int Cout, const
 
 extern "C" int xvb_extractor_add_segment_layer(xvb_extractor_t* h, int Cout, const float* w_host, const float* bias_host,
                                                const float* bn_scale_host, const float* bn_shift_host, int flags) {
-  XVB_CHECK_ARG(h && h->draft && !h->draft->frame.empty(), "xvb_extractor_add_segment_layer: need frame layers first");
+  XVB_CHECK_ARG(is_draft(h) && !h->draft->frame.empty(), "xvb_extractor_add_segment_layer: need frame layers first");
   Model* m = h->draft;
   const int Cin = m->segment.empty() ? 2 * m->frame.back().Cout : m->segment.back().Cout;
   const int ctx0 = 0;
@@ -171,7 +167,7 @@ extern "C" int xvb_extractor_add_segment_layer(xvb_extractor_t* h, int Cout, con
 }
 
 extern "C" int xvb_extractor_finalize(xvb_extractor_t* h, float pooling_eps) {
-  XVB_CHECK_ARG(h && h->draft && !h->draft->frame.empty() && !h->draft->segment.empty(),
+  XVB_CHECK_ARG(is_draft(h) && !h->draft->frame.empty() && !h->draft->segment.empty(),
                 "xvb_extractor_finalize: need >=1 frame and >=1 segment layer");
   Model* m = h->draft;
   m->max_c = 0;
@@ -349,24 +345,21 @@ static int extract_batch(H* h, const float* feats, int B, int T, bool masked, fl
 }
 
 extern "C" int xvb_extractor_extract(xvb_extractor_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_extractor_extract: extractor not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_extractor_extract: extractor not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_extractor_extract: bad arguments");
   return extract_batch(h, feats, B, T, false, emb, stream);
 }
 
 extern "C" int xvb_extractor_extract_lengths(xvb_extractor_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
                                              float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_extractor_extract_lengths: extractor not finalized");
-  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "xvb_extractor_extract_lengths: bad arguments");
-  bool all_T = true;
-  for (int b = 0; b < B; ++b) {
-    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "xvb_extractor_extract_lengths: lengths[%d]=%d outside [1, T=%d]", b,
-                  (int)lengths_host[b], T);
-    all_T = all_T && lengths_host[b] == T;
-  }
-  if (all_T) return extract_batch(h, feats, B, T, false, emb, stream);   // nothing to mask: the unmasked call itself
-  const int rc = reserve(h, B, T, true);   // first, so that the lengths land in the buffer the plans read
+  const char* fn = "xvb_extractor_extract_lengths";
+  XVB_CHECK_ARG(finalized(h), "%s: extractor not finalized", fn);
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "%s: bad arguments", fn);
+  bool all_T;
+  int rc = check_lengths(fn, lengths_host, B, T, &all_T);
   if (rc) return rc;
+  if (all_T) return extract_batch(h, feats, B, T, false, emb, stream);   // nothing to mask: the unmasked call itself
+  if ((rc = reserve(h, B, T, true))) return rc;   // first, so that the lengths land in the buffer the plans read
   // stream-ordered: the previous call's kernels on `stream` have read the old lengths before these land
   XVB_CUDA(cudaMemcpyAsync(h->ws.i32(H::kLengths), lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice,
                            (cudaStream_t)stream));
@@ -374,7 +367,7 @@ extern "C" int xvb_extractor_extract_lengths(xvb_extractor_t* h, const float* fe
 }
 
 extern "C" int xvb_extractor_set_gather(xvb_extractor_t* h, float* const* tables, int ntables, int64_t row0, int64_t ld) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_extractor_set_gather: bad arguments");
+  XVB_CHECK_ARG(finalized(h), "xvb_extractor_set_gather: bad arguments");
   return h->shard.set_gather(tables, ntables, row0, ld, h->m->segment.back().Cout, "xvb_extractor_set_gather");
 }
 
@@ -383,25 +376,22 @@ extern "C" int xvb_extractor_set_gather(xvb_extractor_t* h, float* const* tables
 // and the events of all of them are kept.
 extern "C" int xvb_extractor_extract_shard(xvb_extractor_t* h, const float* feats, int64_t N, int T, int batch, float* emb,
                                            void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_extractor_extract_shard: bad arguments");
+  XVB_CHECK_ARG(h, "xvb_extractor_extract_shard: bad arguments");
   h->events_used = 0;
   h->in_shard = true;
-  const int rc = h->shard.device(h, feats, N, T, batch, emb, stream, h->profiling);
+  const int rc = Shard<H>::device(h, feats, N, T, batch, emb, stream, h->profiling, "xvb_extractor_extract_shard");
   h->in_shard = false;
   return rc;
 }
 
 extern "C" int xvb_extractor_extract_host(xvb_extractor_t* h, const float* feats_host, int B, int T, float* emb_host,
                                           void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && B > 0 && T > 0, "xvb_extractor_extract_host: bad arguments");
-  return h->shard.extract_host(h, feats_host, B, T, emb_host, stream);
+  return Shard<H>::extract_host(h, feats_host, B, T, emb_host, stream, "xvb_extractor_extract_host");
 }
 
 extern "C" int xvb_extractor_submit_host(xvb_extractor_t* h, const float* feats_host, int B, int T, float* emb_host,
                                          int slot, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && B > 0 && T > 0 && (slot == 0 || slot == 1),
-                "xvb_extractor_submit_host: bad arguments (slot must be 0 or 1)");
-  return h->shard.submit(h, feats_host, B, T, emb_host, slot, stream, "xvb_extractor_submit_host");
+  return Shard<H>::submit(h, feats_host, B, T, emb_host, slot, stream, "xvb_extractor_submit_host");
 }
 
 extern "C" int xvb_extractor_wait(xvb_extractor_t* h, int slot) {
@@ -411,9 +401,7 @@ extern "C" int xvb_extractor_wait(xvb_extractor_t* h, int slot) {
 
 extern "C" int xvb_extractor_extract_shard_host(xvb_extractor_t* h, const float* feats_host, int64_t N, int T, int batch,
                                                 float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && N > 0 && T > 0 && batch > 0,
-                "xvb_extractor_extract_shard_host: bad arguments");
-  return h->shard.host(h, feats_host, N, T, batch, emb_host, stream, h->profiling, "xvb_extractor_extract_shard_host");
+  return Shard<H>::host(h, feats_host, N, T, batch, emb_host, stream, h && h->profiling, "xvb_extractor_extract_shard_host");
 }
 
 extern "C" int xvb_extractor_set_fused_pooling(xvb_extractor_t* h, int enable) {

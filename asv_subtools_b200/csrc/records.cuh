@@ -1,9 +1,11 @@
-// Device side of the native extractors' shared plumbing: the packed split-bf16 planes and the arena that owns a model's
-// device weights (every family), the grow-only workspace, the segment level of the 2-D families and the group loop of
-// an extract call.  The record store and the model-file codec are host code in records.h.
+// Device side of the native extractors' shared plumbing: the handle base, the packed split-bf16 planes and the arena
+// that owns a model's device weights (every family), the grow-only workspace, the segment level of the 2-D families,
+// the group loop of an extract call and the lengths check of a masked one.  The record store and the model-file codec
+// are host code in records.h.
 #pragma once
 #include <stdlib.h>
 
+#include <memory>
 #include <vector>
 
 #include "common.cuh"
@@ -207,6 +209,52 @@ struct SegTail {
     return XVB_OK;
   }
 };
+
+// The part of a native extractor handle that is not workspace or per-lane state.  From create until finalize succeeds
+// the handle is a draft: set_layer / add_*_layer write `draft`, the model that `m` owns, so that getters read drafts and
+// finalized handles alike.  Once finalized, the model is immutable and shared by the handle and its second shard lane.
+template <typename Model>
+struct Handle {
+  std::shared_ptr<const Model> m;
+  Model* draft = nullptr;
+  int last_launches = 0;
+
+  Handle() { auto d = std::make_shared<Model>(); draft = d.get(); m = std::move(d); }
+  explicit Handle(std::shared_ptr<const Model> model) : m(std::move(model)) {}   // a lane on a finalized model
+};
+
+template <typename Model> bool finalized(const Handle<Model>* h) { return h && !h->draft; }
+template <typename Model> bool is_draft(const Handle<Model>* h) { return h && h->draft; }
+
+// The finalize of the record-store families (fn: its name): build(fresh, records) makes a new model from the draft's
+// configuration and records, and only a model built without error is published, the records moved into it for save.
+// A failed build is discarded with its device weights and the draft keeps its records, so that the caller can add what
+// was missing and finalize again.
+template <typename Model, typename Build>
+int publish_built(Handle<Model>* h, Build build, const char* fn) {
+  XVB_CHECK_ARG(is_draft(h), "%s: null or finalized model", fn);
+  auto fresh = std::make_shared<Model>();
+  fresh->cfg = h->draft->cfg;
+  h->draft->recs.used.clear();
+  int rc = build(fresh.get(), h->draft->recs);
+  if (rc) return rc;
+  fresh->recs = std::move(h->draft->recs);
+  h->m = std::move(fresh);
+  h->draft = nullptr;
+  return XVB_OK;
+}
+
+// The host lengths of a masked call: each in [1, T], or XVB_EINVAL naming the first that is not (fn: the caller's
+// name).  *all_T: every utterance is T frames long, so that there is nothing to mask.
+inline int check_lengths(const char* fn, const int32_t* lengths_host, int B, int T, bool* all_T) {
+  *all_T = true;
+  for (int b = 0; b < B; ++b) {
+    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "%s: lengths[%d]=%d outside [1, T=%d]", fn, b,
+                  (int)lengths_host[b], T);
+    *all_T = *all_T && lengths_host[b] == T;
+  }
+  return XVB_OK;
+}
 
 // One extract call as groups of floor(budget / per_utt) utterances (at least one): run(first, count) per group.
 template <typename Run>

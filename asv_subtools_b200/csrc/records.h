@@ -31,7 +31,7 @@ struct RecordFormat {
 
 struct RecordStore {
   explicit RecordStore(int nshape) : n(nshape) {}
-  const int n;                        // shape ints per record
+  int n;                              // shape ints per record
   std::map<std::string, Rec> recs;
   std::vector<std::string> order;     // insertion order, for save
   std::set<std::string> used;         // taken by finalize

@@ -63,12 +63,9 @@ std::vector<int> kept_taps(const float* w, int Cout, int Cin, int k) {
 
 }  // namespace
 
-struct xvb_repvgg {
-  Model* m = nullptr;
-  bool finalized = false;
+struct xvb_repvgg : Handle<Model> {
   enum { kX0, kX1, kLast, kPooled, kPooledF32, kSegMid, kSegOut, kBufs };
   Workspace<kBufs> ws;
-  int last_launches = 0;
 };
 
 namespace {
@@ -76,7 +73,7 @@ namespace {
 using H = xvb_repvgg;
 
 int reserve(H* h, int B, int T) {
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   long long t = T, f = m->cfg.feat_dim;
   size_t mx = (size_t)B * t * f * m->cfg.widths[0];
   for (const Block& b : m->blocks) {
@@ -100,7 +97,7 @@ int reserve(H* h, int B, int T) {
 int extract_group(H* h, const float* feats, int B, int T, float* emb, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
-  const Model* m = h->m;
+  const Model* m = h->m.get();
   const xvb_repvgg_config_t& c = m->cfg;
   int Tl = T, Fl = c.feat_dim;
   Planes x = h->ws.planes(H::kX0), y = h->ws.planes(H::kX1);
@@ -160,34 +157,31 @@ extern "C" int xvb_repvgg_create(xvb_repvgg_t** out, const xvb_repvgg_config_t* 
     XVB_CHECK_ARG(c.num_blocks[i] >= 1 && c.num_blocks[i] <= 64, "xvb_repvgg_create: num_blocks[%d] = %d, need 1..64", i,
                   c.num_blocks[i]);
   xvb_repvgg* h = new xvb_repvgg();
-  h->m = new Model();
-  h->m->cfg = c;
+  h->draft->cfg = c;
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_repvgg_set_layer(xvb_repvgg_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
                                     const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
-  XVB_CHECK_ARG(h && !h->finalized && name && strlen(name) > 0 && strlen(name) < 127, "xvb_repvgg_set_layer: bad arguments or finalized model");
+  XVB_CHECK_ARG(is_draft(h) && name && strlen(name) > 0 && strlen(name) < 127, "xvb_repvgg_set_layer: bad arguments or finalized model");
   XVB_CHECK_ARG(ksize == 1 || ksize == 3 || ksize == 5, "xvb_repvgg_set_layer(%s): bad shape %d x %d x k%d", name, Cout, Cin, ksize);
   const char* fn = "xvb_repvgg_set_layer";
   const int shape[3] = {Cout, Cin, ksize};
-  int rc = h->m->recs.check(fn, name, shape, w_host, scale_host, shift_host);
+  int rc = h->draft->recs.check(fn, name, shape, w_host, scale_host, shift_host);
   if (rc) return rc;
   XVB_CHECK_ARG((flags & ~(XVB_RELU | XVB_BN)) == 0, "xvb_repvgg_set_layer(%s): flags %d", name, flags);
   XVB_CHECK_ARG(!(flags & XVB_BN) || scale_host, "xvb_repvgg_set_layer(%s): XVB_BN without scale/shift", name);
-  return h->m->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
+  return h->draft->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
-extern "C" int xvb_repvgg_finalize(xvb_repvgg_t* h) {
-  XVB_CHECK_ARG(h && !h->finalized && h->m, "xvb_repvgg_finalize: null or finalized model");
-  Model* m = h->m;
+static int build(Model* m, RecordStore& recs) {
   const xvb_repvgg_config_t& c = m->cfg;
   const int k = c.ksize;
   // a folded block: (cout, cin, k) with its bias, no scale / shift, flags XVB_RELU
   auto block = [&](const std::string& n, int cout, int cin, const Rec** out) -> int {
     const int shape[3] = {cout, cin, k};
-    int rc = m->recs.take("xvb_repvgg_finalize", n, shape, out);
+    int rc = recs.take("xvb_repvgg_finalize", n, shape, out);
     if (rc) return rc;
     const Rec* r = *out;
     XVB_CHECK_ARG(!r->b.empty() && r->s.empty() && r->flags == XVB_RELU,
@@ -223,18 +217,18 @@ extern "C" int xvb_repvgg_finalize(xvb_repvgg_t* h) {
   m->F4 = f;
   m->C4 = inp;
   // segment level (repvgg_xvector.py:192-206): [fc1 ->] [fc2], as many as the extracted position hands over
-  if ((rc = m->tail.build(m->recs, m->dev, "xvb_repvgg_finalize", 2 * m->F4 * m->C4))) return rc;
-  if ((rc = m->recs.check_all_used("xvb_repvgg_finalize"))) return rc;
-  h->finalized = true;
-  return XVB_OK;
+  if ((rc = m->tail.build(recs, m->dev, "xvb_repvgg_finalize", 2 * m->F4 * m->C4))) return rc;
+  return recs.check_all_used("xvb_repvgg_finalize");
 }
 
-extern "C" int xvb_repvgg_feat_dim(const xvb_repvgg_t* h) { return h && h->m ? h->m->cfg.feat_dim : XVB_EINVAL; }
-extern "C" int xvb_repvgg_embed_dim(const xvb_repvgg_t* h) { return h && h->finalized ? h->m->tail.E : XVB_EINVAL; }
+extern "C" int xvb_repvgg_finalize(xvb_repvgg_t* h) { return publish_built(h, build, "xvb_repvgg_finalize"); }
+
+extern "C" int xvb_repvgg_feat_dim(const xvb_repvgg_t* h) { return h ? h->m->cfg.feat_dim : XVB_EINVAL; }
+extern "C" int xvb_repvgg_embed_dim(const xvb_repvgg_t* h) { return finalized(h) ? h->m->tail.E : XVB_EINVAL; }
 extern "C" int xvb_repvgg_last_launches(const xvb_repvgg_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_repvgg_extract(xvb_repvgg_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && h->finalized, "xvb_repvgg_extract: model not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_repvgg_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_repvgg_extract: bad arguments");
   const long before = g_launches;
   const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->tail.E;
@@ -247,7 +241,7 @@ extern "C" int xvb_repvgg_extract(xvb_repvgg_t* h, const float* feats, int B, in
 
 // ---- "XVBV0001" model files: the configuration, then the records as handed over (save_records) ------------------
 extern "C" int xvb_repvgg_save(const xvb_repvgg_t* h, const char* path) {
-  XVB_CHECK_ARG(h && h->finalized && path, "xvb_repvgg_save: model not finalized");
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_repvgg_save: model not finalized");
   return save_records("xvb_repvgg_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
@@ -261,8 +255,4 @@ extern "C" int xvb_repvgg_load(xvb_repvgg_t** out, const char* path) {
       [](void* h) { return xvb_repvgg_finalize((xvb_repvgg_t*)h); }, [](void* h) { xvb_repvgg_destroy((xvb_repvgg_t*)h); });
 }
 
-extern "C" void xvb_repvgg_destroy(xvb_repvgg_t* h) {
-  if (!h) return;
-  delete h->m;
-  delete h;
-}
+extern "C" void xvb_repvgg_destroy(xvb_repvgg_t* h) { delete h; }

@@ -34,7 +34,12 @@ using namespace xvb;
 // One B*T*F position budget per extract call: larger calls run as consecutive groups of utterances (see xvb200.h).
 constexpr long long kPositionBudget = 256LL * 200 * 80;
 constexpr int kSeMaxK = 9;   // k = 1, 2, ..., 256 for the k-grouped SE mean
-const RecordFormat kFile = {"XVBR0001", 10 * sizeof(int32_t) + sizeof(float), 3, 4096};
+struct Config {   // the create arguments, laid out as the configuration block of a model file
+  int32_t feat_dim = 0, layers[4] = {0}, planes[4] = {0}, pre = 0;
+  float eps = 0.f;   // pooling_eps
+};
+static_assert(sizeof(Config) == 10 * sizeof(int32_t) + sizeof(float), "the XVBR0001 configuration block");
+const RecordFormat kFile = {"XVBR0001", sizeof(Config), 3, 4096};
 struct Bn { float* s = nullptr; float* t = nullptr; };
 struct Se {
   int C = 0, Hp = 0, kmax = 1;           // hidden width padded to a multiple of 4; k = 1 .. kmax (powers of two)
@@ -48,10 +53,8 @@ struct Block {
   bool has_ds = false, has_se = false;
   Se se;
 };
-// Shared read-only by a handle and its second shard lane once finalized.
 struct Model {
-  int feat_dim = 0, layers[4] = {0}, planes[4] = {0}, pre = 0;
-  float eps = 0.f;
+  Config cfg;
   RecordStore recs{kFile.nshape};
   float* head_w = nullptr;
   Bn head_bn;
@@ -63,9 +66,7 @@ struct Model {
 
 }  // namespace
 
-struct xvb_resnet {
-  std::shared_ptr<const Model> m;
-  Model* draft = nullptr;   // the model while it is built: from create until finalize succeeds
+struct xvb_resnet : Handle<Model> {
   // workspace, each buffer grown to the largest call seen: seven rotating (B, T', F', C) plane buffers for the roles
   // block input / activated input / h / identity / z / output / next activated input, picked by index, the fp32
   // last-layer output, then the per-utterance buffers (pooled statistics, SE mean / hidden / gate, segment layers) and
@@ -74,10 +75,9 @@ struct xvb_resnet {
   static constexpr int kLevels = 4;
   enum { kRot0, kLast = kRot0 + kRotating, kPooled, kPooledF32, kSeMean, kSeHidden, kSeGate, kSegMid, kSegOut, kLengths, kBufs };
   Workspace<kBufs> ws;
-  int last_launches = 0;
   Shard<xvb_resnet> shard;
 
-  explicit xvb_resnet(std::shared_ptr<const Model> model) : m(std::move(model)) {}
+  using Handle::Handle;
 };
 
 using H = xvb_resnet;
@@ -88,7 +88,7 @@ struct xvb::ShardFamily<xvb_resnet> {
     return xvb_resnet_extract(h, feats, B, T, emb, stream);
   }
   static xvb_resnet* twin(const xvb_resnet* h) { return new xvb_resnet(h->m); }
-  static int feat_dim(const xvb_resnet* h) { return h->m->feat_dim; }
+  static int feat_dim(const xvb_resnet* h) { return h->m->cfg.feat_dim; }
   static int embed_dim(const xvb_resnet* h) { return h->m->tail.E; }
 };
 
@@ -98,8 +98,8 @@ int log2i(int k) { int l = 0; while ((1 << l) < k) ++l; return l; }
 
 // Position-buffer sizes (elements) of one (B, T) call: the largest (B, T', F', C) tensor and the last layer's output.
 void shapes(const Model* m, int B, int T, size_t* planes, size_t* last) {
-  long long t = T, f = m->feat_dim;
-  size_t mx = (size_t)B * t * f * m->planes[0];
+  long long t = T, f = m->cfg.feat_dim;
+  size_t mx = (size_t)B * t * f * m->cfg.planes[0];
   for (const Block& b : m->blocks) {
     t = (t - 1) / b.stride + 1;
     f = (f - 1) / b.stride + 1;
@@ -174,8 +174,8 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, const int* le
   Planes buf[H::kRotating];
   for (int i = 0; i < H::kRotating; ++i) buf[i] = h->ws.planes(H::kRot0 + i);
   const Model* m = h->m.get();
-  const bool pre = m->pre != 0;
-  int Tl = T, Fl = m->feat_dim;
+  const bool pre = m->cfg.pre != 0;
+  int Tl = T, Fl = m->cfg.feat_dim;
   int xi = 0, ai = pre ? 1 : -1;
   const Bn none;
   int level = 0;
@@ -183,9 +183,9 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, const int* le
   {
     const Bn first = pre ? m->blocks[0].bn1 : none;
     const Planes* a = pre ? &buf[ai] : nullptr;
-    rc = lens ? xvb_conv2d_head_lengths(feats, B, T, Fl, lens, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi,
+    rc = lens ? xvb_conv2d_head_lengths(feats, B, T, Fl, lens, m->head_w, m->cfg.planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi,
                                         buf[xi].lo, first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream)
-              : xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi, buf[xi].lo,
+              : xvb_conv2d_head(feats, B, T, Fl, m->head_w, m->cfg.planes[0], m->head_bn.s, m->head_bn.t, buf[xi].hi, buf[xi].lo,
                                 first.s, first.t, a ? a->hi : nullptr, a ? a->lo : nullptr, stream);
     if (rc) return rc;
   }
@@ -239,7 +239,7 @@ int extract_group(xvb_resnet* h, const float* feats, int B, int T, const int* le
     xi = yi; ai = an; Tl = Tn; Fl = Fn;
     if (st == 2) ++level;
   }
-  return m->tail.run(h->ws.f32(H::kLast), Fl * m->C4, B, Tl, m->eps, h->ws.planes(H::kPooled), h->ws.f32(H::kPooledF32),
+  return m->tail.run(h->ws.f32(H::kLast), Fl * m->C4, B, Tl, m->cfg.eps, h->ws.planes(H::kPooled), h->ws.f32(H::kPooledF32),
                      h->ws.planes(H::kSegMid), h->ws.f32(H::kSegOut), emb, stream, at(level));
 }
 
@@ -256,20 +256,19 @@ extern "C" int xvb_resnet_create(xvb_resnet_t** out, int feat_dim, const int* la
     XVB_CHECK_ARG(planes[i] >= 16 && planes[i] <= 4096 && planes[i] % 16 == 0,
                   "xvb_resnet_create: planes[%d] = %d, need a multiple of 16 for the 2-D conv kernel", i, planes[i]);
   }
-  auto m = std::make_shared<Model>();
-  m->feat_dim = feat_dim;
-  for (int i = 0; i < 4; ++i) { m->layers[i] = layers[i]; m->planes[i] = planes[i]; }
-  m->pre = pre_activation ? 1 : 0;
-  m->eps = pooling_eps;
-  xvb_resnet* h = new xvb_resnet(m);
-  h->draft = m.get();
+  xvb_resnet* h = new xvb_resnet();
+  Config& c = h->draft->cfg;
+  c.feat_dim = feat_dim;
+  for (int i = 0; i < 4; ++i) { c.layers[i] = layers[i]; c.planes[i] = planes[i]; }
+  c.pre = pre_activation ? 1 : 0;
+  c.eps = pooling_eps;
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_resnet_set_layer(xvb_resnet_t* h, const char* name, int Cout, int Cin, int ksize, const float* w_host,
                                     const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
-  XVB_CHECK_ARG(h && h->draft && name && strlen(name) > 0 && strlen(name) < 127, "xvb_resnet_set_layer: bad arguments or finalized model");
+  XVB_CHECK_ARG(is_draft(h) && name && strlen(name) > 0 && strlen(name) < 127, "xvb_resnet_set_layer: bad arguments or finalized model");
   XVB_CHECK_ARG(ksize == 0 || ksize == 1 || ksize == 3, "xvb_resnet_set_layer(%s): bad shape %d x %d x k%d", name, Cout, Cin, ksize);
   const char* fn = "xvb_resnet_set_layer";
   const int shape[3] = {Cout, Cin, ksize};
@@ -279,13 +278,11 @@ extern "C" int xvb_resnet_set_layer(xvb_resnet_t* h, const char* name, int Cout,
   return h->draft->recs.add(fn, name, shape, w_host, bias_host, scale_host, shift_host, flags);
 }
 
-extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
-  XVB_CHECK_ARG(h && h->draft, "xvb_resnet_finalize: null or finalized model");
-  Model* m = h->draft;
+static int build(Model* m, RecordStore& recs) {
   // a record the configuration needs: present, with the expected shape
   auto need = [&](const std::string& n, int cout, int cin, int k, const Rec** out) -> int {
     const int shape[3] = {cout, cin, k};
-    return m->recs.take("xvb_resnet_finalize", n, shape, out);
+    return recs.take("xvb_resnet_finalize", n, shape, out);
   };
   auto bn = [&](const std::string& n, int c, Bn* out) -> int {
     const Rec* r;
@@ -302,28 +299,28 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
   };
   int rc;
   const Rec* r;
-  if ((rc = need("resnet.conv1", m->planes[0], 1, 3, &r)) || (rc = m->dev.upload(&m->head_w, r->w)) || (rc = bn("resnet.bn1", m->planes[0], &m->head_bn)))
+  if ((rc = need("resnet.conv1", m->cfg.planes[0], 1, 3, &r)) || (rc = m->dev.upload(&m->head_w, r->w)) || (rc = bn("resnet.bn1", m->cfg.planes[0], &m->head_bn)))
     return rc;
-  const bool use_se = m->recs.find("resnet.layer1.0.se.fc_1") != nullptr;
-  int inp = m->planes[0], f = m->feat_dim;
+  const bool use_se = recs.find("resnet.layer1.0.se.fc_1") != nullptr;
+  int inp = m->cfg.planes[0], f = m->cfg.feat_dim;
   m->Cmax = 0; m->Hmax = 0;
   for (int li = 0; li < 4; ++li) {
-    const int p = m->planes[li];
+    const int p = m->cfg.planes[li];
     if (li) f = (f - 1) / 2 + 1;
-    for (int i = 0; i < m->layers[li]; ++i) {
+    for (int i = 0; i < m->cfg.layers[li]; ++i) {
       const std::string pre = "resnet.layer" + std::to_string(li + 1) + "." + std::to_string(i) + ".";
       Block b;
       b.stride = (li > 0 && i == 0) ? 2 : 1;
       b.cin = i == 0 ? inp : p;
       b.cout = p;
       if ((rc = conv_rec(pre + "conv1", p, b.cin, 3, &b.conv1)) || (rc = conv_rec(pre + "conv2", p, p, 3, &b.conv2)) ||
-          (rc = bn(pre + "bn1", m->pre ? b.cin : p, &b.bn1)) || (rc = bn(pre + "bn2", p, &b.bn2)))
+          (rc = bn(pre + "bn1", m->cfg.pre ? b.cin : p, &b.bn1)) || (rc = bn(pre + "bn2", p, &b.bn2)))
         return rc;
       b.has_ds = i == 0 && (li > 0 || inp != p);   // resnet.py:324-328
       if (b.has_ds && ((rc = conv_rec(pre + "downsample.0", p, inp, 1, &b.ds)) || (rc = bn(pre + "downsample.1", p, &b.dsbn)))) return rc;
       b.has_se = use_se;
       if (use_se) {
-        const Rec* r1 = m->recs.find(pre + "se.fc_1");
+        const Rec* r1 = recs.find(pre + "se.fc_1");
         XVB_CHECK_ARG(r1, "xvb_resnet_finalize: record '%sse.fc_1' is missing (the first block has SE)", pre.c_str());
         const int hid = r1->shape[0];
         const Rec* r2;
@@ -358,23 +355,23 @@ extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) {
     inp = p;
   }
   m->F4 = f;
-  m->C4 = m->planes[3];
+  m->C4 = m->cfg.planes[3];
   // segment level (resnet_xvector.py:194-206): [fc1 ->] [fc2], as many as the extracted position hands over
-  if ((rc = m->tail.build(m->recs, m->dev, "xvb_resnet_finalize", 2 * m->F4 * m->C4))) return rc;
-  if ((rc = m->recs.check_all_used("xvb_resnet_finalize"))) return rc;
-  h->draft = nullptr;
-  return XVB_OK;
+  if ((rc = m->tail.build(recs, m->dev, "xvb_resnet_finalize", 2 * m->F4 * m->C4))) return rc;
+  return recs.check_all_used("xvb_resnet_finalize");
 }
 
-extern "C" int xvb_resnet_feat_dim(const xvb_resnet_t* h) { return h ? h->m->feat_dim : XVB_EINVAL; }
-extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return h && !h->draft ? h->m->tail.E : XVB_EINVAL; }
+extern "C" int xvb_resnet_finalize(xvb_resnet_t* h) { return publish_built(h, build, "xvb_resnet_finalize"); }
+
+extern "C" int xvb_resnet_feat_dim(const xvb_resnet_t* h) { return h ? h->m->cfg.feat_dim : XVB_EINVAL; }
+extern "C" int xvb_resnet_embed_dim(const xvb_resnet_t* h) { return finalized(h) ? h->m->tail.E : XVB_EINVAL; }
 extern "C" int xvb_resnet_last_launches(const xvb_resnet_t* h) { return h ? h->last_launches : 0; }
 
 extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, int T, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_resnet_extract: model not finalized");
+  XVB_CHECK_ARG(finalized(h), "xvb_resnet_extract: model not finalized");
   XVB_CHECK_ARG(feats && emb && B > 0 && T > 0, "xvb_resnet_extract: bad arguments");
   const long before = g_launches;
-  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->tail.E;
   int rc = for_groups(B, (long long)per_utt, kPositionBudget,
                       [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, nullptr, 0, emb + i * E, stream); });
   if (rc) return rc;
@@ -384,14 +381,12 @@ extern "C" int xvb_resnet_extract(xvb_resnet_t* h, const float* feats, int B, in
 
 extern "C" int xvb_resnet_extract_lengths(xvb_resnet_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
                                           float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft, "xvb_resnet_extract_lengths: model not finalized");
-  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "xvb_resnet_extract_lengths: bad arguments");
-  bool all_T = true;
-  for (int b = 0; b < B; ++b) {
-    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "xvb_resnet_extract_lengths: lengths[%d]=%d outside [1, T=%d]", b,
-                  (int)lengths_host[b], T);
-    all_T = all_T && lengths_host[b] == T;
-  }
+  const char* fn = "xvb_resnet_extract_lengths";
+  XVB_CHECK_ARG(finalized(h), "%s: model not finalized", fn);
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "%s: bad arguments", fn);
+  bool all_T;
+  int rc = check_lengths(fn, lengths_host, B, T, &all_T);
+  if (rc) return rc;
   if (all_T) return xvb_resnet_extract(h, feats, B, T, emb, stream);   // nothing to mask: the unmasked call itself
   // level l + 1 = ceil(level l / 2): every stride-2 conv's output length, (L + 2 * pad - k) / 2 + 1 for k = 3 and 1
   std::vector<int32_t> table((size_t)H::kLevels * B);
@@ -403,13 +398,12 @@ extern "C" int xvb_resnet_extract_lengths(xvb_resnet_t* h, const float* feats, c
   bool planes[H::kBufs] = {false};
   need[H::kLengths] = table.size();
   uint64_t grown;
-  int rc = h->ws.reserve(need, planes, &grown);
-  if (rc) return rc;
+  if ((rc = h->ws.reserve(need, planes, &grown))) return rc;
   int* lens = h->ws.i32(H::kLengths);
   // stream-ordered: the previous call's kernels on `stream` have read the old table before this one lands
   XVB_CUDA(cudaMemcpyAsync(lens, table.data(), table.size() * sizeof(int32_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
   const long before = g_launches;
-  const size_t per_utt = (size_t)T * h->m->feat_dim, E = (size_t)h->m->tail.E;
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->tail.E;
   rc = for_groups(B, (long long)per_utt, kPositionBudget,
                   [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, lens + i, B, emb + i * E, stream); });
   if (rc) return rc;
@@ -418,40 +412,31 @@ extern "C" int xvb_resnet_extract_lengths(xvb_resnet_t* h, const float* feats, c
 }
 
 extern "C" int xvb_resnet_extract_host(xvb_resnet_t* h, const float* feats_host, int B, int T, float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && B > 0 && T > 0, "xvb_resnet_extract_host: bad arguments");
-  return h->shard.extract_host(h, feats_host, B, T, emb_host, stream);
+  return Shard<H>::extract_host(h, feats_host, B, T, emb_host, stream, "xvb_resnet_extract_host");
 }
 
 // ---- whole shards: the protocol of shard.cuh ---------------------------------------------------------------------
 extern "C" int xvb_resnet_extract_shard(xvb_resnet_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats && emb && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard: bad arguments");
-  return h->shard.device(h, feats, N, T, batch, emb, stream, false);
+  return Shard<H>::device(h, feats, N, T, batch, emb, stream, false, "xvb_resnet_extract_shard");
 }
 
 extern "C" int xvb_resnet_extract_shard_host(xvb_resnet_t* h, const float* feats_host, int64_t N, int T, int batch,
                                              float* emb_host, void* stream) {
-  XVB_CHECK_ARG(h && !h->draft && feats_host && emb_host && N > 0 && T > 0 && batch > 0, "xvb_resnet_extract_shard_host: bad arguments");
-  return h->shard.host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_resnet_extract_shard_host");
+  return Shard<H>::host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_resnet_extract_shard_host");
 }
 
 // ---- "XVBR0001" model files: the create arguments, then the named records as handed over (save_records) -----------
 extern "C" int xvb_resnet_save(const xvb_resnet_t* h, const char* path) {
-  XVB_CHECK_ARG(h && !h->draft && path, "xvb_resnet_save: model not finalized");
-  const Model* m = h->m.get();
-  int32_t cfg[11] = {m->feat_dim, m->layers[0], m->layers[1], m->layers[2], m->layers[3],
-                     m->planes[0], m->planes[1], m->planes[2], m->planes[3], m->pre};
-  memcpy(cfg + 10, &m->eps, sizeof(float));   // pooling_eps as f32
-  return save_records("xvb_resnet_save", path, kFile, cfg, m->recs);
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_resnet_save: model not finalized");
+  return save_records("xvb_resnet_save", path, kFile, &h->m->cfg, h->m->recs);
 }
 
 extern "C" int xvb_resnet_load(xvb_resnet_t** out, const char* path) {
   return load_records(
       "xvb_resnet_load", path, kFile, (void**)out,
       [](void** h, const void* cfg) {
-        const int32_t* v = (const int32_t*)cfg;
-        float eps;
-        memcpy(&eps, v + 10, sizeof eps);
-        return xvb_resnet_create((xvb_resnet_t**)h, v[0], v + 1, v + 5, v[9], eps);
+        const Config* c = (const Config*)cfg;
+        return xvb_resnet_create((xvb_resnet_t**)h, c->feat_dim, c->layers, c->planes, c->pre, c->eps);
       },
       [](void* h, const char* name, const int* shape, const float* w, const float* b, const float* s, const float* t, int flags) {
         return xvb_resnet_set_layer((xvb_resnet_t*)h, name, shape[0], shape[1], shape[2], w, b, s, t, flags);

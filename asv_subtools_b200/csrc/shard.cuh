@@ -1,6 +1,6 @@
 // The whole-shard protocol of the TDNN, ECAPA-TDNN and ResNet native extractors, written once: extract_host, the
 // device-resident and the host-buffer shard calls, the pipelined submit / wait of single batches and the replicated
-// embedding table (peer.cu).  A handle type H has a `Shard<H> shard` member and an `int last_launches` member, and
+// embedding table (peer.cu).  A handle type H derives from Handle (records.cuh), has a `Shard<H> shard` member and
 // specialises ShardFamily<H> with
 //   static int extract(H*, const float* feats, int B, int T, float* emb, void* stream)   one batch, sets last_launches
 //   static H* twin(const H*)                    a new handle on the same model: the second lane
@@ -18,6 +18,7 @@
 #include <memory>
 
 #include "common.cuh"
+#include "records.cuh"
 
 namespace xvb {
 
@@ -76,15 +77,18 @@ struct Shard {
     if (copy_stream) cudaStreamDestroy(copy_stream);
   }
 
+  // The four calls below refuse a null or draft handle and bad sizes ("fn: bad arguments") before they touch it.
   // feats (B, T, F) host -> emb (B, E) host through device staging; synchronises `stream`.
-  int extract_host(H* h, const float* feats_host, int B, int T, float* emb_host, void* stream) {
+  static int extract_host(H* h, const float* feats_host, int B, int T, float* emb_host, void* stream, const char* fn) {
+    XVB_CHECK_ARG(finalized(h) && feats_host && emb_host && B > 0 && T > 0, "%s: bad arguments", fn);
+    Shard& d = h->shard;
     const cudaStream_t s = (cudaStream_t)stream;
     const size_t nf = (size_t)B * T * F::feat_dim(h), ne = (size_t)B * F::embed_dim(h);
     int rc;
-    if ((rc = h_feats.reserve(nf)) || (rc = h_emb.reserve(ne))) return rc;
-    XVB_CUDA(cudaMemcpyAsync(h_feats.p, feats_host, nf * sizeof(float), cudaMemcpyHostToDevice, s));
-    if ((rc = F::extract(h, h_feats.p, B, T, h_emb.p, stream))) return rc;
-    XVB_CUDA(cudaMemcpyAsync(emb_host, h_emb.p, ne * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if ((rc = d.h_feats.reserve(nf)) || (rc = d.h_emb.reserve(ne))) return rc;
+    XVB_CUDA(cudaMemcpyAsync(d.h_feats.p, feats_host, nf * sizeof(float), cudaMemcpyHostToDevice, s));
+    if ((rc = F::extract(h, d.h_feats.p, B, T, d.h_emb.p, stream))) return rc;
+    XVB_CUDA(cudaMemcpyAsync(emb_host, d.h_emb.p, ne * sizeof(float), cudaMemcpyDeviceToHost, s));
     XVB_CUDA(cudaStreamSynchronize(s));
     return XVB_OK;
   }
@@ -99,21 +103,24 @@ struct Shard {
   }
 
   // feats (N, T, F) and emb (N, E) on the device; asynchronous on `stream`.
-  int device(H* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream, bool single_lane) {
+  static int device(H* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream, bool single_lane,
+                    const char* fn) {
+    XVB_CHECK_ARG(finalized(h) && feats && emb && N > 0 && T > 0 && batch > 0, "%s: bad arguments", fn);
+    Shard& d = h->shard;
     const size_t Fd = F::feat_dim(h), E = F::embed_dim(h);
     const cudaStream_t s = (cudaStream_t)stream;
     const bool lanes = two_lanes(N, batch, single_lane);
     int rc, launches = 0, k = 0;
-    if (lanes && (rc = fork(h, s))) return rc;
+    if (lanes && (rc = d.fork(h, s))) return rc;
     for (int64_t i = 0; i < N; i += batch, ++k) {
       const int b = (int)(N - i < batch ? N - i : batch);
-      H* lane = (lanes && (k & 1)) ? lane1.get() : h;
-      const cudaStream_t ls = lanes ? lane_stream[k & 1] : s;
+      H* lane = (lanes && (k & 1)) ? d.lane1.get() : h;
+      const cudaStream_t ls = lanes ? d.lane_stream[k & 1] : s;
       if ((rc = F::extract(lane, feats + (size_t)i * T * Fd, b, T, emb + (size_t)i * E, ls))) return rc;
       launches += lane->last_launches;
-      if ((rc = scatter(emb + (size_t)i * E, b, (int)E, i, ls, &launches))) return rc;
+      if ((rc = d.scatter(emb + (size_t)i * E, b, (int)E, i, ls, &launches))) return rc;
     }
-    if (lanes && (rc = join(s))) return rc;
+    if (lanes && (rc = d.join(s))) return rc;
     h->last_launches = launches;
     return XVB_OK;
   }
@@ -121,55 +128,61 @@ struct Shard {
   // The same through host buffers (pinned, so that the copies are asynchronous): batch k's features cross the link on
   // the copy stream into slot k % kSlots while earlier batches run, its embeddings go back on its lane's stream.  Slot
   // reuse is ordered by events on the device; returns when all of emb_host is written.
-  int host(H* h, const float* feats_host, int64_t N, int T, int batch, float* emb_host, void* stream, bool single_lane,
-           const char* fn) {
-    XVB_CHECK_ARG(!slot_busy[0] && !slot_busy[1], "%s: a submit_host slot is still in flight", fn);
+  static int host(H* h, const float* feats_host, int64_t N, int T, int batch, float* emb_host, void* stream,
+                  bool single_lane, const char* fn) {
+    XVB_CHECK_ARG(finalized(h) && feats_host && emb_host && N > 0 && T > 0 && batch > 0, "%s: bad arguments", fn);
+    Shard& d = h->shard;
+    XVB_CHECK_ARG(!d.slot_busy[0] && !d.slot_busy[1], "%s: a submit_host slot is still in flight", fn);
     const size_t Fd = F::feat_dim(h), E = F::embed_dim(h);
     const cudaStream_t s = (cudaStream_t)stream;
     const size_t bmax = (size_t)(N < batch ? N : batch);
     int rc;
-    if ((rc = ensure_copy_stream())) return rc;
+    if ((rc = d.ensure_copy_stream())) return rc;
     for (int slot = 0; slot < kSlots; ++slot)
-      if ((rc = reserve_slot(slot, bmax * T * Fd, bmax * E))) return rc;
+      if ((rc = d.reserve_slot(slot, bmax * T * Fd, bmax * E))) return rc;
     const bool lanes = two_lanes(N, batch, single_lane);
-    if (lanes && (rc = fork(h, s))) return rc;
+    if (lanes && (rc = d.fork(h, s))) return rc;
     int launches = 0, k = 0;
     for (int64_t i = 0; i < N; i += batch, ++k) {
       const int b = (int)(N - i < batch ? N - i : batch);
       const int slot = k % kSlots;
-      H* lane = (lanes && (k & 1)) ? lane1.get() : h;
-      const cudaStream_t ls = lanes ? lane_stream[k & 1] : s;
-      if (k >= kSlots) XVB_CUDA(cudaStreamWaitEvent(copy_stream, ev_done[slot], 0));   // batch k - kSlots has left the slot
-      XVB_CUDA(cudaMemcpyAsync(p_feats[slot].p, feats_host + (size_t)i * T * Fd, (size_t)b * T * Fd * sizeof(float),
-                               cudaMemcpyHostToDevice, copy_stream));
-      XVB_CUDA(cudaEventRecord(ev_h2d[slot], copy_stream));
-      XVB_CUDA(cudaStreamWaitEvent(ls, ev_h2d[slot], 0));
-      if ((rc = F::extract(lane, p_feats[slot].p, b, T, p_emb[slot].p, ls))) return rc;
+      H* lane = (lanes && (k & 1)) ? d.lane1.get() : h;
+      const cudaStream_t ls = lanes ? d.lane_stream[k & 1] : s;
+      if (k >= kSlots) XVB_CUDA(cudaStreamWaitEvent(d.copy_stream, d.ev_done[slot], 0));   // batch k - kSlots has left the slot
+      XVB_CUDA(cudaMemcpyAsync(d.p_feats[slot].p, feats_host + (size_t)i * T * Fd, (size_t)b * T * Fd * sizeof(float),
+                               cudaMemcpyHostToDevice, d.copy_stream));
+      XVB_CUDA(cudaEventRecord(d.ev_h2d[slot], d.copy_stream));
+      XVB_CUDA(cudaStreamWaitEvent(ls, d.ev_h2d[slot], 0));
+      if ((rc = F::extract(lane, d.p_feats[slot].p, b, T, d.p_emb[slot].p, ls))) return rc;
       launches += lane->last_launches;
-      if ((rc = scatter(p_emb[slot].p, b, (int)E, i, ls, &launches))) return rc;
-      XVB_CUDA(cudaMemcpyAsync(emb_host + (size_t)i * E, p_emb[slot].p, (size_t)b * E * sizeof(float), cudaMemcpyDeviceToHost, ls));
-      XVB_CUDA(cudaEventRecord(ev_done[slot], ls));
+      if ((rc = d.scatter(d.p_emb[slot].p, b, (int)E, i, ls, &launches))) return rc;
+      XVB_CUDA(cudaMemcpyAsync(emb_host + (size_t)i * E, d.p_emb[slot].p, (size_t)b * E * sizeof(float), cudaMemcpyDeviceToHost,
+                               ls));
+      XVB_CUDA(cudaEventRecord(d.ev_done[slot], ls));
     }
-    if (lanes && (rc = join(s))) return rc;
+    if (lanes && (rc = d.join(s))) return rc;
     XVB_CUDA(cudaStreamSynchronize(s));
     h->last_launches = launches;
     return XVB_OK;
   }
 
   // One batch into slot 0 or 1 without waiting: the H2D on the copy stream, the stack and the D2H on `stream`.
-  int submit(H* h, const float* feats_host, int B, int T, float* emb_host, int slot, void* stream, const char* fn) {
-    XVB_CHECK_ARG(!slot_busy[slot], "%s: slot %d still in flight (call the wait of this handle)", fn, slot);
+  static int submit(H* h, const float* feats_host, int B, int T, float* emb_host, int slot, void* stream, const char* fn) {
+    XVB_CHECK_ARG(finalized(h) && feats_host && emb_host && B > 0 && T > 0 && (slot == 0 || slot == 1),
+                  "%s: bad arguments (slot must be 0 or 1)", fn);
+    Shard& d = h->shard;
+    XVB_CHECK_ARG(!d.slot_busy[slot], "%s: slot %d still in flight (call the wait of this handle)", fn, slot);
     const cudaStream_t s = (cudaStream_t)stream;
     const size_t nf = (size_t)B * T * F::feat_dim(h), ne = (size_t)B * F::embed_dim(h);
     int rc;
-    if ((rc = ensure_copy_stream()) || (rc = reserve_slot(slot, nf, ne))) return rc;
-    XVB_CUDA(cudaMemcpyAsync(p_feats[slot].p, feats_host, nf * sizeof(float), cudaMemcpyHostToDevice, copy_stream));
-    XVB_CUDA(cudaEventRecord(ev_h2d[slot], copy_stream));
-    XVB_CUDA(cudaStreamWaitEvent(s, ev_h2d[slot], 0));
-    if ((rc = F::extract(h, p_feats[slot].p, B, T, p_emb[slot].p, stream))) return rc;
-    XVB_CUDA(cudaMemcpyAsync(emb_host, p_emb[slot].p, ne * sizeof(float), cudaMemcpyDeviceToHost, s));
-    XVB_CUDA(cudaEventRecord(ev_done[slot], s));
-    slot_busy[slot] = true;
+    if ((rc = d.ensure_copy_stream()) || (rc = d.reserve_slot(slot, nf, ne))) return rc;
+    XVB_CUDA(cudaMemcpyAsync(d.p_feats[slot].p, feats_host, nf * sizeof(float), cudaMemcpyHostToDevice, d.copy_stream));
+    XVB_CUDA(cudaEventRecord(d.ev_h2d[slot], d.copy_stream));
+    XVB_CUDA(cudaStreamWaitEvent(s, d.ev_h2d[slot], 0));
+    if ((rc = F::extract(h, d.p_feats[slot].p, B, T, d.p_emb[slot].p, stream))) return rc;
+    XVB_CUDA(cudaMemcpyAsync(emb_host, d.p_emb[slot].p, ne * sizeof(float), cudaMemcpyDeviceToHost, s));
+    XVB_CUDA(cudaEventRecord(d.ev_done[slot], s));
+    d.slot_busy[slot] = true;
     return XVB_OK;
   }
 
