@@ -113,6 +113,7 @@ SIGNATURES = {
     "xvb_plane_mean": (_i, [_p, _p, _i64, _i, _i, _i, _p, _p, _p, _i64, _p]),
     "xvb_plane_mean_lengths": (_i, [_p, _p, _i64, _i, _i, _i, _p, _i, _p, _p, _p, _i64, _p]),
     "xvb_res2net_block": (_i, [_p, _p, _i64, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _i, _i, _p]),
+    "xvb_res2net_block_ex": (_i, [_p, _p, _i64, _p, _p, _p, _p, _p, _i, _i, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_copy_rows": (_i, [_p, _i64, _p, _i64, _i64, _i64, _p]),
     "xvb_se_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_attn_stats_pool": (_i, [_p, _i64, _p, _i64, _i, _i, _i, _f, _p, _p, _p, _i64, _p]),

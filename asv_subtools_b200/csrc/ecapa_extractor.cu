@@ -113,7 +113,9 @@ extern "C" int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, i
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(out && feat_dim > 0 && channels > 0 && mfa_dim > 0 && att_hidden > 0 && embed_dim > 0, "xvb_ecapa_create: bad arguments");
-  XVB_CHECK_ARG(channels % 64 == 0 && channels / 8 == 128, "xvb_ecapa_create: the Res2Net chain kernel is built for scale 8 x width 128 (channels = 1024), got %d", channels);
+  XVB_CHECK_ARG(channels == 8 * 64 || channels == 8 * 128,
+                "xvb_ecapa_create: the Res2Net chain kernel is built for scale 8 x width 64 or 128 (channels = 512 or 1024), got %d",
+                channels);
   XVB_CHECK_ARG(mfa_dim % 8 == 0 && att_hidden % 8 == 0 && embed_dim % 4 == 0, "xvb_ecapa_create: mfa_dim/att_hidden must be multiples of 8, embed_dim of 4");
   xvb_ecapa* h = new xvb_ecapa();
   Model* m = h->draft;
@@ -407,8 +409,8 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
     const std::string p = "layer" + std::to_string(b + 2) + ".";
     r = Run{}; r.B = B; r.T = T; r.L = L(p + "bn1"); r.x = cur; r.y = h->Hh;
     if ((rc = launch(r, stream))) return rc;
-    if ((rc = xvb_res2net_block(h->Hh.hi, h->Hh.lo, C, m->res_w[b].hi, m->res_w[b].lo, m->res_bias[b], m->res_scale[b],
-                                m->res_shift[b], m->dilation[b], m->scale, h->R.hi, h->R.lo, C, B, T, stream)))
+    if ((rc = xvb_res2net_block_ex(h->Hh.hi, h->Hh.lo, C, m->res_w[b].hi, m->res_w[b].lo, m->res_bias[b], m->res_scale[b],
+                                   m->res_shift[b], m->dilation[b], m->scale, h->R.hi, h->R.lo, C, B, T, C / m->scale, stream)))
       return rc;
     r = Run{}; r.B = B; r.T = T; r.L = L(p + "bn2"); r.x = h->R; r.y = h->Z;
     if ((rc = launch(r, stream))) return rc;

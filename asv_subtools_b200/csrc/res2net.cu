@@ -13,198 +13,25 @@
 // step i-1: the only synchronisation is CTA-local (the consumers fence their stores, then release
 // the producer through an mbarrier), no grid-wide barrier and no extra launches.  Chunk 0 is copied
 // through by the consumer warps on the way.
-#include <cuda.h>
-#include <cuda_bf16.h>
-#include <cuda_runtime.h>
-
-#include "common.cuh"
-#include "ptx.cuh"
+#include "res2net.cuh"
 
 namespace xvb {
-
-constexpr int kRW = 128;                           // Res2Net width: channels per chunk = tile N
-constexpr int kRStages = 3;
-constexpr int kRABytes = 128 * 64 * 2;             // one plane of a 128-row x 64-channel A tile
-constexpr int kRBBytes = kRW * 64 * 2;             // one plane of the 128 x 64 weight tile
-constexpr int kRStageBytes = 2 * kRABytes + 2 * kRBBytes;   // 64 KB
-constexpr int kRConsumers = 256;                   // two warpgroups, 64 frames each
-constexpr int kRThreads = kRConsumers + 32;        // + the TMA producer warp
-constexpr int kRSmemBytes = kRStages * kRStageBytes + 1024 + 256;
-
-struct Res2Params {
-  int B, T, C;            // C = scale * 128 channels of the block input / output
-  int num_steps;          // scale - 1 (= 7)
-  int dilation;
-  int num_m;              // ceil(T / 128)
-  const float* bias;      // [num_steps][128]
-  const float* scale;
-  const float* shift;
-  const __nv_bfloat16* x_hi;   // block input planes (B,T,ldx): chunk 0 is passed through
-  const __nv_bfloat16* x_lo;
-  __nv_bfloat16* y_hi;         // block output planes (B,T,ldy)
-  __nv_bfloat16* y_lo;
-  long long ldx, ldy;
-};
-
-__global__ void __launch_bounds__(kRThreads, 1)
-res2net_chain_kernel(const __grid_constant__ CUtensorMap map_x_hi, const __grid_constant__ CUtensorMap map_x_lo,
-                     const __grid_constant__ CUtensorMap map_yin_hi, const __grid_constant__ CUtensorMap map_yin_lo,
-                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                     const __grid_constant__ Res2Params p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kRStages * kRStageBytes);
-  uint64_t* empty_bar = full_bar + kRStages;
-  uint64_t* step_bar = empty_bar + kRStages;      // completes once per step: that step's outputs are in global memory
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int producer_warp = kRConsumers / 32;
-  if (warp == producer_warp && lane == 0) {
-    tma_prefetch_desc(&map_x_hi); tma_prefetch_desc(&map_x_lo);
-    tma_prefetch_desc(&map_yin_hi); tma_prefetch_desc(&map_yin_lo);
-    tma_prefetch_desc(&map_w_hi); tma_prefetch_desc(&map_w_lo);
-    for (int i = 0; i < kRStages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kRConsumers / 32); }
-    mbar_init(step_bar, 1);
-    fence_barrier_init();
-  }
-  __syncthreads();
-  const int d = p.dilation;
-
-  if (warp == producer_warp) {
-    // ================================ TMA producer ================================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0, steps_done = 0;   // number of completed step_bar phases this thread has consumed
-      for (int b = blockIdx.x; b < p.B; b += gridDim.x) {
-        for (int st = 0; st < p.num_steps; ++st) {
-          for (int m = 0; m < p.num_m; ++m) {
-            const int t0 = m * 128;
-            for (int src = 0; src < (st == 0 ? 1 : 2); ++src) {
-              if (src == 1 && m == 0) {
-                // outputs of step st-1 (all tiles of this utterance) must have landed before we read them back
-                mbar_wait(step_bar, steps_done & 1);
-                ++steps_done;
-                asm volatile("fence.proxy.async;" ::: "memory");
-              }
-              const CUtensorMap* mh = src == 0 ? &map_x_hi : &map_yin_hi;
-              const CUtensorMap* ml = src == 0 ? &map_x_lo : &map_yin_lo;
-              const int cbase = src == 0 ? (st + 1) * kRW : st * kRW;   // chunk st+1 of x, chunk st of y
-              for (int tap = 0; tap < 3; ++tap) {
-                const int tt = t0 + (tap - 1) * d;
-                for (int cb = 0; cb < 2; ++cb) {
-                  mbar_wait(&empty_bar[stage], phase ^ 1);
-                  uint8_t* s = smem + stage * kRStageBytes;
-                  mbar_expect_tx(&full_bar[stage], kRStageBytes);
-                  tma_load_3d(s, mh, &full_bar[stage], cbase + cb * 64, tt, b);
-                  tma_load_3d(s + kRABytes, ml, &full_bar[stage], cbase + cb * 64, tt, b);
-                  const int kw = tap * kRW + cb * 64;
-                  tma_load_2d(s + 2 * kRABytes, &map_w_hi, &full_bar[stage], kw, st * kRW);
-                  tma_load_2d(s + 2 * kRABytes + kRBBytes, &map_w_lo, &full_bar[stage], kw, st * kRW);
-                  if (++stage == kRStages) { stage = 0; phase ^= 1; }
-                }
-              }
-            }
-          }
-        }
-        // the consumers also release the last step of an utterance; consume that phase too so the parity
-        // bookkeeping stays in step
-        mbar_wait(step_bar, steps_done & 1);
-        ++steps_done;
-      }
-    }
-    return;
-  }
-
-  // ================================ consumers: wgmma + epilogue ================================
-  const int wg = warp >> 2, q4 = lane & 3;
-  const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // this thread's frames: t0 + row0 and t0 + row0 + 8
-  const int etid = threadIdx.x;
-  float acc[kRW / 2];
-#pragma unroll
-  for (int i = 0; i < kRW / 2; ++i) acc[i] = 0.f;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int b = blockIdx.x; b < p.B; b += gridDim.x) {
-    // chunk 0 passes through (ecapa_tdnn_xvector.py:63-64): 16-byte vectors, 16 per row and plane
-    for (int i = etid; i < p.T * 16 * 2; i += kRConsumers) {
-      const int plane = i / (p.T * 16), r = (i % (p.T * 16)) >> 4, v = i & 15;
-      const __nv_bfloat16* src = (plane ? p.x_lo : p.x_hi) + ((long long)b * p.T + r) * p.ldx + v * 8;
-      __nv_bfloat16* dst = (plane ? p.y_lo : p.y_hi) + ((long long)b * p.T + r) * p.ldy + v * 8;
-      *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(src);
-    }
-    for (int st = 0; st < p.num_steps; ++st) {
-      const int nkb = (st == 0 ? 1 : 2) * 6;
-      for (int m = 0; m < p.num_m; ++m) {
-        int prev_stage = -1;
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint32_t sa = smem_u32(smem + stage * kRStageBytes);
-          const uint64_t m_off = (uint64_t)((wg * 64 * 128) >> 4);
-          const uint64_t da_hi = make_sw128_desc(sa) + m_off, da_lo = make_sw128_desc(sa + kRABytes) + m_off;
-          const uint64_t db_hi = make_sw128_desc(sa + 2 * kRABytes);
-          const uint64_t db_lo = make_sw128_desc(sa + 2 * kRABytes + kRBBytes);
-          wgmma_fence();
-#pragma unroll
-          for (int s = 0; s < 4; ++s) {
-            const uint64_t koff = (uint64_t)(s * 32 >> 4);
-            wgmma_bf16<kRW>(acc, da_lo + koff, db_hi + koff, (kb | s) ? 1u : 0u);
-            wgmma_bf16<kRW>(acc, da_hi + koff, db_lo + koff, 1);
-            wgmma_bf16<kRW>(acc, da_hi + koff, db_hi + koff, 1);
-          }
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-          prev_stage = stage;
-          if (++stage == kRStages) { stage = 0; phase ^= 1; }
-        }
-        wgmma_wait<0>();
-        wgmma_fence_operands(acc);
-        if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        // epilogue: +bias -> ReLU -> BN -> split -> output chunk st+1
-        const int t0 = m * 128;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int t = t0 + row0 + 8 * h;
-          if (t >= p.T) continue;
-          __nv_bfloat16* yh = p.y_hi + ((long long)b * p.T + t) * p.ldy + (st + 1) * kRW;
-          __nv_bfloat16* yl = p.y_lo + ((long long)b * p.T + t) * p.ldy + (st + 1) * kRW;
-#pragma unroll
-          for (int i = 0; i < kRW / 8; ++i) {
-            const int c = 8 * i + 2 * q4;
-            const int pc = st * kRW + c;
-            const float f0 = fmaf(fmaxf(acc[4 * i + 2 * h] + __ldg(p.bias + pc), 0.f), __ldg(p.scale + pc), __ldg(p.shift + pc));
-            const float f1 = fmaf(fmaxf(acc[4 * i + 2 * h + 1] + __ldg(p.bias + pc + 1), 0.f), __ldg(p.scale + pc + 1),
-                                  __ldg(p.shift + pc + 1));
-            __nv_bfloat16 h0, l0, h1, l1;
-            split_bf16(f0, h0, l0);
-            split_bf16(f1, h1, l1);
-            *reinterpret_cast<uint32_t*>(yh + c) = pack_bf16x2(h0, h1);
-            *reinterpret_cast<uint32_t*>(yl + c) = pack_bf16x2(l0, l1);
-          }
-        }
-      }
-      // step finished: make this step's stores visible to the producer's TMA reads, then release it
-      __threadfence_block();
-      asm volatile("fence.proxy.async;" ::: "memory");
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (etid == 0) mbar_arrive(step_bar);
-    }
-  }
-}
-
+template int launch_chain<128>(const Res2Params&, const uint16_t*, const uint16_t*, int64_t, const uint16_t*, const uint16_t*,
+                               uint16_t*, uint16_t*, int64_t, int, cudaStream_t);
 }  // namespace xvb
 
 using namespace xvb;
 
-extern "C" int xvb_res2net_block(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, const uint16_t* w_hi,
-                                 const uint16_t* w_lo, const float* bias, const float* bn_scale, const float* bn_shift,
-                                 int dilation, int scale, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, int B, int T,
-                                 void* stream) {
+extern "C" int xvb_res2net_block_ex(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, const uint16_t* w_hi,
+                                    const uint16_t* w_lo, const float* bias, const float* bn_scale, const float* bn_shift,
+                                    int dilation, int scale, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, int B, int T,
+                                    int width, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
+  XVB_CHECK_ARG(width == 64 || width == 128, "xvb_res2net_block: the chain kernel is built for widths 64 and 128, got %d", width);
   XVB_CHECK_ARG(x_hi && x_lo && w_hi && w_lo && bias && bn_scale && bn_shift && y_hi && y_lo, "xvb_res2net_block: null pointer");
   XVB_CHECK_ARG(B > 0 && T > 0 && scale >= 2 && scale <= 16 && dilation >= 1, "xvb_res2net_block: bad shape");
-  const int C = scale * kRW;
+  const int C = scale * width;
   XVB_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0 && ldx >= C && ldy >= C, "xvb_res2net_block: pitches must be >= %d and multiples of 8", C);
   XVB_CHECK_ARG(((uintptr_t)x_hi | (uintptr_t)x_lo | (uintptr_t)y_hi | (uintptr_t)y_lo | (uintptr_t)w_hi | (uintptr_t)w_lo) % 16 == 0,
                 "xvb_res2net_block: pointers must be 16-byte aligned");
@@ -215,23 +42,14 @@ extern "C" int xvb_res2net_block(const uint16_t* x_hi, const uint16_t* x_lo, int
   p.x_hi = reinterpret_cast<const __nv_bfloat16*>(x_hi); p.x_lo = reinterpret_cast<const __nv_bfloat16*>(x_lo);
   p.y_hi = reinterpret_cast<__nv_bfloat16*>(y_hi); p.y_lo = reinterpret_cast<__nv_bfloat16*>(y_lo);
   p.ldx = ldx; p.ldy = ldy;
-  CUtensorMap mx_hi, mx_lo, myi_hi, myi_lo, mw_hi, mw_lo;
-  const unsigned long long dx[3] = {(unsigned long long)C, (unsigned long long)T, (unsigned long long)B};
-  const unsigned long long sx[2] = {(unsigned long long)ldx * 2, (unsigned long long)ldx * 2 * T};
-  const unsigned long long sy[2] = {(unsigned long long)ldy * 2, (unsigned long long)ldy * 2 * T};
-  const unsigned box_a[3] = {64u, 128u, 1u};
-  if ((rc = make_tensor_map(&mx_hi, x_hi, 2, 3, dx, sx, box_a, 128))) return rc;
-  if ((rc = make_tensor_map(&mx_lo, x_lo, 2, 3, dx, sx, box_a, 128))) return rc;
-  if ((rc = make_tensor_map(&myi_hi, y_hi, 2, 3, dx, sy, box_a, 128))) return rc;
-  if ((rc = make_tensor_map(&myi_lo, y_lo, 2, 3, dx, sy, box_a, 128))) return rc;
-  const unsigned long long dw[2] = {(unsigned long long)3 * kRW, (unsigned long long)(scale - 1) * kRW};
-  const unsigned long long sw[1] = {(unsigned long long)3 * kRW * 2};
-  const unsigned box_w[2] = {64u, (unsigned)kRW};
-  if ((rc = make_tensor_map(&mw_hi, w_hi, 2, 2, dw, sw, box_w, 128))) return rc;
-  if ((rc = make_tensor_map(&mw_lo, w_lo, 2, 2, dw, sw, box_w, 128))) return rc;
-  XVB_ENSURE_DYN_SMEM((res2net_chain_kernel), kRSmemBytes);
-  const int grid = B < sm_count() ? B : sm_count();
-  res2net_chain_kernel<<<grid, kRThreads, kRSmemBytes, (cudaStream_t)stream>>>(mx_hi, mx_lo, myi_hi, myi_lo, mw_hi, mw_lo, p);
-  XVB_LAUNCH_CHECK();
-  return XVB_OK;
+  return width == 128 ? launch_chain<128>(p, x_hi, x_lo, ldx, w_hi, w_lo, y_hi, y_lo, ldy, scale, (cudaStream_t)stream)
+                      : launch_chain<64>(p, x_hi, x_lo, ldx, w_hi, w_lo, y_hi, y_lo, ldy, scale, (cudaStream_t)stream);
+}
+
+extern "C" int xvb_res2net_block(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, const uint16_t* w_hi,
+                                 const uint16_t* w_lo, const float* bias, const float* bn_scale, const float* bn_shift,
+                                 int dilation, int scale, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, int B, int T,
+                                 void* stream) {
+  return xvb_res2net_block_ex(x_hi, x_lo, ldx, w_hi, w_lo, bias, bn_scale, bn_shift, dilation, scale, y_hi, y_lo, ldy, B, T,
+                              128, stream);
 }

@@ -145,7 +145,7 @@ class ECAPA_TDNN(TopVirtualNnet):
         elif self.extracted_embedding not in ("near", "near_affine"):
             raise TypeError("Expected far or near position, but got {}".format(self.extracted_embedding))
         dev = self.device_for_extraction()
-        if os.environ.get("XVB_ECAPA_NATIVE", "1") == "0" or self.layer1.affine.output_dim != 1024:
+        if os.environ.get("XVB_ECAPA_NATIVE", "1") == "0" or self.layer1.affine.output_dim not in NATIVE_CHANNELS:
             return EcapaExtractor(self, dev)       # op-by-op twin; also the path for other channel counts
         return NativeEcapaExtractor(self, dev)
 
@@ -222,6 +222,9 @@ def _mqmha_attention(st):
     return out
 
 
+# channel counts the native extractor and the Res2Net chain kernel take: scale 8 x width 64 (C512) or 128 (C1024)
+NATIVE_CHANNELS = (512, 1024)
+CHAIN_WIDTHS = (64, 128)
 _PROFILE = None  # list of (label, cuda event) when profiling (tools/bench_ecapa.py --profile)
 SMALL_ROWS = os.environ.get("XVB_ECAPA_SMALL", "1") != "0"   # segment-level layers on CUDA cores (csrc/ecapa.cu small_affine)
 
@@ -392,9 +395,9 @@ class EcapaExtractor:
         for li, blk in enumerate(self.blocks):
             w = blk["width"]
             blk["bn1"].run(cur, y=H)
-            if self.chain and w == 128:
+            if self.chain and w in CHAIN_WIDTHS:
                 ops.res2net_block(H, blk["res_w_hi"], blk["res_w_lo"], blk["res_bias"], blk["res_scale"], blk["res_shift"],
-                                  blk["dilation"], blk["nscale"], R)
+                                  blk["dilation"], blk["nscale"], R, width=w)
                 _mark("res2net chain kernel")
             else:
                 ops.copy_planes(H.slice(0, w), R.slice(0, w))   # chunk 0 passes through (ecapa_tdnn_xvector.py:63-64)

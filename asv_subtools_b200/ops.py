@@ -183,12 +183,12 @@ def plane_mean(x, planes=True, lengths=None, rows_per_length=1):
     return out, op
 
 
-def res2net_block(x, w_hi, w_lo, bias, scale, shift, dilation, nscale, y):
-    """One-kernel Res2Net block: x, y SplitPlanes (B,T,nscale*128); stacked packed weights/params."""
+def res2net_block(x, w_hi, w_lo, bias, scale, shift, dilation, nscale, y, width=128):
+    """One-kernel Res2Net block: x, y SplitPlanes (B,T,nscale*width), width 64 or 128; stacked packed weights/params."""
     b, t = x.hi.shape[0], x.hi.shape[1]
-    check(lib.xvb_res2net_block(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, _ptr(w_hi), _ptr(w_lo), _ptr(bias), _ptr(scale),
-                                _ptr(shift), int(dilation), int(nscale), y.hi.data_ptr(), y.lo.data_ptr(), y.ld, b, t,
-                                _stream()), "xvb_res2net_block")
+    check(lib.xvb_res2net_block_ex(x.hi.data_ptr(), x.lo.data_ptr(), x.ld, _ptr(w_hi), _ptr(w_lo), _ptr(bias), _ptr(scale),
+                                   _ptr(shift), int(dilation), int(nscale), y.hi.data_ptr(), y.lo.data_ptr(), y.ld, b, t,
+                                   int(width), _stream()), "xvb_res2net_block_ex")
 
 
 def copy_planes(src, dst):

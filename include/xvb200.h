@@ -205,6 +205,12 @@ int xvb_plane_mean_lengths(const uint16_t* x_hi, const uint16_t* x_lo, int64_t l
 int xvb_res2net_block(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, const uint16_t* w_hi, const uint16_t* w_lo,
                       const float* bias, const float* bn_scale, const float* bn_shift, int dilation, int scale,
                       uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, int B, int T, void* stream);
+/* The same block at Res2Net width `width` (channels per chunk), 64 or 128: x, y are (B,T,scale*width) with
+ * ldx, ldy >= scale*width, the packed weights are each (width, 3*width) and the parameters (scale-1, width).
+ * Any other width returns XVB_EINVAL with nothing launched.  xvb_res2net_block is width 128. */
+int xvb_res2net_block_ex(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, const uint16_t* w_hi, const uint16_t* w_lo,
+                         const float* bias, const float* bn_scale, const float* bn_shift, int dilation, int scale,
+                         uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, int B, int T, int width, void* stream);
 
 /* Strided row copy (16-byte granularity): the pass-through of Res2Net's first chunk
  * (ecapa_tdnn_xvector.py:63-64) between two channel-slice views. */
@@ -721,11 +727,12 @@ void xvb_fbank_destroy(xvb_fbank_t* h);
  * :403-426; canonical c1024 parameters runEcapaXvector_online.py:221-263).  Layers are set by name with the
  * weights as the state_dict stores them (host fp32 (Cout, Cin, tot_context); eval BatchNorm folded to
  * scale/shift; flags XVB_RELU | XVB_BN):
- *   "layer1"; for L in 2..4: "layerL.bn1", "layerL.res0".."layerL.res6" (128 -> 128, [-d,0,d]),
+ *   "layer1"; for L in 2..4: "layerL.bn1", "layerL.res0".."layerL.res6" (W -> W, [-d,0,d], W = channels / 8),
  *   "layerL.bn2", "layerL.se1" (ReLU), "layerL.se2"; "mfa"; "att_x" = the first attention conv's columns
  *   over x with its ReLU + BatchNorm, "att_gs" = its columns over [mean | std] plus its bias (:179),
  *   "att2"; "fc2" with bn_stats folded into the weight (and fc2's own BatchNorm for position "near").
- * channels must be 1024 (Res2Net scale 8 x width 128, the chain kernel's shape).
+ * channels must be 512 or 1024 (Res2Net scale 8 x width 64 or 128, the chain kernel's two instances: ECAPA C512
+ * and C1024).
  * ------------------------------------------------------------------------------------------- */
 typedef struct xvb_ecapa xvb_ecapa_t;
 int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, int mfa_dim, int att_hidden, int embed_dim);

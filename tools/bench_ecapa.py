@@ -2,6 +2,9 @@
 """ECAPA-TDNN c1024 throughput (BASELINE configs[2]: 80-d fbank, 300-frame chunks, batch 128) --
 a side measurement, not the bench.py contract line.
 
+--channels 512: the C512 model (ecapa_params={"channels": 512}, Res2Net width 64) instead; the default, 1024, keeps the
+c1024 line.  XVB_ECAPA_NATIVE=0 / XVB_ECAPA_RES2NET=gemm select the twin / its per-scale GEMMs as for the c1024 model.
+
 --pooling mqmha: the roadmap launcher's model (runEcapaXvector_roadmap.py:220-250: MQMHASP 2 queries x 2 heads, hidden
 64, share=False, time attention) next to the attentive-pooling model in the same call, and CUDA-event times of its two
 attention GEMMs in the layer kernel's grouped mode against their block-diagonal expansions."""
@@ -93,13 +96,24 @@ def main_mqmha(steps):
     print(json.dumps(res))
 
 
+def macs_per_frame(C, F=80, D=1536, H=128):
+    """Contraction MACs per frame from the shapes: layer1 (5 taps), per block bn1 + 7 Res2Net steps (3 taps, width C/8)
+    + bn2, mfa, the two attention convs (the per-utterance SE and segment layers are left out)."""
+    W = C // 8
+    return 5 * F * C + 3 * (2 * C * C + 7 * 3 * W * W) + 3 * C * D + 2 * D * H
+
+
 def main():
     B, T, F = 128, 300, 80
     steps = int(sys.argv[1]) if len(sys.argv) > 1 and sys.argv[1].isdigit() else 10
     if "--pooling" in sys.argv and sys.argv[sys.argv.index("--pooling") + 1] == "mqmha":
         return main_mqmha(steps)
-    m = ECAPA_TDNN(F, 10, **CANON)
-    m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F), 201), strict=True)
+    channels = int(sys.argv[sys.argv.index("--channels") + 1]) if "--channels" in sys.argv else 1024
+    if channels not in (512, 1024):
+        raise SystemExit("--channels takes 512 or 1024")
+    kw = dict(CANON, ecapa_params=dict(CANON["ecapa_params"], channels=channels))
+    m = ECAPA_TDNN(F, 10, **kw)
+    m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F, channels=channels), 201), strict=True)
     m.cuda().eval()
     if "--profile" in sys.argv:
         os.environ["XVB_ECAPA_NATIVE"] = "0"   # per-op CUDA events live in the op-by-op Python twin
@@ -115,7 +129,7 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / steps
-    flop = 25701908 * B * T  # SURVEY 8(d)
+    flop = (25701908 if channels == 1024 else 2 * macs_per_frame(channels)) * B * T  # c1024: SURVEY 8(d)
     if "--profile" in sys.argv:
         import collections
         from asv_subtools_b200.model import ecapa_tdnn_xvector as mod
@@ -135,7 +149,7 @@ def main():
             tot += per_call * n
             print("%-28s x%-3d %8.1f us each %9.1f us total" % (k, n, per_call * 1e3, per_call * n * 1e3))
         print("sum %.1f us" % (tot * 1e3))
-    print(json.dumps({"workload": "ECAPA-TDNN c1024, 80-d fbank, 300-frame chunks, batch 128",
+    print(json.dumps({"workload": "ECAPA-TDNN c{}, 80-d fbank, 300-frame chunks, batch 128".format(channels),
                       "ms_per_step": ms, "frames_per_s": B * T / (ms * 1e-3),
                       "algorithmic_tflops": flop / (ms * 1e-3) / 1e12, "finite": bool(torch.isfinite(out).all()),
                       "extractor": type(ex).__name__, "launches": getattr(ex, "last_launches", None)}))
