@@ -254,6 +254,7 @@ SIGNATURES = {
     "xvb_campp_destroy": (None, [_p]),
     "xvb_campp_chunk_sizes": (_i, [_i, _i, _ip, _i]),
     "xvb_extractor_load": (_i, [C.POINTER(_p), C.c_char_p]),
+    "xvb_extractor_save": (_i, [_p, C.c_char_p]),
     "xvb_extractor_feat_dim": (_i, [C.c_char_p]),
     "xvb_ark_reader_open": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_ark_reader_next": (_i, [_p, C.POINTER(C.c_char_p), _ip, _ip, C.POINTER(C.POINTER(C.c_float))]),

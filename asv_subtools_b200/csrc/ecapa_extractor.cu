@@ -14,13 +14,12 @@
 // Layers are handed over by NAME with the weights as the state_dict stores them (host fp32, eval BatchNorm
 // folded to scale/shift by the caller); the two derived layers of the attention conv ("att_x": its columns
 // over x, "att_gs": its columns over [mean | std] plus the bias) and "fc2" (bn_stats folded into its weight)
-// are prepared by the caller -- see EcapaExtractor.save() / the Python blueprint.
+// are prepared by the caller -- see the Python blueprint.  The handle keeps the layers as handed over and builds the
+// model from them at finalize; xvb_ecapa_save writes them back (the XVBE0001 / XVBE0002 layouts are in model_file.cpp).
 #include <cuda_runtime.h>
-#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -33,20 +32,23 @@ namespace {
 
 using namespace xvb;
 
-struct ELayer {
-  int Cin = 0, Cout = 0, ntaps = 0, flags = 0, tot = 0;
-  int ctx[XVB_MAX_TAPS] = {0};
-  Planes w;
-  float* bias = nullptr;
-  float* scale = nullptr;
-  float* shift = nullptr;
+struct ELayer : TapLayer {
   float* w_f32 = nullptr;   // (Cout, Cin) fp32 as stored, kept for one-tap layers: the segment-level ones run on CUDA cores
   // grouped 1x1 conv (the MQMHA attention convs): Cin is the per-group width; packed compactly for the layer kernel's
   // grouped mode, or as the block-diagonal expansion (expanded) when the shape does not fit that mode
   int groups = 1;
   bool expanded = false;
-  // host copies for save()
-  std::vector<float> hw, hb, hs, ht;
+};
+
+// One SE-Res2Net block ("layer2." .. "layer4."): its 1x1 convs and SE gate, and its scale - 1 Res2Net convs ("res0" ..)
+// stacked for the chain kernel, packed weights along rows and parameters back to back.
+struct Block {
+  ELayer bn1, bn2, se1, se2;
+  Planes res_w;
+  float* res_bias = nullptr;
+  float* res_scale = nullptr;
+  float* res_shift = nullptr;
+  int dilation = 0;
 };
 
 // split planes with their row pitch
@@ -57,25 +59,26 @@ struct View {
   View slice(int c0) const { return View{hi + c0, lo + c0, ld}; }
 };
 
-// The layers and what finalize fixes; shared read-only by a handle and its second shard lane once finalized.
-struct Model {
-  int feat_dim = 0, ldf = 0, C = 0, D = 0, H = 0, E = 0, scale = 8, se_dim = 0;
-  int dilation[3] = {2, 3, 4};
-  std::map<std::string, ELayer> layers;
-  std::vector<std::string> order;   // insertion order, for save()
-  // stacked Res2Net parameters per block
-  Planes res_w[3];
-  float* res_bias[3] = {nullptr, nullptr, nullptr};
-  float* res_scale[3] = {nullptr, nullptr, nullptr};
-  float* res_shift[3] = {nullptr, nullptr, nullptr};
-  int fc1_dim = 0;
+struct Config {
+  int feat_dim = 0, ldf = 0, C = 0, D = 0, H = 0, E = 0, scale = 8;
   // multi-query multi-head attention pooling (xvb_ecapa_set_mqmha); mq == 0: ECAPA's own attentive pooling
   int mq = 0, mq_heads = 1, mq_q = 1, mq_hidden = 0, mq_share = 0, mq_layers = 2, mq_tatt = 1, mq_stddev = 1;
   // widths derived from the pooling: att_x outputs AX, the logits NL (row pitch ldlog), the pooled statistics P of the
   // P2-wide [mean | std] buffer (default model: AX = H, NL = D, P = P2 = 2D)
   int AX = 0, NL = 0, ldlog = 0, P = 0, P2 = 0;
+};
+
+// The layers and what finalize fixes; shared read-only by a handle and its second shard lane once finalized.
+struct Model {
+  Config cfg;
+  std::vector<TapRec> recs;   // as handed over, in order
+  // built at finalize, by role; a layer that the configuration does without has Cout 0
+  ELayer layer1;
+  Block blocks[3];
+  ELayer mfa, att_x, att_gs, att2, fc1, fc2;
+  int se_dim = 0, fc1_dim = 0;
   Im2col im2col;   // layer1 as an im2col view (records.cuh)
-  Weights dev{"xvb_ecapa_set_layer"};
+  Weights dev{"xvb_ecapa_finalize"};
 };
 
 }  // namespace
@@ -105,8 +108,8 @@ struct xvb::ShardFamily<xvb_ecapa> {
     return xvb_ecapa_extract(h, feats, B, T, emb, stream);
   }
   static xvb_ecapa* twin(const xvb_ecapa* h) { return new xvb_ecapa(h->m); }
-  static int feat_dim(const xvb_ecapa* h) { return h->m->feat_dim; }
-  static int embed_dim(const xvb_ecapa* h) { return h->m->E; }
+  static int feat_dim(const xvb_ecapa* h) { return h->m->cfg.feat_dim; }
+  static int embed_dim(const xvb_ecapa* h) { return h->m->cfg.E; }
 };
 
 extern "C" int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, int mfa_dim, int att_hidden, int embed_dim) {
@@ -119,40 +122,46 @@ extern "C" int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, i
   XVB_CHECK_ARG(mfa_dim % 8 == 0 && att_hidden % 8 == 0 && embed_dim % 4 == 0, "xvb_ecapa_create: mfa_dim/att_hidden must be multiples of 8, embed_dim of 4");
   xvb_ecapa* h = new xvb_ecapa();
   Model* m = h->draft;
-  m->feat_dim = feat_dim; m->ldf = (int)round_up(feat_dim, 8);
-  m->C = channels; m->D = mfa_dim; m->H = att_hidden; m->E = embed_dim;
-  m->AX = att_hidden; m->NL = mfa_dim; m->ldlog = mfa_dim; m->P = 2 * mfa_dim; m->P2 = 2 * mfa_dim;
+  m->cfg.feat_dim = feat_dim; m->cfg.ldf = (int)round_up(feat_dim, 8);
+  m->cfg.C = channels; m->cfg.D = mfa_dim; m->cfg.H = att_hidden; m->cfg.E = embed_dim;
+  m->cfg.AX = att_hidden; m->cfg.NL = mfa_dim; m->cfg.ldlog = mfa_dim; m->cfg.P = 2 * mfa_dim; m->cfg.P2 = 2 * mfa_dim;
   *out = h;
   return XVB_OK;
 }
 
 extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int share, int affine_layers,
                                    int time_attention, int stddev) {
-  XVB_CHECK_ARG(is_draft(h) && h->draft->layers.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
+  XVB_CHECK_ARG(is_draft(h) && h->draft->recs.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
   Model* m = h->draft;
-  XVB_CHECK_ARG(num_head >= 1 && num_q >= 1 && hidden >= 1 && (affine_layers == 1 || affine_layers == 2) && m->D % num_head == 0 &&
-                (m->D / num_head) % 4 == 0 && hidden * num_head * num_q == m->H,
+  XVB_CHECK_ARG(num_head >= 1 && num_q >= 1 && hidden >= 1 && (affine_layers == 1 || affine_layers == 2) && m->cfg.D % num_head == 0 &&
+                (m->cfg.D / num_head) % 4 == 0 && hidden * num_head * num_q == m->cfg.H,
                 "xvb_ecapa_set_mqmha: need %d channels in heads of a multiple of 4, 1 or 2 affine layers and att_hidden = "
-                "hidden * num_head * num_q (= %d)", m->D, m->H);
-  const int cg = m->D / num_head, hq = num_head * num_q;
-  m->mq = 1; m->mq_heads = num_head; m->mq_q = num_q; m->mq_hidden = hidden; m->mq_share = share ? 1 : 0;
-  m->mq_layers = affine_layers; m->mq_tatt = time_attention ? 1 : 0; m->mq_stddev = stddev ? 1 : 0;
-  m->NL = hq * (share ? 1 : cg);
-  m->ldlog = (int)round_up(m->NL, 4);
-  m->AX = affine_layers == 2 ? m->H : m->NL;
-  XVB_CHECK_ARG(!time_attention || m->AX % 4 == 0, "xvb_ecapa_set_mqmha: the time-constant columns of the first attention conv "
-                "become a per-utterance bias, which needs a multiple of 4 outputs (got %d)", m->AX);
-  m->P2 = 2 * num_q * m->D;
-  m->P = stddev ? m->P2 : num_q * m->D;
+                "hidden * num_head * num_q (= %d)", m->cfg.D, m->cfg.H);
+  const int cg = m->cfg.D / num_head, hq = num_head * num_q;
+  m->cfg.mq = 1; m->cfg.mq_heads = num_head; m->cfg.mq_q = num_q; m->cfg.mq_hidden = hidden; m->cfg.mq_share = share ? 1 : 0;
+  m->cfg.mq_layers = affine_layers; m->cfg.mq_tatt = time_attention ? 1 : 0; m->cfg.mq_stddev = stddev ? 1 : 0;
+  m->cfg.NL = hq * (share ? 1 : cg);
+  m->cfg.ldlog = (int)round_up(m->cfg.NL, 4);
+  m->cfg.AX = affine_layers == 2 ? m->cfg.H : m->cfg.NL;
+  XVB_CHECK_ARG(!time_attention || m->cfg.AX % 4 == 0, "xvb_ecapa_set_mqmha: the time-constant columns of the first attention conv "
+                "become a per-utterance bias, which needs a multiple of 4 outputs (got %d)", m->cfg.AX);
+  m->cfg.P2 = 2 * num_q * m->cfg.D;
+  m->cfg.P = stddev ? m->cfg.P2 : num_q * m->cfg.D;
   return XVB_OK;
 }
 
 // Groups of a layer as the state_dict stores it: the MQMHA attention convs are grouped (pooling.py:665-698)
-static int layer_groups(const Model* m, const std::string& n) {
-  if (!m->mq) return 1;
-  if (n == "att_x") return m->mq_heads;
-  if (n == "att2") return m->mq_heads * m->mq_q;
+static int layer_groups(const Config& c, const std::string& n) {
+  if (!c.mq) return 1;
+  if (n == "att_x") return c.mq_heads;
+  if (n == "att2") return c.mq_heads * c.mq_q;
   return 1;
+}
+
+static const TapRec* find(const std::vector<TapRec>& recs, const std::string& n) {
+  for (const TapRec& r : recs)
+    if (r.name == n) return &r;
+  return nullptr;
 }
 
 extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
@@ -162,133 +171,134 @@ extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, i
   Model* m = h->draft;
   XVB_CHECK_ARG(Cout > 0 && Cin > 0 && ntaps >= 1 && ntaps <= XVB_MAX_TAPS, "xvb_ecapa_set_layer(%s): bad shape", name);
   XVB_CHECK_ARG(!(flags & XVB_BN) || (bn_scale_host && bn_shift_host), "xvb_ecapa_set_layer(%s): XVB_BN without scale/shift", name);
-  XVB_CHECK_ARG(m->layers.find(name) == m->layers.end(), "xvb_ecapa_set_layer: layer '%s' set twice", name);
-  ELayer L;
-  L.Cin = Cin; L.Cout = Cout; L.ntaps = ntaps; L.flags = flags;
-  for (int i = 0; i < ntaps; ++i) L.ctx[i] = context_host[i];
-  const int left = L.ctx[0] < 0 ? L.ctx[0] : 0, right = L.ctx[ntaps - 1] > 0 ? L.ctx[ntaps - 1] : 0;
-  L.tot = right - left + 1;
-  const size_t wn = (size_t)Cout * Cin * L.tot;
-  L.hw.assign(w_host, w_host + wn);
-  if (bias_host) L.hb.assign(bias_host, bias_host + Cout);
-  if (flags & XVB_BN) { L.hs.assign(bn_scale_host, bn_scale_host + Cout); L.ht.assign(bn_shift_host, bn_shift_host + Cout); }
-  L.groups = layer_groups(m, name);
-  XVB_CHECK_ARG(L.groups == 1 || (ntaps == 1 && L.tot == 1 && Cout % L.groups == 0),
-                "xvb_ecapa_set_layer(%s): a grouped layer is a 1x1 conv with Cout divisible by its %d groups", name, L.groups);
-  // a grouped shape the layer kernel's grouped mode does not take runs as its block-diagonal expansion
-  L.expanded = L.groups > 1 && !xvb_tdnn_grouped_fits(Cin * L.groups, Cout, L.groups);
-  std::vector<float> dense;
-  int cin_pack = Cin;
-  if (L.expanded) {
-    const int G = L.groups, co = Cout / G;
-    cin_pack = Cin * G;
-    dense.assign((size_t)Cout * cin_pack, 0.f);
-    for (int n = 0; n < Cout; ++n)
-      memcpy(&dense[(size_t)n * cin_pack + (size_t)(n / co) * Cin], w_host + (size_t)n * Cin, Cin * sizeof(float));
-  }
-  int rc;
-  if ((rc = m->dev.pack(&L.w, L.expanded ? dense : L.hw, Cout, cin_pack, L.tot, L.ctx, ntaps))) return rc;
-  // one tap: (Cout, Cin, 1) is the (N, K) matrix xvb_small_affine takes
-  if (L.tot == 1 && Cin % 4 == 0 && L.groups == 1 && (rc = m->dev.upload(&L.w_f32, L.hw))) return rc;
-  if ((rc = m->dev.upload(&L.bias, L.hb)) || (rc = m->dev.upload(&L.scale, L.hs)) || (rc = m->dev.upload(&L.shift, L.ht))) return rc;
-  m->layers[name] = L;
-  m->order.push_back(name);
+  XVB_CHECK_ARG(!find(m->recs, name), "xvb_ecapa_set_layer: layer '%s' set twice", name);
+  TapRec r = tap_record(name, Cout, Cin, context_host, ntaps, w_host, bias_host, bn_scale_host, bn_shift_host, flags);
+  const int groups = layer_groups(m->cfg, name);
+  XVB_CHECK_ARG(groups == 1 || (ntaps == 1 && r.tot() == 1 && Cout % groups == 0),
+                "xvb_ecapa_set_layer(%s): a grouped layer is a 1x1 conv with Cout divisible by its %d groups", name, groups);
+  m->recs.push_back(std::move(r));
   return XVB_OK;
 }
 
-static const ELayer* find(const Model* m, const std::string& n) {
-  auto it = m->layers.find(n);
-  return it == m->layers.end() ? nullptr : &it->second;
+// r on the device as L.  A grouped shape the layer kernel's grouped mode does not take runs as its block-diagonal
+// expansion.
+static int build_layer(Model* m, const TapRec& r, ELayer* L) {
+  L->groups = layer_groups(m->cfg, r.name);
+  L->expanded = L->groups > 1 && !xvb_tdnn_grouped_fits(r.Cin * L->groups, r.Cout, L->groups);
+  std::vector<float> dense;
+  int cin_pack = r.Cin;
+  if (L->expanded) {
+    const int G = L->groups, co = r.Cout / G;
+    cin_pack = r.Cin * G;
+    dense.assign((size_t)r.Cout * cin_pack, 0.f);
+    for (int n = 0; n < r.Cout; ++n)
+      memcpy(&dense[(size_t)n * cin_pack + (size_t)(n / co) * r.Cin], &r.w[(size_t)n * r.Cin], r.Cin * sizeof(float));
+  }
+  int rc;
+  if ((rc = pack_tap(m->dev, r, L, L->expanded ? dense : r.w, cin_pack))) return rc;
+  // one tap: (Cout, Cin, 1) is the (N, K) matrix xvb_small_affine takes
+  if (r.tot() == 1 && r.Cin % 4 == 0 && L->groups == 1 && (rc = m->dev.upload(&L->w_f32, r.w))) return rc;
+  return XVB_OK;
 }
 
-extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
-  XVB_CHECK_ARG(is_draft(h), "xvb_ecapa_finalize: null or finalized model");
-  Model* m = h->draft;
-  const int C = m->C, W = C / m->scale;
-  auto need = [&](const std::string& n, int cin, int cout, int ntaps) -> int {
-    const ELayer* L = find(m, n);
+// The model of the draft's configuration and layers, each layer built into its role.
+static int build(Model* m, const std::vector<TapRec>& recs) {
+  const Config& c = m->cfg;
+  const int C = c.C, W = C / c.scale;
+  // *out: the layer n, which must have this shape
+  auto need = [&](const std::string& n, int cin, int cout, int ntaps, const TapRec** out) -> int {
+    const TapRec* L = *out = find(recs, n);
     XVB_CHECK_ARG(L, "xvb_ecapa_finalize: layer '%s' is missing", n.c_str());
     XVB_CHECK_ARG(L->Cin == cin && L->Cout == cout && L->ntaps == ntaps, "xvb_ecapa_finalize: layer '%s' is %d->%d x%d taps, expected %d->%d x%d",
                   n.c_str(), L->Cin, L->Cout, L->ntaps, cin, cout, ntaps);
     return XVB_OK;
   };
-  int rc;
-  rc = need("layer1", m->feat_dim, C, find(m, "layer1") ? find(m, "layer1")->ntaps : 5);
+  auto take = [&](const std::string& n, int cin, int cout, int ntaps, ELayer* L) -> int {
+    const TapRec* r;
+    const int rc = need(n, cin, cout, ntaps, &r);
+    return rc ? rc : build_layer(m, *r, L);
+  };
+  const TapRec* r = find(recs, "layer1");
+  int rc = take("layer1", c.feat_dim, C, r ? r->ntaps : 5, &m->layer1);
   if (rc) return rc;
   for (int b = 0; b < 3; ++b) {
+    Block& k = m->blocks[b];
     const std::string p = "layer" + std::to_string(b + 2) + ".";
-    if ((rc = need(p + "bn1", C, C, 1)) || (rc = need(p + "bn2", C, C, 1))) return rc;
-    const ELayer* se1 = find(m, p + "se1");
+    if ((rc = take(p + "bn1", C, C, 1, &k.bn1)) || (rc = take(p + "bn2", C, C, 1, &k.bn2))) return rc;
+    const TapRec* se1 = find(recs, p + "se1");
     XVB_CHECK_ARG(se1 && se1->Cin == C, "xvb_ecapa_finalize: layer '%sse1' is missing", p.c_str());
     if (b == 0) m->se_dim = se1->Cout;
     XVB_CHECK_ARG(se1->Cout == m->se_dim && m->se_dim % 8 == 0, "xvb_ecapa_finalize: SE bottleneck must be a multiple of 8 and equal in all blocks");
-    rc = need(p + "se2", m->se_dim, C, 1);
-    if (rc) return rc;
-    // stack the scale-1 Res2Net layers: packed weights along rows, parameters back to back
+    if ((rc = build_layer(m, *se1, &k.se1)) || (rc = take(p + "se2", m->se_dim, C, 1, &k.se2))) return rc;
+    // the scale-1 Res2Net layers, each packed straight into its slot of the block's stack
     const size_t pw = (size_t)xvb_packed_weight_elems(W, W, 3);
-    if ((rc = m->dev.alloc(&m->res_w[b].hi, pw * (m->scale - 1))) || (rc = m->dev.alloc(&m->res_w[b].lo, pw * (m->scale - 1))) ||
-        (rc = m->dev.alloc(&m->res_bias[b], (size_t)W * (m->scale - 1))) || (rc = m->dev.alloc(&m->res_scale[b], (size_t)W * (m->scale - 1))) ||
-        (rc = m->dev.alloc(&m->res_shift[b], (size_t)W * (m->scale - 1))))
+    if ((rc = m->dev.alloc(&k.res_w.hi, pw * (c.scale - 1))) || (rc = m->dev.alloc(&k.res_w.lo, pw * (c.scale - 1))) ||
+        (rc = m->dev.alloc(&k.res_bias, (size_t)W * (c.scale - 1))) || (rc = m->dev.alloc(&k.res_scale, (size_t)W * (c.scale - 1))) ||
+        (rc = m->dev.alloc(&k.res_shift, (size_t)W * (c.scale - 1))))
       return rc;
-    for (int i = 0; i < m->scale - 1; ++i) {
+    for (int i = 0; i < c.scale - 1; ++i) {
       const std::string n = p + "res" + std::to_string(i);
-      if ((rc = need(n, W, W, 3))) return rc;
-      const ELayer* L = find(m, n);
-      XVB_CHECK_ARG(L->ctx[0] == -L->ctx[2] && L->ctx[1] == 0 && L->bias && L->scale && L->shift && (L->flags & XVB_RELU),
+      if ((rc = need(n, W, W, 3, &r))) return rc;
+      XVB_CHECK_ARG(r->ctx[0] == -r->ctx[2] && r->ctx[1] == 0 && !r->b.empty() && !r->s.empty() && (r->flags & XVB_RELU),
                     "xvb_ecapa_finalize: '%s' must be a [-d,0,d] TDNN-ReLU-BN layer with bias", n.c_str());
-      if (i == 0) m->dilation[b] = L->ctx[2];
-      XVB_CHECK_ARG(L->ctx[2] == m->dilation[b], "xvb_ecapa_finalize: '%s' has another dilation than its block", n.c_str());
-      XVB_CUDA(cudaMemcpy(m->res_w[b].hi + pw * i, L->w.hi, pw * 2, cudaMemcpyDeviceToDevice));
-      XVB_CUDA(cudaMemcpy(m->res_w[b].lo + pw * i, L->w.lo, pw * 2, cudaMemcpyDeviceToDevice));
-      XVB_CUDA(cudaMemcpy(m->res_bias[b] + (size_t)W * i, L->bias, W * sizeof(float), cudaMemcpyDeviceToDevice));
-      XVB_CUDA(cudaMemcpy(m->res_scale[b] + (size_t)W * i, L->scale, W * sizeof(float), cudaMemcpyDeviceToDevice));
-      XVB_CUDA(cudaMemcpy(m->res_shift[b] + (size_t)W * i, L->shift, W * sizeof(float), cudaMemcpyDeviceToDevice));
+      if (i == 0) k.dilation = r->ctx[2];
+      XVB_CHECK_ARG(r->ctx[2] == k.dilation, "xvb_ecapa_finalize: '%s' has another dilation than its block", n.c_str());
+      if ((rc = m->dev.pack_into(Planes{k.res_w.hi + pw * i, k.res_w.lo + pw * i}, r->w, W, W, r->tot(), r->ctx, 3))) return rc;
+      XVB_CUDA(cudaMemcpy(k.res_bias + (size_t)W * i, r->b.data(), W * sizeof(float), cudaMemcpyHostToDevice));
+      XVB_CUDA(cudaMemcpy(k.res_scale + (size_t)W * i, r->s.data(), W * sizeof(float), cudaMemcpyHostToDevice));
+      XVB_CUDA(cudaMemcpy(k.res_shift + (size_t)W * i, r->t.data(), W * sizeof(float), cudaMemcpyHostToDevice));
     }
   }
-  rc = need("mfa", 3 * C, m->D, 1);
+  rc = take("mfa", 3 * C, c.D, 1, &m->mfa);
   if (rc) return rc;
-  if (!m->mq) {
-    if ((rc = need("att_x", m->D, m->H, 1)) || (rc = need("att_gs", 2 * m->D, m->H, 1)) || (rc = need("att2", m->H, m->D, 1)))
+  if (!c.mq) {
+    if ((rc = take("att_x", c.D, c.H, 1, &m->att_x)) || (rc = take("att_gs", 2 * c.D, c.H, 1, &m->att_gs)) ||
+        (rc = take("att2", c.H, c.D, 1, &m->att2)))
       return rc;
   } else {   // per-group input widths: att_x reads a head's Cg channels of x, att2 one query's hidden units
-    rc = need("att_x", m->D / m->mq_heads, m->AX, 1);
+    rc = take("att_x", c.D / c.mq_heads, c.AX, 1, &m->att_x);
     if (rc) return rc;
-    if (m->mq_layers == 2 && (rc = need("att2", m->mq_hidden, m->NL, 1))) return rc;
-    XVB_CHECK_ARG(m->mq_layers == 2 || !find(m, "att2"), "xvb_ecapa_finalize: one-layer attention has no 'att2'");
-    if (m->mq_tatt && (rc = need("att_gs", (m->mq_stddev ? 2 : 1) * m->D, m->AX, 1))) return rc;
-    XVB_CHECK_ARG(m->mq_tatt || !find(m, "att_gs"), "xvb_ecapa_finalize: 'att_gs' without time attention");
+    if (c.mq_layers == 2 && (rc = take("att2", c.mq_hidden, c.NL, 1, &m->att2))) return rc;
+    XVB_CHECK_ARG(c.mq_layers == 2 || !find(recs, "att2"), "xvb_ecapa_finalize: one-layer attention has no 'att2'");
+    if (c.mq_tatt && (rc = take("att_gs", (c.mq_stddev ? 2 : 1) * c.D, c.AX, 1, &m->att_gs))) return rc;
+    XVB_CHECK_ARG(c.mq_tatt || !find(recs, "att_gs"), "xvb_ecapa_finalize: 'att_gs' without time attention");
   }
   // segment level (ecapa_tdnn_xvector.py:412-422): [fc1 ->] [fc2]; "far" hands over fc1 alone, fc1=False fc2 alone
-  if (const ELayer* fc1 = find(m, "fc1")) {
-    XVB_CHECK_ARG(fc1->Cin == m->P && fc1->ntaps == 1 && fc1->w_f32, "xvb_ecapa_finalize: 'fc1' must be a one-tap layer over the %d pooled statistics", m->P);
-    if (find(m, "fc2")) {
-      rc = need("fc2", fc1->Cout, m->E, 1);
+  if (const TapRec* fc1 = find(recs, "fc1")) {
+    if ((rc = build_layer(m, *fc1, &m->fc1))) return rc;
+    XVB_CHECK_ARG(fc1->Cin == c.P && fc1->ntaps == 1 && m->fc1.w_f32, "xvb_ecapa_finalize: 'fc1' must be a one-tap layer over the %d pooled statistics", c.P);
+    if (find(recs, "fc2")) {
+      rc = take("fc2", fc1->Cout, c.E, 1, &m->fc2);
       if (rc) return rc;
     } else {
-      XVB_CHECK_ARG(fc1->Cout == m->E, "xvb_ecapa_finalize: 'fc1' alone must produce the %d-d embedding", m->E);
+      XVB_CHECK_ARG(fc1->Cout == c.E, "xvb_ecapa_finalize: 'fc1' alone must produce the %d-d embedding", c.E);
     }
     m->fc1_dim = fc1->Cout;
   } else {
-    rc = need("fc2", m->P, m->E, 1);
+    rc = take("fc2", c.P, c.E, 1, &m->fc2);
     if (rc) return rc;
   }
-  const ELayer* L0 = find(m, "layer1");
-  m->im2col = h->im2col = im2col_choice(L0->ctx, L0->ntaps, m->feat_dim);
-  h->draft = nullptr;
+  m->im2col = im2col_choice(m->layer1.ctx, m->layer1.ntaps, c.feat_dim);
   return XVB_OK;
 }
 
-extern "C" int xvb_ecapa_embed_dim(const xvb_ecapa_t* h) { return h ? h->m->E : XVB_EINVAL; }
-extern "C" int xvb_ecapa_feat_dim(const xvb_ecapa_t* h) { return h ? h->m->feat_dim : XVB_EINVAL; }
+extern "C" int xvb_ecapa_finalize(xvb_ecapa_t* h) {
+  const int rc = publish_built(h, build, "xvb_ecapa_finalize");
+  if (rc == XVB_OK) h->im2col = h->m->im2col;
+  return rc;
+}
+
+extern "C" int xvb_ecapa_embed_dim(const xvb_ecapa_t* h) { return h ? h->m->cfg.E : XVB_EINVAL; }
+extern "C" int xvb_ecapa_feat_dim(const xvb_ecapa_t* h) { return h ? h->m->cfg.feat_dim : XVB_EINVAL; }
 extern "C" int xvb_ecapa_last_launches(const xvb_ecapa_t* h) { return h ? h->last_launches : 0; }
 
 static int reserve(xvb_ecapa* h, int B, int T) {
   using H = xvb_ecapa;
   const Model* m = h->m.get();
-  const size_t b = (size_t)B, f = (size_t)B * T, C = (size_t)m->C, D = (size_t)m->D;
-  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->ldf, f * C, f * C, f * C, f * C,
-                                 f * C, f * 3 * C, f * D, f * m->H, b * 2 * D, b * m->se_dim, b * C, b * m->P2,
-                                 f * D, f * m->ldlog, b * C, b * m->AX, b * C, b * 2 * D, b * m->P2, b * m->se_dim,
+  const size_t b = (size_t)B, f = (size_t)B * T, C = (size_t)m->cfg.C, D = (size_t)m->cfg.D;
+  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->cfg.ldf, f * C, f * C, f * C, f * C,
+                                 f * C, f * 3 * C, f * D, f * m->cfg.H, b * 2 * D, b * m->se_dim, b * C, b * m->cfg.P2,
+                                 f * D, f * m->cfg.ldlog, b * C, b * m->cfg.AX, b * C, b * 2 * D, b * m->cfg.P2, b * m->se_dim,
                                  b * m->fc1_dim};
   bool planes[H::kBufs];
   for (int i = 0; i < H::kBufs; ++i) planes[i] = i <= H::kPp;
@@ -296,10 +306,10 @@ static int reserve(xvb_ecapa* h, int B, int T) {
   const int rc = h->ws.reserve(need, planes, &grown);
   if (rc) return rc;
   auto view = [&](int i, int64_t ld) { const Planes p = h->ws.planes(i); return View{p.hi, p.lo, ld}; };
-  h->in = view(H::kIn, m->ldf); h->X = view(H::kX, C); h->Hh = view(H::kH, C); h->R = view(H::kR, C);
+  h->in = view(H::kIn, m->cfg.ldf); h->X = view(H::kX, C); h->Hh = view(H::kH, C); h->R = view(H::kR, C);
   h->Z = view(H::kZ, C); h->N = view(H::kN, C); h->CAT = view(H::kCat, 3 * C); h->M = view(H::kM, D);
-  h->A1 = view(H::kA1, m->H); h->gp = view(H::kGp, 2 * D); h->s1 = view(H::kS1, m->se_dim); h->zm = view(H::kZm, C);
-  h->pp = view(H::kPp, m->P2);
+  h->A1 = view(H::kA1, m->cfg.H); h->gp = view(H::kGp, 2 * D); h->s1 = view(H::kS1, m->se_dim); h->zm = view(H::kZm, C);
+  h->pp = view(H::kPp, m->cfg.P2);
   h->MF = h->ws.f32(H::kMF); h->LOG = h->ws.f32(H::kLog); h->gate = h->ws.f32(H::kGate); h->ub = h->ws.f32(H::kUb);
   h->zmean = h->ws.f32(H::kZmean); h->gstat = h->ws.f32(H::kGstat); h->pstat = h->ws.f32(H::kPstat);
   h->s1f = h->ws.f32(H::kS1f); h->f1 = h->ws.f32(H::kF1);
@@ -353,30 +363,30 @@ int launch(const Run& r, void* stream) {
 // the head-width map: pooled channel (h*Q + q)*Cg + c is x channel h*Cg + c under the alpha of logit (h*Q + q)[*Cg + c].
 static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
   const Model* m = h->m.get();
-  const int D = m->D, cg = D / m->mq_heads;
-  const ELayer* ax = find(m, "att_x");
+  const int D = m->cfg.D, cg = D / m->cfg.mq_heads;
+  const ELayer* ax = &m->att_x;
   int rc;
-  if (m->mq_tatt) {
+  if (m->cfg.mq_tatt) {
     if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 0, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
-    const ELayer* gs = find(m, "att_gs");
+    const ELayer* gs = &m->att_gs;
     if (small_ok(gs)) {
-      if ((rc = small_layer(gs, h->gstat, 2 * D, B, h->ub, m->AX, 0, stream))) return rc;
+      if ((rc = small_layer(gs, h->gstat, 2 * D, B, h->ub, m->cfg.AX, 0, stream))) return rc;
     } else {
-      Run r{}; r.B = B; r.T = 1; r.L = gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->AX;
+      Run r{}; r.B = B; r.T = 1; r.L = gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->cfg.AX;
       if ((rc = launch(r, stream))) return rc;
     }
   }
   Run r{}; r.B = B; r.T = T; r.L = ax; r.x = h->M;
-  if (m->mq_tatt) { r.utt_bias = h->ub; r.ld_utt = m->AX; }
-  if (m->mq_layers == 2) { r.y = h->A1; r.extra_flags = XVB_TANH; }
-  else { r.y_f32 = h->LOG; r.ldyf = m->ldlog; }
+  if (m->cfg.mq_tatt) { r.utt_bias = h->ub; r.ld_utt = m->cfg.AX; }
+  if (m->cfg.mq_layers == 2) { r.y = h->A1; r.extra_flags = XVB_TANH; }
+  else { r.y_f32 = h->LOG; r.ldyf = m->cfg.ldlog; }
   if ((rc = launch(r, stream))) return rc;
-  if (m->mq_layers == 2) {
-    r = Run{}; r.B = B; r.T = T; r.L = find(m, "att2"); r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = m->ldlog;
+  if (m->cfg.mq_layers == 2) {
+    r = Run{}; r.B = B; r.T = T; r.L = &m->att2; r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = m->cfg.ldlog;
     if ((rc = launch(r, stream))) return rc;
   }
-  return xvb_attn_head_stats_pool_mq(h->LOG, m->ldlog, m->NL, h->MF, D, B, T, D, m->mq_q * D, m->mq_share ? cg : 1, cg, m->mq_q,
-                                     1e-5f, 0, h->pstat, h->pp.hi, h->pp.lo, m->P2, stream);
+  return xvb_attn_head_stats_pool_mq(h->LOG, m->cfg.ldlog, m->cfg.NL, h->MF, D, B, T, D, m->cfg.mq_q * D, m->cfg.mq_share ? cg : 1, cg, m->cfg.mq_q,
+                                     1e-5f, 0, h->pstat, h->pp.hi, h->pp.lo, m->cfg.P2, stream);
 }
 
 extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int T, float* emb, void* stream) {
@@ -386,18 +396,17 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   int rc = reserve(h, B, T);
   if (rc) return rc;
   const long before = g_launches;
-  const int C = m->C, D = m->D;
-  auto L = [&](const std::string& n) { return find(m, n); };
+  const int C = m->cfg.C, D = m->cfg.D;
   const Im2col& im = h->im2col;
   if (im.on)
-    rc = xvb_split_frames(feats, B, T, m->feat_dim, h->in.hi, h->in.lo, m->ldf, im.pad_front, im.pad_back, stream);
+    rc = xvb_split_frames(feats, B, T, m->cfg.feat_dim, h->in.hi, h->in.lo, m->cfg.ldf, im.pad_front, im.pad_back, stream);
   else
-    rc = xvb_split_f32(feats, (int64_t)B * T, m->feat_dim, m->feat_dim, h->in.hi, h->in.lo, m->ldf, stream);
+    rc = xvb_split_f32(feats, (int64_t)B * T, m->cfg.feat_dim, m->cfg.feat_dim, h->in.hi, h->in.lo, m->cfg.ldf, stream);
   if (rc) return rc;
   Run r{};
   r.B = B; r.T = T;
-  r.L = L("layer1"); r.x = h->in; r.y = h->X;
-  if (im.on) { r.im2col_taps = r.L->ntaps; r.x_batch_stride = (int64_t)(T + im.pad_front + im.pad_back) * m->ldf; }
+  r.L = &m->layer1; r.x = h->in; r.y = h->X;
+  if (im.on) { r.im2col_taps = r.L->ntaps; r.x_batch_stride = (int64_t)(T + im.pad_front + im.pad_back) * m->cfg.ldf; }
   rc = launch(r, stream);
   if (rc && im.on) {   // overlapping tensor map refused by the driver: plain path from now on
     h->im2col = Im2col{};
@@ -406,24 +415,24 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   if (rc) return rc;
   View cur = h->X;
   for (int b = 0; b < 3; ++b) {
-    const std::string p = "layer" + std::to_string(b + 2) + ".";
-    r = Run{}; r.B = B; r.T = T; r.L = L(p + "bn1"); r.x = cur; r.y = h->Hh;
+    const Block& k = m->blocks[b];
+    r = Run{}; r.B = B; r.T = T; r.L = &k.bn1; r.x = cur; r.y = h->Hh;
     if ((rc = launch(r, stream))) return rc;
-    if ((rc = xvb_res2net_block_ex(h->Hh.hi, h->Hh.lo, C, m->res_w[b].hi, m->res_w[b].lo, m->res_bias[b], m->res_scale[b],
-                                   m->res_shift[b], m->dilation[b], m->scale, h->R.hi, h->R.lo, C, B, T, C / m->scale, stream)))
+    if ((rc = xvb_res2net_block_ex(h->Hh.hi, h->Hh.lo, C, k.res_w.hi, k.res_w.lo, k.res_bias, k.res_scale, k.res_shift,
+                                   k.dilation, m->cfg.scale, h->R.hi, h->R.lo, C, B, T, C / m->cfg.scale, stream)))
       return rc;
-    r = Run{}; r.B = B; r.T = T; r.L = L(p + "bn2"); r.x = h->R; r.y = h->Z;
+    r = Run{}; r.B = B; r.T = T; r.L = &k.bn2; r.x = h->R; r.y = h->Z;
     if ((rc = launch(r, stream))) return rc;
     if ((rc = xvb_plane_mean(h->Z.hi, h->Z.lo, C, B, T, C, h->zmean, h->zm.hi, h->zm.lo, C, stream))) return rc;
-    if (small_ok(L(p + "se1")) && small_ok(L(p + "se2"))) {
-      rc = small_layer(L(p + "se1"), h->zmean, C, B, h->s1f, m->se_dim, 0, stream);
+    if (small_ok(&k.se1) && small_ok(&k.se2)) {
+      rc = small_layer(&k.se1, h->zmean, C, B, h->s1f, m->se_dim, 0, stream);
       if (rc) return rc;
-      rc = small_layer(L(p + "se2"), h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream);
+      rc = small_layer(&k.se2, h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream);
       if (rc) return rc;
     } else {
-      r = Run{}; r.B = B; r.T = 1; r.L = L(p + "se1"); r.x = h->zm; r.y = h->s1;
+      r = Run{}; r.B = B; r.T = 1; r.L = &k.se1; r.x = h->zm; r.y = h->s1;
       if ((rc = launch(r, stream))) return rc;
-      r = Run{}; r.B = B; r.T = 1; r.L = L(p + "se2"); r.x = h->s1; r.y_f32 = h->gate; r.ldyf = C; r.extra_flags = XVB_SIGMOID;
+      r = Run{}; r.B = B; r.T = 1; r.L = &k.se2; r.x = h->s1; r.y_f32 = h->gate; r.ldyf = C; r.extra_flags = XVB_SIGMOID;
       if ((rc = launch(r, stream))) return rc;
     }
     const bool last = b == 2;
@@ -433,39 +442,40 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
       return rc;
     cur = h->N;
   }
-  r = Run{}; r.B = B; r.T = T; r.L = L("mfa"); r.x = h->CAT; r.y = h->M; r.y_f32 = h->MF; r.ldyf = D;
+  r = Run{}; r.B = B; r.T = T; r.L = &m->mfa; r.x = h->CAT; r.y = h->M; r.y_f32 = h->MF; r.ldyf = D;
   if ((rc = launch(r, stream))) return rc;
-  if (m->mq) {
+  if (m->cfg.mq) {
     if ((rc = mqmha_pool(h, B, T, stream))) return rc;
   } else {
   if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
-  if (small_ok(L("att_gs"))) {
-    rc = small_layer(L("att_gs"), h->gstat, 2 * D, B, h->ub, m->H, 0, stream);
+  if (small_ok(&m->att_gs)) {
+    rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream);
       if (rc) return rc;
   } else {
-    r = Run{}; r.B = B; r.T = 1; r.L = L("att_gs"); r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->H;
+    r = Run{}; r.B = B; r.T = 1; r.L = &m->att_gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->cfg.H;
     if ((rc = launch(r, stream))) return rc;
   }
-  r = Run{}; r.B = B; r.T = T; r.L = L("att_x"); r.x = h->M; r.y = h->A1; r.utt_bias = h->ub; r.ld_utt = m->H; r.extra_flags = XVB_TANH;
+  r = Run{}; r.B = B; r.T = T; r.L = &m->att_x; r.x = h->M; r.y = h->A1; r.utt_bias = h->ub; r.ld_utt = m->cfg.H; r.extra_flags = XVB_TANH;
   if ((rc = launch(r, stream))) return rc;
-  r = Run{}; r.B = B; r.T = T; r.L = L("att2"); r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = D;
+  r = Run{}; r.B = B; r.T = T; r.L = &m->att2; r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = D;
   if ((rc = launch(r, stream))) return rc;
   if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, h->pp.hi, h->pp.lo, 2 * D, stream))) return rc;
   }
-  if (const ELayer* fc1 = L("fc1")) {              // fc1 [-> fc2] on CUDA cores (fp32)
-    const ELayer* fc2 = L("fc2");
-    rc = small_layer(fc1, h->pstat, m->P2, B, fc2 ? h->f1 : emb, fc1->Cout, 0, stream);
+  if (m->fc1.Cout) {              // fc1 [-> fc2] on CUDA cores (fp32)
+    const ELayer* fc1 = &m->fc1;
+    const ELayer* fc2 = m->fc2.Cout ? &m->fc2 : nullptr;
+    rc = small_layer(fc1, h->pstat, m->cfg.P2, B, fc2 ? h->f1 : emb, fc1->Cout, 0, stream);
     if (rc) return rc;
     if (fc2) {
       XVB_CHECK_ARG(fc2->w_f32, "xvb_ecapa_extract: 'fc2' after 'fc1' needs an input width that is a multiple of 4");
-      rc = small_layer(fc2, h->f1, fc1->Cout, B, emb, m->E, 0, stream);
+      rc = small_layer(fc2, h->f1, fc1->Cout, B, emb, m->cfg.E, 0, stream);
       if (rc) return rc;
     }
-  } else if (small_ok(L("fc2"))) {
-    rc = small_layer(L("fc2"), h->pstat, m->P2, B, emb, m->E, 0, stream);
+  } else if (small_ok(&m->fc2)) {
+    rc = small_layer(&m->fc2, h->pstat, m->cfg.P2, B, emb, m->cfg.E, 0, stream);
       if (rc) return rc;
   } else {
-    r = Run{}; r.B = B; r.T = 1; r.L = L("fc2"); r.x = h->pp; r.y_f32 = emb; r.ldyf = m->E;   // reads the first P of P2 columns
+    r = Run{}; r.B = B; r.T = 1; r.L = &m->fc2; r.x = h->pp; r.y_f32 = emb; r.ldyf = m->cfg.E;   // reads the first P of P2 columns
     if ((rc = launch(r, stream))) return rc;
   }
   h->last_launches = (int)(g_launches - before);
@@ -480,7 +490,7 @@ extern "C" int xvb_ecapa_extract_host(xvb_ecapa_t* h, const float* feats_host, i
 // extract_embeddings.py:73-83), device-resident / through pinned host buffers with the copies overlapped (shard.cuh).
 extern "C" int xvb_ecapa_set_gather(xvb_ecapa_t* h, float* const* tables, int ntables, int64_t row0, int64_t ld) {
   XVB_CHECK_ARG(finalized(h), "xvb_ecapa_set_gather: bad arguments");
-  return h->shard.set_gather(tables, ntables, row0, ld, h->m->E, "xvb_ecapa_set_gather");
+  return h->shard.set_gather(tables, ntables, row0, ld, h->m->cfg.E, "xvb_ecapa_set_gather");
 }
 
 extern "C" int xvb_ecapa_extract_shard(xvb_ecapa_t* h, const float* feats, int64_t N, int T, int batch, float* emb, void* stream) {
@@ -492,77 +502,15 @@ extern "C" int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_h
   return Shard<xvb_ecapa>::host(h, feats_host, N, T, batch, emb_host, stream, false, "xvb_ecapa_extract_shard_host");
 }
 
-// ---- .xvbm files for ECAPA ("XVBE0001"): dims, then named layer records -------------------------------------
-// "XVBE0002" (MQMHA pooling): the same with the pooling record {num_head, num_q, hidden, share, affine_layers,
-// time_attention, stddev} after the dims; layers of grouped convs are stored as the state_dict holds them.
 extern "C" int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path) {
   XVB_CHECK_ARG(finalized(h) && path, "xvb_ecapa_save: model not finalized");
-  const Model* m = h->m.get();
-  FILE* f = fopen(path, "wb");
-  XVB_CHECK_ARG(f, "xvb_ecapa_save: cannot open '%s'", path);
-  bool ok = fwrite(m->mq ? "XVBE0002" : "XVBE0001", 1, 8, f) == 8;
-  const int32_t hd[6] = {m->feat_dim, m->C, m->D, m->H, m->E, (int32_t)m->order.size()};
-  ok = ok && fwrite(hd, 4, 6, f) == 6;
-  if (m->mq) {
-    const int32_t pr[7] = {m->mq_heads, m->mq_q, m->mq_hidden, m->mq_share, m->mq_layers, m->mq_tatt, m->mq_stddev};
-    ok = ok && fwrite(pr, 4, 7, f) == 7;
-  }
-  for (const std::string& n : m->order) {
-    const ELayer& L = m->layers.at(n);
-    const int32_t nl = (int32_t)n.size();
-    const int32_t rec[7] = {L.Cout, L.Cin, L.ntaps, L.tot, L.flags, (int32_t)!L.hb.empty(), (int32_t)!L.hs.empty()};
-    ok = ok && fwrite(&nl, 4, 1, f) == 1 && fwrite(n.data(), 1, n.size(), f) == n.size() && fwrite(rec, 4, 7, f) == 7 &&
-         fwrite(L.ctx, 4, L.ntaps, f) == (size_t)L.ntaps && fwrite(L.hw.data(), 4, L.hw.size(), f) == L.hw.size();
-    if (!L.hb.empty()) ok = ok && fwrite(L.hb.data(), 4, L.hb.size(), f) == L.hb.size();
-    if (!L.hs.empty()) ok = ok && fwrite(L.hs.data(), 4, L.hs.size(), f) == L.hs.size() && fwrite(L.ht.data(), 4, L.ht.size(), f) == L.ht.size();
-  }
-  ok = fclose(f) == 0 && ok;
-  XVB_CHECK_ARG(ok, "xvb_ecapa_save: write to '%s' failed", path);
-  return XVB_OK;
-}
-
-extern "C" int xvb_ecapa_load(xvb_ecapa_t** out, const char* path) {
-  XVB_CHECK_ARG(out && path, "xvb_ecapa_load: null argument");
-  FILE* f = fopen(path, "rb");
-  XVB_CHECK_ARG(f, "xvb_ecapa_load: cannot open '%s'", path);
-  auto rd = [&](void* p, size_t n) { return fread(p, 1, n, f) == n; };
-  char magic[8];
-  int32_t hd[6];
-  xvb_ecapa_t* h = nullptr;
-  int rc = XVB_EINVAL;
-  do {
-    int32_t pr[7];
-    const bool ok_magic = rd(magic, 8) && (memcmp(magic, "XVBE0001", 8) == 0 || memcmp(magic, "XVBE0002", 8) == 0);
-    const bool mq = ok_magic && magic[7] == '2';
-    if (!ok_magic || !rd(hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(pr, sizeof pr))) {
-      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 file", path);
-      break;
-    }
-    if ((rc = xvb_ecapa_create(&h, hd[0], hd[1], hd[2], hd[3], hd[4]))) break;
-    if (mq && (rc = xvb_ecapa_set_mqmha(h, pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]))) break;
-    std::vector<float> w, b, s, t;
-    for (int i = 0; i < hd[5] && rc == XVB_OK; ++i) {
-      int32_t nl = 0, rec[7], ctx[XVB_MAX_TAPS];
-      char name[128];
-      bool ok = rd(&nl, 4) && nl > 0 && nl < 127 && rd(name, (size_t)nl) && rd(rec, sizeof rec) && rec[0] > 0 && rec[1] > 0 &&
-                rec[2] >= 1 && rec[2] <= XVB_MAX_TAPS && rec[3] >= rec[2] && rec[3] < 4096 && rd(ctx, 4 * (size_t)rec[2]);
-      if (ok) {
-        name[nl] = 0;
-        w.resize((size_t)rec[0] * rec[1] * rec[3]);
-        ok = rd(w.data(), w.size() * 4);
-        if (ok && rec[5]) { b.resize(rec[0]); ok = rd(b.data(), b.size() * 4); }
-        if (ok && rec[6]) { s.resize(rec[0]); t.resize(rec[0]); ok = rd(s.data(), s.size() * 4) && rd(t.data(), t.size() * 4); }
-      }
-      if (!ok) { set_error("xvb_ecapa_load: '%s' is truncated or corrupt at layer %d", path, i); rc = XVB_EINVAL; break; }
-      rc = xvb_ecapa_set_layer(h, name, rec[0], rec[1], ctx, rec[2], w.data(), rec[5] ? b.data() : nullptr,
-                               rec[6] ? s.data() : nullptr, rec[6] ? t.data() : nullptr, rec[4]);
-    }
-    if (rc == XVB_OK) rc = xvb_ecapa_finalize(h);
-  } while (0);
-  fclose(f);
-  if (rc != XVB_OK) { if (h) xvb_ecapa_destroy(h); return rc; }
-  *out = h;
-  return XVB_OK;
+  const Config& c = h->m->cfg;
+  const int32_t head[13] = {c.feat_dim, c.C, c.D, c.H, c.E, (int32_t)h->m->recs.size(),   // then XVBE0002's pooling
+                            c.mq_heads, c.mq_q, c.mq_hidden, c.mq_share, c.mq_layers, c.mq_tatt, c.mq_stddev};
+  std::vector<const TapRec*> layers;
+  for (const TapRec& r : h->m->recs) layers.push_back(&r);
+  return save_tap_file("xvb_ecapa_save", path, c.mq ? "XVBE0002" : "XVBE0001", head, (c.mq ? 13 : 6) * sizeof(int32_t),
+                       layers, true);
 }
 
 extern "C" void xvb_ecapa_destroy(xvb_ecapa_t* h) { delete h; }

@@ -15,9 +15,9 @@
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
 // the input side.  The model file is any of the six families, told apart by its magic: TDNN x-vector
-// (XVBM0001, ops.Extractor.save), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
+// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
-// subsampling) or CAM++ x-vector (XVBP0001), the last four written by the native extractors' save().  What it adds:
+// subsampling) or CAM++ x-vector (XVBP0001), each written by its native extractor's save() (model_file.cpp).  What it adds:
 // utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector and ResNet
 // x-vector files) chunks of different lengths share masked batches (plan_mixed_batches, xvb_extractor_extract_lengths /
 // xvb_resnet_extract_lengths), which fills batches on a real corpus where most frame counts occur a few times only.

@@ -18,23 +18,19 @@ namespace {
 
 using namespace xvb;
 
-struct Layer {
-  int Cin = 0, Cout = 0, ntaps = 0, flags = 0;
-  int ctx[XVB_MAX_TAPS] = {0};
-  Planes w;
-  float* bias = nullptr;
-  float* scale = nullptr;
-  float* shift = nullptr;
-};
+struct Config { int feat_dim = 0, ldf = 0; };
+
+struct Layers { std::vector<TapRec> frame, segment; };   // as handed over, in order
 
 // The layers and what finalize fixes; shared read-only by a handle and its second shard lane once finalized.
 struct Model {
-  int feat_dim = 0, ldf = 0;
+  Config cfg;
+  Layers recs;
   float pooling_eps = 1e-10f;
-  std::vector<Layer> frame, segment;
+  std::vector<TapLayer> frame, segment;   // recs on the device, built at finalize
   int max_c = 0, max_seg_c = 0;
   Im2col im2col;   // the first layer as an im2col view (records.cuh)
-  Weights dev{"xvb_extractor_add_layer"};
+  Weights dev{"xvb_extractor_finalize"};
 };
 
 // Everything one (B, T) batch shape needs besides launches: a GemmPlan per layer (tensor maps over the
@@ -110,29 +106,16 @@ struct xvb::ShardFamily<xvb_extractor> {
     c->fused_pooling = h->fused_pooling;
     return c;
   }
-  static int feat_dim(const xvb_extractor* h) { return h->m->feat_dim; }
+  static int feat_dim(const xvb_extractor* h) { return h->m->cfg.feat_dim; }
   static int embed_dim(const xvb_extractor* h) { return h->m->segment.back().Cout; }
 };
 
-static int add_layer(Model* m, std::vector<Layer>& dst, int Cin, int Cout, const int* ctx, int ntaps, const float* w_host,
+static int add_layer(std::vector<TapRec>& dst, int Cin, int Cout, const int* ctx, int ntaps, const float* w_host,
                      const float* bias_host, const float* scale_host, const float* shift_host, int flags) {
   XVB_CHECK_ARG(ntaps >= 1 && ntaps <= XVB_MAX_TAPS && ctx && w_host, "add layer: bad taps/weights");
   XVB_CHECK_ARG(!(flags & XVB_BN) || (scale_host && shift_host), "add layer: XVB_BN without scale/shift");
   for (int i = 1; i < ntaps; ++i) XVB_CHECK_ARG(ctx[i] > ctx[i - 1], "add layer: context must be strictly increasing");
-  // left/right/total context exactly as TdnnAffine.__init__ (components.py:50-53)
-  const int left = ctx[0] < 0 ? ctx[0] : 0;
-  const int right = ctx[ntaps - 1] > 0 ? ctx[ntaps - 1] : 0;
-  const int tot = right - left + 1;
-  Layer L;
-  L.Cin = Cin; L.Cout = Cout; L.ntaps = ntaps; L.flags = flags;
-  for (int i = 0; i < ntaps; ++i) L.ctx[i] = ctx[i];
-  const bool bn = flags & XVB_BN;
-  int rc;
-  if ((rc = m->dev.pack(&L.w, std::vector<float>(w_host, w_host + (size_t)Cout * Cin * tot), Cout, Cin, tot, ctx, ntaps)) ||
-      (rc = m->dev.upload(&L.bias, bias_host, Cout)) || (rc = m->dev.upload(&L.scale, bn ? scale_host : nullptr, Cout)) ||
-      (rc = m->dev.upload(&L.shift, bn ? shift_host : nullptr, Cout)))
-    return rc;
-  dst.push_back(L);
+  dst.push_back(tap_record("", Cout, Cin, ctx, ntaps, w_host, bias_host, scale_host, shift_host, flags));
   return XVB_OK;
 }
 
@@ -141,8 +124,8 @@ extern "C" int xvb_extractor_create(xvb_extractor_t** out, int feat_dim) {
   if (rc) return rc;
   XVB_CHECK_ARG(out && feat_dim > 0, "xvb_extractor_create: bad arguments");
   xvb_extractor* h = new xvb_extractor();
-  h->draft->feat_dim = feat_dim;
-  h->draft->ldf = (int)round_up(feat_dim, 8);
+  h->draft->cfg.feat_dim = feat_dim;
+  h->draft->cfg.ldf = (int)round_up(feat_dim, 8);
   *out = h;
   return XVB_OK;
 }
@@ -151,45 +134,61 @@ extern "C" int xvb_extractor_add_frame_layer(xvb_extractor_t* h, int Cout, const
                                              const float* w_host, const float* bias_host, const float* bn_scale_host,
                                              const float* bn_shift_host, int flags) {
   XVB_CHECK_ARG(is_draft(h), "xvb_extractor_add_frame_layer: null or finalized extractor");
-  Model* m = h->draft;
-  XVB_CHECK_ARG(m->segment.empty(), "xvb_extractor_add_frame_layer: frame layers must precede segment layers");
-  const int Cin = m->frame.empty() ? m->feat_dim : m->frame.back().Cout;
-  return add_layer(m, m->frame, Cin, Cout, context_host, ntaps, w_host, bias_host, bn_scale_host, bn_shift_host, flags);
+  Layers& r = h->draft->recs;
+  XVB_CHECK_ARG(r.segment.empty(), "xvb_extractor_add_frame_layer: frame layers must precede segment layers");
+  const int Cin = r.frame.empty() ? h->draft->cfg.feat_dim : r.frame.back().Cout;
+  return add_layer(r.frame, Cin, Cout, context_host, ntaps, w_host, bias_host, bn_scale_host, bn_shift_host, flags);
 }
 
 extern "C" int xvb_extractor_add_segment_layer(xvb_extractor_t* h, int Cout, const float* w_host, const float* bias_host,
                                                const float* bn_scale_host, const float* bn_shift_host, int flags) {
-  XVB_CHECK_ARG(is_draft(h) && !h->draft->frame.empty(), "xvb_extractor_add_segment_layer: need frame layers first");
-  Model* m = h->draft;
-  const int Cin = m->segment.empty() ? 2 * m->frame.back().Cout : m->segment.back().Cout;
+  XVB_CHECK_ARG(is_draft(h) && !h->draft->recs.frame.empty(), "xvb_extractor_add_segment_layer: need frame layers first");
+  Layers& r = h->draft->recs;
+  const int Cin = r.segment.empty() ? 2 * r.frame.back().Cout : r.segment.back().Cout;
   const int ctx0 = 0;
-  return add_layer(m, m->segment, Cin, Cout, &ctx0, 1, w_host, bias_host, bn_scale_host, bn_shift_host, flags);
+  return add_layer(r.segment, Cin, Cout, &ctx0, 1, w_host, bias_host, bn_scale_host, bn_shift_host, flags);
 }
 
 extern "C" int xvb_extractor_finalize(xvb_extractor_t* h, float pooling_eps) {
-  XVB_CHECK_ARG(is_draft(h) && !h->draft->frame.empty() && !h->draft->segment.empty(),
+  XVB_CHECK_ARG(is_draft(h) && !h->draft->recs.frame.empty() && !h->draft->recs.segment.empty(),
                 "xvb_extractor_finalize: need >=1 frame and >=1 segment layer");
-  Model* m = h->draft;
-  m->max_c = 0;
-  for (size_t i = 0; i + 1 < m->frame.size(); ++i) {
-    XVB_CHECK_ARG(m->frame[i].Cout % 8 == 0, "frame layer %d: Cout=%d must be a multiple of 8", (int)i, m->frame[i].Cout);
-    if (m->frame[i].Cout > m->max_c) m->max_c = m->frame[i].Cout;
-  }
-  XVB_CHECK_ARG(m->frame.back().Cout % 4 == 0, "last frame layer: Cout=%d must be a multiple of 4", m->frame.back().Cout);
-  m->max_seg_c = 0;
-  for (size_t i = 0; i + 1 < m->segment.size(); ++i) {
-    XVB_CHECK_ARG(m->segment[i].Cout % 8 == 0, "segment layer %d: Cout must be a multiple of 8", (int)i);
-    if (m->segment[i].Cout > m->max_seg_c) m->max_seg_c = m->segment[i].Cout;
-  }
-  XVB_CHECK_ARG(m->segment.back().Cout % 4 == 0, "last segment layer: Cout must be a multiple of 4");
-  m->pooling_eps = pooling_eps;
-  m->im2col = h->im2col = im2col_choice(m->frame[0].ctx, m->frame[0].ntaps, m->feat_dim);
-  h->draft = nullptr;
-  return XVB_OK;
+  auto build = [&](Model* m, const Layers& r) -> int {
+    for (size_t i = 0; i + 1 < r.frame.size(); ++i) {
+      XVB_CHECK_ARG(r.frame[i].Cout % 8 == 0, "frame layer %d: Cout=%d must be a multiple of 8", (int)i, r.frame[i].Cout);
+      if (r.frame[i].Cout > m->max_c) m->max_c = r.frame[i].Cout;
+    }
+    XVB_CHECK_ARG(r.frame.back().Cout % 4 == 0, "last frame layer: Cout=%d must be a multiple of 4", r.frame.back().Cout);
+    for (size_t i = 0; i + 1 < r.segment.size(); ++i) {
+      XVB_CHECK_ARG(r.segment[i].Cout % 8 == 0, "segment layer %d: Cout must be a multiple of 8", (int)i);
+      if (r.segment[i].Cout > m->max_seg_c) m->max_seg_c = r.segment[i].Cout;
+    }
+    XVB_CHECK_ARG(r.segment.back().Cout % 4 == 0, "last segment layer: Cout must be a multiple of 4");
+    int rc = XVB_OK;
+    for (const TapRec& rec : r.frame) if (!rc) rc = pack_tap(m->dev, rec, &m->frame.emplace_back());
+    for (const TapRec& rec : r.segment) if (!rc) rc = pack_tap(m->dev, rec, &m->segment.emplace_back());
+    if (rc) return rc;
+    m->pooling_eps = pooling_eps;
+    m->im2col = im2col_choice(r.frame[0].ctx, r.frame[0].ntaps, m->cfg.feat_dim);
+    return XVB_OK;
+  };
+  const int rc = publish_built(h, build, "xvb_extractor_finalize");
+  if (rc == XVB_OK) h->im2col = h->m->im2col;
+  return rc;
 }
 
 extern "C" int xvb_extractor_embed_dim(const xvb_extractor_t* h) {
-  return (h && !h->m->segment.empty()) ? h->m->segment.back().Cout : XVB_ESTATE;
+  return (h && !h->m->recs.segment.empty()) ? h->m->recs.segment.back().Cout : XVB_ESTATE;
+}
+
+extern "C" int xvb_extractor_save(const xvb_extractor_t* h, const char* path) {
+  XVB_CHECK_ARG(finalized(h) && path, "xvb_extractor_save: extractor not finalized");
+  const Model* m = h->m.get();
+  const struct { int32_t feat_dim; float pooling_eps; int32_t n_frame, n_segment; } head = {
+      m->cfg.feat_dim, m->pooling_eps, (int32_t)m->recs.frame.size(), (int32_t)m->recs.segment.size()};
+  std::vector<const TapRec*> layers;
+  for (const auto* v : {&m->recs.frame, &m->recs.segment})
+    for (const TapRec& r : *v) layers.push_back(&r);
+  return save_tap_file("xvb_extractor_save", path, "XVBM0001", &head, sizeof head, layers, false);
 }
 
 // Grows the workspace to what one (B, T, masked) call needs.  Any reallocation drops the launch plans, which hold the
@@ -198,7 +197,7 @@ static int reserve(H* h, int B, int T, bool masked) {
   const Model* m = h->m.get();
   const size_t b = (size_t)B, f = (size_t)B * T, cl = (size_t)m->frame.back().Cout;
   const size_t pool = h->fused_pooling && !masked ? (size_t)xvb_pool_partial_blocks(B, T, nullptr) * b * 2 * cl : 0;
-  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->ldf,
+  const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->cfg.ldf,
                                  f * m->max_c, f * m->max_c, f * cl, b * 2 * cl, b * m->segment.back().Cout, b * 2 * cl,
                                  b * m->max_seg_c, b * m->max_seg_c, pool, masked ? b : 0};
   const bool planes[H::kBufs] = {true, true, true, false, false, false, true, true, true, false, false};
@@ -220,7 +219,7 @@ static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
   int rc;
   sp->pool_blocks = xvb_pool_partial_blocks(B, T, &sp->pool_tb);
   Planes x = h->ws.planes(H::kIn);
-  int64_t ldx = m->ldf;
+  int64_t ldx = m->cfg.ldf;
   auto add = [&](std::vector<GemmPlan*>& dst, const xvb_tdnn_args_t& a) -> int {
     void* scratch = nullptr;
     const size_t need = gemm_plan_scratch_bytes(a);
@@ -235,7 +234,7 @@ static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
     return XVB_OK;
   };
   for (size_t i = 0; i < m->frame.size(); ++i) {
-    const Layer& L = m->frame[i];
+    const TapLayer& L = m->frame[i];
     const bool last = i + 1 == m->frame.size();
     const Planes y = last ? Planes{} : h->ws.planes(H::kAct0 + (i & 1));
     xvb_tdnn_args_t a{};
@@ -263,7 +262,7 @@ static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
   const int cl = m->frame.back().Cout;
   x = h->ws.planes(H::kStatsPlanes); ldx = 2 * cl;
   for (size_t i = 0; i < m->segment.size(); ++i) {
-    const Layer& L = m->segment[i];
+    const TapLayer& L = m->segment[i];
     const bool last = i + 1 == m->segment.size();
     const Planes y = last ? Planes{} : h->ws.planes(H::kSeg0 + (i & 1));
     xvb_tdnn_args_t a{};
@@ -313,9 +312,9 @@ static int extract_batch(H* h, const float* feats, int B, int T, bool masked, fl
   const int* lens = masked ? h->ws.i32(H::kLengths) : nullptr;
   const Planes in = h->ws.planes(H::kIn);
   if (h->im2col.on || masked)
-    rc = split_frames(feats, B, T, m->feat_dim, in.hi, in.lo, m->ldf, h->im2col.pad_front, h->im2col.pad_back, lens, stream);
+    rc = split_frames(feats, B, T, m->cfg.feat_dim, in.hi, in.lo, m->cfg.ldf, h->im2col.pad_front, h->im2col.pad_back, lens, stream);
   else
-    rc = xvb_split_f32(feats, (int64_t)B * T, m->feat_dim, m->feat_dim, in.hi, in.lo, m->ldf, stream);
+    rc = xvb_split_f32(feats, (int64_t)B * T, m->cfg.feat_dim, m->cfg.feat_dim, in.hi, in.lo, m->cfg.ldf, stream);
   if (rc) return rc;
   if ((rc = h->mark(cs))) return rc;
   // 2. frame-level TDNN stack (xvector.py:85-89)

@@ -1,11 +1,12 @@
 // Device side of the native extractors' shared plumbing: the handle base, the packed split-bf16 planes and the arena
-// that owns a model's device weights (every family), the grow-only workspace, the segment level of the 2-D families,
-// the group loop of an extract call and the lengths check of a masked one.  The record store and the model-file codec
-// are host code in records.h.
+// that owns a model's device weights (every family), the device tap layer of the TDNN and ECAPA-TDNN, the grow-only
+// workspace, the segment level of the 2-D families, the group loop of an extract call and the lengths check of a masked
+// one.  The host records and the model-file codecs are host code in records.h.
 #pragma once
 #include <stdlib.h>
 
 #include <memory>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -37,20 +38,26 @@ struct Weights {
     return XVB_OK;
   }
   int upload(float** d, const std::vector<float>& v) { return upload(d, v.data(), v.size()); }
-  // (Cout, Cin, tot) fp32 host -> packed planes of the taps ctx[0..n) (ops.pack_tdnn_weight / pack_conv2d_weight).
+  // (Cout, Cin, tot) fp32 host -> newly allocated packed planes of the taps ctx[0..n).
+  int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int tot, const int* ctx, int n) {
+    const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, n);
+    int rc;
+    if ((rc = alloc(&c->hi, pn)) || (rc = alloc(&c->lo, pn))) return rc;
+    return pack_into(*c, w, Cout, Cin, tot, ctx, n);
+  }
+  // (Cout, Cin, tot) fp32 host -> the packed planes of the taps ctx[0..n) at c (ops.pack_tdnn_weight /
+  // pack_conv2d_weight), xvb_packed_weight_elems(Cout, Cin, n) elements each.
   // xvb_pack_tdnn_weight takes at most XVB_MAX_TAPS taps per call: a longer list is packed in pieces of that many taps
   // (the last one shorter), each piece's rows then copied into its K range of every output row, as pack_conv2d_weight
   // concatenates the pieces along K.  Up to XVB_MAX_TAPS taps it is the one call straight into the planes.
-  int pack(Planes* c, const std::vector<float>& w, int Cout, int Cin, int tot, const int* ctx, int n) {
+  int pack_into(Planes c, const std::vector<float>& w, int Cout, int Cin, int tot, const int* ctx, int n) {
     float* w_dev = nullptr;
     XVB_CUDA(cudaMalloc((void**)&w_dev, w.size() * sizeof(float)));
     cudaError_t e = cudaMemcpy(w_dev, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice);
     const int left = ctx[0] < 0 ? ctx[0] : 0;
     const size_t pn = (size_t)xvb_packed_weight_elems(Cout, Cin, n);
     int rc = e != cudaSuccess ? XVB_ECUDA : XVB_OK;
-    if (!rc) rc = alloc(&c->hi, pn);
-    if (!rc) rc = alloc(&c->lo, pn);
-    if (!rc && n <= XVB_MAX_TAPS) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx, n, c->hi, c->lo, nullptr);
+    if (!rc && n <= XVB_MAX_TAPS) rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx, n, c.hi, c.lo, nullptr);
     Planes piece;
     if (!rc && n > XVB_MAX_TAPS) {
       const size_t tap = pn / ((size_t)Cout * n);   // packed elements of one tap in one output row (Cin padded to 16)
@@ -64,7 +71,7 @@ struct Weights {
         rc = xvb_pack_tdnn_weight(w_dev, Cout, Cin, tot, left, ctx + i, m, piece.hi, piece.lo, nullptr);
         const size_t dpitch = (size_t)n * tap * sizeof(uint16_t), spitch = (size_t)m * tap * sizeof(uint16_t);
         for (int p = 0; p < 2 && !rc; ++p) {
-          uint16_t* dst = (p ? c->lo : c->hi) + (size_t)i * tap;
+          uint16_t* dst = (p ? c.lo : c.hi) + (size_t)i * tap;
           const cudaError_t ce = cudaMemcpy2D(dst, dpitch, p ? piece.lo : piece.hi, spitch, spitch, (size_t)Cout,
                                               cudaMemcpyDeviceToDevice);
           if (ce != cudaSuccess) { set_error("%s: joining the packed pieces failed: %s", fn, cudaGetErrorString(ce)); rc = XVB_ECUDA; }
@@ -78,6 +85,26 @@ struct Weights {
     return rc;
   }
 };
+
+// A TDNN or ECAPA-TDNN layer on the device: its record's shape, packed weight and parameters.
+struct TapLayer : TapShape {
+  Planes w;
+  float* bias = nullptr;
+  float* scale = nullptr;
+  float* shift = nullptr;
+};
+
+// r on the device: its shape, the (Cout, cin, tot) weight w packed (r.w over r.Cin, or what stands in for it, such as
+// the block-diagonal expansion of a grouped layer) and r's bias, scale and shift.
+inline int pack_tap(Weights& dev, const TapRec& r, TapLayer* L, const std::vector<float>& w, int cin) {
+  static_cast<TapShape&>(*L) = r;
+  int rc;
+  if ((rc = dev.pack(&L->w, w, r.Cout, cin, r.tot(), r.ctx, r.ntaps)) || (rc = dev.upload(&L->bias, r.b)) ||
+      (rc = dev.upload(&L->scale, r.s)) || (rc = dev.upload(&L->shift, r.t)))
+    return rc;
+  return XVB_OK;
+}
+inline int pack_tap(Weights& dev, const TapRec& r, TapLayer* L) { return pack_tap(dev, r, L, r.w, r.Cin); }
 
 // taps 0 .. n-1 of a weight packed over its whole span
 constexpr int kTaps[9] = {0, 1, 2, 3, 4, 5, 6, 7, 8};
@@ -226,8 +253,8 @@ struct Handle {
 template <typename Model> bool finalized(const Handle<Model>* h) { return h && !h->draft; }
 template <typename Model> bool is_draft(const Handle<Model>* h) { return h && h->draft; }
 
-// The finalize of the record-store families (fn: its name): build(fresh, records) makes a new model from the draft's
-// configuration and records, and only a model built without error is published, the records moved into it for save.
+// The finalize of every family (fn: its name): build(fresh, records) makes a new model from the draft's configuration
+// and records, and only a model built without error is published, the records moved into it for save and the getters.
 // A failed build is discarded with its device weights and the draft keeps its records, so that the caller can add what
 // was missing and finalize again.
 template <typename Model, typename Build>
@@ -235,7 +262,7 @@ int publish_built(Handle<Model>* h, Build build, const char* fn) {
   XVB_CHECK_ARG(is_draft(h), "%s: null or finalized model", fn);
   auto fresh = std::make_shared<Model>();
   fresh->cfg = h->draft->cfg;
-  h->draft->recs.used.clear();
+  if constexpr (std::is_same_v<decltype(h->draft->recs), RecordStore>) h->draft->recs.used.clear();
   int rc = build(fresh.get(), h->draft->recs);
   if (rc) return rc;
   fresh->recs = std::move(h->draft->recs);

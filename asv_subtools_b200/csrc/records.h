@@ -1,9 +1,10 @@
-// Named-record model store and model-file codec of the ResNet, Conformer and CAM++ native extractors (host code; the
-// device-weight arena and the workspace are in records.cuh).
+// Host records of the native extractors and their model-file codecs (host code in model_file.cpp; the device-weight
+// arena and the workspace are in records.cuh).
 //
-// A family's set_layer hands over one record per state_dict module path: a small fixed shape, flags and up to four
-// fp32 arrays.  The store keeps host copies in insertion order, so that save() writes the records exactly as they were
-// handed over, and finalize() takes each record its configuration needs and then refuses any record it did not take.
+// The TDNN and ECAPA-TDNN hand over tap layers (TapRec).  The ResNet, RepVGG, Conformer and CAM++ set_layer hands over
+// one record per state_dict module path: a small fixed shape, flags and up to four fp32 arrays.  The store keeps host
+// copies in insertion order, so that save() writes the records exactly as they were handed over, and finalize() takes
+// each record its configuration needs and then refuses any record it did not take.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -13,7 +14,35 @@
 #include <string>
 #include <vector>
 
+#include "../../include/xvb200.h"
+
 namespace xvb {
+
+// The shape of a TDNN layer as TdnnAffine stores it: Cout x Cin over the taps ctx[0..ntaps), strictly increasing; the
+// weight spans the whole context from min(ctx[0], 0) to max(ctx[ntaps-1], 0) (components.py:50-53), unused taps
+// included.
+struct TapShape {
+  int Cout = 0, Cin = 0, ntaps = 0, flags = 0;
+  int ctx[XVB_MAX_TAPS] = {0};
+  int left() const { return ctx[0] < 0 ? ctx[0] : 0; }
+  int tot() const { return (ctx[ntaps - 1] > 0 ? ctx[ntaps - 1] : 0) - left() + 1; }
+};
+
+// One TDNN or ECAPA-TDNN layer exactly as handed over: w (Cout, Cin, tot), the bias when given, scale and shift when
+// flags has XVB_BN.  name: the ECAPA-TDNN layer name; empty in the TDNN, whose layers are positional.
+struct TapRec : TapShape {
+  std::string name;
+  std::vector<float> w, b, s, t;
+};
+
+// Host copies of a layer's arrays (the caller has checked the taps and that XVB_BN comes with scale and shift).
+TapRec tap_record(const char* name, int Cout, int Cin, const int* ctx, int ntaps, const float* w, const float* b,
+                  const float* s, const float* t, int flags);
+
+// The tap-layer files ("XVBM0001" TDNN, "XVBE0001" / "XVBE0002" ECAPA-TDNN; layouts in model_file.cpp): magic, the
+// family's header block, then the layers in order, each preceded by its name when `named` (fn: the caller's name).
+int save_tap_file(const char* fn, const char* path, const char* magic, const void* head, size_t head_bytes,
+                  const std::vector<const TapRec*>& layers, bool named);
 
 struct Rec {   // one named record exactly as handed over
   int shape[3] = {0, 0, 0};        // rows, cols (CAM++, Conformer) or Cout, Cin, ksize (ResNet)

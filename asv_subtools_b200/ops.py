@@ -771,7 +771,7 @@ def trial_histogram(enroll, enroll_spk, test, test_spk, lo, hi, nbins=2048, row_
 # ------------------------------------------------------------------ whole-model extractor
 class Extractor(ShardExtractor):
     """Owner of a native xvb_extractor_t (packed weights + workspace on the current device), built layer by layer with
-    add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file."""
+    add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file; save() writes that file."""
 
     TAKES_LENGTHS = True
 
@@ -783,9 +783,6 @@ class Extractor(ShardExtractor):
         self._h = C.c_void_p()
         check(lib.xvb_extractor_create(C.byref(self._h), int(feat_dim)), "xvb_extractor_create")
         self.feat_dim = int(feat_dim)
-        self._keep = []
-        self._saved = []      # (kind, context, w, b, scale, shift, flags): what save() writes
-        self._eps = None
 
     @staticmethod
     def _np(a):
@@ -802,7 +799,6 @@ class Extractor(ShardExtractor):
         flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0)
         check(lib.xvb_extractor_add_frame_layer(self._h, w.shape[0], int_array(context), len(context), wp, bp, sp, tp,
                                                 flags), "xvb_extractor_add_frame_layer")
-        self._saved.append(("frame", [int(c) for c in context], w, b, s, t, flags))
 
     def add_segment_layer(self, weight, bias, bn_scale=None, bn_shift=None, relu=False):
         w, wp = self._np(weight)
@@ -812,33 +808,10 @@ class Extractor(ShardExtractor):
         flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0)
         check(lib.xvb_extractor_add_segment_layer(self._h, w.shape[0], wp, bp, sp, tp, flags),
               "xvb_extractor_add_segment_layer")
-        self._saved.append(("segment", [0], w, b, s, t, flags))
 
     def finalize(self, pooling_eps=1e-10):
         check(lib.xvb_extractor_finalize(self._h, pooling_eps), "xvb_extractor_finalize")
         self.embed_dim = lib.xvb_extractor_embed_dim(self._h)
-        self._eps = float(pooling_eps)
-
-    def save(self, path):
-        """Write the layer list as an .xvbm file (csrc/model_file.cpp) for xvb_extractor_load /
-        the Python-free `bin/xvb-extract`."""
-        import struct
-        if self._eps is None:
-            raise RuntimeError("Extractor.save: finalize() first")
-        frames = [l for l in self._saved if l[0] == "frame"]
-        segs = [l for l in self._saved if l[0] == "segment"]
-        with open(path, "wb") as f:
-            f.write(b"XVBM0001" + struct.pack("<ifii", self.feat_dim, self._eps, len(frames), len(segs)))
-            for _, ctx, w, b, s, t, flags in frames + segs:
-                w3 = w.reshape(w.shape[0], w.shape[1], -1)
-                f.write(struct.pack("<7i", w3.shape[0], w3.shape[1], len(ctx), w3.shape[2], flags, int(b is not None),
-                                    int(s is not None)))
-                f.write(struct.pack("<%di" % len(ctx), *ctx))
-                f.write(np.ascontiguousarray(w3, dtype="<f4").tobytes())
-                if b is not None:
-                    f.write(np.ascontiguousarray(b, dtype="<f4").tobytes())
-                if s is not None:
-                    f.write(np.ascontiguousarray(s, dtype="<f4").tobytes() + np.ascontiguousarray(t, dtype="<f4").tobytes())
 
     @classmethod
     def load(cls, path):
@@ -849,7 +822,6 @@ class Extractor(ShardExtractor):
         check(lib.xvb_extractor_load(C.byref(self._h), str(path).encode()), "xvb_extractor_load")
         self.feat_dim = lib.xvb_extractor_feat_dim(str(path).encode())
         self.embed_dim = lib.xvb_extractor_embed_dim(self._h)
-        self._keep, self._saved, self._eps = [], [], None
         return self
 
     def extract(self, feats, lengths=None):

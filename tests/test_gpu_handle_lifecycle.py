@@ -16,6 +16,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 sys.path.insert(0, HERE)
 import campplus_oracle as cpo  # noqa: E402
 import conformer_oracle as co  # noqa: E402
+import ecapa_mqmha_oracle as mo  # noqa: E402
 import repvgg_oracle as rvo  # noqa: E402
 import resnet_oracle as ro  # noqa: E402
 from asv_subtools_b200 import ops  # noqa: E402
@@ -31,7 +32,6 @@ pytestmark = pytest.mark.gpu
 
 EINVAL, XVB_ESTATE = -1, -4
 FAMILIES = ["extractor", "ecapa", "resnet", "repvgg", "conformer", "campp"]
-RECORD_FAMILIES = ["resnet", "repvgg", "conformer", "campp"]
 
 
 def _resnet():
@@ -65,7 +65,24 @@ def _campp():
     return NativeCamPPExtractor, m, fdim, 40, "xvector.block2.tdnnd1.linear1"
 
 
+def _ecapa(mqmha, held):
+    """ECAPA-TDNN (the default model, or MQMHA pooling with fc1) holding back `held`: "mfa" is refused after the Res2Net
+    stacks are built, "layer4.res6" while the last one is."""
+    def make():
+        if mqmha:
+            kwargs, _, _, seed, _ = mo.CASES["fc1"]
+            m = ECAPA_TDNN(80, 10, training=False, extracted_embedding="near", **kwargs)
+            m.load_state_dict(onn.make_state_dict(mo.ecapa_mqmha_spec(kwargs), seed), strict=True)
+        else:
+            m = ECAPA_TDNN(80, 10, training=False)
+            m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(80, fc2_bn_affine=True), 201), strict=True)
+        return NativeEcapaExtractor, m, 80, 40, held
+    return make
+
+
 RECORD_MODELS = {"resnet": _resnet, "repvgg": _repvgg, "conformer": _conformer, "campp": _campp}
+RETRY_MODELS = dict(RECORD_MODELS, **{"ecapa{}-{}".format("_mqmha" if mq else "", held): _ecapa(mq, held)
+                                     for mq in (False, True) for held in ("mfa", "layer4.res6")})
 
 
 def _draft(cls, m):
@@ -129,8 +146,7 @@ def test_a_draft_refuses_every_extract_and_save(family, tmp_path):
         calls["extract_shard_host"] = lambda: fn("extract_shard_host")(h, hp(host_feats), B, T, 1, hp(host_emb), _stream())
     if family == "extractor":
         calls["submit_host"] = lambda: fn("submit_host")(h, hp(host_feats), B, T, hp(host_emb), 0, _stream())
-    else:   # the TDNN's model files are written by Python (ops.Extractor.save)
-        calls["save"] = lambda: fn("save")(h, str(tmp_path / "draft.bin").encode())
+    calls["save"] = lambda: fn("save")(h, str(tmp_path / "draft.bin").encode())
     try:
         for name, call in calls.items():
             assert call() == EINVAL, (family, name)
@@ -157,7 +173,7 @@ def _tdnn_layers(seed=5):
     return frame, seg
 
 
-def test_tdnn_finalize_retries_after_the_missing_segment_layer():
+def test_tdnn_finalize_retries_after_the_missing_segment_layer(tmp_path):
     frame, seg = _tdnn_layers()
     retried, fresh = ops.Extractor(24), ops.Extractor(24)
     for wt, b, ctx in frame:
@@ -173,6 +189,9 @@ def test_tdnn_finalize_retries_after_the_missing_segment_layer():
     x = torch.from_numpy(onn.synthetic_feats(3, 50, 24, 9)).cuda()
     got, want = retried.extract(x), fresh.extract(x)
     assert torch.equal(got, want) and retried.last_launches == fresh.last_launches
+    retried.save(tmp_path / "retried.bin")
+    fresh.save(tmp_path / "fresh.bin")
+    assert (tmp_path / "retried.bin").read_bytes() == (tmp_path / "fresh.bin").read_bytes()
     wt, b, ctx = frame[0]
     w_np = np.ascontiguousarray(wt)
     for h in (retried, fresh):   # finalized: no more layers
@@ -194,9 +213,9 @@ def test_ecapa_set_layer_refuses_a_finalized_handle():
     assert ex.extract(torch.from_numpy(onn.synthetic_feats(2, 40, 80, 3)).cuda()).shape == (2, 192)
 
 
-@pytest.mark.parametrize("family", RECORD_FAMILIES)
+@pytest.mark.parametrize("family", sorted(RETRY_MODELS))
 def test_finalize_after_a_missing_record_equals_a_fresh_handle(family, tmp_path):
-    cls, m, fdim, T, held = RECORD_MODELS[family]()
+    cls, m, fdim, T, held = RETRY_MODELS[family]()
     m = m.cuda().eval()
     records = list(cls.__new__(cls)._layers(m))
     order = [r for r in records if r[0] != held] + [r for r in records if r[0] == held]
@@ -206,7 +225,8 @@ def test_finalize_after_a_missing_record_equals_a_fresh_handle(family, tmp_path)
     for rec in order[:-1]:
         assert _set(retried, rec) == 0, last_error()
     assert _finalize(retried) == EINVAL
-    assert "record '{}' is missing".format(held) in last_error(), last_error()
+    what = "layer" if family.startswith("ecapa") else "record"
+    assert "{} '{}' is missing".format(what, held) in last_error(), last_error()
     assert _set(retried, order[-1]) == 0, last_error()
     assert _finalize(retried) == 0, last_error()
 

@@ -2,7 +2,7 @@
 the H100, over every case of the three families' fixtures: save() writes exactly the bytes of a writer of the documented
 layout fed the records the handle was built from; load() then save() reproduces the file byte for byte; and corrupt files
 are refused with an error naming the magic or the damage, without a crash.  The ECAPA-TDNN files (XVBE0001, XVBE0002
-with MQMHA pooling) are checked the same way against a writer of their own layout."""
+with MQMHA pooling) and the TDNN files (XVBM0001) are checked the same way against writers of their own layouts."""
 import struct
 
 import numpy as np
@@ -13,6 +13,7 @@ import conformer_2sub_oracle as c2
 import conformer_oracle as co
 import ecapa_mqmha_oracle as mo
 import resnet_oracle as ro
+from asv_subtools_b200 import _lib, ops
 from asv_subtools_b200._lib import CamPPConfig, ConformerConfig
 from asv_subtools_b200.model.campplus_xvector import CamPPXvector, NativeCamPPExtractor, native_config as campp_config
 from asv_subtools_b200.model.ecapa_tdnn_xvector import ECAPA_TDNN, NativeEcapaExtractor
@@ -171,3 +172,115 @@ def test_ecapa_model_file_bytes_and_roundtrip(tmp_path, magic):
     loaded.close()
     assert open(again, "rb").read() == data
     ex.close()
+
+
+class _Recorded(ops.Extractor):
+    """ops.Extractor keeping what it is handed, for the writer below."""
+
+    def __init__(self, feat_dim):
+        super().__init__(feat_dim)
+        self.handed = {"frame": [], "segment": []}
+
+    def add_frame_layer(self, weight, bias, context, bn_scale=None, bn_shift=None, relu=True):
+        super().add_frame_layer(weight, bias, context, bn_scale, bn_shift, relu)
+        self.handed["frame"].append(([int(c) for c in context], weight, bias, bn_scale, bn_shift, relu))
+
+    def add_segment_layer(self, weight, bias, bn_scale=None, bn_shift=None, relu=False):
+        super().add_segment_layer(weight, bias, bn_scale, bn_shift, relu)
+        self.handed["segment"].append(([0], weight, bias, bn_scale, bn_shift, relu))
+
+    def finalize(self, pooling_eps=1e-10):
+        super().finalize(pooling_eps)
+        self.eps = pooling_eps
+
+
+def _xvbm_write(ex):
+    """The XVBM0001 layout: magic | i32 feat_dim | f32 pooling_eps | i32 n_frame, n_segment, then per layer, frame layers
+    first: i32 Cout, Cin, ntaps, tot_context, flags, has_bias, has_bn | i32 ctx[ntaps] | f32 w (Cout, Cin, tot_context)
+    | f32 bias? | f32 scale, shift?"""
+    frames, segs = ex.handed["frame"], ex.handed["segment"]
+    out = bytearray(b"XVBM0001" + struct.pack("<ifii", ex.feat_dim, ex.eps, len(frames), len(segs)))
+    for ctx, w, b, s, t, relu in frames + segs:
+        flags = (_lib.RELU if relu else 0) | (_lib.BN if s is not None else 0)
+        w3 = np.asarray(w, np.float32).reshape(w.shape[0], w.shape[1], -1)
+        out += struct.pack("<7i", w3.shape[0], w3.shape[1], len(ctx), w3.shape[2], flags, b is not None, s is not None)
+        out += struct.pack("<%di" % len(ctx), *ctx)
+        for a in (w3, b, s, t):
+            if a is not None:
+                out += np.ascontiguousarray(np.asarray(a, np.float32), dtype="<f4").tobytes()
+    return bytes(out)
+
+
+def _hand_built():
+    """Frame layers over the contexts [-2..2], [-2,0,2], [-3,0,3] and [0], with and without bias, BatchNorm and ReLU."""
+    r = np.random.default_rng(11)
+    w = lambda *s: (r.standard_normal(s) / np.sqrt(np.prod(s[1:]))).astype(np.float32)   # noqa: E731
+    v = lambda n: r.standard_normal(n).astype(np.float32)   # noqa: E731
+    ex = _Recorded(24)
+    ex.add_frame_layer(w(64, 24, 5), v(64), [-2, -1, 0, 1, 2], v(64) + 2, v(64))
+    ex.add_frame_layer(w(64, 64, 5), None, [-2, 0, 2])
+    ex.add_frame_layer(w(64, 64, 7), v(64), [-3, 0, 3], relu=False)
+    ex.add_frame_layer(w(32, 64, 1), v(32), [0], v(32) + 2, v(32))
+    ex.add_segment_layer(w(24, 64), v(24), v(24) + 2, v(24), relu=True)
+    ex.add_segment_layer(w(16, 24), None)
+    ex.finalize(pooling_eps=1e-6)
+    return ex
+
+
+TDNN_CASES = {"xvector_far": ("xvector", 23, 101, "far"), "xvector_near": ("xvector", 23, 101, "near"),
+              "extended_near": ("extended", 80, 103, "near"), "snowdar_near_full": ("snowdar", 40, 301, "near"),
+              "hand_built": None}
+
+
+def _tdnn(case, monkeypatch):
+    if TDNN_CASES[case] is None:
+        return _hand_built()
+    kind, dim, seed, pos = TDNN_CASES[case]
+    if kind == "xvector":
+        from asv_subtools_b200.model.xvector import Xvector as cls
+        spec = onn.xvector_spec(dim)
+    elif kind == "extended":
+        from asv_subtools_b200.model.extended_xvector import ExtendedXvector as cls
+        spec = onn.extended_xvector_spec(dim)
+    else:   # the snowdar Xvector's "near" is the whole last layer (built as near_full)
+        from asv_subtools_b200.model.snowdar_xvector import Xvector as cls
+        spec = onn.snowdar_xvector_spec(dim)
+    m = cls(dim, 10, training=False, extracted_embedding=pos)
+    m.load_state_dict(onn.make_state_dict(spec, seed), strict=True)
+    monkeypatch.setattr(ops, "Extractor", _Recorded)   # build_tdnn_extractor hands its layers to a _Recorded
+    ex = m.cuda().eval().extractor()
+    assert isinstance(ex, _Recorded)
+    return ex
+
+
+@pytest.mark.parametrize("case", sorted(TDNN_CASES))
+def test_tdnn_model_file_bytes_roundtrip_and_rejects(tmp_path, monkeypatch, case):
+    ex = _tdnn(case, monkeypatch)
+    path, again, bad = str(tmp_path / "model.xvbm"), str(tmp_path / "again.xvbm"), str(tmp_path / "bad.xvbm")
+    ex.save(path)
+    data = open(path, "rb").read()
+    assert data == _xvbm_write(ex)
+    loaded = _Recorded.load(path)
+    assert (loaded.feat_dim, loaded.embed_dim) == (ex.feat_dim, ex.embed_dim)
+    loaded.save(again)
+    assert open(again, "rb").read() == data
+
+    def patched(offset, value):
+        b = bytearray(data)
+        b[offset:offset + 4] = struct.pack("<i", value)
+        return bytes(b)
+
+    layer0 = 24   # after magic, feat_dim, pooling_eps, n_frame, n_segment
+    blobs = [(data[:-100], "is truncated in layer"),                      # cut inside the last layer's arrays
+             (data[:layer0 + 52], "is truncated in layer 0"),             # cut inside the first weight
+             (data[:layer0 + 10], "bad layer 0 header"),                  # cut inside the first layer's ints
+             (patched(layer0, 0), "bad layer 0 header"),                  # Cout 0
+             (patched(layer0 + 8, 17), "bad layer 0 header"),             # more taps than XVB_MAX_TAPS
+             (patched(layer0 + 12, 4096), "bad layer 0 header"),          # tot_context out of range
+             (patched(16, 0), "bad header"),                              # no frame layer
+             (b"XVBM0002" + data[8:], "is not an XVBM0001 file")]
+    for blob, msg in blobs:
+        with open(bad, "wb") as f:
+            f.write(blob)
+        with pytest.raises(RuntimeError, match=msg):
+            _Recorded.load(bad)
