@@ -17,7 +17,6 @@
 // are prepared by the caller -- see the Python blueprint.  The handle keeps the layers as handed over and builds the
 // model from them at finalize; xvb_ecapa_save writes them back (the XVBE0001 / XVBE0002 layouts are in model_file.cpp).
 #include <cuda_runtime.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <memory>
@@ -86,12 +85,11 @@ struct Model {
 using namespace xvb;
 
 struct xvb_ecapa : Handle<Model> {
-  // workspace, each buffer grown to the largest call seen: the plane buffers up to kPp, then the fp32 ones
-  enum { kIn, kX, kH, kR, kZ, kN, kCat, kM, kA1, kGp, kS1, kZm, kPp, kMF, kLog, kGate, kUb, kZmean, kGstat, kPstat, kS1f,
-         kF1, kBufs };
+  // workspace, each buffer grown to the largest call seen: the plane buffers up to kA1, then the fp32 ones
+  enum { kIn, kX, kH, kR, kZ, kN, kCat, kM, kA1, kMF, kLog, kGate, kUb, kZmean, kGstat, kPstat, kS1f, kF1, kBufs };
   Workspace<kBufs> ws;
   // the workspace's buffers as reserve last left them: planes with their row pitch, and fp32
-  View in, X, Hh, R, Z, N, CAT, M, A1, gp, s1, zm, pp;
+  View in, X, Hh, R, Z, N, CAT, M, A1;
   float *MF = nullptr, *LOG = nullptr, *gate = nullptr, *ub = nullptr, *zmean = nullptr, *gstat = nullptr, *pstat = nullptr;
   float* s1f = nullptr;   // (B, se_dim) fp32: hidden vector of the SE gate
   float* f1 = nullptr;    // (B, fc1_dim) fp32: output of fc1 when the model has one
@@ -297,19 +295,17 @@ static int reserve(xvb_ecapa* h, int B, int T) {
   const Model* m = h->m.get();
   const size_t b = (size_t)B, f = (size_t)B * T, C = (size_t)m->cfg.C, D = (size_t)m->cfg.D;
   const size_t need[H::kBufs] = {(f + b * (h->im2col.pad_front + h->im2col.pad_back)) * m->cfg.ldf, f * C, f * C, f * C, f * C,
-                                 f * C, f * 3 * C, f * D, f * m->cfg.H, b * 2 * D, b * m->se_dim, b * C, b * m->cfg.P2,
-                                 f * D, f * m->cfg.ldlog, b * C, b * m->cfg.AX, b * C, b * 2 * D, b * m->cfg.P2, b * m->se_dim,
-                                 b * m->fc1_dim};
+                                 f * C, f * 3 * C, f * D, f * m->cfg.H, f * D, f * m->cfg.ldlog, b * C, b * m->cfg.AX, b * C,
+                                 b * 2 * D, b * m->cfg.P2, b * m->se_dim, b * m->fc1_dim};
   bool planes[H::kBufs];
-  for (int i = 0; i < H::kBufs; ++i) planes[i] = i <= H::kPp;
+  for (int i = 0; i < H::kBufs; ++i) planes[i] = i <= H::kA1;
   uint64_t grown;
   const int rc = h->ws.reserve(need, planes, &grown);
   if (rc) return rc;
   auto view = [&](int i, int64_t ld) { const Planes p = h->ws.planes(i); return View{p.hi, p.lo, ld}; };
   h->in = view(H::kIn, m->cfg.ldf); h->X = view(H::kX, C); h->Hh = view(H::kH, C); h->R = view(H::kR, C);
   h->Z = view(H::kZ, C); h->N = view(H::kN, C); h->CAT = view(H::kCat, 3 * C); h->M = view(H::kM, D);
-  h->A1 = view(H::kA1, m->cfg.H); h->gp = view(H::kGp, 2 * D); h->s1 = view(H::kS1, m->se_dim); h->zm = view(H::kZm, C);
-  h->pp = view(H::kPp, m->cfg.P2);
+  h->A1 = view(H::kA1, m->cfg.H);
   h->MF = h->ws.f32(H::kMF); h->LOG = h->ws.f32(H::kLog); h->gate = h->ws.f32(H::kGate); h->ub = h->ws.f32(H::kUb);
   h->zmean = h->ws.f32(H::kZmean); h->gstat = h->ws.f32(H::kGstat); h->pstat = h->ws.f32(H::kPstat);
   h->s1f = h->ws.f32(H::kS1f); h->f1 = h->ws.f32(H::kF1);
@@ -333,10 +329,6 @@ struct Run {   // one layer launch: fill only what differs from the defaults
 int small_layer(const ELayer* L, const float* x, int64_t ldx, int B, float* y, int64_t ldy, int extra_flags, void* stream) {
   return xvb_small_affine(x, ldx, L->w_f32, B, L->Cin, L->Cout, L->bias, L->scale, L->shift, L->flags | extra_flags, y, ldy,
                           nullptr, nullptr, 0, stream);
-}
-bool small_ok(const ELayer* L) {
-  static const int knob = getenv("XVB_ECAPA_SMALL") ? atoi(getenv("XVB_ECAPA_SMALL")) : 1;
-  return knob && L->w_f32 != nullptr;
 }
 int launch(const Run& r, void* stream) {
   xvb_tdnn_args_t a{};
@@ -367,14 +359,8 @@ static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
   const ELayer* ax = &m->att_x;
   int rc;
   if (m->cfg.mq_tatt) {
-    if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 0, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
-    const ELayer* gs = &m->att_gs;
-    if (small_ok(gs)) {
-      if ((rc = small_layer(gs, h->gstat, 2 * D, B, h->ub, m->cfg.AX, 0, stream))) return rc;
-    } else {
-      Run r{}; r.B = B; r.T = 1; r.L = gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->cfg.AX;
-      if ((rc = launch(r, stream))) return rc;
-    }
+    if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 0, h->gstat, nullptr, nullptr, 0, stream))) return rc;
+    if ((rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.AX, 0, stream))) return rc;
   }
   Run r{}; r.B = B; r.T = T; r.L = ax; r.x = h->M;
   if (m->cfg.mq_tatt) { r.utt_bias = h->ub; r.ld_utt = m->cfg.AX; }
@@ -386,7 +372,7 @@ static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
     if ((rc = launch(r, stream))) return rc;
   }
   return xvb_attn_head_stats_pool_mq(h->LOG, m->cfg.ldlog, m->cfg.NL, h->MF, D, B, T, D, m->cfg.mq_q * D, m->cfg.mq_share ? cg : 1, cg, m->cfg.mq_q,
-                                     1e-5f, 0, h->pstat, h->pp.hi, h->pp.lo, m->cfg.P2, stream);
+                                     1e-5f, 0, h->pstat, nullptr, nullptr, 0, stream);
 }
 
 extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int T, float* emb, void* stream) {
@@ -423,18 +409,10 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
       return rc;
     r = Run{}; r.B = B; r.T = T; r.L = &k.bn2; r.x = h->R; r.y = h->Z;
     if ((rc = launch(r, stream))) return rc;
-    if ((rc = xvb_plane_mean(h->Z.hi, h->Z.lo, C, B, T, C, h->zmean, h->zm.hi, h->zm.lo, C, stream))) return rc;
-    if (small_ok(&k.se1) && small_ok(&k.se2)) {
-      rc = small_layer(&k.se1, h->zmean, C, B, h->s1f, m->se_dim, 0, stream);
-      if (rc) return rc;
-      rc = small_layer(&k.se2, h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream);
-      if (rc) return rc;
-    } else {
-      r = Run{}; r.B = B; r.T = 1; r.L = &k.se1; r.x = h->zm; r.y = h->s1;
-      if ((rc = launch(r, stream))) return rc;
-      r = Run{}; r.B = B; r.T = 1; r.L = &k.se2; r.x = h->s1; r.y_f32 = h->gate; r.ldyf = C; r.extra_flags = XVB_SIGMOID;
-      if ((rc = launch(r, stream))) return rc;
-    }
+    if ((rc = xvb_plane_mean(h->Z.hi, h->Z.lo, C, B, T, C, h->zmean, nullptr, nullptr, 0, stream)) ||
+        (rc = small_layer(&k.se1, h->zmean, C, B, h->s1f, m->se_dim, 0, stream)) ||
+        (rc = small_layer(&k.se2, h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream)))
+      return rc;
     const bool last = b == 2;
     const View slot = h->CAT.slice(C * b);
     if ((rc = xvb_se_apply(h->Z.hi, h->Z.lo, C, cur.hi, cur.lo, cur.ld, h->gate, slot.hi, slot.lo, slot.ld,
@@ -447,19 +425,14 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   if (m->cfg.mq) {
     if ((rc = mqmha_pool(h, B, T, stream))) return rc;
   } else {
-  if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, h->gp.hi, h->gp.lo, 2 * D, stream))) return rc;
-  if (small_ok(&m->att_gs)) {
-    rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream);
-      if (rc) return rc;
-  } else {
-    r = Run{}; r.B = B; r.T = 1; r.L = &m->att_gs; r.x = h->gp; r.y_f32 = h->ub; r.ldyf = m->cfg.H;
-    if ((rc = launch(r, stream))) return rc;
-  }
+  if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, nullptr, nullptr, 0, stream)) ||
+      (rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream)))
+    return rc;
   r = Run{}; r.B = B; r.T = T; r.L = &m->att_x; r.x = h->M; r.y = h->A1; r.utt_bias = h->ub; r.ld_utt = m->cfg.H; r.extra_flags = XVB_TANH;
   if ((rc = launch(r, stream))) return rc;
   r = Run{}; r.B = B; r.T = T; r.L = &m->att2; r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = D;
   if ((rc = launch(r, stream))) return rc;
-  if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, h->pp.hi, h->pp.lo, 2 * D, stream))) return rc;
+  if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, nullptr, nullptr, 0, stream))) return rc;
   }
   if (m->fc1.Cout) {              // fc1 [-> fc2] on CUDA cores (fp32)
     const ELayer* fc1 = &m->fc1;
@@ -471,12 +444,8 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
       rc = small_layer(fc2, h->f1, fc1->Cout, B, emb, m->cfg.E, 0, stream);
       if (rc) return rc;
     }
-  } else if (small_ok(&m->fc2)) {
-    rc = small_layer(&m->fc2, h->pstat, m->cfg.P2, B, emb, m->cfg.E, 0, stream);
-      if (rc) return rc;
-  } else {
-    r = Run{}; r.B = B; r.T = 1; r.L = &m->fc2; r.x = h->pp; r.y_f32 = emb; r.ldyf = m->cfg.E;   // reads the first P of P2 columns
-    if ((rc = launch(r, stream))) return rc;
+  } else if ((rc = small_layer(&m->fc2, h->pstat, m->cfg.P2, B, emb, m->cfg.E, 0, stream))) {
+    return rc;
   }
   h->last_launches = (int)(g_launches - before);
   return XVB_OK;

@@ -21,6 +21,7 @@ build_extractor() returns NativeCamPPExtractor: the same launch sequence in the 
 which also writes XVBP0001 model files for bin/xvb-extract.  XVB_CAMPP_NATIVE=0 selects CamPPExtractor, the Python driver
 of the same kernels with the same embeddings bit for bit."""
 import ctypes as C
+import math
 import os
 import sys
 from collections import OrderedDict
@@ -246,20 +247,11 @@ def _fold(w, bn, bias=None):
     return w.detach().float() * s.view(-1, *([1] * (w.dim() - 1))), b
 
 
-class _Conv:
-    """A bias-free Conv2d packed for xvb_conv2d, with its eval BatchNorm as the epilogue's scale / shift."""
-
-    def __init__(self, conv, bn, device):
-        self.w = ops.pack_conv2d_weight(conv.weight.detach().float().to(device).contiguous())
-        s, t = fold_batchnorm(bn)
-        self.scale, self.shift = torch.from_numpy(s).to(device), torch.from_numpy(t).to(device)
-
-
 class _Lin:
-    """A kernel-size-1 (or dilated k = 3) Conv1d packed for the layer kernel, with its bias and ReLU."""
+    """A kernel-size-1 (or dilated k = 3) Conv1d record packed for the layer kernel, with its bias and ReLU."""
 
     def __init__(self, w, bias, device, context=(0,), relu=False):
-        w = w.detach().float().to(device)
+        w = _vec(w, device)
         self.cout = w.shape[0]
         self.context = list(context)
         w = w.reshape(self.cout, w.shape[1], -1)
@@ -269,7 +261,7 @@ class _Lin:
             full[:, :, [c - self.context[0] for c in self.context]] = w
             w = full
         self.w = ops.pack_tdnn_weight(w.contiguous(), self.context)
-        self.bias = bias.detach().float().to(device).contiguous() if bias is not None else None
+        self.bias = _vec(bias, device) if bias is not None else None
         self.relu = relu
 
     def run(self, x, **kw):
@@ -282,49 +274,61 @@ def _vec(t, device):
 
 class CamPPExtractor:
     """Folded weights on one device + the launch sequence of CamPP.forward for one chunk per utterance (all utterances of
-    a call have the same length), driven from Python over a workspace reused while the batch shape stays the same."""
+    a call have the same length), driven from Python over a workspace reused while the batch shape stays the same.  The
+    weights are the records and configuration the native handle takes (native_records, native_config), each reshaped
+    back from its (rows, cols) form."""
 
     def __init__(self, m, device):
-        self.device, self.feat_dim, self.embed_dim = device, m.inputs_dim, m.embd_dim
-        self.f8 = m.inputs_dim // 8
-        h = m.head
-        s1, t1 = fold_batchnorm(h.bn1)
-        self.conv1 = (_vec(h.conv1.weight, device), _vec(s1, device), _vec(t1, device))   # fp32 as stored: xvb_conv2d_head
+        from asv_subtools_b200._lib import RELU
+        recs = {r[0]: r[1:] for r in native_records(m)}
+        cfg = native_config(m)
+        self.device, self.feat_dim, self.embed_dim = device, cfg["feat_dim"], cfg["embd_dim"]
+        self.f8 = self.feat_dim // 8
+        self.g, self.bn_ch = cfg["growth_rate"], cfg["bn_size"] * cfg["growth_rate"]
+
+        def conv(name, cin):
+            """(fp32 weight (Cout, Cin, k, k), scale, shift) of a bias-free Conv2d record with its folded BatchNorm."""
+            w, _, sc, sh, _, _ = recs[name]
+            k = math.isqrt(w.shape[1] // cin)
+            return _vec(w.reshape(w.shape[0], cin, k, k), device), _vec(sc, device), _vec(sh, device)
+
+        def packed(name):
+            w, sc, sh = conv(name, M_CHANNELS)
+            return ops.pack_conv2d_weight(w), sc, sh
+
+        self.conv1 = conv("head.conv1", 1)      # fp32 as stored: xvb_conv2d_head
         self.res_blocks = []
-        for layer in (h.layer1, h.layer2):
-            for blk in layer:
-                sc = _Conv(blk.shortcut[0], blk.shortcut[1], device) if len(blk.shortcut) else None
-                self.res_blocks.append((blk.stride, _Conv(blk.conv1, blk.bn1, device), _Conv(blk.conv2, blk.bn2, device), sc))
-        self.conv2 = _Conv(h.conv2, h.bn2, device)
-        xv = m.xvector
-        w, b = _fold(tdnn_im2col_weight(xv.tdnn.linear.weight.detach().float(), M_CHANNELS, self.f8).to(device),
-                     xv.tdnn.nonlinear[0], xv.tdnn.linear.bias.to(device))
+        for li in (1, 2):
+            for i in range(2):
+                p = "head.layer{}.{}.".format(li, i)
+                sc = packed(p + "shortcut.0") if p + "shortcut.0" in recs else None
+                self.res_blocks.append((2 if i == 0 else 1, packed(p + "conv1"), packed(p + "conv2"), sc))
+        self.conv2 = packed("head.conv2")
+        w, b = recs["xvector.tdnn.linear"][:2]
         self.tdnn = _Lin(w, b, device, relu=True)
-        self.g, self.bn_ch = m.growth_rate, m.bn_channels
-        self.blocks, self.transits = [], []
+        self.blocks, self.transits, self.widths = [], [], []
         for i, (layers, dilation) in enumerate(BLOCKS):
-            blk = getattr(xv, "block%d" % (i + 1))
             L = []
-            for layer in blk:
-                s1, t1 = fold_batchnorm(layer.nonlinear1.batchnorm)
-                w1, b1 = _fold(layer.linear1.weight.to(device), layer.nonlinear2.batchnorm)
-                cam = layer.cam_layer
+            for li in range(layers):
+                p = "xvector.block{}.tdnnd{}.".format(i + 1, li + 1)
+                q = p + "cam_layer."
+                s1, t1 = recs[p + "nonlinear1"][2:4]
+                w1, b1 = recs[p + "linear1"][:2]
+                local = recs[q + "linear_local"][0]
                 L.append({"s1": _vec(s1, device), "t1": _vec(t1, device), "lin1": _Lin(w1, b1, device, relu=True),
-                          "local": _Lin(cam.linear_local.weight, None, device, context=(-dilation, 0, dilation)),
-                          "gate": tuple(_vec(p.reshape(p.shape[0], -1), device) for p in
-                                        (cam.linear1.weight, cam.linear1.bias, cam.linear2.weight, cam.linear2.bias))})
+                          "local": _Lin(local.reshape(local.shape[0], self.bn_ch, -1), None, device,
+                                        context=(-dilation, 0, dilation)),
+                          "gate": tuple(_vec(a.reshape(a.shape[0], -1), device)
+                                        for name in ("linear1", "linear2") for a in recs[q + name][:2])})
             self.blocks.append(L)
-            tr = getattr(xv, "transit%d" % (i + 1))
-            s, t = fold_batchnorm(tr.nonlinear.batchnorm)
-            if i < 2:
-                lin = _Lin(tr.linear.weight, None, device)
-            else:                                   # out_nonlinear's BN -> ReLU folded into transit3
-                wt, bt = _fold(tr.linear.weight.to(device), xv.out_nonlinear.batchnorm)
-                lin = _Lin(wt, bt, device, relu=True)
-            self.transits.append((_vec(s, device), _vec(t, device), lin))
-        self.widths = list(m.widths)
-        ds, dt = fold_batchnorm(xv.dense.nonlinear[1])
-        self.dense = (_vec(xv.dense.linear.weight.reshape(self.embed_dim, -1), device), _vec(ds, device), _vec(dt, device))
+            p = "xvector.transit{}.".format(i + 1)
+            s, sh = recs[p + "nonlinear"][2:4]
+            w, b, _, _, flags, _ = recs[p + "linear"]
+            self.transits.append((_vec(s, device), _vec(sh, device),
+                                  _Lin(w, b, device, relu=bool(flags & RELU))))
+            self.widths.append(s.shape[0])
+        w, _, ds, dt, _, _ = recs["xvector.dense.linear"]
+        self.dense = (_vec(w, device), _vec(ds, device), _vec(dt, device))
         self._ws_key, self._ws = None, None
         self.last_launches = 0
 
@@ -371,14 +375,14 @@ class CamPPExtractor:
             res = x
             if sc is not None:
                 res = ws["s%d" % j]
-                ops.conv2d(x, sc.w, m, 1, stride, sc.scale, sc.shift, y=res, stride_t=1)
+                ops.conv2d(x, sc[0], m, 1, stride, sc[1], sc[2], y=res, stride_t=1)
                 n += 1
-            ops.conv2d(x, c1.w, m, 3, stride, c1.scale, c1.shift, relu=True, y=ws["a%d" % j], stride_t=1)
-            ops.conv2d(ws["a%d" % j], c2.w, m, 3, 1, c2.scale, c2.shift, res=res, relu=True, y=ws["o%d" % j])
+            ops.conv2d(x, c1[0], m, 3, stride, c1[1], c1[2], relu=True, y=ws["a%d" % j], stride_t=1)
+            ops.conv2d(ws["a%d" % j], c2[0], m, 3, 1, c2[1], c2[2], res=res, relu=True, y=ws["o%d" % j])
             n += 2
             x = ws["o%d" % j]
         c = self.conv2
-        ops.conv2d(x, c.w, m, 3, 2, c.scale, c.shift, relu=True, y=ws["c2"], stride_t=1)
+        ops.conv2d(x, c[0], m, 3, 2, c[1], c[2], relu=True, y=ws["c2"], stride_t=1)
         # the head output into the time-padded copy: one row of T * F'' * C elements per utterance
         row = self.f8 * m
         pad, src = ws["pad"], ws["c2"]
@@ -439,9 +443,9 @@ def native_config(m):
 
 
 def native_records(m):
-    """(name, w, bias, scale, shift, flags, keys) records for xvb_campp_set_layer, after the hand-over folds of
-    CamPPExtractor.__init__: every BatchNorm folded to scale / shift or into the preceding conv, the `tdnn` weight in the
-    im2col column order, out_nonlinear folded into transit3.  `keys` are the state_dict entries the record carries."""
+    """(name, w, bias, scale, shift, flags, keys) records for xvb_campp_set_layer and CamPPExtractor, after the hand-over
+    folds: every BatchNorm folded to scale / shift or into the preceding conv, the `tdnn` weight in the im2col column
+    order, out_nonlinear folded into transit3.  `keys` are the state_dict entries the record carries."""
     from asv_subtools_b200._lib import BN, RELU
     f = lambda t: None if t is None else (t.detach().float().cpu().numpy() if isinstance(t, torch.Tensor) else t)  # noqa: E731
     out = []

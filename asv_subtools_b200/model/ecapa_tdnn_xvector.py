@@ -151,12 +151,14 @@ class ECAPA_TDNN(TopVirtualNnet):
 
 
 class _Layer:
-    """Device-side packed parameters of one TDNN / 1x1-conv layer.  groups > 1: a grouped 1x1 conv with its weight as
-    stored, (Cout, Cin/groups, 1), packed compactly for the layer kernel's grouped mode, or as its block-diagonal
-    expansion when the shape does not fit that mode (ops.tdnn_grouped_fits)."""
+    """Device-side packed parameters of one TDNN / 1x1-conv layer record of _named_layers (name, weight (Cout, Cin, tot),
+    bias, context, scale, shift, relu).  groups > 1: a grouped 1x1 conv with its weight as stored, (Cout, Cin/groups, 1),
+    packed compactly for the layer kernel's grouped mode, or as its block-diagonal expansion when the shape does not fit
+    that mode (ops.tdnn_grouped_fits)."""
 
-    def __init__(self, weight, bias, context, bn=None, relu=False, device=None, scale_shift=None, groups=1):
-        w = weight.detach().float().to(device).contiguous()
+    def __init__(self, rec, device, groups=1):
+        _, w, bias, context, scale, shift, relu = rec
+        w = torch.from_numpy(w).to(device).contiguous()
         self.context = list(context)
         self.groups = 1
         if groups > 1:
@@ -168,9 +170,8 @@ class _Layer:
         self.cout = w.shape[0]
         # one-tap layers keep the (N, K) fp32 matrix too: the segment-level ones run on CUDA cores (ops.small_affine)
         self.w_f32 = w[:, :, 0].contiguous() if w.shape[2] == 1 and w.shape[1] % 4 == 0 else None
-        self.bias = bias.detach().float().to(device).contiguous() if bias is not None else None
+        self.bias = torch.from_numpy(bias).to(device).contiguous() if bias is not None else None
         self.relu = relu
-        scale, shift = scale_shift if scale_shift is not None else fold_batchnorm(bn)
         self.scale = torch.from_numpy(scale).to(device) if scale is not None else None
         self.shift = torch.from_numpy(shift).to(device) if shift is not None else None
 
@@ -226,7 +227,6 @@ def _mqmha_attention(st):
 NATIVE_CHANNELS = (512, 1024)
 CHAIN_WIDTHS = (64, 128)
 _PROFILE = None  # list of (label, cuda event) when profiling (tools/bench_ecapa.py --profile)
-SMALL_ROWS = os.environ.get("XVB_ECAPA_SMALL", "1") != "0"   # segment-level layers on CUDA cores (csrc/ecapa.cu small_affine)
 
 
 def _mark(label):
@@ -294,6 +294,17 @@ def _segment_layers(m):
     return out
 
 
+def native_config(m):
+    """{"create": the arguments of xvb_ecapa_create after the handle, "mqmha": those of xvb_ecapa_set_mqmha, or None for
+    the attentive pooling} for model m."""
+    st = m.stats
+    mq = isinstance(st, MQMHASP)
+    hidden = st.hidden_size * st.num_head * st.num_q if mq else st.attention[0].out_channels
+    return {"create": (m.inputs_dim, m.layer1.affine.output_dim, st.in_dim, hidden, m.embd_dim),
+            "mqmha": (st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers, int(st.time_attention),
+                      int(st.stddev)) if mq else None}
+
+
 class NativeEcapaExtractor(ShardExtractor):
     """xvb_ecapa_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
     current when it is built (or loaded from an XVBE0001 / XVBE0002 file)."""
@@ -301,15 +312,12 @@ class NativeEcapaExtractor(ShardExtractor):
     PREFIX = "ecapa"
 
     def _create_args(self, m):
-        st = m.stats
-        hidden = st.hidden_size * st.num_head * st.num_q if isinstance(st, MQMHASP) else st.attention[0].out_channels
-        return m.inputs_dim, m.layer1.affine.output_dim, st.in_dim, hidden, m.embd_dim
+        return native_config(m)["create"]
 
     def _configure(self, m):
-        st = m.stats
-        if isinstance(st, MQMHASP):
-            self._call("set_mqmha", self._h, st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers,
-                       int(st.time_attention), int(st.stddev))
+        mq = native_config(m)["mqmha"]
+        if mq is not None:
+            self._call("set_mqmha", self._h, *mq)
 
     def _layers(self, m):
         from asv_subtools_b200._lib import int_array
@@ -323,56 +331,50 @@ class NativeEcapaExtractor(ShardExtractor):
 class EcapaExtractor:
     """Packed weights on one device + the launch sequence of ECAPA_TDNN.extract_embedding (:403-426), driven from
     Python op by op: the A/B and profiling twin of NativeEcapaExtractor (XVB_ECAPA_NATIVE=0, tools/bench_ecapa.py
-    --profile)."""
+    --profile), and the path for channel counts the handle does not take.  The weights are the records and configuration
+    the handle takes (_named_layers, native_config); the Res2Net stack, its dilation, scale and width come from the
+    layerN.resI records, and the MQMHA attention convs are grouped by the handle's rule (att_x: heads, att2: heads x
+    queries)."""
 
     def __init__(self, m, device):
+        recs = {r[0]: r for r in _named_layers(m)}
+        cfg = native_config(m)
         self.device = device
-        self.feat_dim = m.inputs_dim
-        self.ldf = (m.inputs_dim + 7) // 8 * 8
+        self.feat_dim, self.channels, self.mfa_dim, _, self.embed_dim = cfg["create"]
+        self.ldf = (self.feat_dim + 7) // 8 * 8
         self.last_launches = 0
-
-        def tdnn(layer):
-            return _Layer(layer.affine.weight, layer.affine.bias, layer.affine.context, bn=layer.batchnorm,
-                          relu=layer.relu, device=device)
-
-        self.layer1 = tdnn(m.layer1)
+        mq = cfg["mqmha"]
+        self.mq = None if mq is None else dict(zip(("heads", "q", "hidden", "share", "layers", "tatt", "stddev"), mq))
+        # groups of the MQMHA attention convs as the state_dict stores them (pooling.py:665-698)
+        groups = {} if mq is None else {"att_x": self.mq["heads"], "att2": self.mq["heads"] * self.mq["q"]}
+        layer = lambda name: _Layer(recs[name], device, groups.get(name, 1))  # noqa: E731
+        self.layer1 = layer("layer1")
         self.blocks = []
         self.chain = os.environ.get("XVB_ECAPA_RES2NET", "chain") != "gemm"   # one persistent kernel per Res2Net block
-        for blk in (m.layer2, m.layer3, m.layer4):
-            res = [tdnn(b) for b in blk.res2net_block.blocks]
+        for li in (2, 3, 4):
+            p = "layer{}.".format(li)
+            res = [layer(n) for n in recs if n.startswith(p + "res")]      # res0 .. res{scale - 2}, in order
             self.blocks.append({
-                "bn1": tdnn(blk.conv_relu_bn1),
+                "bn1": layer(p + "bn1"),
                 "res": res,
                 "res_w_hi": torch.cat([r.w.hi for r in res], dim=0).contiguous(),
                 "res_w_lo": torch.cat([r.w.lo for r in res], dim=0).contiguous(),
                 "res_bias": torch.cat([r.bias for r in res]).contiguous(),
                 "res_scale": torch.cat([r.scale for r in res]).contiguous(),
                 "res_shift": torch.cat([r.shift for r in res]).contiguous(),
-                "dilation": blk.res2net_block.context[-1],
-                "nscale": blk.res2net_block.scale,
-                "width": blk.res2net_block.width,
-                "bn2": tdnn(blk.conv_relu_bn2),
-                "se1": _Layer(blk.se.se[1].weight, blk.se.se[1].bias, [0], relu=True, device=device),
-                "se2": _Layer(blk.se.se[3].weight, blk.se.se[3].bias, [0], device=device),
+                "dilation": res[0].context[-1],
+                "nscale": len(res) + 1,
+                "width": res[0].cout,
+                "bn2": layer(p + "bn2"),
+                "se1": layer(p + "se1"),
+                "se2": layer(p + "se2"),
             })
-        self.channels = m.layer1.affine.output_dim
-        self.mfa = tdnn(m.mfa)
-        self.mfa_dim = m.stats.in_dim
-        self.segment = [_Layer(torch.from_numpy(w), torch.from_numpy(b), ctx, relu=relu, device=device, scale_shift=(scale, shift))
-                        for _, w, b, ctx, scale, shift, relu in _segment_layers(m)]
-        self.embed_dim = m.embd_dim
-        self.mq = m.stats if isinstance(m.stats, MQMHASP) else None
+        self.mfa = layer("mfa")
+        self.segment = [layer(name) for name in ("fc1", "fc2") if name in recs]
         if self.mq is not None:
-            self.att = {name: _Layer(torch.from_numpy(w), None if b is None else torch.from_numpy(b), [0], relu=relu, device=device,
-                                     scale_shift=bn if bn is not None else (None, None), groups=g)
-                        for name, w, b, bn, relu, g in _mqmha_attention(self.mq)}
+            self.att = {name: layer(name) for name in ("att_x", "att_gs", "att2") if name in recs}
             return
-        att = m.stats.attention
-        c = m.stats.in_dim
-        w0 = att[0].weight.detach().float()
-        self.att_x = _Layer(w0[:, :c].contiguous(), None, [0], bn=att[2], relu=True, device=device)
-        self.att_gs = _Layer(w0[:, c:].contiguous(), att[0].bias, [0], device=device)  # [mean | std] columns
-        self.att2 = _Layer(att[4].weight, att[4].bias, [0], device=device)
+        self.att_x, self.att_gs, self.att2 = layer("att_x"), layer("att_gs"), layer("att2")
 
     def extract(self, feats):
         """feats (B,T,F) fp32 CUDA -> (B, embd_dim) fp32 CUDA (asynchronous on the current stream)."""
@@ -389,8 +391,6 @@ class EcapaExtractor:
         H, R, Z = P.empty((B, T, C), dev), P.empty((B, T, C), dev), P.empty((B, T, C), dev)
         N = P.empty((B, T, C), dev)
         CAT = P.empty((B, T, 3 * C), dev)
-        gate = torch.empty(B, 1, C, dtype=torch.float32, device=dev)
-        s1 = P.empty((B, 1, self.blocks[0]["se1"].cout), dev)
         cur = X
         for li, blk in enumerate(self.blocks):
             w = blk["width"]
@@ -406,13 +406,9 @@ class EcapaExtractor:
                     layer.run(H.slice(w * (i + 1), w * (i + 2)), x2=R.slice(w * i, w * (i + 1)) if i >= 1 else None,
                               y=R.slice(w * (i + 1), w * (i + 2)))
             blk["bn2"].run(R, y=Z)
-            zmean, zm = ops.plane_mean(Z)
+            zmean, _ = ops.plane_mean(Z, planes=False)
             _mark("plane_mean")
-            if SMALL_ROWS:
-                gate = blk["se2"].run_rows(blk["se1"].run_rows(zmean), sigmoid=True).view(B, 1, C)
-            else:
-                blk["se1"].run(zm, y=s1)
-                blk["se2"].run(s1, sigmoid=True, y_f32=gate)
+            gate = blk["se2"].run_rows(blk["se1"].run_rows(zmean), sigmoid=True)
             last = li + 1 == len(self.blocks)
             ops.se_apply(Z, cur, gate.view(B, C), CAT.slice(C * li, C * (li + 1)), None if last else N)
             _mark("se_apply")
@@ -423,65 +419,45 @@ class EcapaExtractor:
         self.mfa.run(CAT, y=M, y_f32=MF)
         if self.mq is not None:
             return self._mqmha_tail(M, MF)
-        gstat, gp = ops.stats_pool_ex(MF, 1e-5, 1, planes=True)      # global mean | sqrt(var_unbiased + 1e-5)
+        gstat = ops.stats_pool_ex(MF, 1e-5, 1)      # global mean | sqrt(var_unbiased + 1e-5)
         _mark("stats_pool(global)")
-        if SMALL_ROWS:
-            ub = self.att_gs.run_rows(gstat)
-        else:
-            ub = torch.empty(B, 1, self.att_gs.cout, dtype=torch.float32, device=dev)
-            self.att_gs.run(gp, y_f32=ub)
+        ub = self.att_gs.run_rows(gstat)
         A1 = P.empty((B, T, self.att_x.cout), dev)
         self.att_x.run(M, utt_bias=ub.view(B, -1), tanh=True, y=A1)
         LOG = torch.empty(B, T, D, dtype=torch.float32, device=dev)
         self.att2.run(A1, y_f32=LOG)
-        pstat, pp = ops.attn_stats_pool(LOG, MF, 1e-5, planes=True)
+        x = ops.attn_stats_pool(LOG, MF, 1e-5)
         _mark("attn_stats_pool")
-        if SMALL_ROWS or len(self.segment) > 1:
-            x = pstat
-            for layer in self.segment:
-                x = layer.run_rows(x)
-            return x
-        emb = torch.empty(B, 1, self.embed_dim, dtype=torch.float32, device=dev)
-        self.segment[0].run(pp, y_f32=emb)
-        return emb.view(B, self.embed_dim)
+        for layer in self.segment:
+            x = layer.run_rows(x)
+        return x
 
     def _mqmha_tail(self, M, MF):
         """MQMHASP.forward (pooling.py:627-663) + the segment layers, in the native extractor's launch order."""
-        st, att = self.mq, self.att
+        mq, att = self.mq, self.att
         B, T, D = MF.shape
         dev = MF.device
         P = ops.SplitPlanes
+        cg = D // mq["heads"]
         ub = None
-        if st.time_attention:        # egrecho's compute_statistics: biased variance clamped at 1e-5
-            gstat, gp = ops.stats_pool_ex(MF, 1e-5, 0, planes=True)
+        if mq["tatt"]:        # egrecho's compute_statistics: biased variance clamped at 1e-5
+            gstat = ops.stats_pool_ex(MF, 1e-5, 0)
             _mark("stats_pool(global)")
-            if SMALL_ROWS:
-                ub = att["att_gs"].run_rows(gstat[:, :att["att_gs"].w_f32.shape[1]].contiguous())
-            else:
-                ub = torch.empty(B, 1, att["att_gs"].cout, dtype=torch.float32, device=dev)
-                att["att_gs"].run(gp.slice(0, att["att_gs"].w_f32.shape[1]), y_f32=ub)
-            ub = ub.view(B, -1)
-        nl = st.num_logits()
+            ub = att["att_gs"].run_rows(gstat[:, :att["att_gs"].w_f32.shape[1]].contiguous()).view(B, -1)
+        nl = (1 if mq["share"] else cg) * mq["heads"] * mq["q"]
         LOG = torch.empty(B, T, (nl + 3) // 4 * 4, dtype=torch.float32, device=dev)
-        if st.affine_layers == 2:
+        if mq["layers"] == 2:
             A1 = P.empty((B, T, att["att_x"].cout), dev)
             att["att_x"].run(M, utt_bias=ub, tanh=True, y=A1)
             att["att2"].run(A1, y_f32=LOG)
         else:
             att["att_x"].run(M, utt_bias=ub, y_f32=LOG)
-        cg = st.head_width()
-        pstat, pp = ops.attn_head_stats_pool_mq(LOG[..., :nl], MF, st.num_q * D, cg if st.share else 1, cg, st.num_q, floor=1e-5,
-                                                planes=True)
+        pstat = ops.attn_head_stats_pool_mq(LOG[..., :nl], MF, mq["q"] * D, cg if mq["share"] else 1, cg, mq["q"], floor=1e-5)
         _mark("attn_head_stats_pool_mq")
-        width = st.get_output_dim()
-        if SMALL_ROWS or len(self.segment) > 1:
-            x = pstat[:, :width].contiguous()
-            for layer in self.segment:
-                x = layer.run_rows(x)
-            return x
-        emb = torch.empty(B, 1, self.embed_dim, dtype=torch.float32, device=dev)
-        self.segment[0].run(pp.slice(0, width), y_f32=emb)
-        return emb.view(B, self.embed_dim)
+        x = pstat[:, :(2 if mq["stddev"] else 1) * mq["q"] * D].contiguous()
+        for layer in self.segment:
+            x = layer.run_rows(x)
+        return x
 
     def close(self):
         pass

@@ -290,7 +290,7 @@ def _named_records(m):
     for name, blk in zip(_block_names(m), m.repvgg.blocks()):
         w, b = fold_block(blk)
         out.append((name, f(w), f(b), None, None, True))
-    for name, _, w, b, scale, shift, relu in _segment_chain(m, m.repvgg.get_output_planes()):
+    for name, w, b, scale, shift, relu in _segment_chain(m, m.repvgg.get_output_planes()):
         out.append((name, f(w)[:, :, 0], f(b) if b is not None else None, scale, shift, relu))
     return out
 
@@ -326,27 +326,28 @@ class NativeRepVGGExtractor(NativeExtractor):
 class RepVGGExtractor:
     """Folded weights on one device + the launch sequence of RepVggXvector.extract_embedding (:181-208), driven from
     Python like ResNetExtractor: the head conv (stage0), one tap-list conv per block (bias and ReLU in the epilogue; the
-    last one writes fp32), statistics pooling, the segment layers."""
+    last one writes fp32), statistics pooling, the segment layers.  The weights are the records and configuration the
+    native handle takes (_named_records, native_config)."""
 
     def __init__(self, m, device):
-        blocks = m.repvgg.blocks()
-        w, b = fold_block(blocks[0])
-        self.head_w = w.float().to(device).contiguous()
+        recs = {r[0]: r[1:] for r in _named_records(m)}
+        cfg = native_config(m)
+        w, b = (torch.from_numpy(a) for a in recs["repvgg.stage0"][:2])
+        self.head_w = w.to(device).contiguous()
         self.head_scale = torch.ones(w.shape[0], dtype=torch.float32, device=device)
-        self.head_shift = b.float().to(device)
-        self.feat_dim = m.inputs_dim
+        self.head_shift = b.to(device)
+        self.feat_dim = cfg["feat_dim"]
         self.blocks = []
-        for blk in blocks[1:]:
-            w, b = fold_block(blk)
-            w = w.float()
-            taps = kept_taps(w)
-            self.blocks.append({"stride": blk.stride, "cout": blk.out_channels, "k": blk.window, "taps": taps,
-                                "w": ops.pack_conv2d_weight(w.to(device).contiguous(), taps),
-                                "scale": torch.ones(blk.out_channels, dtype=torch.float32, device=device),
-                                "shift": b.float().to(device)})
-        self.segment = [_PackedAffine(layer.affine, device, relu=relu, arrays=(w, b, scale, shift))
-                        for _, layer, w, b, scale, shift, relu in _segment_chain(m, m.repvgg.get_output_planes())]
-        self.eps = m.stats.eps
+        for si, n in enumerate(cfg["num_blocks"]):
+            for i in range(n):
+                w, b = (torch.from_numpy(a) for a in recs["repvgg.stage{}.{}".format(si + 1, i)][:2])
+                taps = kept_taps(w)
+                self.blocks.append({"stride": cfg["strides"][si + 1] if i == 0 else 1, "cout": w.shape[0],
+                                    "k": cfg["ksize"], "taps": taps, "w": ops.pack_conv2d_weight(w.to(device).contiguous(), taps),
+                                    "scale": torch.ones(w.shape[0], dtype=torch.float32, device=device),
+                                    "shift": b.to(device)})
+        self.segment = [_PackedAffine.from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
+        self.eps = cfg["pooling_eps"]
         self.embed_dim = self.segment[-1].cout_real
 
     def extract(self, feats):

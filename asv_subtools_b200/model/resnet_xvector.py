@@ -183,11 +183,11 @@ def _stats_column_order(c, f):
 
 
 def _segment_chain(m, channels=None):
-    """The segment layers the extracted position uses (:194-206) as (name, layer, w, b, scale, shift, relu): "far" =
-    fc1.affine alone, otherwise [fc1 whole ->] fc2 whole ("near") or fc2.affine ("near_affine"); whole layers through
-    export() (BatchNorm folded to scale / shift, or into the weight for "bn-relu"), the first layer's input columns
-    permuted to the pooling order of (B, T', F', C) frames.  Shared by ResNetExtractor, the native handle and the
-    RepVGG blueprint, which passes the channel count of its last stage (default: the ResNet's last conv2)."""
+    """The segment layers the extracted position uses (:194-206) as (name, w, b, scale, shift, relu): "far" = fc1.affine
+    alone, otherwise [fc1 whole ->] fc2 whole ("near") or fc2.affine ("near_affine"); whole layers through export()
+    (BatchNorm folded to scale / shift, or into the weight for "bn-relu"), the first layer's input columns permuted to the
+    pooling order of (B, T', F', C) frames.  Shared by the ResNet and RepVGG records; RepVGG passes the channel count of
+    its last stage (default: the ResNet's last conv2)."""
     if channels is None:
         channels = m.resnet.blocks()[-1].conv2.out_channels
     perm = torch.from_numpy(_stats_column_order(channels, m.out_freq))
@@ -202,8 +202,16 @@ def _segment_chain(m, channels=None):
             w, b, scale, shift, relu = layer.affine.dense_weight(), layer.affine.bias.detach().float(), None, None, False
         if i == 0:
             w = w[:, perm]
-        out.append((name, layer, w.contiguous(), b, scale, shift, relu))
+        out.append((name, w.contiguous(), b, scale, shift, relu))
     return out
+
+
+def native_config(m):
+    """The arguments of xvb_resnet_create for model m."""
+    r = m.resnet
+    stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
+    return {"feat_dim": m.inputs_dim, "layers": [len(s) for s in stages], "planes": [s[0].conv1.out_channels for s in stages],
+            "pre_activation": r.full_pre_activation, "pooling_eps": float(m.stats.eps)}
 
 
 def _named_records(m):
@@ -237,17 +245,17 @@ def _named_records(m):
             if blk.se is not None:
                 out.append((p + "se.fc_1", f(blk.se.fc_1.weight), f(blk.se.fc_1.bias), None, None, False))
                 out.append((p + "se.fc_2", f(blk.se.fc_2.weight), f(blk.se.fc_2.bias), None, None, False))
-    for name, _, w, b, scale, shift, relu in _segment_chain(m):
+    for name, w, b, scale, shift, relu in _segment_chain(m):
         out.append((name, f(w)[:, :, 0], f(b) if b is not None else None, scale, shift, relu))
     return out
 
 
-def _se_rows(se, device):
-    """SE weights for xvb_small_affine (K % 4 == 0): the hidden width C/r is zero-padded to a multiple of 4; the padded
-    units are relu(0) = 0 and meet zero columns of fc_2, so the gate is unchanged.  fc_1 also comes as
-    w1k[k] = [w1 / k, ..., w1 / k] (k copies, k a power of two, k * C <= 256): fc_1 applied to the mean of k-position
-    groups (see ResNetExtractor._se_gate), which is fc_1 of the mean over all positions."""
-    w1, b1, w2, b2 = (t.detach().float().cpu() for t in (se.fc_1.weight, se.fc_1.bias, se.fc_2.weight, se.fc_2.bias))
+def _se_rows(w1, b1, w2, b2, device):
+    """SE weights (the se.fc_1 / se.fc_2 records) for xvb_small_affine (K % 4 == 0): the hidden width C/r is zero-padded
+    to a multiple of 4; the padded units are relu(0) = 0 and meet zero columns of fc_2, so the gate is unchanged.  fc_1
+    also comes as w1k[k] = [w1 / k, ..., w1 / k] (k copies, k a power of two, k * C <= 256): fc_1 applied to the mean of
+    k-position groups (see ResNetExtractor._se_gate), which is fc_1 of the mean over all positions."""
+    w1, b1, w2, b2 = (torch.from_numpy(a) for a in (w1, b1, w2, b2))
     pad = (-w1.shape[0]) % 4
     if pad:
         w1 = torch.cat([w1, torch.zeros(pad, w1.shape[1])])
@@ -264,34 +272,33 @@ def _se_rows(se, device):
 class ResNetExtractor:
     """Packed weights on one device + the launch sequence of ResNetXvector.extract_embedding (:183-208), driven from Python
     like AttentionPoolingExtractor: per block two convs (+ a 1x1 stride-2 downsample in the first block of layers 2-4)
-    [+ plane mean, two small affines and the SE scaling], then statistics pooling and the segment layers."""
+    [+ plane mean, two small affines and the SE scaling], then statistics pooling and the segment layers.  The weights
+    are the records and configuration the native handle takes (_named_records, native_config)."""
 
     TAKES_LENGTHS = True
 
     def __init__(self, m, device):
-        def bn(b):
-            s, t = fold_batchnorm(b)
-            return torch.from_numpy(s).to(device), torch.from_numpy(t).to(device)
-
-        r = m.resnet
-        self.feat_dim = m.inputs_dim
-        self.pre = r.full_pre_activation
-        self.head_w = r.conv1.weight.detach().float().to(device).contiguous()
-        self.head_bn = bn(r.bn1)
+        recs = {r[0]: r[1:] for r in _named_records(m)}
+        cfg = native_config(m)
+        dev = lambda a: torch.from_numpy(a).to(device)  # noqa: E731
+        conv = lambda name: ops.pack_conv2d_weight(dev(recs[name][0]).contiguous())  # noqa: E731
+        bn = lambda name: (dev(recs[name][2]), dev(recs[name][3]))  # noqa: E731
+        self.feat_dim = cfg["feat_dim"]
+        self.pre = cfg["pre_activation"]
+        self.head_w = dev(recs["resnet.conv1"][0]).contiguous()
+        self.head_bn = bn("resnet.bn1")
         self.blocks = []
-        for blk in r.blocks():
-            ds = blk.downsample
-            self.blocks.append({
-                "stride": blk.stride, "cout": blk.conv1.out_channels,
-                "conv1": ops.pack_conv2d_weight(blk.conv1.weight.detach().float().to(device).contiguous()),
-                "conv2": ops.pack_conv2d_weight(blk.conv2.weight.detach().float().to(device).contiguous()),
-                "bn1": bn(blk.bn1), "bn2": bn(blk.bn2),
-                "ds": None if ds is None else (ops.pack_conv2d_weight(ds[0].weight.detach().float().to(device).contiguous()),
-                                               bn(ds[1])),
-                "se": None if blk.se is None else _se_rows(blk.se, device)})
-        self.segment = [_PackedAffine(layer.affine, device, relu=relu, arrays=(w, b, scale, shift))
-                        for _, layer, w, b, scale, shift, relu in _segment_chain(m)]
-        self.eps = m.stats.eps
+        for li, (n, co) in enumerate(zip(cfg["layers"], cfg["planes"])):
+            for i in range(n):
+                p = "resnet.layer{}.{}.".format(li + 1, i)
+                self.blocks.append({
+                    "stride": 2 if li > 0 and i == 0 else 1, "cout": co,
+                    "conv1": conv(p + "conv1"), "conv2": conv(p + "conv2"), "bn1": bn(p + "bn1"), "bn2": bn(p + "bn2"),
+                    "ds": (conv(p + "downsample.0"), bn(p + "downsample.1")) if p + "downsample.0" in recs else None,
+                    "se": _se_rows(*recs[p + "se.fc_1"][:2], *recs[p + "se.fc_2"][:2], device)
+                    if p + "se.fc_1" in recs else None})
+        self.segment = [_PackedAffine.from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
+        self.eps = cfg["pooling_eps"]
         self.embed_dim = self.segment[-1].cout_real
 
     def _se_gate(self, z, se, lengths=None):
@@ -392,10 +399,9 @@ class NativeResNetExtractor(ShardExtractor):
 
     def _create_args(self, m):
         from asv_subtools_b200._lib import int_array
-        r = m.resnet
-        stages = [getattr(r, "layer{}".format(li)) for li in range(1, 5)]
-        return (m.inputs_dim, int_array([len(s) for s in stages]), int_array([s[0].conv1.out_channels for s in stages]),
-                1 if r.full_pre_activation else 0, float(m.stats.eps))
+        c = native_config(m)
+        return (c["feat_dim"], int_array(c["layers"]), int_array(c["planes"]), 1 if c["pre_activation"] else 0,
+                c["pooling_eps"])
 
     def _layers(self, m):
         for name, w, b, scale, shift, relu in _named_records(m):

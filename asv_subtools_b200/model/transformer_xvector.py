@@ -45,7 +45,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
-from asv_subtools_b200._lib import ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH  # noqa: E402
+from asv_subtools_b200._lib import ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH, BN, RELU, SWISH  # noqa: E402
 from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import TdnnAffine, fold_batchnorm  # noqa: E402
 from asv_subtools_b200.native import NativeExtractor  # noqa: E402
@@ -405,119 +405,93 @@ def softmax_plus_multiplier(frames, train_len):
 
 
 class _Lin:
-    """A Linear / kernel-size-1 conv packed for the wgmma layer kernel: y = epi(W x + b) with ReLU or swish, and an eval
-    BatchNorm (or a constant scale) as the epilogue's scale / shift."""
+    """A Linear / kernel-size-1 conv record (name, w (Cout, Cin), bias, scale, shift, flags, ...) packed for the wgmma layer
+    kernel: y = epi(W x + b) with the record's ReLU or swish, and its folded BatchNorm (or constant scale) as the
+    epilogue's scale / shift."""
 
-    def __init__(self, weight, bias, device, act=ACT_NONE, scale=None, shift=None):
-        w = weight.detach().float().reshape(weight.shape[0], -1)
+    def __init__(self, rec, device):
+        w, b, scale, shift, flags = rec[1:6]
         self.cout, self.cin = w.shape
-        self.w = ops.pack_tdnn_weight(w.to(device).unsqueeze(-1).contiguous(), [0])
-        self.bias = bias.detach().float().to(device).contiguous() if bias is not None else None
-        self.scale = torch.as_tensor(scale, dtype=torch.float32).to(device).contiguous() if scale is not None else None
-        self.shift = torch.as_tensor(shift, dtype=torch.float32).to(device).contiguous() if shift is not None else None
-        self.relu, self.swish = act == ACT_RELU, act == ACT_SWISH
+        self.w = ops.pack_tdnn_weight(_vec(w, device).unsqueeze(-1).contiguous(), [0])
+        self.bias, self.scale, self.shift = _vec(b, device), _vec(scale, device), _vec(shift, device)
+        self.relu, self.swish = bool(flags & RELU), bool(flags & SWISH)
 
     def run(self, x, y=None, y_f32=None):
         ops.tdnn_affine_ex(x, self.w, self.cout, [0], bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
                            relu=self.relu, swish=self.swish, y=y, y_f32=y_f32)
 
 
-def _vec(t, device):
-    return t.detach().float().to(device).contiguous() if t is not None else None
-
-
-def _ln_params(ln, device):
-    return _vec(ln.weight, device), _vec(ln.bias, device)
+def _vec(a, device):
+    return torch.from_numpy(a).to(device).contiguous() if a is not None else None
 
 
 class ConformerExtractor:
     """Folded weights on one device + the launch sequence of TransformerXvector.extract_embedding for one chunk per
-    utterance (all utterances of a call have the same length), driven from Python."""
+    utterance (all utterances of a call have the same length), driven from Python.  The weights and tables are the
+    records and configuration the native handle takes (native_records, native_config)."""
 
     def __init__(self, m, device):
-        enc = m.transformer
-        p = enc.p
-        self.device, self.feat_dim = device, m.inputs_dim
-        self.D, self.H = p["attention_dim"], p["attention_heads"]
+        recs = {r[0]: r for r in native_records(m)}
+        cfg = native_config(m)
+        lin = lambda name: _Lin(recs[name], device)  # noqa: E731
+        norm = lambda name: (_vec(recs[name][3], device), _vec(recs[name][4], device))  # noqa: E731
+
+        def tdnn(name):
+            """(_Lin with the record's activation [and folded BatchNorm], LayerNorm (gamma, beta) or None)."""
+            return lin(name + ".affine"), norm(name + ".batchnorm") if name + ".batchnorm" in recs else None
+
+        self.device, self.feat_dim = device, cfg["feat_dim"]
+        self.D, self.H = cfg["D"], cfg["H"]
         self.dk = self.D // self.H
-        self.pos = p["pos_enc_type"]
-        self.rotary_value = self.pos == "rot_pos" and bool(p["rotary_value"])
-        self.softmax_plus = p["attention_norm_args"]["norm_method"] == "softmax_plus"
-        self.act = ACT_SWISH if p["activation_type"] == "swish" else ACT_RELU
-        self.subsampling = enc.subsampling
-        emb = enc.embed
-        self.head_w = _vec(emb.conv[0].weight, device)
-        self.head_b = _vec(emb.conv[0].bias, device)
-        w2 = emb.conv[2].weight.detach().float().transpose(2, 3).contiguous()   # (C, C, kt, kf) -> (C, C, kf, kt)
-        self.conv2_w = ops.pack_conv2d_weight(w2.to(device))
+        self.pos = ("no_pos", "abs_pos", "rot_pos")[cfg["pos"]]
+        self.rotary_value = self.pos == "rot_pos" and bool(cfg["rotary_value"])
+        self.softmax_plus = bool(cfg["softmax_plus"])
+        self.act = cfg["act"]
+        self.subsampling = cfg["subsampling"]
+        e = "transformer.embed."
+        self.head_w = _vec(recs[e + "conv.0"][1].reshape(self.D, 1, 3, 3), device)
+        self.head_b = _vec(recs[e + "conv.0"][2], device)
+        self.conv2_w = ops.pack_conv2d_weight(_vec(recs[e + "conv.2"][1].reshape(self.D, self.D, 3, 3), device))
         self.conv2_scale = torch.ones(self.D, dtype=torch.float32, device=device)
-        self.conv2_shift = _vec(emb.conv[2].bias, device)
-        self.f2 = subsampled_shape(self.subsampling, MIN_FRAMES, self.feat_dim)[1]
-        lw, xscale = _embed_out_weight(m)
-        self.embed_out = _Lin(lw, emb.out[0].bias, device, scale=xscale,
-                              shift=None if xscale is None else np.zeros(self.D, np.float32))
+        self.conv2_shift = _vec(recs[e + "conv.2"][2], device)
+        self.embed_out = lin(e + "out.0")
         self.layers = []
-        for layer in enc.encoders:
-            a, cm = layer.self_attn, layer.conv_module
-            L = {"ff_mac": (_Lin(layer.feed_forward_macaron.w_1.weight, layer.feed_forward_macaron.w_1.bias, device, self.act),
-                            _Lin(layer.feed_forward_macaron.w_2.weight, layer.feed_forward_macaron.w_2.bias, device)),
-                 "ff": (_Lin(layer.feed_forward.w_1.weight, layer.feed_forward.w_1.bias, device, self.act),
-                        _Lin(layer.feed_forward.w_2.weight, layer.feed_forward.w_2.bias, device)),
-                 "qkv": _Lin(torch.cat([a.linear_q.weight, a.linear_k.weight, a.linear_v.weight], 0),
-                             torch.cat([a.linear_q.bias, a.linear_k.bias, a.linear_v.bias], 0), device),
-                 "out": _Lin(a.linear_out.weight, a.linear_out.bias, device),
-                 "pw1": _Lin(cm.pointwise_conv1.weight, cm.pointwise_conv1.bias, device),
-                 "pw2": _Lin(cm.pointwise_conv2.weight, cm.pointwise_conv2.bias, device),
-                 "dw_w": _vec(cm.depthwise_conv.weight.reshape(self.D, -1), device),
-                 "dw_b": _vec(cm.depthwise_conv.bias, device),
-                 "train_len": a.att_norm.train_len if self.softmax_plus else None}
-            if isinstance(cm.norm, nn.BatchNorm1d):
-                s, t = fold_batchnorm(cm.norm)
-                L["cm_norm"] = (torch.from_numpy(s).to(device), torch.from_numpy(t).to(device), True)
-            else:
-                L["cm_norm"] = _ln_params(cm.norm, device) + (False,)
+        for i in range(cfg["blocks"]):
+            q = "transformer.encoders.{}.".format(i)
+            cm = q + "conv_module."
+            L = {"ff_mac": (lin(q + "feed_forward_macaron.w_1"), lin(q + "feed_forward_macaron.w_2")),
+                 "ff": (lin(q + "feed_forward.w_1"), lin(q + "feed_forward.w_2")),
+                 "qkv": lin(q + "self_attn.linear_qkv"),
+                 "out": lin(q + "self_attn.linear_out"),
+                 "pw1": lin(cm + "pointwise_conv1"),
+                 "pw2": lin(cm + "pointwise_conv2"),
+                 "dw_w": _vec(recs[cm + "depthwise_conv"][1], device),
+                 "dw_b": _vec(recs[cm + "depthwise_conv"][2], device),
+                 "cm_norm": norm(cm + "norm") + (bool(recs[cm + "norm"][5] & BN),),
+                 "att_norm": recs[q + "self_attn.att_norm"][1][0] if self.softmax_plus else None}
             for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
-                L[name] = _ln_params(getattr(layer, name), device)
+                L[name] = norm(q + name)
             self.layers.append(L)
-        self.after_norm = _ln_params(enc.after_norm, device)
+        self.after_norm = norm("transformer.after_norm")
         # transform_out: affine -> activation -> LayerNorm (its own kernel) or BatchNorm (the epilogue)
-        self.transform = self._tdnn(m.transform_out, device)
-        att = m.stats.attention
-        self.att1 = _Lin(att[0].weight, att[0].bias, device, ACT_RELU)
-        self.att_ln = _ln_params(att[2], device)
-        self.att2 = _Lin(att[4].weight, att[4].bias, device)
-        self.norm_stats = _ln_params(m.stats.norm_stats, device)
-        pos = m.extracted_embedding
-        if pos == "far":
-            self.segment = [(_Lin(m.fc1.affine.weight, m.fc1.affine.bias, device), None)]
-        else:
-            self.segment = ([self._tdnn(m.fc1, device)] if m.fc1 is not None else []) + \
-                ([self._tdnn(m.fc2, device)] if pos == "near" else [(_Lin(m.fc2.affine.weight, m.fc2.affine.bias, device), None)])
-        self.embed_dim = m.embd_dim
-        self._rope = rotary_table(self.dk) if self.pos == "rot_pos" else None
-        self._abs = sinusoid_table(self.D) if self.pos == "abs_pos" else None
+        self.transform = tdnn("transform_out")
+        self.att1 = lin("stats.attention.0")
+        self.att_ln = norm("stats.attention.2")
+        self.att2 = lin("stats.attention.4")
+        self.norm_stats = norm("stats.norm_stats")
+        self.segment = [tdnn(name) for name in ("fc1", "fc2") if name + ".affine" in recs]
+        self.embed_dim = self.segment[-1][0].cout
+        self._pos_table = recs["pos_table"][1] if "pos_table" in recs else None
         self._tables = {}
         self.last_launches = 0
-
-    @staticmethod
-    def _tdnn(layer, device):
-        """(_Lin with the activation [and the folded BatchNorm], LayerNorm (gamma, beta) or None)."""
-        w, b = layer.affine.weight, layer.affine.bias
-        if layer.batchnorm is not None and not layer.ln:
-            s, t = fold_batchnorm(layer.batchnorm)
-            return _Lin(w, b, device, layer.act, s, t), None
-        lin = _Lin(w, b, device, layer.act)
-        if layer.batchnorm is None:
-            return lin, None
-        return lin, (_vec(layer.batchnorm.weight, device), _vec(layer.batchnorm.bias, device))
 
     def _tables_for(self, t):
         if t not in self._tables:
             if t >= TABLE_ROWS:
                 raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' {}".format(t, TABLE_ROWS))
-            rope = self._rope[:t].to(self.device).contiguous() if self._rope is not None else None
-            absp = self._abs[:t].to(self.device).contiguous() if self._abs is not None else None
-            mults = [softmax_plus_multiplier(t, L["train_len"]) if self.softmax_plus else 1.0 for L in self.layers]
+            table = _vec(self._pos_table[:t], self.device) if self._pos_table is not None else None
+            rope, absp = (table, None) if self.pos == "rot_pos" else (None, table)
+            mults = [float(L["att_norm"][t]) if self.softmax_plus else 1.0 for L in self.layers]
             self._tables[t] = (rope, absp, mults)
         return self._tables[t]
 
@@ -654,9 +628,9 @@ def native_config(m):
 
 
 def native_records(m):
-    """(name, w, bias, scale, shift, flags, keys) records and tables for xvb_conformer_set_layer, after the hand-over
-    transforms of ConformerExtractor.__init__: the concatenated Q/K/V, the subsampling Linear's column permutation and
-    xscale, the second subsampling conv transposed to (C, C, kf, kt), folded BatchNorms.  `keys` are the state_dict
+    """(name, w, bias, scale, shift, flags, keys) records and tables for xvb_conformer_set_layer and ConformerExtractor,
+    after the hand-over transforms: the concatenated Q/K/V, the subsampling Linear's column permutation and xscale, the
+    second subsampling conv transposed to (C, C, kf, kt), folded BatchNorms.  `keys` are the state_dict
     entries the record carries.  Tables: "pos_table" (rotary_table or sinusoid_table) and, for softmax_plus, each
     block's "self_attn.att_norm" = softmax_plus_multiplier for T' = 1 .. 4999 (index 0 unused, 0)."""
     from asv_subtools_b200._lib import BN, RELU, SWISH

@@ -218,6 +218,12 @@ class _PackedAffine:
         w, b, scale, shift, relu = layer.export()
         return cls(layer.affine, device, relu=relu, arrays=(w, b, scale, shift))
 
+    @classmethod
+    def from_record(cls, w, b, scale, shift, relu, device):
+        """A segment-layer record: w (Cout, Cin) and b, scale, shift (or None) as fp32 ndarrays, at context [0]."""
+        b = torch.from_numpy(b) if b is not None else None
+        return cls(None, device, relu=relu, arrays=(torch.from_numpy(w)[:, :, None], b, scale, shift))
+
     def __init__(self, affine, device, bn=None, relu=False, pad_to=8, row_scale=None, arrays=None):
         from .. import ops
         from .components import fold_batchnorm
@@ -232,7 +238,7 @@ class _PackedAffine:
         if pad:
             w = torch.cat([w, torch.zeros(pad, w.shape[1], w.shape[2], device=device)], 0)
             b = torch.cat([b, torch.zeros(pad, device=device)], 0) if b is not None else None
-        self.context, self.cout = list(affine.context), w.shape[0]
+        self.context, self.cout = list(affine.context) if affine is not None else [0], w.shape[0]
         self.w = ops.pack_tdnn_weight(w.contiguous(), self.context)
         self.bias = b.contiguous() if b is not None else None
         scale, shift = (arrays[2], arrays[3]) if arrays is not None else fold_batchnorm(bn)
