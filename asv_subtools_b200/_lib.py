@@ -106,6 +106,7 @@ SIGNATURES = {
     "xvb_stats_pool_ex": (_i, [_p, _i64, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
     "xvb_tdnn_affine_ex": (_i, [_p, _p]),
     "xvb_split_frames": (_i, [_p, _i, _i, _i, _p, _p, _i64, _i, _i, _p]),
+    "xvb_split_frames_lengths": (_i, [_p, _i, _i, _i, _p, _p, _i64, _i, _i, _p, _p]),
     "xvb_pool_partial_blocks": (_i, [_i, _i, _ip]),
     "xvb_pool_finalize": (_i, [_p, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
     "xvb_stats_pool_lengths": (_i, [_p, _i64, _i, _i, _i, _f, _i, _p, _p, _p, _p, _i64, _p]),
@@ -136,6 +137,8 @@ SIGNATURES = {
     "xvb_small_affine": (_i, [_p, _i64, _p, _i, _i, _i, _p, _p, _p, _i, _p, _i64, _p, _p, _i64, _p]),
     "xvb_attn_head_stats_pool": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
     "xvb_attn_head_stats_pool_prior": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _f, _i, _p, _p, _i, _p, _p, _p, _i64, _p]),
+    "xvb_attn_head_stats_pool_lengths": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _f, _i, _p, _p, _i, _p, _p, _p, _p,
+                                              _i64, _p]),
     "xvb_attn_head_stats_pool_mq": (_i, [_p, _i64, _i, _p, _i64, _i, _i, _i, _i, _i, _i, _i, _f, _i, _p, _p, _p, _i64, _p]),
     "xvb_tdnn_grouped_fits": (_i, [_i, _i, _i]),
     "xvb_topn_mean_std": (_i, [_p, _i64, _i64, _i, _i, _p, _p, _p]),

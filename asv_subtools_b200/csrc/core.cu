@@ -206,6 +206,12 @@ extern "C" int xvb_split_frames(const float* x, int B, int T, int C, uint16_t* h
   return split_frames(x, B, T, C, hi, lo, ldp, pad_front, pad_back, nullptr, stream);
 }
 
+extern "C" int xvb_split_frames_lengths(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp,
+                                        int pad_front, int pad_back, const int* lengths, void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_split_frames_lengths: null lengths");
+  return split_frames(x, B, T, C, hi, lo, ldp, pad_front, pad_back, lengths, stream);
+}
+
 int xvb::split_frames(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front, int pad_back,
                       const int* lengths, void* stream) {
   int rc = require_sm90();

@@ -466,14 +466,19 @@ struct OnlineU {
 // xi-vector form (xivec_stdinit_softplus2_prec_pooling, pooling.py:165-212): the raw logit z becomes 2 log(softplus(z)) (a frame's
 // log-precision, :189-190) and the softmax runs over T + 1 elements, the extra one being the prior (logit prior_logit[c], value
 // prior_x[c], :194-202): it initialises the online-softmax state of warp 0.
+// A masked batch (lengths != NULL, device int32[B]) reduces utterance b over frames [0, lengths[b]) only, with the batch
+// stride still T rows: the frame walk (warp w takes frames w, w + 8, ...) is the same as a call on that utterance alone,
+// so the row is bit-identical to it, and the frames past its end are never loaded.
 template <int kRows>
 __global__ void __launch_bounds__(kApWarps * 32)
 attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, const float* __restrict__ x, long long ldx,
                             int T, int C, int O, int gdiv, int head_width, int rep, float floor_, int unweighted_var,
                             const float* __restrict__ prior_logit,
-                            const float* __restrict__ prior_x, int softplus2log, float* __restrict__ out,
-                            __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol, long long ldo) {
+                            const float* __restrict__ prior_x, int softplus2log, const int* __restrict__ lengths,
+                            float* __restrict__ out, __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol,
+                            long long ldo) {
   const int b = blockIdx.y;
+  const int Tb = lengths ? __ldg(lengths + b) : T;   // a masked batch reduces utterance b over its own frames only
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int o = blockIdx.x * 128 + lane * 4;
   const bool active = o < O;   // O % 4 == 0, C % 4 == 0: the four outputs read four consecutive input channels
@@ -495,12 +500,12 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
     const float* lb = logits + (long long)b * T * ldl;
     const float* xb = x + (long long)b * T * ldx + c;
     const bool vec_logits = gdiv == 1 && (ldl & 3) == 0 && ((uintptr_t)lb & 15) == 0;   // per-channel logits: 16-byte loads
-    for (int t0 = warp; t0 < T; t0 += kApWarps * kRows) {
+    for (int t0 = warp; t0 < Tb; t0 += kApWarps * kRows) {
       float4 xv[kRows], lv[kRows];                       // kRows frames in flight per thread before any is consumed
 #pragma unroll
       for (int r = 0; r < kRows; ++r) {
         const int t = t0 + r * kApWarps;
-        if (t < T) {
+        if (t < Tb) {
           xv[r] = __ldcs(reinterpret_cast<const float4*>(xb + (long long)t * ldx));
           const float* lr = lb + (long long)t * ldl;
           if (vec_logits) lv[r] = __ldcs(reinterpret_cast<const float4*>(lr + o));
@@ -509,7 +514,7 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
       }
 #pragma unroll
       for (int r = 0; r < kRows; ++r) {
-        if (t0 + r * kApWarps >= T) continue;
+        if (t0 + r * kApWarps >= Tb) continue;
         const float xs[4] = {xv[r].x, xv[r].y, xv[r].z, xv[r].w};
         const float ls[4] = {lv[r].x, lv[r].y, lv[r].z, lv[r].w};
 #pragma unroll
@@ -555,7 +560,7 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
         }
       }
       mu[k] = a.s1 / a.s0;
-      const float var = unweighted_var ? (a.u2 - 2.f * mu[k] * a.u1) / (float)T + mu[k] * mu[k]
+      const float var = unweighted_var ? (a.u2 - 2.f * mu[k] * a.u1) / (float)Tb + mu[k] * mu[k]
                                        : a.s2 / a.s0 - mu[k] * mu[k];
       sd[k] = sqrtf(fmaxf(var, floor_));
     }
@@ -578,15 +583,16 @@ attn_head_stats_pool_kernel(const float* __restrict__ logits, long long ldl, con
 
 static int launch_attn_head_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C, int O,
                                       int gdiv, int head_width, int rep, float floor_, int unweighted_var, const float* prior_logit,
-                                      const float* prior_x, int softplus2log, float* out, uint16_t* out_hi, uint16_t* out_lo,
-                                      int64_t ldo, void* stream) {
+                                      const float* prior_x, int softplus2log, const int* lengths, float* out, uint16_t* out_hi,
+                                      uint16_t* out_lo, int64_t ldo, void* stream) {
   dim3 grid((O + 127) / 128, B);
   // frames in flight per thread (XVB_ATTN_ROWS = 1, 2 or 4): 1 by default, since the extra registers of the unrolled
   // forms can cost more occupancy than they hide latency
   static const int rows_knob = getenv("XVB_ATTN_ROWS") ? atoi(getenv("XVB_ATTN_ROWS")) : 1;
   auto* kern = rows_knob == 1 ? attn_head_stats_pool_kernel<1> : rows_knob == 2 ? attn_head_stats_pool_kernel<2> : attn_head_stats_pool_kernel<4>;
   kern<<<grid, kApWarps * 32, 0, (cudaStream_t)stream>>>(
-      logits, ldl, x, ldx, T, C, O, gdiv, head_width, rep, floor_, unweighted_var, prior_logit, prior_x, softplus2log, out,
+      logits, ldl, x, ldx, T, C, O, gdiv, head_width, rep, floor_, unweighted_var, prior_logit, prior_x, softplus2log, lengths,
+      out,
       reinterpret_cast<__nv_bfloat16*>(out_hi), reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
@@ -636,17 +642,11 @@ extern "C" int xvb_small_affine(const float* x, int64_t ldx, const float* w, int
   return XVB_OK;
 }
 
-extern "C" int xvb_attn_head_stats_pool(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
-                                        int C, int O, int gdiv, float floor_, int unweighted_var, float* out,
-                                        uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
-  return xvb_attn_head_stats_pool_prior(logits, ldl, G, x, ldx, B, T, C, O, gdiv, floor_, unweighted_var, nullptr, nullptr, 0, out,
-                                        out_hi, out_lo, ldo, stream);
-}
-
-extern "C" int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
-                                              int C, int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
-                                              const float* prior_x, int softplus2log, float* out, uint16_t* out_hi,
-                                              uint16_t* out_lo, int64_t ldo, void* stream) {
+// The checks and launch of xvb_attn_head_stats_pool_prior and _lengths (lengths NULL: every utterance has T frames).
+static int attn_head_stats_pool_run(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T, int C,
+                                    int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
+                                    const float* prior_x, int softplus2log, const int* lengths, float* out, uint16_t* out_hi,
+                                    uint16_t* out_lo, int64_t ldo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG((prior_logit != nullptr) == (prior_x != nullptr) && (!prior_logit || (O == C && !unweighted_var)),
@@ -659,7 +659,32 @@ extern "C" int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, 
   XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "xvb_attn_head_stats_pool: out_hi/out_lo must both be set or both NULL");
   if (out_hi) XVB_CHECK_ARG(ldo % 4 == 0 && ldo >= 2 * (int64_t)O, "xvb_attn_head_stats_pool: ldo too small / unaligned");
   return launch_attn_head_stats_pool(logits, ldl, x, ldx, B, T, C, O, gdiv, C, O / C, floor_, unweighted_var, prior_logit,
-                                     prior_x, softplus2log, out, out_hi, out_lo, ldo, stream);
+                                     prior_x, softplus2log, lengths, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_attn_head_stats_pool(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
+                                        int C, int O, int gdiv, float floor_, int unweighted_var, float* out,
+                                        uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
+  return xvb_attn_head_stats_pool_prior(logits, ldl, G, x, ldx, B, T, C, O, gdiv, floor_, unweighted_var, nullptr, nullptr, 0, out,
+                                        out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
+                                              int C, int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
+                                              const float* prior_x, int softplus2log, float* out, uint16_t* out_hi,
+                                              uint16_t* out_lo, int64_t ldo, void* stream) {
+  return attn_head_stats_pool_run(logits, ldl, G, x, ldx, B, T, C, O, gdiv, floor_, unweighted_var, prior_logit, prior_x,
+                                  softplus2log, nullptr, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_attn_head_stats_pool_lengths(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B,
+                                                int T, int C, int O, int gdiv, float floor_, int unweighted_var,
+                                                const float* prior_logit, const float* prior_x, int softplus2log,
+                                                const int* lengths, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo,
+                                                void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_attn_head_stats_pool_lengths: null lengths");
+  return attn_head_stats_pool_run(logits, ldl, G, x, ldx, B, T, C, O, gdiv, floor_, unweighted_var, prior_logit, prior_x,
+                                  softplus2log, lengths, out, out_hi, out_lo, ldo, stream);
 }
 
 extern "C" int xvb_attn_head_stats_pool_mq(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
@@ -676,7 +701,7 @@ extern "C" int xvb_attn_head_stats_pool_mq(const float* logits, int64_t ldl, int
   XVB_CHECK_ARG((out_hi != nullptr) == (out_lo != nullptr), "xvb_attn_head_stats_pool_mq: out_hi/out_lo must both be set or both NULL");
   if (out_hi) XVB_CHECK_ARG(ldo % 4 == 0 && ldo >= 2 * (int64_t)O, "xvb_attn_head_stats_pool_mq: ldo too small / unaligned");
   return launch_attn_head_stats_pool(logits, ldl, x, ldx, B, T, C, O, gdiv, head_width, rep, floor_, unweighted_var, nullptr,
-                                     nullptr, 0, out, out_hi, out_lo, ldo, stream);
+                                     nullptr, 0, nullptr, out, out_hi, out_lo, ldo, stream);
 }
 
 namespace {

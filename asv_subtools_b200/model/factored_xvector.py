@@ -14,6 +14,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
+from asv_subtools_b200.native import device_lengths  # noqa: E402
 from asv_subtools_b200.nnet import FTdnnBlock, ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 
@@ -67,7 +68,10 @@ class _Affine:
 
 
 class FtdnnExtractor:
-    """Packed weights on one device + the launch sequence of Xvector.extract_embedding (factored_xvector.py:99-122)."""
+    """Packed weights on one device + the launch sequence of Xvector.extract_embedding (factored_xvector.py:99-122).
+    Takes masked batches of utterances of different lengths (TAKES_LENGTHS)."""
+
+    TAKES_LENGTHS = True
 
     def __init__(self, m, device):
         self.feat_dim, self.embed_dim = m.inputs_dim, m.embd_dim
@@ -84,14 +88,15 @@ class FtdnnExtractor:
         self.e2 = None if self.far else _Affine(m.embedding2.affine, device)
         self.last_launches = 0
 
-    def _block(self, i, x, out, tmp256, tmpo):
-        """FTdnnBlock i: x -> out (SplitPlanes views).  tmp256 / tmpo: scratch planes (B,T,256) / (B,T,1024)."""
+    def _block(self, i, x, out, tmp256, tmpo, lens=None):
+        """FTdnnBlock i: x -> out (SplitPlanes views).  tmp256 / tmpo: scratch planes (B,T,256) / (B,T,1024).  lens: the
+        device lengths of a masked batch; the bypass sum needs none, both of its inputs being zero past each end."""
         factor, affine, bypass = self.blocks[i]
-        factor.run(x, y=tmp256)
+        factor.run(x, y=tmp256, lengths=lens)
         if bypass == 0:
-            affine.run(tmp256, y=out)
+            affine.run(tmp256, y=out, lengths=lens)
         else:
-            affine.run(tmp256, y=tmpo)
+            affine.run(tmp256, y=tmpo, lengths=lens)
             gate = self._gate(bypass, x.hi.shape[0], x.channels, x.hi.device)
             ops.se_apply(x, tmpo, gate, out)              # out = x * bypass + bn(relu(affine(factor(x))))
 
@@ -101,29 +106,40 @@ class FtdnnExtractor:
             self._gate_key, self._gate_t = key, torch.full((b, c), float(value), dtype=torch.float32, device=dev)
         return self._gate_t
 
-    def extract(self, feats):
+    def extract(self, feats, lengths=None):
+        """feats (B, T, F) fp32 CUDA -> (B, embed_dim) fp32 CUDA, asynchronous on the current stream.  lengths (B,) host
+        ints, 1 <= lengths[b] <= T: a masked batch, row b being feats[b, :lengths[b]] extracted alone; layer10 then
+        writes fp32 frames and the standalone pooling reduces each utterance's own (the fused pooling epilogue takes
+        equal lengths only).  Every length equal to T runs the unmasked sequence."""
         if feats.shape[2] != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
         B, T, _ = feats.shape
         dev, P = feats.device, ops.SplitPlanes
-        xin = ops.split_f32(feats, ld=(self.feat_dim + 7) // 8 * 8)
+        lens = None if lengths is None else device_lengths(lengths, B, T, dev)
+        ld = (self.feat_dim + 7) // 8 * 8
+        xin = ops.split_f32(feats, ld=ld) if lens is None else ops.split_frames(feats.contiguous(), ld=ld, lengths=lens)
         x1 = P.empty((B, T, 512), dev)
-        self.l01.run(xin, y=x1)
+        self.l01.run(xin, y=x1, lengths=lens)
         t256, to = P.empty((B, T, 256), dev), P.empty((B, T, 1024), dev)
         cat7, cat9 = P.empty((B, T, 2048), dev), P.empty((B, T, 3072), dev)      # [x_2 | x_4], [x_4 | x_6 | x_8]
         x3, x5, x7, x9 = (P.empty((B, T, 1024), dev) for _ in range(4))
         x2, x4 = cat7.slice(0, 1024), cat7.slice(1024, 2048)
-        self._block(2, x1, x2, t256, to)
-        self._block(3, x2, x3, t256, to)
-        self._block(4, x3, x4, t256, to)
+        self._block(2, x1, x2, t256, to, lens)
+        self._block(3, x2, x3, t256, to, lens)
+        self._block(4, x3, x4, t256, to, lens)
         ops.copy_planes(x4, cat9.slice(0, 1024))
-        self._block(5, x3, x5, t256, to)
-        self._block(6, x5, cat9.slice(1024, 2048), t256, to)
-        self._block(7, cat7, x7, t256, to)
-        self._block(8, x7, cat9.slice(2048, 3072), t256, to)
-        self._block(9, cat9, x9, t256, to)
-        _, stats = ops.fused_pool_layer(x9, self.l10.w, self.l10.cout, self.l10.context, self.l10.bias, self.l10.scale,
-                                        self.l10.shift, relu=self.l10.relu, eps=self.eps, planes=True)
+        self._block(5, x3, x5, t256, to, lens)
+        self._block(6, x5, cat9.slice(1024, 2048), t256, to, lens)
+        self._block(7, cat7, x7, t256, to, lens)
+        self._block(8, x7, cat9.slice(2048, 3072), t256, to, lens)
+        self._block(9, cat9, x9, t256, to, lens)
+        if lens is None:
+            _, stats = ops.fused_pool_layer(x9, self.l10.w, self.l10.cout, self.l10.context, self.l10.bias, self.l10.scale,
+                                            self.l10.shift, relu=self.l10.relu, eps=self.eps, planes=True)
+        else:
+            x10 = torch.empty(B, T, self.l10.cout, dtype=torch.float32, device=dev)
+            self.l10.run(x9, y_f32=x10, lengths=lens)
+            _, stats = ops.stats_pool_ex(x10, self.eps, 0, planes=True, lengths=lens)
         emb = torch.empty(B, 1, self.embed_dim, dtype=torch.float32, device=dev)
         if self.far:
             self.e1.run(stats, y_f32=emb)

@@ -28,6 +28,18 @@ def host_lengths(lengths, b):
     return np.clip(lens, -2 ** 31, 2 ** 31 - 1).astype(np.int32)
 
 
+def device_lengths(lengths, b, t, device):
+    """The lengths of a masked batch of the Python launch sequences, checked on the host: ValueError naming the first
+    entry outside [1, t]; None when every entry equals t (the unmasked sequence runs), else a device int32 (B,) tensor."""
+    lens = host_lengths(lengths, b)
+    bad = np.flatnonzero((lens < 1) | (lens > t))
+    if bad.size:
+        raise ValueError("lengths[{}]={} outside [1, T={}]".format(bad[0], lens[bad[0]], t))
+    if (lens == t).all():
+        return None
+    return torch.from_numpy(lens).pin_memory().to(device, non_blocking=True)   # no host wait on the stream
+
+
 class NativeExtractor:
     """xvb_<PREFIX>_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
     current when it is built from a model `m` (or loaded from a model file at `path`).

@@ -154,7 +154,8 @@ class TopVirtualNnet(torch.nn.Module):
         ndarray; T <= maxChunk) -> (B, D) CUDA tensor.  Same arithmetic as B calls of
         extract_embedding().  lengths (B,) host ints, 1 <= lengths[b] <= T: utterances of different lengths padded to
         T, row b being the embedding of feats[b, :lengths[b]] (what is past it is ignored); models whose extractor
-        declares TAKES_LENGTHS (the TDNN x-vector with statistics pooling, the ResNet x-vector) only."""
+        declares TAKES_LENGTHS only: the TDNN x-vector family with statistics or attention pooling (attentive,
+        multi-head, multi-resolution, xi-vector; not LDE), the F-TDNN x-vector and the ResNet x-vector."""
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:
@@ -167,7 +168,8 @@ class TopVirtualNnet(torch.nn.Module):
             ex = self.extractor()
             if not getattr(ex, "TAKES_LENGTHS", False):
                 raise NotImplementedError("{}: extract_embedding_batch(lengths=...) needs an extractor that takes lengths (the "
-                                          "TDNN x-vector with statistics pooling or the ResNet x-vector); this model runs on "
+                                          "TDNN x-vector family with statistics or attention pooling other than LDE, the "
+                                          "F-TDNN x-vector or the ResNet x-vector); this model runs on "
                                           "{}".format(type(self).__name__, type(ex).__name__))
             return ex.extract(x, lengths)
 
@@ -265,7 +267,12 @@ class AttentionPoolingExtractor:
     layers on the wgmma layer kernel (the last one also writes fp32, the pooling kernel's x), then either the attention
     affines as GEMMs (grouped weights expanded block-diagonally, temperature folded into the last affine, logits fp32) +
     softmax over time + weighted mean / std in one pass (`xvb_attn_head_stats_pool`), or the dictionary encoding
-    (`xvb_lde_pool`); then the segment layers on T = 1."""
+    (`xvb_lde_pool`); then the segment layers on T = 1.
+
+    TAKES_LENGTHS: every attention pooling (attentive, multi-head, global / multi-resolution, xi-vector) runs masked
+    batches of utterances of different lengths; an LDE instance does not."""
+
+    TAKES_LENGTHS = True
 
     def __init__(self, model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, position):
         dev = model.device_for_extraction()
@@ -284,6 +291,7 @@ class AttentionPoolingExtractor:
         if hasattr(stats, "mu"):                                 # LDEPooling: no attention network
             self.lde = (stats.mu.detach().float().to(dev).contiguous(), stats.neg_beta().to(dev).contiguous())
             self.first = self.last = None
+            self.TAKES_LENGTHS = False
             self._segments(dev, tdnn6, tdnn7, position)
             return
         att = stats.attention
@@ -309,16 +317,28 @@ class AttentionPoolingExtractor:
         self.embed_dim = self.segment[-1].cout_real
         self.last_launches = 0
 
-    def extract(self, feats):
+    def extract(self, feats, lengths=None):
+        """feats (B, T, F) fp32 CUDA -> (B, embed_dim) fp32 CUDA, asynchronous on the current stream.  lengths (B,) host
+        ints, 1 <= lengths[b] <= T (attention poolings): a masked batch, row b being feats[b, :lengths[b]] extracted
+        alone.  The staging, every frame layer and attention affine store zeros past each end and the pooling reduces
+        each utterance's own frames, so what lies past them is never read.  Every length equal to T runs the unmasked
+        sequence."""
         from .. import ops
+        from ..native import device_lengths
         if feats.shape[2] != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
         B, T, _ = feats.shape
         dev, P = feats.device, ops.SplitPlanes
-        x = ops.split_f32(feats, ld=(self.feat_dim + 7) // 8 * 8)
+        lens = None
+        if lengths is not None:
+            if not self.TAKES_LENGTHS:
+                raise NotImplementedError("LDE pooling does not take lengths")
+            lens = device_lengths(lengths, B, T, dev)
+        ld = (self.feat_dim + 7) // 8 * 8
+        x = ops.split_f32(feats, ld=ld) if lens is None else ops.split_frames(feats.contiguous(), ld=ld, lengths=lens)
         for layer in self.frames[:-1]:
             y, view = layer.planes(B, T, dev)
-            layer.run(x, y=y)
+            layer.run(x, y=y, lengths=lens)
             x = view
         top = self.frames[-1]
         y, xp = top.planes(B, T, dev)
@@ -327,21 +347,22 @@ class AttentionPoolingExtractor:
             top.run(x, y_f32=xf)
             _, x = ops.lde_pool(xf[..., :top.cout_real], self.lde[0], self.lde[1], planes=True)
         else:
-            top.run(x, y=y, y_f32=xf)
+            top.run(x, y=y, y_f32=xf, lengths=lens)
             h = xp
             if self.first is not None:
                 y, h = self.first.planes(B, T, dev)
-                self.first.run(xp, y=y)
+                self.first.run(xp, y=y, lengths=lens)
             logits = torch.empty(B, T, self.last.cout, dtype=torch.float32, device=dev)
-            self.last.run(h, y_f32=logits)
+            self.last.run(h, y_f32=logits, lengths=lens)
             if self.xi is not None:
                 _, x = ops.attn_head_stats_pool(logits[..., :self.last.cout_real], xf[..., :top.cout_real], self.pooled, 1, floor=self.eps,
-                                                planes=True, prior_logit=self.xi[0], prior_x=self.xi[1], softplus2log=True)
+                                                planes=True, prior_logit=self.xi[0], prior_x=self.xi[1], softplus2log=True,
+                                                lengths=lens)
                 if not self.xi[2]:                               # post-mean variant: phi alone
                     x = x.slice(0, self.pooled)
             else:
                 _, x = ops.attn_head_stats_pool(logits[..., :self.last.cout_real], xf[..., :top.cout_real], self.pooled, self.gdiv,
-                                                floor=self.eps, unweighted_var=self.unweighted, planes=True)
+                                                floor=self.eps, unweighted_var=self.unweighted, planes=True, lengths=lens)
         for i, layer in enumerate(self.segment):
             if i + 1 == len(self.segment):
                 emb = torch.empty(B, 1, layer.cout, dtype=torch.float32, device=dev)

@@ -62,6 +62,24 @@ def split_f32(x, ld=None):
     return SplitPlanes(hi, lo, c)
 
 
+def split_frames(x, ld=None, pad_front=0, pad_back=0, lengths=None):
+    """(B, T, C) fp32 -> SplitPlanes (B, pad_front + T + pad_back, ld) with zero frames around every utterance
+    (xvb_split_frames).  lengths: int32 CUDA (B,) tensor of a masked batch (xvb_split_frames_lengths): the frames
+    t >= lengths[b] are written as zeros and never read."""
+    x = _req(x, torch.float32, "x")
+    b, t, c = x.shape
+    ld = ld or (c + 7) // 8 * 8
+    hi = torch.empty(b, pad_front + t + pad_back, ld, dtype=torch.bfloat16, device=x.device)
+    lo = torch.empty_like(hi)
+    args = (_ptr(x), b, t, c, _ptr(hi), _ptr(lo), ld, pad_front, pad_back)
+    if lengths is None:
+        check(lib.xvb_split_frames(*args, _stream()), "xvb_split_frames")
+    else:
+        check(lib.xvb_split_frames_lengths(*args, _ptr(_req(lengths, torch.int32, "lengths")), _stream()),
+              "xvb_split_frames_lengths")
+    return SplitPlanes(hi, lo, c)
+
+
 def context_span(context):
     """left/right/total context as TdnnAffine.__init__ (components.py:50-53)."""
     left = context[0] if context[0] < 0 else 0
@@ -505,10 +523,12 @@ def small_affine(x, w, bias=None, bn_scale=None, bn_shift=None, relu=False, sigm
 
 
 def attn_head_stats_pool(logits, x, out_channels, gdiv, floor=1e-10, unweighted_var=False, planes=False, prior_logit=None,
-                         prior_x=None, softplus2log=False):
+                         prior_x=None, softplus2log=False, lengths=None):
     """Attention pooling with a head map (xvb_attn_head_stats_pool): logits (B,T,G) fp32 (any row pitch >= G), x (B,T,C)
     fp32; output channel o pools x[..., o % C] with softmax_T(logits[..., o // gdiv]).  -> (B, 2*out_channels).
-    prior_logit / prior_x (C,) + softplus2log: the xi-vector form (a prior element in the softmax, logits = 2 log softplus)."""
+    prior_logit / prior_x (C,) + softplus2log: the xi-vector form (a prior element in the softmax, logits = 2 log softplus).
+    lengths: int32 CUDA (B,) tensor of a masked batch (xvb_attn_head_stats_pool_lengths): utterance b pools its first
+    lengths[b] frames."""
     for name, v in (("logits", logits), ("x", x)):       # channel-slice views of wider buffers are fine: rows stay contiguous
         if v.dtype != torch.float32 or not v.is_cuda or v.dim() != 3 or v.stride(-1) != 1 or v.stride(0) != v.shape[1] * v.stride(1):
             raise TypeError("{} must be a (B,T,*) CUDA float32 tensor with contiguous rows".format(name))
@@ -516,11 +536,14 @@ def attn_head_stats_pool(logits, x, out_channels, gdiv, floor=1e-10, unweighted_
     g = logits.shape[-1]
     out = torch.empty(b, 2 * out_channels, dtype=torch.float32, device=x.device)
     op = SplitPlanes.empty((b, 1, 2 * out_channels), x.device) if planes else None
-    check(lib.xvb_attn_head_stats_pool_prior(_ptr(logits), logits.stride(-2), g, _ptr(x), x.stride(-2), b, t, c, out_channels,
-                                             int(gdiv), floor, 1 if unweighted_var else 0, _ptr(prior_logit), _ptr(prior_x),
-                                             1 if softplus2log else 0, _ptr(out), op.hi.data_ptr() if op else None,
-                                             op.lo.data_ptr() if op else None, 2 * out_channels, _stream()),
-          "xvb_attn_head_stats_pool")
+    head = (_ptr(logits), logits.stride(-2), g, _ptr(x), x.stride(-2), b, t, c, out_channels, int(gdiv), floor,
+            1 if unweighted_var else 0, _ptr(prior_logit), _ptr(prior_x), 1 if softplus2log else 0)
+    tail = (_ptr(out), op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, 2 * out_channels, _stream())
+    if lengths is None:
+        check(lib.xvb_attn_head_stats_pool_prior(*head, *tail), "xvb_attn_head_stats_pool")
+    else:
+        check(lib.xvb_attn_head_stats_pool_lengths(*head, _ptr(_req(lengths, torch.int32, "lengths")), *tail),
+              "xvb_attn_head_stats_pool_lengths")
     return (out, op) if planes else out
 
 

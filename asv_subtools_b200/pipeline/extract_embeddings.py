@@ -14,9 +14,9 @@ per-utterance `extract_embedding()` with the reference's chunk rule.  One `FV` v
 input key (bucket order).  `--shard i/n` keeps every n-th utterance (one process per GPU without
 pre-splitting the scp).
 
-`--mixed-lengths` (models whose extractor takes lengths: the TDNN x-vector with statistics pooling and the ResNet
-x-vector): the maxChunk rule cuts every utterance first, and the
-chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
+`--mixed-lengths` (models whose extractor takes lengths: the TDNN x-vector family with statistics pooling or an attention
+pooling other than LDE -- attentive, multi-head, multi-resolution, xi-vector --, the F-TDNN x-vector and the ResNet
+x-vector): the maxChunk rule cuts every utterance first, and the chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
 call, `extract_embedding_batch(x, lengths)`, and each utterance's embedding is sum(len_i * emb_i) / frames over its
 chunks, as `bin/xvb-extract --mixed-lengths` does.  The pooling merge order depends on the batch shape, so the vectors
 differ from the default mode's at the rounding level.
@@ -203,7 +203,7 @@ def main(argv=None):
     ap.add_argument("--shard", type=str, default="0/1", help="i/n: keep utterances with index %% n == i")
     ap.add_argument("--mixed-lengths", action="store_true",
                     help="batch utterances of different lengths (padding at most 1/8 of a batch); TDNN x-vector models with "
-                         "statistics pooling and ResNet x-vector models only")
+                         "statistics or attention pooling (not LDE), F-TDNN and ResNet x-vector models only")
     ap.add_argument("--blueprint-dir", type=str, default="",
                     help="take the blueprint of the same file name from this directory (asv_subtools_b200/model) instead of "
                          "the path stored in nnet.config, so a reference model dir is used as it is")
@@ -234,8 +234,9 @@ def main(argv=None):
         if args.mixed_lengths:
             ex = model.extractor()
             if not getattr(ex, "TAKES_LENGTHS", False):
-                print("ERROR: --mixed-lengths needs a TDNN x-vector model with statistics pooling or a ResNet x-vector; {} "
-                      "runs on {}".format(type(model).__name__, type(ex).__name__), file=sys.stderr)
+                print("ERROR: --mixed-lengths needs a TDNN x-vector model with statistics or attention pooling (not LDE), an "
+                      "F-TDNN or a ResNet x-vector; {} runs on {}".format(type(model).__name__, type(ex).__name__),
+                      file=sys.stderr)
                 sys.exit(1)
         # native ark reader (csrc/ark_io.cpp): the reference's byte-at-a-time key loop is the wall at GPU rates
         with kaldi_io.open_or_fd(args.vectors_wspecifier, "wb") as w:

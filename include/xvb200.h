@@ -80,6 +80,10 @@ int xvb_split_f32(const float* x, int64_t rows, int C, int64_t ldx, uint16_t* hi
  * TdnnAffine.forward (components.py:117) made explicit, for the im2col view of xvb_tdnn_args_t. */
 int xvb_split_frames(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front,
                      int pad_back, void* stream);
+/* xvb_split_frames over a masked batch: utterance b owns frames [0, lengths[b]) (DEVICE int32[B], 1 <= lengths[b] <= T);
+ * the frames past them are written as zeros in both planes and never read.  XVB_EINVAL on a NULL lengths. */
+int xvb_split_frames_lengths(const float* x, int B, int T, int C, uint16_t* hi, uint16_t* lo, int64_t ldp, int pad_front,
+                             int pad_back, const int* lengths, void* stream);
 int64_t xvb_packed_weight_elems(int Cout, int Cin, int ntaps);
 int xvb_pack_tdnn_weight(const float* w, int Cout, int Cin, int tot_context, int left_context, const int* context_host,
                          int ntaps, uint16_t* w_hi, uint16_t* w_lo, void* stream);
@@ -263,6 +267,15 @@ int xvb_attn_head_stats_pool_prior(const float* logits, int64_t ldl, int G, cons
                                    int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
                                    const float* prior_x, int softplus2log, float* out, uint16_t* out_hi, uint16_t* out_lo,
                                    int64_t ldo, void* stream);
+/* xvb_attn_head_stats_pool_prior over a masked batch: utterance b reduces its first lengths[b] frames (DEVICE int32[B],
+ * 1 <= lengths[b] <= T; the batch stride stays T rows of x and of the logits), so the softmax of the xi-vector form runs
+ * over lengths[b] + 1 elements and the unweighted variance divides by lengths[b].  The frames past each end are never
+ * read, and each row is bit-identical to a call on that utterance alone.  prior_logit / prior_x may be NULL (the plain
+ * attention poolings).  XVB_EINVAL on a NULL lengths. */
+int xvb_attn_head_stats_pool_lengths(const float* logits, int64_t ldl, int G, const float* x, int64_t ldx, int B, int T,
+                                     int C, int O, int gdiv, float floor_, int unweighted_var, const float* prior_logit,
+                                     const float* prior_x, int softplus2log, const int* lengths, float* out, uint16_t* out_hi,
+                                     uint16_t* out_lo, int64_t ldo, void* stream);
 /* The same kernel with a head-width map, for multi-query multi-head attention pooling (MQMHASP, libs/nnet/pooling.py:589-
  * 698): x's C channels form C / head_width heads of head_width channels, each pooled `rep` times (once per query), so
  * output channel o pools x channel (o / (rep*head_width))*head_width + o % head_width with the alpha of logit o / gdiv.

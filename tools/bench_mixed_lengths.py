@@ -1,15 +1,18 @@
 #!/usr/bin/env python
-"""Throughput of the TDNN or ResNet x-vector handle on a corpus of utterances of different lengths -- a side
-measurement, not the bench.py line.
+"""Throughput of an x-vector extractor on a corpus of utterances of different lengths -- a side measurement, not the
+bench.py line.
 
-    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet] [--utts N] [--min-frames A] [--max-frames B]
-                                        [--batch N] [--dim F]
+    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn] [--utts N]
+                                        [--min-frames A] [--max-frames B] [--batch N] [--dim F]
 
 The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
 numpy.random.RandomState(2026), run through one handle under two batch policies.  --model xvector (the default): an
 Xvector(F, far) handle (default F = 23, batch 256).  --model resnet: the online launcher's SE ResNet34 of
 tools/bench_resnet.py (post-activation blocks with SE, fc1=False, position near) on 80-d features (--dim is ignored),
-batch 128 by default, as bench_resnet.py times it.
+batch 128 by default, as bench_resnet.py times it.  --model multihead / xivector / ftdnn: the Python launch sequences of
+the golden configurations at 40-d features (--dim is ignored), position far -- the snowdar x-vector with shared-weight
+four-head attention pooling (tests/golden/make_golden_snowdar.py "mha_share"), the xi-vector posterior-distribution
+pooling ("xi_dist") and the factored F-TDNN (make_golden_ftdnn.py); batch 256, 256 and 128 by default.
 
   * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
     up to `batch` utterances of exactly the same frame count, one xvb_<handle>_extract call each;
@@ -41,6 +44,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import resnet_oracle as ro  # noqa: E402
 
 
+# the golden configurations of tests/golden/make_golden_snowdar.py that --model multihead / xivector run
+SNOWDAR = {"multihead": ("multi-head", {"num_head": 4}, 313),
+           "xivector": ("xi-postdist-softplus2", {"hidden_size": 64, "num_nodes": 200}, 320)}
+
+
 def equal_length_batches(lengths, batch):
     """Exact-length buckets in batches of up to `batch` (the default mode of both CLIs)."""
     buckets = {}
@@ -55,9 +63,9 @@ def main():
     ap.add_argument("--utts", type=int, default=4000)
     ap.add_argument("--min-frames", type=int, default=200)
     ap.add_argument("--max-frames", type=int, default=2000)
-    ap.add_argument("--batch", type=int, default=None, help="default 256 (xvector) or 128 (resnet)")
+    ap.add_argument("--batch", type=int, default=None, help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn)")
     ap.add_argument("--dim", type=int, default=23)
-    ap.add_argument("--model", choices=["xvector", "resnet"], default="xvector")
+    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn"], default="xvector")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_mixed_lengths.py needs a GPU")
@@ -71,6 +79,22 @@ def main():
         m = ResNetXvector(F, 10, training=False, extracted_embedding="near", **ro.ONLINE)
         m.load_state_dict(onn.make_state_dict(ro.resnet_spec(F, ro.ONLINE), 301), strict=True)
         workload = "online SE ResNet34 (80-d, near)"
+    elif args.model in ("multihead", "xivector"):
+        from asv_subtools_b200.model.snowdar_xvector import Xvector as SnowdarXvector
+        F = 40
+        args.batch = args.batch or 256
+        pooling, pp, seed = SNOWDAR[args.model]
+        m = SnowdarXvector(F, 10, training=False, extracted_embedding="far", pooling=pooling, pooling_params=pp)
+        m.load_state_dict(onn.make_state_dict(onn.snowdar_xvector_spec(F, pooling=pooling, pooling_params=pp), seed),
+                          strict=True)
+        workload = "snowdar Xvector(40) far, pooling {} {}".format(pooling, pp)
+    elif args.model == "ftdnn":
+        from asv_subtools_b200.model.factored_xvector import Xvector as FactoredXvector
+        F = 40
+        args.batch = args.batch or 128
+        m = FactoredXvector(F, 10, training=False, extracted_embedding="far")
+        m.load_state_dict(onn.make_state_dict(onn.factored_xvector_spec(F), 401), strict=True)
+        workload = "factored F-TDNN Xvector(40) far"
     else:
         F = args.dim
         args.batch = args.batch or 256
