@@ -40,6 +40,11 @@ struct FbankDev {
 
 constexpr int kFbankWarps = 8;
 
+// Floats of shared memory per warp: N samples (M float2), M + 4 spectrum values, 128 log-mel energies.  Rounded up to
+// a multiple of 4 so that every warp's slice starts 16-byte aligned: the float2 accesses to z compile to 8-byte
+// vector loads and stores, and N = 2 (M = 1) would otherwise leave odd warps 4 bytes off.
+__host__ __device__ constexpr int fbank_warp_floats(int N) { return (N + (N / 2 + 4) + 128 + 3) & ~3; }
+
 __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
@@ -51,8 +56,7 @@ fbank_kernel(const float* __restrict__ wave, const long long* __restrict__ sampl
   extern __shared__ float smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int M = d.N >> 1;
-  const int per_warp = d.N + (M + 4) + 128;
-  float* xs = smem + warp * per_warp;            // N floats == M float2
+  float* xs = smem + warp * fbank_warp_floats(d.N);            // N floats == M float2
   float2* z = reinterpret_cast<float2*>(xs);
   float* P = xs + d.N;                           // M + 1 spectrum values
   float* lm = P + (M + 4);                       // log-mel energies (MFCC)
@@ -280,8 +284,7 @@ extern "C" int xvb_fbank_compute(xvb_fbank_t* h, const float* wave, const int64_
   XVB_CHECK_ARG(h && wave && sample_offsets && frame_offsets && feats && num_utts > 0, "xvb_fbank_compute: bad arguments");
   XVB_CHECK_ARG(total_frames >= 0 && total_frames < (1ll << 31) * kFbankWarps, "xvb_fbank_compute: too many frames for one call");
   if (total_frames == 0) return XVB_OK;
-  const int M = h->d.N / 2;
-  const size_t smem = (size_t)kFbankWarps * (h->d.N + (M + 4) + 128) * sizeof(float);
+  const size_t smem = (size_t)kFbankWarps * fbank_warp_floats(h->d.N) * sizeof(float);
   XVB_ENSURE_DYN_SMEM((fbank_kernel), 200 * 1024);
   static_assert(sizeof(long long) == sizeof(int64_t), "offset type");
   const unsigned grid = (unsigned)((total_frames + kFbankWarps - 1) / kFbankWarps);

@@ -25,7 +25,7 @@ def vad_energy(feats, energy_threshold=5.0, energy_mean_scale=0.5, frames_contex
                 den += 1
                 if log_energy[t2] > thr:
                     num += 1
-        out[t] = 1 if num >= den * proportion_threshold else 0
+        out[t] = 1 if np.float32(num) >= np.float32(den) * np.float32(proportion_threshold) else 0   # float, as the reference
     return out
 
 

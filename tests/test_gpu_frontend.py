@@ -29,7 +29,7 @@ def test_vad_cmn_select_match_oracle():
         for i, u in enumerate(utts):
             ref = ofe.vad_energy(u, 5.5, scale, ctx, prop)
             got = v[o[i]:o[i + 1]]
-            assert (got != ref).mean() <= 0.01, (ctx, prop, i)     # borderline frames: float summation order of the mean
+            assert (got != ref).mean() <= 0.01, (ctx, prop, i)     # energies next to the threshold: summation order of the mean
             assert counts[i].item() == got.sum()
         y, new_off = fe.select_frames(x, off, voiced, counts)
         parts = fe.unpack(y, new_off)
