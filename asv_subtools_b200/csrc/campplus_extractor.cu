@@ -42,20 +42,13 @@ struct Conv {   // a bias-free Conv2d with its eval BatchNorm as the epilogue's 
   float* scale = nullptr; float* shift = nullptr;
 };
 
-struct Lin {   // a Conv1d on the wgmma layer kernel: y = [relu](W x + b) over the taps of `ctx`
-  Planes w;
-  float* bias = nullptr;
-  int cin = 0, cout = 0, flags = 0;
-  std::vector<int> ctx{0};
-};
-
 struct Dense {   // one CAMDenseTDNNLayer
   float* s1 = nullptr; float* t1 = nullptr;
-  Lin lin1, local;
+  Affine lin1, local;
   float* gw1 = nullptr; float* gb1 = nullptr; float* gw2 = nullptr; float* gb2 = nullptr;
 };
 
-struct Transit { float* s = nullptr; float* t = nullptr; Lin lin; };
+struct Transit { float* s = nullptr; float* t = nullptr; Affine lin; };
 
 struct ResBlk { int stride = 1; bool has_sc = false; Conv c1, c2, sc; };
 
@@ -65,7 +58,7 @@ struct Model {
   float* conv1_w = nullptr; float* conv1_s = nullptr; float* conv1_t = nullptr;
   ResBlk res[kResBlocks];
   Conv conv2;
-  Lin tdnn;
+  Affine tdnn;
   std::vector<Dense> layers[kBlocks];
   Transit transit[kBlocks];
   float* dense_w = nullptr; float* dense_s = nullptr; float* dense_t = nullptr;
@@ -122,19 +115,13 @@ int reserve(H* h, int B, int T) {
 
 Planes offset(Planes p, size_t n) { return {p.hi + n, p.lo + n}; }
 
-// _Lin.run / ops.tdnn_affine_ex: x planes (B, T, Cin) with row pitch ldx -> y planes (pitch ldy) or y_f32 (pitch ldyf)
-int lin(const Lin& l, Planes x, int64_t ldx, int Cin, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
+// ops.PackedAffine.run: x planes (B, T, l.Cin) with row pitch ldx -> y planes (pitch ldy) or yf (pitch ldyf); a nonzero
+// x_batch_stride makes x an im2col view (xvb_tdnn_args_t)
+int lin(const Affine& l, Planes x, int64_t ldx, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
         int64_t x_batch_stride, void* stream) {
-  xvb_tdnn_args_t a{};
-  a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
-  a.w_hi = l.w.hi; a.w_lo = l.w.lo;
-  a.bias = l.bias;
-  a.flags = l.flags;
-  a.context_host = l.ctx.data(); a.ntaps = (int)l.ctx.size();
+  xvb_tdnn_args_t a = affine_args(l, x, ldx, B, T);
   if (y) { a.y_hi = y->hi; a.y_lo = y->lo; a.ldy = ldy; }
-  if (yf) { a.y_f32 = yf; a.ldyf = ldyf; }
-  a.B = B; a.T = T; a.Cin = Cin; a.Cout = l.cout;
-  a.groups = 1;
+  a.y_f32 = yf; a.ldyf = ldyf;
   a.x_batch_stride = x_batch_stride;
   return xvb_tdnn_affine_ex(&a, stream);
 }
@@ -206,12 +193,12 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
   // tdnn: Conv1d(k = 5, stride 2, padding 2) as a 1-tap layer over 5-frame windows that start every 2 frames
   Planes bufs[kBlocks];
   for (int i = 0; i < kBlocks; ++i) bufs[i] = h->ws.planes(H::kBuf0 + i);
-  if ((rc = lin(m->tdnn, pad, 2 * row, 5 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, stream)))
+  if ((rc = lin(m->tdnn, pad, 2 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, stream)))
     return rc;
   *n += 1;
   const Planes pre = h->ws.planes(H::kPre), hh = h->ws.planes(H::kH), z = h->ws.planes(H::kZ);
   float* gate = h->ws.f32(H::kGate);
-  int c0 = m->tdnn.cout;
+  int c0 = m->tdnn.Cout;
   float* stats = h->ws.f32(H::kStats);
   for (int bi = 0; bi < kBlocks; ++bi) {
     const Planes buf = bufs[bi];
@@ -221,9 +208,9 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
       const int cin = c0 + li * g;
       Planes out = offset(buf, cin);
       if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, cin, L.s1, L.t1, pre.hi, pre.lo, m->maxw, stream)) ||
-          (rc = lin(L.lin1, pre, m->maxw, cin, B, T2, &hh, m->bn, nullptr, 0, 0, stream)) ||
+          (rc = lin(L.lin1, pre, m->maxw, B, T2, &hh, m->bn, nullptr, 0, 0, stream)) ||
           (rc = xvb_cam_gate(hh.hi, hh.lo, m->bn, B, T2, m->bn, kSegLen, L.gw1, L.gb1, m->bn / 2, L.gw2, L.gb2, g, gate, stream)) ||
-          (rc = lin(L.local, hh, m->bn, m->bn, B, T2, &z, g, nullptr, 0, 0, stream)) ||
+          (rc = lin(L.local, hh, m->bn, B, T2, &z, g, nullptr, 0, 0, stream)) ||
           (rc = xvb_seg_gate_apply(z.hi, z.lo, g, nullptr, nullptr, 0, gate, kSegLen, out.hi, out.lo, width, B, T2, g, stream)))
         return rc;
       *n += 5;
@@ -232,13 +219,13 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, width, tr.s, tr.t, pre.hi, pre.lo, m->maxw, stream))) return rc;
     *n += 1;
     if (bi + 1 < kBlocks) {
-      if ((rc = lin(tr.lin, pre, m->maxw, width, B, T2, &bufs[bi + 1], m->widths[bi + 1], nullptr, 0, 0, stream))) return rc;
+      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, &bufs[bi + 1], m->widths[bi + 1], nullptr, 0, 0, stream))) return rc;
       *n += 1;
-      c0 = tr.lin.cout;
+      c0 = tr.lin.Cout;
     } else {
       // out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance
       float* pool = h->ws.f32(H::kPool);
-      if ((rc = lin(tr.lin, pre, m->maxw, width, B, T2, nullptr, 0, pool, m->c3, 0, stream)) ||
+      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, nullptr, 0, pool, m->c3, 0, stream)) ||
           (rc = xvb_stats_pool_ex(pool, m->c3, B, T2, m->c3, 0.0f, 1, stats, nullptr, nullptr, 2 * m->c3, stream)))
         return rc;
       *n += 2;
@@ -316,13 +303,10 @@ static int build(Model* m, RecordStore& recs) {
       return rc;
     return XVB_OK;
   };
-  auto linear = [&](const std::string& n, int cout, int cin, bool bias, int flags, Lin* l) -> int {
+  auto linear = [&](const std::string& n, int cout, int cin, bool bias, int flags, Affine* l) -> int {
     const Rec* r;
     int rc = need(n, cout, cin, bias, false, flags, &r);
-    if (rc) return rc;
-    l->cin = cin; l->cout = cout; l->flags = flags;
-    if ((rc = m->dev.pack(&l->w, r->w, cout, cin, 1, l->ctx.data(), (int)l->ctx.size())) || (rc = m->dev.upload(&l->bias, r->b))) return rc;
-    return XVB_OK;
+    return rc ? rc : pack_affine(m->dev, l, r->w, cout, cin, kTaps, 1, r->b, r->s, r->t, flags);
   };
   auto norm = [&](const std::string& n, int C, float** s, float** t) -> int {
     const Rec* r;
@@ -364,16 +348,16 @@ static int build(Model* m, RecordStore& recs) {
       Dense L;
       if ((rc = norm(q + "nonlinear1", cin, &L.s1, &L.t1)) || (rc = linear(q + "linear1", m->bn, cin, true, XVB_RELU, &L.lin1)))
         return rc;
-      // linear_local: the dilated k = 3 kernel packed over its whole span, the gap taps as zeros (as _Lin packs it)
+      // linear_local: the dilated k = 3 kernel packed over its whole span, the gap taps as zeros (as ops.PackedAffine
+      // packs it)
       const std::string ln = q + "cam_layer.linear_local";
       if ((rc = need(ln, g, m->bn * 3, false, false, 0, &r))) return rc;
       const int span = 2 * d + 1;
       std::vector<float> full((size_t)g * m->bn * span, 0.f);
       for (size_t oc = 0; oc < (size_t)g * m->bn; ++oc)
         for (int k = 0; k < 3; ++k) full[oc * span + k * d] = r->w[oc * 3 + k];
-      L.local.cin = m->bn; L.local.cout = g; L.local.flags = 0;
-      L.local.ctx = {-d, 0, d};
-      if ((rc = m->dev.pack(&L.local.w, full, g, m->bn, span, L.local.ctx.data(), (int)L.local.ctx.size()))) return rc;
+      const int ctx[3] = {-d, 0, d};
+      if ((rc = pack_affine(m->dev, &L.local, full, g, m->bn, ctx, 3, r->b, r->s, r->t, 0))) return rc;
       if ((rc = plain(q + "cam_layer.linear1", m->bn / 2, m->bn, &L.gw1, &L.gb1)) ||
           (rc = plain(q + "cam_layer.linear2", g, m->bn / 2, &L.gw2, &L.gb2)))
         return rc;

@@ -34,19 +34,14 @@ constexpr int kMinFrames = 7;
 static_assert(sizeof(xvb_conformer_config_t) == 17 * sizeof(int32_t), "the XVBC0001 configuration block");
 const RecordFormat kFile = {"XVBC0001", sizeof(xvb_conformer_config_t), 2, 65536};
 
-struct Lin {   // a Linear / 1x1 conv on the wgmma layer kernel: y = epi(W x + b)
-  Planes w;
-  float* bias = nullptr; float* scale = nullptr; float* shift = nullptr;
-  int cin = 0, cout = 0, flags = 0;
-};
 struct Ln { float* g = nullptr; float* b = nullptr; };
 struct Layer {
-  Lin ff_mac1, ff_mac2, ff1, ff2, qkv, out, pw1, pw2;
+  Affine ff_mac1, ff_mac2, ff1, ff2, qkv, out, pw1, pw2;
   float* dw_w = nullptr; float* dw_b = nullptr;
   Ln cm_norm, norm_ff, norm_mha, norm_ff_macaron, norm_conv, norm_final;
   std::vector<float> mult;   // softmax_plus score multiplier per T' (host; passed by value to the kernel)
 };
-struct Seg { Lin lin; bool ln = false; Ln norm; };
+struct Seg { Affine lin; bool ln = false; Ln norm; };
 
 struct Model {
   xvb_conformer_config_t cfg{};
@@ -54,11 +49,11 @@ struct Model {
   float* head_w = nullptr; float* head_b = nullptr;
   Planes conv2_w;
   float* conv2_scale = nullptr; float* conv2_shift = nullptr;
-  Lin embed_out;
+  Affine embed_out;
   float* table = nullptr;
   std::vector<Layer> layers;
   Ln after_norm;
-  Lin transform, att1, att2;
+  Affine transform, att1, att2;
   bool transform_ln = false;
   Ln transform_norm, att_ln, norm_stats;
   std::vector<Seg> seg;
@@ -99,7 +94,7 @@ int reserve(xvb_conformer* h, int B, int T) {
   const size_t b = (size_t)B, D = (size_t)c.D, r2 = b * T2, od = (size_t)c.out_dim;
   const size_t units = (size_t)c.linear_units > D ? (size_t)c.linear_units : D;
   size_t seg = 8;
-  for (const Seg& s : h->m->seg) seg = (size_t)s.lin.cout > seg ? (size_t)s.lin.cout : seg;
+  for (const Seg& s : h->m->seg) seg = (size_t)s.lin.Cout > seg ? (size_t)s.lin.Cout : seg;
   const size_t need[xvb_conformer::kBufs] = {
       b * T1 * F1 * D, b * T2 * F2 * D, r2 * D, r2 * D, r2 * units, r2 * 2 * D, r2 * 3 * D, r2 * od, r2 * od,
       r2 * c.pool_hidden, r2 * c.pool_hidden, r2 * od, b * 2 * od, b * 2 * od, b * 2 * od, b * seg, b * seg};
@@ -107,20 +102,12 @@ int reserve(xvb_conformer* h, int B, int T) {
   return h->ws.reserve(need, kPlanes, &grown);
 }
 
-// _Lin.run: x planes (B, T, Cin) with row pitch ldx -> y planes (pitch ldy) and / or y_f32 (pitch ldyf)
-int lin(const Lin& l, Planes x, int64_t ldx, int Cin, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
+// ops.PackedAffine.run: x planes (B, T, l.Cin) with row pitch ldx -> y planes (pitch ldy) and / or yf (pitch ldyf)
+int lin(const Affine& l, Planes x, int64_t ldx, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
         void* stream) {
-  static const int ctx0 = 0;
-  xvb_tdnn_args_t a{};
-  a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
-  a.w_hi = l.w.hi; a.w_lo = l.w.lo;
-  a.bias = l.bias; a.bn_scale = l.scale; a.bn_shift = l.shift;
-  a.flags = l.flags;
-  a.context_host = &ctx0; a.ntaps = 1;
+  xvb_tdnn_args_t a = affine_args(l, x, ldx, B, T);
   if (y) { a.y_hi = y->hi; a.y_lo = y->lo; a.ldy = ldy; }
-  if (yf) { a.y_f32 = yf; a.ldyf = ldyf; }
-  a.B = B; a.T = T; a.Cin = Cin; a.Cout = l.cout;
-  a.groups = 1;
+  a.y_f32 = yf; a.ldyf = ldyf;
   return xvb_tdnn_affine_ex(&a, stream);
 }
 
@@ -176,7 +163,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     if ((rc = xvb_conv2d_valid(&a, stream)) != XVB_OK) return rc;
   }
   float* r = h->ws.f32(xvb_conformer::kR);
-  if ((rc = lin(m->embed_out, x2, (int64_t)F2 * D, F2 * D, B, T2, nullptr, 0, r, D, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->embed_out, x2, (int64_t)F2 * D, B, T2, nullptr, 0, r, D, stream)) != XVB_OK) return rc;
   *n += 3;
   const int units = c.linear_units;
   const int hid_ld = units > D ? units : D;
@@ -186,9 +173,9 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   float* d1 = delta;   // delta[..., :D], pitch 2D
   const float* rope = c.pos == 2 ? m->table : nullptr;
   const float* absp = c.pos == 1 ? m->table : nullptr;
-  auto ffn = [&](const Lin& a, const Lin& b) -> int {
-    int e = lin(a, hh, D, D, B, T2, &hid, hid_ld, nullptr, 0, stream);
-    return e ? e : lin(b, hid, hid_ld, units, B, T2, nullptr, 0, d1, 2 * D, stream);
+  auto ffn = [&](const Affine& a, const Affine& b) -> int {
+    int e = lin(a, hh, D, B, T2, &hid, hid_ld, nullptr, 0, stream);
+    return e ? e : lin(b, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream);
   };
   {
     LnCall l{rows, D, r, D};
@@ -209,20 +196,20 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     l.n = L.norm_mha;
     l.y = &hh; l.ldy = D;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
-    if ((rc = lin(L.qkv, hh, D, D, B, T2, nullptr, 0, qkv, 3 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.qkv, hh, D, B, T2, nullptr, 0, qkv, 3 * D, stream)) != XVB_OK) return rc;
     const float mult = c.softmax_plus ? L.mult[T2] : 1.0f;
     if ((rc = xvb_rope_attention(qkv, 3 * D, B, T2, c.H, m->dk, rope, c.rotary_value && rope ? 1 : 0, mult, hid.hi, hid.lo,
                                  hid_ld, stream)))
       return rc;
-    if ((rc = lin(L.out, hid, hid_ld, D, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.out, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
     l.delta_scale = 1.0f;
     l.n = L.norm_conv;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
-    if ((rc = lin(L.pw1, hh, D, D, B, T2, nullptr, 0, delta, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.pw1, hh, D, B, T2, nullptr, 0, delta, 2 * D, stream)) != XVB_OK) return rc;
     if ((rc = xvb_conv_module(delta, 2 * D, B, T2, D, L.dw_w, L.dw_b, c.conv_kernel, L.cm_norm.g, L.cm_norm.b, c.cm_norm,
                               1e-5f, c.act, hid.hi, hid.lo, hid_ld, stream)))
       return rc;
-    if ((rc = lin(L.pw2, hid, hid_ld, D, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.pw2, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
     l.n = L.norm_ff;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
     if ((rc = ffn(L.ff1, L.ff2)) != XVB_OK) return rc;
@@ -238,10 +225,10 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   float* xo = h->ws.f32(xvb_conformer::kXo);
   const Planes xp = h->ws.planes(xvb_conformer::kXp);
   if (!m->transform_ln) {
-    if ((rc = lin(m->transform, hh, D, D, B, T2, &xp, od, xo, od, stream)) != XVB_OK) return rc;
+    if ((rc = lin(m->transform, hh, D, B, T2, &xp, od, xo, od, stream)) != XVB_OK) return rc;
     *n += 1;
   } else {
-    if ((rc = lin(m->transform, hh, D, D, B, T2, nullptr, 0, xo, od, stream)) != XVB_OK) return rc;
+    if ((rc = lin(m->transform, hh, D, B, T2, nullptr, 0, xo, od, stream)) != XVB_OK) return rc;
     LnCall l{rows, od, xo, od};
     l.n = m->transform_norm;
     l.y = &xp; l.ldy = od;
@@ -251,7 +238,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   }
   // AttentiveStatsPool
   float* a1 = h->ws.f32(xvb_conformer::kA1);
-  if ((rc = lin(m->att1, xp, od, od, B, T2, nullptr, 0, a1, hd, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->att1, xp, od, B, T2, nullptr, 0, a1, hd, stream)) != XVB_OK) return rc;
   const Planes ap = h->ws.planes(xvb_conformer::kAp);
   {
     LnCall l{rows, hd, a1, hd};
@@ -261,7 +248,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
   }
   float* logits = h->ws.f32(xvb_conformer::kLogits);
-  if ((rc = lin(m->att2, ap, hd, hd, B, T2, nullptr, 0, logits, od, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->att2, ap, hd, B, T2, nullptr, 0, logits, od, stream)) != XVB_OK) return rc;
   float* stats = h->ws.f32(xvb_conformer::kStats);
   if ((rc = xvb_attn_stats_pool(logits, od, xo, od, B, T2, od, 1e-5f, stats, nullptr, nullptr, 2 * od, stream)) != XVB_OK) return rc;
   Planes z = h->ws.planes(xvb_conformer::kZ);
@@ -279,9 +266,9 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   for (int j = 0; j < ns; ++j) {
     const Seg& s = m->seg[j];
     const bool last = j + 1 == ns;
-    const int co = s.lin.cout;
+    const int co = s.lin.Cout;
     float* y = last ? emb : h->ws.f32(xvb_conformer::kSegY);
-    if ((rc = lin(s.lin, z, zc, zc, B, 1, nullptr, 0, y, co, stream)) != XVB_OK) return rc;
+    if ((rc = lin(s.lin, z, zc, B, 1, nullptr, 0, y, co, stream)) != XVB_OK) return rc;
     *n += 1;
     const Planes yp = h->ws.planes(xvb_conformer::kSegP);
     if (s.ln) {
@@ -352,19 +339,15 @@ static int build(Model* m, RecordStore& recs) {
     return recs.take("xvb_conformer_finalize", n, shape, out);
   };
   // a Linear: weight and bias; the folded BatchNorm / xscale and the activation as flagged
-  auto linear = [&](const std::string& n, int cout, int cin, Lin* l) -> int {
+  auto linear = [&](const std::string& n, int cout, int cin, Affine* l) -> int {
     const Rec* r;
     int rc = need(n, cout, cin, &r);
     if (rc) return rc;
     XVB_CHECK_ARG(!r->b.empty(), "xvb_conformer_finalize: record '%s' needs its bias", n.c_str());
     XVB_CHECK_ARG(r->s.empty() || (r->flags & XVB_BN), "xvb_conformer_finalize: record '%s' has scale/shift without XVB_BN", n.c_str());
-    l->cin = cin; l->cout = cout; l->flags = r->flags;
-    if ((rc = m->dev.pack(&l->w, r->w, cout, cin, 1, kTaps, 1)) || (rc = m->dev.upload(&l->bias, r->b)) || (rc = m->dev.upload(&l->scale, r->s)) ||
-        (rc = m->dev.upload(&l->shift, r->t)))
-      return rc;
-    return XVB_OK;
+    return pack_affine(m->dev, l, r->w, cout, cin, kTaps, 1, r->b, r->s, r->t, r->flags);
   };
-  auto plain = [&](const std::string& n, int cout, int cin, Lin* l) -> int {
+  auto plain = [&](const std::string& n, int cout, int cin, Affine* l) -> int {
     int rc = linear(n, cout, cin, l);
     if (rc) return rc;
     XVB_CHECK_ARG(l->flags == 0, "xvb_conformer_finalize: record '%s' must be a plain affine (flags %d)", n.c_str(), l->flags);
@@ -457,14 +440,14 @@ static int build(Model* m, RecordStore& recs) {
     XVB_CHECK_ARG(ra, "xvb_conformer_finalize: record '%s' is missing", a.c_str());
     Seg s;
     if ((rc = w.whole ? linear(a, ra->shape[0], cin, &s.lin) : plain(a, ra->shape[0], cin, &s.lin)) != XVB_OK) return rc;
-    XVB_CHECK_ARG(s.lin.cout % 8 == 0, "xvb_conformer_finalize: record '%s' has %d rows, need a multiple of 8", a.c_str(), s.lin.cout);
+    XVB_CHECK_ARG(s.lin.Cout % 8 == 0, "xvb_conformer_finalize: record '%s' has %d rows, need a multiple of 8", a.c_str(), s.lin.Cout);
     s.ln = w.whole && recs.find(b) != nullptr;
-    if (s.ln && (rc = norm(b, s.lin.cout, false, &s.norm))) return rc;
+    if (s.ln && (rc = norm(b, s.lin.Cout, false, &s.norm))) return rc;
     XVB_CHECK_ARG(!(s.ln && (s.lin.flags & XVB_BN)), "xvb_conformer_finalize: '%s' has both a LayerNorm and a folded BatchNorm", w.name);
     m->seg.push_back(s);
-    cin = s.lin.cout;
+    cin = s.lin.Cout;
   }
-  m->E = m->seg.back().lin.cout;
+  m->E = m->seg.back().lin.Cout;
   return recs.check_all_used("xvb_conformer_finalize");
 }
 

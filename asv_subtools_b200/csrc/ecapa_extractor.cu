@@ -31,12 +31,8 @@ namespace {
 
 using namespace xvb;
 
-struct ELayer : TapLayer {
+struct ELayer : Affine {
   float* w_f32 = nullptr;   // (Cout, Cin) fp32 as stored, kept for one-tap layers: the segment-level ones run on CUDA cores
-  // grouped 1x1 conv (the MQMHA attention convs): Cin is the per-group width; packed compactly for the layer kernel's
-  // grouped mode, or as the block-diagonal expansion (expanded) when the shape does not fit that mode
-  int groups = 1;
-  bool expanded = false;
 };
 
 // One SE-Res2Net block ("layer2." .. "layer4."): its 1x1 convs and SE gate, and its scale - 1 Res2Net convs ("res0" ..)
@@ -178,24 +174,23 @@ extern "C" int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, i
   return XVB_OK;
 }
 
-// r on the device as L.  A grouped shape the layer kernel's grouped mode does not take runs as its block-diagonal
-// expansion.
+// r on the device as L.  A grouped layer (the MQMHA attention convs, r.Cin the per-group width) is packed compactly for
+// the layer kernel's grouped mode, or as its block-diagonal expansion when the shape does not fit that mode.
 static int build_layer(Model* m, const TapRec& r, ELayer* L) {
-  L->groups = layer_groups(m->cfg, r.name);
-  L->expanded = L->groups > 1 && !xvb_tdnn_grouped_fits(r.Cin * L->groups, r.Cout, L->groups);
-  std::vector<float> dense;
-  int cin_pack = r.Cin;
-  if (L->expanded) {
-    const int G = L->groups, co = r.Cout / G;
-    cin_pack = r.Cin * G;
-    dense.assign((size_t)r.Cout * cin_pack, 0.f);
-    for (int n = 0; n < r.Cout; ++n)
-      memcpy(&dense[(size_t)n * cin_pack + (size_t)(n / co) * r.Cin], &r.w[(size_t)n * r.Cin], r.Cin * sizeof(float));
-  }
+  const int G = layer_groups(m->cfg, r.name), cin = r.Cin * G;
   int rc;
-  if ((rc = pack_tap(m->dev, r, L, L->expanded ? dense : r.w, cin_pack))) return rc;
+  if (G > 1 && !xvb_tdnn_grouped_fits(cin, r.Cout, G)) {
+    const int co = r.Cout / G;
+    std::vector<float> dense((size_t)r.Cout * cin, 0.f);
+    for (int n = 0; n < r.Cout; ++n)
+      memcpy(&dense[(size_t)n * cin + (size_t)(n / co) * r.Cin], &r.w[(size_t)n * r.Cin], r.Cin * sizeof(float));
+    rc = pack_affine(m->dev, L, dense, r.Cout, cin, r.ctx, r.ntaps, r.b, r.s, r.t, r.flags);
+  } else {
+    rc = pack_affine(m->dev, L, r.w, r.Cout, cin, r.ctx, r.ntaps, r.b, r.s, r.t, r.flags, G);
+  }
+  if (rc) return rc;
   // one tap: (Cout, Cin, 1) is the (N, K) matrix xvb_small_affine takes
-  if (r.tot() == 1 && r.Cin % 4 == 0 && L->groups == 1 && (rc = m->dev.upload(&L->w_f32, r.w))) return rc;
+  if (r.tot() == 1 && r.Cin % 4 == 0 && G == 1 && (rc = m->dev.upload(&L->w_f32, r.w))) return rc;
   return XVB_OK;
 }
 
@@ -313,38 +308,17 @@ static int reserve(xvb_ecapa* h, int B, int T) {
 }
 
 namespace {
-struct Run {   // one layer launch: fill only what differs from the defaults
-  const ELayer* L;
-  View x, y;
-  float* y_f32 = nullptr;
-  int64_t ldyf = 0;
-  const float* utt_bias = nullptr;
-  int64_t ld_utt = 0;
-  int extra_flags = 0;
-  int B, T;
-  int im2col_taps = 0;          // > 0: one-tap view, Cin = taps * L->Cin, rows overlap (x_batch_stride)
-  int64_t x_batch_stride = 0;
-};
+// The layer-kernel arguments of L over x at (B, T) into the planes y and / or the fp32 yf (row pitch ldyf)
+xvb_tdnn_args_t layer_args(const ELayer& L, const View& x, int B, int T, const View& y, float* yf = nullptr, int64_t ldyf = 0) {
+  xvb_tdnn_args_t a = affine_args(L, Planes{x.hi, x.lo}, x.ld, B, T);
+  a.y_hi = y.hi; a.y_lo = y.lo; a.ldy = y.ld;
+  a.y_f32 = yf; a.ldyf = ldyf;
+  return a;
+}
 // segment-level layer (one row per utterance) on CUDA cores: fp32 in, fp32 out
 int small_layer(const ELayer* L, const float* x, int64_t ldx, int B, float* y, int64_t ldy, int extra_flags, void* stream) {
   return xvb_small_affine(x, ldx, L->w_f32, B, L->Cin, L->Cout, L->bias, L->scale, L->shift, L->flags | extra_flags, y, ldy,
                           nullptr, nullptr, 0, stream);
-}
-int launch(const Run& r, void* stream) {
-  xvb_tdnn_args_t a{};
-  a.x_hi = r.x.hi; a.x_lo = r.x.lo; a.ldx = r.x.ld;
-  a.w_hi = r.L->w.hi; a.w_lo = r.L->w.lo;
-  a.bias = r.L->bias; a.bn_scale = r.L->scale; a.bn_shift = r.L->shift;
-  a.flags = r.L->flags | r.extra_flags;
-  a.utt_bias = r.utt_bias; a.ld_utt_bias = r.ld_utt;
-  a.context_host = r.L->ctx; a.ntaps = r.L->ntaps;
-  const int ctx0 = 0;
-  if (r.im2col_taps > 0) { a.context_host = &ctx0; a.ntaps = 1; a.x_batch_stride = r.x_batch_stride; }
-  a.y_hi = r.y.hi; a.y_lo = r.y.lo; a.ldy = r.y.ld;
-  a.y_f32 = r.y_f32; a.ldyf = r.ldyf;
-  a.B = r.B; a.T = r.T; a.Cin = r.im2col_taps > 0 ? r.im2col_taps * r.L->Cin : r.L->Cin * r.L->groups; a.Cout = r.L->Cout;
-  a.groups = r.L->expanded ? 1 : r.L->groups;
-  return xvb_tdnn_affine_ex(&a, stream);
 }
 }  // namespace
 
@@ -356,20 +330,20 @@ int launch(const Run& r, void* stream) {
 static int mqmha_pool(xvb_ecapa* h, int B, int T, void* stream) {
   const Model* m = h->m.get();
   const int D = m->cfg.D, cg = D / m->cfg.mq_heads;
-  const ELayer* ax = &m->att_x;
   int rc;
   if (m->cfg.mq_tatt) {
     if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 0, h->gstat, nullptr, nullptr, 0, stream))) return rc;
     if ((rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.AX, 0, stream))) return rc;
   }
-  Run r{}; r.B = B; r.T = T; r.L = ax; r.x = h->M;
-  if (m->cfg.mq_tatt) { r.utt_bias = h->ub; r.ld_utt = m->cfg.AX; }
-  if (m->cfg.mq_layers == 2) { r.y = h->A1; r.extra_flags = XVB_TANH; }
-  else { r.y_f32 = h->LOG; r.ldyf = m->cfg.ldlog; }
-  if ((rc = launch(r, stream))) return rc;
-  if (m->cfg.mq_layers == 2) {
-    r = Run{}; r.B = B; r.T = T; r.L = &m->att2; r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = m->cfg.ldlog;
-    if ((rc = launch(r, stream))) return rc;
+  const bool two = m->cfg.mq_layers == 2;
+  xvb_tdnn_args_t a = two ? layer_args(m->att_x, h->M, B, T, h->A1)
+                          : layer_args(m->att_x, h->M, B, T, View{}, h->LOG, m->cfg.ldlog);
+  if (two) a.flags |= XVB_TANH;
+  if (m->cfg.mq_tatt) { a.utt_bias = h->ub; a.ld_utt_bias = m->cfg.AX; }
+  if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
+  if (two) {
+    a = layer_args(m->att2, h->A1, B, T, View{}, h->LOG, m->cfg.ldlog);
+    if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
   }
   return xvb_attn_head_stats_pool_mq(h->LOG, m->cfg.ldlog, m->cfg.NL, h->MF, D, B, T, D, m->cfg.mq_q * D, m->cfg.mq_share ? cg : 1, cg, m->cfg.mq_q,
                                      1e-5f, 0, h->pstat, nullptr, nullptr, 0, stream);
@@ -389,11 +363,12 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   else
     rc = xvb_split_f32(feats, (int64_t)B * T, m->cfg.feat_dim, m->cfg.feat_dim, h->in.hi, h->in.lo, m->cfg.ldf, stream);
   if (rc) return rc;
-  Run r{};
-  r.B = B; r.T = T;
-  r.L = &m->layer1; r.x = h->in; r.y = h->X;
-  if (im.on) { r.im2col_taps = r.L->ntaps; r.x_batch_stride = (int64_t)(T + im.pad_front + im.pad_back) * m->cfg.ldf; }
-  rc = launch(r, stream);
+  xvb_tdnn_args_t a = layer_args(m->layer1, h->in, B, T, h->X);
+  if (im.on) {   // window of ntaps consecutive frames = one long row of the padded planes
+    a.context_host = kTaps; a.ntaps = 1; a.Cin = m->layer1.ntaps * m->layer1.Cin;
+    a.x_batch_stride = (int64_t)(T + im.pad_front + im.pad_back) * m->cfg.ldf;
+  }
+  rc = xvb_tdnn_affine_ex(&a, stream);
   if (rc && im.on) {   // overlapping tensor map refused by the driver: plain path from now on
     h->im2col = Im2col{};
     return xvb_ecapa_extract(h, feats, B, T, emb, stream);
@@ -402,13 +377,13 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   View cur = h->X;
   for (int b = 0; b < 3; ++b) {
     const Block& k = m->blocks[b];
-    r = Run{}; r.B = B; r.T = T; r.L = &k.bn1; r.x = cur; r.y = h->Hh;
-    if ((rc = launch(r, stream))) return rc;
+    a = layer_args(k.bn1, cur, B, T, h->Hh);
+    if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
     if ((rc = xvb_res2net_block_ex(h->Hh.hi, h->Hh.lo, C, k.res_w.hi, k.res_w.lo, k.res_bias, k.res_scale, k.res_shift,
                                    k.dilation, m->cfg.scale, h->R.hi, h->R.lo, C, B, T, C / m->cfg.scale, stream)))
       return rc;
-    r = Run{}; r.B = B; r.T = T; r.L = &k.bn2; r.x = h->R; r.y = h->Z;
-    if ((rc = launch(r, stream))) return rc;
+    a = layer_args(k.bn2, h->R, B, T, h->Z);
+    if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
     if ((rc = xvb_plane_mean(h->Z.hi, h->Z.lo, C, B, T, C, h->zmean, nullptr, nullptr, 0, stream)) ||
         (rc = small_layer(&k.se1, h->zmean, C, B, h->s1f, m->se_dim, 0, stream)) ||
         (rc = small_layer(&k.se2, h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream)))
@@ -420,18 +395,19 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
       return rc;
     cur = h->N;
   }
-  r = Run{}; r.B = B; r.T = T; r.L = &m->mfa; r.x = h->CAT; r.y = h->M; r.y_f32 = h->MF; r.ldyf = D;
-  if ((rc = launch(r, stream))) return rc;
+  a = layer_args(m->mfa, h->CAT, B, T, h->M, h->MF, D);
+  if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
   if (m->cfg.mq) {
     if ((rc = mqmha_pool(h, B, T, stream))) return rc;
   } else {
   if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, nullptr, nullptr, 0, stream)) ||
       (rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream)))
     return rc;
-  r = Run{}; r.B = B; r.T = T; r.L = &m->att_x; r.x = h->M; r.y = h->A1; r.utt_bias = h->ub; r.ld_utt = m->cfg.H; r.extra_flags = XVB_TANH;
-  if ((rc = launch(r, stream))) return rc;
-  r = Run{}; r.B = B; r.T = T; r.L = &m->att2; r.x = h->A1; r.y_f32 = h->LOG; r.ldyf = D;
-  if ((rc = launch(r, stream))) return rc;
+  a = layer_args(m->att_x, h->M, B, T, h->A1);
+  a.flags |= XVB_TANH; a.utt_bias = h->ub; a.ld_utt_bias = m->cfg.H;
+  if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
+  a = layer_args(m->att2, h->A1, B, T, View{}, h->LOG, D);
+  if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
   if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, nullptr, nullptr, 0, stream))) return rc;
   }
   if (m->fc1.Cout) {              // fc1 [-> fc2] on CUDA cores (fp32)

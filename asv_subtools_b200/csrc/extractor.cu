@@ -27,7 +27,7 @@ struct Model {
   Config cfg;
   Layers recs;
   float pooling_eps = 1e-10f;
-  std::vector<TapLayer> frame, segment;   // recs on the device, built at finalize
+  std::vector<Affine> frame, segment;   // recs on the device, built at finalize
   int max_c = 0, max_seg_c = 0;
   Im2col im2col;   // the first layer as an im2col view (records.cuh)
   Weights dev{"xvb_extractor_finalize"};
@@ -234,19 +234,14 @@ static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
     return XVB_OK;
   };
   for (size_t i = 0; i < m->frame.size(); ++i) {
-    const TapLayer& L = m->frame[i];
+    const Affine& L = m->frame[i];
     const bool last = i + 1 == m->frame.size();
     const Planes y = last ? Planes{} : h->ws.planes(H::kAct0 + (i & 1));
-    xvb_tdnn_args_t a{};
-    a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
-    a.bias = L.bias; a.bn_scale = L.scale; a.bn_shift = L.shift; a.flags = L.flags;
-    a.context_host = L.ctx; a.ntaps = L.ntaps;
+    xvb_tdnn_args_t a = affine_args(L, x, ldx, B, T);
     a.y_hi = y.hi; a.y_lo = y.lo; a.ldy = L.Cout;
-    a.B = B; a.T = T; a.Cin = L.Cin; a.Cout = L.Cout;
     a.lengths = masked ? h->ws.i32(H::kLengths) : nullptr;
-    const int ctx0 = 0;
     if (i == 0 && h->im2col.on) {   // window of ntaps consecutive frames = one long row of the padded planes
-      a.context_host = &ctx0; a.ntaps = 1; a.Cin = L.ntaps * L.Cin;
+      a.context_host = kTaps; a.ntaps = 1; a.Cin = L.ntaps * L.Cin;
       a.x_batch_stride = (int64_t)(T + h->im2col.pad_front + h->im2col.pad_back) * ldx;
     }
     if (last && h->fused_pooling && !masked) {
@@ -262,16 +257,12 @@ static int build_step_plan(H* h, int B, int T, bool masked, StepPlan** out) {
   const int cl = m->frame.back().Cout;
   x = h->ws.planes(H::kStatsPlanes); ldx = 2 * cl;
   for (size_t i = 0; i < m->segment.size(); ++i) {
-    const TapLayer& L = m->segment[i];
+    const Affine& L = m->segment[i];
     const bool last = i + 1 == m->segment.size();
     const Planes y = last ? Planes{} : h->ws.planes(H::kSeg0 + (i & 1));
-    xvb_tdnn_args_t a{};
-    a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx; a.w_hi = L.w.hi; a.w_lo = L.w.lo;
-    a.bias = L.bias; a.bn_scale = L.scale; a.bn_shift = L.shift; a.flags = L.flags;
-    a.context_host = L.ctx; a.ntaps = 1;
+    xvb_tdnn_args_t a = affine_args(L, x, ldx, B, 1);
     a.y_hi = y.hi; a.y_lo = y.lo; a.ldy = L.Cout;
     if (last) { a.y_f32 = h->ws.f32(H::kEmb); a.ldyf = L.Cout; }   // redirected to the caller's matrix at launch
-    a.B = B; a.T = 1; a.Cin = L.Cin; a.Cout = L.Cout;
     if ((rc = add(sp->segment, a))) return rc;
     x = y; ldx = L.Cout;
   }

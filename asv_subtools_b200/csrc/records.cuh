@@ -1,6 +1,6 @@
 // Device side of the native extractors' shared plumbing: the handle base, the packed split-bf16 planes and the arena
-// that owns a model's device weights (every family), the device tap layer of the TDNN and ECAPA-TDNN, the grow-only
-// workspace, the segment level of the 2-D families, the group loop of an extract call and the lengths check of a masked
+// that owns a model's device weights (every family), the packed affine layer and its layer-kernel arguments (every
+// family), the grow-only workspace, the segment level of the 2-D families, the group loop of an extract call and the lengths check of a masked
 // one.  The host records and the model-file codecs are host code in records.h.
 #pragma once
 #include <stdlib.h>
@@ -86,25 +86,48 @@ struct Weights {
   }
 };
 
-// A TDNN or ECAPA-TDNN layer on the device: its record's shape, packed weight and parameters.
-struct TapLayer : TapShape {
+// One affine layer on the wgmma layer kernel, in every family: its shape (Cout, Cin, the taps of ctx, the epilogue
+// flags), packed weight, bias, scale and shift.  Cin and groups are what the kernel is called with: a compact grouped
+// layer keeps its whole input width and its G groups, a block-diagonal expansion its whole input width and 1.
+struct Affine : TapShape {
   Planes w;
   float* bias = nullptr;
   float* scale = nullptr;
   float* shift = nullptr;
+  int groups = 1;
 };
 
-// r on the device: its shape, the (Cout, cin, tot) weight w packed (r.w over r.Cin, or what stands in for it, such as
-// the block-diagonal expansion of a grouped layer) and r's bias, scale and shift.
-inline int pack_tap(Weights& dev, const TapRec& r, TapLayer* L, const std::vector<float>& w, int cin) {
-  static_cast<TapShape&>(*L) = r;
+// L on the device: w (Cout, Cin / groups, tot) fp32 host over the taps ctx[0..ntaps) packed, and b, s, t uploaded (each
+// empty when the layer has none).
+inline int pack_affine(Weights& dev, Affine* L, const std::vector<float>& w, int Cout, int Cin, const int* ctx, int ntaps,
+                       const std::vector<float>& b, const std::vector<float>& s, const std::vector<float>& t, int flags,
+                       int groups = 1) {
+  L->Cout = Cout; L->Cin = Cin; L->ntaps = ntaps; L->flags = flags; L->groups = groups;
+  for (int i = 0; i < ntaps; ++i) L->ctx[i] = ctx[i];
   int rc;
-  if ((rc = dev.pack(&L->w, w, r.Cout, cin, r.tot(), r.ctx, r.ntaps)) || (rc = dev.upload(&L->bias, r.b)) ||
-      (rc = dev.upload(&L->scale, r.s)) || (rc = dev.upload(&L->shift, r.t)))
+  if ((rc = dev.pack(&L->w, w, Cout, Cin / groups, L->tot(), ctx, ntaps)) || (rc = dev.upload(&L->bias, b)) ||
+      (rc = dev.upload(&L->scale, s)) || (rc = dev.upload(&L->shift, t)))
     return rc;
   return XVB_OK;
 }
-inline int pack_tap(Weights& dev, const TapRec& r, TapLayer* L) { return pack_tap(dev, r, L, r.w, r.Cin); }
+inline int pack_tap(Weights& dev, const TapRec& r, Affine* L) {
+  return pack_affine(dev, L, r.w, r.Cout, r.Cin, r.ctx, r.ntaps, r.b, r.s, r.t, r.flags);
+}
+
+// The layer-kernel arguments of L over the planes x (row pitch ldx) at (B, T): input, weight, parameters, flags, taps,
+// Cin, Cout and groups.  The caller sets what is its own: the outputs, and any utt_bias, x2, lengths, pool_partial,
+// x_batch_stride or im2col view.
+inline xvb_tdnn_args_t affine_args(const Affine& L, Planes x, int64_t ldx, int B, int T) {
+  xvb_tdnn_args_t a{};
+  a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
+  a.w_hi = L.w.hi; a.w_lo = L.w.lo;
+  a.bias = L.bias; a.bn_scale = L.scale; a.bn_shift = L.shift;
+  a.flags = L.flags;
+  a.context_host = L.ctx; a.ntaps = L.ntaps;
+  a.B = B; a.T = T; a.Cin = L.Cin; a.Cout = L.Cout;
+  a.groups = L.groups;
+  return a;
+}
 
 // taps 0 .. n-1 of a weight packed over its whole span
 constexpr int kTaps[9] = {0, 1, 2, 3, 4, 5, 6, 7, 8};
@@ -162,15 +185,9 @@ inline Im2col im2col_choice(const int* ctx, int ntaps, int feat_dim) {
 }
 
 // The segment level of the 2-D families (ResNet, RepVGG): statistics pooling of the last conv's fp32 (B, T', F' * C)
-// output with planes out, then [fc1 ->] fc2 on the wgmma layer kernel at T = 1, each as _PackedAffine runs it.
-struct SegLayer {   // one segment layer, output rows padded to a multiple of 8
-  Planes w;
-  float* bias = nullptr; float* scale = nullptr; float* shift = nullptr;
-  int Cin = 0, Cout = 0, Cout_real = 0, flags = 0;
-};
-
+// output with planes out, then [fc1 ->] fc2 on the wgmma layer kernel at T = 1, each as ops.PackedAffine runs it.
 struct SegTail {
-  std::vector<SegLayer> seg;
+  std::vector<Affine> seg;   // output rows padded to a multiple of 8
   int E = 0;     // the embedding dim, the last layer's real rows
   int mid = 0;   // the first layer's padded rows when there are two layers, else 0
 
@@ -184,21 +201,17 @@ struct SegTail {
       const int shape[3] = {s->shape[0], cin, 1};
       int rc = recs.take(fn, n, shape, &s);
       if (rc) return rc;
-      SegLayer g;
-      g.Cin = cin; g.Cout_real = s->shape[0]; g.Cout = (s->shape[0] + 7) / 8 * 8;
-      g.flags = (s->flags & XVB_RELU) | (s->s.empty() ? 0 : XVB_BN);
+      E = s->shape[0];
+      const int Cout = (E + 7) / 8 * 8;
       std::vector<float> w(s->w), b(s->b), sc(s->s), sh(s->t);
-      w.resize((size_t)g.Cout * cin, 0.f);
-      if (!b.empty()) b.resize(g.Cout, 0.f);
-      if (!sc.empty()) { sc.resize(g.Cout, 0.f); sh.resize(g.Cout, 0.f); }
-      if ((rc = dev.pack(&g.w, w, g.Cout, cin, 1, kTaps, 1)) || (rc = dev.upload(&g.bias, b)) || (rc = dev.upload(&g.scale, sc)) ||
-          (rc = dev.upload(&g.shift, sh)))
-        return rc;
-      seg.push_back(g);
-      cin = s->shape[0];
+      w.resize((size_t)Cout * cin, 0.f);
+      if (!b.empty()) b.resize(Cout, 0.f);
+      if (!sc.empty()) { sc.resize(Cout, 0.f); sh.resize(Cout, 0.f); }
+      const int flags = (s->flags & XVB_RELU) | (s->s.empty() ? 0 : XVB_BN);
+      if ((rc = pack_affine(dev, &seg.emplace_back(), w, Cout, cin, kTaps, 1, b, sc, sh, flags))) return rc;
+      cin = E;
     }
     XVB_CHECK_ARG(!seg.empty(), "%s: record 'fc1' or 'fc2' is missing (no segment layer)", fn);
-    E = seg.back().Cout_real;
     mid = seg.size() > 1 ? seg[0].Cout : 0;
     return XVB_OK;
   }
@@ -213,23 +226,15 @@ struct SegTail {
     if ((rc = stats_pool(last, pc, B, T, pc, eps, 0, lengths, pooled_f32, pooled.hi, pooled.lo, 2 * pc, stream))) return rc;
     Planes x = pooled;
     int64_t ldx = 2 * pc;
-    const int ctx0 = 0;
     for (size_t j = 0; j < seg.size(); ++j) {
-      const SegLayer& s = seg[j];
-      const bool fin = j + 1 == seg.size();
-      xvb_tdnn_args_t a{};
-      a.x_hi = x.hi; a.x_lo = x.lo; a.ldx = ldx;
-      a.w_hi = s.w.hi; a.w_lo = s.w.lo;
-      a.bias = s.bias; a.bn_scale = s.scale; a.bn_shift = s.shift;
-      a.flags = s.flags;
-      a.context_host = &ctx0; a.ntaps = 1;
-      if (fin) { a.y_f32 = s.Cout == E ? emb : out; a.ldyf = s.Cout; }
+      const Affine& s = seg[j];
+      xvb_tdnn_args_t a = affine_args(s, x, ldx, B, 1);
+      if (j + 1 == seg.size()) { a.y_f32 = s.Cout == E ? emb : out; a.ldyf = s.Cout; }
       else { a.y_hi = mid_planes.hi; a.y_lo = mid_planes.lo; a.ldy = s.Cout; }
-      a.B = B; a.T = 1; a.Cin = s.Cin; a.Cout = s.Cout;
       if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
       x = mid_planes; ldx = s.Cout;
     }
-    const SegLayer& s = seg.back();
+    const Affine& s = seg.back();
     if (s.Cout != E)
       XVB_CUDA(cudaMemcpy2DAsync(emb, (size_t)E * sizeof(float), out, (size_t)s.Cout * sizeof(float), (size_t)E * sizeof(float),
                                  (size_t)B, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));

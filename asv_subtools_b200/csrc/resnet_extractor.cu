@@ -10,8 +10,8 @@
 //   (ReLU, sigmoid) -> SE scaling + residual -> statistics pooling (planes out) -> segment layers.
 //
 // Records are handed over by their state_dict module path with the weights as stored (host fp32), eval BatchNorm
-// folded to (scale, shift) by the caller; the segment layers arrive as the Python hands them to _PackedAffine (fc1 /
-// fc2 export(), the first one's input columns already permuted to the (B, T', F', C) pooling order).  This file only
+// folded to (scale, shift) by the caller; the segment layers arrive as the Python hands them to ops.PackedAffine (fc1
+// / fc2 export(), the first one's input columns already permuted to the (B, T', F', C) pooling order).  This file only
 // packs and pads: conv weights through xvb_pack_tdnn_weight, the SE hidden width zero-padded to a multiple of 4 with
 // fc_1 replicated k times (divided by k) for the k-grouped plane mean, segment rows padded to a multiple of 8.
 #include <cuda_runtime.h>

@@ -247,31 +247,6 @@ def _fold(w, bn, bias=None):
     return w.detach().float() * s.view(-1, *([1] * (w.dim() - 1))), b
 
 
-class _Lin:
-    """A kernel-size-1 (or dilated k = 3) Conv1d record packed for the layer kernel, with its bias and ReLU."""
-
-    def __init__(self, w, bias, device, context=(0,), relu=False):
-        w = _vec(w, device)
-        self.cout = w.shape[0]
-        self.context = list(context)
-        w = w.reshape(self.cout, w.shape[1], -1)
-        span = self.context[-1] - self.context[0] + 1
-        if w.shape[2] != span:              # a dilated kernel: the packer takes the whole span, the gaps as zero taps
-            full = torch.zeros(self.cout, w.shape[1], span, device=device)
-            full[:, :, [c - self.context[0] for c in self.context]] = w
-            w = full
-        self.w = ops.pack_tdnn_weight(w.contiguous(), self.context)
-        self.bias = _vec(bias, device) if bias is not None else None
-        self.relu = relu
-
-    def run(self, x, **kw):
-        ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, relu=self.relu, **kw)
-
-
-def _vec(t, device):
-    return torch.as_tensor(t).detach().float().to(device).contiguous()
-
-
 class CamPPExtractor:
     """Folded weights on one device + the launch sequence of CamPP.forward for one chunk per utterance (all utterances of
     a call have the same length), driven from Python over a workspace reused while the batch shape stays the same.  The
@@ -290,7 +265,7 @@ class CamPPExtractor:
             """(fp32 weight (Cout, Cin, k, k), scale, shift) of a bias-free Conv2d record with its folded BatchNorm."""
             w, _, sc, sh, _, _ = recs[name]
             k = math.isqrt(w.shape[1] // cin)
-            return _vec(w.reshape(w.shape[0], cin, k, k), device), _vec(sc, device), _vec(sh, device)
+            return ops.to_device(w.reshape(w.shape[0], cin, k, k), device), ops.to_device(sc, device), ops.to_device(sh, device)
 
         def packed(name):
             w, sc, sh = conv(name, M_CHANNELS)
@@ -305,7 +280,7 @@ class CamPPExtractor:
                 self.res_blocks.append((2 if i == 0 else 1, packed(p + "conv1"), packed(p + "conv2"), sc))
         self.conv2 = packed("head.conv2")
         w, b = recs["xvector.tdnn.linear"][:2]
-        self.tdnn = _Lin(w, b, device, relu=True)
+        self.tdnn = ops.PackedAffine(w, device, bias=b, relu=True)
         self.blocks, self.transits, self.widths = [], [], []
         for i, (layers, dilation) in enumerate(BLOCKS):
             L = []
@@ -315,20 +290,21 @@ class CamPPExtractor:
                 s1, t1 = recs[p + "nonlinear1"][2:4]
                 w1, b1 = recs[p + "linear1"][:2]
                 local = recs[q + "linear_local"][0]
-                L.append({"s1": _vec(s1, device), "t1": _vec(t1, device), "lin1": _Lin(w1, b1, device, relu=True),
-                          "local": _Lin(local.reshape(local.shape[0], self.bn_ch, -1), None, device,
-                                        context=(-dilation, 0, dilation)),
-                          "gate": tuple(_vec(a.reshape(a.shape[0], -1), device)
+                L.append({"s1": ops.to_device(s1, device), "t1": ops.to_device(t1, device),
+                          "lin1": ops.PackedAffine(w1, device, bias=b1, relu=True),
+                          "local": ops.PackedAffine(local.reshape(local.shape[0], self.bn_ch, -1), device,
+                                                    (-dilation, 0, dilation)),
+                          "gate": tuple(ops.to_device(a.reshape(a.shape[0], -1), device)
                                         for name in ("linear1", "linear2") for a in recs[q + name][:2])})
             self.blocks.append(L)
             p = "xvector.transit{}.".format(i + 1)
             s, sh = recs[p + "nonlinear"][2:4]
             w, b, _, _, flags, _ = recs[p + "linear"]
-            self.transits.append((_vec(s, device), _vec(sh, device),
-                                  _Lin(w, b, device, relu=bool(flags & RELU))))
+            self.transits.append((ops.to_device(s, device), ops.to_device(sh, device),
+                                  ops.PackedAffine(w, device, bias=b, relu=bool(flags & RELU))))
             self.widths.append(s.shape[0])
         w, _, ds, dt, _, _ = recs["xvector.dense.linear"]
-        self.dense = (_vec(w, device), _vec(ds, device), _vec(dt, device))
+        self.dense = (ops.to_device(w, device), ops.to_device(ds, device), ops.to_device(dt, device))
         self._ws_key, self._ws = None, None
         self.last_launches = 0
 

@@ -150,34 +150,18 @@ class ECAPA_TDNN(TopVirtualNnet):
         return NativeEcapaExtractor(self, dev)
 
 
-class _Layer:
-    """Device-side packed parameters of one TDNN / 1x1-conv layer record of _named_layers (name, weight (Cout, Cin, tot),
-    bias, context, scale, shift, relu).  groups > 1: a grouped 1x1 conv with its weight as stored, (Cout, Cin/groups, 1),
-    packed compactly for the layer kernel's grouped mode, or as its block-diagonal expansion when the shape does not fit
-    that mode (ops.tdnn_grouped_fits)."""
+class _Layer(ops.PackedAffine):
+    """One TDNN / 1x1-conv layer record of _named_layers (name, weight (Cout, Cin, tot), bias, context, scale, shift, relu)
+    as an ops.PackedAffine, groups > 1 for a grouped 1x1 conv, with each launch marked for the profile.  Ungrouped
+    one-tap layers keep the (N, K) fp32 matrix too: the segment-level ones run on CUDA cores (ops.small_affine)."""
 
     def __init__(self, rec, device, groups=1):
         _, w, bias, context, scale, shift, relu = rec
-        w = torch.from_numpy(w).to(device).contiguous()
-        self.context = list(context)
-        self.groups = 1
-        if groups > 1:
-            if ops.tdnn_grouped_fits(w.shape[1] * groups, w.shape[0], groups):
-                self.groups = groups
-            else:
-                w = _block_diagonal(w, groups)
-        self.w = ops.pack_tdnn_weight(w, self.context)
-        self.cout = w.shape[0]
-        # one-tap layers keep the (N, K) fp32 matrix too: the segment-level ones run on CUDA cores (ops.small_affine)
-        self.w_f32 = w[:, :, 0].contiguous() if w.shape[2] == 1 and w.shape[1] % 4 == 0 else None
-        self.bias = torch.from_numpy(bias).to(device).contiguous() if bias is not None else None
-        self.relu = relu
-        self.scale = torch.from_numpy(scale).to(device) if scale is not None else None
-        self.shift = torch.from_numpy(shift).to(device) if shift is not None else None
+        super().__init__(w, device, context, bias, scale, shift, relu=relu, groups=groups)
+        self.w_f32 = ops.to_device(w[:, :, 0], device) if groups == 1 and w.shape[2] == 1 and w.shape[1] % 4 == 0 else None
 
     def run(self, x, **kw):
-        ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
-                           relu=self.relu, groups=self.groups, **kw)
+        super().run(x, **kw)
         _mark("gemm K={}x{} N={}".format(len(self.context), x.channels, self.cout))
 
     def run_rows(self, x, sigmoid=False):
@@ -187,13 +171,8 @@ class _Layer:
         return y
 
 
-def _block_diagonal(w, groups):
-    """(Cout, Cin/G, k) grouped weight -> (Cout, Cin, k) with group g's block at rows g*Cout/G, columns g*Cin/G (conv1d's rule)."""
-    co, ci = w.shape[0] // groups, w.shape[1]
-    dense = w.new_zeros(w.shape[0], ci * groups, w.shape[2])
-    for g in range(groups):
-        dense[g * co:(g + 1) * co, g * ci:(g + 1) * ci] = w[g * co:(g + 1) * co]
-    return dense
+# the block-diagonal expansion of a grouped weight, under the name the grouped-mode test imports
+_block_diagonal = ops.block_diagonal
 
 
 def _mqmha_attention(st):

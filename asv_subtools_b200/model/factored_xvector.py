@@ -8,7 +8,6 @@ fused multiply-add kernel with a constant gate, and layer10 pools over time in i
 import os
 import sys
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
@@ -51,20 +50,9 @@ class Xvector(TopVirtualNnet):
         return FtdnnExtractor(self, self.device_for_extraction())
 
 
-class _Affine:
-    def __init__(self, affine, device, bn=None, relu=False):
-        w = affine.weight.detach().float().to(device).contiguous()
-        self.context, self.cout = list(affine.context), w.shape[0]
-        self.w = ops.pack_tdnn_weight(w, self.context)
-        self.bias = affine.bias.detach().float().to(device).contiguous() if affine.bias is not None else None
-        scale, shift = fold_batchnorm(bn)
-        self.scale = torch.from_numpy(scale).to(device) if scale is not None else None
-        self.shift = torch.from_numpy(shift).to(device) if shift is not None else None
-        self.relu = relu
-
-    def run(self, x, **kw):
-        ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
-                           relu=self.relu, **kw)
+def _affine(affine, device, bn=None, relu=False):
+    """A TdnnAffine with its weight as stored, [ReLU and] the eval BatchNorm bn folded in, as an ops.PackedAffine."""
+    return ops.PackedAffine(affine.weight, device, affine.context, affine.bias, *fold_batchnorm(bn), relu=relu)
 
 
 class FtdnnExtractor:
@@ -75,17 +63,17 @@ class FtdnnExtractor:
 
     def __init__(self, m, device):
         self.feat_dim, self.embed_dim = m.inputs_dim, m.embd_dim
-        self.l01 = _Affine(m.layer01.affine, device, m.layer01.batchnorm, m.layer01.relu)
+        self.l01 = _affine(m.layer01.affine, device, m.layer01.batchnorm, m.layer01.relu)
         self.blocks = {}
         for i in range(2, 10):
             blk = getattr(m, "layer{:02d}".format(i))
-            self.blocks[i] = (_Affine(blk.factor, device), _Affine(blk.affine, device, blk.bn, relu=True), blk.bypass_scale)
-        self.l10 = _Affine(m.layer10.affine, device, m.layer10.batchnorm, m.layer10.relu)
+            self.blocks[i] = (_affine(blk.factor, device), _affine(blk.affine, device, blk.bn, relu=True), blk.bypass_scale)
+        self.l10 = _affine(m.layer10.affine, device, m.layer10.batchnorm, m.layer10.relu)
         self.eps = m.stats.eps
         self.far = m.extracted_embedding == "far"
         e1 = m.embedding1
-        self.e1 = _Affine(e1.affine, device) if self.far else _Affine(e1.affine, device, e1.batchnorm, e1.relu)
-        self.e2 = None if self.far else _Affine(m.embedding2.affine, device)
+        self.e1 = _affine(e1.affine, device) if self.far else _affine(e1.affine, device, e1.batchnorm, e1.relu)
+        self.e2 = None if self.far else _affine(m.embedding2.affine, device)
         self.last_launches = 0
 
     def _block(self, i, x, out, tmp256, tmpo, lens=None):

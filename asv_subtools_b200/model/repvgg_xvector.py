@@ -34,7 +34,7 @@ from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200.model.resnet_xvector import _assign, _segment_chain  # noqa: E402
 from asv_subtools_b200.native import NativeExtractor  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
-from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
+from asv_subtools_b200.nnet.framework import from_record  # noqa: E402
 
 _GROUPWISE_LAYERS = range(2, 27, 2)
 
@@ -346,7 +346,7 @@ class RepVGGExtractor:
                                     "k": cfg["ksize"], "taps": taps, "w": ops.pack_conv2d_weight(w.to(device).contiguous(), taps),
                                     "scale": torch.ones(w.shape[0], dtype=torch.float32, device=device),
                                     "shift": b.to(device)})
-        self.segment = [_PackedAffine.from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
+        self.segment = [from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
         self.eps = cfg["pooling_eps"]
         self.embed_dim = self.segment[-1].cout_real
 

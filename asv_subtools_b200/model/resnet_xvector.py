@@ -33,7 +33,7 @@ from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200.native import ShardExtractor, host_lengths  # noqa: E402
 from asv_subtools_b200.nnet import ReluBatchNormTdnnLayer, StatisticsPooling, TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
-from asv_subtools_b200.nnet.framework import _PackedAffine  # noqa: E402
+from asv_subtools_b200.nnet.framework import from_record  # noqa: E402
 
 
 def _assign(defaults, given):
@@ -297,7 +297,7 @@ class ResNetExtractor:
                     "ds": (conv(p + "downsample.0"), bn(p + "downsample.1")) if p + "downsample.0" in recs else None,
                     "se": _se_rows(*recs[p + "se.fc_1"][:2], *recs[p + "se.fc_2"][:2], device)
                     if p + "se.fc_1" in recs else None})
-        self.segment = [_PackedAffine.from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
+        self.segment = [from_record(*recs[name], device) for name in ("fc1", "fc2") if name in recs]
         self.eps = cfg["pooling_eps"]
         self.embed_dim = self.segment[-1].cout_real
 

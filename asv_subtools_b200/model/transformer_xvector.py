@@ -404,25 +404,12 @@ def softmax_plus_multiplier(frames, train_len):
     return float(torch.log(l) / train_len.detach().float().cpu() * mask + 1 - mask)
 
 
-class _Lin:
-    """A Linear / kernel-size-1 conv record (name, w (Cout, Cin), bias, scale, shift, flags, ...) packed for the wgmma layer
-    kernel: y = epi(W x + b) with the record's ReLU or swish, and its folded BatchNorm (or constant scale) as the
-    epilogue's scale / shift."""
-
-    def __init__(self, rec, device):
-        w, b, scale, shift, flags = rec[1:6]
-        self.cout, self.cin = w.shape
-        self.w = ops.pack_tdnn_weight(_vec(w, device).unsqueeze(-1).contiguous(), [0])
-        self.bias, self.scale, self.shift = _vec(b, device), _vec(scale, device), _vec(shift, device)
-        self.relu, self.swish = bool(flags & RELU), bool(flags & SWISH)
-
-    def run(self, x, y=None, y_f32=None):
-        ops.tdnn_affine_ex(x, self.w, self.cout, [0], bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
-                           relu=self.relu, swish=self.swish, y=y, y_f32=y_f32)
-
-
-def _vec(a, device):
-    return torch.from_numpy(a).to(device).contiguous() if a is not None else None
+def _lin(rec, device):
+    """A Linear / kernel-size-1 conv record (name, w (Cout, Cin), bias, scale, shift, flags, ...) as an ops.PackedAffine:
+    y = epi(W x + b) with the record's ReLU or swish, and its folded BatchNorm (or constant scale) as the epilogue's
+    scale / shift."""
+    w, b, scale, shift, flags = rec[1:6]
+    return ops.PackedAffine(w, device, bias=b, scale=scale, shift=shift, relu=bool(flags & RELU), swish=bool(flags & SWISH))
 
 
 class ConformerExtractor:
@@ -433,11 +420,11 @@ class ConformerExtractor:
     def __init__(self, m, device):
         recs = {r[0]: r for r in native_records(m)}
         cfg = native_config(m)
-        lin = lambda name: _Lin(recs[name], device)  # noqa: E731
-        norm = lambda name: (_vec(recs[name][3], device), _vec(recs[name][4], device))  # noqa: E731
+        lin = lambda name: _lin(recs[name], device)  # noqa: E731
+        norm = lambda name: (ops.to_device(recs[name][3], device), ops.to_device(recs[name][4], device))  # noqa: E731
 
         def tdnn(name):
-            """(_Lin with the record's activation [and folded BatchNorm], LayerNorm (gamma, beta) or None)."""
+            """(_lin with the record's activation [and folded BatchNorm], LayerNorm (gamma, beta) or None)."""
             return lin(name + ".affine"), norm(name + ".batchnorm") if name + ".batchnorm" in recs else None
 
         self.device, self.feat_dim = device, cfg["feat_dim"]
@@ -449,11 +436,11 @@ class ConformerExtractor:
         self.act = cfg["act"]
         self.subsampling = cfg["subsampling"]
         e = "transformer.embed."
-        self.head_w = _vec(recs[e + "conv.0"][1].reshape(self.D, 1, 3, 3), device)
-        self.head_b = _vec(recs[e + "conv.0"][2], device)
-        self.conv2_w = ops.pack_conv2d_weight(_vec(recs[e + "conv.2"][1].reshape(self.D, self.D, 3, 3), device))
+        self.head_w = ops.to_device(recs[e + "conv.0"][1].reshape(self.D, 1, 3, 3), device)
+        self.head_b = ops.to_device(recs[e + "conv.0"][2], device)
+        self.conv2_w = ops.pack_conv2d_weight(ops.to_device(recs[e + "conv.2"][1].reshape(self.D, self.D, 3, 3), device))
         self.conv2_scale = torch.ones(self.D, dtype=torch.float32, device=device)
-        self.conv2_shift = _vec(recs[e + "conv.2"][2], device)
+        self.conv2_shift = ops.to_device(recs[e + "conv.2"][2], device)
         self.embed_out = lin(e + "out.0")
         self.layers = []
         for i in range(cfg["blocks"]):
@@ -465,8 +452,8 @@ class ConformerExtractor:
                  "out": lin(q + "self_attn.linear_out"),
                  "pw1": lin(cm + "pointwise_conv1"),
                  "pw2": lin(cm + "pointwise_conv2"),
-                 "dw_w": _vec(recs[cm + "depthwise_conv"][1], device),
-                 "dw_b": _vec(recs[cm + "depthwise_conv"][2], device),
+                 "dw_w": ops.to_device(recs[cm + "depthwise_conv"][1], device),
+                 "dw_b": ops.to_device(recs[cm + "depthwise_conv"][2], device),
                  "cm_norm": norm(cm + "norm") + (bool(recs[cm + "norm"][5] & BN),),
                  "att_norm": recs[q + "self_attn.att_norm"][1][0] if self.softmax_plus else None}
             for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
@@ -489,7 +476,7 @@ class ConformerExtractor:
         if t not in self._tables:
             if t >= TABLE_ROWS:
                 raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' {}".format(t, TABLE_ROWS))
-            table = _vec(self._pos_table[:t], self.device) if self._pos_table is not None else None
+            table = ops.to_device(self._pos_table[:t], self.device) if self._pos_table is not None else None
             rope, absp = (table, None) if self.pos == "rot_pos" else (None, table)
             mults = [float(L["att_norm"][t]) if self.softmax_plus else 1.0 for L in self.layers]
             self._tables[t] = (rope, absp, mults)

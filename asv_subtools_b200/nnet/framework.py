@@ -209,57 +209,26 @@ def build_tdnn_extractor(model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, e
     return ex
 
 
-class _PackedAffine:
-    """One TdnnAffine (+ optional ReLU / folded eval-BatchNorm) packed for the wgmma layer kernel on `device`:
-    block-diagonal expansion for groups > 1, output rows zero-padded to a multiple of `pad_to`, `row_scale` folded into
-    weight and bias (per-head temperature of the attention logits)."""
+def from_layer(layer, device):
+    """A whole ReluBatchNormTdnnLayer as an ops.PackedAffine with its output rows padded to a multiple of 8 (its
+    `export()` folds the BatchNorm in for the "bn-relu" order)."""
+    from .. import ops
+    w, b, scale, shift, relu = layer.export()
+    return ops.PackedAffine(w, device, layer.affine.context, b, scale, shift, relu=relu, pad_to=8)
 
-    @classmethod
-    def from_layer(cls, layer, device):
-        """A whole ReluBatchNormTdnnLayer (its `export()` folds the BatchNorm in for the "bn-relu" order)."""
-        w, b, scale, shift, relu = layer.export()
-        return cls(layer.affine, device, relu=relu, arrays=(w, b, scale, shift))
 
-    @classmethod
-    def from_record(cls, w, b, scale, shift, relu, device):
-        """A segment-layer record: w (Cout, Cin) and b, scale, shift (or None) as fp32 ndarrays, at context [0]."""
-        b = torch.from_numpy(b) if b is not None else None
-        return cls(None, device, relu=relu, arrays=(torch.from_numpy(w)[:, :, None], b, scale, shift))
+def from_affine(affine, device, relu=False, row_scale=None):
+    """A TdnnAffine alone (grouped weights expanded block-diagonally) as an ops.PackedAffine, rows padded to a multiple of 8."""
+    from .. import ops
+    return ops.PackedAffine(affine.dense_weight(), device, affine.context, affine.bias, relu=relu, pad_to=8,
+                            row_scale=row_scale)
 
-    def __init__(self, affine, device, bn=None, relu=False, pad_to=8, row_scale=None, arrays=None):
-        from .. import ops
-        from .components import fold_batchnorm
-        w = (arrays[0] if arrays is not None else affine.dense_weight()).to(device)
-        b = arrays[1] if arrays is not None else (affine.bias.detach().float() if affine.bias is not None else None)
-        b = b.to(device) if b is not None else None
-        if row_scale is not None:
-            w = w * row_scale.to(device).view(-1, 1, 1)
-            b = b * row_scale.to(device) if b is not None else None
-        self.cout_real = w.shape[0]
-        pad = (-w.shape[0]) % pad_to
-        if pad:
-            w = torch.cat([w, torch.zeros(pad, w.shape[1], w.shape[2], device=device)], 0)
-            b = torch.cat([b, torch.zeros(pad, device=device)], 0) if b is not None else None
-        self.context, self.cout = list(affine.context) if affine is not None else [0], w.shape[0]
-        self.w = ops.pack_tdnn_weight(w.contiguous(), self.context)
-        self.bias = b.contiguous() if b is not None else None
-        scale, shift = (arrays[2], arrays[3]) if arrays is not None else fold_batchnorm(bn)
-        if scale is not None and pad:                            # padded output channels come out as exact zeros
-            scale, shift = np.concatenate([scale, np.zeros(pad, np.float32)]), np.concatenate([shift, np.zeros(pad, np.float32)])
-        self.scale = torch.from_numpy(scale).to(device) if scale is not None else None
-        self.shift = torch.from_numpy(shift).to(device) if shift is not None else None
-        self.relu = relu
 
-    def run(self, x, **kw):
-        from .. import ops
-        ops.tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
-                           relu=self.relu, **kw)
-
-    def planes(self, b, t, device):
-        """(buffer to write, view of the real channels for the next layer)."""
-        from .. import ops
-        y = ops.SplitPlanes.empty((b, t, self.cout), device)
-        return y, (y if self.cout == self.cout_real else y.slice(0, self.cout_real))
+def from_record(w, b, scale, shift, relu, device):
+    """A segment-layer record as an ops.PackedAffine, rows padded to a multiple of 8: w (Cout, Cin) and b, scale, shift (or
+    None) as fp32 ndarrays, at context [0]."""
+    from .. import ops
+    return ops.PackedAffine(w, device, bias=b, scale=scale, shift=shift, relu=relu, pad_to=8)
 
 
 class AttentionPoolingExtractor:
@@ -277,11 +246,11 @@ class AttentionPoolingExtractor:
     def __init__(self, model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, position):
         dev = model.device_for_extraction()
         self.feat_dim = inputs_dim
-        self.frames = [_PackedAffine.from_layer(l, dev) for l in frame_layers]
+        self.frames = [from_layer(l, dev) for l in frame_layers]
         self.lde = self.xi = None
         if hasattr(stats, "prior_logprec"):                      # xi-vector: precision network + prior element
-            self.first = _PackedAffine.from_layer(stats.lin1_relu_bn, dev)
-            self.last = _PackedAffine(stats.lin2, dev)
+            self.first = from_layer(stats.lin1_relu_bn, dev)
+            self.last = from_affine(stats.lin2, dev)
             self.xi = (stats.prior_logprec.detach().float().reshape(-1).to(dev).contiguous(),
                        stats.prior_mean.detach().float().reshape(-1).to(dev).contiguous(), bool(stats.stddev))
             self.channels, self.pooled, self.gdiv = stats.input_dim, stats.input_dim, 1
@@ -295,25 +264,25 @@ class AttentionPoolingExtractor:
             self._segments(dev, tdnn6, tdnn7, position)
             return
         att = stats.attention
-        self.first = _PackedAffine(att.first_affine, dev, relu=True) if att.relu_affine else None
+        self.first = from_affine(att.first_affine, dev, relu=True) if att.relu_affine else None
         temps = att.head_temperatures()
         row_scale = None
         if temps is not None:                                    # logits of head h are divided by t_h (pooling.py:314-316)
             row_scale = (1.0 / temps).repeat_interleave(att.final_dim)
-        self.last = _PackedAffine(att.last_affine, dev, row_scale=row_scale)
+        self.last = from_affine(att.last_affine, dev, row_scale=row_scale)
         self.channels, self.pooled, self.gdiv = stats.input_dim, stats.pooled_channels(), stats.logit_divisor()
         self.eps, self.unweighted = stats.eps, not stats.stddev_attention
         self._segments(dev, tdnn6, tdnn7, position)
 
     def _segments(self, dev, tdnn6, tdnn7, position):
         if position == "far":
-            self.segment = [_PackedAffine(tdnn6.affine, dev)]
+            self.segment = [from_affine(tdnn6.affine, dev)]
         else:
-            self.segment = [_PackedAffine.from_layer(tdnn6, dev)]
+            self.segment = [from_layer(tdnn6, dev)]
             if position == "near_full":
-                self.segment.append(_PackedAffine.from_layer(tdnn7, dev))
+                self.segment.append(from_layer(tdnn7, dev))
             else:
-                self.segment.append(_PackedAffine(tdnn7.affine, dev))
+                self.segment.append(from_affine(tdnn7.affine, dev))
         self.embed_dim = self.segment[-1].cout_real
         self.last_launches = 0
 

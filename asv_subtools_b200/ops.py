@@ -185,6 +185,70 @@ def tdnn_affine_ex(x, w, cout, context, x2=None, bias=None, bn_scale=None, bn_sh
     check(lib.xvb_tdnn_affine_ex(C.byref(a), _stream()), "xvb_tdnn_affine_ex")
 
 
+def to_device(a, device):
+    """An array (ndarray or tensor) as a contiguous fp32 tensor on `device`; None stays None."""
+    return None if a is None else torch.as_tensor(a).detach().float().to(device).contiguous()
+
+
+def block_diagonal(w, groups):
+    """(Cout, Cin/G, k) grouped weight -> (Cout, Cin, k) with group g's block at rows g*Cout/G, columns g*Cin/G (conv1d's rule)."""
+    co, ci = w.shape[0] // groups, w.shape[1]
+    dense = w.new_zeros(w.shape[0], ci * groups, w.shape[2])
+    for g in range(groups):
+        dense[g * co:(g + 1) * co, g * ci:(g + 1) * ci] = w[g * co:(g + 1) * co]
+    return dense
+
+
+class PackedAffine:
+    """One affine layer packed on `device` for the wgmma layer kernel (tdnn_affine_ex): weight w (Cout, Cin, tot) over
+    `context`, or (Cout, Cin) at one tap, with its bias, its folded eval BatchNorm (scale, shift) and ReLU / swish as the
+    epilogue.  A weight whose kernel axis holds only the listed taps of a dilated context is spread over the span, the
+    gaps as zero taps.  groups > 1: a grouped 1x1 conv with its weight as stored, (Cout, Cin/groups, 1), packed compactly
+    for the grouped mode, or as its block-diagonal expansion when the shape does not fit that mode (tdnn_grouped_fits).
+    row_scale: a per-output factor folded into weight and bias.  pad_to: output rows zero-padded to a multiple of it, the
+    padded outputs exact zeros; the first cout_real rows are the layer's own."""
+
+    def __init__(self, w, device, context=(0,), bias=None, scale=None, shift=None, relu=False, swish=False, groups=1,
+                 pad_to=1, row_scale=None):
+        w = to_device(w, device)
+        w = w.reshape(w.shape[0], w.shape[1], -1)
+        self.context = list(context)
+        left, _, tot = context_span(self.context)
+        if w.shape[2] != tot:
+            full = w.new_zeros(w.shape[0], w.shape[1], tot)
+            full[:, :, [c - left for c in self.context]] = w
+            w = full
+        self.groups = 1
+        if groups > 1:
+            if tdnn_grouped_fits(w.shape[1] * groups, w.shape[0], groups):
+                self.groups = groups
+            else:
+                w = block_diagonal(w, groups)
+        bias, scale, shift = (to_device(v, device) for v in (bias, scale, shift))
+        if row_scale is not None:
+            row_scale = to_device(row_scale, device)
+            w = w * row_scale.view(-1, 1, 1)
+            bias = bias * row_scale if bias is not None else None
+        self.cout_real = w.shape[0]
+        pad = (-w.shape[0]) % pad_to
+        if pad:
+            w = torch.cat([w, w.new_zeros(pad, w.shape[1], w.shape[2])], 0)
+            bias, scale, shift = (torch.cat([v, v.new_zeros(pad)]) if v is not None else None for v in (bias, scale, shift))
+        self.cout = w.shape[0]
+        self.w = pack_tdnn_weight(w.contiguous(), self.context)
+        self.bias, self.scale, self.shift = bias, scale, shift
+        self.relu, self.swish = relu, swish
+
+    def run(self, x, **kw):
+        tdnn_affine_ex(x, self.w, self.cout, self.context, bias=self.bias, bn_scale=self.scale, bn_shift=self.shift,
+                       relu=self.relu, swish=self.swish, groups=self.groups, **kw)
+
+    def planes(self, b, t, device):
+        """(buffer to write, view of the real channels for the next layer)."""
+        y = SplitPlanes.empty((b, t, self.cout), device)
+        return y, (y if self.cout == self.cout_real else y.slice(0, self.cout_real))
+
+
 def plane_mean(x, planes=True, lengths=None, rows_per_length=1):
     """Mean over T of SplitPlanes (B,T,C) -> (fp32 (B,C), SplitPlanes (B,1,C) | None).  lengths: int32 CUDA (B,) tensor
     of a masked batch: utterance b averages its first lengths[b] * rows_per_length rows (xvb_plane_mean_lengths)."""

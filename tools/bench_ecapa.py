@@ -64,7 +64,7 @@ def main_mqmha(steps):
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
     import ecapa_mqmha_oracle as mo
     from asv_subtools_b200 import ops
-    from asv_subtools_b200.model.ecapa_tdnn_xvector import _block_diagonal, _mqmha_attention
+    from asv_subtools_b200.model.ecapa_tdnn_xvector import _mqmha_attention
     B, T, F = 128, 300, 80
     xs = [torch.randn(B, T, F, device="cuda") for _ in range(4)]
     base = ECAPA_TDNN(F, 10, **CANON)
@@ -88,7 +88,7 @@ def main_mqmha(steps):
         w = torch.from_numpy(w).cuda()
         cout = w.shape[0]
         y = torch.empty(B, T, cout, device="cuda")
-        wg, wd = ops.pack_tdnn_weight(w, [0]), ops.pack_tdnn_weight(_block_diagonal(w, g).contiguous(), [0])
+        wg, wd = ops.pack_tdnn_weight(w, [0]), ops.pack_tdnn_weight(ops.block_diagonal(w, g).contiguous(), [0])
         tg = _gemm_ms(lambda: ops.tdnn_affine_ex(src, wg, cout, [0], y_f32=y, groups=g))
         td = _gemm_ms(lambda: ops.tdnn_affine_ex(src, wd, cout, [0], y_f32=y))
         res[name + "_gemm_us"] = {"shape": "{}x{}->{} groups {}".format(B * T, src.channels, cout, g),
