@@ -11,11 +11,16 @@
 //   first attention conv -> attention conv 1 (ReLU, BN, tanh; time-constant columns as utt_bias) ->
 //   attention conv 2 -> online-softmax weighted moments -> fc2 (bn_stats folded in; own BN for "near").
 //
+// egrecho's EcapaXvector (subtools2/egrecho/models/ecapa/ecapa_xvector.py:420-427) chains its blocks instead
+// (xvb_ecapa_set_chained): block b + 1 reads block b's output straight from its slot of the MFA input, at row pitch
+// 3C, as the input of its first 1x1 layer and as its residual, and no running sum is written.
+//
 // Layers are handed over by NAME with the weights as the state_dict stores them (host fp32, eval BatchNorm
 // folded to scale/shift by the caller); the two derived layers of the attention conv ("att_x": its columns
 // over x, "att_gs": its columns over [mean | std] plus the bias) and "fc2" (bn_stats folded into its weight)
 // are prepared by the caller -- see the Python blueprint.  The handle keeps the layers as handed over and builds the
-// model from them at finalize; xvb_ecapa_save writes them back (the XVBE0001 / XVBE0002 layouts are in model_file.cpp).
+// model from them at finalize; xvb_ecapa_save writes them back (the XVBE0001 / XVBE0002 / XVBG0001 layouts are in
+// model_file.cpp).
 #include <cuda_runtime.h>
 #include <string.h>
 
@@ -58,6 +63,8 @@ struct Config {
   int feat_dim = 0, ldf = 0, C = 0, D = 0, H = 0, E = 0, scale = 8;
   // multi-query multi-head attention pooling (xvb_ecapa_set_mqmha); mq == 0: ECAPA's own attentive pooling
   int mq = 0, mq_heads = 1, mq_q = 1, mq_hidden = 0, mq_share = 0, mq_layers = 2, mq_tatt = 1, mq_stddev = 1;
+  // residual form (xvb_ecapa_set_chained): 0 dense, block b + 1 reads x + x1 (+ x2); 1 chained, it reads block b's output
+  int chained = 0;
   // widths derived from the pooling: att_x outputs AX, the logits NL (row pitch ldlog), the pooled statistics P of the
   // P2-wide [mean | std] buffer (default model: AX = H, NL = D, P = P2 = 2D)
   int AX = 0, NL = 0, ldlog = 0, P = 0, P2 = 0;
@@ -141,6 +148,13 @@ extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int 
                 "become a per-utterance bias, which needs a multiple of 4 outputs (got %d)", m->cfg.AX);
   m->cfg.P2 = 2 * num_q * m->cfg.D;
   m->cfg.P = stddev ? m->cfg.P2 : num_q * m->cfg.D;
+  return XVB_OK;
+}
+
+extern "C" int xvb_ecapa_set_chained(xvb_ecapa_t* h, int chained) {
+  XVB_CHECK_ARG(is_draft(h) && h->draft->recs.empty(), "xvb_ecapa_set_chained: call it between xvb_ecapa_create and the first set_layer");
+  XVB_CHECK_ARG(chained == 0 || chained == 1, "xvb_ecapa_set_chained: chained must be 0 or 1, got %d", chained);
+  h->draft->cfg.chained = chained;
   return XVB_OK;
 }
 
@@ -388,12 +402,13 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
         (rc = small_layer(&k.se1, h->zmean, C, B, h->s1f, m->se_dim, 0, stream)) ||
         (rc = small_layer(&k.se2, h->s1f, m->se_dim, B, h->gate, C, XVB_SIGMOID, stream)))
       return rc;
-    const bool last = b == 2;
+    // dense: the running sum x + x1 (+ x2) goes to N for the next block; chained: the next block reads this slot
+    const bool next = b < 2 && !m->cfg.chained;
     const View slot = h->CAT.slice(C * b);
     if ((rc = xvb_se_apply(h->Z.hi, h->Z.lo, C, cur.hi, cur.lo, cur.ld, h->gate, slot.hi, slot.lo, slot.ld,
-                           last ? nullptr : h->N.hi, last ? nullptr : h->N.lo, C, B, T, C, stream)))
+                           next ? h->N.hi : nullptr, next ? h->N.lo : nullptr, C, B, T, C, stream)))
       return rc;
-    cur = h->N;
+    cur = m->cfg.chained ? slot : h->N;
   }
   a = layer_args(m->mfa, h->CAT, B, T, h->M, h->MF, D);
   if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
@@ -450,12 +465,14 @@ extern "C" int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_h
 extern "C" int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path) {
   XVB_CHECK_ARG(finalized(h) && path, "xvb_ecapa_save: model not finalized");
   const Config& c = h->m->cfg;
-  const int32_t head[13] = {c.feat_dim, c.C, c.D, c.H, c.E, (int32_t)h->m->recs.size(),   // then XVBE0002's pooling
-                            c.mq_heads, c.mq_q, c.mq_hidden, c.mq_share, c.mq_layers, c.mq_tatt, c.mq_stddev};
+  XVB_CHECK_ARG(c.mq || !c.chained, "xvb_ecapa_save: an XVBG0001 file holds a chained model with MQMHA pooling");
+  const int32_t head[14] = {c.feat_dim, c.C, c.D, c.H, c.E, (int32_t)h->m->recs.size(),   // then XVBE0002's pooling
+                            c.mq_heads, c.mq_q, c.mq_hidden, c.mq_share, c.mq_layers, c.mq_tatt, c.mq_stddev,
+                            c.chained};                                                   // then XVBG0001's residual form
   std::vector<const TapRec*> layers;
   for (const TapRec& r : h->m->recs) layers.push_back(&r);
-  return save_tap_file("xvb_ecapa_save", path, c.mq ? "XVBE0002" : "XVBE0001", head, (c.mq ? 13 : 6) * sizeof(int32_t),
-                       layers, true);
+  const char* magic = c.chained ? "XVBG0001" : c.mq ? "XVBE0002" : "XVBE0001";
+  return save_tap_file("xvb_ecapa_save", path, magic, head, (c.chained ? 14 : c.mq ? 13 : 6) * sizeof(int32_t), layers, true);
 }
 
 extern "C" void xvb_ecapa_destroy(xvb_ecapa_t* h) { delete h; }

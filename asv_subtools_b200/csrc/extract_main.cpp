@@ -15,7 +15,8 @@
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
 // the input side.  The model file is any of the six families, told apart by its magic: TDNN x-vector
-// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling),
+// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling, or XVBG0001 for
+// egrecho's EcapaXvector with chained blocks),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), each written by its native extractor's save() (model_file.cpp).  What it adds:
 // utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector and ResNet
@@ -24,7 +25,7 @@
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
-//   * a CAM++ model keeps egrecho's rule instead (CamPPModel.extract_embedding, XvectorMixin.split_chunks with
+//   * a CAM++ or egrecho ECAPA (XVBG0001) model keeps egrecho's rule instead (CamPPModel.extract_embedding, XvectorMixin.split_chunks with
 //     even=False, xvb_campp_chunk_sizes): max-chunk-long chunks, the last two re-split evenly (9000 -> 4000, 2500,
 //     2500); its default max-chunk is 4000;
 //   * one "FV" vector per input key (order follows batch completion, which the wspecifier allows);
@@ -77,7 +78,7 @@ struct Family {
   int (*extract)(void* h, const float* feats, int B, int T, float* emb);
   void (*destroy)(void* h);
   int max_chunk;
-  bool campp_chunks;       // egrecho's split_chunks(even=False) through xvb_campp_chunk_sizes
+  bool egrecho_chunks;     // egrecho's split_chunks(even=False) through xvb_campp_chunk_sizes
   // masked batch of different lengths (host lengths), or nullptr: the family batches equal lengths only
   int (*extract_lengths)(void* h, const float* feats, const int32_t* lengths, int B, int T, float* emb);
 };
@@ -99,6 +100,7 @@ const Family kFamilies[] = {
     {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false, nullptr},
     {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false, nullptr},
     {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true, nullptr},
+    {{"XVBG0001", nullptr}, "loading the egrecho ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 4000, true, nullptr},
     // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
     {{nullptr, nullptr}, "loading the model", "xvb_extractor_extract",
      [](void** h, const char* path) { return xvb_extractor_load((xvb_extractor_t**)h, path); },
@@ -307,12 +309,13 @@ int main(int argc, char** argv) {
              "                   [--mixed-lengths] [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), 2-D ResNet x-vector (XVBR0001),\n"
-             "RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001) or CAM++ x-vector (XVBP0001) model,\n"
-             "recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the model's own chunk rule),\n"
-             "4000 for CAM++ and 10000 otherwise.  A Conformer chunk needs at least 7 frames and fewer than 5000 subsampled\n"
-             "frames.  CAM++ cuts an utterance with egrecho's rule (max-chunk-long chunks, the last two re-split evenly:\n"
-             "9000 -> 4000, 2500, 2500); a chunk needs at least 3 frames.\n"
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), egrecho ECAPA-TDNN (XVBG0001),\n"
+             "2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001) or CAM++\n"
+             "x-vector (XVBP0001) model, recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the\n"
+             "model's own chunk rule), 4000 for CAM++ and egrecho ECAPA-TDNN and 10000 otherwise.  A Conformer chunk needs at\n"
+             "least 7 frames and fewer than 5000 subsampled frames.  CAM++ and egrecho ECAPA-TDNN cut an utterance with\n"
+             "egrecho's rule (max-chunk-long chunks, the last two re-split evenly: 9000 -> 4000, 2500, 2500); a CAM++ chunk\n"
+             "needs at least 3 frames.\n"
              "--mixed-lengths (TDNN x-vector and ResNet x-vector models): after the chunk rule, chunks of different\n"
              "lengths share batches of up to --batch, taken in ascending length, with at most 1/8 of a batch's frames\n"
              "padding; the summary line also reports the padded frames.  Vectors differ from the default mode's at the\n"
@@ -431,10 +434,10 @@ int main(int argc, char** argv) {
     u.key = key;
     u.frames = rows;
     std::vector<int> lens;
-    if (r.fam->campp_chunks) {   // egrecho's split_chunks(even=False)
+    if (r.fam->egrecho_chunks) {   // egrecho's split_chunks(even=False)
       lens.resize((size_t)rows / max_chunk + 1);
       const int n = xvb_campp_chunk_sizes(rows, max_chunk, lens.data(), (int)lens.size());
-      if (n < 1) die("planning the CAM++ chunks");
+      if (n < 1) die("planning the egrecho chunks");
       lens.resize(n);
     } else {
       const int num_split = (rows + max_chunk - 1) / max_chunk, split = rows / num_split;

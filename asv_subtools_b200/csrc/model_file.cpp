@@ -13,6 +13,8 @@
 //              | per layer: i32 name_len | name (no NUL) | tap record
 //   "XVBE0002" (ECAPA-TDNN with MQMHA pooling): the same with the pooling record {num_head, num_q, hidden, share,
 //              affine_layers, time_attention, stddev} after the dims; grouped convs stored as the state_dict holds them.
+//   "XVBG0001" (egrecho's ECAPA-TDNN, chained blocks): the XVBE0002 header with i32 residual_form (1: chained,
+//              xvb_ecapa_set_chained) after the pooling record, then the named tap records.
 //
 // The named-record files of the native ResNet, RepVGG, Conformer and CAM++ extractors (save_records / load_records
 // below) and the record store behind them (records.h).
@@ -298,15 +300,18 @@ extern "C" int xvb_ecapa_load(xvb_ecapa_t** out, const char* path) {
   xvb_ecapa_t* h = nullptr;
   int rc = XVB_EINVAL;
   do {
-    int32_t pr[7];
-    const bool ok_magic = rd(f, magic, 8) && (memcmp(magic, "XVBE0001", 8) == 0 || memcmp(magic, "XVBE0002", 8) == 0);
-    const bool mq = ok_magic && magic[7] == '2';
-    if (!ok_magic || !rd(f, hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(f, pr, sizeof pr))) {
-      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 file", path);
+    int32_t pr[8];   // the pooling record, then XVBG0001's residual form
+    const bool got = rd(f, magic, 8);
+    const bool g = got && memcmp(magic, "XVBG0001", 8) == 0;
+    const bool mq = g || (got && memcmp(magic, "XVBE0002", 8) == 0);
+    const bool ok_magic = mq || (got && memcmp(magic, "XVBE0001", 8) == 0);
+    if (!ok_magic || !rd(f, hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(f, pr, (g ? 8 : 7) * sizeof(int32_t)))) {
+      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 / XVBG0001 file", path);
       break;
     }
     if ((rc = xvb_ecapa_create(&h, hd[0], hd[1], hd[2], hd[3], hd[4]))) break;
     if (mq && (rc = xvb_ecapa_set_mqmha(h, pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]))) break;
+    if (g && (rc = xvb_ecapa_set_chained(h, pr[7]))) break;
     xvb::TapRec r;
     for (int i = 0; i < hd[5] && rc == XVB_OK; ++i) {
       int32_t nl = 0;

@@ -149,6 +149,13 @@ class ECAPA_TDNN(TopVirtualNnet):
             return EcapaExtractor(self, dev)       # op-by-op twin; also the path for other channel counts
         return NativeEcapaExtractor(self, dev)
 
+    # the records and configuration the extractors below take (egrecho_ecapa_xvector.EcapaXvector has its own)
+    def native_records(self):
+        return _named_layers(self)
+
+    def native_config(self):
+        return native_config(self)
+
 
 class _Layer(ops.PackedAffine):
     """One TDNN / 1x1-conv layer record of _named_layers (name, weight (Cout, Cin, tot), bias, context, scale, shift, relu)
@@ -179,14 +186,17 @@ def _mqmha_attention(st):
     """The MQMHASP attention as extractor records (name, weight, bias, bn (scale, shift) | None, relu, groups):
     "att_x" = the first conv's x columns as stored (per head [x_h | mean_h | std_h], pooling.py:636-648), "att_gs" = its
     [mean_h | std_h] columns as ONE block-diagonal (Cout, 2C) matrix over the utterance's [mean | std] plus the conv's bias
-    (time attention only: the time-constant part becomes a per-utterance bias), "att2" = the second conv."""
+    (time attention only: the time-constant part becomes a per-utterance bias), "att2" = the second conv.  The first
+    conv is att[0], or `attention` itself where one affine layer is a bare conv (egrecho's MQMHASP); without a
+    BatchNorm in the attention (egrecho's norm_type="") att_x has none."""
     f = lambda t: t.detach().float().cpu().numpy()  # noqa: E731
     att, H, cg = st.attention, st.num_head, st.head_width()
-    w0, b0 = f(att[0].weight), f(att[0].bias)
+    first = att[0] if isinstance(att, nn.Sequential) else att
+    w0, b0 = f(first.weight), f(first.bias)
     cout = w0.shape[0]
     xcols = np.ascontiguousarray(w0[:, :cg])
     two = st.affine_layers == 2
-    bn = fold_batchnorm(att[2]) if two else None
+    bn = fold_batchnorm(att[2]) if two and isinstance(att[2], nn.BatchNorm1d) else None
     out = [("att_x", xcols, None if st.time_attention else b0, bn, two, H)]
     if st.time_attention:
         ns = 2 if st.stddev else 1
@@ -275,32 +285,36 @@ def _segment_layers(m):
 
 def native_config(m):
     """{"create": the arguments of xvb_ecapa_create after the handle, "mqmha": those of xvb_ecapa_set_mqmha, or None for
-    the attentive pooling} for model m."""
+    the attentive pooling, "chained": False (dense blocks, xvb_ecapa_set_chained)} for model m."""
     st = m.stats
     mq = isinstance(st, MQMHASP)
     hidden = st.hidden_size * st.num_head * st.num_q if mq else st.attention[0].out_channels
     return {"create": (m.inputs_dim, m.layer1.affine.output_dim, st.in_dim, hidden, m.embd_dim),
             "mqmha": (st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers, int(st.time_attention),
-                      int(st.stddev)) if mq else None}
+                      int(st.stddev)) if mq else None,
+            "chained": False}
 
 
 class NativeEcapaExtractor(ShardExtractor):
     """xvb_ecapa_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
-    current when it is built (or loaded from an XVBE0001 / XVBE0002 file)."""
+    current when it is built (or loaded from an XVBE0001 / XVBE0002 / XVBG0001 file), from the model's native_records()
+    and native_config()."""
 
     PREFIX = "ecapa"
 
     def _create_args(self, m):
-        return native_config(m)["create"]
+        return m.native_config()["create"]
 
     def _configure(self, m):
-        mq = native_config(m)["mqmha"]
-        if mq is not None:
-            self._call("set_mqmha", self._h, *mq)
+        cfg = m.native_config()
+        if cfg["mqmha"] is not None:
+            self._call("set_mqmha", self._h, *cfg["mqmha"])
+        if cfg["chained"]:
+            self._call("set_chained", self._h, 1)
 
     def _layers(self, m):
         from asv_subtools_b200._lib import int_array
-        for name, w, b, ctx, scale, shift, relu in _named_layers(m):
+        for name, w, b, ctx, scale, shift, relu in m.native_records():
             w = np.asarray(w, dtype=np.float32)
             w3 = w.reshape(w.shape[0], w.shape[1], -1)
             yield name, (w3.shape[0], w3.shape[1], int_array(ctx), len(ctx)), (w3, b, scale, shift), \
@@ -311,15 +325,16 @@ class EcapaExtractor:
     """Packed weights on one device + the launch sequence of ECAPA_TDNN.extract_embedding (:403-426), driven from
     Python op by op: the A/B and profiling twin of NativeEcapaExtractor (XVB_ECAPA_NATIVE=0, tools/bench_ecapa.py
     --profile), and the path for channel counts the handle does not take.  The weights are the records and configuration
-    the handle takes (_named_layers, native_config); the Res2Net stack, its dilation, scale and width come from the
+    the handle takes (the model's native_records and native_config); the Res2Net stack, its dilation, scale and width come from the
     layerN.resI records, and the MQMHA attention convs are grouped by the handle's rule (att_x: heads, att2: heads x
     queries)."""
 
     def __init__(self, m, device):
-        recs = {r[0]: r for r in _named_layers(m)}
-        cfg = native_config(m)
+        recs = {r[0]: r for r in m.native_records()}
+        cfg = m.native_config()
         self.device = device
         self.feat_dim, self.channels, self.mfa_dim, _, self.embed_dim = cfg["create"]
+        self.chained = cfg["chained"]
         self.ldf = (self.feat_dim + 7) // 8 * 8
         self.last_launches = 0
         mq = cfg["mqmha"]
@@ -388,10 +403,12 @@ class EcapaExtractor:
             zmean, _ = ops.plane_mean(Z, planes=False)
             _mark("plane_mean")
             gate = blk["se2"].run_rows(blk["se1"].run_rows(zmean), sigmoid=True)
-            last = li + 1 == len(self.blocks)
-            ops.se_apply(Z, cur, gate.view(B, C), CAT.slice(C * li, C * (li + 1)), None if last else N)
+            # dense: the running sum x + x1 (+ x2) into N for the next block; chained: the next block reads this slot
+            slot = CAT.slice(C * li, C * (li + 1))
+            nxt = li + 1 < len(self.blocks) and not self.chained
+            ops.se_apply(Z, cur, gate.view(B, C), slot, N if nxt else None)
             _mark("se_apply")
-            cur = N
+            cur = slot if self.chained else N
         D = self.mfa_dim
         M = P.empty((B, T, D), dev)
         MF = torch.empty(B, T, D, dtype=torch.float32, device=dev)

@@ -758,6 +758,10 @@ int xvb_ecapa_create(xvb_ecapa_t** out, int feat_dim, int channels, int mfa_dim,
  * the 2 * num_q * mfa_dim pooled statistics (num_q * mfa_dim without stddev). */
 int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int share, int affine_layers, int time_attention,
                         int stddev);
+/* Residual form of the three SE-Res2Net blocks: 0 (the default) is ECAPA_TDNN's dense form, block 2 reading x + x1 and
+ * block 3 x + x1 + x2; 1 is egrecho's EcapaXvector (subtools2/egrecho/models/ecapa/ecapa_xvector.py:420-427), each block
+ * reading the previous block's output.  Call between create and the first set_layer; the layers are the same. */
+int xvb_ecapa_set_chained(xvb_ecapa_t* h, int chained);
 int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
                         const float* w_host, const float* bias_host, const float* bn_scale_host,
                         const float* bn_shift_host, int flags);
@@ -778,7 +782,8 @@ int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_host, int64_
                                  void* stream);
 int xvb_ecapa_last_launches(const xvb_ecapa_t* h);
 /* "XVBE0001" model files: the named layers as handed to xvb_ecapa_set_layer; "XVBE0002" for MQMHA models adds the
- * xvb_ecapa_set_mqmha record.  Both load. */
+ * xvb_ecapa_set_mqmha record; "XVBG0001" for chained models (egrecho's, MQMHA pooling only) adds the residual form
+ * after it.  All three load. */
 int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path);
 int xvb_ecapa_load(xvb_ecapa_t** out, const char* path);
 void xvb_ecapa_destroy(xvb_ecapa_t* h);

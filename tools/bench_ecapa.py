@@ -7,7 +7,12 @@ c1024 line.  XVB_ECAPA_NATIVE=0 / XVB_ECAPA_RES2NET=gemm select the twin / its p
 
 --pooling mqmha: the roadmap launcher's model (runEcapaXvector_roadmap.py:220-250: MQMHASP 2 queries x 2 heads, hidden
 64, share=False, time attention) next to the attentive-pooling model in the same call, and CUDA-event times of its two
-attention GEMMs in the layer kernel's grouped mode against their block-diagonal expansions."""
+attention GEMMs in the layer kernel's grouped mode against their block-diagonal expansions.
+
+--egrecho [--channels 512|1024]: egrecho's EcapaXvector (EcapaConfig's pooling: one head, one query, hidden 128, time
+attention) at 128 x 300 on the native handle in its chained form, on its Python twin and as the torch fp32 restatement
+(tests/egrecho_ecapa_oracle.py, TF32 off), with the dense ECAPA_TDNN handle of the same width next to it; the four run in
+alternating rounds in one process, and each one's median round is reported."""
 import json
 import os
 import sys
@@ -96,6 +101,50 @@ def main_mqmha(steps):
     print(json.dumps(res))
 
 
+def main_egrecho(steps, channels, rounds=5):
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import egrecho_ecapa_oracle as eo
+    from asv_subtools_b200.model import ecapa_tdnn_xvector as etx
+    from asv_subtools_b200.model.egrecho_ecapa_xvector import EcapaXvector
+    B, T, F = 128, 300, 80
+    dev = torch.device("cuda")
+    xs = [torch.randn(B, T, F, device=dev) for _ in range(4)]
+    m = EcapaXvector(F, 10, channels=channels)
+    keys = ["{}:{}".format(k, ",".join(str(d) for d in v.shape)) for k, v in m.state_dict().items()]
+    sd = eo.seeded_state_dict(keys, 41)
+    m.load_state_dict(sd, strict=True)
+    m.to(dev).eval()
+    dense = ECAPA_TDNN(F, 10, **dict(CANON, ecapa_params=dict(CANON["ecapa_params"], channels=channels)))
+    dense.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F, channels=channels), 201), strict=True)
+    dense.to(dev).eval()
+    sd_dev = {k: v.to(dev) for k, v in sd.items()}
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+
+    class Torch:
+        def extract(self, x):
+            with torch.no_grad():
+                return eo.forward(sd_dev, x, {"inputs_dim": F, "channels": channels})[0]
+
+    runs = {"native": m.extractor(), "twin": etx.EcapaExtractor(m, dev), "torch_fp32": Torch(),
+            "ecapa_tdnn_dense_native": dense.extractor()}
+    times = {k: [] for k in runs}
+    for _ in range(rounds):
+        for name, ex in runs.items():
+            times[name].append(_rate(ex, xs, steps)[0])
+    x = xs[0]
+    nat, twin, ref = (runs[k].extract(x) for k in ("native", "twin", "torch_fp32"))
+    res = {"card": _card(), "workload": "egrecho EcapaXvector C{}, 80-d fbank, 300-frame chunks, batch 128".format(channels),
+           "native_equals_twin": bool(torch.equal(nat, twin)),
+           "native_vs_torch_rel": float((nat - ref).abs().max() / ref.abs().max()),
+           "launches": runs["native"].last_launches}
+    for name, v in times.items():
+        ms = sorted(v)[len(v) // 2]
+        res[name] = {"ms_per_batch": round(ms, 3), "frames_per_s": round(B * T / (ms * 1e-3)),
+                     "rounds_ms": [round(t, 3) for t in v]}
+    print(json.dumps(res))
+
+
 def macs_per_frame(C, F=80, D=1536, H=128):
     """Contraction MACs per frame from the shapes: layer1 (5 taps), per block bn1 + 7 Res2Net steps (3 taps, width C/8)
     + bn2, mfa, the two attention convs (the per-utterance SE and segment layers are left out)."""
@@ -111,6 +160,8 @@ def main():
     channels = int(sys.argv[sys.argv.index("--channels") + 1]) if "--channels" in sys.argv else 1024
     if channels not in (512, 1024):
         raise SystemExit("--channels takes 512 or 1024")
+    if "--egrecho" in sys.argv:
+        return main_egrecho(steps, channels)
     kw = dict(CANON, ecapa_params=dict(CANON["ecapa_params"], channels=channels))
     m = ECAPA_TDNN(F, 10, **kw)
     m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F, channels=channels), 201), strict=True)
