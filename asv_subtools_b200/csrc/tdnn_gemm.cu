@@ -46,8 +46,9 @@ constexpr int kProducerWarp = kNumConsumers / 32;
 constexpr int kSlabBytes = 16384;                // trial histogram: 2 x hist_bins u32 counters
 // Staged layer epilogue (outputs leave through shared memory and TMA stores): each consumer warpgroup owns one piece of
 // 64 rows x 64 channels x both planes, swizzled like the operand tiles, and the bias, scale and shift of its 64 columns.
-// The two ping-pong warpgroups can be in their epilogues at once, so they share nothing.  The histogram's slab is the
-// first 16 KB of the same region: no instance has both.
+// The two ping-pong warpgroups can be in their epilogues at once, so they share nothing.  The fused pooling epilogue
+// stages a tile's partials in the same 16 KB per warpgroup.  The histogram's slab is the first 16 KB of the region: no
+// instance has both.
 constexpr int kStagePlaneBytes = 64 * kBlockK * 2;
 constexpr int kStageOutBytes = 2 * kStagePlaneBytes;
 constexpr int kCoefBytes = 3 * kBlockK * 4;
@@ -122,11 +123,11 @@ template <int BLOCK_N, bool kPool, bool kHist>
 __host__ __device__ constexpr bool staged_epilogue() { return !kPool && !kHist && BLOCK_N % kBlockK == 0; }
 
 // One CTA per 128 x BLOCK_N tile; operand stages as deep as 192 KB of shared memory allows.  Behind them the staged
-// instances have the epilogue region; the others keep the 16 KB slab alone, and with it the shared memory they leave
-// to a kernel of another stream.
-template <int BLOCK_N, bool kStagedEpi>
+// layer and fused pooling instances have the epilogue region; the others keep the 16 KB slab alone, and with it the
+// shared memory they leave to a kernel of another stream.
+template <int BLOCK_N, bool kPool, bool kHist>
 struct GemmCfg {
-  static constexpr int kTailBytes = kStagedEpi ? kEpiBytes : kSlabBytes;
+  static constexpr int kTailBytes = (staged_epilogue<BLOCK_N, kPool, kHist>() || kPool) ? kEpiBytes : kSlabBytes;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;          // one plane of the weight tile
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
   static constexpr int kStages = (192 * 1024) / kStageBytes > 6 ? 6 : (192 * 1024) / kStageBytes;
@@ -139,7 +140,7 @@ struct GemmCfg {
 // kPool: fused statistics pooling.  The MMA operands swap roles -- the weight tile is the M side
 // (128 output channels = accumulator rows), the frame tile the N side (128 frames = accumulator
 // columns) -- so pooling over time becomes a reduction along a thread's own columns plus at most
-// two quad shuffles, with no shared memory and no (B,T,C) output at all.
+// two quad shuffles, with no (B,T,C) output at all.
 // Tile index -> (M unit, N block).  Layers: N fastest, so the CTAs running together share the frame
 // (A) tile and walk the small, L2-resident weight matrix.  Score matrices (kHist): both operands are
 // huge, so tiles are rastered in bands of `hist_group` M units x all N blocks, M fastest -- the CTAs in
@@ -210,7 +211,7 @@ __device__ __noinline__ void epi_zero_row(const TdnnGemmParams& p, long long gro
 // clock's rate.  Plain stores: a printf or any other call would serialise the MMAs (C7510).
 #ifdef XVB_TILE_TIMELINE
 #define XVB_TL(...) __VA_ARGS__
-constexpr int kTimelineHead = 8, kTimelineRec = 8;
+constexpr int kTimelineHead = 8, kTimelineRec = 12;
 static unsigned long long* g_timeline = nullptr;
 static int g_timeline_tiles = 0;
 static bool g_timeline_direct = false;
@@ -243,7 +244,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                         const __grid_constant__ TdnnGemmParams p) {
   // the staged epilogue moves 64-channel boxes; the 32-wide instances keep the direct stores
   constexpr bool kStaged = staged_epilogue<BLOCK_N, kPool, kHist>();
-  using Cfg = GemmCfg<BLOCK_N, kStaged>;
+  using Cfg = GemmCfg<BLOCK_N, kPool, kHist>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kBBytes = Cfg::kBBytes;
   constexpr int kStageBytes = Cfg::kStageBytes;
@@ -267,7 +268,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     tma_prefetch_desc(&map_a_lo);
     tma_prefetch_desc(&map_w_hi);
     tma_prefetch_desc(&map_w_lo);
-    if (kStaged && p.tma_store) {
+    if ((kStaged || kPool) && p.tma_store) {
       tma_prefetch_desc(&map_y_hi);
       tma_prefetch_desc(&map_y_lo);
     }
@@ -383,6 +384,9 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
 
   XVB_TL(
     long long tl_start = 0, tl_first = 0, tl_issued = 0, tl_retired = 0, tl_wait = 0;
+    long long tl_ep[4] = {0, 0, 0, 0};                 // epilogue sub-phases: TMA read wait, coefficients + barrier, arithmetic, store issue
+    long long tl_t = 0;
+    auto tl_mark = [&](int ph) { const long long t = clock64(); tl_ep[ph] += t - tl_t; tl_t = t; };
     unsigned long long* tl_cta = p.timeline ? p.timeline + (size_t)blockIdx.x * (kTimelineHead + (size_t)kTimelineRec * p.timeline_tiles) : nullptr;
     if (tl_cta && threadIdx.x == 0) { tl_cta[0] = global_timer(); tl_cta[1] = (unsigned long long)clock64(); }
   )
@@ -393,6 +397,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       r[0] = (unsigned long long)tl_start; r[1] = (unsigned long long)tl_first; r[2] = (unsigned long long)tl_issued;
       r[3] = (unsigned long long)tl_retired; r[4] = (unsigned long long)clock64(); r[5] = (unsigned long long)tl_wait;
       r[6] = (unsigned long long)wg; r[7] = 1ull;
+      for (int ph = 0; ph < 4; ++ph) r[8 + ph] = (unsigned long long)tl_ep[ph];
     }
   };)
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tj) {
@@ -410,10 +415,14 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         stage %= kStages;
         continue;
       }
-      if (tj > 0) asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
+      if (tj > 0) {
+        // fused pooling: the warpgroup's previous TMA store has read the staging buffer, for all its threads past here
+        if (kPool && (threadIdx.x & 127) == 0) tma_store_wait_read<0>();
+        asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
+      }
     }
     ++it;
-    XVB_TL(tl_start = clock64(); tl_wait = 0;)
+    XVB_TL(tl_start = clock64(); tl_wait = 0; tl_ep[0] = tl_ep[1] = tl_ep[2] = tl_ep[3] = 0;)
     // ---- main loop: one k block (64 channels of one tap and source) per operand stage
     // The stage before `stage` in the ring is the one whose MMAs retire next.  It is derived, and so is the tile's
     // first MMA (which overwrites the accumulators), rather than carried: the ping-pong main loop has no register to spare.
@@ -454,7 +463,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     if (kPingPong && tile + gridDim.x < p.num_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(3 - wg) : "memory");
     XVB_TL(tl_issued = clock64();)
     wgmma_wait<0>();
-    XVB_TL(tl_retired = clock64();)
+    XVB_TL(tl_retired = clock64(); tl_t = tl_retired;)
 #pragma unroll
     for (int hh = 0; hh < kHalves; ++hh) wgmma_fence_operands(acc[hh]);
     if (kb_end > kb_begin && lane == 0) mbar_arrive(&empty_bar[stage_before()]);
@@ -469,6 +478,10 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       nv = nv < 0 ? 0 : (nv > p.Tb ? p.Tb : nv);
       const int tblk = m_unit % p.num_t_blk;
       const int gl = p.Tb < 8 ? p.Tb : 8;              // columns of one group inside one 8-column chunk
+      // Full 8-frame time blocks (below) stage the tile's partials in the warpgroup's 16 KB, [utterance][mean | M2][128
+      // channels] fp32, and one thread stores them with one TMA store through the (Cout, 2, B, time block) map of
+      // pool_partial, whose extents clip the channels past Cout and the utterances past B.  The previous tile's store
+      // has read the buffer: its thread waited for that before the turn barrier of this tile's main loop.
 #pragma unroll 1
       for (int hh = 0; hh < kHalves; ++hh) {
       if (hh > 0) half_down();
@@ -486,7 +499,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       // they are exact except where d * d * n overflows, and there they give what chan_merge gives), so the partials
       // are bit-identical to the general path's on finite data.  No summary carries from one chunk to the next, so
       // the 16 chunks of a row are independent chains that the compiler interleaves.
-      if (p.Tb == 8 && nvh == 8 XVB_TL(&& !p.timeline_general)) {
+      if (p.tma_store && p.Tb == 8 && nvh == 8 XVB_TL(&& !p.timeline_general)) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
@@ -494,8 +507,10 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
           const float bias_c = (cvalid && p.bias) ? __ldg(p.bias + cch) : 0.f;
           const float scale_c = (cvalid && bn) ? __ldg(p.scale + cch) : 1.f;
           const float shift_c = (cvalid && bn) ? __ldg(p.shift + cch) : 0.f;
-          float* dst0 = p.pool_partial + ((long long)tblk * p.B + b0h) * (2LL * p.Cout) + cch;
-          const bool writer = cvalid && q4 == 0;
+          int tid = threadIdx.x;                          // opaque, as b0h: derived per use, not kept live
+          asm volatile("" : "+r"(tid));
+          const uint32_t dst0 = smem_u32(slab_base) + (tid >> 7) * kStageOutBytes +
+                                4 * (16 * ((tid >> 5) & 3) + ((tid & 31) >> 2) + 64 * hh + 8 * h);
 #pragma unroll
           for (int i = 0; i < BLOCK_N / 8; ++i) {
             const float x0 = fmaf(fmaxf(acc[0][4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
@@ -510,13 +525,13 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             m2b = __shfl_xor_sync(0xffffffffu, m2, 2);
             mean = fmaf(d, 0.5f, mean);
             m2 += m2b + d * d * 4.f * 0.5f;
-            if (writer && b0h + i < p.B) {
-              float* dst = dst0 + (long long)i * (2LL * p.Cout);
-              dst[0] = mean;
-              dst[p.Cout] = m2;
+            if (q4 == 0) {
+              st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i, mean);
+              st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i + 4 * BLOCK_N, m2);
             }
           }
         }
+        XVB_TL(tl_mark(2);)
         continue;
       }
 #pragma unroll
@@ -560,6 +575,17 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
           }
         }
       }
+      }
+      XVB_TL(tl_mark(2);)
+      if (p.tma_store && p.Tb == 8 && nv == 8 XVB_TL(&& !p.timeline_general)) {
+        fence_proxy_async();                             // the staged partials become visible to the TMA unit
+        asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
+        XVB_TL(tl_mark(1);)
+        if ((threadIdx.x & 127) == 0) {
+          tma_store_4d(&map_y_hi, smem_u32(slab_base) + wg * kStageOutBytes, n0, 0, b0, tblk);
+          tma_store_commit();
+        }
+        XVB_TL(tl_mark(3);)
       }
       XVB_TL(tl_flush();)
       continue;
@@ -641,6 +667,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             const int c0 = n0 + kBlockK * cr;
             if (c0 >= p.Cout) break;
             if (wtid == 0) tma_store_wait_read<0>();      // the previous piece has left the staging buffer
+            XVB_TL(tl_mark(0);)
             if (wtid < kBlockK) {
               const int c = c0 + wtid;
               const bool in = c < p.Cout;
@@ -649,6 +676,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
               st_shared_f32(coefs + 4 * (2 * kBlockK + wtid), (in && bn) ? __ldg(p.shift + c) : 0.f);
             }
             asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
+            XVB_TL(tl_mark(1);)
 #pragma unroll
             for (int i = 0; i < kBlockK / 8; ++i) {
               const float2 bias_c = ld_shared_f2(coef + 32 * i), scale_c = ld_shared_f2(coef + 32 * i + 4 * kBlockK),
@@ -677,6 +705,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
                 st_shared_u32(at + kStagePlaneBytes, pack_bf16x2(l0, l1) & keep[r]);
               }
             }
+            XVB_TL(tl_mark(2);)
             fence_proxy_async();                          // the staged piece becomes visible to the TMA unit
             asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
             if (wtid == 0) {
@@ -685,6 +714,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
               tma_store_3d(&map_y_lo, stg + kStagePlaneBytes, c0, ht, hb);
               tma_store_commit();
             }
+            XVB_TL(tl_mark(3);)
           }
         }
         XVB_TL(tl_flush();)
@@ -769,7 +799,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
     }
   }
   if constexpr (kHist) hist_flush();
-  if constexpr (kStaged) {
+  if constexpr (kStaged || kPool) {
     if (p.tma_store && (threadIdx.x & 127) == 0) tma_store_wait_done<0>();   // this thread's stores have landed
   }
   XVB_TL(if (tl_cta && (threadIdx.x & 127) == 0) { tl_cta[2 + 2 * wg] = global_timer(); tl_cta[3 + 2 * wg] = (unsigned long long)clock64(); })
@@ -867,6 +897,15 @@ static int make_store_map(CUtensorMap* m, const void* base, int Cout, int T, int
   return make_tensor_map(m, base, 2, 3, dims, strides, box, 128);
 }
 
+// Store map of the fused pooling's partials, pool_partial as (Cout, 2, B, time blocks) fp32 ([mean | M2] per time block
+// and utterance); box = 128 channels x both x the 16 utterances of a tile with 8-frame time blocks x one time block.
+static int make_partial_map(CUtensorMap* m, const float* base, int Cout, int B, int nblk) {
+  const unsigned long long dims[4] = {(unsigned long long)Cout, 2ull, (unsigned long long)B, (unsigned long long)nblk};
+  const unsigned long long strides[3] = {4ull * Cout, 8ull * Cout, 8ull * Cout * (unsigned long long)B};
+  const unsigned box[4] = {(unsigned)kBlockM, 2u, 16u, 1u};
+  return make_tensor_map(m, base, 4, 4, dims, strides, box, 0);
+}
+
 // (K, Cout) bf16 packed weight, K contiguous; box = 64 x block_n.
 static int make_weight_map(CUtensorMap* m, const void* base, long long K, int Cout, int block_n) {
   PFN_encodeTiled enc = get_encode();
@@ -922,7 +961,7 @@ struct GemmPlan {
 
 template <int BLOCK_N, bool kPool, bool kHist, bool kSwish>
 static int launch_inst(const GemmPlan& pl, const TdnnGemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, staged_epilogue<BLOCK_N, kPool, kHist>()>;
+  using Cfg = GemmCfg<BLOCK_N, kPool, kHist>;
   XVB_ENSURE_DYN_SMEM((tdnn_gemm_bf16x3_kernel<BLOCK_N, kPool, kHist, kSwish>), Cfg::kSmemBytes);
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(pl.grid);
@@ -955,8 +994,13 @@ static int prepare_gemm(GemmPlan& pl, const void* w_hi, const void* w_lo) {
   // whole, up to 7 channels past Cout (in a channel slice of a wider buffer, another tensor's channels).
   p.tma_store = staged_epilogue<BLOCK_N, kPool, kHist>() && p.y_hi && !p.y_f32 && p.k_slices == 1 && !p.row_bias && !p.utt_bias &&
                 p.Cout % 8 == 0;
+  // Fused pooling: the full 8-frame time blocks' partials leave through one TMA store per tile (the kernel's map_y_hi).
+  if (kPool) p.tma_store = p.Tb == 8;
   XVB_TL(if (g_timeline_direct) p.tma_store = 0;)
-  if (p.tma_store) {
+  if (kPool && p.tma_store) {
+    if ((rc = make_partial_map(&pl.my_hi, p.pool_partial, p.Cout, p.B, p.num_t_blk))) return rc;
+    pl.my_lo = pl.mw_lo;   // unused
+  } else if (p.tma_store) {
     if ((rc = make_store_map(&pl.my_hi, p.y_hi, p.Cout, p.T, p.B, p.ldy, p.Tb))) return rc;
     if ((rc = make_store_map(&pl.my_lo, p.y_lo, p.Cout, p.T, p.B, p.ldy, p.Tb))) return rc;
   } else {

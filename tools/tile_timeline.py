@@ -13,7 +13,9 @@ the CTA's head carries %globaltimer and clock64 at both ends, which converts clo
 Printed per layer, medians over all tiles of one launch (after two warm-up launches): main loop (start to MMAs
 retired), epilogue (MMAs retired to epilogue end), the wait on the operand ring's full barriers inside the main loop,
 and the share of the CTAs' time during which neither warpgroup had MMAs in flight (from a tile's first operands
-arriving to its MMAs retiring).  --direct-stores keeps the plans on the direct-store layer epilogue and the fused
+arriving to its MMAs retiring).  The epilogue is then split into the time warpgroup thread 0 spent waiting for
+the TMA reads of the staging buffer, loading coefficients and on the epilogue's named barriers, on the arithmetic and
+staging (or, without staging, the stores), and issuing the TMA stores.  --direct-stores keeps the plans on the direct-store layer epilogue and the fused
 pooling epilogue on its general path."""
 import argparse
 import ctypes as C
@@ -22,7 +24,7 @@ import sys
 
 HERE = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(HERE, "tools"))
-HEAD, REC = 8, 8
+HEAD, REC = 8, 12
 
 
 def main():
@@ -56,8 +58,9 @@ def main():
     print("card: {}, {} SMs".format(card(), sms))
     print("B={} T={}, {} epilogue of the layer kernel (timeline build)".format(
         B, T, "direct-store / general pooling" if args.direct_stores else "staged TMA-store / full-block pooling"))
-    print("{:6s} {:>9s} {:>10s} {:>9s} {:>9s} {:>12s} {:>10s}".format(
-        "layer", "tiles/CTA", "main loop", "epilogue", "op. wait", "no MMA", "CTA time"))
+    print("{:6s} {:>9s} {:>10s} {:>9s} {:>9s} {:>12s} {:>10s} | {:>9s} {:>10s} {:>9s} {:>9s}".format(
+        "layer", "tiles/CTA", "main loop", "epilogue", "op. wait", "no MMA", "CTA time",
+        "TMA read", "coef+bar", "arith", "store"))
     for name, cin, cout, ctx, im2col, pool in LAYERS:
         span = ctx[-1] - min(ctx[0], 0) + 1
         w = torch.randn(cout, cin, span, device=dev) / np.sqrt(cin * len(ctx))
@@ -103,13 +106,15 @@ def main():
         clk_end = np.maximum(head[:, 3], head[:, 5])
         gt_end = np.maximum(head[:, 2], head[:, 4])
         us_per_clk = (gt_end - head[:, 0]) * 1e-3 / np.maximum(clk_end - head[:, 1], 1)    # per CTA
-        main, epi, wait, idle_share = [], [], [], []
+        main, epi, wait, idle_share, phases = [], [], [], [], [[], [], [], []]
         for cta in range(grid):
             r = rec[cta][rec[cta][:, 7] == 1]
             k = us_per_clk[cta]
             main += list((r[:, 3] - r[:, 0]) * k)
             epi += list((r[:, 4] - r[:, 3]) * k)
             wait += list(r[:, 5] * k)
+            for ph in range(4):
+                phases[ph] += list(r[:, 8 + ph] * k)
             # union of [first operands, MMAs retired) over both warpgroups' tiles
             busy, end = 0, head[cta, 1]
             for s, e in sorted(zip(r[:, 1], r[:, 3])):
@@ -118,9 +123,9 @@ def main():
                     busy += e - s
                     end = e
             idle_share.append(1.0 - busy / max(clk_end[cta] - head[cta, 1], 1))
-        print("{:6s} {:9d} {:7.2f} us {:6.2f} us {:6.2f} us {:10.1f} % {:7.1f} us".format(
+        print("{:6s} {:9d} {:7.2f} us {:6.2f} us {:6.2f} us {:10.1f} % {:7.1f} us | {:6.2f} us {:7.2f} us {:6.2f} us {:6.2f} us".format(
             name, per_cta, np.median(main), np.median(epi), np.median(wait), 100 * np.median(idle_share),
-            np.median((gt_end - head[:, 0]) * 1e-3)))
+            np.median((gt_end - head[:, 0]) * 1e-3), *[np.median(ph) for ph in phases]))
 
 
 if __name__ == "__main__":
