@@ -199,6 +199,7 @@ SIGNATURES = {
     "xvb_ecapa_create": (_i, [C.POINTER(_p), _i, _i, _i, _i, _i]),
     "xvb_ecapa_set_mqmha": (_i, [_p, _i, _i, _i, _i, _i, _i, _i]),
     "xvb_ecapa_set_chained": (_i, [_p, _i]),
+    "xvb_ecapa_set_attention": (_i, [_p, _i, _f]),
     "xvb_ecapa_set_layer": (_i, [_p, C.c_char_p, _i, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_ecapa_finalize": (_i, [_p]),
     "xvb_ecapa_embed_dim": (_i, [_p]),

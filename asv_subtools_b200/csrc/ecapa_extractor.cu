@@ -15,12 +15,16 @@
 // (xvb_ecapa_set_chained): block b + 1 reads block b's output straight from its slot of the MFA input, at row pitch
 // 3C, as the input of its first 1x1 layer and as its residual, and no running sum is written.
 //
+// The launcher model of runEcapaXvector.py (pytorch/model/ecapa-tdnn-xvector.py) pools without global context
+// (xvb_ecapa_set_attention(h, 0, 1e-9f)): attention conv 1 reads x alone, with its own bias, and no ReLU or BN before the
+// tanh, so the global mean/std pass and "att_gs" are left out, and the weighted std is floored at the given variance.
+//
 // Layers are handed over by NAME with the weights as the state_dict stores them (host fp32, eval BatchNorm
 // folded to scale/shift by the caller); the two derived layers of the attention conv ("att_x": its columns
 // over x, "att_gs": its columns over [mean | std] plus the bias) and "fc2" (bn_stats folded into its weight)
 // are prepared by the caller -- see the Python blueprint.  The handle keeps the layers as handed over and builds the
 // model from them at finalize; xvb_ecapa_save writes them back (the XVBE0001 / XVBE0002 / XVBG0001 layouts are in
-// model_file.cpp).
+// model_file.cpp, with XVBE0003 for the attention without global context).
 #include <cuda_runtime.h>
 #include <string.h>
 
@@ -65,6 +69,11 @@ struct Config {
   int mq = 0, mq_heads = 1, mq_q = 1, mq_hidden = 0, mq_share = 0, mq_layers = 2, mq_tatt = 1, mq_stddev = 1;
   // residual form (xvb_ecapa_set_chained): 0 dense, block b + 1 reads x + x1 (+ x2); 1 chained, it reads block b's output
   int chained = 0;
+  // attentive pooling (xvb_ecapa_set_attention): global context (1: [x | mean | std] into the first attention conv) and the
+  // variance floor of the pooled std
+  int gctx = 1;
+  float floor = 1e-5f;
+  bool attention_set = false;   // xvb_ecapa_set_attention was called (it excludes set_mqmha and set_chained)
   // widths derived from the pooling: att_x outputs AX, the logits NL (row pitch ldlog), the pooled statistics P of the
   // P2-wide [mean | std] buffer (default model: AX = H, NL = D, P = P2 = 2D)
   int AX = 0, NL = 0, ldlog = 0, P = 0, P2 = 0;
@@ -134,6 +143,7 @@ extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int 
                                    int time_attention, int stddev) {
   XVB_CHECK_ARG(is_draft(h) && h->draft->recs.empty(), "xvb_ecapa_set_mqmha: call it between xvb_ecapa_create and the first set_layer");
   Model* m = h->draft;
+  XVB_CHECK_ARG(!m->cfg.attention_set, "xvb_ecapa_set_mqmha: the model's attentive pooling is set by xvb_ecapa_set_attention");
   XVB_CHECK_ARG(num_head >= 1 && num_q >= 1 && hidden >= 1 && (affine_layers == 1 || affine_layers == 2) && m->cfg.D % num_head == 0 &&
                 (m->cfg.D / num_head) % 4 == 0 && hidden * num_head * num_q == m->cfg.H,
                 "xvb_ecapa_set_mqmha: need %d channels in heads of a multiple of 4, 1 or 2 affine layers and att_hidden = "
@@ -154,7 +164,20 @@ extern "C" int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int 
 extern "C" int xvb_ecapa_set_chained(xvb_ecapa_t* h, int chained) {
   XVB_CHECK_ARG(is_draft(h) && h->draft->recs.empty(), "xvb_ecapa_set_chained: call it between xvb_ecapa_create and the first set_layer");
   XVB_CHECK_ARG(chained == 0 || chained == 1, "xvb_ecapa_set_chained: chained must be 0 or 1, got %d", chained);
+  XVB_CHECK_ARG(!h->draft->cfg.attention_set, "xvb_ecapa_set_chained: the chained form has MQMHA pooling, not xvb_ecapa_set_attention's");
   h->draft->cfg.chained = chained;
+  return XVB_OK;
+}
+
+extern "C" int xvb_ecapa_set_attention(xvb_ecapa_t* h, int global_context, float floor) {
+  XVB_CHECK_ARG(is_draft(h) && h->draft->recs.empty(), "xvb_ecapa_set_attention: call it between xvb_ecapa_create and the first set_layer");
+  Config& c = h->draft->cfg;
+  XVB_CHECK_ARG(!c.mq && !c.chained, "xvb_ecapa_set_attention: not with xvb_ecapa_set_mqmha or xvb_ecapa_set_chained, which have "
+                "their own attention and residual forms");
+  XVB_CHECK_ARG(global_context == 0 || global_context == 1, "xvb_ecapa_set_attention: global_context must be 0 or 1, got %d",
+                global_context);
+  XVB_CHECK_ARG(floor > 0.f && floor < 1.f, "xvb_ecapa_set_attention: the variance floor must lie in (0, 1), got %g", (double)floor);
+  c.gctx = global_context; c.floor = floor; c.attention_set = true;
   return XVB_OK;
 }
 
@@ -259,9 +282,10 @@ static int build(Model* m, const std::vector<TapRec>& recs) {
   rc = take("mfa", 3 * C, c.D, 1, &m->mfa);
   if (rc) return rc;
   if (!c.mq) {
-    if ((rc = take("att_x", c.D, c.H, 1, &m->att_x)) || (rc = take("att_gs", 2 * c.D, c.H, 1, &m->att_gs)) ||
+    if ((rc = take("att_x", c.D, c.H, 1, &m->att_x)) || (c.gctx && (rc = take("att_gs", 2 * c.D, c.H, 1, &m->att_gs))) ||
         (rc = take("att2", c.H, c.D, 1, &m->att2)))
       return rc;
+    XVB_CHECK_ARG(c.gctx || !find(recs, "att_gs"), "xvb_ecapa_finalize: 'att_gs' in an attention without global context");
   } else {   // per-group input widths: att_x reads a head's Cg channels of x, att2 one query's hidden units
     rc = take("att_x", c.D / c.mq_heads, c.AX, 1, &m->att_x);
     if (rc) return rc;
@@ -415,15 +439,17 @@ extern "C" int xvb_ecapa_extract(xvb_ecapa_t* h, const float* feats, int B, int 
   if (m->cfg.mq) {
     if ((rc = mqmha_pool(h, B, T, stream))) return rc;
   } else {
-  if ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, nullptr, nullptr, 0, stream)) ||
-      (rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream)))
+  // global context: the time-constant [mean | std] columns of attention conv 1 become the per-utterance bias
+  if (m->cfg.gctx && ((rc = xvb_stats_pool_ex(h->MF, D, B, T, D, 1e-5f, 1, h->gstat, nullptr, nullptr, 0, stream)) ||
+                      (rc = small_layer(&m->att_gs, h->gstat, 2 * D, B, h->ub, m->cfg.H, 0, stream))))
     return rc;
   a = layer_args(m->att_x, h->M, B, T, h->A1);
-  a.flags |= XVB_TANH; a.utt_bias = h->ub; a.ld_utt_bias = m->cfg.H;
+  a.flags |= XVB_TANH;
+  if (m->cfg.gctx) { a.utt_bias = h->ub; a.ld_utt_bias = m->cfg.H; }
   if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
   a = layer_args(m->att2, h->A1, B, T, View{}, h->LOG, D);
   if ((rc = xvb_tdnn_affine_ex(&a, stream))) return rc;
-  if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, 1e-5f, h->pstat, nullptr, nullptr, 0, stream))) return rc;
+  if ((rc = xvb_attn_stats_pool(h->LOG, D, h->MF, D, B, T, D, m->cfg.floor, h->pstat, nullptr, nullptr, 0, stream))) return rc;
   }
   if (m->fc1.Cout) {              // fc1 [-> fc2] on CUDA cores (fp32)
     const ELayer* fc1 = &m->fc1;
@@ -466,11 +492,17 @@ extern "C" int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path) {
   XVB_CHECK_ARG(finalized(h) && path, "xvb_ecapa_save: model not finalized");
   const Config& c = h->m->cfg;
   XVB_CHECK_ARG(c.mq || !c.chained, "xvb_ecapa_save: an XVBG0001 file holds a chained model with MQMHA pooling");
+  std::vector<const TapRec*> layers;
+  for (const TapRec& r : h->m->recs) layers.push_back(&r);
+  if (c.gctx != 1 || c.floor != 1e-5f) {   // XVBE0003: XVBE0001's header, then the attention of xvb_ecapa_set_attention
+    int32_t fbits;
+    memcpy(&fbits, &c.floor, sizeof fbits);
+    const int32_t head3[8] = {c.feat_dim, c.C, c.D, c.H, c.E, (int32_t)h->m->recs.size(), c.gctx, fbits};
+    return save_tap_file("xvb_ecapa_save", path, "XVBE0003", head3, sizeof head3, layers, true);
+  }
   const int32_t head[14] = {c.feat_dim, c.C, c.D, c.H, c.E, (int32_t)h->m->recs.size(),   // then XVBE0002's pooling
                             c.mq_heads, c.mq_q, c.mq_hidden, c.mq_share, c.mq_layers, c.mq_tatt, c.mq_stddev,
                             c.chained};                                                   // then XVBG0001's residual form
-  std::vector<const TapRec*> layers;
-  for (const TapRec& r : h->m->recs) layers.push_back(&r);
   const char* magic = c.chained ? "XVBG0001" : c.mq ? "XVBE0002" : "XVBE0001";
   return save_tap_file("xvb_ecapa_save", path, magic, head, (c.chained ? 14 : c.mq ? 13 : 6) * sizeof(int32_t), layers, true);
 }

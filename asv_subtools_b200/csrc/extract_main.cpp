@@ -15,7 +15,8 @@
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
 // the input side.  The model file is any of the six families, told apart by its magic: TDNN x-vector
-// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling, or XVBG0001 for
+// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling, or XVBE0003 for the
+// launcher model of pytorch/model/ecapa-tdnn-xvector.py, whose attentive pooling has no global context, or XVBG0001 for
 // egrecho's EcapaXvector with chained blocks),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), each written by its native extractor's save() (model_file.cpp).  What it adds:
@@ -100,6 +101,7 @@ const Family kFamilies[] = {
     {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false, nullptr},
     {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false, nullptr},
     {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true, nullptr},
+    {{"XVBE0003", nullptr}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false, nullptr},
     {{"XVBG0001", nullptr}, "loading the egrecho ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 4000, true, nullptr},
     // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
     {{nullptr, nullptr}, "loading the model", "xvb_extractor_extract",
@@ -309,7 +311,7 @@ int main(int argc, char** argv) {
              "                   [--mixed-lengths] [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002), egrecho ECAPA-TDNN (XVBG0001),\n"
+             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002 / XVBE0003), egrecho ECAPA-TDNN (XVBG0001),\n"
              "2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001) or CAM++\n"
              "x-vector (XVBP0001) model, recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the\n"
              "model's own chunk rule), 4000 for CAM++ and egrecho ECAPA-TDNN and 10000 otherwise.  A Conformer chunk needs at\n"

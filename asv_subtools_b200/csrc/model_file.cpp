@@ -15,6 +15,10 @@
 //              affine_layers, time_attention, stddev} after the dims; grouped convs stored as the state_dict holds them.
 //   "XVBG0001" (egrecho's ECAPA-TDNN, chained blocks): the XVBE0002 header with i32 residual_form (1: chained,
 //              xvb_ecapa_set_chained) after the pooling record, then the named tap records.
+//   "XVBE0003" (ECAPA-TDNN whose attentive pooling is set by xvb_ecapa_set_attention, e.g. the launcher model of
+//              pytorch/model/ecapa-tdnn-xvector.py): the XVBE0001 header with i32 global_context and the f32 variance
+//              floor after the dims, then the named tap records.  Written only for an attention other than the default
+//              (1, 1e-5), so XVBE0001 / XVBE0002 / XVBG0001 files are written as before.
 //
 // The named-record files of the native ResNet, RepVGG, Conformer and CAM++ extractors (save_records / load_records
 // below) and the record store behind them (records.h).
@@ -300,18 +304,30 @@ extern "C" int xvb_ecapa_load(xvb_ecapa_t** out, const char* path) {
   xvb_ecapa_t* h = nullptr;
   int rc = XVB_EINVAL;
   do {
-    int32_t pr[8];   // the pooling record, then XVBG0001's residual form
+    int32_t pr[8];   // the pooling record, then XVBG0001's residual form; or XVBE0003's attention record
     const bool got = rd(f, magic, 8);
     const bool g = got && memcmp(magic, "XVBG0001", 8) == 0;
     const bool mq = g || (got && memcmp(magic, "XVBE0002", 8) == 0);
-    const bool ok_magic = mq || (got && memcmp(magic, "XVBE0001", 8) == 0);
-    if (!ok_magic || !rd(f, hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(f, pr, (g ? 8 : 7) * sizeof(int32_t)))) {
-      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 / XVBG0001 file", path);
+    const bool att = got && memcmp(magic, "XVBE0003", 8) == 0;
+    const bool ok_magic = mq || att || (got && memcmp(magic, "XVBE0001", 8) == 0);
+    if (!ok_magic || !rd(f, hd, sizeof hd) || hd[5] < 1 || hd[5] > 256 || (mq && !rd(f, pr, (g ? 8 : 7) * sizeof(int32_t))) ||
+        (att && !rd(f, pr, 2 * sizeof(int32_t)))) {
+      set_error("xvb_ecapa_load: '%s' is not an XVBE0001 / XVBE0002 / XVBE0003 / XVBG0001 file", path);
       break;
     }
     if ((rc = xvb_ecapa_create(&h, hd[0], hd[1], hd[2], hd[3], hd[4]))) break;
     if (mq && (rc = xvb_ecapa_set_mqmha(h, pr[0], pr[1], pr[2], pr[3], pr[4], pr[5], pr[6]))) break;
     if (g && (rc = xvb_ecapa_set_chained(h, pr[7]))) break;
+    if (att) {
+      float floor_;
+      memcpy(&floor_, &pr[1], sizeof floor_);
+      if (pr[0] == 1 && floor_ == 1e-5f) {   // the default attention is written as XVBE0001
+        set_error("xvb_ecapa_load: '%s' is an XVBE0003 file with the default attention", path);
+        rc = XVB_EINVAL;
+        break;
+      }
+      if ((rc = xvb_ecapa_set_attention(h, pr[0], floor_))) break;
+    }
     xvb::TapRec r;
     for (int i = 0; i < hd[5] && rc == XVB_OK; ++i) {
       int32_t nl = 0;

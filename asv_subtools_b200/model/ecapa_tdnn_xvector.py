@@ -285,19 +285,20 @@ def _segment_layers(m):
 
 def native_config(m):
     """{"create": the arguments of xvb_ecapa_create after the handle, "mqmha": those of xvb_ecapa_set_mqmha, or None for
-    the attentive pooling, "chained": False (dense blocks, xvb_ecapa_set_chained)} for model m."""
+    the attentive pooling, "chained": False (dense blocks, xvb_ecapa_set_chained), "attention": None (the default
+    attentive pooling; else the arguments of xvb_ecapa_set_attention)} for model m."""
     st = m.stats
     mq = isinstance(st, MQMHASP)
     hidden = st.hidden_size * st.num_head * st.num_q if mq else st.attention[0].out_channels
     return {"create": (m.inputs_dim, m.layer1.affine.output_dim, st.in_dim, hidden, m.embd_dim),
             "mqmha": (st.num_head, st.num_q, st.hidden_size, int(st.share), st.affine_layers, int(st.time_attention),
                       int(st.stddev)) if mq else None,
-            "chained": False}
+            "chained": False, "attention": None}
 
 
 class NativeEcapaExtractor(ShardExtractor):
     """xvb_ecapa_t: packed weights, workspace and the whole launch sequence in the C library, on the device that is
-    current when it is built (or loaded from an XVBE0001 / XVBE0002 / XVBG0001 file), from the model's native_records()
+    current when it is built (or loaded from an XVBE0001 / XVBE0002 / XVBE0003 / XVBG0001 file), from the model's native_records()
     and native_config()."""
 
     PREFIX = "ecapa"
@@ -311,6 +312,8 @@ class NativeEcapaExtractor(ShardExtractor):
             self._call("set_mqmha", self._h, *cfg["mqmha"])
         if cfg["chained"]:
             self._call("set_chained", self._h, 1)
+        if cfg.get("attention") is not None:
+            self._call("set_attention", self._h, *cfg["attention"])
 
     def _layers(self, m):
         from asv_subtools_b200._lib import int_array
@@ -335,6 +338,8 @@ class EcapaExtractor:
         self.device = device
         self.feat_dim, self.channels, self.mfa_dim, _, self.embed_dim = cfg["create"]
         self.chained = cfg["chained"]
+        # (global_context, floor) of the attentive pooling (xvb_ecapa_set_attention); the default is ECAPA_TDNN's
+        self.global_context, self.floor = cfg.get("attention") or (1, 1e-5)
         self.ldf = (self.feat_dim + 7) // 8 * 8
         self.last_launches = 0
         mq = cfg["mqmha"]
@@ -368,7 +373,8 @@ class EcapaExtractor:
         if self.mq is not None:
             self.att = {name: layer(name) for name in ("att_x", "att_gs", "att2") if name in recs}
             return
-        self.att_x, self.att_gs, self.att2 = layer("att_x"), layer("att_gs"), layer("att2")
+        self.att_x, self.att2 = layer("att_x"), layer("att2")
+        self.att_gs = layer("att_gs") if self.global_context else None
 
     def extract(self, feats):
         """feats (B,T,F) fp32 CUDA -> (B, embd_dim) fp32 CUDA (asynchronous on the current stream)."""
@@ -415,14 +421,16 @@ class EcapaExtractor:
         self.mfa.run(CAT, y=M, y_f32=MF)
         if self.mq is not None:
             return self._mqmha_tail(M, MF)
-        gstat = ops.stats_pool_ex(MF, 1e-5, 1)      # global mean | sqrt(var_unbiased + 1e-5)
-        _mark("stats_pool(global)")
-        ub = self.att_gs.run_rows(gstat)
+        ub = None
+        if self.global_context:
+            gstat = ops.stats_pool_ex(MF, 1e-5, 1)      # global mean | sqrt(var_unbiased + 1e-5)
+            _mark("stats_pool(global)")
+            ub = self.att_gs.run_rows(gstat).view(B, -1)
         A1 = P.empty((B, T, self.att_x.cout), dev)
-        self.att_x.run(M, utt_bias=ub.view(B, -1), tanh=True, y=A1)
+        self.att_x.run(M, utt_bias=ub, tanh=True, y=A1)
         LOG = torch.empty(B, T, D, dtype=torch.float32, device=dev)
         self.att2.run(A1, y_f32=LOG)
-        x = ops.attn_stats_pool(LOG, MF, 1e-5)
+        x = ops.attn_stats_pool(LOG, MF, self.floor)
         _mark("attn_stats_pool")
         for layer in self.segment:
             x = layer.run_rows(x)

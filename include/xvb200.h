@@ -762,6 +762,12 @@ int xvb_ecapa_set_mqmha(xvb_ecapa_t* h, int num_head, int num_q, int hidden, int
  * block 3 x + x1 + x2; 1 is egrecho's EcapaXvector (subtools2/egrecho/models/ecapa/ecapa_xvector.py:420-427), each block
  * reading the previous block's output.  Call between create and the first set_layer; the layers are the same. */
 int xvb_ecapa_set_chained(xvb_ecapa_t* h, int chained);
+/* The attentive pooling of the default model: global_context = 1 with floor 1e-5 (the default) is ECAPA_TDNN's, attention
+ * conv 1 reading [x | mean | std] ("att_x" + "att_gs") and the pooled std floored at variance 1e-5; global_context = 0 is
+ * the AttentiveStatsPool of pytorch/model/ecapa-tdnn-xvector.py:120-134, alpha = softmax(att2(tanh(att_x(x)))) with
+ * "att_x" the first conv with its own bias and no ReLU or BatchNorm, no "att_gs", and the std floored at `floor`
+ * (1e-9 there).  Call between create and the first set_layer; not with xvb_ecapa_set_mqmha or xvb_ecapa_set_chained. */
+int xvb_ecapa_set_attention(xvb_ecapa_t* h, int global_context, float floor);
 int xvb_ecapa_set_layer(xvb_ecapa_t* h, const char* name, int Cout, int Cin, const int* context_host, int ntaps,
                         const float* w_host, const float* bias_host, const float* bn_scale_host,
                         const float* bn_shift_host, int flags);
@@ -783,7 +789,8 @@ int xvb_ecapa_extract_shard_host(xvb_ecapa_t* h, const float* feats_host, int64_
 int xvb_ecapa_last_launches(const xvb_ecapa_t* h);
 /* "XVBE0001" model files: the named layers as handed to xvb_ecapa_set_layer; "XVBE0002" for MQMHA models adds the
  * xvb_ecapa_set_mqmha record; "XVBG0001" for chained models (egrecho's, MQMHA pooling only) adds the residual form
- * after it.  All three load. */
+ * after it; "XVBE0003" for an attention other than the default adds the xvb_ecapa_set_attention record to XVBE0001's
+ * header.  All four load. */
 int xvb_ecapa_save(const xvb_ecapa_t* h, const char* path);
 int xvb_ecapa_load(xvb_ecapa_t** out, const char* path);
 void xvb_ecapa_destroy(xvb_ecapa_t* h);

@@ -12,7 +12,12 @@ attention GEMMs in the layer kernel's grouped mode against their block-diagonal 
 --egrecho [--channels 512|1024]: egrecho's EcapaXvector (EcapaConfig's pooling: one head, one query, hidden 128, time
 attention) at 128 x 300 on the native handle in its chained form, on its Python twin and as the torch fp32 restatement
 (tests/egrecho_ecapa_oracle.py, TF32 off), with the dense ECAPA_TDNN handle of the same width next to it; the four run in
-alternating rounds in one process, and each one's median round is reported."""
+alternating rounds in one process, and each one's median round is reported.
+
+--lawlict [--channels 512|1024]: the ECAPA_TDNN of pytorch/model/ecapa-tdnn-xvector.py (runEcapaXvector.py's model:
+attentive pooling without global context, hidden 128) at 128 x 300 on the native handle, on its Python twin and as the
+torch fp32 restatement (tests/lawlict_ecapa_oracle.py, TF32 off), with the dense ECAPA_TDNN handle of the same width next
+to it, in alternating rounds as for --egrecho."""
 import json
 import os
 import sys
@@ -145,6 +150,57 @@ def main_egrecho(steps, channels, rounds=5):
     print(json.dumps(res))
 
 
+def main_lawlict(steps, channels, rounds=5):
+    import importlib.util
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    sys.path.insert(0, os.path.join(root, "tests"))
+    import lawlict_ecapa_oracle as lo
+    from asv_subtools_b200.model import ecapa_tdnn_xvector as etx
+    spec = importlib.util.spec_from_file_location("lawlict_ecapa_blueprint",
+                                                  os.path.join(root, "asv_subtools_b200", "model", "ecapa-tdnn-xvector.py"))
+    bp = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(bp)
+    B, T, F = 128, 300, 80
+    dev = torch.device("cuda")
+    xs = [torch.randn(B, T, F, device=dev) for _ in range(4)]
+    kw = lo.kwargs(channels=channels)
+    m = bp.ECAPA_TDNN(F, 1211, **kw)
+    sd = onn.make_state_dict(lo.spec(F, kw), 41)
+    m.load_state_dict(sd, strict=True)
+    m.to(dev).eval()
+    dense = ECAPA_TDNN(F, 10, **dict(CANON, ecapa_params=dict(CANON["ecapa_params"], channels=channels)))
+    dense.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F, channels=channels), 201), strict=True)
+    dense.to(dev).eval()
+    sd_dev = {k: v.to(dev) for k, v in sd.items()}
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.backends.cudnn.allow_tf32 = False
+
+    class Torch:
+        def extract(self, x):
+            with torch.no_grad():
+                return lo.forward(sd_dev, x.transpose(1, 2), kw)[:, :, 0]
+
+    runs = {"native": m.extractor(), "twin": etx.EcapaExtractor(m, dev), "torch_fp32": Torch(),
+            "ecapa_tdnn_dense_native": dense.extractor()}
+    times = {k: [] for k in runs}
+    for _ in range(rounds):
+        for name, ex in runs.items():
+            times[name].append(_rate(ex, xs, steps)[0])
+    x = xs[0]
+    nat, twin, ref = (runs[k].extract(x) for k in ("native", "twin", "torch_fp32"))
+    runs["ecapa_tdnn_dense_native"].extract(x)
+    res = {"card": _card(), "workload": "ecapa-tdnn-xvector.py ECAPA_TDNN C{}, 80-d fbank, 300-frame chunks, batch 128".format(
+               channels),
+           "native_equals_twin": bool(torch.equal(nat, twin)),
+           "native_vs_torch_rel": float((nat - ref).abs().max() / ref.abs().max()),
+           "launches": runs["native"].last_launches, "dense_launches": runs["ecapa_tdnn_dense_native"].last_launches}
+    for name, v in times.items():
+        ms = sorted(v)[len(v) // 2]
+        res[name] = {"ms_per_batch": round(ms, 3), "frames_per_s": round(B * T / (ms * 1e-3)),
+                     "rounds_ms": [round(t, 3) for t in v]}
+    print(json.dumps(res))
+
+
 def macs_per_frame(C, F=80, D=1536, H=128):
     """Contraction MACs per frame from the shapes: layer1 (5 taps), per block bn1 + 7 Res2Net steps (3 taps, width C/8)
     + bn2, mfa, the two attention convs (the per-utterance SE and segment layers are left out)."""
@@ -162,6 +218,8 @@ def main():
         raise SystemExit("--channels takes 512 or 1024")
     if "--egrecho" in sys.argv:
         return main_egrecho(steps, channels)
+    if "--lawlict" in sys.argv:
+        return main_lawlict(steps, channels)
     kw = dict(CANON, ecapa_params=dict(CANON["ecapa_params"], channels=channels))
     m = ECAPA_TDNN(F, 10, **kw)
     m.load_state_dict(onn.make_state_dict(onn.ecapa_spec(F, channels=channels), 201), strict=True)
