@@ -157,6 +157,9 @@ SIGNATURES = {
     "xvb_plda_normalize_rows": (_i, [_p, _p, _p, _i64, _i, _i, _p]),
     "xvb_plda_llr_operands": (_i, [_p, _p, _p, _i64, _i, _i, _p, _p, _p]),
     "xvb_trial_histogram": (_i, [_p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i, _i, _i, _f, _f, _i, _p, _p]),
+    "xvb_topk_merge": (_i, [_p, _i64, _i64, _i64, _i64, _i, _p, _p, _p, _p]),
+    "xvb_retrieve_topk_slab_bytes": (_i64, [_i64, _i64]),
+    "xvb_retrieve_topk": (_i, [_p, _i64, _p, _i64, _i, _p, _p, _i, _p, _i64, _p, _p, _p]),
     "xvb_conv2d": (_i, [_p, _p]),
     "xvb_conv2d_head": (_i, [_p, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_conv2d_taps": (_i, [_p, _ip, _i, _p]),

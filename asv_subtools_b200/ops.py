@@ -855,6 +855,38 @@ def trial_histogram(enroll, enroll_spk, test, test_spk, lo, hi, nbins=2048, row_
     return out
 
 
+# Test columns scored per GEMM call.  tools/bench_retrieval.py (H100 80GB HBM3, 700 W, N = 10^6, D = 256): 16 384,
+# 65 536 and 262 144 columns ran within 2.6 % of each other at M = 1 000; at M = 10 000, 16 384 was the fastest.
+RETRIEVE_SLAB_COLS = 16384
+RETRIEVE_SLAB_BYTES = 1 << 30   # the default slab is narrowed so that M x slab_cols fp32 scores stay within 1 GiB
+
+
+def retrieve_topk(enroll, test, k, row_bias=None, col_bias=None, slab_cols=None):
+    """(scores (M, k) fp32, indices (M, k) int64): the k best test rows of every enroll row under
+    enroll . test^T + row_bias[i] + col_bias[j], best first, equal scores by lower test index.  A row with fewer
+    than k test rows has (-inf, -1) in its empty slots.  The (M, N) score matrix is never stored: the test set is
+    scored `slab_cols` rows at a time (a multiple of 4) and merged into running lists."""
+    a = _req(enroll, torch.float32, "enroll")
+    b = _req(test, torch.float32, "test")
+    if a.dim() != 2 or b.dim() != 2 or a.shape[1] != b.shape[1]:
+        raise ValueError("retrieve_topk: enroll (M, D) and test (N, D) must share D")
+    for t, n, name in ((row_bias, a.shape[0], "row_bias"), (col_bias, b.shape[0], "col_bias")):
+        if t is not None and (_req(t, torch.float32, name).numel() != n):
+            raise ValueError("retrieve_topk: {} must hold {} values".format(name, n))
+    m, n = a.shape[0], b.shape[0]
+    if slab_cols is None:
+        fit = max(4, RETRIEVE_SLAB_BYTES // (4 * m) // 4 * 4)
+        slab_cols = min(RETRIEVE_SLAB_COLS, fit, (n + 3) // 4 * 4)
+    nbytes = lib.xvb_retrieve_topk_slab_bytes(m, int(slab_cols))
+    check(0 if nbytes > 0 else nbytes, "xvb_retrieve_topk_slab_bytes")
+    slab = torch.empty(nbytes // 4, dtype=torch.float32, device=a.device)
+    scores = torch.empty(m, int(k), dtype=torch.float32, device=a.device)
+    idx = torch.empty(m, int(k), dtype=torch.int64, device=a.device)
+    check(lib.xvb_retrieve_topk(_ptr(a), m, _ptr(b), n, a.shape[1], _ptr(row_bias), _ptr(col_bias), int(k), _ptr(slab),
+                                int(slab_cols), _ptr(scores), _ptr(idx), _stream()), "xvb_retrieve_topk")
+    return scores, idx
+
+
 # ------------------------------------------------------------------ whole-model extractor
 class Extractor(ShardExtractor):
     """Owner of a native xvb_extractor_t (packed weights + workspace on the current device), built layer by layer with

@@ -82,3 +82,43 @@ def eer_kaldi(scores, labels):
 
 
 METHODS = {"bosaris": eer_bosaris, "det": eer_det, "kaldi": eer_kaldi}
+
+
+def retrieval_map(top_lines, meta_lines):
+    """mAP of a speaker-retrieval top-k file, computed exactly as recipe/cnsrc/sr/cal_mAP.py does, quirks included.
+    `top_lines`: the lines of the top-k file (`spk utt1 ... uttk`); `meta_lines`: the lines of the test metadata
+    (`<dir>/<utt>.wav <spk>-<...> ...`).  Returns the float cal_mAP.py prints as "mAP=%.3f"."""
+    targets = {}
+    for line in meta_lines:
+        fields = line.strip("\n").split(" ")
+        spk = fields[1].split("-")[0]                 # the speaker is field 2 up to its first '-'
+        # strip('.wav') removes any of the characters '.', 'w', 'a', 'v' from both ends (a character set, not a
+        # suffix): "pool/utt13a.wav" -> "pool/utt13", "wav/abc.wav" -> "/abc"; then the part after the first '/'
+        # is the utterance, so an utterance whose name ends in one of those characters never counts as a hit
+        utt = fields[0].strip(".wav").split("/")[1]
+        targets.setdefault(spk, set()).add(utt)
+    total, rows = 0.0, 0
+    for line in top_lines:
+        fields = line.strip("\n").split(" ")
+        rows += 1
+        if fields[0] not in targets:
+            raise KeyError("speaker {} of the top-k file is not in the test metadata".format(fields[0]))
+        mine = targets[fields[0]]
+        hits, score = 0, 0.0
+        for i in range(1, len(fields)):
+            if fields[i] in mine:
+                hits += 1
+            score += hits / i                          # every position adds precision@i, hit or not
+        score /= 10                                    # the constant 10 of the recipe, whatever the list length
+        total += score
+    if rows == 0:
+        raise ValueError("empty top-k file")
+    return total / rows
+
+
+def retrieval_map_files(top_path, meta_path):
+    with open(meta_path, encoding="utf-8") as f:
+        meta = f.readlines()
+    with open(top_path, encoding="utf-8") as f:
+        top = f.readlines()
+    return retrieval_map(top, meta)

@@ -607,6 +607,37 @@ int xvb_trial_histogram(const float* enroll, int64_t Ne, const int32_t* enroll_s
                         int unit_first, int unit_stride, float lo, float hi, int nbins, unsigned long long* hist,
                         void* stream);
 
+/* Speaker retrieval, task 2 of the CN-Celeb recipe (recipe/cnsrc/sr/run-cnsrc_sr.sh stage 4: all-pairs scores,
+ * then trans_score_format.py's groupby('spk-id').nlargest(10, 'scores')): the k best test columns of every
+ * enroll row, without storing the score matrix.  Order: higher score first; equal scores by lower column index
+ * (nlargest(keep='first') over a score file in trials order, and xvb_topn_indices' rule).  1 <= k <= 256; at most
+ * 2^31 - 1 columns in all.
+ *
+ * xvb_topk_merge: merges the columns of a score slab S (rows, ncols), pitch lds (a multiple of 4, S 16-byte aligned),
+ * whose column j is column col0 + j of the full test set, into running per-row lists top_score (rows, k) fp32 /
+ * top_idx (rows, k) int64, sorted best first.  Start the lists at (-inf, -1): a row that has seen fewer than k columns
+ * keeps (-inf, -1) in its empty slots.  A column that does not beat a row's k-th entry is dropped without a sort.
+ * A NaN score is never ranked: the row index is atomicMin'ed into *nan_row (device; set it to ~0 first).
+ *
+ * xvb_retrieve_topk: out (M, k) = the k best columns of a (M, K) . b (N, K)^T + row_bias[i] + col_bias[j] (biases may
+ * be NULL).  Walks b in slabs of slab_cols rows (a positive multiple of 4): each slab is scored by xvb_matmul_nt into
+ * `slab` (xvb_retrieve_topk_slab_bytes(M, slab_cols) bytes, 16-byte aligned, pitch slab_cols) and merged by
+ * xvb_topk_merge, so the scores ranked are the bytes xvb_matmul_nt writes.  Any N: the last 1..3 test rows are scored
+ * from a zero-padded copy and the padded columns are not merged.  Cosine: length-normalised rows, NULL biases.
+ * Kaldi PLDA: the xvb_plda_llr_operands operands and terms (enroll side 0 -> a, row_bias; test side 1 -> b, col_bias).
+ * The layer epilogue turns a NaN accumulator into -inf, so the operands and terms are checked first: a NaN or infinity
+ * in a / row_bias or b / col_bias returns XVB_EINVAL naming the enroll or test row, as does a NaN that reaches a slab,
+ * and like a bad argument writes nothing to out_score / out_idx.  The refusal covers non-finite inputs only: finite
+ * operands whose products overflow fp32 make an infinite or NaN accumulator, which is stored as +inf or -inf and
+ * ranked as such.  To know, the call synchronises `stream` once at the end. */
+int xvb_topk_merge(const float* S, int64_t lds, int64_t rows, int64_t ncols, int64_t col0, int k, float* top_score,
+                   int64_t* top_idx, uint64_t* nan_row, void* stream);
+/* Bytes of the slab buffer xvb_retrieve_topk needs (M * slab_cols * 4), or XVB_EINVAL. */
+int64_t xvb_retrieve_topk_slab_bytes(int64_t M, int64_t slab_cols);
+int xvb_retrieve_topk(const float* a, int64_t M, const float* b, int64_t N, int K, const float* row_bias,
+                      const float* col_bias, int k, float* slab, int64_t slab_cols, float* out_score, int64_t* out_idx,
+                      void* stream);
+
 /* ---------------------------------------------------------------------------------------------
  * Whole-model extractor (x-vector TDNN family): owns packed weights + workspace on the current
  * device; replaces Xvector.extract_embedding (pytorch/model/xvector.py:77-98) for a whole batch
