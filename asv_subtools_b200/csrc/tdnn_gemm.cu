@@ -210,7 +210,7 @@ __device__ __noinline__ void epi_zero_row(const TdnnGemmParams& p, long long gro
 // barriers.  The CTA's head holds %globaltimer and clock64 at its start and at each warpgroup's end, which gives the
 // clock's rate.  Plain stores: a printf or any other call would serialise the MMAs (C7510).
 #ifdef XVB_TILE_TIMELINE
-#define XVB_TL(...) __VA_ARGS__
+#define XVB_TL(...) __VA_ARGS__   // host side: the plan's timeline fields
 constexpr int kTimelineHead = 8, kTimelineRec = 12;
 static unsigned long long* g_timeline = nullptr;
 static int g_timeline_tiles = 0;
@@ -220,218 +220,251 @@ __device__ __forceinline__ unsigned long long global_timer() {
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
+// keep the fused pooling epilogue on its general path (tile_timeline.py --direct-stores)
+__device__ __forceinline__ bool timeline_general(const TdnnGemmParams& p) { return p.timeline_general; }
+struct TileClock {
+  unsigned long long* cta;   // this CTA's part of the buffer, or NULL
+  long long start = 0, first = 0, issued = 0, retired = 0, wait = 0, w0 = 0, t = 0;
+  long long ep[4] = {0, 0, 0, 0};   // epilogue sub-phases: TMA read wait, coefficients + barrier, arithmetic, store issue
+  __device__ __forceinline__ explicit TileClock(const TdnnGemmParams& p)
+      : cta(p.timeline ? p.timeline + (size_t)blockIdx.x * (kTimelineHead + (size_t)kTimelineRec * p.timeline_tiles)
+                       : nullptr) {
+    if (cta && threadIdx.x == 0) { cta[0] = global_timer(); cta[1] = (unsigned long long)clock64(); }
+  }
+  __device__ __forceinline__ void tile_start() { start = clock64(); wait = 0; ep[0] = ep[1] = ep[2] = ep[3] = 0; }
+  __device__ __forceinline__ void wait_begin() { w0 = clock64(); }
+  __device__ __forceinline__ void wait_end(bool first_stage) {
+    const long long w1 = clock64();
+    wait += w1 - w0;
+    first = first_stage ? w1 : first;
+  }
+  __device__ __forceinline__ void mmas_issued() { issued = clock64(); }
+  __device__ __forceinline__ void mmas_retired() { retired = clock64(); t = retired; }
+  __device__ __forceinline__ void mark(int ph) { const long long now = clock64(); ep[ph] += now - t; t = now; }
+  __device__ __forceinline__ void flush(const TdnnGemmParams& p, int tj, int wg) const {
+    if (cta && (threadIdx.x & 127) == 0 && tj < p.timeline_tiles) {
+      unsigned long long* r = cta + kTimelineHead + (size_t)kTimelineRec * tj;
+      r[0] = (unsigned long long)start; r[1] = (unsigned long long)first; r[2] = (unsigned long long)issued;
+      r[3] = (unsigned long long)retired; r[4] = (unsigned long long)clock64(); r[5] = (unsigned long long)wait;
+      r[6] = (unsigned long long)wg; r[7] = 1ull;
+      for (int ph = 0; ph < 4; ++ph) r[8 + ph] = (unsigned long long)ep[ph];
+    }
+  }
+  __device__ __forceinline__ void end(int wg) const {
+    if (cta && (threadIdx.x & 127) == 0) { cta[2 + 2 * wg] = global_timer(); cta[3 + 2 * wg] = (unsigned long long)clock64(); }
+  }
+};
 #else
 #define XVB_TL(...)
+__device__ __forceinline__ bool timeline_general(const TdnnGemmParams&) { return false; }
+struct TileClock {
+  __device__ __forceinline__ explicit TileClock(const TdnnGemmParams&) {}
+  __device__ __forceinline__ void tile_start() {}
+  __device__ __forceinline__ void wait_begin() {}
+  __device__ __forceinline__ void wait_end(bool) {}
+  __device__ __forceinline__ void mmas_issued() {}
+  __device__ __forceinline__ void mmas_retired() {}
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void flush(const TdnnGemmParams&, int, int) const {}
+  __device__ __forceinline__ void end(int) const {}
+};
 #endif
 
+// A position in the ring of operand stages.  Full and empty barriers are waited on by phase parity.
+template <int kStages>
+struct RingPos {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void next() { if (++stage == kStages) { stage = 0; phase ^= 1; } }
+  __device__ __forceinline__ void skip(int n) {
+    stage += n;
+    phase ^= (uint32_t)(stage / kStages) & 1u;
+    stage %= kStages;
+  }
+  // the stage before `stage`, whose MMAs retire next.  Derived rather than carried: the ping-pong main loop has no
+  // register to spare.
+  __device__ __forceinline__ int before() const { return stage == 0 ? kStages - 1 : stage - 1; }
+};
+
+// The epilogue switches of p.flags.
+struct EpiFlags {
+  bool bn, act_sigmoid, act_tanh;
+  float relu_floor;   // branch-free ReLU switch
+  __device__ __forceinline__ explicit EpiFlags(int flags)
+      : bn((flags & XVB_BN) != 0), act_sigmoid((flags & XVB_SIGMOID) != 0), act_tanh((flags & XVB_TANH) != 0),
+        relu_floor((flags & XVB_RELU) != 0 ? 0.f : -INFINITY) {}
+  // The layer epilogues' chain after the pre-activation sum: ReLU -> swish -> BN -> tanh / sigmoid.
+  template <bool kSwish>
+  __device__ __forceinline__ float activate(float v, float scale, float shift) const {
+    v = fmaxf(v, relu_floor);
+    if constexpr (kSwish) v = v / (1.f + expf(-v));
+    if (bn) v = fmaf(v, scale, shift);
+    if (act_tanh) v = epi_tanh(v);
+    if (act_sigmoid) v = epi_sigmoid(v);
+    return v;
+  }
+};
+
+// Fused pooling: one output channel's bias, scale and shift, and the value it pools, BN(ReLU(acc + bias)).
+struct PoolChannel {
+  bool valid;
+  float bias, scale, shift;
+  __device__ __forceinline__ PoolChannel(const TdnnGemmParams& p, int c, bool bn)
+      : valid(c < p.Cout), bias((valid && p.bias) ? __ldg(p.bias + c) : 0.f), scale((valid && bn) ? __ldg(p.scale + c) : 1.f),
+        shift((valid && bn) ? __ldg(p.shift + c) : 0.f) {}
+  __device__ __forceinline__ float operator()(float acc, float relu_floor) const {
+    return fmaf(fmaxf(acc + bias, relu_floor), scale, shift);
+  }
+};
+
+// Fused trial histogram (scoring.cu): score -> bin -> shared-memory counter of its class (same / different speaker).
+// The 16 KB slab holds 2 x hist_bins u32 counters; out-of-window scores (the vast majority in a zoomed pass) are counted
+// branch-free in registers.
+struct TrialHistogram {
+  uint32_t slab;
+  uint32_t below[2] = {0u, 0u}, above[2] = {0u, 0u};
+  uint32_t tiles = 0;
+  __device__ __forceinline__ explicit TrialHistogram(const uint8_t* slab_base) : slab(smem_u32(slab_base)) {}
+  __device__ __forceinline__ void clear(const TdnnGemmParams& p) const {
+    for (int e = threadIdx.x; e < 2 * p.hist_bins; e += kNumConsumers)
+      asm volatile("st.shared.u32 [%0], %1;" ::"r"(slab + e * 4), "r"(0u) : "memory");
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+  template <int BLOCK_N>
+  __device__ __forceinline__ void count(const TdnnGemmParams& p, const float (&acc)[BLOCK_N / 2], int b0, int t0, int n0,
+                                        int row0) {
+    const int q4 = threadIdx.x & 3;
+    const float top = (float)(p.hist_bins - 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row0 + 8 * h;
+      const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
+      const bool valid = (b < p.B) && (t < p.T);
+      const float rbias = (p.row_bias && valid) ? __ldg(p.row_bias + (long long)b * p.T + t) : 0.f;
+      const int lab_r = valid ? __ldg(p.row_label + b) : -1;
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = n0 + 8 * i + 2 * q4 + e;
+          const bool in = c < p.Cout;
+          const uint32_t ok = (valid && in && (!p.hist_sym || c > b)) ? 1u : 0u;
+          const float sc = acc[4 * i + 2 * h + e] + ((in && p.bias) ? __ldg(p.bias + c) : 0.f) + rbias;
+          const float x = (sc - p.hist_lo) * p.hist_inv_w;
+          const uint32_t cls = (in && __ldg(p.col_label + c) == lab_r) ? 1u : 0u;
+          const uint32_t bl = x < 0.f ? ok : 0u;
+          const uint32_t ab = !(x < top) ? ok : 0u;          // also catches NaN
+          below[0] += bl & (cls ^ 1u); below[1] += bl & cls;
+          above[0] += ab & (cls ^ 1u); above[1] += ab & cls;
+          if (ok & ~(bl | ab))
+            asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(slab + ((int)cls * p.hist_bins + 1 + (int)x) * 4), "r"(1u) : "memory");
+        }
+      }
+    }
+    if ((++tiles & 0x3fffu) == 0) flush(p);   // u32 counters: <= 2^14 tiles x 2^14 scores between flushes
+  }
+  // adds the slab and the register counts to p.hist and clears them
+  __device__ __forceinline__ void flush(const TdnnGemmParams& p) {
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      if (below[c]) asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(slab + (c * p.hist_bins) * 4), "r"(below[c]) : "memory");
+      if (above[c]) asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(slab + (c * p.hist_bins + p.hist_bins - 1) * 4), "r"(above[c]) : "memory");
+      below[c] = 0u; above[c] = 0u;
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    for (int e = threadIdx.x; e < 2 * p.hist_bins; e += kNumConsumers) {
+      uint32_t c;
+      asm volatile("ld.shared.u32 %0, [%1];" : "=r"(c) : "r"(slab + e * 4) : "memory");
+      if (c) {
+        atomicAdd(p.hist + e, (unsigned long long)c);
+        asm volatile("st.shared.u32 [%0], %1;" ::"r"(slab + e * 4), "r"(0u) : "memory");
+      }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+  }
+};
+
+// The roles of one instance of the layer kernel: the TMA producer, the consumers' main loop and their epilogues.
+//
 // kSwish: the layer epilogue applies x * sigmoid(x) after the ReLU (XVB_SWISH).  A template flag rather than a runtime
 // one, so that the instantiations without it compile to the same code as before the flag existed.
 //
-// Ping-pong (the 128-wide layer and fused-pooling instances): tile j of the CTA's list (blockIdx.x + j * gridDim.x)
-// belongs to warpgroup j & 1, which computes all 128 of its rows as two m64 halves.  Each warpgroup finds its place in
-// the operand ring from a running count of the K blocks of all the CTA's tiles, the other warpgroup's included.  Both
-// wait on the ring's full barriers by phase parity, which only tells the phase being waited for from the one before it:
-// a warpgroup that started waiting on its next tile's first stage while the producer was still more than one lap of
-// the ring behind would take an older load of that stage for its own.  So the main loops take turns on named barriers
-// 2 + wg ("warpgroup wg may start its main loop"): a warpgroup starts one only after the other has issued the previous
-// tile's MMAs, and the epilogue of that tile then runs under the other's main loop.
-template <int BLOCK_N, bool kPool, bool kHist, bool kSwish = false>
-__global__ void __launch_bounds__(gemm_threads<BLOCK_N, kHist, kSwish>(), 1)
-tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                        const __grid_constant__ CUtensorMap map_a2_hi, const __grid_constant__ CUtensorMap map_a2_lo,
-                        const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                        const __grid_constant__ CUtensorMap map_y_hi, const __grid_constant__ CUtensorMap map_y_lo,
-                        const __grid_constant__ TdnnGemmParams p) {
+// Every function is force-inlined: a call would serialise every wgmma of the kernel (C7510).
+template <int BLOCK_N, bool kPool, bool kHist, bool kSwish>
+struct LayerKernel {
   // the staged epilogue moves 64-channel boxes; the 32-wide instances keep the direct stores
-  constexpr bool kStaged = staged_epilogue<BLOCK_N, kPool, kHist>();
+  static constexpr bool kStaged = staged_epilogue<BLOCK_N, kPool, kHist>();
   using Cfg = GemmCfg<BLOCK_N, kPool, kHist>;
-  constexpr int kStages = Cfg::kStages;
-  constexpr int kBBytes = Cfg::kBBytes;
-  constexpr int kStageBytes = Cfg::kStageBytes;
+  static constexpr int kStages = Cfg::kStages;
+  static constexpr int kBBytes = Cfg::kBBytes;
+  static constexpr int kStageBytes = Cfg::kStageBytes;
+  static constexpr int kAccRegs = Cfg::kAccRegs;
   static_assert(!kPool || BLOCK_N == kBlockM, "fused pooling: 128 channels x 128 frames per tile");
-  constexpr bool kPingPong = ping_pong<BLOCK_N, kHist, kSwish>();
-  constexpr int kHalves = kPingPong ? 2 : 1;                  // 64-row accumulator halves per consumer thread
-  constexpr int kReleaseWarps = kPingPong ? 4 : kNumConsumers / 32;   // warps that consume (and release) one stage
+  static constexpr bool kPingPong = ping_pong<BLOCK_N, kHist, kSwish>();
+  static constexpr int kHalves = kPingPong ? 2 : 1;                          // 64-row accumulator halves per consumer thread
+  static constexpr int kReleaseWarps = kPingPong ? 4 : kNumConsumers / 32;   // warps that consume (and release) one stage
+  using Acc = float[kHalves][kAccRegs];
+  using Ring = RingPos<kStages>;
 
-  extern __shared__ uint8_t smem_raw[];
-  // SWIZZLE_128B tiles need 1024-byte alignment
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* slab_base = smem + kStages * kStageBytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slab_base + Cfg::kTailBytes);
-  uint64_t* empty_bar = full_bar + kStages;
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == kProducerWarp && lane == 0) {
-    tma_prefetch_desc(&map_a_hi);
-    tma_prefetch_desc(&map_a_lo);
-    tma_prefetch_desc(&map_w_hi);
-    tma_prefetch_desc(&map_w_lo);
-    if ((kStaged || kPool) && p.tma_store) {
-      tma_prefetch_desc(&map_y_hi);
-      tma_prefetch_desc(&map_y_lo);
-    }
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(&full_bar[i], 1);                   // producer arrival + all TMA bytes
-      mbar_init(&empty_bar[i], kReleaseWarps);      // one arrival per consumer warp of the stage's warpgroup(s)
-    }
-    fence_barrier_init();
+  // The epilogues take the halves one after the other through the same code on acc[0] (a rolled loop): unrolled over
+  // both, the ping-pong instances' code was twice as large, more than the instruction cache holds.
+  static __device__ __forceinline__ void half_down(Acc& acc) {
+#pragma unroll
+    for (int i = 0; i < kAccRegs; ++i) acc[0][i] = acc[kHalves - 1][i];
   }
-  __syncthreads();
-  // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) may overlap the
-  // tail of the previous kernel in the stream; its results are needed from here on.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  // the previous kernel may have written our operands with ordinary (generic-proxy) stores -- the staging
-  // / pooling kernels do -- while we read them through TMA (async proxy): order the two proxies explicitly,
-  // a kernel boundary would have done it for us
-  asm volatile("fence.proxy.async;" ::: "memory");
 
-  const int num_kblk = p.num_src * p.ntaps * p.num_cblk;
-
-  if (warp >= kProducerWarp) {
-    // ================================ TMA producer ================================
-    if constexpr (kPingPong) setmaxnreg_dec<kProducerRegs>();   // the whole producer warpgroup
-    if (warp == kProducerWarp && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-        int m_unit, n_blk, slice;
-        if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;   // e.g. entirely on or below the diagonal
-        const int cb_begin = slice * p.kb_per_slice;                        // (0, num_cblk) unless split-K
-        const int cb_end = p.k_slices > 1 ? min(p.num_cblk, cb_begin + p.kb_per_slice) : p.num_cblk;
-        const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;  // may be fully out of
-        const int n0 = n_blk * BLOCK_N;                                                    // range: TMA zero-fills
-        const int a_c0 = p.group_ng ? (n0 / p.group_ng) * p.group_kg : 0;                  // grouped: this group's K slice
-        for (int src = 0; src < p.num_src; ++src) {
-          const CUtensorMap* ma_hi = src == 0 ? &map_a_hi : &map_a2_hi;
-          const CUtensorMap* ma_lo = src == 0 ? &map_a_lo : &map_a2_lo;
-          for (int tap = 0; tap < p.ntaps; ++tap) {
-            const int tt = t0 + p.ctx[tap];
-            for (int cb = cb_begin; cb < cb_end; ++cb) {
-              mbar_wait(&empty_bar[stage], phase ^ 1);
-              uint8_t* s = smem + stage * kStageBytes;
-              const int kw = tap * p.cin_p16 + cb * kBlockK;
-              mbar_expect_tx(&full_bar[stage], kStageBytes);
-              tma_load_3d(s, ma_hi, &full_bar[stage], a_c0 + cb * kBlockK, tt, b0);
-              tma_load_3d(s + kABytes, ma_lo, &full_bar[stage], a_c0 + cb * kBlockK, tt, b0);
-              tma_load_2d(s + 2 * kABytes, &map_w_hi, &full_bar[stage], kw, n0);
-              tma_load_2d(s + 2 * kABytes + kBBytes, &map_w_lo, &full_bar[stage], kw, n0);
-              if (++stage == kStages) { stage = 0; phase ^= 1; }
-            }
+  // ================================ TMA producer (one thread) ================================
+  static __device__ __forceinline__ void produce(const TdnnGemmParams& p, uint8_t* smem, uint64_t* full_bar,
+                                                 uint64_t* empty_bar, const CUtensorMap* map_a_hi,
+                                                 const CUtensorMap* map_a_lo, const CUtensorMap* map_a2_hi,
+                                                 const CUtensorMap* map_a2_lo, const CUtensorMap* map_w_hi,
+                                                 const CUtensorMap* map_w_lo) {
+    Ring ring;
+    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      int m_unit, n_blk, slice;
+      if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;   // e.g. entirely on or below the diagonal
+      const int cb_begin = slice * p.kb_per_slice;                        // (0, num_cblk) unless split-K
+      const int cb_end = p.k_slices > 1 ? min(p.num_cblk, cb_begin + p.kb_per_slice) : p.num_cblk;
+      const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;  // may be fully out of
+      const int n0 = n_blk * BLOCK_N;                                                    // range: TMA zero-fills
+      const int a_c0 = p.group_ng ? (n0 / p.group_ng) * p.group_kg : 0;                  // grouped: this group's K slice
+      for (int src = 0; src < p.num_src; ++src) {
+        const CUtensorMap* ma_hi = src == 0 ? map_a_hi : map_a2_hi;
+        const CUtensorMap* ma_lo = src == 0 ? map_a_lo : map_a2_lo;
+        for (int tap = 0; tap < p.ntaps; ++tap) {
+          const int tt = t0 + p.ctx[tap];
+          for (int cb = cb_begin; cb < cb_end; ++cb) {
+            mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+            uint8_t* s = smem + ring.stage * kStageBytes;
+            const int kw = tap * p.cin_p16 + cb * kBlockK;
+            mbar_expect_tx(&full_bar[ring.stage], kStageBytes);
+            tma_load_3d(s, ma_hi, &full_bar[ring.stage], a_c0 + cb * kBlockK, tt, b0);
+            tma_load_3d(s + kABytes, ma_lo, &full_bar[ring.stage], a_c0 + cb * kBlockK, tt, b0);
+            tma_load_2d(s + 2 * kABytes, map_w_hi, &full_bar[ring.stage], kw, n0);
+            tma_load_2d(s + 2 * kABytes + kBBytes, map_w_lo, &full_bar[ring.stage], kw, n0);
+            ring.next();
           }
         }
       }
     }
-    return;
   }
 
-  // ================================ consumers: wgmma + epilogue ================================
-  if constexpr (kPingPong) setmaxnreg_inc<kConsumerRegs>();
-  const int wg = warp >> 2;                         // split tiles: accumulator rows 64*wg .. 64*wg+63
-  const int q4 = lane & 3;
-  const int row_base = kPingPong ? 0 : 64 * wg;      // first accumulator row of this warpgroup's (first) half
-  // this thread's rows: row0 + 64 * hh + 8 * h for half hh < kHalves and h < 2
-  const int row0 = row_base + 16 * (warp & 3) + (lane >> 2);
-  const int etid = threadIdx.x;                      // 0..255
-  const bool relu = (p.flags & XVB_RELU) != 0;
-  const bool bn = (p.flags & XVB_BN) != 0;
-  const bool act_sigmoid = (p.flags & XVB_SIGMOID) != 0;
-  const bool act_tanh = (p.flags & XVB_TANH) != 0;
-  const float relu_floor = relu ? 0.f : -INFINITY;   // branch-free ReLU switch
-  float acc[kHalves][Cfg::kAccRegs];
-#pragma unroll
-  for (int hh = 0; hh < kHalves; ++hh)
-#pragma unroll
-    for (int i = 0; i < Cfg::kAccRegs; ++i) acc[hh][i] = 0.f;
-  // The epilogues take the halves one after the other through the same code on acc[0] (a rolled loop): unrolled over
-  // both, the ping-pong instances' code was twice as large, more than the instruction cache holds.
-  auto half_down = [&]() {
-#pragma unroll
-    for (int i = 0; i < Cfg::kAccRegs; ++i) acc[0][i] = acc[kHalves - 1][i];
-  };
-  int stage = 0;
-  uint32_t phase = 0;
-  uint32_t it = 0;
-
-  // fused trial histogram: the 16 KB slab holds 2 x hist_bins u32 counters
-  uint32_t h_below[2] = {0u, 0u}, h_above[2] = {0u, 0u};   // out-of-window scores: counted in registers
-  const uint32_t hslab = smem_u32(slab_base);
-  auto hist_flush = [&]() {
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      if (h_below[c]) asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(hslab + (c * p.hist_bins) * 4), "r"(h_below[c]) : "memory");
-      if (h_above[c]) asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(hslab + (c * p.hist_bins + p.hist_bins - 1) * 4), "r"(h_above[c]) : "memory");
-      h_below[c] = 0u; h_above[c] = 0u;
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    for (int e = etid; e < 2 * p.hist_bins; e += kNumConsumers) {
-      uint32_t c;
-      asm volatile("ld.shared.u32 %0, [%1];" : "=r"(c) : "r"(hslab + e * 4) : "memory");
-      if (c) {
-        atomicAdd(p.hist + e, (unsigned long long)c);
-        asm volatile("st.shared.u32 [%0], %1;" ::"r"(hslab + e * 4), "r"(0u) : "memory");
-      }
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-  };
-  if constexpr (kHist) {
-    for (int e = etid; e < 2 * p.hist_bins; e += kNumConsumers)
-      asm volatile("st.shared.u32 [%0], %1;" ::"r"(hslab + e * 4), "r"(0u) : "memory");
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-  }
-
-  XVB_TL(
-    long long tl_start = 0, tl_first = 0, tl_issued = 0, tl_retired = 0, tl_wait = 0;
-    long long tl_ep[4] = {0, 0, 0, 0};                 // epilogue sub-phases: TMA read wait, coefficients + barrier, arithmetic, store issue
-    long long tl_t = 0;
-    auto tl_mark = [&](int ph) { const long long t = clock64(); tl_ep[ph] += t - tl_t; tl_t = t; };
-    unsigned long long* tl_cta = p.timeline ? p.timeline + (size_t)blockIdx.x * (kTimelineHead + (size_t)kTimelineRec * p.timeline_tiles) : nullptr;
-    if (tl_cta && threadIdx.x == 0) { tl_cta[0] = global_timer(); tl_cta[1] = (unsigned long long)clock64(); }
-  )
-  int tj = 0;                                        // index of the tile in the CTA's list
-  XVB_TL(auto tl_flush = [&]() {
-    if (tl_cta && (threadIdx.x & 127) == 0 && tj < p.timeline_tiles) {
-      unsigned long long* r = tl_cta + kTimelineHead + (size_t)kTimelineRec * tj;
-      r[0] = (unsigned long long)tl_start; r[1] = (unsigned long long)tl_first; r[2] = (unsigned long long)tl_issued;
-      r[3] = (unsigned long long)tl_retired; r[4] = (unsigned long long)clock64(); r[5] = (unsigned long long)tl_wait;
-      r[6] = (unsigned long long)wg; r[7] = 1ull;
-      for (int ph = 0; ph < 4; ++ph) r[8 + ph] = (unsigned long long)tl_ep[ph];
-    }
-  };)
-  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tj) {
-    int m_unit, n_blk, slice;
-    if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;
-    int kb_begin = 0, kb_end = num_kblk;
-    if (p.k_slices > 1) {
-      kb_begin = slice * p.kb_per_slice;
-      kb_end = min(num_kblk, kb_begin + p.kb_per_slice);
-    }
-    if constexpr (kPingPong) {
-      if ((tj & 1) != wg) {                          // the other warpgroup's tile: skip its stages in the ring
-        stage += kb_end - kb_begin;
-        phase ^= (uint32_t)(stage / kStages) & 1u;
-        stage %= kStages;
-        continue;
-      }
-      if (tj > 0) {
-        // fused pooling: the warpgroup's previous TMA store has read the staging buffer, for all its threads past here
-        if (kPool && (threadIdx.x & 127) == 0) tma_store_wait_read<0>();
-        asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
-      }
-    }
-    ++it;
-    XVB_TL(tl_start = clock64(); tl_wait = 0; tl_ep[0] = tl_ep[1] = tl_ep[2] = tl_ep[3] = 0;)
-    // ---- main loop: one k block (64 channels of one tap and source) per operand stage
-    // The stage before `stage` in the ring is the one whose MMAs retire next.  It is derived, and so is the tile's
-    // first MMA (which overwrites the accumulators), rather than carried: the ping-pong main loop has no register to spare.
-    auto stage_before = [&]() { return stage == 0 ? kStages - 1 : stage - 1; };
+  // ================================ consumer main loop ================================
+  // One tile's K blocks [kb_begin, kb_end), one (64 channels of one tap and source) per operand stage from `ring` on.
+  // Returns with the accumulators retired and the last stage released.  Ping-pong: once this tile's MMAs are issued, the
+  // warpgroup of the CTA's next tile (if any) may start its main loop (named barrier 3 - wg).
+  static __device__ __forceinline__ void main_loop(const TdnnGemmParams& p, Acc& acc, uint8_t* smem, uint64_t* full_bar,
+                                                   uint64_t* empty_bar, Ring& ring, int kb_begin, int kb_end, int tile,
+                                                   int wg, TileClock& clk) {
+    const int lane = threadIdx.x & 31;
+    const int row_base = kPingPong ? 0 : 64 * wg;   // first accumulator row of this warpgroup's (first) half
+    // The tile's first MMA (which overwrites the accumulators) is derived from kb, not carried, as is ring.before().
     for (int kb = kb_begin; kb < kb_end; ++kb) {
-      XVB_TL(const long long tl_w0 = clock64();)
-      mbar_wait(&full_bar[stage], phase);
-      XVB_TL(const long long tl_w1 = clock64(); tl_wait += tl_w1 - tl_w0; tl_first = kb == kb_begin ? tl_w1 : tl_first;)
-      const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+      clk.wait_begin();
+      mbar_wait(&full_bar[ring.stage], ring.phase);
+      clk.wait_end(kb == kb_begin);
+      const uint32_t sa = smem_u32(smem + ring.stage * kStageBytes);
       const uint64_t dx_hi = make_sw128_desc(sa), dx_lo = make_sw128_desc(sa + kABytes);
       const uint64_t dw_hi = make_sw128_desc(sa + 2 * kABytes), dw_lo = make_sw128_desc(sa + 2 * kABytes + kBBytes);
       // M side: 64 rows per half (8 KB each into the 128-row tile); N side: the whole other tile
@@ -456,275 +489,246 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
       }
       wgmma_commit();
       wgmma_wait<1>();                               // the previous stage's MMAs have retired: release it
-      if (kb != kb_begin && lane == 0) mbar_arrive(&empty_bar[stage_before()]);
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      if (kb != kb_begin && lane == 0) mbar_arrive(&empty_bar[ring.before()]);
+      ring.next();
     }
     // the next tile's warpgroup may start its main loop
     if (kPingPong && tile + gridDim.x < p.num_tiles) asm volatile("bar.arrive %0, 256;" ::"r"(3 - wg) : "memory");
-    XVB_TL(tl_issued = clock64();)
+    clk.mmas_issued();
     wgmma_wait<0>();
-    XVB_TL(tl_retired = clock64(); tl_t = tl_retired;)
+    clk.mmas_retired();
 #pragma unroll
     for (int hh = 0; hh < kHalves; ++hh) wgmma_fence_operands(acc[hh]);
-    if (kb_end > kb_begin && lane == 0) mbar_arrive(&empty_bar[stage_before()]);
+    if (kb_end > kb_begin && lane == 0) mbar_arrive(&empty_bar[ring.before()]);
+  }
 
-    const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;
-    const int n0 = n_blk * BLOCK_N;
+  // ================================ fused statistics pooling epilogue ================================
+  // Rows = channels, columns = the tile's 128 frames.  Time block g of the tile is columns [g*Tb, (g+1)*Tb) = utterance
+  // b0+g, frames t0.. ; the first nv of them exist.
+  //
+  // Full 8-frame time blocks (Tb == 8 and all 8 frames exist; uniform per tile) stage the tile's partials in the
+  // warpgroup's 16 KB, [utterance][mean | M2][128 channels] fp32, and one thread stores them with one TMA store through
+  // the (Cout, 2, B, time block) map of pool_partial, whose extents clip the channels past Cout and the utterances past
+  // B.  The previous tile's store has read the buffer: its thread waited for that before the turn barrier of this
+  // tile's main loop.
+  static __device__ __forceinline__ bool pool_full_blocks(const TdnnGemmParams& p, int nv) {
+    return p.tma_store && p.Tb == 8 && nv == 8 && !timeline_general(p);
+  }
 
-    if constexpr (kPool) {
-      // ---- fused statistics pooling: rows = channels, columns = the tile's 128 frames.  Time block g of the
-      // tile is columns [g*Tb, (g+1)*Tb) = utterance b0+g, frames t0.. ; the first nv of them exist.
-      int nv = p.T - t0;
-      nv = nv < 0 ? 0 : (nv > p.Tb ? p.Tb : nv);
-      const int tblk = m_unit % p.num_t_blk;
-      const int gl = p.Tb < 8 ? p.Tb : 8;              // columns of one group inside one 8-column chunk
-      // Full 8-frame time blocks (below) stage the tile's partials in the warpgroup's 16 KB, [utterance][mean | M2][128
-      // channels] fp32, and one thread stores them with one TMA store through the (Cout, 2, B, time block) map of
-      // pool_partial, whose extents clip the channels past Cout and the utterances past B.  The previous tile's store
-      // has read the buffer: its thread waited for that before the turn barrier of this tile's main loop.
+  static __device__ __forceinline__ void pool_epilogue(const TdnnGemmParams& p, Acc& acc, uint8_t* slab_base, int b0,
+                                                       int t0, int tblk, int n0, int row0, int wg, const EpiFlags& f,
+                                                       const CUtensorMap* map_pool, TileClock& clk) {
+    int nv = p.T - t0;
+    nv = nv < 0 ? 0 : (nv > p.Tb ? p.Tb : nv);
 #pragma unroll 1
-      for (int hh = 0; hh < kHalves; ++hh) {
-      if (hh > 0) half_down();
+    for (int hh = 0; hh < kHalves; ++hh) {
+      if (hh > 0) half_down(acc);
       // opaque per half: hoisted out of the rolled loop, the store addresses and validity masks derived from them
       // stayed live through both halves and spilled
       int b0h = b0, nvh = nv;
       asm volatile("" : "+r"(b0h), "+r"(nvh));
-      // Full 8-frame time blocks (Tb == 8 and all 8 frames exist; uniform per tile): block i of the tile is exactly the
-      // 8-column chunk i, and every Chan merge in it has known counts, so the divisions fold.  With chan_merge's names:
-      //   pair into the empty summary: n = 0, nb = tot = 2, wb = 1: d = pm - 0 = pm, mean = fmaf(pm, 1, 0) = pm + 0 (a -0
-      //     becomes +0), m2 = 0 + (pm2 + pm * pm * 0 * 1) = pm2, since pm2 >= 0 and the product is +0 on finite data;
-      //   lanes q4 ^ 1: n = nb = 2, tot = 4, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 2 * 0.5;
-      //   lanes q4 ^ 2: n = nb = 4, tot = 8, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 4 * 0.5.
-      // Every operation that rounds is kept, in chan_merge's order (the two multiplications by powers of two as well:
-      // they are exact except where d * d * n overflows, and there they give what chan_merge gives), so the partials
-      // are bit-identical to the general path's on finite data.  No summary carries from one chunk to the next, so
-      // the 16 chunks of a row are independent chains that the compiler interleaves.
-      if (p.tma_store && p.Tb == 8 && nvh == 8 XVB_TL(&& !p.timeline_general)) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
-          const bool cvalid = cch < p.Cout;
-          const float bias_c = (cvalid && p.bias) ? __ldg(p.bias + cch) : 0.f;
-          const float scale_c = (cvalid && bn) ? __ldg(p.scale + cch) : 1.f;
-          const float shift_c = (cvalid && bn) ? __ldg(p.shift + cch) : 0.f;
-          int tid = threadIdx.x;                          // opaque, as b0h: derived per use, not kept live
-          asm volatile("" : "+r"(tid));
-          const uint32_t dst0 = smem_u32(slab_base) + (tid >> 7) * kStageOutBytes +
-                                4 * (16 * ((tid >> 5) & 3) + ((tid & 31) >> 2) + 64 * hh + 8 * h);
-#pragma unroll
-          for (int i = 0; i < BLOCK_N / 8; ++i) {
-            const float x0 = fmaf(fmaxf(acc[0][4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
-            const float x1 = fmaf(fmaxf(acc[0][4 * i + 2 * h + 1] + bias_c, relu_floor), scale_c, shift_c);
-            float mean = 0.5f * (x0 + x1) + 0.f;
-            float m2 = 0.5f * (x0 - x1) * (x0 - x1);
-            float d = __shfl_xor_sync(0xffffffffu, mean, 1) - mean;
-            float m2b = __shfl_xor_sync(0xffffffffu, m2, 1);
-            mean = fmaf(d, 0.5f, mean);
-            m2 += m2b + d * d * 2.f * 0.5f;
-            d = __shfl_xor_sync(0xffffffffu, mean, 2) - mean;
-            m2b = __shfl_xor_sync(0xffffffffu, m2, 2);
-            mean = fmaf(d, 0.5f, mean);
-            m2 += m2b + d * d * 4.f * 0.5f;
-            if (q4 == 0) {
-              st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i, mean);
-              st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i + 4 * BLOCK_N, m2);
-            }
-          }
-        }
-        XVB_TL(tl_mark(2);)
+      if (pool_full_blocks(p, nvh)) {
+        pool_full_block_half(p, acc[0], slab_base, hh, n0 + row0 + 64 * hh, f);
+        clk.mark(2);
         continue;
       }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int cch = n0 + row0 + 64 * hh + 8 * h;   // this thread's output channel
-        const bool cvalid = cch < p.Cout;
-        const float bias_c = (cvalid && p.bias) ? __ldg(p.bias + cch) : 0.f;
-        const float scale_c = (cvalid && bn) ? __ldg(p.scale + cch) : 1.f;
-        const float shift_c = (cvalid && bn) ? __ldg(p.shift + cch) : 0.f;
-        auto emit = [&](int col, float mean, float m2) {
-          const int bb = b0h + (col >> p.log2_tb);
-          if (cvalid && bb < p.B) {
-            float* dst = p.pool_partial + ((long long)tblk * p.B + bb) * (2LL * p.Cout) + cch;
-            dst[0] = mean;
-            dst[p.Cout] = m2;
-          }
-        };
-        float rn = 0.f, rmean = 0.f, rm2 = 0.f;
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / 8; ++i) {
-          const int col = 8 * i + 2 * q4;
-          const float x0 = fmaf(fmaxf(acc[0][4 * i + 2 * h] + bias_c, relu_floor), scale_c, shift_c);
-          const float x1 = fmaf(fmaxf(acc[0][4 * i + 2 * h + 1] + bias_c, relu_floor), scale_c, shift_c);
-          if (p.Tb == 1) {
-            if (nvh > 0) { emit(col, x0, 0.f); emit(col + 1, x1, 0.f); }
-            continue;
-          }
-          const int j = col & (p.Tb - 1);              // frame offset of x0 inside its time block
-          const bool v0 = j < nvh, v1 = j + 1 < nvh;
-          const float pn = (float)v0 + (float)v1;
-          const float pm = v1 ? 0.5f * (x0 + x1) : (v0 ? x0 : 0.f);
-          const float pm2 = v1 ? 0.5f * (x0 - x1) * (x0 - x1) : 0.f;
-          chan_merge(rn, rmean, rm2, pn, pm, pm2);
-          if (((col - 2 * q4 + 8) & (p.Tb - 1)) == 0) {  // a time block ends in this chunk (warp-uniform)
-            if (gl >= 4) chan_merge(rn, rmean, rm2, __shfl_xor_sync(0xffffffffu, rn, 1),
-                                    __shfl_xor_sync(0xffffffffu, rmean, 1), __shfl_xor_sync(0xffffffffu, rm2, 1));
-            if (gl >= 8) chan_merge(rn, rmean, rm2, __shfl_xor_sync(0xffffffffu, rn, 2),
-                                    __shfl_xor_sync(0xffffffffu, rmean, 2), __shfl_xor_sync(0xffffffffu, rm2, 2));
-            if (((2 * q4) & (gl - 1)) == 0 && rn > 0.f) emit(col & ~(p.Tb - 1), rmean, rm2);
-            rn = 0.f; rmean = 0.f; rm2 = 0.f;
-          }
-        }
-      }
-      }
-      XVB_TL(tl_mark(2);)
-      if (p.tma_store && p.Tb == 8 && nv == 8 XVB_TL(&& !p.timeline_general)) {
-        fence_proxy_async();                             // the staged partials become visible to the TMA unit
-        asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
-        XVB_TL(tl_mark(1);)
-        if ((threadIdx.x & 127) == 0) {
-          tma_store_4d(&map_y_hi, smem_u32(slab_base) + wg * kStageOutBytes, n0, 0, b0, tblk);
-          tma_store_commit();
-        }
-        XVB_TL(tl_mark(3);)
-      }
-      XVB_TL(tl_flush();)
-      continue;
+      pool_general_half(p, acc[0], b0h, nvh, tblk, n0 + row0 + 64 * hh, f);
     }
+    clk.mark(2);
+    if (pool_full_blocks(p, nv)) {
+      fence_proxy_async();                             // the staged partials become visible to the TMA unit
+      asm volatile("bar.sync %0, 128;" ::"r"(4 + wg) : "memory");
+      clk.mark(1);
+      if ((threadIdx.x & 127) == 0) {
+        tma_store_4d(map_pool, smem_u32(slab_base) + wg * kStageOutBytes, n0, 0, b0, tblk);
+        tma_store_commit();
+      }
+      clk.mark(3);
+    }
+  }
 
-    if constexpr (kHist) {
-      // trial histogram: score -> bin -> shared-memory counter of its class (same / different speaker).
-      // Branch-free counting of the out-of-window scores (the vast majority in a zoomed pass).
-      const float top = (float)(p.hist_bins - 2);
+  // Full 8-frame time blocks: block i of the tile is exactly the 8-column chunk i, and every Chan merge in it has known
+  // counts, so the divisions fold.  With chan_merge's names:
+  //   pair into the empty summary: n = 0, nb = tot = 2, wb = 1: d = pm - 0 = pm, mean = fmaf(pm, 1, 0) = pm + 0 (a -0
+  //     becomes +0), m2 = 0 + (pm2 + pm * pm * 0 * 1) = pm2, since pm2 >= 0 and the product is +0 on finite data;
+  //   lanes q4 ^ 1: n = nb = 2, tot = 4, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 2 * 0.5;
+  //   lanes q4 ^ 2: n = nb = 4, tot = 8, wb = 0.5: mean = fmaf(d, 0.5, mean), m2 += m2b + d * d * 4 * 0.5.
+  // Every operation that rounds is kept, in chan_merge's order (the two multiplications by powers of two as well: they
+  // are exact except where d * d * n overflows, and there they give what chan_merge gives), so the partials are
+  // bit-identical to the general path's on finite data.  No summary carries from one chunk to the next, so the 16
+  // chunks of a row are independent chains that the compiler interleaves.  `ch0`: this thread's first output channel.
+  static __device__ __forceinline__ void pool_full_block_half(const TdnnGemmParams& p, const float (&a)[kAccRegs],
+                                                              uint8_t* slab_base, int hh, int ch0, const EpiFlags& f) {
+    const int q4 = threadIdx.x & 3;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = row0 + 8 * h;
-        const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
-        const bool valid = (b < p.B) && (t < p.T);
-        const float rbias = (p.row_bias && valid) ? __ldg(p.row_bias + (long long)b * p.T + t) : 0.f;
-        const int lab_r = valid ? __ldg(p.row_label + b) : -1;
+    for (int h = 0; h < 2; ++h) {
+      const PoolChannel ch(p, ch0 + 8 * h, f.bn);
+      int tid = threadIdx.x;                          // opaque, as b0h: derived per use, not kept live
+      asm volatile("" : "+r"(tid));
+      const uint32_t dst0 = smem_u32(slab_base) + (tid >> 7) * kStageOutBytes +
+                            4 * (16 * ((tid >> 5) & 3) + ((tid & 31) >> 2) + 64 * hh + 8 * h);
 #pragma unroll
-        for (int i = 0; i < BLOCK_N / 8; ++i) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int c = n0 + 8 * i + 2 * q4 + e;
-            const bool in = c < p.Cout;
-            const uint32_t ok = (valid && in && (!p.hist_sym || c > b)) ? 1u : 0u;
-            const float sc = acc[0][4 * i + 2 * h + e] + ((in && p.bias) ? __ldg(p.bias + c) : 0.f) + rbias;
-            const float x = (sc - p.hist_lo) * p.hist_inv_w;
-            const uint32_t cls = (in && __ldg(p.col_label + c) == lab_r) ? 1u : 0u;
-            const uint32_t bl = x < 0.f ? ok : 0u;
-            const uint32_t ab = !(x < top) ? ok : 0u;          // also catches NaN
-            h_below[0] += bl & (cls ^ 1u); h_below[1] += bl & cls;
-            h_above[0] += ab & (cls ^ 1u); h_above[1] += ab & cls;
-            if (ok & ~(bl | ab))
-              asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(hslab + ((int)cls * p.hist_bins + 1 + (int)x) * 4), "r"(1u) : "memory");
-          }
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const float x0 = ch(a[4 * i + 2 * h], f.relu_floor);
+        const float x1 = ch(a[4 * i + 2 * h + 1], f.relu_floor);
+        float mean = 0.5f * (x0 + x1) + 0.f;
+        float m2 = 0.5f * (x0 - x1) * (x0 - x1);
+        float d = __shfl_xor_sync(0xffffffffu, mean, 1) - mean;
+        float m2b = __shfl_xor_sync(0xffffffffu, m2, 1);
+        mean = fmaf(d, 0.5f, mean);
+        m2 += m2b + d * d * 2.f * 0.5f;
+        d = __shfl_xor_sync(0xffffffffu, mean, 2) - mean;
+        m2b = __shfl_xor_sync(0xffffffffu, m2, 2);
+        mean = fmaf(d, 0.5f, mean);
+        m2 += m2b + d * d * 4.f * 0.5f;
+        if (q4 == 0) {
+          st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i, mean);
+          st_shared_f32(dst0 + 2 * 4 * BLOCK_N * i + 4 * BLOCK_N, m2);
         }
       }
-      if ((it & 0x3fffu) == 0) hist_flush();         // u32 counters: <= 2^14 tiles x 2^14 scores between flushes
-      continue;
     }
+  }
 
-    // ---- layer epilogue: +bias (+ row / utterance terms) -> ReLU -> swish -> BN -> tanh / sigmoid -> fp32 and/or split
-    // planes
-    // Column pairs outer, rows inner: a thread's two rows of a half share its columns, so bias, scale and shift are
-    // loaded once per column and half.
-    // Staged path (p.tma_store, one uniform branch per tile): a 64-row half leaves in pieces of 64 channels.  Per piece
-    // the warpgroup puts the 64 columns' bias, scale and shift into shared memory once, every thread applies the same
-    // arithmetic in the same order as the direct path below and writes its packed hi and lo pairs into the warpgroup's
-    // staging buffer, and one thread stores the two planes with TMA.  The buffer has the 128-byte swizzle of the store
-    // maps (16-byte chunk index ^ row & 7): a warp's eight rows fall into eight different chunks, so its stores do not
-    // conflict.  The maps' extents (Cout, T, B) clip the rows past T or B and the channels past Cout, so there are no
-    // tail branches; rows past an utterance's length are staged as zeros.
-    if constexpr (kStaged) {
-      if (p.tma_store) {
-        // Everything below derives from an opaque copy of the thread index, per tile: hoisted out of the tile loop, these
-        // addresses stayed live through the main loop, which has no register to spare, and spilled more.
-        int tid = threadIdx.x;
-        asm volatile("" : "+r"(tid));
-        const int wgo = tid >> 7, wtid = tid & 127, q4o = tid & 3;
-        const int prow = 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2);   // this thread's first row of a 64-row piece
-        const uint32_t stg = smem_u32(slab_base) + wgo * kStageOutBytes;
-        const uint32_t coefs = smem_u32(slab_base) + 2 * kStageOutBytes + wgo * kCoefBytes;
-        const int ebar = 4 + wgo;                         // named barrier of this warpgroup's epilogue
-        const uint32_t coef = coefs + 8 * q4o;            // this thread's column pair of the first 8 columns
-        // this thread's 4 bytes of 16-byte chunk 0 of its first row (the second is 8 rows on, with the same row & 7):
-        // chunk i of the row is at my ^ (i << 4), the swizzle being an XOR on those three address bits
-        const uint32_t my = stg + (uint32_t)prow * 128u + ((uint32_t)(prow & 7) << 4) + 4u * q4o;
+  // General path (masked, ragged or Tb != 8): Chan merges within each thread and across the quad, direct stores.
+  static __device__ __forceinline__ void pool_general_half(const TdnnGemmParams& p, const float (&a)[kAccRegs], int b0h,
+                                                           int nvh, int tblk, int ch0, const EpiFlags& f) {
+    const int q4 = threadIdx.x & 3;
+    const int gl = p.Tb < 8 ? p.Tb : 8;              // columns of one group inside one 8-column chunk
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int cch = ch0 + 8 * h;                   // this thread's output channel
+      const PoolChannel ch(p, cch, f.bn);
+      auto emit = [&](int col, float mean, float m2) {
+        const int bb = b0h + (col >> p.log2_tb);
+        if (ch.valid && bb < p.B) {
+          float* dst = p.pool_partial + ((long long)tblk * p.B + bb) * (2LL * p.Cout) + cch;
+          dst[0] = mean;
+          dst[p.Cout] = m2;
+        }
+      };
+      float rn = 0.f, rmean = 0.f, rm2 = 0.f;
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 8; ++i) {
+        const int col = 8 * i + 2 * q4;
+        const float x0 = ch(a[4 * i + 2 * h], f.relu_floor);
+        const float x1 = ch(a[4 * i + 2 * h + 1], f.relu_floor);
+        if (p.Tb == 1) {
+          if (nvh > 0) { emit(col, x0, 0.f); emit(col + 1, x1, 0.f); }
+          continue;
+        }
+        const int j = col & (p.Tb - 1);              // frame offset of x0 inside its time block
+        const bool v0 = j < nvh, v1 = j + 1 < nvh;
+        const float pn = (float)v0 + (float)v1;
+        const float pm = v1 ? 0.5f * (x0 + x1) : (v0 ? x0 : 0.f);
+        const float pm2 = v1 ? 0.5f * (x0 - x1) * (x0 - x1) : 0.f;
+        chan_merge(rn, rmean, rm2, pn, pm, pm2);
+        if (((col - 2 * q4 + 8) & (p.Tb - 1)) == 0) {  // a time block ends in this chunk (warp-uniform)
+          if (gl >= 4) chan_merge(rn, rmean, rm2, __shfl_xor_sync(0xffffffffu, rn, 1),
+                                  __shfl_xor_sync(0xffffffffu, rmean, 1), __shfl_xor_sync(0xffffffffu, rm2, 1));
+          if (gl >= 8) chan_merge(rn, rmean, rm2, __shfl_xor_sync(0xffffffffu, rn, 2),
+                                  __shfl_xor_sync(0xffffffffu, rmean, 2), __shfl_xor_sync(0xffffffffu, rm2, 2));
+          if (((2 * q4) & (gl - 1)) == 0 && rn > 0.f) emit(col & ~(p.Tb - 1), rmean, rm2);
+          rn = 0.f; rmean = 0.f; rm2 = 0.f;
+        }
+      }
+    }
+  }
+
+  // ================================ layer epilogues ================================
+  // +bias (+ row / utterance terms) -> ReLU -> swish -> BN -> tanh / sigmoid -> fp32 and/or split planes.
+  //
+  // Staged (p.tma_store, one uniform branch per tile): a 64-row half leaves in pieces of 64 channels.  Per piece the
+  // warpgroup puts the 64 columns' bias, scale and shift into shared memory once, every thread applies the same
+  // arithmetic in the same order as the direct path and writes its packed hi and lo pairs into the warpgroup's staging
+  // buffer, and one thread stores the two planes with TMA.  The buffer has the 128-byte swizzle of the store maps
+  // (16-byte chunk index ^ row & 7): a warp's eight rows fall into eight different chunks, so its stores do not
+  // conflict.  The maps' extents (Cout, T, B) clip the rows past T or B and the channels past Cout, so there are no
+  // tail branches; rows past an utterance's length are staged as zeros.
+  static __device__ __forceinline__ void layer_epilogue_staged(const TdnnGemmParams& p, Acc& acc, uint8_t* slab_base,
+                                                               int b0, int t0, int n0, const EpiFlags& f,
+                                                               const CUtensorMap* map_y_hi, const CUtensorMap* map_y_lo,
+                                                               TileClock& clk) {
+    // Everything below derives from an opaque copy of the thread index, per tile: hoisted out of the tile loop, these
+    // addresses stayed live through the main loop, which has no register to spare, and spilled more.
+    int tid = threadIdx.x;
+    asm volatile("" : "+r"(tid));
+    const int wgo = tid >> 7, wtid = tid & 127, q4o = tid & 3;
+    const int prow = 16 * ((tid >> 5) & 3) + ((tid & 31) >> 2);   // this thread's first row of a 64-row piece
+    const uint32_t stg = smem_u32(slab_base) + wgo * kStageOutBytes;
+    const uint32_t coefs = smem_u32(slab_base) + 2 * kStageOutBytes + wgo * kCoefBytes;
+    const int ebar = 4 + wgo;                         // named barrier of this warpgroup's epilogue
+    const uint32_t coef = coefs + 8 * q4o;            // this thread's column pair of the first 8 columns
+    // this thread's 4 bytes of 16-byte chunk 0 of its first row (the second is 8 rows on, with the same row & 7):
+    // chunk i of the row is at my ^ (i << 4), the swizzle being an XOR on those three address bits
+    const uint32_t my = stg + (uint32_t)prow * 128u + ((uint32_t)(prow & 7) << 4) + 4u * q4o;
 #pragma unroll 1
-        for (int hh = 0; hh < kHalves; ++hh) {
-          if (hh > 0) half_down();
-          const int hrow = (kPingPong ? 0 : 64 * wgo) + 64 * hh;   // the half's first row of the tile: a box of the store maps
-          uint32_t keep[2];                               // 0 for a masked batch's rows past the utterance's end
+    for (int hh = 0; hh < kHalves; ++hh) {
+      if (hh > 0) half_down(acc);
+      const int hrow = (kPingPong ? 0 : 64 * wgo) + 64 * hh;   // the half's first row of the tile: a box of the store maps
+      uint32_t keep[2];                               // 0 for a masked batch's rows past the utterance's end
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        const int row = hrow + prow + 8 * r;
+        const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
+        keep[r] = (p.lengths && b < p.B && t >= __ldg(p.lengths + b)) ? 0u : 0xffffffffu;
+      }
+#pragma unroll
+      for (int cr = 0; cr < BLOCK_N / kBlockK; ++cr) {
+        const int c0 = n0 + kBlockK * cr;
+        if (c0 >= p.Cout) break;
+        if (wtid == 0) tma_store_wait_read<0>();      // the previous piece has left the staging buffer
+        clk.mark(0);
+        if (wtid < kBlockK) {
+          const int c = c0 + wtid;
+          const bool in = c < p.Cout;
+          st_shared_f32(coefs + 4 * wtid, (in && p.bias) ? __ldg(p.bias + c) : 0.f);
+          st_shared_f32(coefs + 4 * (kBlockK + wtid), (in && f.bn) ? __ldg(p.scale + c) : 1.f);
+          st_shared_f32(coefs + 4 * (2 * kBlockK + wtid), (in && f.bn) ? __ldg(p.shift + c) : 0.f);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
+        clk.mark(1);
+#pragma unroll
+        for (int i = 0; i < kBlockK / 8; ++i) {
+          const float2 bias_c = ld_shared_f2(coef + 32 * i), scale_c = ld_shared_f2(coef + 32 * i + 4 * kBlockK),
+                       shift_c = ld_shared_f2(coef + 32 * i + 8 * kBlockK);
+          const float bias_e[2] = {bias_c.x, bias_c.y}, scale_e[2] = {scale_c.x, scale_c.y},
+                      shift_e[2] = {shift_c.x, shift_c.y};
 #pragma unroll
           for (int r = 0; r < 2; ++r) {
-            const int row = hrow + prow + 8 * r;
-            const int b = b0 + (row >> p.log2_tb), t = t0 + (row & (p.Tb - 1));
-            keep[r] = (p.lengths && b < p.B && t >= __ldg(p.lengths + b)) ? 0u : 0xffffffffu;
-          }
+            float x[2] = {acc[0][4 * (8 * cr + i) + 2 * r], acc[0][4 * (8 * cr + i) + 2 * r + 1]};
 #pragma unroll
-          for (int cr = 0; cr < BLOCK_N / kBlockK; ++cr) {
-            const int c0 = n0 + kBlockK * cr;
-            if (c0 >= p.Cout) break;
-            if (wtid == 0) tma_store_wait_read<0>();      // the previous piece has left the staging buffer
-            XVB_TL(tl_mark(0);)
-            if (wtid < kBlockK) {
-              const int c = c0 + wtid;
-              const bool in = c < p.Cout;
-              st_shared_f32(coefs + 4 * wtid, (in && p.bias) ? __ldg(p.bias + c) : 0.f);
-              st_shared_f32(coefs + 4 * (kBlockK + wtid), (in && bn) ? __ldg(p.scale + c) : 1.f);
-              st_shared_f32(coefs + 4 * (2 * kBlockK + wtid), (in && bn) ? __ldg(p.shift + c) : 0.f);
-            }
-            asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
-            XVB_TL(tl_mark(1);)
-#pragma unroll
-            for (int i = 0; i < kBlockK / 8; ++i) {
-              const float2 bias_c = ld_shared_f2(coef + 32 * i), scale_c = ld_shared_f2(coef + 32 * i + 4 * kBlockK),
-                           shift_c = ld_shared_f2(coef + 32 * i + 8 * kBlockK);
-              const float bias_e[2] = {bias_c.x, bias_c.y}, scale_e[2] = {scale_c.x, scale_c.y},
-                          shift_e[2] = {shift_c.x, shift_c.y};
-#pragma unroll
-              for (int r = 0; r < 2; ++r) {
-                float x[2] = {acc[0][4 * (8 * cr + i) + 2 * r], acc[0][4 * (8 * cr + i) + 2 * r + 1]};
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  // + 0.f: the direct path adds its (absent) row term here, which turns a -0 sum into +0
-                  float v = x[e] + bias_e[e] + 0.f;
-                  v = fmaxf(v, relu_floor);
-                  if constexpr (kSwish) v = v / (1.f + expf(-v));
-                  if (bn) v = fmaf(v, scale_e[e], shift_e[e]);
-                  if (act_tanh) v = epi_tanh(v);
-                  if (act_sigmoid) v = epi_sigmoid(v);
-                  x[e] = v;
-                }
-                __nv_bfloat16 h0, l0, h1, l1;
-                split_bf16(x[0], h0, l0);
-                split_bf16(x[1], h1, l1);
-                const uint32_t at = (my ^ ((uint32_t)i << 4)) + 1024u * r;
-                st_shared_u32(at, pack_bf16x2(h0, h1) & keep[r]);
-                st_shared_u32(at + kStagePlaneBytes, pack_bf16x2(l0, l1) & keep[r]);
-              }
-            }
-            XVB_TL(tl_mark(2);)
-            fence_proxy_async();                          // the staged piece becomes visible to the TMA unit
-            asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
-            if (wtid == 0) {
-              const int hb = b0 + (hrow >> p.log2_tb), ht = t0 + (hrow & (p.Tb - 1));
-              tma_store_3d(&map_y_hi, stg, c0, ht, hb);
-              tma_store_3d(&map_y_lo, stg + kStagePlaneBytes, c0, ht, hb);
-              tma_store_commit();
-            }
-            XVB_TL(tl_mark(3);)
+            for (int e = 0; e < 2; ++e)   // + 0.f: the direct path adds its (absent) row term here, which turns a -0 sum into +0
+              x[e] = f.activate<kSwish>(x[e] + bias_e[e] + 0.f, scale_e[e], shift_e[e]);
+            __nv_bfloat16 h0, l0, h1, l1;
+            split_bf16(x[0], h0, l0);
+            split_bf16(x[1], h1, l1);
+            const uint32_t at = (my ^ ((uint32_t)i << 4)) + 1024u * r;
+            st_shared_u32(at, pack_bf16x2(h0, h1) & keep[r]);
+            st_shared_u32(at + kStagePlaneBytes, pack_bf16x2(l0, l1) & keep[r]);
           }
         }
-        XVB_TL(tl_flush();)
-        continue;
+        clk.mark(2);
+        fence_proxy_async();                          // the staged piece becomes visible to the TMA unit
+        asm volatile("bar.sync %0, 128;" ::"r"(ebar) : "memory");
+        if (wtid == 0) {
+          const int hb = b0 + (hrow >> p.log2_tb), ht = t0 + (hrow & (p.Tb - 1));
+          tma_store_3d(map_y_hi, stg, c0, ht, hb);
+          tma_store_3d(map_y_lo, stg + kStagePlaneBytes, c0, ht, hb);
+          tma_store_commit();
+        }
+        clk.mark(3);
       }
     }
-    if constexpr (!kPool && !kHist) {
+  }
+
+  // Direct stores.  Column pairs outer, rows inner: a thread's two rows of a half share its columns, so bias, scale and
+  // shift are loaded once per column and half.
+  static __device__ __forceinline__ void layer_epilogue_direct(const TdnnGemmParams& p, Acc& acc, int b0, int t0, int n0,
+                                                               int slice, int row0, const EpiFlags& f) {
+    const int q4 = threadIdx.x & 3;
 #pragma unroll 1
-      for (int hh = 0; hh < kHalves; ++hh) {
-      if (hh > 0) half_down();
+    for (int hh = 0; hh < kHalves; ++hh) {
+      if (hh > 0) half_down(acc);
       constexpr int kRows = 2;
       bool live[kRows];                               // row exists and is not masked
       float rbias[kRows];
@@ -754,8 +758,8 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
         for (int e = 0; e < 2; ++e) {
           const bool in = e == 0 || has1;
           bias_c[e] = (in && p.bias) ? __ldg(p.bias + c + e) : 0.f;
-          scale_c[e] = (in && bn) ? __ldg(p.scale + c + e) : 1.f;
-          shift_c[e] = (in && bn) ? __ldg(p.shift + c + e) : 0.f;
+          scale_c[e] = (in && f.bn) ? __ldg(p.scale + c + e) : 1.f;
+          shift_c[e] = (in && f.bn) ? __ldg(p.shift + c + e) : 0.f;
         }
 #pragma unroll
         for (int r = 0; r < kRows; ++r) {
@@ -766,12 +770,7 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
             if (e == 1 && !has1) break;
             float v = x[e] + bias_c[e] + rbias[r];
             if (ub[r]) v += __ldg(ub[r] + c + e);
-            v = fmaxf(v, relu_floor);
-            if constexpr (kSwish) v = v / (1.f + expf(-v));
-            if (bn) v = fmaf(v, scale_c[e], shift_c[e]);
-            if (act_tanh) v = epi_tanh(v);
-            if (act_sigmoid) v = epi_sigmoid(v);
-            x[e] = v;
+            x[e] = f.activate<kSwish>(v, scale_c[e], shift_c[e]);
           }
           if (p.y_hi) {
             __nv_bfloat16 h0, l0, h1, l1;
@@ -794,15 +793,127 @@ tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __gr
           }
         }
       }
-      }
-      XVB_TL(tl_flush();)
     }
   }
-  if constexpr (kHist) hist_flush();
-  if constexpr (kStaged || kPool) {
+};
+
+// Ping-pong (the 128-wide layer and fused-pooling instances): tile j of the CTA's list (blockIdx.x + j * gridDim.x)
+// belongs to warpgroup j & 1, which computes all 128 of its rows as two m64 halves.  Each warpgroup finds its place in
+// the operand ring from a running count of the K blocks of all the CTA's tiles, the other warpgroup's included.  Both
+// wait on the ring's full barriers by phase parity, which only tells the phase being waited for from the one before it:
+// a warpgroup that started waiting on its next tile's first stage while the producer was still more than one lap of
+// the ring behind would take an older load of that stage for its own.  So the main loops take turns on named barriers
+// 2 + wg ("warpgroup wg may start its main loop"): a warpgroup starts one only after the other has issued the previous
+// tile's MMAs, and the epilogue of that tile then runs under the other's main loop.
+template <int BLOCK_N, bool kPool, bool kHist, bool kSwish = false>
+__global__ void __launch_bounds__(gemm_threads<BLOCK_N, kHist, kSwish>(), 1)
+tdnn_gemm_bf16x3_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
+                        const __grid_constant__ CUtensorMap map_a2_hi, const __grid_constant__ CUtensorMap map_a2_lo,
+                        const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
+                        const __grid_constant__ CUtensorMap map_y_hi, const __grid_constant__ CUtensorMap map_y_lo,
+                        const __grid_constant__ TdnnGemmParams p) {
+  using K = LayerKernel<BLOCK_N, kPool, kHist, kSwish>;
+
+  extern __shared__ uint8_t smem_raw[];
+  // SWIZZLE_128B tiles need 1024-byte alignment
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* slab_base = smem + K::kStages * K::kStageBytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slab_base + K::Cfg::kTailBytes);
+  uint64_t* empty_bar = full_bar + K::kStages;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+
+  if (warp == kProducerWarp && lane == 0) {
+    tma_prefetch_desc(&map_a_hi);
+    tma_prefetch_desc(&map_a_lo);
+    tma_prefetch_desc(&map_w_hi);
+    tma_prefetch_desc(&map_w_lo);
+    if ((K::kStaged || kPool) && p.tma_store) {
+      tma_prefetch_desc(&map_y_hi);
+      tma_prefetch_desc(&map_y_lo);
+    }
+    for (int i = 0; i < K::kStages; ++i) {
+      mbar_init(&full_bar[i], 1);                      // producer arrival + all TMA bytes
+      mbar_init(&empty_bar[i], K::kReleaseWarps);      // one arrival per consumer warp of the stage's warpgroup(s)
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) may overlap the
+  // tail of the previous kernel in the stream; its results are needed from here on.
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  // the previous kernel may have written our operands with ordinary (generic-proxy) stores -- the staging
+  // / pooling kernels do -- while we read them through TMA (async proxy): order the two proxies explicitly,
+  // a kernel boundary would have done it for us
+  asm volatile("fence.proxy.async;" ::: "memory");
+
+  if (warp >= kProducerWarp) {
+    if constexpr (K::kPingPong) setmaxnreg_dec<kProducerRegs>();   // the whole producer warpgroup
+    if (warp == kProducerWarp && lane == 0)
+      K::produce(p, smem, full_bar, empty_bar, &map_a_hi, &map_a_lo, &map_a2_hi, &map_a2_lo, &map_w_hi, &map_w_lo);
+    return;
+  }
+
+  // ================================ consumers: wgmma + epilogue ================================
+  if constexpr (K::kPingPong) setmaxnreg_inc<kConsumerRegs>();
+  const int wg = warp >> 2;                          // split tiles: accumulator rows 64*wg .. 64*wg+63
+  // this thread's rows: row0 + 64 * hh + 8 * h for half hh < kHalves and h < 2
+  const int row0 = (K::kPingPong ? 0 : 64 * wg) + 16 * (warp & 3) + (lane >> 2);
+  const EpiFlags f(p.flags);
+  typename K::Acc acc;
+#pragma unroll
+  for (int hh = 0; hh < K::kHalves; ++hh)
+#pragma unroll
+    for (int i = 0; i < K::kAccRegs; ++i) acc[hh][i] = 0.f;
+  typename K::Ring ring;
+  TrialHistogram hist(slab_base);
+  if constexpr (kHist) hist.clear(p);
+  TileClock clk(p);
+  const int num_kblk = p.num_src * p.ntaps * p.num_cblk;
+
+  int tj = 0;                                        // index of the tile in the CTA's list
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++tj) {
+    int m_unit, n_blk, slice;
+    if (!decode_tile<kHist>(p, tile, m_unit, n_blk, slice)) continue;
+    int kb_begin = 0, kb_end = num_kblk;
+    if (p.k_slices > 1) {
+      kb_begin = slice * p.kb_per_slice;
+      kb_end = min(num_kblk, kb_begin + p.kb_per_slice);
+    }
+    if constexpr (K::kPingPong) {
+      if ((tj & 1) != wg) {                          // the other warpgroup's tile: skip its stages in the ring
+        ring.skip(kb_end - kb_begin);
+        continue;
+      }
+      if (tj > 0) {
+        // fused pooling: the warpgroup's previous TMA store has read the staging buffer, for all its threads past here
+        if (kPool && (threadIdx.x & 127) == 0) tma_store_wait_read<0>();
+        asm volatile("bar.sync %0, 256;" ::"r"(2 + wg) : "memory");   // the other's main loop is issued
+      }
+    }
+    clk.tile_start();
+    K::main_loop(p, acc, smem, full_bar, empty_bar, ring, kb_begin, kb_end, tile, wg, clk);
+
+    const int b0 = (m_unit / p.num_t_blk) * p.Bb, t0 = (m_unit % p.num_t_blk) * p.Tb;
+    const int n0 = n_blk * BLOCK_N;
+    if constexpr (kHist) {
+      hist.count<BLOCK_N>(p, acc[0], b0, t0, n0, row0);
+      continue;
+    } else if constexpr (kPool) {
+      K::pool_epilogue(p, acc, slab_base, b0, t0, m_unit % p.num_t_blk, n0, row0, wg, f, &map_y_hi, clk);
+    } else if (K::kStaged && p.tma_store) {
+      K::layer_epilogue_staged(p, acc, slab_base, b0, t0, n0, f, &map_y_hi, &map_y_lo, clk);
+    } else {
+      K::layer_epilogue_direct(p, acc, b0, t0, n0, slice, row0, f);
+    }
+    clk.flush(p, tj, wg);
+  }
+  if constexpr (kHist) hist.flush(p);
+  if constexpr (K::kStaged || kPool) {
     if (p.tma_store && (threadIdx.x & 127) == 0) tma_store_wait_done<0>();   // this thread's stores have landed
   }
-  XVB_TL(if (tl_cta && (threadIdx.x & 127) == 0) { tl_cta[2 + 2 * wg] = global_timer(); tl_cta[3 + 2 * wg] = (unsigned long long)clock64(); })
+  clk.end(wg);
 }
 
 // Split-K tail: y[b,c] = epi(sum_s part[b,s,c]) with the slices added in index order (deterministic),
