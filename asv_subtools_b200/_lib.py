@@ -173,6 +173,7 @@ SIGNATURES = {
     "xvb_conv_module": (_i, [_p, _i64, _i, _i, _i, _p, _p, _i, _p, _p, _i, _f, _i, _p, _p, _i64, _p]),
     "xvb_bn_relu_planes": (_i, [_p, _p, _i64, _i64, _i, _p, _p, _p, _p, _i64, _p]),
     "xvb_cam_gate": (_i, [_p, _p, _i64, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p]),
+    "xvb_cam_gate_lengths": (_i, [_p, _p, _i64, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p, _p]),
     "xvb_seg_gate_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _i, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_se_residual": (_i, [_p, _p, _p, _p, _p, _i, _i64, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
     "xvb_se_residual_lengths": (_i, [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p]),
@@ -257,6 +258,7 @@ SIGNATURES = {
     "xvb_campp_embed_dim": (_i, [_p]),
     "xvb_campp_last_launches": (_i, [_p]),
     "xvb_campp_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_campp_extract_lengths": (_i, [_p, _p, _p, _i, _i, _p, _p]),
     "xvb_campp_save": (_i, [_p, C.c_char_p]),
     "xvb_campp_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_campp_destroy": (None, [_p]),

@@ -76,7 +76,7 @@ int res_freq(int F, int j) {
 
 struct xvb_campp : Handle<Model> {
   enum { kX0, kA0, kO0 = kA0 + kResBlocks, kS0 = kO0 + kResBlocks, kC2 = kS0 + kResBlocks, kPad, kBuf0, kPre = kBuf0 + kBlocks,
-         kH, kZ, kPool, kGate, kStats, kBufs };
+         kH, kZ, kPool, kGate, kStats, kLengths, kBufs };
   Workspace<kBufs> ws;
   int pad_B = -1, pad_T = -1;          // the (B, T) layout whose pad frames are zero
 };
@@ -105,8 +105,9 @@ int reserve(H* h, int B, int T) {
   need[H::kPool] = b * t2 * m->c3;
   need[H::kGate] = b * nseg * m->cfg.growth_rate;
   need[H::kStats] = b * 2 * m->c3;
+  need[H::kLengths] = 0;   // sized by xvb_campp_extract_lengths for the whole call, before its groups run
   bool planes[H::kBufs];
-  for (int i = 0; i < H::kBufs; ++i) planes[i] = i != H::kPool && i != H::kGate && i != H::kStats;
+  for (int i = 0; i < H::kBufs; ++i) planes[i] = i != H::kPool && i != H::kGate && i != H::kStats && i != H::kLengths;
   uint64_t grown;
   const int rc = h->ws.reserve(need, planes, &grown);
   if (grown >> H::kPad & 1) h->pad_B = h->pad_T = -1;
@@ -116,20 +117,23 @@ int reserve(H* h, int B, int T) {
 Planes offset(Planes p, size_t n) { return {p.hi + n, p.lo + n}; }
 
 // ops.PackedAffine.run: x planes (B, T, l.Cin) with row pitch ldx -> y planes (pitch ldy) or yf (pitch ldyf); a nonzero
-// x_batch_stride makes x an im2col view (xvb_tdnn_args_t)
+// x_batch_stride makes x an im2col view (xvb_tdnn_args_t); lens: NULL, or a masked batch's output lengths
 int lin(const Affine& l, Planes x, int64_t ldx, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
-        int64_t x_batch_stride, void* stream) {
+        int64_t x_batch_stride, const int* lens, void* stream) {
   xvb_tdnn_args_t a = affine_args(l, x, ldx, B, T);
   if (y) { a.y_hi = y->hi; a.y_lo = y->lo; a.ldy = ldy; }
   a.y_f32 = yf; a.ldyf = ldyf;
   a.x_batch_stride = x_batch_stride;
+  a.lengths = lens;
   return xvb_tdnn_affine_ex(&a, stream);
 }
 
 // ops.conv2d: x (B, T, F, 32) planes -> y (B, T, F', 32) with F' = ceil(F / stride); stride_t 0 or 1 as the driver passes it
+// (the time axis is never strided, so a masked batch's lens are the input's and the output's frame counts)
 int conv(const Conv& c, Planes x, int B, int T, int F, int ksize, int stride, int stride_t, const Planes* res, bool relu, Planes y,
-         void* stream) {
+         const int* lens, void* stream) {
   xvb_conv2d_args_t a{};
+  a.lengths = lens;
   a.x_hi = x.hi; a.x_lo = x.lo;
   a.w_hi = c.w.hi; a.w_lo = c.w.lo;
   a.B = B; a.T = T; a.F = F; a.Cin = kM; a.Cout = kM; a.ksize = ksize; a.stride = stride; a.stride_t = stride_t;
@@ -140,8 +144,11 @@ int conv(const Conv& c, Planes x, int B, int T, int F, int ksize, int stride, in
   return xvb_conv2d(&a, stream);
 }
 
-// One group of utterances: CamPPExtractor.extract.  *n counts the launches as the driver does.
-int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, void* stream) {
+// One group of utterances: CamPPExtractor.extract.  *n counts the launches as the driver does.  A masked group passes
+// lens, its frame counts in row 0 of the workspace's (2, ld) table and their ceil(L / 2) after the stride-2 tdnn in row 1;
+// NULL otherwise.  Every tensor of a masked group then holds exact zeros past each utterance's length at its own time
+// resolution, except `pre`, whose only consumers are 1x1 layers that store zeros there themselves.
+int extract_group(H* h, const float* feats, int B, int T, const int* lens, int ld, float* emb, int* n, void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
   const Model* m = h->m.get();
@@ -159,10 +166,13 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     }
     h->pad_B = B; h->pad_T = T;
   }
+  const int* lens2 = lens ? lens + ld : nullptr;   // after the stride-2 tdnn
   Planes x = h->ws.planes(H::kX0);
-  if ((rc = xvb_conv2d_head(feats, B, T, c.feat_dim, m->conv1_w, kM, m->conv1_s, m->conv1_t, x.hi, x.lo, nullptr, nullptr,
-                            nullptr, nullptr, stream)))
-    return rc;
+  rc = lens ? xvb_conv2d_head_lengths(feats, B, T, c.feat_dim, lens, m->conv1_w, kM, m->conv1_s, m->conv1_t, x.hi, x.lo, nullptr,
+                                      nullptr, nullptr, nullptr, stream)
+            : xvb_conv2d_head(feats, B, T, c.feat_dim, m->conv1_w, kM, m->conv1_s, m->conv1_t, x.hi, x.lo, nullptr, nullptr,
+                              nullptr, nullptr, stream);
+  if (rc) return rc;
   *n += 1;
   int F = c.feat_dim;
   for (int j = 0; j < kResBlocks; ++j) {
@@ -171,19 +181,19 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     Planes res = x;
     if (r.has_sc) {
       res = h->ws.planes(H::kS0 + j);
-      if ((rc = conv(r.sc, x, B, T, F, 1, r.stride, 1, nullptr, false, res, stream))) return rc;
+      if ((rc = conv(r.sc, x, B, T, F, 1, r.stride, 1, nullptr, false, res, lens, stream))) return rc;
       *n += 1;
     }
     const Planes a = h->ws.planes(H::kA0 + j), o = h->ws.planes(H::kO0 + j);
-    if ((rc = conv(r.c1, x, B, T, F, 3, r.stride, 1, nullptr, true, a, stream)) ||
-        (rc = conv(r.c2, a, B, T, Fo, 3, 1, 0, &res, true, o, stream)))
+    if ((rc = conv(r.c1, x, B, T, F, 3, r.stride, 1, nullptr, true, a, lens, stream)) ||
+        (rc = conv(r.c2, a, B, T, Fo, 3, 1, 0, &res, true, o, lens, stream)))
       return rc;
     *n += 2;
     x = o;
     F = Fo;
   }
   const Planes c2 = h->ws.planes(H::kC2);
-  if ((rc = conv(m->conv2, x, B, T, F, 3, 2, 1, nullptr, true, c2, stream))) return rc;
+  if ((rc = conv(m->conv2, x, B, T, F, 3, 2, 1, nullptr, true, c2, lens, stream))) return rc;
   // the head output into the time-padded copy: one row of T * F'' * C elements per utterance
   const int64_t tb = (int64_t)T * row * sizeof(uint16_t), pb = (int64_t)(T + 4) * row * sizeof(uint16_t);
   if ((rc = xvb_copy_rows(c2.hi, tb, pad.hi + 2 * row, pb, B, tb, stream)) ||
@@ -193,7 +203,7 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
   // tdnn: Conv1d(k = 5, stride 2, padding 2) as a 1-tap layer over 5-frame windows that start every 2 frames
   Planes bufs[kBlocks];
   for (int i = 0; i < kBlocks; ++i) bufs[i] = h->ws.planes(H::kBuf0 + i);
-  if ((rc = lin(m->tdnn, pad, 2 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, stream)))
+  if ((rc = lin(m->tdnn, pad, 2 * row, B, T2, &bufs[0], m->widths[0], nullptr, 0, (int64_t)(T + 4) * row, lens2, stream)))
     return rc;
   *n += 1;
   const Planes pre = h->ws.planes(H::kPre), hh = h->ws.planes(H::kH), z = h->ws.planes(H::kZ);
@@ -208,9 +218,12 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
       const int cin = c0 + li * g;
       Planes out = offset(buf, cin);
       if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, cin, L.s1, L.t1, pre.hi, pre.lo, m->maxw, stream)) ||
-          (rc = lin(L.lin1, pre, m->maxw, B, T2, &hh, m->bn, nullptr, 0, 0, stream)) ||
-          (rc = xvb_cam_gate(hh.hi, hh.lo, m->bn, B, T2, m->bn, kSegLen, L.gw1, L.gb1, m->bn / 2, L.gw2, L.gb2, g, gate, stream)) ||
-          (rc = lin(L.local, hh, m->bn, B, T2, &z, g, nullptr, 0, 0, stream)) ||
+          (rc = lin(L.lin1, pre, m->maxw, B, T2, &hh, m->bn, nullptr, 0, 0, lens2, stream)) ||
+          (rc = lens2 ? xvb_cam_gate_lengths(hh.hi, hh.lo, m->bn, B, T2, m->bn, kSegLen, L.gw1, L.gb1, m->bn / 2, L.gw2, L.gb2, g,
+                                             lens2, gate, stream)
+                      : xvb_cam_gate(hh.hi, hh.lo, m->bn, B, T2, m->bn, kSegLen, L.gw1, L.gb1, m->bn / 2, L.gw2, L.gb2, g, gate,
+                                     stream)) ||
+          (rc = lin(L.local, hh, m->bn, B, T2, &z, g, nullptr, 0, 0, lens2, stream)) ||
           (rc = xvb_seg_gate_apply(z.hi, z.lo, g, nullptr, nullptr, 0, gate, kSegLen, out.hi, out.lo, width, B, T2, g, stream)))
         return rc;
       *n += 5;
@@ -219,14 +232,15 @@ int extract_group(H* h, const float* feats, int B, int T, float* emb, int* n, vo
     if ((rc = xvb_bn_relu_planes(buf.hi, buf.lo, width, rows, width, tr.s, tr.t, pre.hi, pre.lo, m->maxw, stream))) return rc;
     *n += 1;
     if (bi + 1 < kBlocks) {
-      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, &bufs[bi + 1], m->widths[bi + 1], nullptr, 0, 0, stream))) return rc;
+      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, &bufs[bi + 1], m->widths[bi + 1], nullptr, 0, 0, lens2, stream))) return rc;
       *n += 1;
       c0 = tr.lin.Cout;
     } else {
       // out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance
       float* pool = h->ws.f32(H::kPool);
-      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, nullptr, 0, pool, m->c3, 0, stream)) ||
-          (rc = xvb_stats_pool_ex(pool, m->c3, B, T2, m->c3, 0.0f, 1, stats, nullptr, nullptr, 2 * m->c3, stream)))
+      if ((rc = lin(tr.lin, pre, m->maxw, B, T2, nullptr, 0, pool, m->c3, 0, lens2, stream)) ||
+          (rc = lens2 ? xvb_stats_pool_lengths(pool, m->c3, B, T2, m->c3, 0.0f, 1, lens2, stats, nullptr, nullptr, 2 * m->c3, stream)
+                      : xvb_stats_pool_ex(pool, m->c3, B, T2, m->c3, 0.0f, 1, stats, nullptr, nullptr, 2 * m->c3, stream)))
         return rc;
       *n += 2;
     }
@@ -394,7 +408,39 @@ extern "C" int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int 
   const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->cfg.embd_dim;
   int n = 0;
   int rc = for_groups(B, T, kFrameBudget,
-                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, &n, stream); });
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, nullptr, 0, emb + i * E, &n, stream); });
+  if (rc) return rc;
+  h->last_launches = n;
+  return XVB_OK;
+}
+
+extern "C" int xvb_campp_extract_lengths(xvb_campp_t* h, const float* feats, const int32_t* lengths_host, int B, int T, float* emb,
+                                         void* stream) {
+  const char* fn = "xvb_campp_extract_lengths";
+  XVB_CHECK_ARG(finalized(h), "%s: model not finalized", fn);
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "%s: bad arguments", fn);
+  bool all_T;
+  int rc = check_lengths(fn, lengths_host, B, T, &all_T, kMinFrames);
+  if (rc) return rc;
+  if (all_T) return xvb_campp_extract(h, feats, B, T, emb, stream);   // nothing to mask: the unmasked call itself
+  // row 0: L at the head's resolution; row 1: L' = ceil(L / 2), the output length of the stride-2 tdnn (k = 5, pad 2)
+  std::vector<int32_t> table((size_t)2 * B);
+  for (int b = 0; b < B; ++b) {
+    table[b] = lengths_host[b];
+    table[(size_t)B + b] = (lengths_host[b] + 1) / 2;
+  }
+  size_t need[H::kBufs] = {0};
+  bool planes[H::kBufs] = {false};
+  need[H::kLengths] = table.size();
+  uint64_t grown;
+  if ((rc = h->ws.reserve(need, planes, &grown))) return rc;
+  int* lens = h->ws.i32(H::kLengths);
+  // stream-ordered: the previous call's kernels on `stream` have read the old table before this one lands
+  XVB_CUDA(cudaMemcpyAsync(lens, table.data(), table.size() * sizeof(int32_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->cfg.embd_dim;
+  int n = 0;
+  rc = for_groups(B, T, kFrameBudget,
+                  [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, lens + i, B, emb + i * E, &n, stream); });
   if (rc) return rc;
   h->last_launches = n;
   return XVB_OK;

@@ -276,13 +276,13 @@ int publish_built(Handle<Model>* h, Build build, const char* fn) {
   return XVB_OK;
 }
 
-// The host lengths of a masked call: each in [1, T], or XVB_EINVAL naming the first that is not (fn: the caller's
+// The host lengths of a masked call: each in [min_len, T], or XVB_EINVAL naming the first that is not (fn: the caller's
 // name).  *all_T: every utterance is T frames long, so that there is nothing to mask.
-inline int check_lengths(const char* fn, const int32_t* lengths_host, int B, int T, bool* all_T) {
+inline int check_lengths(const char* fn, const int32_t* lengths_host, int B, int T, bool* all_T, int min_len = 1) {
   *all_T = true;
   for (int b = 0; b < B; ++b) {
-    XVB_CHECK_ARG(lengths_host[b] >= 1 && lengths_host[b] <= T, "%s: lengths[%d]=%d outside [1, T=%d]", fn, b,
-                  (int)lengths_host[b], T);
+    XVB_CHECK_ARG(lengths_host[b] >= min_len && lengths_host[b] <= T, "%s: lengths[%d]=%d outside [%d, T=%d]", fn, b,
+                  (int)lengths_host[b], min_len, T);
     *all_T = *all_T && lengths_host[b] == T;
   }
   return XVB_OK;

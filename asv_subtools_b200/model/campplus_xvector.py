@@ -15,7 +15,9 @@ output, every dense layer as BN1 -> ReLU (xvb_bn_relu_planes) -> linear1 with BN
 context-aware mask (xvb_cam_gate) -> linear_local -> y * m written into the layer's column slice of the block's
 concatenation buffer (xvb_seg_gate_apply); transit3 carries out_nonlinear, xvb_stats_pool_ex takes [mean | unbiased std];
 dense is xvb_small_affine.  extract_embedding applies CamPPModel's 4000-frame chunk rule (XvectorMixin.split_chunks with
-even=False).
+even=False).  extract_embedding_batch(feats, lengths) takes a masked batch of chunks of different lengths: every layer
+then stores exact zeros past each utterance's end at its own time resolution (xvb_cam_gate_lengths gives each utterance
+the context of its own frames), and each row is the chunk extracted alone, bit for bit.
 
 build_extractor() returns NativeCamPPExtractor: the same launch sequence in the C library (csrc/campplus_extractor.cu),
 which also writes XVBP0001 model files for bin/xvb-extract.  XVB_CAMPP_NATIVE=0 selects CamPPExtractor, the Python driver
@@ -33,7 +35,7 @@ import torch.nn as nn
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 
 from asv_subtools_b200 import ops  # noqa: E402
-from asv_subtools_b200.native import NativeExtractor  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor, host_lengths  # noqa: E402
 from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import fold_batchnorm  # noqa: E402
 
@@ -153,7 +155,12 @@ def backbone_state_dict(state_dict):
 
 
 class CamPPXvector(TopVirtualNnet):
-    """CAM++: FCM 2-D head, densely connected TDNN blocks with context-aware masking, statistics pooling, dense."""
+    """CAM++: FCM 2-D head, densely connected TDNN blocks with context-aware masking, statistics pooling, dense.
+
+    `masked_chunks`, set by init: extract_embedding_batch takes lengths (a masked batch of single chunks) on this
+    instance.  An instance that init did not build -- a blueprint that borrows these extraction methods (egrecho's
+    EcapaXvector), or an object that was never constructed -- refuses lengths with NotImplementedError before it reads
+    any configuration."""
 
     def init(self, inputs_dim, num_targets, embd_dim=512, init_channels=128, growth_rate=32, bn_size=4,
              memory_efficient=True):
@@ -166,6 +173,7 @@ class CamPPXvector(TopVirtualNnet):
         if init_channels % 8:
             _unsupported("init_channels", init_channels, "the first block's width must be a multiple of 8")
         self.inputs_dim, self.embd_dim = inputs_dim, embd_dim
+        self.masked_chunks = True
         self.growth_rate, self.bn_channels = growth_rate, bn_channels
         self.head = _FCM(inputs_dim)
         xv = OrderedDict([("tdnn", _TDNNBlock(self.head.out_channels, init_channels, 5, stride=2))])
@@ -205,14 +213,24 @@ class CamPPXvector(TopVirtualNnet):
         return self.extract_embedding_batch(torch.as_tensor(np.asarray(feats) if not isinstance(feats, torch.Tensor)
                                                             else feats)[None])[0].cpu()
 
+    def chunk_sizes(self, num_frames):
+        """The chunk lengths extract_embedding cuts a num_frames-long utterance into (CamPPModel's 4000-frame rule);
+        pipeline/extract_embeddings.py --mixed-lengths cuts utterances with it before batching them."""
+        return chunk_sizes(num_frames)
+
     def extract_embedding_batch(self, feats, lengths=None):
         """Equal-length utterances (B, T, F) float32 -> (B, embd_dim) CUDA tensor, the same arithmetic as B calls of
         extract_embedding(): each chunk position of chunk_sizes(T) runs as one batch, and the chunk embeddings are
-        combined as sum_i size_i * emb_i / T in chunk order."""
+        combined as sum_i size_i * emb_i / T in chunk order.
+
+        lengths (B,) host ints: a masked batch of single chunks of different lengths padded to T <= 4000, row b being
+        the embedding of feats[b, :lengths[b]] extracted alone (what is past it is never read).  ValueError for T > 4000
+        (cut utterances with chunk_sizes first) and for a length outside [3, T], naming the first such entry."""
         if lengths is not None:
-            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN and ResNet x-vector "
-                                      "blueprints only"
-                                      .format(type(self).__name__))
+            if not getattr(self, "masked_chunks", False):
+                raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector, ResNet "
+                                          "x-vector and CAM++ blueprints only".format(type(self).__name__))
+            return self._extract_masked(feats, lengths)
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:
@@ -228,6 +246,31 @@ class CamPPXvector(TopVirtualNnet):
                 acc = e * s if acc is None else acc + s * e
                 off += s
             return acc / sum(sizes)
+
+    def _extract_masked(self, feats, lengths):
+        with torch.no_grad():
+            x = torch.as_tensor(feats)
+            if x.dtype != torch.float32:
+                raise TypeError("extract_embedding_batch expects float32 features")
+            B, T, Fd = x.shape
+            if Fd != self.inputs_dim:
+                raise ValueError("expected feature dim {}, got {}".format(self.inputs_dim, Fd))
+            if T > MAX_CHUNK:
+                raise ValueError("extract_embedding_batch(lengths=...) takes one chunk per row, T <= {}, got T={}: cut the "
+                                 "utterances with chunk_sizes first".format(MAX_CHUNK, T))
+            lens = _checked_lengths(lengths, B, T)
+            x = x.to(self.device_for_extraction(), non_blocking=True).contiguous()
+            return self.extractor().extract(x, lens)
+
+
+def _checked_lengths(lengths, b, t):
+    """Host int32 (B,) lengths of a masked CAM++ batch; ValueError naming the first entry outside [MIN_FRAMES, t]."""
+    lens = host_lengths(lengths, b)
+    bad = np.flatnonzero((lens < MIN_FRAMES) | (lens > t))
+    if bad.size:
+        raise ValueError("lengths[{}]={} outside [{}, T={}]: a CAM++ chunk needs at least {} frames".format(
+            bad[0], lens[bad[0]], MIN_FRAMES, t, MIN_FRAMES))
+    return lens
 
 
 def tdnn_im2col_weight(weight, channels, freq):
@@ -249,9 +292,11 @@ def _fold(w, bn, bias=None):
 
 class CamPPExtractor:
     """Folded weights on one device + the launch sequence of CamPP.forward for one chunk per utterance (all utterances of
-    a call have the same length), driven from Python over a workspace reused while the batch shape stays the same.  The
-    weights are the records and configuration the native handle takes (native_records, native_config), each reshaped
-    back from its (rows, cols) form."""
+    a call have the same length, or a masked batch gives each its own), driven from Python over a workspace reused while
+    the batch shape stays the same.  The weights are the records and configuration the native handle takes
+    (native_records, native_config), each reshaped back from its (rows, cols) form."""
+
+    TAKES_LENGTHS = True
 
     def __init__(self, m, device):
         from asv_subtools_b200._lib import RELU
@@ -333,32 +378,41 @@ class CamPPExtractor:
             self._ws_key, self._ws = (B, T), ws
         return self._ws
 
-    def extract(self, feats):
+    def extract(self, feats, lengths=None):
         """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embd_dim) fp32 CUDA, asynchronous on the current
-        stream."""
+        stream.  lengths (B,) host ints, 3 <= lengths[b] <= T: a masked batch as xvb_campp_extract_lengths runs it, row b
+        being feats[b, :lengths[b]] extracted alone (every length equal to T: the unmasked sequence).  Every workspace
+        tensor then holds exact zeros past each utterance's length at its own resolution, except `pre`, whose only
+        consumers are 1x1 layers that store zeros there themselves."""
         B, T, Fd = feats.shape
         if Fd != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, Fd))
         if T < MIN_FRAMES:
             raise ValueError("CAM++ needs at least {} frames, got {}".format(MIN_FRAMES, T))
+        l1 = l2 = None    # a masked batch's lengths at the head's resolution and after the stride-2 tdnn, ceil(L / 2)
+        if lengths is not None:
+            lens = _checked_lengths(lengths, B, T)
+            if (lens != T).any():
+                table = torch.from_numpy(np.stack([lens, (lens + 1) // 2])).to(feats.device)
+                l1, l2 = table[0], table[1]
         feats = feats.contiguous()
         ws = self._workspace(B, T)
         P, m = ops.SplitPlanes, M_CHANNELS
-        ops.conv2d_head(feats, *self.conv1, ws["x0"])
+        ops.conv2d_head(feats, *self.conv1, ws["x0"], lengths=l1)
         n = 1
         x = ws["x0"]
         for j, (stride, c1, c2, sc) in enumerate(self.res_blocks):
             res = x
             if sc is not None:
                 res = ws["s%d" % j]
-                ops.conv2d(x, sc[0], m, 1, stride, sc[1], sc[2], y=res, stride_t=1)
+                ops.conv2d(x, sc[0], m, 1, stride, sc[1], sc[2], y=res, stride_t=1, lengths=l1)
                 n += 1
-            ops.conv2d(x, c1[0], m, 3, stride, c1[1], c1[2], relu=True, y=ws["a%d" % j], stride_t=1)
-            ops.conv2d(ws["a%d" % j], c2[0], m, 3, 1, c2[1], c2[2], res=res, relu=True, y=ws["o%d" % j])
+            ops.conv2d(x, c1[0], m, 3, stride, c1[1], c1[2], relu=True, y=ws["a%d" % j], stride_t=1, lengths=l1)
+            ops.conv2d(ws["a%d" % j], c2[0], m, 3, 1, c2[1], c2[2], res=res, relu=True, y=ws["o%d" % j], lengths=l1)
             n += 2
             x = ws["o%d" % j]
         c = self.conv2
-        ops.conv2d(x, c[0], m, 3, 2, c[1], c[2], relu=True, y=ws["c2"], stride_t=1)
+        ops.conv2d(x, c[0], m, 3, 2, c[1], c[2], relu=True, y=ws["c2"], stride_t=1, lengths=l1)
         # the head output into the time-padded copy: one row of T * F'' * C elements per utterance
         row = self.f8 * m
         pad, src = ws["pad"], ws["c2"]
@@ -371,7 +425,7 @@ class CamPPExtractor:
         win = P(pad.hi.as_strided((B, T2, 2 * row), ((T + 4) * row, 2 * row, 1)),
                 pad.lo.as_strided((B, T2, 2 * row), ((T + 4) * row, 2 * row, 1)), 5 * row)
         bufs, pre = ws["bufs"], ws["pre"]
-        self.tdnn.run(win, y=bufs[0].slice(0, self.tdnn.cout), x_batch_stride=(T + 4) * row)
+        self.tdnn.run(win, y=bufs[0].slice(0, self.tdnn.cout), x_batch_stride=(T + 4) * row, lengths=l2)
         n += 1
         c0 = self.tdnn.cout
         h, z, gate = ws["h"], ws["z"], ws["gate"]
@@ -382,9 +436,9 @@ class CamPPExtractor:
                 xin = buf.slice(0, cin)
                 pv = pre.slice(0, cin)
                 ops.bn_relu_planes(xin, L["s1"], L["t1"], pv)
-                L["lin1"].run(pv, y=h)
-                ops.cam_gate(h, *L["gate"], seg_len=SEG_LEN, out=gate)
-                L["local"].run(h, y=z)
+                L["lin1"].run(pv, y=h, lengths=l2)
+                ops.cam_gate(h, *L["gate"], seg_len=SEG_LEN, out=gate, lengths=l2)
+                L["local"].run(h, y=z, lengths=l2)
                 ops.seg_gate_apply(z, gate, SEG_LEN, buf.slice(cin, cin + self.g))
                 n += 5
             s, t, lin = self.transits[bi]
@@ -393,15 +447,15 @@ class CamPPExtractor:
             ops.bn_relu_planes(buf if buf.channels == width else buf.slice(0, width), s, t, pv)
             n += 1
             if bi + 1 < len(self.blocks):
-                lin.run(pv, y=bufs[bi + 1].slice(0, lin.cout))
+                lin.run(pv, y=bufs[bi + 1].slice(0, lin.cout), lengths=l2)
                 n += 1
                 c0 = lin.cout
             else:
                 # out_nonlinear in the epilogue, then [mean | unbiased std] over T' (no eps) per utterance.  Not the fused
                 # pooling epilogue: its time blocking follows the batch shape, so a batch would not reproduce
                 # per-utterance calls bit for bit; the fp32 round trip costs ~80 MB of traffic at 128 x 300.
-                lin.run(pv, y_f32=ws["pool_in"])
-                stats = ops.stats_pool_ex(ws["pool_in"], 0.0, 1)
+                lin.run(pv, y_f32=ws["pool_in"], lengths=l2)
+                stats = ops.stats_pool_ex(ws["pool_in"], 0.0, 1, lengths=l2)
                 n += 2
         wd, sd, td = self.dense
         emb = ops.small_affine(stats, wd, bn_scale=sd, bn_shift=td)
@@ -490,6 +544,7 @@ class NativeCamPPExtractor(NativeExtractor):
     device that is current when it is built (or loaded from an XVBP0001 file)."""
 
     PREFIX = "campp"
+    TAKES_LENGTHS = True
 
     def _create_args(self, m):
         from asv_subtools_b200._lib import CamPPConfig

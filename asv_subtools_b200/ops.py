@@ -310,9 +310,11 @@ def bn_relu_planes(x, scale, shift, y):
                                  y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_bn_relu_planes")
 
 
-def cam_gate(h, w1, b1, w2, b2, seg_len=100, out=None):
+def cam_gate(h, w1, b1, w2, b2, seg_len=100, out=None, lengths=None):
     """CAMLayer's per-segment mask (xvb_cam_gate): h SplitPlanes (B, T, C); w1 (R, C), b1 (R,), w2 (G, R), b2 (G,) fp32
-    -> gate (B, ceil(T / seg_len), G) fp32 (written into `out` when given)."""
+    -> gate (B, ceil(T / seg_len), G) fp32 (written into `out` when given).  lengths: int32 CUDA (B,) tensor of a masked
+    batch (xvb_cam_gate_lengths): utterance b takes its context from its first lengths[b] frames, and its gate rows past
+    its last segment are zeros."""
     b, t, c = h.hi.shape[0], h.hi.shape[1], h.channels
     w1, w2 = _req(w1, torch.float32, "w1"), _req(w2, torch.float32, "w2")
     r, g = w1.shape[0], w2.shape[0]
@@ -321,9 +323,13 @@ def cam_gate(h, w1, b1, w2, b2, seg_len=100, out=None):
         out = torch.empty(b, nseg, g, dtype=torch.float32, device=h.hi.device)
     elif _req(out, torch.float32, "out").shape != (b, nseg, g):
         raise ValueError("out must be ({}, {}, {})".format(b, nseg, g))
-    check(lib.xvb_cam_gate(h.hi.data_ptr(), h.lo.data_ptr(), h.ld, b, t, c, int(seg_len), _ptr(w1),
-                           _ptr(_req(b1, torch.float32, "b1")), r, _ptr(w2), _ptr(_req(b2, torch.float32, "b2")), g, _ptr(out),
-                           _stream()), "xvb_cam_gate")
+    args = (h.hi.data_ptr(), h.lo.data_ptr(), h.ld, b, t, c, int(seg_len), _ptr(w1), _ptr(_req(b1, torch.float32, "b1")), r,
+            _ptr(w2), _ptr(_req(b2, torch.float32, "b2")), g)
+    if lengths is None:
+        check(lib.xvb_cam_gate(*args, _ptr(out), _stream()), "xvb_cam_gate")
+    else:
+        check(lib.xvb_cam_gate_lengths(*args, _ptr(_req(lengths, torch.int32, "lengths")), _ptr(out), _stream()),
+              "xvb_cam_gate_lengths")
     return out
 
 

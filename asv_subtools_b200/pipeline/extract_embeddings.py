@@ -15,8 +15,9 @@ input key (bucket order).  `--shard i/n` keeps every n-th utterance (one process
 pre-splitting the scp).
 
 `--mixed-lengths` (models whose extractor takes lengths: the TDNN x-vector family with statistics pooling or an attention
-pooling other than LDE -- attentive, multi-head, multi-resolution, xi-vector --, the F-TDNN x-vector and the ResNet
-x-vector): the maxChunk rule cuts every utterance first, and the chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
+pooling other than LDE -- attentive, multi-head, multi-resolution, xi-vector --, the F-TDNN x-vector, the ResNet x-vector
+and CAM++): the model's chunk rule cuts every utterance first (the maxChunk rule, or the model's own `chunk_sizes` where
+it has one: CAM++'s 4000-frame egrecho rule), and the chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
 call, `extract_embedding_batch(x, lengths)`, and each utterance's embedding is sum(len_i * emb_i) / frames over its
 chunks, as `bin/xvb-extract --mixed-lengths` does.  The pooling merge order depends on the batch shape, so the vectors
 differ from the default mode's at the rounding level.
@@ -112,6 +113,13 @@ def chunk_lengths(frames, max_chunk=MAX_CHUNK):
     return [split] * (num_split - 1) + [frames - split * (num_split - 1)]
 
 
+def model_chunk_lengths(model, frames):
+    """The chunks --mixed-lengths cuts a `frames`-long utterance into for `model`: its own rule when the blueprint has
+    one (`model.chunk_sizes(frames)`, e.g. CAM++'s 4000-frame egrecho rule), else the maxChunk rule (chunk_lengths)."""
+    own = getattr(model, "chunk_sizes", None)
+    return list(own(frames)) if own is not None else chunk_lengths(frames)
+
+
 def extract_stream_mixed(model, reader, writer, batch_size=256, shard=(0, 1), log=print, max_pending_frames=4_000_000):
     """--mixed-lengths form of extract_stream.  Returns (utterances, batches, padded frames, batch frames)."""
     utts, items = [], []              # utts: [key, frames, chunks pending, sum(len_i * emb_i)]; items: (utt, chunk)
@@ -148,7 +156,7 @@ def extract_stream_mixed(model, reader, writer, batch_size=256, shard=(0, 1), lo
         if feats.dtype != np.float32:
             raise TypeError("features of {} are {}, the extractor takes float32 (FM/CM) matrices".format(key, feats.dtype))
         count += 1
-        lens = chunk_lengths(feats.shape[0])
+        lens = model_chunk_lengths(model, feats.shape[0])
         utts.append([key, feats.shape[0], len(lens), np.float32(0)])
         off = 0
         for n in lens:
@@ -203,7 +211,7 @@ def main(argv=None):
     ap.add_argument("--shard", type=str, default="0/1", help="i/n: keep utterances with index %% n == i")
     ap.add_argument("--mixed-lengths", action="store_true",
                     help="batch utterances of different lengths (padding at most 1/8 of a batch); TDNN x-vector models with "
-                         "statistics or attention pooling (not LDE), F-TDNN and ResNet x-vector models only")
+                         "statistics or attention pooling (not LDE), F-TDNN, ResNet x-vector and CAM++ models only")
     ap.add_argument("--blueprint-dir", type=str, default="",
                     help="take the blueprint of the same file name from this directory (asv_subtools_b200/model) instead of "
                          "the path stored in nnet.config, so a reference model dir is used as it is")
@@ -235,7 +243,8 @@ def main(argv=None):
             ex = model.extractor()
             if not getattr(ex, "TAKES_LENGTHS", False):
                 print("ERROR: --mixed-lengths needs a TDNN x-vector model with statistics or attention pooling (not LDE), an "
-                      "F-TDNN or a ResNet x-vector; {} runs on {}".format(type(model).__name__, type(ex).__name__),
+                      "F-TDNN, a ResNet x-vector or a CAM++ model; {} runs on {}".format(type(model).__name__,
+                                                                                        type(ex).__name__),
                       file=sys.stderr)
                 sys.exit(1)
         # native ark reader (csrc/ark_io.cpp): the reference's byte-at-a-time key loop is the wall at GPU rates

@@ -453,6 +453,15 @@ int xvb_bn_relu_planes(const uint16_t* x_hi, const uint16_t* x_lo, int64_t ldx, 
  * ceil(T / seg_len), G) fp32.  C % 8 == 0, C <= 2048. */
 int xvb_cam_gate(const uint16_t* h_hi, const uint16_t* h_lo, int64_t ldh, int B, int T, int C, int seg_len, const float* w1,
                  const float* b1, int R, const float* w2, const float* b2, int G, float* gate, void* stream);
+/* xvb_cam_gate over a masked batch: utterance b owns frames [0, lengths[b]) (DEVICE int32[B], 1 <= lengths[b] <= T, at
+ * the gate's own time resolution).  Its context is the mean over its own L frames plus the mean of each of its segments
+ * [s*seg_len, min(L, (s+1)*seg_len)), s < ceil(L / seg_len), in the reduction order of xvb_cam_gate at T = L, so a row
+ * is bit for bit the unmasked call on the utterance alone.  The gate rows of segments wholly past L are written as
+ * zeros; the frames t >= L are never read.  gate keeps the (B, ceil(T / seg_len), G) layout.  XVB_EINVAL on a NULL
+ * lengths. */
+int xvb_cam_gate_lengths(const uint16_t* h_hi, const uint16_t* h_lo, int64_t ldh, int B, int T, int C, int seg_len,
+                         const float* w1, const float* b1, int R, const float* w2, const float* b2, int G, const int* lengths,
+                         float* gate, void* stream);
 
 /* out = z * gate[b, t / seg_len, :] [+ in] over (B, T, C) planes: the kernel of xvb_se_apply with a gate row per
  * seg_len-frame segment (gate (B, ceil(T / seg_len), C) fp32, e.g. from xvb_cam_gate) and an optional `in` (NULL: no
@@ -1066,6 +1075,17 @@ int xvb_campp_last_launches(const xvb_campp_t* h);
 /* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embd_dim) fp32 on the device;
  * asynchronous on `stream`. */
 int xvb_campp_extract(xvb_campp_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* A batch of utterances of different lengths, one chunk each: feats (B, T, feat_dim) fp32 on the device, utterance b in
+ * its first lengths_host[b] frames (HOST int32[B], 3 <= lengths_host[b] <= T; the frames past them are never read,
+ * whatever they hold).  Row b of emb is the embedding of feats[b, :lengths_host[b]] extracted alone, bit for bit: every
+ * kernel reduces an utterance's own frames in the same order whatever the padded T.  The lengths are checked (XVB_EINVAL
+ * naming the first bad one, nothing launched); when all equal T this is xvb_campp_extract.  Otherwise a (2, B) table of
+ * L and L' = ceil(L / 2) (after the stride-2 tdnn) is copied into the workspace on `stream` (the host array may be
+ * reused when the call returns), and every layer stores exact zeros past each utterance's length at its own
+ * resolution, so that the time-padded head copy gives each utterance its own zero padding.  Frame-budget groups as in
+ * xvb_campp_extract. */
+int xvb_campp_extract_lengths(xvb_campp_t* h, const float* feats, const int32_t* lengths_host, int B, int T, float* emb,
+                              void* stream);
 /* "XVBP0001" model files: the configuration, then the records as handed to xvb_campp_set_layer (layout at
  * save_records in csrc/model_file.cpp). */
 int xvb_campp_save(const xvb_campp_t* h, const char* path);

@@ -2,7 +2,7 @@
 """Throughput of an x-vector extractor on a corpus of utterances of different lengths -- a side measurement, not the
 bench.py line.
 
-    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn] [--utts N]
+    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn|campplus] [--utts N]
                                         [--min-frames A] [--max-frames B] [--batch N] [--dim F]
 
 The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
@@ -12,7 +12,10 @@ tools/bench_resnet.py (post-activation blocks with SE, fc1=False, position near)
 batch 128 by default, as bench_resnet.py times it.  --model multihead / xivector / ftdnn: the Python launch sequences of
 the golden configurations at 40-d features (--dim is ignored), position far -- the snowdar x-vector with shared-weight
 four-head attention pooling (tests/golden/make_golden_snowdar.py "mha_share"), the xi-vector posterior-distribution
-pooling ("xi_dist") and the factored F-TDNN (make_golden_ftdnn.py); batch 256, 256 and 128 by default.
+pooling ("xi_dist") and the factored F-TDNN (make_golden_ftdnn.py); batch 256, 256 and 128 by default.  --model
+campplus: the native CAM++ handle with egrecho's default CamPPConfig (embd_dim 512, init_channels 128, growth_rate 32,
+bn_size 4) on 80-d features (--dim is ignored), batch 128 by default, as tools/bench_campplus.py times it; every
+utterance of the default corpus is one chunk of its own length under CAM++'s 4000-frame chunk rule.
 
   * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
     up to `batch` utterances of exactly the same frame count, one xvb_<handle>_extract call each;
@@ -63,9 +66,10 @@ def main():
     ap.add_argument("--utts", type=int, default=4000)
     ap.add_argument("--min-frames", type=int, default=200)
     ap.add_argument("--max-frames", type=int, default=2000)
-    ap.add_argument("--batch", type=int, default=None, help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn)")
+    ap.add_argument("--batch", type=int, default=None,
+                    help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn, campplus)")
     ap.add_argument("--dim", type=int, default=23)
-    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn"], default="xvector")
+    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn", "campplus"], default="xvector")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_mixed_lengths.py needs a GPU")
@@ -95,6 +99,17 @@ def main():
         m = FactoredXvector(F, 10, training=False, extracted_embedding="far")
         m.load_state_dict(onn.make_state_dict(onn.factored_xvector_spec(F), 401), strict=True)
         workload = "factored F-TDNN Xvector(40) far"
+    elif args.model == "campplus":
+        import campplus_oracle as co
+        from asv_subtools_b200.model.campplus_xvector import CamPPXvector
+        F = 80
+        args.batch = args.batch or 128
+        if args.max_frames > 4000:
+            raise SystemExit("--model campplus: every utterance must be one chunk, --max-frames <= 4000")
+        keys = np.load(os.path.join(ROOT, "tests", "golden", "campplus.npz"))["keys_default"]
+        m = CamPPXvector(F, 10)
+        m.load_state_dict(co.seeded_state_dict(keys, 401), strict=True)
+        workload = "CAM++ CamPPConfig defaults (80-d, embd_dim 512)"
     else:
         F = args.dim
         args.batch = args.batch or 256
