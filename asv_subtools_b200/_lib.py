@@ -118,6 +118,7 @@ SIGNATURES = {
     "xvb_copy_rows": (_i, [_p, _i64, _p, _i64, _i64, _i64, _p]),
     "xvb_se_apply": (_i, [_p, _p, _i64, _p, _p, _i64, _p, _p, _p, _i64, _p, _p, _i64, _i, _i, _i, _p]),
     "xvb_attn_stats_pool": (_i, [_p, _i64, _p, _i64, _i, _i, _i, _f, _p, _p, _p, _i64, _p]),
+    "xvb_attn_stats_pool_lengths": (_i, [_p, _i64, _p, _i64, _i, _i, _i, _f, _p, _p, _p, _p, _i64, _p]),
     "xvb_vad_energy": (_i, [_p, _p, _i, _i, _f, _f, _i, _f, _p, _p, _p]),
     "xvb_cmn": (_i, [_p, _p, _i, _i, _i, _p, _p]),
     "xvb_select_frames": (_i, [_p, _p, _p, _p, _i, _i, _p, _p]),
@@ -168,8 +169,10 @@ SIGNATURES = {
     "xvb_conv2d_valid": (_i, [_p, _p]),
     "xvb_subsample_head": (_i, [_p, _i, _i, _i, _p, _p, _i, _p, _p, _p]),
     "xvb_subsample_head_stride": (_i, [_p, _i, _i, _i, _p, _p, _i, _i, _p, _p, _p]),
+    "xvb_subsample_head_lengths": (_i, [_p, _i, _i, _i, _p, _p, _p, _i, _i, _p, _p, _p]),
     "xvb_layer_norm": (_i, [_p, _p]),
     "xvb_rope_attention": (_i, [_p, _i64, _i, _i, _i, _i, _p, _i, _f, _p, _p, _i64, _p]),
+    "xvb_rope_attention_lengths": (_i, [_p, _i64, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _p, _i64, _p]),
     "xvb_conv_module": (_i, [_p, _i64, _i, _i, _i, _p, _p, _i, _p, _p, _i, _f, _i, _p, _p, _i64, _p]),
     "xvb_bn_relu_planes": (_i, [_p, _p, _i64, _i64, _i, _p, _p, _p, _p, _i64, _p]),
     "xvb_cam_gate": (_i, [_p, _p, _i64, _i, _i, _i, _i, _p, _p, _i, _p, _p, _i, _p, _p]),
@@ -248,6 +251,7 @@ SIGNATURES = {
     "xvb_conformer_embed_dim": (_i, [_p]),
     "xvb_conformer_last_launches": (_i, [_p]),
     "xvb_conformer_extract": (_i, [_p, _p, _i, _i, _p, _p]),
+    "xvb_conformer_extract_lengths": (_i, [_p, _p, _p, _i, _i, _p, _p]),
     "xvb_conformer_save": (_i, [_p, C.c_char_p]),
     "xvb_conformer_load": (_i, [C.POINTER(_p), C.c_char_p]),
     "xvb_conformer_destroy": (None, [_p]),

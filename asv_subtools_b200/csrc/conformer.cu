@@ -10,6 +10,8 @@
 //     AttentiveStatsPool's LayerNorms, transformer_xvector.py:39-50);
 //   * multi-head self-attention with rotary position encoding and softmax / softmax_plus (attention.py:255-304,
 //     :640-728), keys tiled with an online softmax so any length works;
+// The head conv and the attention also take a masked batch (lengths): utterance b then runs the unmasked code at its
+// own length, and its rows past that length are written as exact zeros.
 //   * the middle of the convolution module: GLU, depthwise conv, LayerNorm / eval BatchNorm, activation
 //     (convolution.py:87-130).
 #include <cuda_bf16.h>
@@ -68,10 +70,14 @@ __device__ __forceinline__ void warp_layer_norm(float* v, int C, float eps, cons
 
 // ---- the subsampling's first conv: one thread per (output position, 8 channels) --------------------------------------
 // Time stride 2, feature stride sf (2: Conv2dSubsampling4, 1: SVConv2dSubsampling2).  32-bit index arithmetic (the host
-// checks total < 2^31), so decoding the flat index takes no emulated 64-bit division.
-__global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F, int sf, const float* __restrict__ w,
-                                      const float* __restrict__ bias, int C, int T1, int F1, __nv_bfloat16* __restrict__ yh,
-                                      __nv_bfloat16* __restrict__ yl, unsigned total) {
+// checks total < 2^31), so decoding the flat index takes no emulated 64-bit division.  lengths (NULL: every utterance has
+// T frames): the output rows t >= (lengths[b] - 1) / 2 of utterance b are written as zeros and load nothing, so no
+// frame past its end is read; the rows before are computed as for T = lengths[b].  The launch bounds keep the 32
+// registers that fit eight 256-thread CTAs per SM, which the lengths operand would otherwise push to 40.
+__global__ void __launch_bounds__(256, 8)
+subsample_head_kernel(const float* __restrict__ x, int T, int F, int sf, const float* __restrict__ w, const float* __restrict__ bias,
+                      int C, int T1, int F1, const int* __restrict__ lengths, __nv_bfloat16* __restrict__ yh,
+                      __nv_bfloat16* __restrict__ yl, unsigned total) {
   const unsigned groups = (unsigned)C / 8;
   for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
     const int c0 = (int)(i % groups) * 8;
@@ -81,11 +87,12 @@ __global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F,
     const unsigned bt = pos_u / (unsigned)F1;
     const int t = (int)(bt % (unsigned)T1);
     const long long b = bt / (unsigned)T1;
+    const bool live = !lengths || t < (__ldg(lengths + b) - 1) / 2;
     float in[9];
 #pragma unroll
     for (int kt = 0; kt < 3; ++kt)
 #pragma unroll
-      for (int kf = 0; kf < 3; ++kf) in[kt * 3 + kf] = __ldg(x + (b * T + 2 * t + kt) * F + sf * f + kf);
+      for (int kf = 0; kf < 3; ++kf) in[kt * 3 + kf] = live ? __ldg(x + (b * T + 2 * t + kt) * F + sf * f + kf) : 0.f;
     float y[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
@@ -97,6 +104,7 @@ __global__ void subsample_head_kernel(const float* __restrict__ x, int T, int F,
     }
     uint4 h, l;
     pack8(y, h, l);
+    if (!live) h = l = make_uint4(0u, 0u, 0u, 0u);
     *reinterpret_cast<uint4*>(yh + pos * C + c0) = h;
     *reinterpret_cast<uint4*>(yl + pos * C + c0) = l;
   }
@@ -158,6 +166,10 @@ __global__ void layer_norm_kernel(const LnParams p) {
 // One CTA per (utterance, head, 8 queries), one warp per query.  Keys and values are staged 32 at a time (rotated as
 // they are loaded); lane j scores key j of the tile, the running max / sum / output are rescaled per tile (online
 // softmax), and lane l accumulates output dimensions l, l + 32, ...
+// lengths (NULL: every utterance has T frames): utterance b attends over its keys [0, Tb) only, Tb = lengths[b], with the
+// same tiles from key 0, so its rows are those of a call at T = Tb; its query rows past Tb are written as zeros, and a
+// query block wholly past Tb loads nothing.  The score multiplier is mult_table[Tb] when mult_table is set, else mult.
+// The batch stride stays T rows.
 constexpr int kAttnQ = 8;
 constexpr int kAttnK = 32;
 
@@ -172,7 +184,9 @@ __device__ __forceinline__ void rotate_pair(float& a, float& b, const float* rop
 template <int DK>
 __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __restrict__ qkv, long long ldq, int T, int H,
                                                              const float* __restrict__ rope, int rope_v, float sqrt_dk,
-                                                             float mult, __nv_bfloat16* __restrict__ yh,
+                                                             float mult, const int* __restrict__ lengths,
+                                                             const float* __restrict__ mult_table,
+                                                             __nv_bfloat16* __restrict__ yh,
                                                              __nv_bfloat16* __restrict__ yl, long long ldy) {
   __shared__ float Qs[kAttnQ][DK];
   __shared__ float Ks[kAttnK][DK + 1];
@@ -184,11 +198,22 @@ __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __rest
   const int D = H * DK;
   const float* base = qkv + b * T * ldq;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int Tb = lengths ? __ldg(lengths + b) : T;
+  if (mult_table) mult = __ldg(mult_table + Tb);
+  if (qb * kAttnQ >= Tb) {   // a query block wholly past the utterance's end (masked batches only): zero rows
+    const int tq = qb * kAttnQ + warp;
+    if (tq < T) {
+      const long long off = (b * T + tq) * ldy + h * DK + lane;
+#pragma unroll
+      for (int i = 0; i < DK / 32; ++i) store_plane(yh, yl, off + 32 * i, 0.f);
+    }
+    return;
+  }
 
   for (int i = threadIdx.x; i < kAttnQ * DK / 2; i += blockDim.x) {
     const int r = i / (DK / 2), j = i % (DK / 2), t = qb * kAttnQ + r;
     float a = 0.f, c = 0.f;
-    if (t < T) {
+    if (t < Tb) {
       const float* q = base + t * ldq + h * DK;
       a = q[2 * j];
       c = q[2 * j + 1];
@@ -201,12 +226,12 @@ __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __rest
   float m = -INFINITY, l = 0.f, o[DK / 32];
 #pragma unroll
   for (int i = 0; i < DK / 32; ++i) o[i] = 0.f;
-  for (int k0 = 0; k0 < T; k0 += kAttnK) {
+  for (int k0 = 0; k0 < Tb; k0 += kAttnK) {
     __syncthreads();   // Q staged / the previous tile consumed
     for (int i = threadIdx.x; i < kAttnK * DK / 2; i += blockDim.x) {
       const int r = i / (DK / 2), j = i % (DK / 2), t = k0 + r;
       float ka = 0.f, kc = 0.f, va = 0.f, vc = 0.f;
-      if (t < T) {
+      if (t < Tb) {
         const float* row = base + t * ldq + h * DK;
         ka = row[D + 2 * j];
         kc = row[D + 2 * j + 1];
@@ -223,7 +248,7 @@ __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __rest
       Vs[r][2 * j + 1] = vc;
     }
     __syncthreads();
-    const bool valid = k0 + lane < T;
+    const bool valid = k0 + lane < Tb;
     float s = -INFINITY;
     if (valid) {
       float d = 0.f;
@@ -237,7 +262,7 @@ __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __rest
     l = fmaf(l, corr, warp_sum(pj));
 #pragma unroll
     for (int i = 0; i < DK / 32; ++i) o[i] *= corr;
-    const int nk = min(kAttnK, T - k0);
+    const int nk = min(kAttnK, Tb - k0);
     for (int j = 0; j < nk; ++j) {
       const float pb = __shfl_sync(0xffffffffu, pj, j);
 #pragma unroll
@@ -248,9 +273,10 @@ __global__ void __launch_bounds__(256) rope_attention_kernel(const float* __rest
   const int tq = qb * kAttnQ + warp;
   if (tq < T) {
     const float inv = 1.f / l;
+    const bool live = tq < Tb;
     const long long off = (b * T + tq) * ldy + h * DK + lane;
 #pragma unroll
-    for (int i = 0; i < DK / 32; ++i) store_plane(yh, yl, off + 32 * i, o[i] * inv);
+    for (int i = 0; i < DK / 32; ++i) store_plane(yh, yl, off + 32 * i, live ? o[i] * inv : 0.f);
   }
 }
 
@@ -313,8 +339,8 @@ int grid_cap(long long want) {
 
 using namespace xvb;
 
-extern "C" int xvb_subsample_head_stride(const float* x, int B, int T, int F, const float* w, const float* bias, int C,
-                                         int stride_f, uint16_t* y_hi, uint16_t* y_lo, void* stream) {
+static int subsample_head(const float* x, int B, int T, int F, const int* lengths, const float* w, const float* bias, int C,
+                          int stride_f, uint16_t* y_hi, uint16_t* y_lo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(x && w && bias && y_hi && y_lo, "xvb_subsample_head: null pointer");
@@ -326,10 +352,22 @@ extern "C" int xvb_subsample_head_stride(const float* x, int B, int T, int F, co
   const long long total = (long long)B * T1 * F1 * (C / 8);
   XVB_CHECK_ARG(total < (1LL << 31), "xvb_subsample_head: %lld (position, 8-channel) items exceed one launch", total);
   subsample_head_kernel<<<grid_cap((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-      x, T, F, stride_f, w, bias, C, T1, F1, reinterpret_cast<__nv_bfloat16*>(y_hi), reinterpret_cast<__nv_bfloat16*>(y_lo),
-      (unsigned)total);
+      x, T, F, stride_f, w, bias, C, T1, F1, lengths, reinterpret_cast<__nv_bfloat16*>(y_hi),
+      reinterpret_cast<__nv_bfloat16*>(y_lo), (unsigned)total);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
+}
+
+extern "C" int xvb_subsample_head_stride(const float* x, int B, int T, int F, const float* w, const float* bias, int C,
+                                         int stride_f, uint16_t* y_hi, uint16_t* y_lo, void* stream) {
+  return subsample_head(x, B, T, F, nullptr, w, bias, C, stride_f, y_hi, y_lo, stream);
+}
+
+extern "C" int xvb_subsample_head_lengths(const float* x, int B, int T, int F, const int* lengths, const float* w,
+                                          const float* bias, int C, int stride_f, uint16_t* y_hi, uint16_t* y_lo,
+                                          void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_subsample_head_lengths: null lengths");
+  return subsample_head(x, B, T, F, lengths, w, bias, C, stride_f, y_hi, y_lo, stream);
 }
 
 extern "C" int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, const float* bias, int C, uint16_t* y_hi,
@@ -372,8 +410,9 @@ extern "C" int xvb_layer_norm(const xvb_layer_norm_args_t* a, void* stream) {
   return XVB_OK;
 }
 
-extern "C" int xvb_rope_attention(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
-                                  float score_mult, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream) {
+static int rope_attention(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
+                          float score_mult, const int* lengths, const float* mult_table, uint16_t* y_hi, uint16_t* y_lo,
+                          int64_t ldy, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(qkv && y_hi && y_lo, "xvb_rope_attention: null pointer");
@@ -388,13 +427,31 @@ extern "C" int xvb_rope_attention(const float* qkv, int64_t ldq, int B, int T, i
   auto* yl = reinterpret_cast<__nv_bfloat16*>(y_lo);
   cudaStream_t s = (cudaStream_t)stream;
   if (dk == 32)
-    rope_attention_kernel<32><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, yh, yl, ldy);
+    rope_attention_kernel<32><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, lengths, mult_table,
+                                                             yh, yl, ldy);
   else if (dk == 64)
-    rope_attention_kernel<64><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, yh, yl, ldy);
+    rope_attention_kernel<64><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, lengths, mult_table,
+                                                             yh, yl, ldy);
   else
-    rope_attention_kernel<128><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, yh, yl, ldy);
+    rope_attention_kernel<128><<<(unsigned)grid, 256, 0, s>>>(qkv, ldq, T, H, rope, rope_v, sq, score_mult, lengths,
+                                                              mult_table, yh, yl, ldy);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
+}
+
+extern "C" int xvb_rope_attention(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
+                                  float score_mult, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream) {
+  return rope_attention(qkv, ldq, B, T, H, dk, rope, rope_v, score_mult, nullptr, nullptr, y_hi, y_lo, ldy, stream);
+}
+
+extern "C" int xvb_rope_attention_lengths(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope,
+                                          int rope_v, const int* lengths, const float* mult_table, int mult_rows,
+                                          uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_rope_attention_lengths: null lengths");
+  // lengths[b] <= T < mult_rows keeps every mult_table[lengths[b]] inside the table
+  XVB_CHECK_ARG(!mult_table || (mult_rows > 0 && T < mult_rows),
+                "xvb_rope_attention_lengths: T=%d needs a multiplier table of more than T rows (mult_rows=%d)", T, mult_rows);
+  return rope_attention(qkv, ldq, B, T, H, dk, rope, rope_v, 1.0f, lengths, mult_table, y_hi, y_lo, ldy, stream);
 }
 
 extern "C" int xvb_conv_module(const float* x, int64_t ldx, int B, int T, int C, const float* dw_w, const float* dw_b, int K,

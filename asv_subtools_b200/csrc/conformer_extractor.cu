@@ -12,6 +12,10 @@
 // Records arrive by state_dict module path after the Python side's hand-over transforms (see xvb200.h); this file only
 // packs them.  The positional table and the softmax_plus score multipliers are handed over too, so nothing here
 // computes a transcendental value the driver takes from torch.
+//
+// A masked batch (xvb_conformer_extract_lengths) runs the same sequence with each utterance's lengths: the head conv,
+// every frame-level linear, the attention and the attentive pooling run masked; the valid conv, the convolution module
+// and the LayerNorms need no mask (see extract_group).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -40,6 +44,7 @@ struct Layer {
   float* dw_w = nullptr; float* dw_b = nullptr;
   Ln cm_norm, norm_ff, norm_mha, norm_ff_macaron, norm_conv, norm_final;
   std::vector<float> mult;   // softmax_plus score multiplier per T' (host; passed by value to the kernel)
+  float* mult_dev = nullptr;  // the same table on the device, indexed by each utterance's T' in a masked batch
 };
 struct Seg { Affine lin; bool ln = false; Ln norm; };
 
@@ -78,14 +83,14 @@ void sub_shape(const xvb_conformer_config_t& c, int T, int* T1, int* F1, int* T2
 }  // namespace
 
 struct xvb_conformer : Handle<Model> {
-  enum { kX1, kX2, kR, kH, kHid, kDelta, kQkv, kXo, kXp, kA1, kAp, kLogits, kStats, kZ, kZf, kSegY, kSegP, kBufs };
+  enum { kX1, kX2, kR, kH, kHid, kDelta, kQkv, kXo, kXp, kA1, kAp, kLogits, kStats, kZ, kZf, kSegY, kSegP, kLengths, kBufs };
   Workspace<kBufs> ws;
 };
 
 namespace {
 
 const bool kPlanes[xvb_conformer::kBufs] = {true, true, false, true, true, false, false, false, true, false, true, false,
-                                            false, true, false, false, true};
+                                            false, true, false, false, true, false};
 
 int reserve(xvb_conformer* h, int B, int T) {
   const xvb_conformer_config_t& c = h->m->cfg;
@@ -97,17 +102,20 @@ int reserve(xvb_conformer* h, int B, int T) {
   for (const Seg& s : h->m->seg) seg = (size_t)s.lin.Cout > seg ? (size_t)s.lin.Cout : seg;
   const size_t need[xvb_conformer::kBufs] = {
       b * T1 * F1 * D, b * T2 * F2 * D, r2 * D, r2 * D, r2 * units, r2 * 2 * D, r2 * 3 * D, r2 * od, r2 * od,
-      r2 * c.pool_hidden, r2 * c.pool_hidden, r2 * od, b * 2 * od, b * 2 * od, b * 2 * od, b * seg, b * seg};
+      r2 * c.pool_hidden, r2 * c.pool_hidden, r2 * od, b * 2 * od, b * 2 * od, b * 2 * od, b * seg, b * seg,
+      0};   // kLengths: sized by xvb_conformer_extract_lengths for the whole call, before its groups run
   uint64_t grown;
   return h->ws.reserve(need, kPlanes, &grown);
 }
 
-// ops.PackedAffine.run: x planes (B, T, l.Cin) with row pitch ldx -> y planes (pitch ldy) and / or yf (pitch ldyf)
+// ops.PackedAffine.run: x planes (B, T, l.Cin) with row pitch ldx -> y planes (pitch ldy) and / or yf (pitch ldyf);
+// lens: NULL, or a masked batch's frame counts (the rows past them store zeros)
 int lin(const Affine& l, Planes x, int64_t ldx, int B, int T, const Planes* y, int64_t ldy, float* yf, int64_t ldyf,
-        void* stream) {
+        const int* lens, void* stream) {
   xvb_tdnn_args_t a = affine_args(l, x, ldx, B, T);
   if (y) { a.y_hi = y->hi; a.y_lo = y->lo; a.ldy = ldy; }
   a.y_f32 = yf; a.ldyf = ldyf;
+  a.lengths = lens;
   return xvb_tdnn_affine_ex(&a, stream);
 }
 
@@ -136,8 +144,15 @@ int layer_norm(const LnCall& c, void* stream) {
   return xvb_layer_norm(&a, stream);
 }
 
-// One group of utterances: ConformerExtractor.extract.  *n counts the launches as the driver does.
-int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb, int* n, void* stream) {
+// One group of utterances: ConformerExtractor.extract.  *n counts the launches as the driver does.  A masked group passes
+// lens, its frame counts L in row 0 of the workspace's (2, ld) table and their subsampled lengths L' in row 1; NULL
+// otherwise.  Masked, the head conv zeroes its rows t1 >= (L - 1) / 2, and every frame-level linear, the attention and the
+// pooling take L'.  Three kernels need no mask: the valid conv's rows t' < L' read only head rows below (L - 1) / 2; the
+// convolution module reads pointwise_conv1's exact zeros past L' (GLU(0, 0) = 0), which is the zero padding an
+// utterance alone gets; and the LayerNorms work row by row, their rows past L' staying finite and read by nothing that
+// crosses frames.  So each row is its utterance extracted alone.
+int extract_group(xvb_conformer* h, const float* feats, int B, int T, const int* lens, int ld, float* emb, int* n,
+                  void* stream) {
   int rc = reserve(h, B, T);
   if (rc) return rc;
   const Model* m = h->m.get();
@@ -147,7 +162,11 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   sub_shape(c, T, &T1, &F1, &T2, &F2);
   const long long rows = (long long)B * T2;
   const Planes x1 = h->ws.planes(xvb_conformer::kX1), x2 = h->ws.planes(xvb_conformer::kX2);
-  if (c.subsampling == 4)
+  const int* lens2 = lens ? lens + ld : nullptr;   // L', after the subsampling
+  if (lens)
+    rc = xvb_subsample_head_lengths(feats, B, T, c.feat_dim, lens, m->head_w, m->head_b, D, c.subsampling == 4 ? 2 : 1, x1.hi,
+                                    x1.lo, stream);
+  else if (c.subsampling == 4)
     rc = xvb_subsample_head(feats, B, T, c.feat_dim, m->head_w, m->head_b, D, x1.hi, x1.lo, stream);
   else
     rc = xvb_subsample_head_stride(feats, B, T, c.feat_dim, m->head_w, m->head_b, D, 1, x1.hi, x1.lo, stream);
@@ -163,7 +182,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     if ((rc = xvb_conv2d_valid(&a, stream)) != XVB_OK) return rc;
   }
   float* r = h->ws.f32(xvb_conformer::kR);
-  if ((rc = lin(m->embed_out, x2, (int64_t)F2 * D, B, T2, nullptr, 0, r, D, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->embed_out, x2, (int64_t)F2 * D, B, T2, nullptr, 0, r, D, lens2, stream)) != XVB_OK) return rc;
   *n += 3;
   const int units = c.linear_units;
   const int hid_ld = units > D ? units : D;
@@ -174,8 +193,8 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   const float* rope = c.pos == 2 ? m->table : nullptr;
   const float* absp = c.pos == 1 ? m->table : nullptr;
   auto ffn = [&](const Affine& a, const Affine& b) -> int {
-    int e = lin(a, hh, D, B, T2, &hid, hid_ld, nullptr, 0, stream);
-    return e ? e : lin(b, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream);
+    int e = lin(a, hh, D, B, T2, &hid, hid_ld, nullptr, 0, lens2, stream);
+    return e ? e : lin(b, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, lens2, stream);
   };
   {
     LnCall l{rows, D, r, D};
@@ -196,20 +215,24 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     l.n = L.norm_mha;
     l.y = &hh; l.ldy = D;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
-    if ((rc = lin(L.qkv, hh, D, B, T2, nullptr, 0, qkv, 3 * D, stream)) != XVB_OK) return rc;
-    const float mult = c.softmax_plus ? L.mult[T2] : 1.0f;
-    if ((rc = xvb_rope_attention(qkv, 3 * D, B, T2, c.H, m->dk, rope, c.rotary_value && rope ? 1 : 0, mult, hid.hi, hid.lo,
-                                 hid_ld, stream)))
-      return rc;
-    if ((rc = lin(L.out, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.qkv, hh, D, B, T2, nullptr, 0, qkv, 3 * D, lens2, stream)) != XVB_OK) return rc;
+    const int rope_v = c.rotary_value && rope ? 1 : 0;
+    if (lens2)
+      rc = xvb_rope_attention_lengths(qkv, 3 * D, B, T2, c.H, m->dk, rope, rope_v, lens2, c.softmax_plus ? L.mult_dev : nullptr,
+                                      kTableRows, hid.hi, hid.lo, hid_ld, stream);
+    else
+      rc = xvb_rope_attention(qkv, 3 * D, B, T2, c.H, m->dk, rope, rope_v, c.softmax_plus ? L.mult[T2] : 1.0f, hid.hi, hid.lo,
+                              hid_ld, stream);
+    if (rc) return rc;
+    if ((rc = lin(L.out, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, lens2, stream)) != XVB_OK) return rc;
     l.delta_scale = 1.0f;
     l.n = L.norm_conv;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
-    if ((rc = lin(L.pw1, hh, D, B, T2, nullptr, 0, delta, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.pw1, hh, D, B, T2, nullptr, 0, delta, 2 * D, lens2, stream)) != XVB_OK) return rc;
     if ((rc = xvb_conv_module(delta, 2 * D, B, T2, D, L.dw_w, L.dw_b, c.conv_kernel, L.cm_norm.g, L.cm_norm.b, c.cm_norm,
                               1e-5f, c.act, hid.hi, hid.lo, hid_ld, stream)))
       return rc;
-    if ((rc = lin(L.pw2, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, stream)) != XVB_OK) return rc;
+    if ((rc = lin(L.pw2, hid, hid_ld, B, T2, nullptr, 0, d1, 2 * D, lens2, stream)) != XVB_OK) return rc;
     l.n = L.norm_ff;
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
     if ((rc = ffn(L.ff1, L.ff2)) != XVB_OK) return rc;
@@ -225,10 +248,10 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   float* xo = h->ws.f32(xvb_conformer::kXo);
   const Planes xp = h->ws.planes(xvb_conformer::kXp);
   if (!m->transform_ln) {
-    if ((rc = lin(m->transform, hh, D, B, T2, &xp, od, xo, od, stream)) != XVB_OK) return rc;
+    if ((rc = lin(m->transform, hh, D, B, T2, &xp, od, xo, od, lens2, stream)) != XVB_OK) return rc;
     *n += 1;
   } else {
-    if ((rc = lin(m->transform, hh, D, B, T2, nullptr, 0, xo, od, stream)) != XVB_OK) return rc;
+    if ((rc = lin(m->transform, hh, D, B, T2, nullptr, 0, xo, od, lens2, stream)) != XVB_OK) return rc;
     LnCall l{rows, od, xo, od};
     l.n = m->transform_norm;
     l.y = &xp; l.ldy = od;
@@ -238,7 +261,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
   }
   // AttentiveStatsPool
   float* a1 = h->ws.f32(xvb_conformer::kA1);
-  if ((rc = lin(m->att1, xp, od, B, T2, nullptr, 0, a1, hd, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->att1, xp, od, B, T2, nullptr, 0, a1, hd, lens2, stream)) != XVB_OK) return rc;
   const Planes ap = h->ws.planes(xvb_conformer::kAp);
   {
     LnCall l{rows, hd, a1, hd};
@@ -248,9 +271,11 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     if ((rc = layer_norm(l, stream)) != XVB_OK) return rc;
   }
   float* logits = h->ws.f32(xvb_conformer::kLogits);
-  if ((rc = lin(m->att2, ap, hd, B, T2, nullptr, 0, logits, od, stream)) != XVB_OK) return rc;
+  if ((rc = lin(m->att2, ap, hd, B, T2, nullptr, 0, logits, od, lens2, stream)) != XVB_OK) return rc;
   float* stats = h->ws.f32(xvb_conformer::kStats);
-  if ((rc = xvb_attn_stats_pool(logits, od, xo, od, B, T2, od, 1e-5f, stats, nullptr, nullptr, 2 * od, stream)) != XVB_OK) return rc;
+  rc = lens2 ? xvb_attn_stats_pool_lengths(logits, od, xo, od, B, T2, od, 1e-5f, lens2, stats, nullptr, nullptr, 2 * od, stream)
+             : xvb_attn_stats_pool(logits, od, xo, od, B, T2, od, 1e-5f, stats, nullptr, nullptr, 2 * od, stream);
+  if (rc) return rc;
   Planes z = h->ws.planes(xvb_conformer::kZ);
   float* zf = h->ws.f32(xvb_conformer::kZf);
   {
@@ -268,7 +293,7 @@ int extract_group(xvb_conformer* h, const float* feats, int B, int T, float* emb
     const bool last = j + 1 == ns;
     const int co = s.lin.Cout;
     float* y = last ? emb : h->ws.f32(xvb_conformer::kSegY);
-    if ((rc = lin(s.lin, z, zc, B, 1, nullptr, 0, y, co, stream)) != XVB_OK) return rc;
+    if ((rc = lin(s.lin, z, zc, B, 1, nullptr, 0, y, co, nullptr, stream)) != XVB_OK) return rc;
     *n += 1;
     const Planes yp = h->ws.planes(xvb_conformer::kSegP);
     if (s.ln) {
@@ -410,6 +435,7 @@ static int build(Model* m, RecordStore& recs) {
     if (c.softmax_plus) {
       if ((rc = need(p + "self_attn.att_norm", 1, kTableRows, &r)) != XVB_OK) return rc;
       L.mult = r->w;
+      if ((rc = m->dev.upload(&L.mult_dev, L.mult)) != XVB_OK) return rc;
     }
     m->layers.push_back(std::move(L));
   }
@@ -468,7 +494,41 @@ extern "C" int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int
   const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->E;
   int n = 0;
   int rc = for_groups(B, T, kFrameBudget,
-                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, emb + i * E, &n, stream); });
+                      [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, nullptr, 0, emb + i * E, &n, stream); });
+  if (rc) return rc;
+  h->last_launches = n;
+  return XVB_OK;
+}
+
+extern "C" int xvb_conformer_extract_lengths(xvb_conformer_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
+                                             float* emb, void* stream) {
+  const char* fn = "xvb_conformer_extract_lengths";
+  XVB_CHECK_ARG(finalized(h), "%s: model not finalized", fn);
+  XVB_CHECK_ARG(feats && lengths_host && emb && B > 0 && T > 0, "%s: bad arguments", fn);
+  bool all_T;
+  int rc = check_lengths(fn, lengths_host, B, T, &all_T, kMinFrames);
+  if (rc) return rc;
+  int T1, F1, T2, F2;
+  sub_shape(h->m->cfg, T, &T1, &F1, &T2, &F2);   // the longest utterance's T' bounds every other one
+  XVB_CHECK_ARG(T2 < kTableRows, "%s: a chunk of %d subsampled frames exceeds the positional tables' %d", fn, T2, kTableRows);
+  if (all_T) return xvb_conformer_extract(h, feats, B, T, emb, stream);   // nothing to mask: the unmasked call itself
+  // row 0: L, the head conv's input length; row 1: L', the utterance's length after the subsampling
+  std::vector<int32_t> table((size_t)2 * B);
+  for (int b = 0; b < B; ++b) {
+    table[b] = lengths_host[b];
+    sub_shape(h->m->cfg, lengths_host[b], &T1, &F1, &table[(size_t)B + b], &F2);
+  }
+  size_t need[xvb_conformer::kBufs] = {0};
+  uint64_t grown;
+  need[xvb_conformer::kLengths] = table.size();
+  if ((rc = h->ws.reserve(need, kPlanes, &grown))) return rc;
+  int* lens = h->ws.i32(xvb_conformer::kLengths);
+  // stream-ordered: the previous call's kernels on `stream` have read the old table before this one lands
+  XVB_CUDA(cudaMemcpyAsync(lens, table.data(), table.size() * sizeof(int32_t), cudaMemcpyHostToDevice, (cudaStream_t)stream));
+  const size_t per_utt = (size_t)T * h->m->cfg.feat_dim, E = (size_t)h->m->E;
+  int n = 0;
+  rc = for_groups(B, T, kFrameBudget,
+                  [&](int i, int b) { return extract_group(h, feats + i * per_utt, b, T, lens + i, B, emb + i * E, &n, stream); });
   if (rc) return rc;
   h->last_launches = n;
   return XVB_OK;

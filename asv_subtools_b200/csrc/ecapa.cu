@@ -156,9 +156,12 @@ __device__ __forceinline__ void online_merge(Online& a, const Online& b) {
 
 __global__ void __launch_bounds__(kApWarps * 32)
 attn_stats_pool_kernel(const float* __restrict__ logits, long long ldl, const float* __restrict__ x, long long ldx, int T,
-                       int C, float floor_, float* __restrict__ out, __nv_bfloat16* __restrict__ oh,
-                       __nv_bfloat16* __restrict__ ol, long long ldo) {
+                       int C, float floor_, const int* __restrict__ lengths, float* __restrict__ out,
+                       __nv_bfloat16* __restrict__ oh, __nv_bfloat16* __restrict__ ol, long long ldo) {
   const int b = blockIdx.y;
+  // a masked batch reduces utterance b over its own frames [0, Tb) with the same walk, as a call at T = Tb would; the
+  // batch stride stays T rows and the frames past Tb are never loaded
+  const int Tb = lengths ? __ldg(lengths + b) : T;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int c = blockIdx.x * 128 + lane * 4;
   const bool active = c < C;
@@ -168,19 +171,19 @@ attn_stats_pool_kernel(const float* __restrict__ logits, long long ldl, const fl
   if (active) {
     const float* lb = logits + (long long)b * T * ldl + c;
     const float* xb = x + (long long)b * T * ldx + c;
-    for (int t0 = warp; t0 < T; t0 += kApWarps * kApRows) {
+    for (int t0 = warp; t0 < Tb; t0 += kApWarps * kApRows) {
       float4 lv[kApRows], xv[kApRows];
 #pragma unroll
       for (int r = 0; r < kApRows; ++r) {
         const int t = t0 + r * kApWarps;
-        if (t < T) {
+        if (t < Tb) {
           lv[r] = __ldcs(reinterpret_cast<const float4*>(lb + (long long)t * ldl));
           xv[r] = __ldcs(reinterpret_cast<const float4*>(xb + (long long)t * ldx));
         }
       }
 #pragma unroll
       for (int r = 0; r < kApRows; ++r) {
-        if (t0 + r * kApWarps < T) {
+        if (t0 + r * kApWarps < Tb) {
           online_add(st[0], lv[r].x, xv[r].x);
           online_add(st[1], lv[r].y, xv[r].y);
           online_add(st[2], lv[r].z, xv[r].z);
@@ -786,9 +789,8 @@ extern "C" int xvb_seg_gate_apply(const uint16_t* z_hi, const uint16_t* z_lo, in
                          stream);
 }
 
-extern "C" int xvb_attn_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C,
-                                   float floor_, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo,
-                                   void* stream) {
+static int attn_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C, float floor_,
+                           const int* lengths, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream) {
   int rc = require_sm90();
   if (rc) return rc;
   XVB_CHECK_ARG(logits && x && out, "xvb_attn_stats_pool: null pointer");
@@ -798,8 +800,21 @@ extern "C" int xvb_attn_stats_pool(const float* logits, int64_t ldl, const float
   if (out_hi) XVB_CHECK_ARG(ldo % 4 == 0 && ldo >= 2 * C, "xvb_attn_stats_pool: ldo too small / unaligned");
   dim3 grid((C + 127) / 128, B);
   attn_stats_pool_kernel<<<grid, kApWarps * 32, 0, (cudaStream_t)stream>>>(
-      logits, ldl, x, ldx, T, C, floor_, out, reinterpret_cast<__nv_bfloat16*>(out_hi),
+      logits, ldl, x, ldx, T, C, floor_, lengths, out, reinterpret_cast<__nv_bfloat16*>(out_hi),
       reinterpret_cast<__nv_bfloat16*>(out_lo), ldo);
   XVB_LAUNCH_CHECK();
   return XVB_OK;
+}
+
+extern "C" int xvb_attn_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C,
+                                   float floor_, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo,
+                                   void* stream) {
+  return attn_stats_pool(logits, ldl, x, ldx, B, T, C, floor_, nullptr, out, out_hi, out_lo, ldo, stream);
+}
+
+extern "C" int xvb_attn_stats_pool_lengths(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C,
+                                           float floor_, const int* lengths, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                                           int64_t ldo, void* stream) {
+  XVB_CHECK_ARG(lengths, "xvb_attn_stats_pool_lengths: null lengths");
+  return attn_stats_pool(logits, ldl, x, ldx, B, T, C, floor_, lengths, out, out_hi, out_lo, ldo, stream);
 }

@@ -21,9 +21,9 @@
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), each written by its native extractor's save() (model_file.cpp).  What it adds:
 // utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector, ResNet
-// x-vector and CAM++ files) chunks of different lengths share masked batches (plan_mixed_batches,
-// xvb_extractor_extract_lengths / xvb_resnet_extract_lengths / xvb_campp_extract_lengths), which fills batches on a real
-// corpus where most frame counts occur a few times only.
+// x-vector, Conformer and CAM++ files) chunks of different lengths share masked batches (plan_mixed_batches,
+// xvb_extractor_extract_lengths / xvb_resnet_extract_lengths / xvb_conformer_extract_lengths / xvb_campp_extract_lengths),
+// which fills batches on a real corpus where most frame counts occur a few times only.
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
 //     the last chunk takes the remainder, embedding = sum(len_i * emb_i) / T in fp32.  The default max-chunk is
 //     10000, or 300 for a Conformer model, its own maxChunk (transformer_xvector.py:321);
@@ -100,7 +100,10 @@ const Family kFamilies[] = {
        return xvb_resnet_extract_lengths((xvb_resnet_t*)h, x, lens, B, T, e, nullptr);
      }},
     {{"XVBV0001", nullptr}, "loading the RepVGG model", "xvb_repvgg_extract", HANDLE_FAMILY(repvgg), 10000, false, nullptr},
-    {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false, nullptr},
+    {{"XVBC0001", nullptr}, "loading the Conformer model", "xvb_conformer_extract", HANDLE_FAMILY(conformer), 300, false,
+     [](void* h, const float* x, const int32_t* lens, int B, int T, float* e) {
+       return xvb_conformer_extract_lengths((xvb_conformer_t*)h, x, lens, B, T, e, nullptr);
+     }},
     {{"XVBP0001", nullptr}, "loading the CAM++ model", "xvb_campp_extract", HANDLE_FAMILY(campp), 4000, true,
      [](void* h, const float* x, const int32_t* lens, int B, int T, float* e) {
        return xvb_campp_extract_lengths((xvb_campp_t*)h, x, lens, B, T, e, nullptr);
@@ -322,10 +325,10 @@ int main(int argc, char** argv) {
              "least 7 frames and fewer than 5000 subsampled frames.  CAM++ and egrecho ECAPA-TDNN cut an utterance with\n"
              "egrecho's rule (max-chunk-long chunks, the last two re-split evenly: 9000 -> 4000, 2500, 2500); a CAM++ chunk\n"
              "needs at least 3 frames.\n"
-             "--mixed-lengths (TDNN x-vector, ResNet x-vector and CAM++ models): after the chunk rule, chunks of different\n"
-             "lengths share batches of up to --batch, taken in ascending length, with at most 1/8 of a batch's frames\n"
-             "padding; the summary line also reports the padded frames.  Vectors differ from the default mode's at the\n"
-             "rounding level.\n");
+             "--mixed-lengths (TDNN x-vector, ResNet x-vector, Conformer and CAM++ models): after the chunk rule, chunks of\n"
+             "different lengths share batches of up to --batch, taken in ascending length, with at most 1/8 of a batch's\n"
+             "frames padding; the summary line also reports the padded frames.  Vectors differ from the default mode's at\n"
+             "the rounding level.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -352,8 +355,8 @@ int main(int argc, char** argv) {
     r.D = r.fam->embed_dim(r.model);
     if (!max_chunk_set) max_chunk = r.fam->max_chunk;
     if (mixed && !r.fam->extract_lengths) {
-      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector (XVBM0001), ResNet x-vector (XVBR0001) or "
-                      "CAM++ (XVBP0001) model; '%s' is read with %s\n", pos[0],
+      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector (XVBM0001), ResNet x-vector (XVBR0001), "
+                      "Conformer (XVBC0001) or CAM++ (XVBP0001) model; '%s' is read with %s\n", pos[0],
               r.fam->extract_fn);
       return 1;
     }

@@ -31,7 +31,10 @@ arguments in the same order, kept as the A/B and profiling twin; the two give bi
 extract_embedding keeps the reference's maxChunk = 300 chunk rule (for_extract_embedding, framework.py:12-55): an
 utterance is cut into num_split = ceil(T / 300) chunks, each chunk is extracted on its own and the embeddings are
 averaged weighted by chunk length.  extract_embedding_batch applies the same rule to a batch of equal-length
-utterances with two stack runs (all full chunks, then all last chunks)."""
+utterances with two stack runs (all full chunks, then all last chunks).  extract_embedding_batch(feats, lengths) takes a
+masked batch of single chunks of different lengths (cut by chunk_sizes first): the head conv, every frame-level linear,
+the attention and the attentive pooling then run at each utterance's own length, and each row is its chunk extracted
+alone, bit for bit."""
 import copy
 import ctypes as C
 import math
@@ -48,7 +51,7 @@ from asv_subtools_b200 import ops  # noqa: E402
 from asv_subtools_b200._lib import ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH, BN, RELU, SWISH  # noqa: E402
 from asv_subtools_b200.nnet import TopVirtualNnet  # noqa: E402
 from asv_subtools_b200.nnet.components import TdnnAffine, fold_batchnorm  # noqa: E402
-from asv_subtools_b200.native import NativeExtractor  # noqa: E402
+from asv_subtools_b200.native import NativeExtractor, host_lengths  # noqa: E402
 from asv_subtools_b200.nnet.framework import for_extract_embedding  # noqa: E402
 
 MAX_CHUNK = 300     # @for_extract_embedding(maxChunk=300) of transformer_xvector.py:321
@@ -256,7 +259,11 @@ class _AttentiveStatsPool(nn.Module):
 
 
 class TransformerXvector(TopVirtualNnet):
-    """A Conformer x-vector framework."""
+    """A Conformer x-vector framework.
+
+    `masked_chunks`, set by init: extract_embedding_batch takes lengths (a masked batch of single chunks) on this
+    instance.  An object that init did not build refuses lengths with NotImplementedError before it reads any
+    configuration."""
 
     def init(self, inputs_dim, num_targets, embd_dim=256, training=True,
              extracted_embedding="near", mixup=False, mixup_alpha=1.0, pooling="ecpa-attentive", pooling_params={},
@@ -293,6 +300,7 @@ class TransformerXvector(TopVirtualNnet):
         fc1_params = _assign(default_fc_params, fc1_params)
         fc2_params = _assign(default_fc_params, fc2_params)
         self.inputs_dim = inputs_dim
+        self.masked_chunks = True
         self.extracted_embedding = extracted_embedding
         self.use_step, self.step_params = use_step, step_params
         self.embd_dim = embd_dim
@@ -332,14 +340,25 @@ class TransformerXvector(TopVirtualNnet):
             raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, int(feats.shape[0])))
         return self._extract_embedding_chunked(feats)
 
+    def chunk_sizes(self, num_frames):
+        """The chunk lengths extract_embedding cuts a num_frames-long utterance into (the reference's maxChunk = 300
+        rule, chunk_plan); pipeline/extract_embeddings.py --mixed-lengths cuts utterances with it before batching them."""
+        return chunk_plan(num_frames)[0]
+
     def extract_embedding_batch(self, feats, lengths=None):
         """Equal-length utterances (B, T, F) float32 -> (B, D) CUDA tensor, the same arithmetic as B calls of
         extract_embedding(): the B * (num_split - 1) full chunks run as one batch, the B last chunks as another, and the
-        chunk embeddings are recombined with the reference's length-weighted average."""
+        chunk embeddings are recombined with the reference's length-weighted average.
+
+        lengths (B,) host ints: a masked batch of single chunks of different lengths padded to T, row b being the
+        embedding of feats[b, :lengths[b]] extracted as one chunk (what is past it is never read).  Rows are not cut
+        again: the chunk rule itself gives chunks of up to 300 + num_split - 1 frames.  ValueError for a length outside
+        [7, T], naming the first such entry, and for T' >= 5000 subsampled frames."""
         if lengths is not None:
-            raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN and ResNet x-vector "
-                                      "blueprints only"
-                                      .format(type(self).__name__))
+            if not getattr(self, "masked_chunks", False):
+                raise NotImplementedError("{}: extract_embedding_batch(lengths=...) is for the TDNN x-vector, ResNet "
+                                          "x-vector, CAM++ and Conformer blueprints only".format(type(self).__name__))
+            return self._extract_masked(feats, lengths)
         with torch.no_grad():
             x = torch.as_tensor(feats)
             if x.dtype != torch.float32:
@@ -359,6 +378,32 @@ class TransformerXvector(TopVirtualNnet):
             for i in range(1, ns):
                 acc = acc + split * full[:, i]
             return (acc + lengths[-1] * last) / T
+
+    def _extract_masked(self, feats, lengths):
+        with torch.no_grad():
+            x = torch.as_tensor(feats)
+            if x.dtype != torch.float32:
+                raise TypeError("extract_embedding_batch expects float32 features")
+            B, T, Fd = x.shape
+            if Fd != self.inputs_dim:
+                raise ValueError("expected feature dim {}, got {}".format(self.inputs_dim, Fd))
+            lens = _checked_lengths(lengths, B, T, self.transformer.subsampling)
+            x = x.to(self.device_for_extraction(), non_blocking=True).contiguous()
+            return self.extractor().extract(x, lens)
+
+
+def _checked_lengths(lengths, b, t, subsampling):
+    """Host int32 (B,) lengths of a masked Conformer batch padded to t frames; ValueError naming the first entry outside
+    [MIN_FRAMES, t], or when t subsamples to TABLE_ROWS frames or more."""
+    lens = host_lengths(lengths, b)
+    bad = np.flatnonzero((lens < MIN_FRAMES) | (lens > t))
+    if bad.size:
+        raise ValueError("lengths[{}]={} outside [{}, T={}]: the Conformer needs at least {} frames".format(
+            bad[0], lens[bad[0]], MIN_FRAMES, t, MIN_FRAMES))
+    t2 = subsampled_shape(subsampling, t, MIN_FRAMES)[0]
+    if t2 >= TABLE_ROWS:
+        raise ValueError("a chunk of {} subsampled frames exceeds the positional tables' {}".format(t2, TABLE_ROWS))
+    return lens
 
 
 def chunk_plan(num_frames, max_chunk=MAX_CHUNK):
@@ -414,8 +459,10 @@ def _lin(rec, device):
 
 class ConformerExtractor:
     """Folded weights on one device + the launch sequence of TransformerXvector.extract_embedding for one chunk per
-    utterance (all utterances of a call have the same length), driven from Python.  The weights and tables are the
-    records and configuration the native handle takes (native_records, native_config)."""
+    utterance (all utterances of a call have the same length, or a masked batch gives each its own), driven from Python.
+    The weights and tables are the records and configuration the native handle takes (native_records, native_config)."""
+
+    TAKES_LENGTHS = True
 
     def __init__(self, m, device):
         recs = {r[0]: r for r in native_records(m)}
@@ -456,6 +503,8 @@ class ConformerExtractor:
                  "dw_b": ops.to_device(recs[cm + "depthwise_conv"][2], device),
                  "cm_norm": norm(cm + "norm") + (bool(recs[cm + "norm"][5] & BN),),
                  "att_norm": recs[q + "self_attn.att_norm"][1][0] if self.softmax_plus else None}
+            # the multiplier table on the device, indexed by each utterance's T' in a masked batch
+            L["mult_table"] = ops.to_device(L["att_norm"], device) if self.softmax_plus else None
             for name in ("norm_ff", "norm_mha", "norm_ff_macaron", "norm_conv", "norm_final"):
                 L[name] = norm(q + name)
             self.layers.append(L)
@@ -482,13 +531,22 @@ class ConformerExtractor:
             self._tables[t] = (rope, absp, mults)
         return self._tables[t]
 
-    def extract(self, feats):
+    def extract(self, feats, lengths=None):
         """feats (B, T, F) fp32 CUDA (one chunk per utterance) -> (B, embd_dim) fp32 CUDA, asynchronous on the current
-        stream."""
+        stream.  lengths (B,) host ints, 7 <= lengths[b] <= T: a masked batch as xvb_conformer_extract_lengths runs it,
+        row b being feats[b, :lengths[b]] extracted alone (every length equal to T: the unmasked sequence).  The head
+        conv, every frame-level linear, the attention and the attentive pooling then take each utterance's length."""
         if feats.shape[2] != self.feat_dim:
             raise ValueError("expected feature dim {}, got {}".format(self.feat_dim, feats.shape[2]))
         feats = feats.contiguous()
         B, T, Fd = feats.shape
+        l1 = l2 = None    # a masked batch's lengths L at the input and L' after the subsampling
+        if lengths is not None:
+            lens = _checked_lengths(lengths, B, T, self.subsampling)
+            if (lens != T).any():
+                sub = np.array([subsampled_shape(self.subsampling, int(v), Fd)[0] for v in lens], np.int32)
+                table = torch.from_numpy(np.stack([lens, sub])).to(feats.device)
+                l1, l2 = table[0], table[1]
         if T < MIN_FRAMES:
             raise ValueError("the Conformer needs at least {} frames, got {}".format(MIN_FRAMES, T))
         dev, P, D = feats.device, ops.SplitPlanes, self.D
@@ -499,15 +557,15 @@ class ConformerExtractor:
         n = 0
         x1 = P.empty((B, T1, F1, D), dev)
         if self.subsampling == 4:
-            ops.subsample_head(feats, self.head_w, self.head_b, x1)
+            ops.subsample_head(feats, self.head_w, self.head_b, x1, lengths=l1)
         else:       # SVConv2dSubsampling2: time stride 2, frequency stride 1, then a stride-1 valid conv
-            ops.subsample_head(feats, self.head_w, self.head_b, x1, stride_f=1)
+            ops.subsample_head(feats, self.head_w, self.head_b, x1, stride_f=1, lengths=l1)
         x2 = P.empty((B, T2, F2, D), dev)
         ops.conv2d(x1, self.conv2_w, D, 3, 2 if self.subsampling == 4 else 1, self.conv2_scale, self.conv2_shift, relu=True,
                    y=x2, valid=True)
         del x1
         r = torch.empty(B, T2, D, dtype=torch.float32, device=dev)
-        self.embed_out.run(P(x2.hi.view(B, T2, F2 * D), x2.lo.view(B, T2, F2 * D), F2 * D), y_f32=r)
+        self.embed_out.run(P(x2.hi.view(B, T2, F2 * D), x2.lo.view(B, T2, F2 * D), F2 * D), y_f32=r, lengths=l2)
         n += 3
         units = self.layers[0]["ff"][0].cout if self.layers else 0
         h = P.empty((B, T2, D), dev)
@@ -519,8 +577,8 @@ class ConformerExtractor:
         hid_d = hid if D == hid.channels else hid.slice(0, D)
 
         def ffn(pair, out):
-            pair[0].run(h, y=hid_u)
-            pair[1].run(hid_u, y_f32=out)
+            pair[0].run(h, y=hid_u, lengths=l2)
+            pair[1].run(hid_u, y_f32=out, lengths=l2)
 
         first = self.layers[0] if self.layers else None
         if first is not None:   # r [+ pe] -> r, norm_ff_macaron
@@ -529,14 +587,18 @@ class ConformerExtractor:
         for i, L in enumerate(self.layers):
             ffn(L["ff_mac"], d1)
             ops.layer_norm(r, *L["norm_mha"], delta=d1, delta_scale=0.5, x_out=r, y=h)
-            L["qkv"].run(h, y_f32=qkv)
-            ops.rope_attention(qkv, self.H, self.dk, hid_d, rope=rope, rope_v=self.rotary_value, score_mult=mults[i])
-            L["out"].run(hid_d, y_f32=d1)
+            L["qkv"].run(h, y_f32=qkv, lengths=l2)
+            if l2 is None:
+                ops.rope_attention(qkv, self.H, self.dk, hid_d, rope=rope, rope_v=self.rotary_value, score_mult=mults[i])
+            else:
+                ops.rope_attention(qkv, self.H, self.dk, hid_d, rope=rope, rope_v=self.rotary_value, lengths=l2,
+                                   mult_table=L["mult_table"])
+            L["out"].run(hid_d, y_f32=d1, lengths=l2)
             ops.layer_norm(r, *L["norm_conv"], delta=d1, x_out=r, y=h)
-            L["pw1"].run(h, y_f32=delta)
+            L["pw1"].run(h, y_f32=delta, lengths=l2)
             g, b, bn = L["cm_norm"]
             ops.conv_module(delta, L["dw_w"], L["dw_b"], g, b, hid_d, batch_norm=bn, act=self.act)
-            L["pw2"].run(hid_d, y_f32=d1)
+            L["pw2"].run(hid_d, y_f32=d1, lengths=l2)
             ops.layer_norm(r, *L["norm_ff"], delta=d1, x_out=r, y=h)
             ffn(L["ff"], d1)
             nxt = self.layers[i + 1]["norm_ff_macaron"] if i + 1 < len(self.layers) else self.after_norm
@@ -549,20 +611,20 @@ class ConformerExtractor:
         xo = torch.empty(B, T2, od, dtype=torch.float32, device=dev)
         xp = P.empty((B, T2, od), dev)
         if ln is None:
-            lin.run(h, y=xp, y_f32=xo)
+            lin.run(h, y=xp, y_f32=xo, lengths=l2)
             n += 1
         else:
-            lin.run(h, y_f32=xo)
+            lin.run(h, y_f32=xo, lengths=l2)
             ops.layer_norm(xo, *ln, x_out=None, y=xp, y_f32=xo)
             n += 2
         # AttentiveStatsPool
         a1 = torch.empty(B, T2, self.att1.cout, dtype=torch.float32, device=dev)
-        self.att1.run(xp, y_f32=a1)
+        self.att1.run(xp, y_f32=a1, lengths=l2)
         ap = P.empty((B, T2, self.att1.cout), dev)
         ops.layer_norm(a1, *self.att_ln, act=ACT_TANH, y=ap)
         logits = torch.empty(B, T2, od, dtype=torch.float32, device=dev)
-        self.att2.run(ap, y_f32=logits)
-        stats = ops.attn_stats_pool(logits, xo, floor=1e-5)
+        self.att2.run(ap, y_f32=logits, lengths=l2)
+        stats = ops.attn_stats_pool(logits, xo, floor=1e-5, lengths=l2)
         z = P.empty((B, 1, 2 * od), dev)
         zf = torch.empty(B, 1, 2 * od, dtype=torch.float32, device=dev)
         ops.layer_norm(stats, *self.norm_stats, y=z, y_f32=zf)
@@ -715,6 +777,7 @@ class NativeConformerExtractor(NativeExtractor):
     library, on the device that is current when it is built (or loaded from an XVBC0001 file)."""
 
     PREFIX = "conformer"
+    TAKES_LENGTHS = True
 
     def _create_args(self, m):
         from asv_subtools_b200._lib import ConformerConfig

@@ -435,15 +435,21 @@ def se_residual(z, gate, identity, relu=False, y=None, y_f32=None, scale2=None, 
                               y2h, y2l, _stream()), "xvb_se_residual")
 
 
-def subsample_head(feats, weight, bias, y, stride_f=None):
+def subsample_head(feats, weight, bias, y, stride_f=None, lengths=None):
     """Conv2dSubsampling4's first conv + ReLU (xvb_subsample_head): feats (B, T, F) fp32, weight (C, 1, 3, 3) fp32 as
     stored, bias (C,) -> y SplitPlanes (B, (T - 1) // 2, (F - 1) // 2, C).  stride_f = 1 or 2: the feature stride of
-    xvb_subsample_head_stride (1: SVConv2dSubsampling2's stride (2, 1), y (B, (T - 1) // 2, F - 2, C))."""
+    xvb_subsample_head_stride (1: SVConv2dSubsampling2's stride (2, 1), y (B, (T - 1) // 2, F - 2, C)).  lengths: int32
+    CUDA (B,) tensor of a masked batch, 3 <= lengths[b] <= T (xvb_subsample_head_lengths, stride_f default 2): the rows
+    t1 >= (lengths[b] - 1) // 2 are zeros, and no frame past lengths[b] is read."""
     feats = _req(feats, torch.float32, "feats")
     b, t, f = feats.shape
     args = (_ptr(feats), b, t, f, _ptr(_req(weight, torch.float32, "weight")), _ptr(_req(bias, torch.float32, "bias")),
             weight.shape[0])
-    if stride_f is None:
+    if lengths is not None:
+        check(lib.xvb_subsample_head_lengths(args[0], b, t, f, _ptr(_req(lengths, torch.int32, "lengths")), *args[4:],
+                                             int(stride_f or 2), y.hi.data_ptr(), y.lo.data_ptr(), _stream()),
+              "xvb_subsample_head_lengths")
+    elif stride_f is None:
         check(lib.xvb_subsample_head(*args, y.hi.data_ptr(), y.lo.data_ptr(), _stream()), "xvb_subsample_head")
     else:
         check(lib.xvb_subsample_head_stride(*args, int(stride_f), y.hi.data_ptr(), y.lo.data_ptr(), _stream()),
@@ -498,16 +504,26 @@ def layer_norm(x, gamma=None, beta=None, eps=1e-5, delta=None, delta_scale=1.0, 
     check(lib.xvb_layer_norm(C.byref(a), _stream()), "xvb_layer_norm")
 
 
-def rope_attention(qkv, heads, dk, y, rope=None, rope_v=False, score_mult=1.0):
+def rope_attention(qkv, heads, dk, y, rope=None, rope_v=False, score_mult=1.0, lengths=None, mult_table=None):
     """Self-attention over the fused projection (xvb_rope_attention): qkv (B, T, >= 3 * heads * dk) fp32 rows, rope (T, dk)
-    fp32 [sin | cos] or None -> y SplitPlanes (B, T, heads * dk)."""
+    fp32 [sin | cos] or None -> y SplitPlanes (B, T, heads * dk).  lengths: int32 CUDA (B,) tensor of a masked batch
+    (xvb_rope_attention_lengths): utterance b attends over its first lengths[b] keys and its rows past them are zeros;
+    its score multiplier is then mult_table[lengths[b]] (fp32 CUDA (> T,), softmax_plus), or 1 without a table."""
     _, ldq = _rows(qkv, "qkv")
     b, t = qkv.shape[0], qkv.shape[1]
     if rope is not None and (_req(rope, torch.float32, "rope").dim() != 2 or rope.shape[0] < t or rope.shape[1] != dk):
         raise ValueError("rope must be (>= {}, {}), got {}".format(t, dk, tuple(rope.shape)))
-    check(lib.xvb_rope_attention(qkv.data_ptr(), ldq, b, t, heads, dk,
-                                 _ptr(_req(rope, torch.float32, "rope")) if rope is not None else None, 1 if rope_v else 0,
-                                 float(score_mult), y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_rope_attention")
+    rope_p = _ptr(_req(rope, torch.float32, "rope")) if rope is not None else None
+    if lengths is None:
+        if mult_table is not None:
+            raise ValueError("mult_table is the score multiplier of a masked batch: pass lengths too")
+        check(lib.xvb_rope_attention(qkv.data_ptr(), ldq, b, t, heads, dk, rope_p, 1 if rope_v else 0, float(score_mult),
+                                     y.hi.data_ptr(), y.lo.data_ptr(), y.ld, _stream()), "xvb_rope_attention")
+        return
+    rows = 0 if mult_table is None else _req(mult_table, torch.float32, "mult_table").numel()
+    check(lib.xvb_rope_attention_lengths(qkv.data_ptr(), ldq, b, t, heads, dk, rope_p, 1 if rope_v else 0,
+                                         _ptr(_req(lengths, torch.int32, "lengths")), _ptr(mult_table), rows, y.hi.data_ptr(),
+                                         y.lo.data_ptr(), y.ld, _stream()), "xvb_rope_attention_lengths")
 
 
 def conv_module(x, dw_weight, dw_bias, norm_a, norm_b, y, batch_norm=False, eps=1e-5, act=_lib.ACT_SWISH):
@@ -539,16 +555,21 @@ def stats_pool_ex(x, eps, mode, planes=False, lengths=None):
     return (out, op) if planes else out
 
 
-def attn_stats_pool(logits, x, floor=1e-5, planes=False):
-    """softmax over T of logits (B,T,C) -> weighted mean/std of x (B,T,C): (B,2C)."""
+def attn_stats_pool(logits, x, floor=1e-5, planes=False, lengths=None):
+    """softmax over T of logits (B,T,C) -> weighted mean/std of x (B,T,C): (B,2C).  lengths: int32 CUDA (B,) tensor of a
+    masked batch (xvb_attn_stats_pool_lengths): utterance b reduces its first lengths[b] frames."""
     logits = _req(logits, torch.float32, "logits")
     x = _req(x, torch.float32, "x")
     b, t, c = x.shape
     out = torch.empty(b, 2 * c, dtype=torch.float32, device=x.device)
     op = SplitPlanes.empty((b, 1, 2 * c), x.device) if planes else None
-    check(lib.xvb_attn_stats_pool(_ptr(logits), c, _ptr(x), c, b, t, c, floor, _ptr(out),
-                                  op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, 2 * c, _stream()),
-          "xvb_attn_stats_pool")
+    tail = (_ptr(out), op.hi.data_ptr() if op else None, op.lo.data_ptr() if op else None, 2 * c, _stream())
+    if lengths is None:
+        check(lib.xvb_attn_stats_pool(_ptr(logits), c, _ptr(x), c, b, t, c, floor, *tail), "xvb_attn_stats_pool")
+    else:
+        check(lib.xvb_attn_stats_pool_lengths(_ptr(logits), c, _ptr(x), c, b, t, c, floor,
+                                              _ptr(_req(lengths, torch.int32, "lengths")), *tail),
+              "xvb_attn_stats_pool_lengths")
     return (out, op) if planes else out
 
 

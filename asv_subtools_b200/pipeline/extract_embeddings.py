@@ -15,9 +15,9 @@ input key (bucket order).  `--shard i/n` keeps every n-th utterance (one process
 pre-splitting the scp).
 
 `--mixed-lengths` (models whose extractor takes lengths: the TDNN x-vector family with statistics pooling or an attention
-pooling other than LDE -- attentive, multi-head, multi-resolution, xi-vector --, the F-TDNN x-vector, the ResNet x-vector
-and CAM++): the model's chunk rule cuts every utterance first (the maxChunk rule, or the model's own `chunk_sizes` where
-it has one: CAM++'s 4000-frame egrecho rule), and the chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
+pooling other than LDE -- attentive, multi-head, multi-resolution, xi-vector --, the F-TDNN x-vector, the ResNet x-vector,
+the Conformer x-vector and CAM++): the model's chunk rule cuts every utterance first (the maxChunk rule, or the model's own
+`chunk_sizes` where it has one: the Conformer's 300-frame rule, CAM++'s 4000-frame egrecho rule), and the chunks are batched across lengths instead of by exact frame count (`plan_mixed_batches`); a batch runs as one masked
 call, `extract_embedding_batch(x, lengths)`, and each utterance's embedding is sum(len_i * emb_i) / frames over its
 chunks, as `bin/xvb-extract --mixed-lengths` does.  The pooling merge order depends on the batch shape, so the vectors
 differ from the default mode's at the rounding level.
@@ -115,7 +115,8 @@ def chunk_lengths(frames, max_chunk=MAX_CHUNK):
 
 def model_chunk_lengths(model, frames):
     """The chunks --mixed-lengths cuts a `frames`-long utterance into for `model`: its own rule when the blueprint has
-    one (`model.chunk_sizes(frames)`, e.g. CAM++'s 4000-frame egrecho rule), else the maxChunk rule (chunk_lengths)."""
+    one (`model.chunk_sizes(frames)`, e.g. the Conformer's 300-frame rule or CAM++'s 4000-frame egrecho rule), else the
+    maxChunk rule (chunk_lengths)."""
     own = getattr(model, "chunk_sizes", None)
     return list(own(frames)) if own is not None else chunk_lengths(frames)
 
@@ -211,7 +212,7 @@ def main(argv=None):
     ap.add_argument("--shard", type=str, default="0/1", help="i/n: keep utterances with index %% n == i")
     ap.add_argument("--mixed-lengths", action="store_true",
                     help="batch utterances of different lengths (padding at most 1/8 of a batch); TDNN x-vector models with "
-                         "statistics or attention pooling (not LDE), F-TDNN, ResNet x-vector and CAM++ models only")
+                         "statistics or attention pooling (not LDE), F-TDNN, ResNet x-vector, Conformer and CAM++ models only")
     ap.add_argument("--blueprint-dir", type=str, default="",
                     help="take the blueprint of the same file name from this directory (asv_subtools_b200/model) instead of "
                          "the path stored in nnet.config, so a reference model dir is used as it is")
@@ -243,8 +244,8 @@ def main(argv=None):
             ex = model.extractor()
             if not getattr(ex, "TAKES_LENGTHS", False):
                 print("ERROR: --mixed-lengths needs a TDNN x-vector model with statistics or attention pooling (not LDE), an "
-                      "F-TDNN, a ResNet x-vector or a CAM++ model; {} runs on {}".format(type(model).__name__,
-                                                                                        type(ex).__name__),
+                      "F-TDNN, a ResNet x-vector, a Conformer or a CAM++ model; {} runs on {}".format(type(model).__name__,
+                                                                                                     type(ex).__name__),
                       file=sys.stderr)
                 sys.exit(1)
         # native ark reader (csrc/ark_io.cpp): the reference's byte-at-a-time key loop is the wall at GPU rates

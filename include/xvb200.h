@@ -233,6 +233,13 @@ int xvb_se_apply(const uint16_t* z_hi, const uint16_t* z_lo, int64_t ldz, const 
  * over logits and x (both (B,T,C) fp32) with an online softmax. */
 int xvb_attn_stats_pool(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C, float floor_,
                         float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo, void* stream);
+/* xvb_attn_stats_pool over a masked batch: utterance b reduces its first lengths[b] frames (DEVICE int32[B],
+ * 1 <= lengths[b] <= T; the batch stride stays T rows of x and of the logits) with the frame walk of the unmasked call,
+ * so its row is bit for bit that call on the utterance alone.  The frames past each end are never read.  XVB_EINVAL on
+ * a NULL lengths. */
+int xvb_attn_stats_pool_lengths(const float* logits, int64_t ldl, const float* x, int64_t ldx, int B, int T, int C,
+                                float floor_, const int* lengths, float* out, uint16_t* out_hi, uint16_t* out_lo, int64_t ldo,
+                                void* stream);
 
 /* LDEPooling.forward (libs/nnet/pooling.py:130-162): x (B,T,C) fp32, dictionary mu (C,K) fp32 as the state_dict stores
  * it, neg_beta[k] = -(s_k^2 + eps); w[t,k] = softmax_k(neg_beta[k] * sum_c (x[t,c] - mu[c,k])^2) (distances summed directly
@@ -376,6 +383,12 @@ int xvb_subsample_head(const float* x, int B, int T, int F, const float* w, cons
  * Conv2d(1, C, 3, stride (2, 1)) (subsampling.py:365-415), F1 = F - 2; stride_f = 2 is xvb_subsample_head, bit for bit. */
 int xvb_subsample_head_stride(const float* x, int B, int T, int F, const float* w, const float* bias, int C, int stride_f,
                               uint16_t* y_hi, uint16_t* y_lo, void* stream);
+/* xvb_subsample_head_stride over a masked batch: utterance b owns frames [0, lengths[b]) (DEVICE int32[B],
+ * 3 <= lengths[b] <= T).  Its output rows t1 < (lengths[b] - 1) / 2 are those of the unmasked call on the utterance
+ * alone, bit for bit; the rows past them are written as exact zeros and load nothing, so no frame t >= lengths[b] is
+ * read.  y keeps the (B, T1, F1, C) layout of the padded T.  XVB_EINVAL on a NULL lengths. */
+int xvb_subsample_head_lengths(const float* x, int B, int T, int F, const int* lengths, const float* w, const float* bias,
+                               int C, int stride_f, uint16_t* y_hi, uint16_t* y_lo, void* stream);
 
 /* Residual update + LayerNorm over `rows` rows of C channels (C <= 8192), one pass:
  *   v     = x [+ table[row % table_rows]] [+ delta_scale * delta]     the residual adds of ConformerEncoderLayer
@@ -412,6 +425,15 @@ int xvb_layer_norm(const xvb_layer_norm_args_t* args, void* stream);
  * dk in {32, 64, 128}; any T >= 1 (keys are tiled with an online softmax). */
 int xvb_rope_attention(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
                        float score_mult, uint16_t* y_hi, uint16_t* y_lo, int64_t ldy, void* stream);
+/* xvb_rope_attention over a masked batch: utterance b owns frames [0, lengths[b]) (DEVICE int32[B], 1 <= lengths[b] <= T;
+ * the batch stride stays T rows of qkv and y).  It attends over its keys [0, lengths[b]) only, with the key tiles and
+ * online softmax of a call at T = lengths[b], so its rows are bit for bit that call on the utterance alone; its query
+ * rows past lengths[b] are written as exact zeros, and no frame past its end is read.  The score multiplier is
+ * mult_table[lengths[b]] (DEVICE fp32[mult_rows], softmax_plus's multiplier per length), or 1 (softmax) when mult_table
+ * is NULL.  XVB_EINVAL on a NULL lengths, or a mult_table with mult_rows <= T. */
+int xvb_rope_attention_lengths(const float* qkv, int64_t ldq, int B, int T, int H, int dk, const float* rope, int rope_v,
+                               const int* lengths, const float* mult_table, int mult_rows, uint16_t* y_hi, uint16_t* y_lo,
+                               int64_t ldy, void* stream);
 
 /* ConvolutionModule.forward between its pointwise convs (convolution.py:110-125): x (B, T, >= 2C) fp32 = pointwise_conv1's
  * output; GLU a * sigmoid(b) over the two halves; depthwise Conv1d(C, C, K, padding K/2, groups C) with dw_w (C, K) and
@@ -956,7 +978,8 @@ int xvb_conv2d_kept_taps(const float* w, int Cout, int Cin, int k, int* taps, in
  * Whole-model extractor for the Conformer x-vector (pytorch/model/transformer_xvector.py, extract_embedding :321-346,
  * Conformer encoder with 4x (input_layer "conv2d") or 2x ("conv2d2") subsampling): the launch sequence of
  * xvb_subsample_head[_stride], xvb_conv2d_valid, xvb_tdnn_affine_ex, xvb_layer_norm, xvb_rope_attention,
- * xvb_conv_module, xvb_attn_stats_pool and xvb_split_f32 in C++, one chunk per utterance (the 300-frame chunk rule
+ * xvb_conv_module, xvb_attn_stats_pool and xvb_split_f32 in C++ (the _lengths forms for a masked batch), one chunk per
+ * utterance (the 300-frame chunk rule
  * stays with the caller).  Bit-identical to the op-by-op Python driver of the same kernels (ConformerExtractor,
  * XVB_CONFORMER_NATIVE=0).
  *
@@ -1015,6 +1038,18 @@ int xvb_conformer_last_launches(const xvb_conformer_t* h);
 /* feats (B, T, feat_dim) fp32 on the device, one chunk per utterance -> emb (B, embed_dim) fp32 on the device;
  * asynchronous on `stream`. */
 int xvb_conformer_extract(xvb_conformer_t* h, const float* feats, int B, int T, float* emb, void* stream);
+/* A batch of utterances of different lengths, one chunk each: feats (B, T, feat_dim) fp32 on the device, utterance b in
+ * its first lengths_host[b] frames (HOST int32[B], 7 <= lengths_host[b] <= T, T' < 5000; the frames past them are never
+ * read, whatever they hold).  Row b of emb is the embedding of feats[b, :lengths_host[b]] extracted alone, bit for bit,
+ * except for a chunk of T' = 1: alone, its linears of Cin >= 1536 run at T == 1 on the layer kernel's split-K path, so
+ * it agrees bit for bit only with split-K off (XVB_SPLITK=0) for both calls.  The
+ * lengths are checked (XVB_EINVAL naming the first bad one, nothing launched); when all equal T this is
+ * xvb_conformer_extract.  Otherwise a (2, B) table of L and L' (the subsampled length) is copied into the workspace on
+ * `stream` (the host array may be reused when the call returns); the head conv, every frame-level linear, the
+ * attention (with the block's softmax_plus multiplier for L') and the attentive pooling then run masked.  Frame-budget
+ * groups and launch count as in xvb_conformer_extract. */
+int xvb_conformer_extract_lengths(xvb_conformer_t* h, const float* feats, const int32_t* lengths_host, int B, int T,
+                                  float* emb, void* stream);
 /* "XVBC0001" model files: the configuration, then the records and tables as handed to xvb_conformer_set_layer
  * (layout at save_records in csrc/model_file.cpp). */
 int xvb_conformer_save(const xvb_conformer_t* h, const char* path);

@@ -20,8 +20,8 @@
 #   XVB200_BATCH   utterances per batch (default 256)                      XVB200_REF     the reference script to wrap
 #   XVB200_DRYRUN  non-empty: print the rewritten command lines and exit
 #   XVB200_MIXED_LENGTHS  1: add --mixed-lengths (batches of utterances of different lengths, at most 1/8 padding;
-#                  TDNN x-vector models with statistics or attention pooling other than LDE, F-TDNN and ResNet
-#                  x-vector models only)
+#                  TDNN x-vector models with statistics or attention pooling other than LDE, F-TDNN, ResNet
+#                  x-vector, Conformer and CAM++ models only)
 
 set -e
 XVB200_ROOT=${XVB200_ROOT:-$(cd "$(dirname "${BASH_SOURCE[0]}")/.." && pwd)}

@@ -2,8 +2,8 @@
 """Throughput of an x-vector extractor on a corpus of utterances of different lengths -- a side measurement, not the
 bench.py line.
 
-    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn|campplus] [--utts N]
-                                        [--min-frames A] [--max-frames B] [--batch N] [--dim F]
+    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn|campplus|conformer]
+                                        [--utts N] [--min-frames A] [--max-frames B] [--batch N] [--dim F]
 
 The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
 numpy.random.RandomState(2026), run through one handle under two batch policies.  --model xvector (the default): an
@@ -15,7 +15,11 @@ four-head attention pooling (tests/golden/make_golden_snowdar.py "mha_share"), t
 pooling ("xi_dist") and the factored F-TDNN (make_golden_ftdnn.py); batch 256, 256 and 128 by default.  --model
 campplus: the native CAM++ handle with egrecho's default CamPPConfig (embd_dim 512, init_channels 128, growth_rate 32,
 bn_size 4) on 80-d features (--dim is ignored), batch 128 by default, as tools/bench_campplus.py times it; every
-utterance of the default corpus is one chunk of its own length under CAM++'s 4000-frame chunk rule.
+utterance of the default corpus is one chunk of its own length under CAM++'s 4000-frame chunk rule.  --model conformer:
+the native Conformer handle with the launcher's model as tools/bench_conformer.py builds it (6 blocks, attention_dim 256,
+rot_pos, softmax_plus, 4x subsampling) on 80-d features (--dim is ignored), batch 128 by default; every utterance is cut
+by the 300-frame chunk rule (chunk_plan) first, and both policies batch the chunks.  Frames/s still counts the corpus
+frames.
 
   * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
     up to `batch` utterances of exactly the same frame count, one xvb_<handle>_extract call each;
@@ -67,9 +71,10 @@ def main():
     ap.add_argument("--min-frames", type=int, default=200)
     ap.add_argument("--max-frames", type=int, default=2000)
     ap.add_argument("--batch", type=int, default=None,
-                    help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn, campplus)")
+                    help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn, campplus, conformer)")
     ap.add_argument("--dim", type=int, default=23)
-    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn", "campplus"], default="xvector")
+    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn", "campplus", "conformer"],
+                    default="xvector")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_mixed_lengths.py needs a GPU")
@@ -110,6 +115,15 @@ def main():
         m = CamPPXvector(F, 10)
         m.load_state_dict(co.seeded_state_dict(keys, 401), strict=True)
         workload = "CAM++ CamPPConfig defaults (80-d, embd_dim 512)"
+    elif args.model == "conformer":
+        import conformer_oracle as cfo
+        from asv_subtools_b200.model.transformer_xvector import TransformerXvector
+        F = 80
+        args.batch = args.batch or 128
+        keys = np.load(os.path.join(ROOT, "tests", "golden", "conformer.npz"))["keys_launcher"]
+        m = TransformerXvector(F, 10, training=False, extracted_embedding="near", **cfo.LAUNCHER)
+        m.load_state_dict(cfo.seeded_state_dict(keys, 401), strict=True)
+        workload = "launcher Conformer (6 blocks, d 256, rot_pos, softmax_plus, 80-d, near), 300-frame chunks"
     else:
         F = args.dim
         args.batch = args.batch or 256
@@ -118,18 +132,20 @@ def main():
         workload = "Xvector({}) far".format(F)
     m.cuda().eval()
     ex = m.extractor()
-    base = torch.randn(args.batch * args.max_frames * F, device="cuda")
+    # the items both policies batch: the chunks of the model's own chunk rule where it cuts utterances, else the utterances
+    chunks = [n for u in lengths for n in m.chunk_sizes(u)] if args.model == "conformer" else lengths
+    base = torch.randn(args.batch * max(chunks) * F, device="cuda")
 
     policies = {}
-    for name, plan in (("equal_length", equal_length_batches(lengths, args.batch)),
-                       ("masked", plan_mixed_batches(lengths, args.batch))):
+    for name, plan in (("equal_length", equal_length_batches(chunks, args.batch)),
+                       ("masked", plan_mixed_batches(chunks, args.batch))):
         jobs = []
         for idx in plan:
-            lens = [lengths[i] for i in idx]
+            lens = [chunks[i] for i in idx]
             B, T = len(lens), max(lens)
             jobs.append((B, T, np.asarray(lens, np.int32) if name == "masked" else None))
         computed = sum(B * T for B, T, _ in jobs)
-        policies[name] = {"jobs": jobs, "batches": len(jobs), "padded_share": 1.0 - sum(lengths) / computed, "fps": []}
+        policies[name] = {"jobs": jobs, "batches": len(jobs), "padded_share": 1.0 - sum(chunks) / computed, "fps": []}
 
     def run(jobs):
         for B, T, lens in jobs:
@@ -150,7 +166,7 @@ def main():
                 p["fps"].append(sum(lengths) / (start.elapsed_time(stop) / 1e3))
     out = {"workload": "{}, {} utterances uniform over {}..{} frames (RandomState(2026)), batch {}".format(
                workload, args.utts, args.min_frames, args.max_frames, args.batch),
-           "frames": sum(lengths), "card": smi, "rounds": args.rounds}
+           "frames": sum(lengths), "items": len(chunks), "card": smi, "rounds": args.rounds}
     for name, p in policies.items():
         out[name] = {"frames_per_s": statistics.median(p["fps"]), "frames_per_s_min": min(p["fps"]),
                      "frames_per_s_max": max(p["fps"]), "batches": p["batches"], "padded_share": round(p["padded_share"], 5)}

@@ -1,5 +1,7 @@
 #!/usr/bin/env python
-"""Seeded outputs of the 2-D conv entry points (xvb_conv2d, xvb_conv2d_taps), xvb_se_apply and the layer kernel
+"""Seeded outputs of the 2-D conv entry points (xvb_conv2d, xvb_conv2d_taps), xvb_se_apply, the Conformer's head conv
+(xvb_subsample_head[_stride]) and attention (xvb_rope_attention, softmax and softmax_plus), xvb_attn_stats_pool and the
+layer kernel
 (xvb_tdnn_affine_ex, every existing epilogue flag, the split-K segment path and the fused pooling; the five frame layers of bench.py at
 256 x 200, with the im2col first layer and tdnn5's fused pooling; an ECAPA-sized and a Conformer-sized layer) written to
 one .npz, so that two builds of the library can be compared bit for bit:
@@ -120,6 +122,29 @@ def main():
         for name, p in (("out", out_p), ("next", nxt_p)) if nxt else (("out", out_p),):
             res["se_apply{}_{}_hi".format(i, name)] = p.hi.view(torch.int16).cpu().numpy()
             res["se_apply{}_{}_lo".format(i, name)] = p.lo.view(torch.int16).cpu().numpy()
+    # the Conformer head conv at both feature strides
+    for sf in (2, 1):
+        feats = rnd(3, 301, 80)
+        F1 = (80 - 1) // 2 if sf == 2 else 80 - 2
+        y = ops.SplitPlanes.empty((3, 150, F1, 256), "cuda")
+        ops.subsample_head(feats, rnd(256, 1, 3, 3, scale=1.0 / 3), 0.1 * rnd(256), y, stride_f=None if sf == 2 else 1)
+        res["subsample_head_sf{}_hi".format(sf)] = y.hi.view(torch.int16).cpu().numpy()
+        res["subsample_head_sf{}_lo".format(sf)] = y.lo.view(torch.int16).cpu().numpy()
+    # the attention: each d_k, no rope / rope / rope on the values too, softmax and a softmax_plus multiplier
+    for dk, H, T, rope_mode, mult in ((32, 8, 98, 0, 1.0), (64, 4, 74, 1, 1.0), (128, 2, 240, 2, 1.0), (64, 4, 74, 2, 0.7391),
+                                      (32, 4, 33, 1, 1.3137)):
+        qkv = rnd(3, T, 3 * H * dk)
+        rope = torch.cat([torch.sin(rnd(T, dk // 2)), torch.cos(rnd(T, dk // 2))], 1).contiguous() if rope_mode else None
+        y = ops.SplitPlanes.empty((3, T, H * dk), "cuda")
+        ops.rope_attention(qkv, H, dk, y, rope=rope, rope_v=rope_mode == 2, score_mult=mult)
+        key = "rope_attention_dk{}_T{}_r{}_m{}".format(dk, T, rope_mode, mult)
+        res[key + "_hi"] = y.hi.view(torch.int16).cpu().numpy()
+        res[key + "_lo"] = y.lo.view(torch.int16).cpu().numpy()
+    # xvb_attn_stats_pool: the Conformer's 1536 channels and ECAPA's 3072, with plane outputs, and a channel tail
+    for B, T, C in ((4, 74, 1536), (3, 200, 3072), (2, 33, 200)):
+        st, op = ops.attn_stats_pool(rnd(B, T, C), rnd(B, T, C), floor=1e-5, planes=True)
+        res["attn_stats_pool_{}x{}x{}".format(B, T, C)] = st.cpu().numpy()
+        res["attn_stats_pool_{}x{}x{}_hi".format(B, T, C)] = op.hi.view(torch.int16).cpu().numpy()
     np.savez(out, **res)
     print(out, len(res), "arrays")
 
