@@ -8,6 +8,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("XVB_LIB") or os.path.join(_HERE, "libxvb200.so")
 
 RELU, BN, SIGMOID, TANH, SWISH = 1, 2, 4, 8, 16
+POOL_ATTENTION, POOL_XI_POSTMEAN, POOL_XI_POSTDIST = 1, 2, 3   # xvb_extractor_set_attention_pooling kinds
 ACT_NONE, ACT_RELU, ACT_SWISH, ACT_TANH = 0, 1, 2, 3
 
 
@@ -183,6 +184,8 @@ SIGNATURES = {
     "xvb_extractor_create": (_i, [C.POINTER(_p), _i]),
     "xvb_extractor_add_frame_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_extractor_add_segment_layer": (_i, [_p, _i, _p, _p, _p, _p, _i]),
+    "xvb_extractor_set_attention_pooling": (_i, [_p, _i, _i, _i, _i, _p, _p]),
+    "xvb_extractor_add_attention_layer": (_i, [_p, _i, _ip, _i, _p, _p, _p, _p, _i]),
     "xvb_extractor_finalize": (_i, [_p, _f]),
     "xvb_extractor_embed_dim": (_i, [_p]),
     "xvb_extractor_extract": (_i, [_p, _p, _i, _i, _p, _p]),

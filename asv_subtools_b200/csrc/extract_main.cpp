@@ -15,13 +15,15 @@
 // C++ runtime (runtime/bin/extractor_main.cc + runtime/extractor/torch_asv_extractor.cc:71-122: load
 // a model, optional per-utterance CMN, extract, emit the vector), with features instead of wav on
 // the input side.  The model file is any of the six families, told apart by its magic: TDNN x-vector
-// (XVBM0001), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling, or XVBE0003 for the
+// (XVBM0001, or XVBM0002 for the snowdar x-vector's attentive, multi-head and multi-resolution poolings and the
+// xi-vector), ECAPA-TDNN (XVBE0001, or XVBE0002 with multi-query multi-head attention pooling, or XVBE0003 for the
 // launcher model of pytorch/model/ecapa-tdnn-xvector.py, whose attentive pooling has no global context, or XVBG0001 for
 // egrecho's EcapaXvector with chained blocks),
 // 2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001, 4x or 2x
 // subsampling) or CAM++ x-vector (XVBP0001), each written by its native extractor's save() (model_file.cpp).  What it adds:
-// utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector, ResNet
-// x-vector, Conformer and CAM++ files) chunks of different lengths share masked batches (plan_mixed_batches,
+// utterances of equal length are batched (the reference runs batch 1); with --mixed-lengths (TDNN x-vector with
+// statistics or attention pooling, ResNet x-vector, Conformer and CAM++ files) chunks of different lengths share
+// masked batches (plan_mixed_batches,
 // xvb_extractor_extract_lengths / xvb_resnet_extract_lengths / xvb_conformer_extract_lengths / xvb_campp_extract_lengths),
 // which fills batches on a real corpus where most frame counts occur a few times only.
 //   * chunk rule of framework.py:34-47: T > max-chunk -> num_split = ceil(T/max), split = T/num_split,
@@ -110,8 +112,9 @@ const Family kFamilies[] = {
      }},
     {{"XVBE0003", nullptr}, "loading the ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 10000, false, nullptr},
     {{"XVBG0001", nullptr}, "loading the egrecho ECAPA model", "xvb_ecapa_extract", HANDLE_FAMILY(ecapa), 4000, true, nullptr},
-    // TDNN x-vector (XVBM0001): any other magic, which its loader then checks; its feature dim comes from the file
-    {{nullptr, nullptr}, "loading the model", "xvb_extractor_extract",
+    // TDNN x-vector (XVBM0001, or XVBM0002 with an attention pooling): also any other magic, which its loader then
+    // refuses; its feature dim comes from the file
+    {{"XVBM0001", "XVBM0002"}, "loading the model", "xvb_extractor_extract",
      [](void** h, const char* path) { return xvb_extractor_load((xvb_extractor_t**)h, path); },
      [](const void*, const char* path) { return xvb_extractor_feat_dim(path); },
      [](const void* h) { return xvb_extractor_embed_dim((const xvb_extractor_t*)h); },
@@ -318,17 +321,17 @@ int main(int argc, char** argv) {
              "                   [--mixed-lengths] [--wav fbank|mfcc [--num-mel-bins N] [--num-ceps N] [--low-freq F] [--high-freq F]\n"
              "                    [--frame-length MS] [--frame-shift MS] [--energy-floor E] [--use-energy]]\n"
              "                   <model.xvbm> <feats-rspecifier | wav.scp> <vectors-wspecifier>\n"
-             "The model file is a TDNN x-vector (XVBM0001), ECAPA-TDNN (XVBE0001 / XVBE0002 / XVBE0003), egrecho ECAPA-TDNN (XVBG0001),\n"
+             "The model file is a TDNN x-vector (XVBM0001, or XVBM0002 with an attention or xi-vector pooling), ECAPA-TDNN (XVBE0001 / XVBE0002 / XVBE0003), egrecho ECAPA-TDNN (XVBG0001),\n"
              "2-D ResNet x-vector (XVBR0001), RepVGG / RepSPK x-vector (XVBV0001), Conformer x-vector (XVBC0001) or CAM++\n"
              "x-vector (XVBP0001) model, recognised by its magic.  --max-chunk defaults to 300 frames for a Conformer (the\n"
              "model's own chunk rule), 4000 for CAM++ and egrecho ECAPA-TDNN and 10000 otherwise.  A Conformer chunk needs at\n"
              "least 7 frames and fewer than 5000 subsampled frames.  CAM++ and egrecho ECAPA-TDNN cut an utterance with\n"
              "egrecho's rule (max-chunk-long chunks, the last two re-split evenly: 9000 -> 4000, 2500, 2500); a CAM++ chunk\n"
              "needs at least 3 frames.\n"
-             "--mixed-lengths (TDNN x-vector, ResNet x-vector, Conformer and CAM++ models): after the chunk rule, chunks of\n"
-             "different lengths share batches of up to --batch, taken in ascending length, with at most 1/8 of a batch's\n"
-             "frames padding; the summary line also reports the padded frames.  Vectors differ from the default mode's at\n"
-             "the rounding level.\n");
+             "--mixed-lengths (TDNN x-vector of either file, ResNet x-vector, Conformer and CAM++ models): after the chunk\n"
+             "rule, chunks of different lengths share batches of up to --batch, taken in ascending length, with at most 1/8\n"
+             "of a batch's frames padding; the summary line also reports the padded frames.  Vectors differ from the\n"
+             "default mode's at the rounding level.\n");
       return 0;
     } else if (a.size() > 2 && a[0] == '-' && a[1] == '-') {
       fprintf(stderr, "ERROR: xvb-extract: unknown option %s\n", a.c_str());
@@ -355,7 +358,7 @@ int main(int argc, char** argv) {
     r.D = r.fam->embed_dim(r.model);
     if (!max_chunk_set) max_chunk = r.fam->max_chunk;
     if (mixed && !r.fam->extract_lengths) {
-      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector (XVBM0001), ResNet x-vector (XVBR0001), "
+      fprintf(stderr, "ERROR: xvb-extract: --mixed-lengths needs a TDNN x-vector (XVBM0001 / XVBM0002), ResNet x-vector (XVBR0001), "
                       "Conformer (XVBC0001) or CAM++ (XVBP0001) model; '%s' is read with %s\n", pos[0],
               r.fam->extract_fn);
       return 1;

@@ -9,6 +9,11 @@
 //
 //   "XVBM0001" (TDNN) | i32 feat_dim | f32 pooling_eps | i32 n_frame | i32 n_segment | n_frame + n_segment tap records
 //                       (segment layers with ntaps = tot_context = 1 and ctx = {0})
+//   "XVBM0002" (TDNN with an attention pooling, xvb_extractor_set_attention_pooling): the XVBM0001 header, then the
+//              pooling record i32 kind, pooled, gdiv, unweighted_var, n_attention (AttnPoolRecord) | for the xi-vector
+//              kinds f32 prior_logprec[pooled], prior_mean[pooled] | n_frame + n_attention + n_segment tap records
+//              (the attention affines, 1 or 2, between the frame and the segment layers).  Written only for such a
+//              model, so XVBM0001 files are written as before.
 //   "XVBE0001" (ECAPA-TDNN) | i32 feat_dim, channels, mfa_dim, att_hidden, embed_dim, n_layers
 //              | per layer: i32 name_len | name (no NUL) | tap record
 //   "XVBE0002" (ECAPA-TDNN with MQMHA pooling): the same with the pooling record {num_head, num_q, hidden, share,
@@ -258,20 +263,51 @@ extern "C" int xvb_extractor_load(xvb_extractor_t** out, const char* path) {
   char magic[8];
   int32_t feat_dim = 0, n_frame = 0, n_seg = 0;
   float eps = 0.f;
+  xvb::AttnPoolRecord pool = {0, 0, 0, 0, 0};
   do {
-    if (!rd(f, magic, 8) || memcmp(magic, "XVBM0001", 8) != 0) { set_error("xvb_extractor_load: '%s' is not an XVBM0001 file", path); break; }
+    const bool got_magic = rd(f, magic, 8);
+    const bool att = got_magic && memcmp(magic, "XVBM0002", 8) == 0;
+    if (!att && (!got_magic || memcmp(magic, "XVBM0001", 8) != 0)) {
+      set_error("xvb_extractor_load: '%s' is not an XVBM0001 file or an XVBM0002 file", path);
+      break;
+    }
     if (!rd(f, &feat_dim, 4) || !rd(f, &eps, 4) || !rd(f, &n_frame, 4) || !rd(f, &n_seg, 4) || feat_dim <= 0 ||
         n_frame <= 0 || n_seg <= 0 || n_frame > 64 || n_seg > 64) { set_error("xvb_extractor_load: bad header in '%s'", path); break; }
+    std::vector<float> prior[2];
+    if (att && (!rd(f, &pool, sizeof pool) ||
+                !(pool.kind == XVB_POOL_ATTENTION || pool.kind == XVB_POOL_XI_POSTMEAN || pool.kind == XVB_POOL_XI_POSTDIST) ||
+                pool.pooled <= 0 || pool.pooled > (1 << 20) || pool.n_attention < 1 || pool.n_attention > 2)) {
+      set_error("xvb_extractor_load: '%s' is not an XVBM0001 file or an XVBM0002 file: bad pooling record", path);
+      break;
+    }
+    const bool xi = pool.kind == XVB_POOL_XI_POSTMEAN || pool.kind == XVB_POOL_XI_POSTDIST;
+    if (xi) {
+      prior[0].resize(pool.pooled);
+      prior[1].resize(pool.pooled);
+      if (!rd(f, prior[0].data(), 4 * (size_t)pool.pooled) || !rd(f, prior[1].data(), 4 * (size_t)pool.pooled)) {
+        set_error("xvb_extractor_load: '%s' is truncated in the xi-vector prior", path);
+        break;
+      }
+    }
     if ((rc = xvb_extractor_create(&h, feat_dim)) != XVB_OK) break;
+    if (att && (rc = xvb_extractor_set_attention_pooling(h, pool.kind, pool.pooled, pool.gdiv, pool.unweighted,
+                                                         xi ? prior[0].data() : nullptr, xi ? prior[1].data() : nullptr)))
+      break;
     xvb::TapRec r;
+    const int n_att = pool.n_attention;
     int cin = feat_dim;   // the input width add_*_layer gives the layer
-    for (int i = 0; rc == XVB_OK && i < n_frame + n_seg; ++i) {
-      if (i == n_frame) cin *= 2;   // mean | std
+    int c_last = 0;       // the last frame layer's channels
+    for (int i = 0; rc == XVB_OK && i < n_frame + n_att + n_seg; ++i) {
+      if (i == n_frame) c_last = cin;
+      if (i == n_frame + n_att)   // mean | std, or the attention pooling's own width
+        cin = !att ? 2 * c_last : pool.kind == XVB_POOL_XI_POSTMEAN ? pool.pooled : 2 * pool.pooled;
       const TapRead got = read_tap(f, &r);
       if (got == kBadHeader || r.Cin != cin) { set_error("xvb_extractor_load: bad layer %d header in '%s'", i, path); rc = XVB_EINVAL; break; }
       if (got == kTruncated) { set_error("xvb_extractor_load: '%s' is truncated in layer %d", path, i); rc = XVB_EINVAL; break; }
       if (i < n_frame)
         rc = xvb_extractor_add_frame_layer(h, r.Cout, r.ctx, r.ntaps, r.w.data(), or_null(r.b), or_null(r.s), or_null(r.t), r.flags);
+      else if (i < n_frame + n_att)
+        rc = xvb_extractor_add_attention_layer(h, r.Cout, r.ctx, r.ntaps, r.w.data(), or_null(r.b), or_null(r.s), or_null(r.t), r.flags);
       else
         rc = xvb_extractor_add_segment_layer(h, r.Cout, r.w.data(), or_null(r.b), or_null(r.s), or_null(r.t), r.flags);
       cin = r.Cout;
@@ -289,9 +325,10 @@ extern "C" int xvb_extractor_feat_dim(const char* path) {
   if (!f) { set_error("xvb_extractor_feat_dim: cannot open '%s'", path ? path : "(null)"); return XVB_EINVAL; }
   char magic[8];
   int32_t d = 0;
-  const bool ok = rd(f, magic, 8) && memcmp(magic, "XVBM0001", 8) == 0 && rd(f, &d, 4) && d > 0;
+  const bool ok = rd(f, magic, 8) && (memcmp(magic, "XVBM0001", 8) == 0 || memcmp(magic, "XVBM0002", 8) == 0) &&
+                  rd(f, &d, 4) && d > 0;
   fclose(f);
-  if (!ok) { set_error("xvb_extractor_feat_dim: '%s' is not an XVBM0001 file", path); return XVB_EINVAL; }
+  if (!ok) { set_error("xvb_extractor_feat_dim: '%s' is not an XVBM0001 file or an XVBM0002 file", path); return XVB_EINVAL; }
   return d;
 }
 

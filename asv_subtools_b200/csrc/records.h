@@ -39,6 +39,10 @@ struct TapRec : TapShape {
 TapRec tap_record(const char* name, int Cout, int Cin, const int* ctx, int ntaps, const float* w, const float* b,
                   const float* s, const float* t, int flags);
 
+// The pooling record of an "XVBM0002" file (a TDNN x-vector with an attention pooling; layout in model_file.cpp): the
+// arguments of xvb_extractor_set_attention_pooling and the number of attention affines after the frame layers.
+struct AttnPoolRecord { int32_t kind, pooled, gdiv, unweighted, n_attention; };
+
 // The tap-layer files ("XVBM0001" TDNN, "XVBE0001" / "XVBE0002" ECAPA-TDNN; layouts in model_file.cpp): magic, the
 // family's header block, then the layers in order, each preceded by its name when `named` (fn: the caller's name).
 int save_tap_file(const char* fn, const char* path, const char* magic, const void* head, size_t head_bytes,

@@ -209,19 +209,19 @@ def build_tdnn_extractor(model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, e
     return ex
 
 
-def from_layer(layer, device):
+def from_layer(layer, device, keep_record=False):
     """A whole ReluBatchNormTdnnLayer as an ops.PackedAffine with its output rows padded to a multiple of 8 (its
     `export()` folds the BatchNorm in for the "bn-relu" order)."""
     from .. import ops
     w, b, scale, shift, relu = layer.export()
-    return ops.PackedAffine(w, device, layer.affine.context, b, scale, shift, relu=relu, pad_to=8)
+    return ops.PackedAffine(w, device, layer.affine.context, b, scale, shift, relu=relu, pad_to=8, keep_record=keep_record)
 
 
-def from_affine(affine, device, relu=False, row_scale=None):
+def from_affine(affine, device, relu=False, row_scale=None, keep_record=False):
     """A TdnnAffine alone (grouped weights expanded block-diagonally) as an ops.PackedAffine, rows padded to a multiple of 8."""
     from .. import ops
     return ops.PackedAffine(affine.dense_weight(), device, affine.context, affine.bias, relu=relu, pad_to=8,
-                            row_scale=row_scale)
+                            row_scale=row_scale, keep_record=keep_record)
 
 
 def from_record(w, b, scale, shift, relu, device):
@@ -239,18 +239,22 @@ class AttentionPoolingExtractor:
     (`xvb_lde_pool`); then the segment layers on T = 1.
 
     TAKES_LENGTHS: every attention pooling (attentive, multi-head, global / multi-resolution, xi-vector) runs masked
-    batches of utterances of different lengths; an LDE instance does not."""
+    batches of utterances of different lengths; an LDE instance does not.
+
+    native() hands the same layers to the native TDNN handle (ops.Extractor with an attention pooling), which runs this
+    launch sequence in C++ with bit-identical embeddings; save(path) writes its XVBM0002 model file for bin/xvb-extract.
+    Neither exists for LDE pooling."""
 
     TAKES_LENGTHS = True
 
     def __init__(self, model, inputs_dim, frame_layers, stats, tdnn6, tdnn7, position):
         dev = model.device_for_extraction()
         self.feat_dim = inputs_dim
-        self.frames = [from_layer(l, dev) for l in frame_layers]
+        self.frames = [from_layer(l, dev, keep_record=True) for l in frame_layers]
         self.lde = self.xi = None
         if hasattr(stats, "prior_logprec"):                      # xi-vector: precision network + prior element
-            self.first = from_layer(stats.lin1_relu_bn, dev)
-            self.last = from_affine(stats.lin2, dev)
+            self.first = from_layer(stats.lin1_relu_bn, dev, keep_record=True)
+            self.last = from_affine(stats.lin2, dev, keep_record=True)
             self.xi = (stats.prior_logprec.detach().float().reshape(-1).to(dev).contiguous(),
                        stats.prior_mean.detach().float().reshape(-1).to(dev).contiguous(), bool(stats.stddev))
             self.channels, self.pooled, self.gdiv = stats.input_dim, stats.input_dim, 1
@@ -264,25 +268,25 @@ class AttentionPoolingExtractor:
             self._segments(dev, tdnn6, tdnn7, position)
             return
         att = stats.attention
-        self.first = from_affine(att.first_affine, dev, relu=True) if att.relu_affine else None
+        self.first = from_affine(att.first_affine, dev, relu=True, keep_record=True) if att.relu_affine else None
         temps = att.head_temperatures()
         row_scale = None
         if temps is not None:                                    # logits of head h are divided by t_h (pooling.py:314-316)
             row_scale = (1.0 / temps).repeat_interleave(att.final_dim)
-        self.last = from_affine(att.last_affine, dev, row_scale=row_scale)
+        self.last = from_affine(att.last_affine, dev, row_scale=row_scale, keep_record=True)
         self.channels, self.pooled, self.gdiv = stats.input_dim, stats.pooled_channels(), stats.logit_divisor()
         self.eps, self.unweighted = stats.eps, not stats.stddev_attention
         self._segments(dev, tdnn6, tdnn7, position)
 
     def _segments(self, dev, tdnn6, tdnn7, position):
         if position == "far":
-            self.segment = [from_affine(tdnn6.affine, dev)]
+            self.segment = [from_affine(tdnn6.affine, dev, keep_record=True)]
         else:
-            self.segment = [from_layer(tdnn6, dev)]
+            self.segment = [from_layer(tdnn6, dev, keep_record=True)]
             if position == "near_full":
-                self.segment.append(from_layer(tdnn7, dev))
+                self.segment.append(from_layer(tdnn7, dev, keep_record=True))
             else:
-                self.segment.append(from_affine(tdnn7.affine, dev))
+                self.segment.append(from_affine(tdnn7.affine, dev, keep_record=True))
         self.embed_dim = self.segment[-1].cout_real
         self.last_launches = 0
 
@@ -343,6 +347,48 @@ class AttentionPoolingExtractor:
         self.last_launches = len(self.frames) + (2 if self.lde is not None else (2 if self.first is not None else 1) + 1) + 1 + \
             len(self.segment)
         return emb.view(B, -1)[:, :self.embed_dim]
+
+    def native(self):
+        """The native TDNN handle (ops.Extractor) of this model, built on the current device from the records this
+        sequence packed: the same kernels in the same order, so its embeddings equal extract()'s bit for bit, masked
+        batches included.  It also takes the host-buffer and shard calls, and save() writes its XVBM0002 file."""
+        if self.lde is not None:
+            raise NotImplementedError("LDE pooling has no native handle or model file")
+        from .. import _lib, ops
+
+        def host(v):
+            return None if v is None else v.detach().float().cpu().numpy()
+
+        def add(fn, layer):
+            w, b, s, t = (host(v) for v in layer.record)
+            fn(w, b, layer.context, s, t, relu=layer.relu)
+
+        ex = ops.Extractor(self.feat_dim)
+        if self.xi is not None:
+            kind = _lib.POOL_XI_POSTDIST if self.xi[2] else _lib.POOL_XI_POSTMEAN
+            ex.set_attention_pooling(kind, self.pooled, 1, prior_logprec=host(self.xi[0]), prior_mean=host(self.xi[1]))
+        else:
+            ex.set_attention_pooling(_lib.POOL_ATTENTION, self.pooled, self.gdiv, unweighted_var=self.unweighted)
+        for layer in self.frames:
+            add(ex.add_frame_layer, layer)
+        for layer in (self.first, self.last):
+            if layer is not None:
+                add(ex.add_attention_layer, layer)
+        for layer in self.segment:
+            w, b, s, t = (host(v) for v in layer.record)
+            ex.add_segment_layer(w[:, :, 0], b, s, t, relu=layer.relu)
+        ex.finalize(pooling_eps=self.eps)
+        return ex
+
+    def save(self, path):
+        """Write this model's XVBM0002 file (the native handle's save), which bin/xvb-extract and ops.Extractor.load read."""
+        if self.lde is not None:
+            raise NotImplementedError("LDE pooling has no native handle or model file")
+        ex = self.native()
+        try:
+            ex.save(path)
+        finally:
+            ex.close()
 
     def close(self):
         pass

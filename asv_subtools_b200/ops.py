@@ -206,10 +206,11 @@ class PackedAffine:
     gaps as zero taps.  groups > 1: a grouped 1x1 conv with its weight as stored, (Cout, Cin/groups, 1), packed compactly
     for the grouped mode, or as its block-diagonal expansion when the shape does not fit that mode (tdnn_grouped_fits).
     row_scale: a per-output factor folded into weight and bias.  pad_to: output rows zero-padded to a multiple of it, the
-    padded outputs exact zeros; the first cout_real rows are the layer's own."""
+    padded outputs exact zeros; the first cout_real rows are the layer's own.  keep_record: keep `record`, the unpadded
+    arrays that were packed, for a native handle built from the same layer."""
 
     def __init__(self, w, device, context=(0,), bias=None, scale=None, shift=None, relu=False, swish=False, groups=1,
-                 pad_to=1, row_scale=None):
+                 pad_to=1, row_scale=None, keep_record=False):
         w = to_device(w, device)
         w = w.reshape(w.shape[0], w.shape[1], -1)
         self.context = list(context)
@@ -230,6 +231,9 @@ class PackedAffine:
             w = w * row_scale.view(-1, 1, 1)
             bias = bias * row_scale if bias is not None else None
         self.cout_real = w.shape[0]
+        # keep_record: the layer as a native handle takes it, w (Cout, Cin, tot) over the whole span with row_scale
+        # folded in, and bias / scale / shift, all on `device` and unpadded (groups == 1 only)
+        self.record = (w, bias, scale, shift) if keep_record and self.groups == 1 else None
         pad = (-w.shape[0]) % pad_to
         if pad:
             w = torch.cat([w, w.new_zeros(pad, w.shape[1], w.shape[2])], 0)
@@ -917,7 +921,9 @@ def retrieve_topk(enroll, test, k, row_bias=None, col_bias=None, slab_cols=None)
 # ------------------------------------------------------------------ whole-model extractor
 class Extractor(ShardExtractor):
     """Owner of a native xvb_extractor_t (packed weights + workspace on the current device), built layer by layer with
-    add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file; save() writes that file."""
+    add_frame_layer / add_segment_layer / finalize or loaded from an XVBM0001 file; save() writes that file.  With
+    set_attention_pooling (before the first layer) and add_attention_layer (after the frame layers) the pooling is an
+    attention or xi-vector pooling instead, and the file is XVBM0002."""
 
     TAKES_LENGTHS = True
 
@@ -946,6 +952,27 @@ class Extractor(ShardExtractor):
         check(lib.xvb_extractor_add_frame_layer(self._h, w.shape[0], int_array(context), len(context), wp, bp, sp, tp,
                                                 flags), "xvb_extractor_add_frame_layer")
 
+    def set_attention_pooling(self, kind, pooled, gdiv=1, unweighted_var=False, prior_logprec=None, prior_mean=None):
+        """kind: _lib.POOL_ATTENTION, POOL_XI_POSTMEAN or POOL_XI_POSTDIST (xvb_extractor_set_attention_pooling); the
+        xi-vector kinds take the prior's (pooled,) log-precision and mean."""
+        lp, lpp = self._np(prior_logprec)
+        pm, pmp = self._np(prior_mean)
+        for a in (lp, pm):
+            if a is not None and a.size != pooled:
+                raise ValueError("the xi-vector prior needs {} values, got {}".format(pooled, a.size))
+        check(lib.xvb_extractor_set_attention_pooling(self._h, int(kind), int(pooled), int(gdiv), 1 if unweighted_var else 0,
+                                                      lpp, pmp), "xvb_extractor_set_attention_pooling")
+
+    def add_attention_layer(self, weight, bias, context, bn_scale=None, bn_shift=None, relu=False):
+        """The attention pooling's first affine (ReLU [+ BN]) or last affine (the logits), after the frame layers."""
+        w, wp = self._np(weight)
+        b, bp = self._np(bias)
+        s, sp = self._np(bn_scale)
+        t, tp = self._np(bn_shift)
+        flags = (RELU if relu else 0) | (BN if bn_scale is not None else 0)
+        check(lib.xvb_extractor_add_attention_layer(self._h, w.shape[0], int_array(context), len(context), wp, bp, sp, tp,
+                                                    flags), "xvb_extractor_add_attention_layer")
+
     def add_segment_layer(self, weight, bias, bn_scale=None, bn_shift=None, relu=False):
         w, wp = self._np(weight)
         b, bp = self._np(bias)
@@ -961,7 +988,7 @@ class Extractor(ShardExtractor):
 
     @classmethod
     def load(cls, path):
-        """An extractor straight from an .xvbm file (no Python-side layer objects)."""
+        """An extractor straight from an .xvbm file, XVBM0001 or XVBM0002 (no Python-side layer objects)."""
         self = cls.__new__(cls)
         self._lib, self._check = lib, check
         self._h = C.c_void_p()

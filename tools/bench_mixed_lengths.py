@@ -2,7 +2,7 @@
 """Throughput of an x-vector extractor on a corpus of utterances of different lengths -- a side measurement, not the
 bench.py line.
 
-    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|ftdnn|campplus|conformer]
+    python tools/bench_mixed_lengths.py [rounds] [--model xvector|resnet|multihead|xivector|xi|ftdnn|campplus|conformer]
                                         [--utts N] [--min-frames A] [--max-frames B] [--batch N] [--dim F]
 
 The corpus is N utterances (default 4000) with frame counts drawn uniformly from [A, B] (default 200 .. 2000) by
@@ -19,7 +19,10 @@ utterance of the default corpus is one chunk of its own length under CAM++'s 400
 the native Conformer handle with the launcher's model as tools/bench_conformer.py builds it (6 blocks, attention_dim 256,
 rot_pos, softmax_plus, 4x subsampling) on 80-d features (--dim is ignored), batch 128 by default; every utterance is cut
 by the 300-frame chunk rule (chunk_plan) first, and both policies batch the chunks.  Frames/s still counts the corpus
-frames.
+frames.  --model xi: the xi-vector of pytorch/launcher/runSnowdar_Xivector.py (pooling xi-postdist-softplus2, 1500
+nodes, hidden_size 256, position far) at 40-d features (--dim is ignored), batch 256 by default, on the native TDNN
+handle (AttentionPoolingExtractor.native()); both policies also run on AttentionPoolingExtractor itself, the same
+batches, reported as equal_length_python and masked_python.
 
   * equal_length: today's buckets of xvb-extract / pipeline/extract_embeddings.py without --mixed-lengths -- batches of
     up to `batch` utterances of exactly the same frame count, one xvb_<handle>_extract call each;
@@ -53,7 +56,9 @@ import resnet_oracle as ro  # noqa: E402
 
 # the golden configurations of tests/golden/make_golden_snowdar.py that --model multihead / xivector run
 SNOWDAR = {"multihead": ("multi-head", {"num_head": 4}, 313),
-           "xivector": ("xi-postdist-softplus2", {"hidden_size": 64, "num_nodes": 200}, 320)}
+           "xivector": ("xi-postdist-softplus2", {"hidden_size": 64, "num_nodes": 200}, 320),
+           "xi": ("xi-postdist-softplus2", {"num_nodes": 1500, "num_head": 16, "share": True, "affine_layers": 1,
+                                            "hidden_size": 256, "context": [0], "temperature": False, "fixed": True}, 321)}
 
 
 def equal_length_batches(lengths, batch):
@@ -71,9 +76,9 @@ def main():
     ap.add_argument("--min-frames", type=int, default=200)
     ap.add_argument("--max-frames", type=int, default=2000)
     ap.add_argument("--batch", type=int, default=None,
-                    help="default 256 (xvector, multihead, xivector) or 128 (resnet, ftdnn, campplus, conformer)")
+                    help="default 256 (xvector, multihead, xivector, xi) or 128 (resnet, ftdnn, campplus, conformer)")
     ap.add_argument("--dim", type=int, default=23)
-    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "ftdnn", "campplus", "conformer"],
+    ap.add_argument("--model", choices=["xvector", "resnet", "multihead", "xivector", "xi", "ftdnn", "campplus", "conformer"],
                     default="xvector")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -88,7 +93,7 @@ def main():
         m = ResNetXvector(F, 10, training=False, extracted_embedding="near", **ro.ONLINE)
         m.load_state_dict(onn.make_state_dict(ro.resnet_spec(F, ro.ONLINE), 301), strict=True)
         workload = "online SE ResNet34 (80-d, near)"
-    elif args.model in ("multihead", "xivector"):
+    elif args.model in ("multihead", "xivector", "xi"):
         from asv_subtools_b200.model.snowdar_xvector import Xvector as SnowdarXvector
         F = 40
         args.batch = args.batch or 256
@@ -97,6 +102,8 @@ def main():
         m.load_state_dict(onn.make_state_dict(onn.snowdar_xvector_spec(F, pooling=pooling, pooling_params=pp), seed),
                           strict=True)
         workload = "snowdar Xvector(40) far, pooling {} {}".format(pooling, pp)
+        if args.model == "xi":
+            workload = "launcher xi-vector (runSnowdar_Xivector.py, 40-d, far) on the native handle"
     elif args.model == "ftdnn":
         from asv_subtools_b200.model.factored_xvector import Xvector as FactoredXvector
         F = 40
@@ -132,35 +139,41 @@ def main():
         workload = "Xvector({}) far".format(F)
     m.cuda().eval()
     ex = m.extractor()
+    extractors = {"": ex}
+    if args.model == "xi":   # the native handle, and the Python launch sequence it was built from
+        extractors = {"": ex.native(), "_python": ex}
     # the items both policies batch: the chunks of the model's own chunk rule where it cuts utterances, else the utterances
     chunks = [n for u in lengths for n in m.chunk_sizes(u)] if args.model == "conformer" else lengths
     base = torch.randn(args.batch * max(chunks) * F, device="cuda")
 
     policies = {}
-    for name, plan in (("equal_length", equal_length_batches(chunks, args.batch)),
-                       ("masked", plan_mixed_batches(chunks, args.batch))):
-        jobs = []
-        for idx in plan:
-            lens = [chunks[i] for i in idx]
-            B, T = len(lens), max(lens)
-            jobs.append((B, T, np.asarray(lens, np.int32) if name == "masked" else None))
-        computed = sum(B * T for B, T, _ in jobs)
-        policies[name] = {"jobs": jobs, "batches": len(jobs), "padded_share": 1.0 - sum(chunks) / computed, "fps": []}
+    for suffix, e in extractors.items():
+        for name, plan in (("equal_length", equal_length_batches(chunks, args.batch)),
+                           ("masked", plan_mixed_batches(chunks, args.batch))):
+            jobs = []
+            for idx in plan:
+                lens = [chunks[i] for i in idx]
+                B, T = len(lens), max(lens)
+                jobs.append((B, T, np.asarray(lens, np.int32) if name == "masked" else None))
+            computed = sum(B * T for B, T, _ in jobs)
+            policies[name + suffix] = {"jobs": jobs, "ex": e, "batches": len(jobs),
+                                       "padded_share": 1.0 - sum(chunks) / computed, "fps": []}
 
-    def run(jobs):
-        for B, T, lens in jobs:
+    def run(p):
+        ex = p["ex"]
+        for B, T, lens in p["jobs"]:
             x = base[:B * T * F].view(B, T, F)
             ex.extract(x) if lens is None else ex.extract(x, lens)
 
     with torch.no_grad():
         for p in policies.values():          # warm-up: every plan built, every buffer grown
-            run(p["jobs"])
+            run(p)
         torch.cuda.synchronize()
         for _ in range(args.rounds):
             for p in policies.values():
                 start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 start.record()
-                run(p["jobs"])
+                run(p)
                 stop.record()
                 stop.synchronize()
                 p["fps"].append(sum(lengths) / (start.elapsed_time(stop) / 1e3))
@@ -171,6 +184,9 @@ def main():
         out[name] = {"frames_per_s": statistics.median(p["fps"]), "frames_per_s_min": min(p["fps"]),
                      "frames_per_s_max": max(p["fps"]), "batches": p["batches"], "padded_share": round(p["padded_share"], 5)}
     out["speedup"] = out["masked"]["frames_per_s"] / out["equal_length"]["frames_per_s"]
+    if "masked_python" in out:   # the native handle against the Python launch sequence, per policy
+        out["native_vs_python"] = {k: out[k]["frames_per_s"] / out[k + "_python"]["frames_per_s"]
+                                   for k in ("equal_length", "masked")}
     print(json.dumps(out))
 
 
